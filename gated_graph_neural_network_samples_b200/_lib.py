@@ -35,6 +35,15 @@ class GgnnLayerGrads(C.Structure):
                  "cand_hidden_bias")]
 
 
+class GcnConfig(C.Structure):
+    _fields_ = [("hidden_size", C.c_int32), ("num_layers", C.c_int32), ("use_bias", C.c_int32), ("precision", C.c_int32),
+                ("device", C.c_int32)]
+
+
+class GcnLayerWeights(C.Structure):
+    _fields_ = [("kernel", C.c_void_p), ("bias", C.c_void_p)]
+
+
 # name -> (restype, argtypes): every symbol include/ggnn_b200.h declares
 SYMBOLS = {
     "ggnn_create": (C.c_int, [C.POINTER(GgnnConfig), C.POINTER(C.c_void_p)]),
@@ -83,6 +92,14 @@ SYMBOLS = {
     "ggnn_debug_trace": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     "ggnn_debug_timestamps": (C.c_int, [C.c_void_p, C.c_void_p]),
     "ggnn_plan_description": (C.c_char_p, [C.c_void_p]),
+    "ggnn_gcn_create": (C.c_int, [C.POINTER(GcnConfig), C.POINTER(C.c_void_p)]),
+    "ggnn_gcn_set_weights": (C.c_int, [C.c_void_p, C.POINTER(GcnLayerWeights), C.c_int32]),
+    "ggnn_prepare_graph_gcn": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "ggnn_host_prepare_graph_gcn": (C.c_int, [C.POINTER(GcnConfig), C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p,
+                                              C.POINTER(C.c_void_p)]),
+    "ggnn_set_graph_gcn": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ggnn_prepared_graph_slot_weights": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ggnn_gcn_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GcnLayerWeights), C.c_int32, C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

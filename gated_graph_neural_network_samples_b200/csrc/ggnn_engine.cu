@@ -27,6 +27,7 @@
 #include "ggnn_fwd_ffma.cuh"
 #include "ggnn_fwd_tc.cuh"
 #include "ggnn_fwd_stream.cuh"
+#include "ggnn_gcn.cuh"
 
 using namespace ggnn;
 
@@ -66,10 +67,14 @@ struct HostPinned {
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// which model an engine (and the shadow engine of a prepared graph) was created for: ggnn_create / ggnn_gcn_create
+enum { MODEL_GGNN = 0, MODEL_GCN = 1 };
+
 }  // namespace
 
 struct ggnn_engine {
     // model shape
+    int model = MODEL_GGNN;
     int D = 0, T = 0, L = 0;
     int steps[MAX_LAYERS] = {0};
     int nres[MAX_LAYERS] = {0};
@@ -107,6 +112,8 @@ struct ggnn_engine {
     size_t off_row_ptr = 0, off_src = 0, off_msg = 0, off_indeg = 0, off_denom = 0, off_tiles = 0, off_mask = 0, off_adj = 0;
     size_t off_trow = 0, off_ttgt = 0;   // source-keyed CSR (rows source*T+type -> targets), built when save_for_backward is on
     bool has_transpose = false;
+    size_t off_slotw = 0, off_tslotw = 0;   // GCN: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
+    ggnn_gcn_layer_weights gcn_w[MAX_LAYERS] = {};
     int64_t edges_of_type[32] = {0};
     DevBuf state_buf;   // intermediate layer states (L-1) + 2 ping-pong step buffers, each [V][D]
     DevBuf save_bufs;   // 5 (CudnnCompatibleGRUCell: 6) x total_steps x [V][D]
@@ -178,6 +185,14 @@ struct ggnn_prepared_graph {
 static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers,
                               float* d_h0, ggnn_stream_t stream);
 
+// The calls of the other model refuse a GGNN / GCN engine.
+#define GGNN_REQUIRE_MODEL(e, m)                                                                                          \
+    do {                                                                                                                  \
+        if ((e)->model != (m))                                                                                            \
+            return (e)->fail(GGNN_ESTATE, "%s is a %s call; this engine was created with %s", __func__,                   \
+                             (m) == MODEL_GCN ? "GCN" : "GGNN", (e)->model == MODEL_GCN ? "ggnn_gcn_create" : "ggnn_create"); \
+    } while (0)
+
 // ------------------------------------------------------------------------------------------ kernel table
 namespace {
 
@@ -224,7 +239,10 @@ size_t fwd_smem_bytes(int variant, int nb1, int D, int T) {
 
 // Decide tile size / mode, then pack tiles greedily between `cuts` (sorted node indices where the batch
 // may be split, cuts.front()==0, cuts.back()==V).
+int build_plan_gcn(ggnn_engine* e, const std::vector<int>& cuts, std::vector<int>& tile_start);
+
 int build_plan(ggnn_engine* e, const std::vector<int>& cuts, std::vector<int>& tile_start) {
+    if (e->model == MODEL_GCN) return build_plan_gcn(e, cuts, tile_start);
     const int V = e->V, D = e->D;
     int max_span = 0;
     for (size_t i = 1; i < cuts.size(); ++i) max_span = std::max(max_span, cuts[i] - cuts[i - 1]);
@@ -348,6 +366,54 @@ int build_plan(ggnn_engine* e, const std::vector<int>& cuts, std::vector<int>& t
              e->cell == CELL_CUDNN_GRU ? "+cudnn-gru" : "",
              local ? "LOCAL(all layers+steps fused, 1 launch)" : "GLOBAL(1 launch per step)", e->ntiles, MT,
              variant_cs(variant), e->nb1, max_span, fwd_smem_bytes(variant, e->nb1, D, e->T));
+    e->plan_text = buf;
+    return GGNN_OK;
+}
+
+// GCN tile plan.  wgmma path (hidden <= 128, bf16x3 / bf16): LOCAL when every connected component fits a 128-row tile -- tiles are unions of
+// whole components, shrunk like the GGNN plan when the batch cannot fill the chip -- else GLOBAL with fixed 128-row tiles.  fp32 path: fixed
+// 32-row blocks, one launch per layer.
+int build_plan_gcn(ggnn_engine* e, const std::vector<int>& cuts, std::vector<int>& tile_start) {
+    const int V = e->V;
+    int max_span = 0;
+    for (size_t i = 1; i < cuts.size(); ++i) max_span = std::max(max_span, cuts[i] - cuts[i - 1]);
+    e->max_span = max_span;
+    e->stream = false; e->nb1 = 0; e->variant = 4;
+    const bool tcore = e->precision != GGNN_PREC_FP32 && e->DP <= 128;
+    const int fixed = tcore ? tc::TILE_M : gcn::F32_ROWS;
+    const char* fg = getenv("GGNN_FORCE_GLOBAL");
+    e->local = tcore && max_span <= tc::TILE_M && !(fg && fg[0] == '1');
+    int budget = fixed;
+    tile_start.assign(1, 0);
+    if (e->local) {
+        auto pack = [&](int b, std::vector<int>& ts) {
+            ts.assign(1, 0);
+            int cur = 0;
+            for (size_t i = 1; i < cuts.size(); ++i)
+                if (cuts[i] - cur > b) { ts.push_back(cuts[i - 1]); cur = cuts[i - 1]; }
+            if (V > cur) ts.push_back(V);
+        };
+        pack(budget, tile_start);
+        if ((int)tile_start.size() - 1 < e->num_sms) {
+            std::vector<int> trial;
+            for (int b = std::max(32, (max_span + 7) / 8 * 8); b < tc::TILE_M; b += 8) {
+                pack(b, trial);
+                if ((int)trial.size() - 1 <= e->num_sms) { budget = b; tile_start = trial; break; }
+            }
+        }
+    } else {
+        for (int r = fixed; r < V; r += fixed) tile_start.push_back(r);
+        if (V > 0) tile_start.push_back(V);
+    }
+    e->ntiles = (int)tile_start.size() - 1;
+    e->tc_row_budget = budget;
+    char buf[256];
+    if (tcore)
+        snprintf(buf, sizeof buf, "gcn-wgmma-%s %s tiles=%d rows/tile<=%d DP=%d max_component=%d", e->precision == GGNN_PREC_BF16X3 ? "bf16x3" : "bf16",
+                 e->local ? "LOCAL(all layers fused, 1 launch)" : "GLOBAL(1 launch per layer)", e->ntiles, budget, e->DP, max_span);
+    else
+        snprintf(buf, sizeof buf, "gcn-fp32-ffma GLOBAL(weighted gather + FFMA GEMM, 1 launch per layer) blocks=%d rows/block=%d D=%d", e->ntiles,
+                 gcn::F32_ROWS, e->D);
     e->plan_text = buf;
     return GGNN_OK;
 }
@@ -603,11 +669,8 @@ static int init_model_shape(ggnn_engine* e, const ggnn_config* cfg, std::string&
     return GGNN_OK;
 }
 
-int ggnn_create(const ggnn_config* cfg, ggnn_engine** out) {
-    if (!cfg || !out) { g_create_error = "null argument"; return GGNN_EINVAL; }
-    *out = nullptr;
-    ggnn_engine* e = new ggnn_engine();
-    if (int rc = init_model_shape(e, cfg, g_create_error)) { delete e; return rc; }
+// The device half of ggnn_create / ggnn_gcn_create: takes ownership of `e` (deleted on failure) and publishes it in *out.
+static int attach_device(ggnn_engine* e, ggnn_engine** out) {
     cudaError_t st = cudaSetDevice(e->device);
     cudaDeviceProp prop;
     if (st == cudaSuccess) st = cudaGetDeviceProperties(&prop, e->device);
@@ -628,6 +691,14 @@ int ggnn_create(const ggnn_config* cfg, ggnn_engine** out) {
     return GGNN_OK;
 }
 
+int ggnn_create(const ggnn_config* cfg, ggnn_engine** out) {
+    if (!cfg || !out) { g_create_error = "null argument"; return GGNN_EINVAL; }
+    *out = nullptr;
+    ggnn_engine* e = new ggnn_engine();
+    if (int rc = init_model_shape(e, cfg, g_create_error)) { delete e; return rc; }
+    return attach_device(e, out);
+}
+
 int ggnn_destroy(ggnn_engine* e) {
     if (!e) return GGNN_OK;
     cudaSetDevice(e->device);
@@ -644,6 +715,7 @@ int ggnn_destroy(ggnn_engine* e) {
 
 int ggnn_set_weights(ggnn_engine* e, const ggnn_layer_weights* layers, int32_t num_layers) {
     if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
     if (!layers || num_layers != e->L) return e->fail(GGNN_EINVAL, "expected %d layers of weights, got %d", e->L, num_layers);
     for (int l = 0; l < e->L; ++l) {
         const ggnn_layer_weights& w = layers[l];
@@ -673,7 +745,7 @@ static int upload_graph(ggnn_engine* e, size_t bytes, cudaStream_t st) {
 static int reserve_states(ggnn_engine* e) {
     const size_t vd = (size_t)std::max(e->V, 1) * e->D * sizeof(float);
     CU_TRY(e, e->state_buf.reserve(vd * (size_t)(e->L + 1)));
-    if (e->save) CU_TRY(e, e->save_bufs.reserve(vd * (e->cell == CELL_CUDNN_GRU ? 6 : 5) * (size_t)std::max(e->total_steps, 1)));
+    if (e->save && e->model == MODEL_GGNN) CU_TRY(e, e->save_bufs.reserve(vd * (e->cell == CELL_CUDNN_GRU ? 6 : 5) * (size_t)std::max(e->total_steps, 1)));
     return GGNN_OK;
 }
 
@@ -1025,6 +1097,10 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
         e->off_tvp = off;  off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
         e->off_vinfo = off; off = align_up(off + sizeof(int) * 8 * (size_t)std::max(nv, 1), 16);
     }
+    if (e->model == MODEL_GCN) {   // per-slot adjacency weights, filled by build_gcn_image
+        e->off_slotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16);
+        if (e->has_transpose) { e->off_tslotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16); }
+    }
     e->ts_nv = nv;
     for (int t = 0; t < T; ++t) e->edges_of_type[t] = num_edges[t];
     if (g->use_cuda) {
@@ -1180,6 +1256,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
 
 // Model shape (what ggnn_create fixed) -> the shadow engine of a prepared graph.
 static void copy_model_shape(ggnn_engine* dst, const ggnn_engine* src) {
+    dst->model = src->model;
     dst->D = src->D; dst->T = src->T; dst->L = src->L; dst->DP = src->DP;
     memcpy(dst->steps, src->steps, sizeof dst->steps); memcpy(dst->nres, src->nres, sizeof dst->nres);
     memcpy(dst->res, src->res, sizeof dst->res); memcpy(dst->step_base, src->step_base, sizeof dst->step_base);
@@ -1203,6 +1280,7 @@ static void adopt_plan(ggnn_engine* dst, const ggnn_engine* src) {
     dst->has_transpose = src->has_transpose; dst->off_trow = src->off_trow; dst->off_ttgt = src->off_ttgt; dst->off_tslot = src->off_tslot;
     dst->off_pair = src->off_pair; dst->off_vptr = src->off_vptr; dst->off_vsrc = src->off_vsrc; dst->off_tvp = src->off_tvp;
     dst->off_vinfo = src->off_vinfo;
+    dst->off_slotw = src->off_slotw; dst->off_tslotw = src->off_tslotw;
     memcpy(dst->edges_of_type, src->edges_of_type, sizeof dst->edges_of_type);
 }
 
@@ -1273,6 +1351,7 @@ int ggnn_prepare_graph_sparse(const ggnn_engine* e, int32_t save_for_backward, i
     if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
     g->use_cuda = true;
     copy_model_shape(&g->plan, e);
+    GGNN_REQUIRE_MODEL(&g->plan, MODEL_GGNN);
     if (save_for_backward >= 0) g->plan.save = save_for_backward != 0;   // a producer thread says what the batch will be used for
     if (cudaSetDevice(e->device) != cudaSuccess) return g->plan.fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);   // this may be a producer thread
     return build_sparse_image(g, V, adj, num_edges, indeg);
@@ -1283,6 +1362,9 @@ int ggnn_set_graph_prepared(ggnn_engine* e, ggnn_prepared_graph* g, ggnn_stream_
     e->graph_set = false; e->saved_valid = false;
     if (!g || !g->valid) return e->fail(GGNN_ESTATE, "the prepared graph is empty (its build failed or never ran)");
     const ggnn_engine& q = g->plan;
+    if (q.model != e->model)
+        return e->fail(GGNN_ESTATE, "the prepared graph was built for a %s engine, this is a %s engine", q.model == MODEL_GCN ? "GCN" : "GGNN",
+                       e->model == MODEL_GCN ? "GCN" : "GGNN");
     if (q.D != e->D || q.T != e->T || q.precision != e->precision || q.DP != e->DP || q.num_sms != e->num_sms || q.cell != e->cell || q.use_att != e->use_att)
         return e->fail(GGNN_EINVAL, "the prepared graph was built for a different engine configuration");
     if (e->save && !q.has_transpose)
@@ -1307,6 +1389,7 @@ int ggnn_set_graph_prepared(ggnn_engine* e, ggnn_prepared_graph* g, ggnn_stream_
 int ggnn_set_graph_sparse(ggnn_engine* e, int32_t V, const int32_t* const* adj, const int32_t* num_edges,
                           const float* indeg, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
     e->graph_set = false; e->saved_valid = false;
     // the same two halves a caller can run on two threads: build into the engine's own prepared graph, then upload it
     int rc = ggnn_prepare_graph_sparse(e, -1, V, adj, num_edges, indeg, &e->own_prep);
@@ -1424,6 +1507,7 @@ int ggnn_prepare_graph_dense(const ggnn_engine* e, int32_t save_for_backward, in
     if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
     g->use_cuda = true;
     copy_model_shape(&g->plan, e);
+    GGNN_REQUIRE_MODEL(&g->plan, MODEL_GGNN);
     if (save_for_backward >= 0) g->plan.save = save_for_backward != 0;
     if (cudaSetDevice(e->device) != cudaSuccess) return g->plan.fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);
     bool not_binary = false;
@@ -1446,6 +1530,7 @@ int ggnn_host_prepare_graph_dense(const ggnn_config* cfg, int32_t num_sms, int32
 
 int ggnn_set_graph_dense(ggnn_engine* e, int32_t b, int32_t v, const float* adjm, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
     e->graph_set = false; e->saved_valid = false;
     if (b < 0 || v <= 0 || (!adjm && b > 0)) return e->fail(GGNN_EINVAL, "null/negative argument");
     if (e->use_att) return e->fail(GGNN_EUNSUPPORTED, "propagation attention exists only in the sparse model (sparse:170-196)");
@@ -1897,10 +1982,281 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     return GGNN_OK;
 }
 
+// ------------------------------------------------------------------------------------------ sparse GCN (chem_tensorflow_gcn.py:42-82)
+// The model shape of a ggnn_gcn_config: one edge type, one "timestep" per layer (the dropout's global step is the layer index).
+static int init_gcn_shape(ggnn_engine* e, const ggnn_gcn_config* cfg, std::string& err) {
+    if (cfg->hidden_size <= 0 || cfg->hidden_size % 4 != 0) { err = "hidden_size must be a positive multiple of 4"; return GGNN_EINVAL; }
+    if (cfg->hidden_size > 256) { err = "hidden_size > 256 is not supported by this build"; return GGNN_EUNSUPPORTED; }
+    if (cfg->num_layers <= 0 || cfg->num_layers > MAX_LAYERS) { err = "num_layers must be in 1..16"; return GGNN_EINVAL; }
+    if (cfg->precision != GGNN_PREC_FP32 && cfg->precision != GGNN_PREC_BF16X3 && cfg->precision != GGNN_PREC_BF16) { err = "unknown precision"; return GGNN_EINVAL; }
+    e->model = MODEL_GCN;
+    e->D = cfg->hidden_size; e->T = 1; e->L = cfg->num_layers;
+    e->use_bias = cfg->use_bias != 0; e->precision = cfg->precision; e->device = cfg->device;
+    e->cell = CELL_RNN; e->act = ACT_RELU;
+    for (int l = 0; l < e->L; ++l) { e->steps[l] = 1; e->step_base[l] = l; e->nres[l] = 0; }
+    e->total_steps = e->L;
+    e->DP = (e->D + 15) / 16 * 16;
+    return GGNN_OK;
+}
+
+// Host half of a GCN batch: validate the int64 (row i = output, column j = input) list, feed it to the GGNN builder as one edge type
+// (source j -> target i, list order kept), then add the per-slot weights in target-CSR and source-CSR order.
+static int build_gcn_image(ggnn_prepared_graph* g, int32_t V, int64_t nnz, const int64_t* list, const float* w) {
+    ggnn_engine* e = &g->plan;
+    g->valid = false;
+    if (V < 0 || nnz < 0 || (nnz > 0 && (!list || !w))) return e->fail(GGNN_EINVAL, "null/negative argument");
+    if (nnz > 0x7fffffff) return e->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
+    std::vector<int32_t> pairs((size_t)nnz * 2);
+    for (int64_t k = 0; k < nnz; ++k) {
+        const int64_t i = list[2 * k], j = list[2 * k + 1];
+        if (i < 0 || i >= V || j < 0 || j >= V)
+            return e->fail(GGNN_ERANGE, "adjacency_list[%lld] = (%lld, %lld) is out of range for %d nodes", (long long)k, (long long)i, (long long)j, V);
+        pairs[2 * k] = (int32_t)j;
+        pairs[2 * k + 1] = (int32_t)i;
+    }
+    const std::vector<float> indeg((size_t)std::max(V, 1), 0.0f);
+    const int32_t* lists[1] = {pairs.data()};
+    const int32_t counts[1] = {(int32_t)nnz};
+    int rc = build_sparse_image(g, V, lists, counts, indeg.data());
+    if (rc) return rc;
+    char* base = g->image;
+    const int* csr_msg = (const int*)(base + e->off_msg);
+    float* tw = (float*)(base + e->off_slotw);
+    for (int64_t k = 0; k < nnz; ++k) tw[k] = w[csr_msg[k]];
+    if (e->has_transpose) {   // the source-keyed CSR lists the entries of every input column j in list order (build_sparse_image)
+        const int* trow = (const int*)(base + e->off_trow);
+        float* sw = (float*)(base + e->off_tslotw);
+        std::vector<int> cur(trow, trow + V);
+        for (int64_t k = 0; k < nnz; ++k) sw[cur[pairs[2 * k]]++] = w[k];
+    }
+    return GGNN_OK;
+}
+
+int ggnn_gcn_create(const ggnn_gcn_config* cfg, ggnn_engine** out) {
+    if (!cfg || !out) { g_create_error = "null argument"; return GGNN_EINVAL; }
+    *out = nullptr;
+    ggnn_engine* e = new ggnn_engine();
+    if (int rc = init_gcn_shape(e, cfg, g_create_error)) { delete e; return rc; }
+    return attach_device(e, out);
+}
+
+int ggnn_gcn_set_weights(ggnn_engine* e, const ggnn_gcn_layer_weights* layers, int32_t num_layers) {
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GCN);
+    if (!layers || num_layers != e->L) return e->fail(GGNN_EINVAL, "expected %d layers of weights, got %d", e->L, num_layers);
+    for (int l = 0; l < e->L; ++l) {
+        const ggnn_gcn_layer_weights& w = layers[l];
+        if (!w.kernel) return e->fail(GGNN_EINVAL, "layer %d: null kernel", l);
+        if (e->use_bias && !w.bias) return e->fail(GGNN_EINVAL, "layer %d: use_bias set but bias is null", l);
+        if (((uintptr_t)w.kernel & 15) || ((uintptr_t)w.bias & 15)) return e->fail(GGNN_EINVAL, "layer %d: weight pointers must be 16-byte aligned", l);
+    }
+    for (int l = 0; l < e->L; ++l) { e->gcn_w[l] = layers[l]; if (!e->use_bias) e->gcn_w[l].bias = nullptr; }
+    e->weights_set = true;
+    e->weights_dirty = true;
+    return GGNN_OK;
+}
+
+int ggnn_prepare_graph_gcn(const ggnn_engine* e, int32_t save_for_backward, int32_t V, int64_t nnz, const int64_t* list, const float* w,
+                           ggnn_prepared_graph** inout) {
+    if (!e || !inout) return GGNN_EINVAL;
+    ggnn_prepared_graph* g = *inout;
+    if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
+    g->use_cuda = true;
+    copy_model_shape(&g->plan, e);
+    GGNN_REQUIRE_MODEL(&g->plan, MODEL_GCN);
+    if (save_for_backward >= 0) g->plan.save = save_for_backward != 0;
+    if (cudaSetDevice(e->device) != cudaSuccess) return g->plan.fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);
+    return build_gcn_image(g, V, nnz, list, w);
+}
+
+int ggnn_host_prepare_graph_gcn(const ggnn_gcn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t V, int64_t nnz,
+                                const int64_t* list, const float* w, ggnn_prepared_graph** inout) {
+    if (!cfg || !inout || num_sms <= 0) return GGNN_EINVAL;
+    ggnn_prepared_graph* g = *inout;
+    if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
+    g->use_cuda = false;
+    g->valid = false;
+    if (int rc = init_gcn_shape(&g->plan, cfg, g->plan.err)) return rc;
+    g->plan.num_sms = num_sms; g->plan.max_smem = 227 * 1024;
+    g->plan.save = save_for_backward != 0;
+    return build_gcn_image(g, V, nnz, list, w);
+}
+
+int ggnn_set_graph_gcn(ggnn_engine* e, int32_t V, int64_t nnz, const int64_t* list, const float* w, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GCN);
+    e->graph_set = false; e->saved_valid = false;
+    int rc = ggnn_prepare_graph_gcn(e, -1, V, nnz, list, w, &e->own_prep);
+    if (rc) { if (e->own_prep) e->err = e->own_prep->plan.err; return rc; }
+    return ggnn_set_graph_prepared(e, e->own_prep, stream);
+}
+
+int ggnn_prepared_graph_slot_weights(const ggnn_prepared_graph* g, float* target_csr_w, float* source_csr_w) {
+    if (!g || !g->valid || g->plan.model != MODEL_GCN) return GGNN_ESTATE;
+    const ggnn_engine& q = g->plan;
+    if (source_csr_w && !q.has_transpose) return GGNN_ESTATE;
+    if (target_csr_w && q.M) memcpy(target_csr_w, g->image + q.off_slotw, sizeof(float) * (size_t)q.M);
+    if (source_csr_w && q.M) memcpy(source_csr_w, g->image + q.off_tslotw, sizeof(float) * (size_t)q.M);
+    return GGNN_OK;
+}
+
+static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream_t st) {
+    const int D = e->D, DP = e->DP, L = e->L, V = e->V;
+    const bool tcore = e->precision != GGNN_PREC_FP32 && DP <= 128;
+    gcn::GcnParams p;
+    memset(&p, 0, sizeof p);
+    p.V = V; p.D = D; p.DP = DP; p.L = L;
+    p.nparts = e->precision == GGNN_PREC_BF16X3 ? 3 : 1;
+    p.save = e->save ? 1 : 0;
+    char* g = (char*)e->graph_buf.ptr;
+    p.tile_start = (const int*)(g + e->off_tiles);
+    p.row_ptr = (const int*)(g + e->off_row_ptr);
+    p.csr_src = (const int*)(g + e->off_src);
+    p.slot_w = (const float*)(g + e->off_slotw);
+    const size_t vd = (size_t)std::max(V, 1) * D;
+    float* sb = (float*)e->state_buf.ptr;
+    p.state[0] = h0;
+    for (int l = 1; l <= L; ++l) {
+        float* ptr = (l == L) ? h_out : sb + (size_t)(l - 1) * vd;
+        p.state[l] = ptr; p.state_w[l] = ptr;
+    }
+    for (int l = 0; l < L; ++l) { p.kernel[l] = e->gcn_w[l].kernel; p.bias[l] = e->gcn_w[l].bias; }
+    p.drop_keep = e->drop_keep; p.drop_seed = e->drop_seed;
+    p.error_flag = (int*)e->err_flag.ptr;
+    if (tcore) {
+        const int NKS = DP / 16;
+        const size_t per_layer = (size_t)NKS * 64 * DP;   // one DP x DP block, pre-split and pre-tiled
+        if ((size_t)L * per_layer > e->tc_weights.cap) e->weights_dirty = true;
+        CU_TRY(e, e->tc_weights.reserve((size_t)L * per_layer));
+        uint8_t* wb = (uint8_t*)e->tc_weights.ptr;
+        if (e->weights_dirty) {
+            const long long total = (long long)NKS * 2 * DP;
+            for (int l = 0; l < L; ++l) {
+                tc::ggnn_tile_weights_kernel<<<(int)std::min<long long>((total + 255) / 256, 1024), 256, 0, st>>>(e->gcn_w[l].kernel, wb + l * per_layer, D,
+                                                                                                                 DP, 1, 1, D, 0);
+                ++e->last_launches;
+            }
+            e->weights_dirty = false;
+        }
+        for (int l = 0; l < L; ++l) p.w_tiled[l] = wb + l * per_layer;
+        const size_t opb = (size_t)DP * gcn::KGS / 4, slot_b = (size_t)DP * 128, sh_b = e->local ? (size_t)tc::TILE_M * DP * sizeof(float) : 0;
+        const size_t avail = e->max_smem > 1024 ? e->max_smem - 1024 : 0;
+        p.nstages = (int)std::min<size_t>(gcn::MAX_STAGES, avail > opb + sh_b ? (avail - opb - sh_b) / slot_b : 0);
+        if (p.nstages < 2) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the GCN tensor-core tile (DP=%d)", DP);
+        const size_t smem = opb + (size_t)p.nstages * slot_b + sh_b;
+        void (*kern)(gcn::GcnParams) = nullptr;
+        switch (DP / 2) {
+#define GGNN_GCN_CASE(nh) case nh: kern = e->local ? gcn::gcn_wgmma_kernel<true, nh> : gcn::gcn_wgmma_kernel<false, nh>; break;
+            GGNN_GCN_CASE(8) GGNN_GCN_CASE(16) GGNN_GCN_CASE(24) GGNN_GCN_CASE(32) GGNN_GCN_CASE(40) GGNN_GCN_CASE(48) GGNN_GCN_CASE(56) GGNN_GCN_CASE(64)
+#undef GGNN_GCN_CASE
+            default: return e->fail(GGNN_EUNSUPPORTED, "no GCN tensor-core kernel for DP=%d", DP);
+        }
+        CU_TRY(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        for (int l = 0; l < (e->local ? 1 : L); ++l) {
+            p.g_layer = l;
+            kern<<<e->ntiles, tc::NTHREADS, smem, st>>>(p);
+            ++e->last_launches;
+        }
+    } else {
+        const size_t smem = (size_t)gcn::F32_ROWS * D * sizeof(float);
+        CU_TRY(e, cudaFuncSetAttribute(gcn::gcn_fp32_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        for (int l = 0; l < L; ++l) {
+            p.g_layer = l;
+            gcn::gcn_fp32_kernel<<<(V + gcn::F32_ROWS - 1) / gcn::F32_ROWS, gcn::F32_THREADS, smem, st>>>(p);
+            ++e->last_launches;
+        }
+    }
+    CU_TRY(e, cudaGetLastError());
+    if (e->save) { e->saved_valid = true; e->saved_drop_keep = e->drop_keep; e->saved_drop_seed = e->drop_seed; }
+    return GGNN_OK;
+}
+
+// Backward of the GCN layers, fp32 on CUDA cores, per layer in reverse:
+//   dPre = dOut (last layer) or dOut * relu'(y) * mask / keep (gcn_relu_dropout_grad_kernel, from the saved output y)
+//   S    = A . H_l (recomputed from the saved layer input: one gather instead of L saved [V, D] arrays)
+//   dW  += S^T . dPre,  db += sum dPre            (gemm_tn_atomic_kernel, the bias rides along)
+//   dS   = dPre . W^T                             (gemm_nt_kernel)
+//   dH_l = A^T . dS                               (csr_gather_all_kernel over the source-keyed CSR with its per-slot weights: no float atomics)
+int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0, ggnn_stream_t stream) {
+    using namespace ggnn::bwd;
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GCN);
+    if (!e->graph_set || !e->weights_set) return e->fail(GGNN_ESTATE, "no graph / weights set");
+    if (!e->saved_valid) return e->fail(GGNN_ESTATE, "ggnn_gcn_backward needs a preceding ggnn_forward with save_for_backward enabled");
+    if (!e->has_transpose) return e->fail(GGNN_ESTATE, "enable save_for_backward BEFORE setting the graph (the source-keyed CSR is built there)");
+    if (!grads || num_layers != e->L || (!d_h_out && e->V > 0)) return e->fail(GGNN_EINVAL, "bad backward arguments");
+    for (int l = 0; l < e->L; ++l)
+        if (((uintptr_t)grads[l].kernel & 15) || ((uintptr_t)grads[l].bias & 15))
+            return e->fail(GGNN_EINVAL, "layer %d: gradient pointers must be 16-byte aligned", l);
+    if (((uintptr_t)d_h_out & 15) || ((uintptr_t)d_h0 & 15)) return e->fail(GGNN_EINVAL, "d_h_out / d_h0 must be 16-byte aligned");
+    CU_TRY(e, cudaSetDevice(e->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    e->last_launches = 0;
+    const int V = e->V, D = e->D, L = e->L;
+    if (V == 0) return GGNN_OK;
+    const size_t vd = (size_t)V * D;
+    const size_t slab = align_up(vd * sizeof(float), 256);
+    CU_TRY(e, e->bwd_buf.reserve(4 * slab));
+    char* bb = (char*)e->bwd_buf.ptr;
+    float *dH = (float*)bb, *dP = (float*)(bb + slab), *S = (float*)(bb + 2 * slab), *dS = (float*)(bb + 3 * slab);
+    char* g = (char*)e->graph_buf.ptr;
+    const int* row_ptr = (const int*)(g + e->off_row_ptr);
+    const int* csr_src = (const int*)(g + e->off_src);
+    const float* slotw = (const float*)(g + e->off_slotw);
+    const int* trow = (const int*)(g + e->off_trow);
+    const int* ttgt = (const int*)(g + e->off_ttgt);
+    const float* tslotw = (const float*)(g + e->off_tslotw);
+    std::vector<const float*> fstate(L + 1);
+    fstate[0] = e->last_h0; fstate[L] = e->last_out;
+    for (int l = 1; l < L; ++l) fstate[l] = (const float*)e->state_buf.ptr + (size_t)(l - 1) * vd;
+    const long long n = (long long)vd;
+    const int eb = (int)std::min<long long>((n + 255) / 256, 4096);
+    const dim3 gather_grid((V + 7) / 8, 1);
+    const float* dout = d_h_out;
+    for (int l = L - 1; l >= 0; --l) {
+        const float* dpre = dout;
+        if (l < L - 1) {
+            const float keep = e->saved_drop_keep < 1.0f ? e->saved_drop_keep : 1.0f;
+            gcn::gcn_relu_dropout_grad_kernel<<<eb, 256, 0, st>>>(dout, fstate[l + 1], dP, 1.0f / keep, n);
+            ++e->last_launches;
+            dpre = dP;
+        }
+        const ggnn_gcn_layer_grads& gw = grads[l];
+        if (gw.kernel) {
+            GatherJob j{row_ptr, csr_src, fstate[l], S, slotw, nullptr};
+            csr_gather_all_kernel<<<gather_grid, 256, 0, st>>>(j, j, V, D, 1);
+            SegList sl;
+            memset(&sl, 0, sizeof sl);
+            sl.p[0] = S; sl.ld[0] = D;
+            const int kblocks = (D + 63) / 64, tiles = ((D + 63) / 64) * kblocks;
+            const int want = std::max(1, (4 * e->num_sms + tiles - 1) / tiles);
+            const int splits = std::max(1, std::min(want, (V + 63) / 64));
+            const int rps = ((V + splits - 1) / splits + GEMM_BK - 1) / GEMM_BK * GEMM_BK;
+            gemm_tn_atomic_kernel<<<dim3((D + 63) / 64, kblocks, (V + rps - 1) / rps), 64, 0, st>>>(sl, kblocks, 1, dpre, D, gw.kernel, D, 0,
+                                                                                                   e->use_bias ? gw.bias : nullptr, V, D, D, rps);
+            e->last_launches += 2;
+        } else if (e->use_bias && gw.bias) {
+            colsum_atomic_kernel<<<dim3((D + 255) / 256, (V + 511) / 512), 256, 0, st>>>(dpre, D, nullptr, 0, gw.bias, V, D, 512);
+            ++e->last_launches;
+        }
+        if (l == 0 && !d_h0) break;
+        gemm_nt_kernel<false><<<dim3((D + NT_BN - 1) / NT_BN, (V + NT_BM - 1) / NT_BM), 128, 0, st>>>(dpre, D, 0, e->gcn_w[l].kernel, D, 0, 1, dS, D, V,
+                                                                                                      D, D);
+        float* dst = l == 0 ? d_h0 : dH;
+        GatherJob j{trow, ttgt, dS, dst, tslotw, nullptr};
+        csr_gather_all_kernel<<<gather_grid, 256, 0, st>>>(j, j, V, D, 1);
+        e->last_launches += 2;
+        dout = dst;
+    }
+    CU_TRY(e, cudaGetLastError());
+    return GGNN_OK;
+}
+
 int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
-    if (!e->weights_set) return e->fail(GGNN_ESTATE, "ggnn_set_weights has not been called");
-    if (!e->graph_set) return e->fail(GGNN_ESTATE, "no graph set (ggnn_set_graph_sparse/dense)");
+    const bool gcn = e->model == MODEL_GCN;
+    if (!e->weights_set) return e->fail(GGNN_ESTATE, "%s has not been called", gcn ? "ggnn_gcn_set_weights" : "ggnn_set_weights");
+    if (!e->graph_set) return e->fail(GGNN_ESTATE, "no graph set (%s)", gcn ? "ggnn_set_graph_gcn / ggnn_set_graph_prepared" : "ggnn_set_graph_sparse/dense");
     if ((!h0 || !h_out) && e->V > 0) return e->fail(GGNN_EINVAL, "null state pointer");
     if (((uintptr_t)h0 & 15) || ((uintptr_t)h_out & 15)) return e->fail(GGNN_EINVAL, "state pointers must be 16-byte aligned");
     CU_TRY(e, cudaSetDevice(e->device));
@@ -1909,6 +2265,7 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
     e->last_h0 = h0; e->last_out = h_out; e->saved_valid = false;
     if (e->V == 0) return GGNN_OK;
     if (e->save) { int rc = reserve_states(e); if (rc) return rc; }
+    if (e->model == MODEL_GCN) return forward_gcn(e, h0, h_out, st);
     const size_t vd_bytes = (size_t)e->V * e->D * sizeof(float);
     if (e->total_steps == 0) {  // no propagation at all: result is the input (sparse:152 with empty loops)
         if (h_out != h0) CU_TRY(e, cudaMemcpyAsync(h_out, h0, vd_bytes, cudaMemcpyDeviceToDevice, st));
@@ -1956,7 +2313,8 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
 
 int ggnn_forward_host_async(ggnn_engine* e, const float* h0_host, float* h_out_host, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
-    if (!e->graph_set) return e->fail(GGNN_ESTATE, "no graph set (ggnn_set_graph_sparse/dense)");
+    if (!e->graph_set)
+        return e->fail(GGNN_ESTATE, "no graph set (%s)", e->model == MODEL_GCN ? "ggnn_set_graph_gcn / ggnn_set_graph_prepared" : "ggnn_set_graph_sparse/dense");
     if ((!h0_host || !h_out_host) && e->V > 0) return e->fail(GGNN_EINVAL, "null host pointer");
     CU_TRY(e, cudaSetDevice(e->device));
     cudaStream_t st = (cudaStream_t)stream;
@@ -2218,6 +2576,7 @@ int ggnn_state_dropout_mask(int32_t V, int32_t D, int32_t global_step, float kee
 int ggnn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers,
                   float* d_h0, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
     return ggnn_backward_impl(e, d_h_out, grads, num_layers, d_h0, stream);
 }
 

@@ -1,0 +1,289 @@
+// Sparse GCN propagation (Kipf & Welling; chem_tensorflow_gcn.py:59-82), sm_90a.  Per layer l:
+//   S  = A . H        S[i] += w * H[j] over the nonzeros (i, j, w) of the batch, per row in list order (the stable target-sorted CSR
+//                     keeps it: the serial order of TF's CPU sparse_tensor_dense_matmul functor as we recall it from TF's source)
+//   H' = S . W_l (+ b_l),  then relu and state dropout on every layer but the last (the last layer is linear)
+//
+// Two kernels:
+//   gcn_wgmma_kernel  hidden <= 128, bf16x3 / bf16 precision.  One CTA per tile of <= 128 rows.  LOCAL: the tile is a union of whole
+//                     connected components, all layers run in one launch and H stays in shared memory between layers.  GLOBAL: one launch
+//                     per layer, the gather reads the previous layer's fp32 state from global memory (a component larger than a tile).
+//                     Warp roles and operand layouts follow ggnn_fwd_tc.cuh: four worker warpgroups, warpgroup w owns rows 64*(w%2) .. +64 and
+//                     columns NH*(w/2) .. +NH (NH = DP/2) of S . W; S is split into bf16 hi/lo in the canonical no-swizzle K-major layout; one
+//                     producer thread streams the pre-split, pre-tiled W_l (tc::ggnn_tile_weights_kernel) through a cp.async.bulk / mbarrier
+//                     ring; every wait is bounded and a timeout sets the engine's error flag (ggnn_sync_check).
+//   gcn_fp32_kernel   fp32 precision and hidden sizes in (128, 256]: per layer, 32 rows per CTA, weighted CSR gather into shared memory,
+//                     FFMA GEMM with W_l from L1/L2, same epilogue.
+// The backward pass (ggnn_engine.cu) reuses ggnn_bwd.cuh; only the relu / dropout gradient below is GCN-specific.
+#pragma once
+#include "ggnn_common.cuh"
+#include "ggnn_fwd_tc.cuh"
+#include "ggnn_wgmma.cuh"
+
+namespace ggnn {
+namespace gcn {
+
+constexpr int MAX_STAGES = 8;
+constexpr int KGS = 2048;              // A-operand k-group stride: 128 rows x 16 bytes
+constexpr int F32_ROWS = 32;           // rows per CTA of the fp32 kernel
+constexpr int F32_THREADS = 256;
+
+struct GcnParams {
+    int V, D, DP, L;
+    int nparts;                        // 3: bf16x3, 1: bf16
+    int nstages;                       // weight ring depth (slots of two K-step stages)
+    int save;                          // LOCAL: write every layer's output to global memory (backward, ggnn_layer_state)
+    const int* tile_start;             // [ntiles + 1]
+    const int* row_ptr;                // [V + 1] target (output row) CSR
+    const int* csr_src;                // [nnz]   input column of every slot
+    const float* slot_w;               // [nnz]   weight of every slot
+    const float* state[MAX_LAYERS + 1];   // [0] = h0, [L] = result
+    float* state_w[MAX_LAYERS + 1];
+    const uint8_t* w_tiled[MAX_LAYERS];   // pre-split, pre-tiled W_l: DP/16 stages of 64*DP bytes
+    const float* bias[MAX_LAYERS];        // [D] or nullptr
+    const float* kernel[MAX_LAYERS];      // fp32 W_l [D, D] (fp32 kernel)
+    int g_layer;                       // GLOBAL mode / fp32 kernel: the layer of this launch
+    float drop_keep;
+    unsigned long long drop_seed;
+    int* error_flag;
+};
+
+// bias, relu and state dropout of one output element (row, col < D) of layer l
+__device__ __forceinline__ float epilogue(float v, const GcnParams& p, int l, int row, int col) {
+    if (p.bias[l]) v += __ldg(p.bias[l] + col);
+    if (l < p.L - 1) {
+        v = fmaxf(v, 0.0f);
+        if (p.drop_keep < 1.0f) v = dropout_apply(v, p.drop_seed, l, p.V, p.D, row, col, p.drop_keep);
+    }
+    return v;
+}
+
+// ------------------------------------------------------------------------------------------------ tensor cores
+template <bool LOCAL, int NH>
+__global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid_constant__ GcnParams p) {
+    using namespace tc;
+    constexpr int NF = NH / 2;   // accumulator floats per thread (m64 x NH fragment)
+    constexpr int NJ = NH / 8;   // 8-column blocks of a fragment
+    extern __shared__ __align__(1024) uint8_t smem[];
+    __shared__ __align__(8) uint64_t bar_full[MAX_STAGES];
+    __shared__ __align__(8) uint64_t bar_empty[MAX_STAGES];
+    __shared__ int s_abort;
+
+    const int D = p.D, DP = p.DP;
+    const int NKC = DP >> 3, NKS = DP >> 4;
+    const uint32_t PART_B = (uint32_t)DP * KGS / 8u;
+    const uint32_t OPB = 2u * PART_B;
+    const uint32_t STAGE_B = (uint32_t)DP * 64u;
+    uint8_t* opS = smem;
+    uint8_t* ring = opS + OPB;
+    float* sH = reinterpret_cast<float*>(ring + (size_t)p.nstages * 2 * STAGE_B);   // LOCAL: [128][DP] fp32 node states of the tile
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int row0 = p.tile_start[blockIdx.x];
+    const int rows = p.tile_start[blockIdx.x + 1] - row0;
+    const int nst = p.nstages;
+    if (tid == 0) {
+        s_abort = 0;
+        for (int i = 0; i < MAX_STAGES; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], NUM_WORKERS / 32); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    volatile int* abortp = &s_abort;
+    const int l_begin = LOCAL ? 0 : p.g_layer;
+    const int l_end = LOCAL ? p.L : p.g_layer + 1;
+
+    if (warp < WARP_PROD) {
+        // ============================================================ WORKERS
+        const int row = (warp & 3) * 32 + lane, cg = warp >> 2;   // gather view: one row, column chunks cg, cg + 4, ...
+        constexpr int NCG = NUM_WORKERS / 128;
+        const int wgi = warp >> 2, mh = wgi & 1, nh = wgi >> 1;   // fragment view
+        const int fr0 = mh * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int fc0 = nh * NH + (lane & 3) * 2;
+        const bool mma_rows = mh * 64 < rows;
+        const bool x3 = p.nparts == 3;
+        bool ok = true;
+        auto workers_sync = [&]() {
+            uint32_t any;
+            asm volatile("{\n\t.reg .pred pa, pb;\n\tsetp.ne.u32 pa, %1, 0;\n\tbar.red.or.pred pb, 1, %2, pa;\n\tselp.u32 %0, 1, 0, pb;\n\t}\n"
+                         : "=r"(any) : "r"((uint32_t)(*abortp != 0)), "n"(NUM_WORKERS) : "memory");
+            if (any) ok = false;
+        };
+        uint32_t slot = 0, fpar = 0;
+        const uint32_t ring_a = smem_u32(ring);
+        auto take_slot = [&]() -> uint32_t {
+            const uint32_t sl = slot;
+            slot = (slot + 1 == (uint32_t)nst) ? 0u : slot + 1;
+            if (!*abortp && !mbar_wait(&bar_full[sl], (fpar >> sl) & 1u, abortp)) *abortp = 1;
+            fpar ^= 1u << sl;
+            return sl;
+        };
+        auto release_slot = [&](uint32_t sl) { __syncwarp(); if (lane == 0) mbar_arrive(&bar_empty[sl]); };
+        const uint32_t a_row = (uint32_t)mh * 64u * 16u;
+
+        if (LOCAL) {   // the tile's input states -> shared memory (padding columns zero)
+            for (int idx = tid; idx < rows * NKC; idx += NUM_WORKERS) {
+                const int r = idx / NKC, kc = idx - r * NKC;
+                float v[8];
+                load8_guarded(p.state[0] + (size_t)(row0 + r) * D, kc * 8, D, v);
+                float* d = sH + (size_t)r * DP + kc * 8;
+                *reinterpret_cast<float4*>(d) = make_float4(v[0], v[1], v[2], v[3]);
+                *reinterpret_cast<float4*>(d + 4) = make_float4(v[4], v[5], v[6], v[7]);
+            }
+            workers_sync();
+        }
+        for (int l = l_begin; l < l_end && ok; ++l) {
+            // ---- S = A . H for the tile's rows -> operand tile (hi / lo); rows beyond the tile are zero
+            {
+                int beg = 0, end = 0;
+                if (row < rows) { beg = __ldg(p.row_ptr + row0 + row); end = __ldg(p.row_ptr + row0 + row + 1); }
+                const float* gin = p.state[l];
+                for (int kc = cg; kc < NKC; kc += NCG) {
+                    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+                    for (int m = beg; m < end; ++m) {
+                        const int s = __ldg(p.csr_src + m);
+                        const float w = __ldg(p.slot_w + m);
+                        float x[8];
+                        if (LOCAL) lds8(sH + (size_t)(s - row0) * DP + kc * 8, x);
+                        else load8_guarded_cg(gin + (size_t)s * D, kc * 8, D, x);
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) acc[j] = fmaf(w, x[j], acc[j]);
+                    }
+                    store_operand_chunk(opS, KGS, PART_B, kc, row, acc);
+                }
+            }
+            fence_async_smem();
+            workers_sync();
+            // ---- S . W_l on wgmma
+            float acc[NF];
+#pragma unroll
+            for (int i = 0; i < NF; ++i) acc[i] = 0.f;
+            const int nslots = (NKS + 1) / 2;
+            for (int i = 0; i < nslots; ++i) {
+                const uint32_t sl = take_slot();
+                if (mma_rows) {
+                    const uint32_t b0 = ring_a + sl * 2u * STAGE_B + (uint32_t)nh * NH * 16u;
+                    const int nk = (2 * i + 1 < NKS) ? 2 : 1;
+                    wg::fence();
+                    for (int h = 0; h < nk; ++h) {
+                        const uint32_t a = smem_u32(opS) + (uint32_t)(2 * i + h) * 2u * KGS + a_row;
+                        const uint32_t b = b0 + (uint32_t)h * STAGE_B;
+                        const uint64_t ad = wg::make_desc(a, KGS, 128), bd = wg::make_desc(b, 16u * DP, 128);
+                        wg::Mma<NH>::run(acc, ad, bd);
+                        if (x3) {
+                            wg::Mma<NH>::run(acc, ad, wg::make_desc(b + 32u * DP, 16u * DP, 128));
+                            wg::Mma<NH>::run(acc, wg::make_desc(a + PART_B, KGS, 128), bd);
+                        }
+                    }
+                    wg::commit();
+                    wg::wait_all();
+                }
+                release_slot(sl);
+            }
+            // ---- epilogue: bias, relu, dropout; the state goes back to the tile (LOCAL) and to global memory
+            const bool to_smem = LOCAL && l + 1 < l_end;
+            const bool to_global = !LOCAL || l + 1 == l_end || p.save;
+            float* gout = p.state_w[l + 1];
+#pragma unroll
+            for (int j = 0; j < NJ; ++j)
+#pragma unroll
+                for (int hr = 0; hr < 2; ++hr) {
+                    const int r = fr0 + 8 * hr, c = fc0 + 8 * j;
+                    if (r >= rows) continue;
+                    float v0 = 0.f, v1 = 0.f;
+                    if (c < D) {
+                        v0 = epilogue(acc[4 * j + 2 * hr], p, l, row0 + r, c);
+                        v1 = epilogue(acc[4 * j + 2 * hr + 1], p, l, row0 + r, c + 1);
+                        if (to_global) st2(gout + (size_t)(row0 + r) * D + c, v0, v1);
+                    }
+                    if (to_smem) st2(sH + (size_t)r * DP + c, v0, v1);
+                }
+            workers_sync();   // the next layer's gather reads the new states and overwrites the operand tile
+        }
+        if (!ok && tid == 0) atomicExch(p.error_flag, 1);
+    } else if (lane == 0) {
+        // ============================================================ WEIGHT PRODUCER: W_l of every layer, two K-step stages per slot
+        const uint32_t nstg = (uint32_t)nst;
+        uint32_t cur = 0, used = 0, epar = 0;
+        bool ok = true;
+        for (int l = l_begin; l < l_end && ok; ++l) {
+            const uint8_t* src = p.w_tiled[l];
+            for (int i = 0; i < NKS && ok; i += 2) {
+                const uint32_t bytes = (i + 1 < NKS) ? 2u * STAGE_B : STAGE_B;
+                const uint32_t sl = cur;
+                cur = (cur + 1 == nstg) ? 0u : cur + 1;
+                if ((used >> sl) & 1u) {
+                    if (!mbar_wait(&bar_empty[sl], (epar >> sl) & 1u, abortp)) { ok = false; break; }
+                    epar ^= 1u << sl;
+                }
+                used |= 1u << sl;
+                mbar_arrive_expect_tx(&bar_full[sl], bytes);
+                bulk_copy_g2s(ring + sl * 2u * STAGE_B, src + (size_t)i * STAGE_B, bytes, &bar_full[sl]);
+            }
+        }
+        if (!ok) atomicExch(p.error_flag, 3);
+    }
+    __syncthreads();
+}
+
+// ------------------------------------------------------------------------------------------------ fp32 CUDA cores
+// One layer: CTA = 32 output rows, 8 warps.  Gather: warp w sums rows 4w .. 4w+3 (lanes over float4 columns).  GEMM: a thread owns 4 rows
+// x 4 columns per item, W_l rows are read as float4 through L1.
+__global__ void __launch_bounds__(F32_THREADS) gcn_fp32_kernel(const __grid_constant__ GcnParams p) {
+    extern __shared__ __align__(16) float sS[];   // [32][D]
+    const int D = p.D, l = p.g_layer, D4 = D >> 2;
+    const int row0 = blockIdx.x * F32_ROWS;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const float* __restrict__ in = p.state[l];
+    for (int rr = 0; rr < 4; ++rr) {
+        const int r = warp * 4 + rr, v = row0 + r;
+        int beg = 0, end = 0;
+        if (v < p.V) { beg = __ldg(p.row_ptr + v); end = __ldg(p.row_ptr + v + 1); }
+        for (int c4 = lane; c4 < D4; c4 += 32) {
+            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int m = beg; m < end; ++m) {
+                const float w = __ldg(p.slot_w + m);
+                const float4 x = __ldcg(reinterpret_cast<const float4*>(in + (size_t)__ldg(p.csr_src + m) * D) + c4);
+                s.x = fmaf(w, x.x, s.x); s.y = fmaf(w, x.y, s.y); s.z = fmaf(w, x.z, s.z); s.w = fmaf(w, x.w, s.w);
+            }
+            *reinterpret_cast<float4*>(sS + (size_t)r * D + 4 * c4) = s;
+        }
+    }
+    __syncthreads();
+    const float* __restrict__ W = p.kernel[l];
+    float* out = p.state_w[l + 1];
+    for (int it = threadIdx.x; it < (F32_ROWS / 4) * D4; it += F32_THREADS) {
+        const int rq = it / D4, cq = it - rq * D4;
+        float acc[4][4] = {{0.f}};
+        const float* s0 = sS + (size_t)(rq * 4) * D;
+        for (int k = 0; k < D; ++k) {
+            const float4 w = __ldg(reinterpret_cast<const float4*>(W + (size_t)k * D) + cq);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const float a = s0[(size_t)i * D + k];
+                acc[i][0] = fmaf(a, w.x, acc[i][0]); acc[i][1] = fmaf(a, w.y, acc[i][1]);
+                acc[i][2] = fmaf(a, w.z, acc[i][2]); acc[i][3] = fmaf(a, w.w, acc[i][3]);
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int v = row0 + rq * 4 + i;
+            if (v >= p.V) continue;
+            const int c = cq * 4;
+            float4 o;
+            o.x = epilogue(acc[i][0], p, l, v, c); o.y = epilogue(acc[i][1], p, l, v, c + 1);
+            o.z = epilogue(acc[i][2], p, l, v, c + 2); o.w = epilogue(acc[i][3], p, l, v, c + 3);
+            *reinterpret_cast<float4*>(out + (size_t)v * D + c) = o;
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ backward helper
+// gradient through relu and state dropout of a hidden layer, from the layer's saved output y = relu(pre) * mask / keep:
+// y > 0 exactly where the unit was kept and active, so  d pre = y > 0 ? dy / keep : 0  (no mask regeneration needed)
+__global__ void gcn_relu_dropout_grad_kernel(const float* __restrict__ dy, const float* __restrict__ y, float* __restrict__ dpre, float inv_keep,
+                                             long long n) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+        dpre[i] = y[i] > 0.0f ? dy[i] * inv_keep : 0.0f;
+}
+
+}  // namespace gcn
+}  // namespace ggnn

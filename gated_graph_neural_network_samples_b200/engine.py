@@ -76,6 +76,24 @@ class GgnnError(Exception):
     """Raised for every non-zero return of the C ABI (the reference raises plain ``Exception``s too)."""
 
 
+def _gcn_arrays(adjacency_list, adjacency_weights):
+    """The GCN feed as the C ABI takes it: ``[nnz, 2]`` int64 and ``[nnz]`` float32, contiguous (float64 packer weights are cast here,
+    as the reference's float32 placeholder does at the feed)."""
+    lst = np.asarray(adjacency_list)
+    if lst.size == 0:
+        lst = lst.reshape(0, 2)
+    if lst.ndim != 2 or lst.shape[1] != 2:
+        raise GgnnError("adjacency_list must be [nnz, 2] (row i = output, column j = input), got shape %s" % (lst.shape,))
+    lst = np.ascontiguousarray(lst, dtype=np.int64)
+    w = np.asarray(adjacency_weights)
+    if w.ndim != 1:
+        raise GgnnError("adjacency_weights must be [nnz], got shape %s" % (w.shape,))
+    w = np.ascontiguousarray(w, dtype=np.float32)
+    if w.shape[0] != lst.shape[0]:
+        raise GgnnError("adjacency_weights has %d entries for %d adjacency_list rows" % (w.shape[0], lst.shape[0]))
+    return lst, w
+
+
 class PreparedGraph:
     """Handle of a ``ggnn_prepared_graph`` (include/ggnn_b200.h): the host half of one batch's graph structure."""
 
@@ -121,6 +139,33 @@ class PreparedGraph:
         g.V = a.shape[0] * a.shape[2]
         g.T = int(num_edge_types)
         return g
+
+    @classmethod
+    def host_only_gcn(cls, hidden_size: int, num_layers: int, num_nodes: int, adjacency_list, adjacency_weights, use_bias: bool = False,
+                      precision: str = "fp32", num_sms: int = 132, save_for_backward: bool = False,
+                      reuse: Optional["PreparedGraph"] = None) -> "PreparedGraph":
+        """``ggnn_host_prepare_graph_gcn``: a GCN batch (``[nnz, 2]`` int64 (row i = output, column j = input) list and ``[nnz]`` weights)
+        through the same builder, no engine, no GPU."""
+        g = reuse if reuse is not None else cls()
+        cfg = _lib.GcnConfig(int(hidden_size), int(num_layers), int(bool(use_bias)), PRECISIONS[precision], 0)
+        lst, w = _gcn_arrays(adjacency_list, adjacency_weights)
+        h = C.c_void_p(g._h.value)
+        rc = g.lib.ggnn_host_prepare_graph_gcn(C.byref(cfg), int(num_sms), int(bool(save_for_backward)), int(num_nodes), lst.shape[0],
+                                               lst.ctypes.data, w.ctypes.data, C.byref(h))
+        g._h = h
+        if rc != 0:
+            raise GgnnError(g.lib.ggnn_prepared_graph_error(g._h).decode())
+        g.V = int(num_nodes)
+        g.T = 1
+        return g
+
+    def slot_weights(self, source_order: bool = False) -> np.ndarray:
+        """A GCN graph's per-slot adjacency weights in target-CSR order (``source_order``: in source-CSR order, backward graphs only)."""
+        out = np.empty(self.info()["num_messages"], np.float32)
+        rc = self.lib.ggnn_prepared_graph_slot_weights(self._h, None if source_order else out.ctypes.data, out.ctypes.data if source_order else None)
+        if rc != 0:
+            raise GgnnError("not a GCN prepared graph%s" % (" prepared for backward" if source_order else ""))
+        return out
 
     def info(self) -> dict:
         V, M, nt, nb, st = C.c_int32(), C.c_int64(), C.c_int32(), C.c_int64(), C.c_int32()
@@ -480,3 +525,72 @@ class PropagationEngine:
     @property
     def plan(self) -> str:
         return self.lib.ggnn_plan_description(self._h).decode()
+
+
+class GCNEngine(PropagationEngine):
+    """The sparse GCN model (chem_tensorflow_gcn.py:42-82) on the same C ABI: ``ggnn_gcn_create`` / ``ggnn_gcn_set_weights`` /
+    ``ggnn_set_graph_gcn`` / ``ggnn_gcn_backward``; forward, readout, dropout, save-for-backward, prepared graphs and introspection are
+    the inherited calls.  The GGNN-only calls raise ``GgnnError`` (the library refuses them on a GCN engine)."""
+
+    def __init__(self, hidden_size: int, num_layers: int, use_bias: bool = False, device: int = 0, precision: str = "fp32"):
+        self._h = C.c_void_p()
+        self.lib = _lib.load()
+        self.params = {"hidden_size": int(hidden_size), "num_timesteps": int(num_layers), "gcn_use_bias": bool(use_bias)}
+        self.D, self.T, self.L = int(hidden_size), 1, int(num_layers)
+        self.use_bias = bool(use_bias)
+        cfg = _lib.GcnConfig(self.D, self.L, int(self.use_bias), PRECISIONS[precision], int(device))
+        rc = self.lib.ggnn_gcn_create(C.byref(cfg), C.byref(self._h))
+        if rc != 0:
+            self._h = C.c_void_p()
+            raise GgnnError(self.lib.ggnn_last_error(None).decode())
+        self.device = int(device)
+        self.V = 0
+        self._weights_keepalive = None
+        self._graph_keepalive = None
+
+    def set_weights(self, kernels: Sequence, biases: Optional[Sequence] = None):
+        """``kernels[l]``: [D, D] fp32 CUDA tensor (gcn_weights_l); ``biases[l]``: [D] (gcn_bias_l) when the engine uses biases."""
+        arr = (_lib.GcnLayerWeights * len(kernels))()
+        keep = []
+        for l, k in enumerate(kernels):
+            arr[l].kernel = self._f32(k, self.D * self.D, "layer %d kernel" % l)
+            keep.append(k)
+            if self.use_bias:
+                if biases is None:
+                    raise GgnnError("the engine uses biases: pass biases")
+                arr[l].bias = self._f32(biases[l], self.D, "layer %d bias" % l)
+                keep.append(biases[l])
+        self._check(self.lib.ggnn_gcn_set_weights(self._h, arr, len(kernels)))
+        self._weights_keepalive = keep
+
+    def set_graph_gcn(self, num_nodes: int, adjacency_list, adjacency_weights):
+        """The reference's feed (chem_tensorflow_gcn.py:44-47): ``[nnz, 2]`` (row i = output, column j = input) and ``[nnz]`` weights, HOST
+        arrays; validation, stable CSR build, tile plan and upload happen in the library."""
+        lst, w = _gcn_arrays(adjacency_list, adjacency_weights)
+        self._check(self.lib.ggnn_set_graph_gcn(self._h, int(num_nodes), lst.shape[0], lst.ctypes.data, w.ctypes.data, self._stream()))
+        self.V = int(num_nodes)
+        self._graph_keepalive = (lst, w)
+
+    def prepare_graph_gcn(self, num_nodes: int, adjacency_list, adjacency_weights, save_for_backward: Optional[bool] = None,
+                          reuse: Optional[PreparedGraph] = None) -> PreparedGraph:
+        """The HOST half of ``set_graph_gcn`` (may run in a producer thread); adopt the result with ``set_graph_prepared``."""
+        lst, w = _gcn_arrays(adjacency_list, adjacency_weights)
+        g = reuse if reuse is not None else PreparedGraph(self.lib)
+        h = C.c_void_p(g._h.value)
+        rc = self.lib.ggnn_prepare_graph_gcn(self._h, -1 if save_for_backward is None else int(bool(save_for_backward)), int(num_nodes),
+                                             lst.shape[0], lst.ctypes.data, w.ctypes.data, C.byref(h))
+        g._h = h
+        if rc != 0:
+            raise GgnnError(self.lib.ggnn_prepared_graph_error(g._h).decode())
+        g.V = int(num_nodes)
+        g.T = 1
+        return g
+
+    def backward(self, d_out, grads: Sequence[dict], d_h0=None):
+        """``grads[l]``: dict with optional ``kernel`` [D, D] / ``bias`` [D] fp32 CUDA tensors, accumulated into."""
+        arr = (_lib.GcnLayerWeights * len(grads))()
+        for l, g in enumerate(grads):
+            arr[l].kernel = None if g.get("kernel") is None else g["kernel"].data_ptr()
+            arr[l].bias = None if g.get("bias") is None else g["bias"].data_ptr()
+        self._check(self.lib.ggnn_gcn_backward(self._h, d_out.data_ptr(), arr, len(grads), None if d_h0 is None else d_h0.data_ptr(),
+                                               self._stream()))

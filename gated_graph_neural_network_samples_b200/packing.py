@@ -249,3 +249,71 @@ def choose_bucket(graph, bucket_sizes=DEFAULT_BUCKET_SIZES) -> int:
     g = np.asarray(graph).reshape(-1, 3)
     mx = int(max(g[:, 0].max(), g[:, 2].max()))
     return int(np.argmax(np.asarray(bucket_sizes) > mx))
+
+
+# ------------------------------------------------------------------------------------------- sparse GCN
+def graph_to_gcn_adjacency(graph, num_nodes: int):
+    """chem_tensorflow_gcn.py:116-142 in float64: ``A[src, dst] = A[dst, src] = 1`` (assignment: duplicate bonds collapse, bond types are
+    ignored), ``A += I``, ``d = rowsum(A)^-0.5 + 1e-7``, ``diag(d) A diag(d)``; the nonzeros in row-major ``(i, j)`` order as
+    ``([nnz, 2] int64, [nnz] float64)``."""
+    a = np.zeros((num_nodes, num_nodes))
+    g = np.asarray(graph, dtype=np.int64).reshape(-1, 3)
+    a[g[:, 0], g[:, 2]] = 1
+    a[g[:, 2], g[:, 0]] = 1
+    a += np.eye(num_nodes)
+    d = np.diag(np.power(np.sum(a, axis=-1), -0.5).flatten() + 1e-7)
+    a = d.dot(a).dot(d)
+    i, j = np.nonzero(a)   # row-major order, exactly the reference's double loop over w != 0
+    return np.stack([i, j], axis=1).astype(np.int64).reshape(-1, 2), a[i, j]
+
+
+def process_raw_graphs_gcn(raw_data: Iterable[dict], task_ids=(0,)) -> List[dict]:
+    """chem_tensorflow_gcn.py:96-103 without the training-time shuffle / task sub-sampling (caller's business)."""
+    out = []
+    for d in raw_data:
+        lst, w = graph_to_gcn_adjacency(d["graph"], len(d["node_features"]))
+        out.append({"adjacency_list": lst, "adjacency_weights": w, "init": d["node_features"],
+                    "labels": [d["targets"][t][0] for t in task_ids]})
+    return out
+
+
+def pack_gcn_batch(graphs: Sequence[dict], hidden_size: int) -> dict:
+    """One batch of chem_tensorflow_gcn.py:150-197: features padded to ``hidden_size``, adjacency lists offset by the node offset of their
+    graph and concatenated (weights stay float64, as the reference feeds them), ``graph_nodes_list``, targets / mask ``[tasks, graphs]``."""
+    feats, gnl, lists, weights, tv, tm = [], [], [], [], [], []
+    offset = 0
+    for gi, g in enumerate(graphs):
+        init = np.asarray(g["init"], dtype=np.float32)
+        n, ann = init.shape
+        padded = np.zeros((n, hidden_size), dtype=np.float32)                  # gcn:165-167
+        padded[:, :ann] = init
+        feats.append(padded)
+        gnl.append(np.full(n, gi, dtype=np.int32))                             # gcn:169
+        lists.append(np.asarray(g["adjacency_list"], np.int64).reshape(-1, 2) + offset)   # gcn:170
+        weights.append(np.asarray(g["adjacency_weights"], np.float64).reshape(-1))
+        tv.append([0.0 if v is None else v for v in g["labels"]])              # gcn:173-183
+        tm.append([0.0 if v is None else 1.0 for v in g["labels"]])
+        offset += n
+    return {
+        "initial_node_representation": np.concatenate(feats, axis=0) if feats else np.zeros((0, hidden_size), np.float32),
+        "adjacency_list": np.concatenate(lists, axis=0) if lists else np.zeros((0, 2), np.int64),
+        "adjacency_weights": np.concatenate(weights) if weights else np.zeros(0, np.float64),
+        "graph_nodes_list": np.concatenate(gnl) if gnl else np.zeros(0, np.int32),
+        "target_values": np.asarray(tv, dtype=np.float32).T.reshape(-1, len(graphs)),
+        "target_mask": np.asarray(tm, dtype=np.float32).T.reshape(-1, len(graphs)),
+        "num_graphs": len(graphs),
+    }
+
+
+def iter_gcn_minibatches(data: Sequence[dict], batch_size_nodes: int, hidden_size: int):
+    """gcn:150-199: greedy packing while ``node_offset + len(graph) < batch_size`` (strict), like the sparse GGNN packer."""
+    i = 0
+    while i < len(data):
+        start, nodes = i, 0
+        while i < len(data) and nodes + len(data[i]["init"]) < batch_size_nodes:
+            nodes += len(data[i]["init"])
+            i += 1
+        if i == start:
+            raise Exception("graph %d has %d nodes and does not fit batch_size=%d"
+                            % (i, len(data[i]["init"]), batch_size_nodes))  # the reference loops forever here
+        yield pack_gcn_batch(data[start:i], hidden_size)

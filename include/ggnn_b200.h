@@ -250,6 +250,51 @@ int ggnn_host_tile_plan(int32_t hidden_size, int32_t num_edge_types, int32_t pre
                         const int32_t* const* adjacency_lists, const int32_t* num_edges, int32_t* tile_start, int32_t tile_capacity,
                         int32_t* num_tiles, char* plan_text, int32_t plan_text_capacity);
 
+/* ---- Sparse GCN (Kipf & Welling; the reference's chem_tensorflow_gcn.py:42-82) on the same engine handle.
+ * Per layer l:  S = A . H  (A sparse, S[i] += w * H[j] over the nonzeros (i, j, w) in list order),  H' = S . W_l (+ b_l),
+ * then relu and state dropout on every layer but the last (the last layer is linear).
+ * A GCN engine is created with ggnn_gcn_create.  ggnn_set_graph_prepared, ggnn_forward(_host/_host_async), ggnn_sync_check,
+ * ggnn_set_state_dropout (outputs of layers 0..L-2, global step = layer index), ggnn_set_save_for_backward, ggnn_readout_*,
+ * ggnn_layer_state (intermediate layers: after a forward with save_for_backward on), ggnn_plan_description,
+ * ggnn_last_launch_count, ggnn_prepared_graph_info and ggnn_prepared_graph_arrays (T = 1: row_ptr [V+1] keyed by the output row i,
+ * src = the input column j, msg = position in the input list) work on it as on a GGNN engine.  The GGNN-only calls
+ * (ggnn_set_weights, ggnn_set_graph_sparse/dense, ggnn_prepare_graph_sparse/dense, ggnn_run_*, ggnn_backward) return GGNN_ESTATE on a
+ * GCN engine, and the GCN calls below return GGNN_ESTATE on a GGNN engine.
+ * Limits: hidden_size a positive multiple of 4 and <= 256, 1 <= num_layers <= 16.  precision GGNN_PREC_BF16X3 / GGNN_PREC_BF16 run the
+ * wgmma kernel for hidden_size <= 128; GGNN_PREC_FP32, and hidden sizes above 128, run the fp32 CUDA-core kernel. */
+typedef struct ggnn_gcn_config {
+    int32_t hidden_size; /* params['hidden_size'] (D)                   */
+    int32_t num_layers;  /* params['num_timesteps']                     */
+    int32_t use_bias;    /* params['gcn_use_bias']                      */
+    int32_t precision;   /* GGNN_PREC_*                                 */
+    int32_t device;      /* CUDA device ordinal                         */
+} ggnn_gcn_config;
+/* DEVICE pointers, fp32: kernel [D, D] row-major (gcn_weights_l), bias [D] (gcn_bias_l) or NULL when !use_bias. */
+typedef struct ggnn_gcn_layer_weights { const float* kernel; const float* bias; } ggnn_gcn_layer_weights;
+/* Same layout; ggnn_gcn_backward ACCUMULATES into them (caller zeroes; either may be NULL; 16-byte aligned). */
+typedef struct ggnn_gcn_layer_grads { float* kernel; float* bias; } ggnn_gcn_layer_grads;
+int ggnn_gcn_create(const ggnn_gcn_config* cfg, ggnn_engine** out);
+int ggnn_gcn_set_weights(ggnn_engine* e, const ggnn_gcn_layer_weights* layers, int32_t num_layers);
+/* The reference's feed (chem_tensorflow_gcn.py:44-47), HOST pointers: adjacency_list [nnz, 2] int64 with column 0 = the OUTPUT row i and
+ * column 1 = the INPUT column j, adjacency_weights [nnz] fp32.  Any list a TF SparseTensor accepts: unsorted, duplicate (i, j) entries
+ * (summed), rows without entries, nnz = 0; an index outside [0, num_nodes) returns GGNN_ERANGE.  The host half is the GGNN builder (stable
+ * counting sort by output row, tile plan over whole connected components, one pinned image) plus the per-slot weights in target-CSR order
+ * and, when saving for backward, in source-CSR order.  save_for_backward and *inout as for ggnn_prepare_graph_sparse. */
+int ggnn_prepare_graph_gcn(const ggnn_engine* e, int32_t save_for_backward, int32_t num_nodes, int64_t nnz, const int64_t* adjacency_list,
+                           const float* adjacency_weights, ggnn_prepared_graph** inout);
+int ggnn_host_prepare_graph_gcn(const ggnn_gcn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t num_nodes, int64_t nnz,
+                                const int64_t* adjacency_list, const float* adjacency_weights, ggnn_prepared_graph** inout);
+/* ggnn_prepare_graph_gcn into an engine-owned prepared graph + ggnn_set_graph_prepared. */
+int ggnn_set_graph_gcn(ggnn_engine* e, int32_t num_nodes, int64_t nnz, const int64_t* adjacency_list, const float* adjacency_weights,
+                       ggnn_stream_t stream);
+/* Copies of a GCN prepared graph's per-slot weights: target_csr_w [nnz] (= adjacency_weights[msg]), source_csr_w [nnz] (weights in the
+ * order of the source-keyed CSR; only present when the graph was prepared for backward, else GGNN_ESTATE if requested). */
+int ggnn_prepared_graph_slot_weights(const ggnn_prepared_graph* g, float* target_csr_w, float* source_csr_w);
+/* Gradient of the GCN propagation; must follow a ggnn_forward with save_for_backward on.  d_h_out [V, D] DEVICE; grads: one entry per
+ * layer, accumulated into; d_h0 [V, D] DEVICE or NULL.  fp32 on CUDA cores whatever the forward precision. */
+int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0,
+                      ggnn_stream_t stream);
+
 /* Introspection used by the parity tests and the benchmark. */
 int ggnn_num_messages(const ggnn_engine* e, int64_t* out);
 /* Copies the engine's device CSR back: row_ptr [V*T+1] (rows keyed target*T+type), src [M], msg [M]. */
