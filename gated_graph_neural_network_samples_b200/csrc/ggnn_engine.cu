@@ -18,6 +18,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/ggnn_b200.h"
@@ -65,89 +66,48 @@ struct HostPinned {
     void release() { if (ptr) cudaFreeHost(ptr); ptr = nullptr; cap = 0; }
 };
 
+// A host image that one cudaMemcpyAsync uploads: pinned memory, or plain memory for host-only builds, which make no CUDA call.
+struct StagedImage {
+    bool use_cuda = true;
+    char* ptr = nullptr;
+    HostPinned pinned;
+    std::vector<char> plain;
+    cudaEvent_t uploaded = nullptr;   // recorded after the last upload: begin() waits for it before the image is overwritten
+
+    cudaError_t begin(size_t bytes) {
+        if (!use_cuda) {
+            if (plain.size() < bytes) plain.resize(bytes + bytes / 4 + 256);
+            ptr = plain.data();
+            return cudaSuccess;
+        }
+        if (uploaded) {
+            cudaError_t st = cudaEventSynchronize(uploaded);
+            if (st != cudaSuccess) return st;
+        }
+        cudaError_t st = pinned.reserve(bytes);
+        ptr = (char*)pinned.ptr;
+        return st;
+    }
+    cudaError_t upload(void* dev, size_t bytes, cudaStream_t stream) {
+        cudaError_t st = cudaMemcpyAsync(dev, ptr, bytes, cudaMemcpyHostToDevice, stream);
+        if (st != cudaSuccess) return st;
+        if (!use_cuda) return cudaStreamSynchronize(stream);   // a pageable image must be consumed before the caller may reuse it
+        if (!uploaded && (st = cudaEventCreateWithFlags(&uploaded, cudaEventDisableTiming)) != cudaSuccess) return st;
+        return cudaEventRecord(uploaded, stream);
+    }
+    void release() {
+        if (uploaded) { cudaEventSynchronize(uploaded); cudaEventDestroy(uploaded); uploaded = nullptr; }
+        pinned.release();
+    }
+};
+
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// which model an engine (and the shadow engine of a prepared graph) was created for: ggnn_create / ggnn_gcn_create
+// which model an engine or a prepared graph was created for: ggnn_create / ggnn_gcn_create
 enum { MODEL_GGNN = 0, MODEL_GCN = 1 };
 
-}  // namespace
-
-struct ggnn_engine {
-    // model shape
-    int model = MODEL_GGNN;
-    int D = 0, T = 0, L = 0;
-    int steps[MAX_LAYERS] = {0};
-    int nres[MAX_LAYERS] = {0};
-    int res[MAX_LAYERS][MAX_RES] = {{0}};
-    int step_base[MAX_LAYERS] = {0};
-    int total_steps = 0;
-    int use_bias = 0, use_avg = 0, cell = 0, act = 0, precision = 0, device = 0;
-    int num_sms = 132;
-    size_t max_smem = 0;
-    bool weights_set = false;
-    ggnn_layer_weights w[MAX_LAYERS];
-
-    // batch
-    bool graph_set = false;
-    int gather_mode = GATHER_SPARSE;
-    int V = 0, dense_v = 0;
-    int64_t M = 0;
-    // plan
-    int variant = 0;  // 0: RG=8,CS=1 (64-row tiles)   1: RG=4,CS=2 (32-row tiles)
-    int nb1 = 0;
-    bool local = false;
-    int ntiles = 0;
-    int max_span = 0;
-    int max_tile_msgs = 0;   // largest number of messages whose target lies in one tile
-    std::string plan_text;
-
-    // device memory
-    DevBuf graph_buf;   // packed: row_ptr | csr_src | csr_msg | indeg | denom | tile_start | tile_mask | (dense adj)
-    HostPinned graph_stage;
-    // readout (gated_regression): node -> graph map of the current batch
-    DevBuf ro_buf; HostPinned ro_stage; cudaEvent_t ro_stage_done = nullptr;
-    int ro_V = -1, ro_G = 0; bool ro_grouped = false, ro_has_mask = false;
-    size_t ro_off_graph_of = 0, ro_off_start = 0, ro_off_mask = 0, ro_off_val = 0;
-    cudaEvent_t stage_done = nullptr;   // recorded after the staged H2D copy: the next set_graph waits for it before refilling
-    size_t off_row_ptr = 0, off_src = 0, off_msg = 0, off_indeg = 0, off_denom = 0, off_tiles = 0, off_mask = 0, off_adj = 0;
-    size_t off_trow = 0, off_ttgt = 0;   // source-keyed CSR (rows source*T+type -> targets), built when save_for_backward is on
-    bool has_transpose = false;
-    size_t off_slotw = 0, off_tslotw = 0;   // GCN: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
-    ggnn_gcn_layer_weights gcn_w[MAX_LAYERS] = {};
-    int64_t edges_of_type[32] = {0};
-    DevBuf state_buf;   // intermediate layer states (L-1) + 2 ping-pong step buffers, each [V][D]
-    DevBuf save_bufs;   // 5 (CudnnCompatibleGRUCell: 6) x total_steps x [V][D]
-    DevBuf io_buf;      // h0 / h_out staging for ggnn_forward_host
-    DevBuf bwd_buf;     // backward scratch
-    DevBuf tc_weights;  // pre-split, pre-tiled bf16 copies of the weights (tensor-core path)
-    DevBuf tc_respre;   // residual pre-products [ntiles][128][3*DP]
-    DevBuf err_flag;    // device int written by kernels on a barrier timeout
-    DevBuf dbg_buf;     // optional phase timestamps of the streaming kernels (GGNN_TS_DEBUG=1)
-    bool weights_dirty = true;
-    int DP = 0;         // hidden size padded to a multiple of 16 (tensor-core path)
-    size_t tc_off_edge[MAX_LAYERS] = {0}, tc_off_gate[MAX_LAYERS] = {0}, tc_off_cand[MAX_LAYERS] = {0};
-    const float* last_h0 = nullptr;
-    float* last_out = nullptr;
-    bool save = false;
-    bool saved_valid = false;
-    // streaming tensor-core plan (ggnn_fwd_stream.cuh): D > 128, or forced with GGNN_TC_STREAM=1
-    bool stream = false;
-    DevBuf ts_weights, ts_images, ts_u;
-    size_t ts_off_edge[MAX_LAYERS] = {0}, ts_off_gate[MAX_LAYERS] = {0}, ts_off_cand[MAX_LAYERS] = {0};
-    int ts_nc[2] = {0, 0}, ts_nblk[2] = {0, 0};      // [0]: DP-wide outputs (agg, candidate)  [1]: the 2*DP-wide gate output
-    int ts_tiled_nc[2] = {-1, -1};                   // the N-block widths the tiled weights were made for
-    size_t off_pair = 0, off_vptr = 0, off_vsrc = 0, off_tvp = 0, off_vinfo = 0;   // streaming plan: (target,type) -> source table, virtual rows (pairs with several messages)
-    int ts_nv = 0;                                   // number of virtual rows of the current batch
-    DevBuf ts_virt;                                  // their operand image
-    int tc_row_budget = 128, tc_kgs = 2048;   // tensor-core plan: no tile has more rows than the budget; <= 64 selects compact operand tiles
-    int use_att = 0;                 // use_propagation_attention (sparse:170-196): fp32 path only
-    DevBuf att_buf;                  // attention probabilities per target-CSR slot ([steps][M] when saving for backward, else [M])
-    size_t off_tslot = 0;            // source-keyed CSR entry -> target-CSR slot (attention backward)
-    float drop_keep = 1.0f; unsigned long long drop_seed = 0;          // state dropout for the next forward
-    float saved_drop_keep = 1.0f; unsigned long long saved_drop_seed = 0; // ... and what the saved forward used
-    int last_launches = 0;
-    std::vector<int> h_counts, h_diff, h_cursor;   // host scratch of the sparse-graph builder, kept between batches
-    struct ggnn_prepared_graph* own_prep = nullptr;   // the prepared graph ggnn_set_graph_sparse builds and uploads from (reused every batch)
+// The text of the last error of an engine or a prepared graph (ggnn_last_error / ggnn_prepared_graph_error).
+struct ErrorText {
     std::string err;
 
     int fail(int code, const char* fmt, ...) {
@@ -161,19 +121,100 @@ struct ggnn_engine {
     }
 };
 
-// The host half of ggnn_set_graph_sparse as an object: `plan` is a shadow engine that carries the model shape in and the batch / tile-plan
-// fields out and never touches the device; the packed image (CSR, in-degrees, tiles, streaming tables) sits in pinned memory, or in plain
-// memory when no CUDA device is present (host-only construction, CPU test-suite).  Built by a producer thread, uploaded by the engine's
-// thread (ggnn_set_graph_prepared) -- the ThreadedIterator overlap of the reference's training loop (chem_tensorflow.py:225, utils.py:16-36).
-struct ggnn_prepared_graph {
-    ggnn_engine plan;
-    HostPinned stage;
-    std::vector<char> plain;         // image when !use_cuda
-    char* image = nullptr;
+// What ggnn_create / ggnn_gcn_create fix for the engine's lifetime (a host-only prepare call takes it from a config).
+struct ModelShape {
+    int model = MODEL_GGNN;
+    int D = 0, T = 0, L = 0;
+    int DP = 0;         // hidden size padded to a multiple of 16 (tensor-core path)
+    int steps[MAX_LAYERS] = {0};
+    int nres[MAX_LAYERS] = {0};
+    int res[MAX_LAYERS][MAX_RES] = {{0}};
+    int step_base[MAX_LAYERS] = {0};
+    int total_steps = 0;
+    int use_bias = 0, use_avg = 0, cell = 0, act = 0, precision = 0, device = 0;
+    int use_att = 0;    // use_propagation_attention (sparse:170-196): fp32 path only
+    int num_sms = 132;
+    size_t max_smem = 0;
+};
+
+// What build_plan and the image builders derive from one batch: the tile plan and the layout of the graph image.
+struct BatchPlan {
+    int gather_mode = GATHER_SPARSE;
+    int V = 0, dense_v = 0;
+    int64_t M = 0;
+    int variant = 0;  // 0: RG=8,CS=1 (64-row tiles)   1: RG=4,CS=2 (32-row tiles)
+    int nb1 = 0;
+    bool local = false;
+    int ntiles = 0;
+    int max_span = 0;
+    int max_tile_msgs = 0;   // largest number of messages whose target lies in one tile
+    std::string plan_text;
+    // streaming tensor-core plan (ggnn_fwd_stream.cuh): D > 128, or forced with GGNN_TC_STREAM=1
+    bool stream = false;
+    int ts_nc[2] = {0, 0}, ts_nblk[2] = {0, 0};      // [0]: DP-wide outputs (agg, candidate)  [1]: the 2*DP-wide gate output
+    int ts_nv = 0;                                   // number of virtual rows of the current batch
+    int tc_row_budget = 128, tc_kgs = 2048;   // tensor-core plan: no tile has more rows than the budget; <= 64 selects compact operand tiles
+    // the graph image: row_ptr | csr_src | csr_msg | indeg | denom | tile_start | tile_mask | (dense adj) | ...
+    size_t off_row_ptr = 0, off_src = 0, off_msg = 0, off_indeg = 0, off_denom = 0, off_tiles = 0, off_mask = 0, off_adj = 0;
+    size_t off_trow = 0, off_ttgt = 0;   // source-keyed CSR (rows source*T+type -> targets), built when save_for_backward is on
+    bool has_transpose = false;
+    size_t off_tslot = 0;            // source-keyed CSR entry -> target-CSR slot (attention backward)
+    size_t off_pair = 0, off_vptr = 0, off_vsrc = 0, off_tvp = 0, off_vinfo = 0;   // streaming plan: (target,type) -> source table, virtual rows (pairs with several messages)
+    size_t off_slotw = 0, off_tslotw = 0;   // GCN: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
+    int64_t edges_of_type[32] = {0};
+};
+
+}  // namespace
+
+struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
+    bool weights_set = false;
+    ggnn_layer_weights w[MAX_LAYERS];
+    ggnn_gcn_layer_weights gcn_w[MAX_LAYERS] = {};
+    bool graph_set = false;
+
+    // device memory
+    DevBuf graph_buf;   // the graph image of the current batch
+    // readout (gated_regression): node -> graph map of the current batch
+    DevBuf ro_buf; StagedImage ro_stage;
+    int ro_V = -1, ro_G = 0; bool ro_grouped = false, ro_has_mask = false;
+    size_t ro_off_graph_of = 0, ro_off_start = 0, ro_off_mask = 0, ro_off_val = 0;
+    DevBuf state_buf;   // intermediate layer states (L-1) + 2 ping-pong step buffers, each [V][D]
+    DevBuf save_bufs;   // 5 (CudnnCompatibleGRUCell: 6) x total_steps x [V][D]
+    DevBuf io_buf;      // h0 / h_out staging for ggnn_forward_host
+    DevBuf bwd_buf;     // backward scratch
+    DevBuf tc_weights;  // pre-split, pre-tiled bf16 copies of the weights (tensor-core path)
+    DevBuf tc_respre;   // residual pre-products [ntiles][128][3*DP]
+    DevBuf err_flag;    // device int written by kernels on a barrier timeout
+    DevBuf dbg_buf;     // optional phase timestamps of the streaming kernels (GGNN_TS_DEBUG=1)
+    bool weights_dirty = true;
+    size_t tc_off_edge[MAX_LAYERS] = {0}, tc_off_gate[MAX_LAYERS] = {0}, tc_off_cand[MAX_LAYERS] = {0};
+    const float* last_h0 = nullptr;
+    float* last_out = nullptr;
+    bool save = false;
+    bool saved_valid = false;
+    DevBuf ts_weights, ts_images, ts_u;
+    size_t ts_off_edge[MAX_LAYERS] = {0}, ts_off_gate[MAX_LAYERS] = {0}, ts_off_cand[MAX_LAYERS] = {0};
+    int ts_tiled_nc[2] = {-1, -1};                   // the N-block widths the tiled weights were made for
+    DevBuf ts_virt;                                  // the operand image of the streaming plan's virtual rows
+    DevBuf att_buf;                  // attention probabilities per target-CSR slot ([steps][M] when saving for backward, else [M])
+    float drop_keep = 1.0f; unsigned long long drop_seed = 0;          // state dropout for the next forward
+    float saved_drop_keep = 1.0f; unsigned long long saved_drop_seed = 0; // ... and what the saved forward used
+    int last_launches = 0;
+    struct ggnn_prepared_graph* own_prep = nullptr;   // the prepared graph ggnn_set_graph_* build and upload from (reused every batch)
+};
+
+// The host half of ggnn_set_graph_*: the model shape goes in, the batch plan and the packed image (CSR, in-degrees, tiles, streaming
+// tables, or a weighted dense matrix) come out; nothing here touches the device but the pinned image.  Built by a producer thread,
+// uploaded by the engine's thread (ggnn_set_graph_prepared) -- the ThreadedIterator overlap of the reference's training loop
+// (chem_tensorflow.py:225, utils.py:16-36).
+struct ggnn_prepared_graph : ErrorText {
+    ModelShape shape;
+    bool save = false;   // whether the image carries the source-keyed CSR of the backward pass
+    BatchPlan plan;
+    StagedImage image;
     size_t bytes = 0;
-    bool use_cuda = true;
     bool valid = false;
-    cudaEvent_t uploaded = nullptr;  // recorded after the H2D copy of the image: the next build waits for it before overwriting
+    std::vector<int> h_counts, h_diff, h_cursor;   // host scratch of the sparse-graph builder, kept between batches
 };
 
 #define CU_TRY(e, call)                                                                           \
@@ -186,11 +227,13 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
                               float* d_h0, ggnn_stream_t stream);
 
 // The calls of the other model refuse a GGNN / GCN engine.
-#define GGNN_REQUIRE_MODEL(e, m)                                                                                          \
-    do {                                                                                                                  \
-        if ((e)->model != (m))                                                                                            \
-            return (e)->fail(GGNN_ESTATE, "%s is a %s call; this engine was created with %s", __func__,                   \
-                             (m) == MODEL_GCN ? "GCN" : "GGNN", (e)->model == MODEL_GCN ? "ggnn_gcn_create" : "ggnn_create"); \
+static int wrong_model(ErrorText* t, const char* fn, int have, int want) {
+    return t->fail(GGNN_ESTATE, "%s is a %s call; this engine was created with %s", fn, want == MODEL_GCN ? "GCN" : "GGNN",
+                   have == MODEL_GCN ? "ggnn_gcn_create" : "ggnn_create");
+}
+#define GGNN_REQUIRE_MODEL(e, m)                                                  \
+    do {                                                                          \
+        if ((e)->model != (m)) return wrong_model((e), __func__, (e)->model, (m)); \
     } while (0)
 
 // ------------------------------------------------------------------------------------------ kernel table
@@ -237,185 +280,159 @@ size_t fwd_smem_bytes(int variant, int nb1, int D, int T) {
     return sizeof(float) * ((size_t)4 * MT * D + (size_t)2 * KC * pw + (size_t)2 * MT * KC + (size_t)T * D);
 }
 
-// Decide tile size / mode, then pack tiles greedily between `cuts` (sorted node indices where the batch
-// may be split, cuts.front()==0, cuts.back()==V).
-int build_plan_gcn(ggnn_engine* e, const std::vector<int>& cuts, std::vector<int>& tile_start);
+// Tiles of whole components: a tile closes before the component that would take it past `budget` rows.
+void pack_components(const std::vector<int>& cuts, int V, int budget, std::vector<int>& tile_start) {
+    tile_start.assign(1, 0);
+    int cur = 0;
+    for (size_t i = 1; i < cuts.size(); ++i)
+        if (cuts[i] - cur > budget) { tile_start.push_back(cuts[i - 1]); cur = cuts[i - 1]; }
+    if (V > cur) tile_start.push_back(V);
+}
 
-int build_plan(ggnn_engine* e, const std::vector<int>& cuts, std::vector<int>& tile_start) {
-    if (e->model == MODEL_GCN) return build_plan_gcn(e, cuts, tile_start);
-    const int V = e->V, D = e->D;
+// Tiles of `rows` rows each, whatever the components.
+void fixed_tiles(int V, int rows, std::vector<int>& tile_start) {
+    tile_start.assign(1, 0);
+    for (int r = rows; r < V; r += rows) tile_start.push_back(r);
+    if (V > 0) tile_start.push_back(V);
+}
+
+// Whole-component tiles of up to 128 rows = two wgmma M = 64 halves, but a small batch then occupies only V/128 SMs and every tile
+// sees every edge type.  When the batch cannot fill the chip, shrink the row budget to the smallest multiple of 8 that still fits all
+// tiles in one wave: more SMs, and fewer edge-type blocks per tile (absent types are skipped).  Returns the budget.
+int pack_to_fill_chip(const std::vector<int>& cuts, int V, int max_span, int num_sms, std::vector<int>& tile_start) {
+    pack_components(cuts, V, tc::TILE_M, tile_start);
+    if ((int)tile_start.size() - 1 < num_sms) {
+        std::vector<int> trial;
+        for (int b = std::max(32, (max_span + 7) / 8 * 8); b < tc::TILE_M; b += 8) {
+            pack_components(cuts, V, b, trial);
+            if ((int)trial.size() - 1 <= num_sms) { tile_start = trial; return b; }
+        }
+    }
+    return tc::TILE_M;
+}
+
+// The tile plan of a batch of V nodes: which kernel, and the tiles.  `cuts` are the sorted node indices where the batch may be split
+// between connected components (cuts.front() == 0, cuts.back() == V).  Starts `p` afresh; the image builders fill in the rest.
+int build_plan(const ModelShape& s, int V, int gather_mode, const std::vector<int>& cuts, BatchPlan& p, std::vector<int>& tile_start,
+               std::string& err) {
+    p = BatchPlan();
+    p.V = V;
+    p.gather_mode = gather_mode;
     int max_span = 0;
     for (size_t i = 1; i < cuts.size(); ++i) max_span = std::max(max_span, cuts[i] - cuts[i - 1]);
-    e->max_span = max_span;
-    e->stream = false;
-    if (e->precision != GGNN_PREC_FP32) {
+    p.max_span = max_span;
+    const char* fg = getenv("GGNN_FORCE_GLOBAL");
+    const bool force_global = fg && fg[0] == '1';
+    const char* prec = s.precision == GGNN_PREC_BF16X3 ? "bf16x3" : "bf16";
+    char buf[256];
+    if (s.model == MODEL_GCN) {
+        // wgmma path (hidden <= 128, bf16x3 / bf16): LOCAL when every connected component fits a 128-row tile -- tiles are unions of whole
+        // components, shrunk like the GGNN plan when the batch cannot fill the chip -- else GLOBAL with fixed 128-row tiles.  fp32 path:
+        // fixed 32-row blocks, one launch per layer.
+        p.variant = 4;
+        const bool tcore = s.precision != GGNN_PREC_FP32 && s.DP <= 128;
+        p.local = tcore && max_span <= tc::TILE_M && !force_global;
+        p.tc_row_budget = tcore ? tc::TILE_M : gcn::F32_ROWS;
+        if (p.local) p.tc_row_budget = pack_to_fill_chip(cuts, V, max_span, s.num_sms, tile_start);
+        else fixed_tiles(V, p.tc_row_budget, tile_start);
+        p.ntiles = (int)tile_start.size() - 1;
+        if (tcore)
+            snprintf(buf, sizeof buf, "gcn-wgmma-%s %s tiles=%d rows/tile<=%d DP=%d max_component=%d", prec,
+                     p.local ? "LOCAL(all layers fused, 1 launch)" : "GLOBAL(1 launch per layer)", p.ntiles, p.tc_row_budget, s.DP, max_span);
+        else
+            snprintf(buf, sizeof buf, "gcn-fp32-ffma GLOBAL(weighted gather + FFMA GEMM, 1 launch per layer) blocks=%d rows/block=%d D=%d", p.ntiles,
+                     gcn::F32_ROWS, s.D);
+    } else if (s.precision != GGNN_PREC_FP32) {
         const char* fs = getenv("GGNN_TC_STREAM");
-        const char* fgl = getenv("GGNN_FORCE_GLOBAL");
         // a component larger than a tile cannot use the tile-local fused kernel: the streaming plan beats one launch per timestep of that
         // kernel (cfg5 on an H100: 0.77 vs 0.94 ms), so it is the default there; GGNN_TC_STREAM=0/1 and GGNN_FORCE_GLOBAL=1 override
-        const bool big_component = max_span > tc::TILE_M && e->gather_mode == GATHER_SPARSE && !(fgl && fgl[0] == '1') && !(fs && fs[0] == '0');
-        if (e->DP > 128 || big_component || (fs && fs[0] == '1' && e->gather_mode == GATHER_SPARSE)) {
+        const bool big_component = max_span > tc::TILE_M && gather_mode == GATHER_SPARSE && !force_global && !(fs && fs[0] == '0');
+        if (s.DP > 128 || big_component || (fs && fs[0] == '1' && gather_mode == GATHER_SPARSE)) {
             // streaming plan: fixed 128-row tiles (the gather reads the previous state from L2, so tiles need not respect components),
             // one launch per GEMM of a timestep; N blocks sized so that small batches still spread over the chip
-            if (e->gather_mode != GATHER_SPARSE)
-                return e->fail(GGNN_EUNSUPPORTED, "hidden_size > 128 on the tensor-core path needs the CSR graph format (a weighted dense adjacency runs on GGNN_PREC_FP32)");
-            e->stream = true; e->variant = 3; e->nb1 = 0; e->local = false;
-            tile_start.clear(); tile_start.push_back(0);
-            for (int r = ts::TILE_M; r < V; r += ts::TILE_M) tile_start.push_back(r);
-            if (V > 0) tile_start.push_back(V);
-            e->ntiles = (int)tile_start.size() - 1;
+            if (gather_mode != GATHER_SPARSE) {
+                err = "hidden_size > 128 on the tensor-core path needs the CSR graph format (a weighted dense adjacency runs on GGNN_PREC_FP32)";
+                return GGNN_EUNSUPPORTED;
+            }
+            p.stream = true; p.variant = 3;
+            fixed_tiles(V, ts::TILE_M, tile_start);
+            p.ntiles = (int)tile_start.size() - 1;
             for (int i = 0; i < 2; ++i) {
-                const int width = (i + 1) * e->DP;
+                const int width = (i + 1) * s.DP;
                 // one wgmma accumulator of MMA_N columns per CTA (the MMA warpgroup holds both 64-row halves in registers)
-                e->ts_nblk[i] = (width + ts::MMA_N - 1) / ts::MMA_N;
-                e->ts_nc[i] = ts::MMA_N;
+                p.ts_nblk[i] = (width + ts::MMA_N - 1) / ts::MMA_N;
+                p.ts_nc[i] = ts::MMA_N;
             }
-            char buf[256];
             int len = snprintf(buf, sizeof buf, "wgmma-%s STREAM(3 launches per step: gather-GEMM, gate GEMM, candidate GEMM) tiles=%d DP=%d N-blocks agg/cand=%dx%d gate=%dx%d",
-                               e->precision == GGNN_PREC_BF16X3 ? "bf16x3" : "bf16", e->ntiles, e->DP, e->ts_nblk[0], e->ts_nc[0], e->ts_nblk[1], e->ts_nc[1]);
-            if (e->DP <= 128) snprintf(buf + len, sizeof buf - len, " max_component=%d", max_span);   // (not computed for hidden sizes > 128: fixed tiles)
-            e->plan_text = buf;
-            return GGNN_OK;
-        }
-        e->variant = 2;
-        e->nb1 = 0;
-        e->local = max_span <= tc::TILE_M;
-        const char* fg = getenv("GGNN_FORCE_GLOBAL");
-        if (fg && fg[0] == '1') e->local = false;
-        // Rows per tile: 128 = two wgmma M = 64 halves, but a small batch then occupies only V/128 SMs and every tile
-        // sees every edge type.  When the batch cannot fill the chip, shrink the row budget to the smallest multiple of 8
-        // that still fits all tiles in one wave: more SMs, and fewer edge-type blocks per tile (absent types are skipped).
-        auto pack = [&](int budget, std::vector<int>& ts) {
-            ts.clear(); ts.push_back(0);
-            int cur = 0;
-            for (size_t i = 1; i < cuts.size(); ++i)
-                if (cuts[i] - cur > budget) { ts.push_back(cuts[i - 1]); cur = cuts[i - 1]; }
-            if (V > cur) ts.push_back(V);
-        };
-        int budget = tc::TILE_M;
-        if (e->local) {
-            pack(tc::TILE_M, tile_start);
-            const char* tr = getenv("GGNN_TC_TILE_ROWS");
-            if (tr && atoi(tr) >= max_span && atoi(tr) <= tc::TILE_M) { budget = atoi(tr); pack(budget, tile_start); }
-            else if ((int)tile_start.size() - 1 < e->num_sms) {
-                std::vector<int> trial;
-                for (int b = std::max(32, (max_span + 7) / 8 * 8); b < tc::TILE_M; b += 8) {
-                    pack(b, trial);
-                    if ((int)trial.size() - 1 <= e->num_sms) { budget = b; tile_start = trial; break; }
-                }
-            }
+                               prec, p.ntiles, s.DP, p.ts_nblk[0], p.ts_nc[0], p.ts_nblk[1], p.ts_nc[1]);
+            if (s.DP <= 128) snprintf(buf + len, sizeof buf - len, " max_component=%d", max_span);   // (not computed for hidden sizes > 128: fixed tiles)
         } else {
-            tile_start.clear(); tile_start.push_back(0);
-            for (int r = tc::TILE_M; r < V; r += tc::TILE_M) tile_start.push_back(r);
-            if (V > 0) tile_start.push_back(V);
-        }
-        if (V == 0) tile_start.assign(1, 0);
-        e->ntiles = (int)tile_start.size() - 1;
-        e->tc_row_budget = e->local ? budget : tc::TILE_M;
-        // compact operand tiles when no tile exceeds 64 rows (k-group stride 1024 instead of 2048): half the operand bytes, a ~3x deeper ring
-        e->tc_kgs = (e->tc_row_budget <= 64 && !getenv("GGNN_TC_NO_COMPACT")) ? 1024 : 2048;
-        char buf[256];
-        snprintf(buf, sizeof buf, "wgmma-%s %s tiles=%d rows/tile<=%d%s DP=%d max_component=%d",
-                 e->precision == GGNN_PREC_BF16X3 ? "bf16x3" : "bf16", e->local ? "LOCAL(all layers+steps fused, 1 launch)" : "GLOBAL(1 launch per step)",
-                 e->ntiles, budget, e->tc_kgs == 1024 ? " (compact 64-row operand tiles)" : "", e->DP, max_span);
-        e->plan_text = buf;
-        return GGNN_OK;
-    }
-    const bool a_ok = pick_nb1(0, D) > 0 && fwd_smem_bytes(0, pick_nb1(0, D), D, e->T) <= e->max_smem;
-    const bool b_ok = pick_nb1(1, D) > 0 && fwd_smem_bytes(1, pick_nb1(1, D), D, e->T) <= e->max_smem;
-    if (!a_ok && !b_ok) return e->fail(GGNN_EUNSUPPORTED, "hidden_size=%d does not fit any fp32 tile variant", D);
-    const char* force = getenv("GGNN_FFMA_VARIANT");
-    int variant;
-    bool local;
-    const bool a_local = a_ok && max_span <= 64, b_local = b_ok && max_span <= 32;
-    if (force && (force[0] == '0' || force[0] == '1') && ((force[0] == '0') ? a_ok : b_ok)) {
-        variant = force[0] - '0';
-        local = variant == 0 ? a_local : b_local;
-    } else if (b_local && (!a_local || (long)V <= (long)32 * e->num_sms * 2)) {
-        variant = 1; local = true;
-    } else if (a_local) {
-        variant = 0; local = true;
-    } else {
-        variant = a_ok ? 0 : 1; local = false;
-    }
-    const char* force_global = getenv("GGNN_FORCE_GLOBAL");
-    if (force_global && force_global[0] == '1') local = false;
-    e->variant = variant;
-    e->local = local;
-    e->nb1 = pick_nb1(variant, D);
-    const int MT = variant_mt(variant);
-    tile_start.clear();
-    tile_start.push_back(0);
-    if (local) {
-        int cur = 0;
-        for (size_t i = 1; i < cuts.size(); ++i) {
-            if (cuts[i] - cur > MT) {           // adding this component would overflow: close the tile before it
-                tile_start.push_back(cuts[i - 1]);
-                cur = cuts[i - 1];
+            p.variant = 2;
+            p.local = max_span <= tc::TILE_M && !force_global;
+            int budget = tc::TILE_M;
+            if (p.local) {
+                const char* tr = getenv("GGNN_TC_TILE_ROWS");
+                if (tr && atoi(tr) >= max_span && atoi(tr) <= tc::TILE_M) { budget = atoi(tr); pack_components(cuts, V, budget, tile_start); }
+                else budget = pack_to_fill_chip(cuts, V, max_span, s.num_sms, tile_start);
+            } else {
+                fixed_tiles(V, tc::TILE_M, tile_start);
             }
+            p.ntiles = (int)tile_start.size() - 1;
+            p.tc_row_budget = budget;
+            // compact operand tiles when no tile exceeds 64 rows (k-group stride 1024 instead of 2048): half the operand bytes, a ~3x deeper ring
+            p.tc_kgs = (p.tc_row_budget <= 64 && !getenv("GGNN_TC_NO_COMPACT")) ? 1024 : 2048;
+            snprintf(buf, sizeof buf, "wgmma-%s %s tiles=%d rows/tile<=%d%s DP=%d max_component=%d", prec,
+                     p.local ? "LOCAL(all layers+steps fused, 1 launch)" : "GLOBAL(1 launch per step)", p.ntiles, budget,
+                     p.tc_kgs == 1024 ? " (compact 64-row operand tiles)" : "", s.DP, max_span);
         }
-        if (V > cur) tile_start.push_back(V);
     } else {
-        for (int r = MT; r < V; r += MT) tile_start.push_back(r);
-        if (V > 0) tile_start.push_back(V);
+        const int D = s.D;
+        const bool a_ok = pick_nb1(0, D) > 0 && fwd_smem_bytes(0, pick_nb1(0, D), D, s.T) <= s.max_smem;
+        const bool b_ok = pick_nb1(1, D) > 0 && fwd_smem_bytes(1, pick_nb1(1, D), D, s.T) <= s.max_smem;
+        if (!a_ok && !b_ok) {
+            snprintf(buf, sizeof buf, "hidden_size=%d does not fit any fp32 tile variant", D);
+            err = buf;
+            return GGNN_EUNSUPPORTED;
+        }
+        const char* force = getenv("GGNN_FFMA_VARIANT");
+        const bool a_local = a_ok && max_span <= 64, b_local = b_ok && max_span <= 32;
+        if (force && (force[0] == '0' || force[0] == '1') && ((force[0] == '0') ? a_ok : b_ok)) {
+            p.variant = force[0] - '0';
+            p.local = p.variant == 0 ? a_local : b_local;
+        } else if (b_local && (!a_local || (long)V <= (long)32 * s.num_sms * 2)) {
+            p.variant = 1; p.local = true;
+        } else if (a_local) {
+            p.variant = 0; p.local = true;
+        } else {
+            p.variant = a_ok ? 0 : 1; p.local = false;
+        }
+        if (force_global) p.local = false;
+        p.nb1 = pick_nb1(p.variant, D);
+        const int MT = variant_mt(p.variant);
+        if (p.local) pack_components(cuts, V, MT, tile_start);
+        else fixed_tiles(V, MT, tile_start);
+        p.ntiles = (int)tile_start.size() - 1;
+        snprintf(buf, sizeof buf, "fp32-ffma%s%s %s tiles=%d rows/tile<=%d warps=8 colsplit=%d nb1=%d max_component=%d smem=%zuB", s.use_att ? "+attention" : "",
+                 s.cell == CELL_CUDNN_GRU ? "+cudnn-gru" : "",
+                 p.local ? "LOCAL(all layers+steps fused, 1 launch)" : "GLOBAL(1 launch per step)", p.ntiles, MT,
+                 variant_cs(p.variant), p.nb1, max_span, fwd_smem_bytes(p.variant, p.nb1, D, s.T));
     }
-    if (V == 0) tile_start.assign(1, 0);
-    e->ntiles = (int)tile_start.size() - 1;
-    char buf[256];
-    snprintf(buf, sizeof buf, "fp32-ffma%s%s %s tiles=%d rows/tile<=%d warps=8 colsplit=%d nb1=%d max_component=%d smem=%zuB", e->use_att ? "+attention" : "",
-             e->cell == CELL_CUDNN_GRU ? "+cudnn-gru" : "",
-             local ? "LOCAL(all layers+steps fused, 1 launch)" : "GLOBAL(1 launch per step)", e->ntiles, MT,
-             variant_cs(variant), e->nb1, max_span, fwd_smem_bytes(variant, e->nb1, D, e->T));
-    e->plan_text = buf;
+    p.plan_text = buf;
     return GGNN_OK;
 }
 
-// GCN tile plan.  wgmma path (hidden <= 128, bf16x3 / bf16): LOCAL when every connected component fits a 128-row tile -- tiles are unions of
-// whole components, shrunk like the GGNN plan when the batch cannot fill the chip -- else GLOBAL with fixed 128-row tiles.  fp32 path: fixed
-// 32-row blocks, one launch per layer.
-int build_plan_gcn(ggnn_engine* e, const std::vector<int>& cuts, std::vector<int>& tile_start) {
-    const int V = e->V;
-    int max_span = 0;
-    for (size_t i = 1; i < cuts.size(); ++i) max_span = std::max(max_span, cuts[i] - cuts[i - 1]);
-    e->max_span = max_span;
-    e->stream = false; e->nb1 = 0; e->variant = 4;
-    const bool tcore = e->precision != GGNN_PREC_FP32 && e->DP <= 128;
-    const int fixed = tcore ? tc::TILE_M : gcn::F32_ROWS;
-    const char* fg = getenv("GGNN_FORCE_GLOBAL");
-    e->local = tcore && max_span <= tc::TILE_M && !(fg && fg[0] == '1');
-    int budget = fixed;
-    tile_start.assign(1, 0);
-    if (e->local) {
-        auto pack = [&](int b, std::vector<int>& ts) {
-            ts.assign(1, 0);
-            int cur = 0;
-            for (size_t i = 1; i < cuts.size(); ++i)
-                if (cuts[i] - cur > b) { ts.push_back(cuts[i - 1]); cur = cuts[i - 1]; }
-            if (V > cur) ts.push_back(V);
-        };
-        pack(budget, tile_start);
-        if ((int)tile_start.size() - 1 < e->num_sms) {
-            std::vector<int> trial;
-            for (int b = std::max(32, (max_span + 7) / 8 * 8); b < tc::TILE_M; b += 8) {
-                pack(b, trial);
-                if ((int)trial.size() - 1 <= e->num_sms) { budget = b; tile_start = trial; break; }
-            }
+// The cut points of a batch: node boundaries no edge crosses.  The boundary before node i is crossed iff max_{j < i} reach[j] >= i, where
+// reach[j] is the farthest node an edge whose lower end is node j touches.  Without `reach`, the batch is one component.
+void find_cuts(const int* reach, int V, std::vector<int>& cuts) {
+    cuts.assign(1, 0);
+    if (reach) {
+        int far = 0;
+        for (int i = 1; i < V; ++i) {
+            far = std::max(far, reach[i - 1]);
+            if (far < i) cuts.push_back(i);
         }
-    } else {
-        for (int r = fixed; r < V; r += fixed) tile_start.push_back(r);
-        if (V > 0) tile_start.push_back(V);
     }
-    e->ntiles = (int)tile_start.size() - 1;
-    e->tc_row_budget = budget;
-    char buf[256];
-    if (tcore)
-        snprintf(buf, sizeof buf, "gcn-wgmma-%s %s tiles=%d rows/tile<=%d DP=%d max_component=%d", e->precision == GGNN_PREC_BF16X3 ? "bf16x3" : "bf16",
-                 e->local ? "LOCAL(all layers fused, 1 launch)" : "GLOBAL(1 launch per layer)", e->ntiles, budget, e->DP, max_span);
-    else
-        snprintf(buf, sizeof buf, "gcn-fp32-ffma GLOBAL(weighted gather + FFMA GEMM, 1 launch per layer) blocks=%d rows/block=%d D=%d", e->ntiles,
-                 gcn::F32_ROWS, e->D);
-    e->plan_text = buf;
-    return GGNN_OK;
+    if (V > 0) cuts.push_back(V);
 }
 
 }  // namespace
@@ -625,32 +642,40 @@ extern "C" {
 
 const char* ggnn_last_error(const ggnn_engine* e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
-// The model shape of a ggnn_config (what prepare_specific_graph_model fixes) -> e; no CUDA.  Shared by ggnn_create and the host-only
-// constructor of prepared graphs (which may run in any thread: the text goes to `err`, not to a global).  Returns GGNN_OK or an error code.
-static int init_model_shape(ggnn_engine* e, const ggnn_config* cfg, std::string& err) {
+// The checks and fields both model configs have; no CUDA (the text goes to `err`: this may run in any thread).
+static int init_common_shape(ModelShape& s, int hidden_size, int num_layers, int precision, int device, std::string& err) {
+    if (hidden_size <= 0 || hidden_size % 4 != 0) { err = "hidden_size must be a positive multiple of 4"; return GGNN_EINVAL; }
+    if (hidden_size > 256) { err = "hidden_size > 256 is not supported by this build"; return GGNN_EUNSUPPORTED; }
+    if (num_layers <= 0 || num_layers > MAX_LAYERS) { err = "num_layers must be in 1..16"; return GGNN_EINVAL; }
+    if (precision != GGNN_PREC_FP32 && precision != GGNN_PREC_BF16X3 && precision != GGNN_PREC_BF16) { err = "unknown precision"; return GGNN_EINVAL; }
+    s.D = hidden_size; s.L = num_layers; s.precision = precision; s.device = device;
+    s.DP = (s.D + 15) / 16 * 16;
+    return GGNN_OK;
+}
+
+// The model shape of a ggnn_config (what prepare_specific_graph_model fixes).  Shared by ggnn_create and the host-only constructor of
+// prepared graphs.  Returns GGNN_OK or an error code.
+static int init_model_shape(ModelShape& s, const ggnn_config* cfg, std::string& err) {
     auto bad = [&](const char* msg) { err = msg; return (int)GGNN_EINVAL; };
-    if (cfg->hidden_size <= 0 || cfg->hidden_size % 4 != 0) return bad("hidden_size must be a positive multiple of 4");
-    if (cfg->hidden_size > 256) { err = "hidden_size > 256 is not supported by this build"; return GGNN_EUNSUPPORTED; }
+    if (int rc = init_common_shape(s, cfg->hidden_size, cfg->num_layers, cfg->precision, cfg->device, err)) return rc;
     if (cfg->num_edge_types <= 0 || cfg->num_edge_types > 32) return bad("num_edge_types must be in 1..32");
-    if (cfg->num_layers <= 0 || cfg->num_layers > MAX_LAYERS) return bad("num_layers must be in 1..16");
     if (!cfg->layer_timesteps) return bad("layer_timesteps is null");
     if (cfg->cell != GGNN_CELL_GRU && cfg->cell != GGNN_CELL_RNN && cfg->cell != GGNN_CELL_CUDNN_GRU) return bad("Unknown RNN cell type");   // sparse:112
     if (cfg->cell == GGNN_CELL_CUDNN_GRU && cfg->activation != GGNN_ACT_TANH) return bad("CudnnCompatibleGRUCell requires the tanh activation");   // sparse:106
     if (cfg->activation != GGNN_ACT_TANH && cfg->activation != GGNN_ACT_RELU) return bad("Unknown activation function type");  // sparse:81
-    if (cfg->precision != GGNN_PREC_FP32 && cfg->precision != GGNN_PREC_BF16X3 && cfg->precision != GGNN_PREC_BF16) return bad("unknown precision");
-    e->D = cfg->hidden_size; e->T = cfg->num_edge_types; e->L = cfg->num_layers;
-    e->use_bias = cfg->use_edge_bias != 0; e->use_avg = cfg->use_edge_msg_avg_aggregation != 0;
-    e->cell = cfg->cell; e->act = cfg->activation; e->precision = cfg->precision; e->device = cfg->device;
-    e->use_att = cfg->use_propagation_attention != 0;
-    if (e->use_att && e->T > 16) { err = "propagation attention supports at most 16 edge types"; return GGNN_EUNSUPPORTED; }
-    if (e->use_att) e->precision = GGNN_PREC_FP32;   // the softmax-weighted gather lives in the fp32 kernel only (the plan text says so)
-    if (e->cell == CELL_CUDNN_GRU) e->precision = GGNN_PREC_FP32;   // so does the reset-after-matmul candidate of CudnnCompatibleGRUCell
+    s.T = cfg->num_edge_types;
+    s.use_bias = cfg->use_edge_bias != 0; s.use_avg = cfg->use_edge_msg_avg_aggregation != 0;
+    s.cell = cfg->cell; s.act = cfg->activation;
+    s.use_att = cfg->use_propagation_attention != 0;
+    if (s.use_att && s.T > 16) { err = "propagation attention supports at most 16 edge types"; return GGNN_EUNSUPPORTED; }
+    if (s.use_att) s.precision = GGNN_PREC_FP32;   // the softmax-weighted gather lives in the fp32 kernel only (the plan text says so)
+    if (s.cell == CELL_CUDNN_GRU) s.precision = GGNN_PREC_FP32;   // so does the reset-after-matmul candidate of CudnnCompatibleGRUCell
     int total = 0;
-    for (int l = 0; l < e->L; ++l) {
+    for (int l = 0; l < s.L; ++l) {
         if (cfg->layer_timesteps[l] < 0) return bad("negative layer_timesteps entry");
-        e->steps[l] = cfg->layer_timesteps[l];
-        e->step_base[l] = total;
-        total += e->steps[l];
+        s.steps[l] = cfg->layer_timesteps[l];
+        s.step_base[l] = total;
+        total += s.steps[l];
         int nr = 0;
         if (cfg->residual_offsets && cfg->residual_layers) {
             nr = cfg->residual_offsets[l + 1] - cfg->residual_offsets[l];
@@ -659,13 +684,25 @@ static int init_model_shape(ggnn_engine* e, const ggnn_config* cfg, std::string&
                 int r = cfg->residual_layers[cfg->residual_offsets[l] + i];
                 // node_states_per_layer has l+1 entries when layer l is built (sparse:144: IndexError otherwise)
                 if (r < 0 || r > l) return bad("residual connection refers to a layer that does not exist yet");
-                e->res[l][i] = r;
+                s.res[l][i] = r;
             }
         }
-        e->nres[l] = nr;
+        s.nres[l] = nr;
     }
-    e->total_steps = total;
-    e->DP = (e->D + 15) / 16 * 16;
+    s.total_steps = total;
+    return GGNN_OK;
+}
+
+// The model shape of a ggnn_gcn_config (chem_tensorflow_gcn.py:42-82): one edge type, one "timestep" per layer (the dropout's global step
+// is the layer index).
+static int init_gcn_shape(ModelShape& s, const ggnn_gcn_config* cfg, std::string& err) {
+    if (int rc = init_common_shape(s, cfg->hidden_size, cfg->num_layers, cfg->precision, cfg->device, err)) return rc;
+    s.model = MODEL_GCN;
+    s.T = 1;
+    s.use_bias = cfg->use_bias != 0;
+    s.cell = CELL_RNN; s.act = ACT_RELU;
+    for (int l = 0; l < s.L; ++l) { s.steps[l] = 1; s.step_base[l] = l; s.nres[l] = 0; }
+    s.total_steps = s.L;
     return GGNN_OK;
 }
 
@@ -695,7 +732,7 @@ int ggnn_create(const ggnn_config* cfg, ggnn_engine** out) {
     if (!cfg || !out) { g_create_error = "null argument"; return GGNN_EINVAL; }
     *out = nullptr;
     ggnn_engine* e = new ggnn_engine();
-    if (int rc = init_model_shape(e, cfg, g_create_error)) { delete e; return rc; }
+    if (int rc = init_model_shape(*e, cfg, g_create_error)) { delete e; return rc; }
     return attach_device(e, out);
 }
 
@@ -704,10 +741,7 @@ int ggnn_destroy(ggnn_engine* e) {
     cudaSetDevice(e->device);
     e->graph_buf.release(); e->state_buf.release(); e->save_bufs.release(); e->io_buf.release(); e->bwd_buf.release();
     e->tc_weights.release(); e->tc_respre.release(); e->ts_weights.release(); e->ts_images.release(); e->ts_u.release(); e->ts_virt.release(); e->err_flag.release(); e->dbg_buf.release();
-    e->graph_stage.release();
     if (e->own_prep) { ggnn_free_prepared_graph(e->own_prep); e->own_prep = nullptr; }
-    if (e->stage_done) cudaEventDestroy(e->stage_done);
-    if (e->ro_stage_done) cudaEventDestroy(e->ro_stage_done);
     e->ro_buf.release(); e->ro_stage.release(); e->att_buf.release();
     delete e;
     return GGNN_OK;
@@ -731,14 +765,6 @@ int ggnn_set_weights(ggnn_engine* e, const ggnn_layer_weights* layers, int32_t n
     }
     e->weights_set = true;
     e->weights_dirty = true;   // the tensor-core path re-tiles its bf16 copies at the next forward
-    return GGNN_OK;
-}
-
-static int upload_graph(ggnn_engine* e, size_t bytes, cudaStream_t st) {
-    CU_TRY(e, e->graph_buf.reserve(bytes));
-    CU_TRY(e, cudaMemcpyAsync(e->graph_buf.ptr, e->graph_stage.ptr, bytes, cudaMemcpyHostToDevice, st));
-    if (!e->stage_done) CU_TRY(e, cudaEventCreateWithFlags(&e->stage_done, cudaEventDisableTiming));
-    CU_TRY(e, cudaEventRecord(e->stage_done, st));
     return GGNN_OK;
 }
 
@@ -793,7 +819,7 @@ static void number_virtual_rows(int ntiles, int T, const int* tile_start, const 
 }
 
 // The tile plan ggnn_set_graph_sparse would make for this batch, without an engine or a GPU: the cut points (node boundaries no edge
-// crosses, from a difference array over the edge spans) and build_plan() on a scratch engine object that never touches CUDA.
+// crosses, found by a single-threaded pass of its own) and build_plan().
 int ggnn_host_tile_plan(int32_t hidden_size, int32_t num_edge_types, int32_t precision, int32_t num_sms, int32_t V, const int32_t* const* adj,
                         const int32_t* num_edges, int32_t* tile_start, int32_t tile_capacity, int32_t* num_tiles, char* plan_text,
                         int32_t plan_text_capacity) {
@@ -807,24 +833,20 @@ int ggnn_host_tile_plan(int32_t hidden_size, int32_t num_edge_types, int32_t pre
             const int lo = std::min(s, d), hi = std::max(s, d);
             if (hi > reach[lo]) reach[lo] = hi;
         }
-    std::vector<int> cuts(1, 0);
-    int far = 0;
-    for (int i = 1; i < V; ++i) {
-        far = std::max(far, reach[i - 1]);
-        if (far < i) cuts.push_back(i);
-    }
-    if (V > 0) cuts.push_back(V);
-    ggnn_engine scratch;
-    scratch.D = hidden_size; scratch.T = num_edge_types; scratch.precision = precision; scratch.num_sms = num_sms;
-    scratch.max_smem = 227 * 1024; scratch.V = V;
-    if (precision != GGNN_PREC_FP32) scratch.DP = (hidden_size + 15) / 16 * 16;
+    std::vector<int> cuts;
+    find_cuts(reach.data(), V, cuts);
+    ModelShape s;
+    s.D = hidden_size; s.T = num_edge_types; s.precision = precision; s.num_sms = num_sms; s.max_smem = 227 * 1024;
+    if (precision != GGNN_PREC_FP32) s.DP = (hidden_size + 15) / 16 * 16;
+    BatchPlan p;
+    std::string err;
     std::vector<int> ts;
-    int rc = build_plan(&scratch, cuts, ts);
+    int rc = build_plan(s, V, GATHER_SPARSE, cuts, p, ts, err);
     if (rc) return rc;
-    *num_tiles = scratch.ntiles;
+    *num_tiles = p.ntiles;
     if ((int)ts.size() > tile_capacity) return GGNN_EINVAL;
     for (size_t i = 0; i < ts.size(); ++i) tile_start[i] = ts[i];
-    if (plan_text && plan_text_capacity > 0) snprintf(plan_text, (size_t)plan_text_capacity, "%s", scratch.plan_text.c_str());
+    if (plan_text && plan_text_capacity > 0) snprintf(plan_text, (size_t)plan_text_capacity, "%s", p.plan_text.c_str());
     return GGNN_OK;
 }
 
@@ -911,10 +933,10 @@ static bool host_team_is_fast(int team) {
 #endif
 
 // ---- the host half of ggnn_set_graph_sparse: validation, tile plan, stable target-sorted CSR, streaming tables -> g->image.
-// `e` below is the prepared graph's shadow engine (model shape in, batch / plan fields out): nothing here touches the device except the
-// pinned allocation of the image and the wait for the previous upload out of the same image.
+// Nothing here touches the device except the pinned allocation of the image and the wait for the previous upload out of it.
 static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* const* adj, const int32_t* num_edges, const float* indeg) {
-    ggnn_engine* e = &g->plan;
+    const ModelShape& shape = g->shape;
+    BatchPlan& p = g->plan;
     g->valid = false;
     static const bool host_timing = getenv("GGNN_HOST_TIMING") != nullptr;
     const auto t_begin = std::chrono::steady_clock::now();
@@ -925,16 +947,14 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
         t = now;
     };
     auto t_lap = t_begin;
-    e->graph_set = false; e->saved_valid = false;
-    if (V < 0 || !adj || !num_edges || (!indeg && V > 0)) return e->fail(GGNN_EINVAL, "null/negative argument");
-    const int T = e->T;
+    if (V < 0 || !adj || !num_edges || (!indeg && V > 0)) return g->fail(GGNN_EINVAL, "null/negative argument");
+    const int T = shape.T;
     int64_t M = 0;
     for (int t = 0; t < T; ++t) {
-        if (num_edges[t] < 0 || (num_edges[t] > 0 && !adj[t])) return e->fail(GGNN_EINVAL, "adjacency list %d is null/negative", t);
+        if (num_edges[t] < 0 || (num_edges[t] > 0 && !adj[t])) return g->fail(GGNN_EINVAL, "adjacency list %d is null/negative", t);
         M += num_edges[t];
     }
-    if (M > 0x7fffffff || (int64_t)V * T + 1 > 0x7fffffff) return e->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
-    e->V = V; e->M = M; e->gather_mode = GATHER_SPARSE; e->dense_v = 0;
+    if (M > 0x7fffffff || (int64_t)V * T + 1 > 0x7fffffff) return g->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
 
     // ---- host threads.  Every pass below is split over `nth` threads by TARGET ranges (pass 1: equal node ranges; later passes: equal
     // tile ranges): each thread scans the whole edge list (sequential reads) and performs only the scattered writes of its own rows, in the
@@ -953,9 +973,9 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
 #endif
     // ---- pass 1: validate, count per (target,type), mark which node boundaries are spanned by an edge (the cut points of the tile-local
     // plans; the streaming plan of hidden sizes > 128 tiles by fixed 128-row blocks and skips that part)
-    std::vector<int>& counts = e->h_counts;
-    std::vector<int>& reach = e->h_diff;   // reach[j] = the farthest node an edge whose lower end is node j touches
-    const bool need_cuts = !(e->precision != GGNN_PREC_FP32 && e->DP > 128);
+    std::vector<int>& counts = g->h_counts;
+    std::vector<int>& reach = g->h_diff;   // reach[j] = the farthest node an edge whose lower end is node j touches
+    const bool need_cuts = !(shape.precision != GGNN_PREC_FP32 && shape.DP > 128);
     counts.resize((size_t)V * T + 1);
     if (need_cuts) reach.resize((size_t)V + 1);
     std::vector<int64_t> type_base(T + 1, 0);   // position of every type's first message in the reference's type-major message order
@@ -1025,25 +1045,18 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
             for (int i = 0; i < num_edges[t]; ++i) {
                 const int s = adj[t][2 * i], d = adj[t][2 * i + 1];
                 if ((unsigned)s >= (unsigned)V || (unsigned)d >= (unsigned)V)
-                    return e->fail(GGNN_ERANGE, "edge %d of type %d = (%d,%d) is out of range for %d nodes", i, t, s, d, V);
+                    return g->fail(GGNN_ERANGE, "edge %d of type %d = (%d,%d) is out of range for %d nodes", i, t, s, d, V);
             }
     }
     lap("  edges pass 1", t_lap);
     std::vector<int> cuts;
-    cuts.push_back(0);
-    if (need_cuts) {   // the boundary before node i is crossed by an edge iff max_{j < i} reach[j] >= i
-        int far = 0;
-        for (int i = 1; i < V; ++i) {
-            far = std::max(far, reach[i - 1]);
-            if (far < i) cuts.push_back(i);
-        }
-    }
-    if (V > 0) cuts.push_back(V);
+    find_cuts(need_cuts ? reach.data() : nullptr, V, cuts);
     lap("validate+count", t_lap);
     std::vector<int> tile_start;
-    int rc = build_plan(e, cuts, tile_start);
+    int rc = build_plan(shape, V, GATHER_SPARSE, cuts, p, tile_start, g->err);
     if (rc) return rc;
-    const int ntiles = e->ntiles;
+    p.M = M;
+    const int ntiles = p.ntiles;
     lap("tile plan", t_lap);
     nth = std::max(1, std::min(nth, ntiles));
     // tile ranges of the threads for all later passes: tiles [tb[k], tb[k+1]), i.e. nodes [tile_start[tb[k]], tile_start[tb[k+1]])
@@ -1057,7 +1070,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     for (int k = 0; k < nth; ++k) {
         int64_t sm = 0, nv = 0, nvm = 0;
         const size_t k0 = (size_t)tile_start[tb[k]] * T, k1 = (size_t)tile_start[tb[k + 1]] * T;
-        if (e->stream) {
+        if (p.stream) {
             for (size_t r = k0; r < k1; ++r) {
                 const int c = counts[r + 1];
                 sm += c;
@@ -1072,59 +1085,52 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
 
     // ---- layout of the packed upload
     size_t off = 0;
-    e->off_row_ptr = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
-    e->off_src = off;     off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
-    e->off_msg = off;     off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
-    e->off_indeg = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1) * T, 16);
-    e->off_denom = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
-    e->off_tiles = off;   off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
-    e->off_mask = off;    off = align_up(off + sizeof(unsigned) * (size_t)std::max(ntiles, 1), 16);
-    e->off_adj = off;
-    e->has_transpose = e->save;
-    if (e->has_transpose) {
-        e->off_trow = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
-        e->off_ttgt = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
-        e->off_tslot = off;
-        if (e->use_att) off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
+    p.off_row_ptr = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
+    p.off_src = off;     off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
+    p.off_msg = off;     off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
+    p.off_indeg = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1) * T, 16);
+    p.off_denom = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
+    p.off_tiles = off;   off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
+    p.off_mask = off;    off = align_up(off + sizeof(unsigned) * (size_t)std::max(ntiles, 1), 16);
+    p.off_adj = off;
+    p.has_transpose = g->save;
+    if (p.has_transpose) {
+        p.off_trow = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
+        p.off_ttgt = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
+        p.off_tslot = off;
+        if (shape.use_att) off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
     }
     // streaming plan: per (target, type) pair the ONE node to copy from (or none / a virtual row), see ggnn_fwd_stream.cuh
     const int nv = (int)part_nv[nth];
     const int64_t nvm = part_nvm[nth];
-    if (e->stream) {
-        e->off_pair = off; off = align_up(off + sizeof(int) * (size_t)std::max(ntiles, 1) * ts::TILE_M * T, 16);
-        e->off_vptr = off; off = align_up(off + sizeof(int) * (size_t)(nv + 1), 16);
-        e->off_vsrc = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(nvm, 1), 16);
-        e->off_tvp = off;  off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
-        e->off_vinfo = off; off = align_up(off + sizeof(int) * 8 * (size_t)std::max(nv, 1), 16);
+    if (p.stream) {
+        p.off_pair = off; off = align_up(off + sizeof(int) * (size_t)std::max(ntiles, 1) * ts::TILE_M * T, 16);
+        p.off_vptr = off; off = align_up(off + sizeof(int) * (size_t)(nv + 1), 16);
+        p.off_vsrc = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(nvm, 1), 16);
+        p.off_tvp = off;  off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
+        p.off_vinfo = off; off = align_up(off + sizeof(int) * 8 * (size_t)std::max(nv, 1), 16);
     }
-    if (e->model == MODEL_GCN) {   // per-slot adjacency weights, filled by build_gcn_image
-        e->off_slotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16);
-        if (e->has_transpose) { e->off_tslotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16); }
+    if (shape.model == MODEL_GCN) {   // per-slot adjacency weights, filled by build_gcn_image
+        p.off_slotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16);
+        if (p.has_transpose) { p.off_tslotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16); }
     }
-    e->ts_nv = nv;
-    for (int t = 0; t < T; ++t) e->edges_of_type[t] = num_edges[t];
-    if (g->use_cuda) {
-        if (g->uploaded) CU_TRY(e, cudaEventSynchronize(g->uploaded));   // the previous upload may still be reading this image
-        CU_TRY(e, g->stage.reserve(off));
-        g->image = (char*)g->stage.ptr;
-    } else {
-        if (g->plain.size() < off) g->plain.resize(off + off / 4 + 256);
-        g->image = g->plain.data();
-    }
+    p.ts_nv = nv;
+    for (int t = 0; t < T; ++t) p.edges_of_type[t] = num_edges[t];
+    CU_TRY(g, g->image.begin(off));
     g->bytes = off;
-    char* base = g->image;
-    int* row_ptr = (int*)(base + e->off_row_ptr);
-    int* csr_src = (int*)(base + e->off_src);
-    int* csr_msg = (int*)(base + e->off_msg);
-    float* h_indeg = (float*)(base + e->off_indeg);
-    float* h_denom = (float*)(base + e->off_denom);
-    int* h_tiles = (int*)(base + e->off_tiles);
-    unsigned* h_mask = (unsigned*)(base + e->off_mask);
-    int* pair = e->stream ? (int*)(base + e->off_pair) : nullptr;   // streaming plan: (target, type) -> its one source / virtual row
-    int* vptr = e->stream ? (int*)(base + e->off_vptr) : nullptr;
-    int* vsrc = e->stream ? (int*)(base + e->off_vsrc) : nullptr;
-    int* tvp = e->stream ? (int*)(base + e->off_tvp) : nullptr;
-    int* vinfo = e->stream ? (int*)(base + e->off_vinfo) : nullptr;
+    char* base = g->image.ptr;
+    int* row_ptr = (int*)(base + p.off_row_ptr);
+    int* csr_src = (int*)(base + p.off_src);
+    int* csr_msg = (int*)(base + p.off_msg);
+    float* h_indeg = (float*)(base + p.off_indeg);
+    float* h_denom = (float*)(base + p.off_denom);
+    int* h_tiles = (int*)(base + p.off_tiles);
+    unsigned* h_mask = (unsigned*)(base + p.off_mask);
+    int* pair = p.stream ? (int*)(base + p.off_pair) : nullptr;   // streaming plan: (target, type) -> its one source / virtual row
+    int* vptr = p.stream ? (int*)(base + p.off_vptr) : nullptr;
+    int* vsrc = p.stream ? (int*)(base + p.off_vsrc) : nullptr;
+    int* tvp = p.stream ? (int*)(base + p.off_tvp) : nullptr;
+    int* vinfo = p.stream ? (int*)(base + p.off_vinfo) : nullptr;
     lap("stage reserve", t_lap);
 
     // ---- pass 2, per thread over its tile range: exclusive scan of the (target, type) rows -> row_ptr, fill cursors, the tiles'
@@ -1132,7 +1138,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     // lists in the reference's order (type-major, then list order, sparse:124-129) and places the messages of ITS rows, so within a row
     // they stay in message order: this IS NumPy's stable argsort by target, tests pin it bit for bit; then (streaming plan) the gather
     // table and the virtual rows of its range, numbered from the range's offset; then in-degrees / denominators of its nodes.
-    std::vector<int>& cursor = e->h_cursor;   // next free slot of every (target, type) row (its own array: the counts of a range's last
+    std::vector<int>& cursor = g->h_cursor;   // next free slot of every (target, type) row (its own array: the counts of a range's last
     cursor.resize((size_t)V * T + 1);         // row are read by one thread while the next range's thread already writes cursors)
     int max_tile_msgs = 0;
     row_ptr[0] = 0;
@@ -1159,7 +1165,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
         }
         if (k == nth - 1) h_tiles[ntiles] = tile_start[ntiles];
     }
-    e->max_tile_msgs = max_tile_msgs;
+    p.max_tile_msgs = max_tile_msgs;
     lap("row sweep", t_lap);
 #ifdef _OPENMP
 #pragma omp parallel for schedule(static, 1) num_threads(nth) if (nth > 1)
@@ -1226,9 +1232,9 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
         if (pair) { for (size_t r = 0; r < (size_t)ts::TILE_M * T; ++r) pair[r] = -1; tvp[0] = 0; }
     }
     lap("csr fill", t_lap);
-    if (e->has_transpose) {   // messages keyed by (source, type): the scatter of the backward pass becomes a gather
-        int* trow = (int*)(base + e->off_trow);
-        int* ttgt = (int*)(base + e->off_ttgt);
+    if (p.has_transpose) {   // messages keyed by (source, type): the scatter of the backward pass becomes a gather
+        int* trow = (int*)(base + p.off_trow);
+        int* ttgt = (int*)(base + p.off_ttgt);
         std::vector<int> cnt((size_t)V * T + 1, 0);
         for (int t = 0; t < T; ++t)
             for (int i = 0; i < num_edges[t]; ++i) ++cnt[(size_t)adj[t][2 * i] * T + t + 1];
@@ -1236,7 +1242,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
         for (size_t k = 1; k <= (size_t)V * T; ++k) trow[k] = trow[k - 1] + cnt[k];
         for (size_t k = 0; k < (size_t)V * T; ++k) cnt[k] = trow[k];
         std::vector<int> slot_of_msg;
-        int* tslot = e->use_att ? (int*)(base + e->off_tslot) : nullptr;
+        int* tslot = shape.use_att ? (int*)(base + p.off_tslot) : nullptr;
         if (tslot) {
             slot_of_msg.resize((size_t)std::max<int64_t>(M, 1));
             for (int64_t k = 0; k < M; ++k) slot_of_msg[csr_msg[k]] = (int)k;
@@ -1254,60 +1260,66 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     return GGNN_OK;
 }
 
-// Model shape (what ggnn_create fixed) -> the shadow engine of a prepared graph.
-static void copy_model_shape(ggnn_engine* dst, const ggnn_engine* src) {
-    dst->model = src->model;
-    dst->D = src->D; dst->T = src->T; dst->L = src->L; dst->DP = src->DP;
-    memcpy(dst->steps, src->steps, sizeof dst->steps); memcpy(dst->nres, src->nres, sizeof dst->nres);
-    memcpy(dst->res, src->res, sizeof dst->res); memcpy(dst->step_base, src->step_base, sizeof dst->step_base);
-    dst->total_steps = src->total_steps;
-    dst->use_bias = src->use_bias; dst->use_avg = src->use_avg; dst->cell = src->cell; dst->act = src->act;
-    dst->precision = src->precision; dst->device = src->device; dst->num_sms = src->num_sms; dst->max_smem = src->max_smem;
-    dst->use_att = src->use_att;
-    dst->save = src->save;   // decides whether the source-keyed CSR of the backward pass is part of the image
-}
-
-// Batch / tile-plan fields (everything build_plan and build_sparse_image derive from a batch) -> the engine that uploads the image.
-static void adopt_plan(ggnn_engine* dst, const ggnn_engine* src) {
-    dst->V = src->V; dst->M = src->M; dst->gather_mode = src->gather_mode; dst->dense_v = src->dense_v;
-    dst->variant = src->variant; dst->nb1 = src->nb1; dst->local = src->local; dst->ntiles = src->ntiles;
-    dst->max_span = src->max_span; dst->max_tile_msgs = src->max_tile_msgs; dst->plan_text = src->plan_text;
-    dst->stream = src->stream;
-    for (int i = 0; i < 2; ++i) { dst->ts_nc[i] = src->ts_nc[i]; dst->ts_nblk[i] = src->ts_nblk[i]; }
-    dst->ts_nv = src->ts_nv; dst->tc_row_budget = src->tc_row_budget; dst->tc_kgs = src->tc_kgs;
-    dst->off_row_ptr = src->off_row_ptr; dst->off_src = src->off_src; dst->off_msg = src->off_msg; dst->off_indeg = src->off_indeg;
-    dst->off_denom = src->off_denom; dst->off_tiles = src->off_tiles; dst->off_mask = src->off_mask; dst->off_adj = src->off_adj;
-    dst->has_transpose = src->has_transpose; dst->off_trow = src->off_trow; dst->off_ttgt = src->off_ttgt; dst->off_tslot = src->off_tslot;
-    dst->off_pair = src->off_pair; dst->off_vptr = src->off_vptr; dst->off_vsrc = src->off_vsrc; dst->off_tvp = src->off_tvp;
-    dst->off_vinfo = src->off_vinfo;
-    dst->off_slotw = src->off_slotw; dst->off_tslotw = src->off_tslotw;
-    memcpy(dst->edges_of_type, src->edges_of_type, sizeof dst->edges_of_type);
-}
-
 int ggnn_free_prepared_graph(ggnn_prepared_graph* g) {
     if (!g) return GGNN_OK;
-    if (g->use_cuda) {
-        cudaSetDevice(g->plan.device);
-        if (g->uploaded) { cudaEventSynchronize(g->uploaded); cudaEventDestroy(g->uploaded); }
-        g->stage.release();
+    if (g->image.use_cuda) {
+        cudaSetDevice(g->shape.device);
+        g->image.release();
     }
     delete g;
     return GGNN_OK;
 }
 
-const char* ggnn_prepared_graph_error(const ggnn_prepared_graph* g) { return g ? g->plan.err.c_str() : "null prepared graph"; }
+const char* ggnn_prepared_graph_error(const ggnn_prepared_graph* g) { return g ? g->err.c_str() : "null prepared graph"; }
+
+}  // extern "C"
+
+// The prologue of the six prepare calls: reuse or allocate *inout and give it a model shape.  With an engine `e` (which must be a
+// `model` engine, the model of Config), the shape and -- for save_for_backward = -1 -- the save flag are the engine's, and the image
+// is pinned on its device; without one, the shape comes from `cfg` for a host of `num_sms` SMs with 227 KiB of shared memory each,
+// and the image is plain memory.
+template <class Config>
+static int begin_prepare(ggnn_prepared_graph** inout, const ggnn_engine* e, const Config* cfg, int32_t num_sms, int32_t save_for_backward,
+                         const char* fn) {
+    constexpr int model = std::is_same<Config, ggnn_gcn_config>::value ? MODEL_GCN : MODEL_GGNN;
+    if (!inout || (!e && (!cfg || num_sms <= 0))) return GGNN_EINVAL;
+    ggnn_prepared_graph* g = *inout;
+    if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
+    g->valid = false;
+    g->image.use_cuda = e != nullptr;
+    if (e) {
+        g->shape = *e;
+        if (e->model != model) return wrong_model(g, fn, e->model, model);
+        g->save = save_for_backward >= 0 ? save_for_backward != 0 : e->save;   // a producer thread says what the batch will be used for
+        if (cudaSetDevice(e->device) != cudaSuccess) return g->fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);   // this may be a producer thread
+        return GGNN_OK;
+    }
+    g->shape = ModelShape();
+    int rc;
+    if constexpr (model == MODEL_GCN) rc = init_gcn_shape(g->shape, cfg, g->err);
+    else rc = init_model_shape(g->shape, cfg, g->err);
+    if (rc) return rc;
+    g->shape.num_sms = num_sms; g->shape.max_smem = 227 * 1024;
+    g->save = save_for_backward != 0;
+    return GGNN_OK;
+}
+
+// The common body of the ggnn_set_graph_* calls: build(&e->own_prep) prepares the batch in the engine's own prepared graph (the same two
+// halves a caller can run on two threads), then the engine uploads it.
+template <class Build>
+static int set_graph_from_own_prep(ggnn_engine* e, ggnn_stream_t stream, Build build) {
+    e->graph_set = false; e->saved_valid = false;
+    int rc = build(&e->own_prep);
+    if (rc) { if (e->own_prep) e->err = e->own_prep->err; return rc; }
+    return ggnn_set_graph_prepared(e, e->own_prep, stream);
+}
+
+extern "C" {
 
 int ggnn_host_prepare_graph_sparse(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t V, const int32_t* const* adj,
                                    const int32_t* num_edges, const float* indeg, ggnn_prepared_graph** inout) {
-    if (!cfg || !inout || num_sms <= 0) return GGNN_EINVAL;
-    ggnn_prepared_graph* g = *inout;
-    if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
-    g->use_cuda = false;
-    g->valid = false;
-    if (int rc = init_model_shape(&g->plan, cfg, g->plan.err)) return rc;
-    g->plan.num_sms = num_sms; g->plan.max_smem = 227 * 1024;
-    g->plan.save = save_for_backward != 0;
-    return build_sparse_image(g, V, adj, num_edges, indeg);
+    if (int rc = begin_prepare(inout, nullptr, cfg, num_sms, save_for_backward, __func__)) return rc;
+    return build_sparse_image(*inout, V, adj, num_edges, indeg);
 }
 
 int ggnn_prepared_graph_info(const ggnn_prepared_graph* g, int32_t* num_nodes, int64_t* num_messages, int32_t* num_tiles, int64_t* image_bytes,
@@ -1325,9 +1337,9 @@ int ggnn_prepared_graph_info(const ggnn_prepared_graph* g, int32_t* num_nodes, i
 int ggnn_prepared_graph_arrays(const ggnn_prepared_graph* g, int32_t* row_ptr, int32_t* src, int32_t* msg, int32_t* tile_start, float* denom,
                                int32_t* pair_src) {
     if (!g || !g->valid) return GGNN_ESTATE;
-    const ggnn_engine& q = g->plan;
-    const char* base = g->image;
-    const size_t V = (size_t)q.V, T = (size_t)q.T, M = (size_t)q.M;
+    const BatchPlan& q = g->plan;
+    const char* base = g->image.ptr;
+    const size_t V = (size_t)q.V, T = (size_t)g->shape.T, M = (size_t)q.M;
     if (row_ptr) memcpy(row_ptr, base + q.off_row_ptr, sizeof(int) * (V * T + 1));
     if (src && M) memcpy(src, base + q.off_src, sizeof(int) * M);
     if (msg && M) memcpy(msg, base + q.off_msg, sizeof(int) * M);
@@ -1340,46 +1352,32 @@ int ggnn_prepared_graph_arrays(const ggnn_prepared_graph* g, int32_t* row_ptr, i
 int ggnn_prepared_graph_image(const ggnn_prepared_graph* g, void* dst, int64_t capacity) {
     if (!g || !g->valid || !dst) return GGNN_ESTATE;
     if (capacity < (int64_t)g->bytes) return GGNN_EINVAL;
-    memcpy(dst, g->image, g->bytes);
+    memcpy(dst, g->image.ptr, g->bytes);
     return GGNN_OK;
 }
 
 int ggnn_prepare_graph_sparse(const ggnn_engine* e, int32_t save_for_backward, int32_t V, const int32_t* const* adj, const int32_t* num_edges,
                               const float* indeg, ggnn_prepared_graph** inout) {
-    if (!e || !inout) return GGNN_EINVAL;
-    ggnn_prepared_graph* g = *inout;
-    if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
-    g->use_cuda = true;
-    copy_model_shape(&g->plan, e);
-    GGNN_REQUIRE_MODEL(&g->plan, MODEL_GGNN);
-    if (save_for_backward >= 0) g->plan.save = save_for_backward != 0;   // a producer thread says what the batch will be used for
-    if (cudaSetDevice(e->device) != cudaSuccess) return g->plan.fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);   // this may be a producer thread
-    return build_sparse_image(g, V, adj, num_edges, indeg);
+    if (int rc = begin_prepare<ggnn_config>(inout, e, nullptr, 0, save_for_backward, __func__)) return rc;
+    return build_sparse_image(*inout, V, adj, num_edges, indeg);
 }
 
 int ggnn_set_graph_prepared(ggnn_engine* e, ggnn_prepared_graph* g, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
     e->graph_set = false; e->saved_valid = false;
     if (!g || !g->valid) return e->fail(GGNN_ESTATE, "the prepared graph is empty (its build failed or never ran)");
-    const ggnn_engine& q = g->plan;
+    const ModelShape& q = g->shape;
     if (q.model != e->model)
         return e->fail(GGNN_ESTATE, "the prepared graph was built for a %s engine, this is a %s engine", q.model == MODEL_GCN ? "GCN" : "GGNN",
                        e->model == MODEL_GCN ? "GCN" : "GGNN");
     if (q.D != e->D || q.T != e->T || q.precision != e->precision || q.DP != e->DP || q.num_sms != e->num_sms || q.cell != e->cell || q.use_att != e->use_att)
         return e->fail(GGNN_EINVAL, "the prepared graph was built for a different engine configuration");
-    if (e->save && !q.has_transpose)
+    if (e->save && !g->plan.has_transpose)
         return e->fail(GGNN_ESTATE, "save_for_backward is on but the graph was prepared without it (the source-keyed CSR is built at prepare time)");
     CU_TRY(e, cudaSetDevice(e->device));
-    adopt_plan(e, &q);
-    cudaStream_t st = (cudaStream_t)stream;
+    static_cast<BatchPlan&>(*e) = g->plan;
     CU_TRY(e, e->graph_buf.reserve(g->bytes));
-    CU_TRY(e, cudaMemcpyAsync(e->graph_buf.ptr, g->image, g->bytes, cudaMemcpyHostToDevice, st));
-    if (g->use_cuda) {
-        if (!g->uploaded) CU_TRY(e, cudaEventCreateWithFlags(&g->uploaded, cudaEventDisableTiming));
-        CU_TRY(e, cudaEventRecord(g->uploaded, st));
-    } else {
-        CU_TRY(e, cudaStreamSynchronize(st));   // a pageable image (host-only construction) must be consumed before the caller may reuse it
-    }
+    CU_TRY(e, g->image.upload(e->graph_buf.ptr, g->bytes, (cudaStream_t)stream));
     int rc = reserve_states(e);
     if (rc) return rc;
     e->graph_set = true;
@@ -1390,11 +1388,7 @@ int ggnn_set_graph_sparse(ggnn_engine* e, int32_t V, const int32_t* const* adj, 
                           const float* indeg, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
     GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
-    e->graph_set = false; e->saved_valid = false;
-    // the same two halves a caller can run on two threads: build into the engine's own prepared graph, then upload it
-    int rc = ggnn_prepare_graph_sparse(e, -1, V, adj, num_edges, indeg, &e->own_prep);
-    if (rc) { if (e->own_prep) e->err = e->own_prep->plan.err; return rc; }
-    return ggnn_set_graph_prepared(e, e->own_prep, stream);
+    return set_graph_from_own_prep(e, stream, [&](ggnn_prepared_graph** g) { return ggnn_prepare_graph_sparse(e, -1, V, adj, num_edges, indeg, g); });
 }
 
 
@@ -1475,120 +1469,51 @@ static bool scan_binary_dense(int T, int b, int v, const float* adjm, std::vecto
     return binary;
 }
 
-// Host half of ggnn_set_graph_dense for a 0/1 adjacency: scan -> edge lists -> the sparse builder.  *not_binary tells a weighted matrix
-// (GGNN_EUNSUPPORTED) from a real failure.
-static int prepare_dense_into(ggnn_prepared_graph* g, int32_t b, int32_t v, const float* adjm, bool* not_binary) {
-    ggnn_engine* q = &g->plan;
-    g->valid = false;
-    *not_binary = false;
-    if (b < 0 || v <= 0 || (!adjm && b > 0)) return q->fail(GGNN_EINVAL, "null/negative argument");
-    if (q->use_att) return q->fail(GGNN_EUNSUPPORTED, "propagation attention exists only in the sparse model (sparse:170-196)");
-    const int T = q->T;
-    if ((int64_t)b * v > 0x7fffffff / std::max(T, 1)) return q->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
-    std::vector<std::vector<int32_t>> lists;
-    std::vector<float> indeg;
-    if (getenv("GGNN_DENSE_KEEP_MATRIX") || !scan_binary_dense(T, b, v, adjm, lists, indeg)) {
-        *not_binary = true;
-        return q->fail(GGNN_EUNSUPPORTED, "the adjacency matrix is not 0/1: a weighted matrix is fed through ggnn_set_graph_dense (matrix walk)");
-    }
-    std::vector<const int32_t*> ptrs(T);
-    std::vector<int32_t> counts(T);
-    for (int t = 0; t < T; ++t) { ptrs[t] = lists[t].data(); counts[t] = (int32_t)(lists[t].size() / 2); }
-    int rc = build_sparse_image(g, b * v, ptrs.data(), counts.data(), indeg.data());
-    if (rc) return rc;
-    q->dense_v = v;
-    q->plan_text += " [binary dense adjacency -> CSR]";
-    return GGNN_OK;
-}
-
-int ggnn_prepare_graph_dense(const ggnn_engine* e, int32_t save_for_backward, int32_t b, int32_t v, const float* adjm, ggnn_prepared_graph** inout) {
-    if (!e || !inout) return GGNN_EINVAL;
-    ggnn_prepared_graph* g = *inout;
-    if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
-    g->use_cuda = true;
-    copy_model_shape(&g->plan, e);
-    GGNN_REQUIRE_MODEL(&g->plan, MODEL_GGNN);
-    if (save_for_backward >= 0) g->plan.save = save_for_backward != 0;
-    if (cudaSetDevice(e->device) != cudaSuccess) return g->plan.fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);
-    bool not_binary = false;
-    return prepare_dense_into(g, b, v, adjm, &not_binary);
-}
-
-int ggnn_host_prepare_graph_dense(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t b, int32_t v, const float* adjm,
-                                  ggnn_prepared_graph** inout) {
-    if (!cfg || !inout || num_sms <= 0) return GGNN_EINVAL;
-    ggnn_prepared_graph* g = *inout;
-    if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
-    g->use_cuda = false;
-    g->valid = false;
-    if (int rc = init_model_shape(&g->plan, cfg, g->plan.err)) return rc;
-    g->plan.num_sms = num_sms; g->plan.max_smem = 227 * 1024;
-    g->plan.save = save_for_backward != 0;
-    bool not_binary = false;
-    return prepare_dense_into(g, b, v, adjm, &not_binary);
-}
-
-int ggnn_set_graph_dense(ggnn_engine* e, int32_t b, int32_t v, const float* adjm, ggnn_stream_t stream) {
-    if (!e) return GGNN_EINVAL;
-    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
-    e->graph_set = false; e->saved_valid = false;
-    if (b < 0 || v <= 0 || (!adjm && b > 0)) return e->fail(GGNN_EINVAL, "null/negative argument");
-    if (e->use_att) return e->fail(GGNN_EUNSUPPORTED, "propagation attention exists only in the sparse model (sparse:170-196)");
-    CU_TRY(e, cudaSetDevice(e->device));
-    const int T = e->T;
-    if ((int64_t)b * v > 0x7fffffff / std::max(T, 1)) return e->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
-    const int V = b * v;
-    {   // a 0/1 adjacency (all the reference feeds) takes the CSR path: the same two halves as ggnn_set_graph_sparse, on the engine's own prepared graph
-        if (!e->own_prep) e->own_prep = new ggnn_prepared_graph();
-        ggnn_prepared_graph* g = e->own_prep;
-        g->use_cuda = true;
-        copy_model_shape(&g->plan, e);
-        bool not_binary = false;
-        const int rc = prepare_dense_into(g, b, v, adjm, &not_binary);
-        if (rc == GGNN_OK) return ggnn_set_graph_prepared(e, g, stream);
-        if (!not_binary) { e->err = g->plan.err; return rc; }
-    }
-    e->V = V; e->M = 0; e->gather_mode = GATHER_DENSE; e->dense_v = v;
-    e->has_transpose = true;   // the dense adjacency is its own transpose source
-    for (int t = 0; t < T; ++t) e->edges_of_type[t] = 1;
+// Host half of ggnn_set_graph_dense for a weighted matrix (or any matrix under GGNN_DENSE_KEEP_MATRIX): the kernels walk the matrix
+// itself (GATHER_DENSE), so the image carries it along with the row-sum in-degrees, the denominators and the tiles.
+static int build_matrix_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const float* adjm) {
+    BatchPlan& p = g->plan;
+    const int T = g->shape.T, V = b * v;
     std::vector<int> cuts;
-    for (int g = 0; g <= b; ++g) cuts.push_back(g * v);
-    if (b == 0) cuts.assign(1, 0);
+    for (int i = 0; i <= b; ++i) cuts.push_back(i * v);
     std::vector<int> tile_start;
-    int rc = build_plan(e, cuts, tile_start);
+    int rc = build_plan(g->shape, V, GATHER_DENSE, cuts, p, tile_start, g->err);
     if (rc) return rc;
-    const int ntiles = e->ntiles;
+    p.dense_v = v;
+    p.has_transpose = true;   // the dense adjacency is its own transpose source
+    for (int t = 0; t < T; ++t) p.edges_of_type[t] = 1;
+    const int ntiles = p.ntiles;
     const size_t adj_elems = (size_t)b * T * v * v;
     size_t off = 0;
-    e->off_row_ptr = off; off = align_up(off + 16, 16);
-    e->off_src = off; e->off_msg = off;
-    e->off_indeg = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1) * T, 16);
-    e->off_denom = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
-    e->off_tiles = off;   off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
-    e->off_mask = off;    off = align_up(off + sizeof(unsigned) * (size_t)std::max(ntiles, 1), 16);
-    e->off_adj = off;     off = align_up(off + sizeof(float) * std::max<size_t>(adj_elems, 1), 16);
-    if (e->stage_done) CU_TRY(e, cudaEventSynchronize(e->stage_done));   // previous upload may still be reading the stage
-    CU_TRY(e, e->graph_stage.reserve(off));
-    char* base = (char*)e->graph_stage.ptr;
-    float* h_indeg = (float*)(base + e->off_indeg);
-    float* h_denom = (float*)(base + e->off_denom);
-    int* h_tiles = (int*)(base + e->off_tiles);
-    unsigned* h_mask = (unsigned*)(base + e->off_mask);
-    float* h_adj = (float*)(base + e->off_adj);
+    p.off_row_ptr = off; off = align_up(off + 16, 16);
+    p.off_src = off; p.off_msg = off;
+    p.off_indeg = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1) * T, 16);
+    p.off_denom = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
+    p.off_tiles = off;   off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
+    p.off_mask = off;    off = align_up(off + sizeof(unsigned) * (size_t)std::max(ntiles, 1), 16);
+    p.off_adj = off;     off = align_up(off + sizeof(float) * std::max<size_t>(adj_elems, 1), 16);
+    CU_TRY(g, g->image.begin(off));
+    g->bytes = off;
+    char* base = g->image.ptr;
+    float* h_indeg = (float*)(base + p.off_indeg);
+    float* h_denom = (float*)(base + p.off_denom);
+    int* h_tiles = (int*)(base + p.off_tiles);
+    unsigned* h_mask = (unsigned*)(base + p.off_mask);
+    float* h_adj = (float*)(base + p.off_adj);
     if (adj_elems) memcpy(h_adj, adjm, sizeof(float) * adj_elems);
     // in-degree per type = row sums of A_t (the dense model adds the bias to every source row before A.m,
     // dense:107-112, which equals bias * row-sum after the adjacency product)
-    for (int g = 0; g < b; ++g)
+    for (int gi = 0; gi < b; ++gi)
         for (int i = 0; i < v; ++i) {
             float tot = 0.0f;
             for (int t = 0; t < T; ++t) {
-                const float* row = adjm + (((size_t)g * T + t) * v + i) * v;
+                const float* row = adjm + (((size_t)gi * T + t) * v + i) * v;
                 float s = 0.0f;
                 for (int j = 0; j < v; ++j) s += row[j];
-                h_indeg[((size_t)g * v + i) * T + t] = s;
+                h_indeg[((size_t)gi * v + i) * T + t] = s;
                 tot += s;
             }
-            h_denom[(size_t)g * v + i] = tot + 1e-7f;
+            h_denom[(size_t)gi * v + i] = tot + 1e-7f;
         }
     for (int i = 0; i <= ntiles; ++i) h_tiles[i] = tile_start[i];
     for (int i = 0; i < ntiles; ++i) {
@@ -1599,22 +1524,62 @@ int ggnn_set_graph_dense(ggnn_engine* e, int32_t b, int32_t v, const float* adjm
         // rows with cancelling +/- entries would have zero row-sum but non-zero entries: scan those rows fully
         if (mask != ((T >= 32) ? 0xffffffffu : ((1u << T) - 1u))) {
             for (int n = tile_start[i]; n < tile_start[i + 1]; ++n) {
-                const int g = n / v, ii = n % v;
+                const int gi = n / v, ii = n % v;
                 for (int t = 0; t < T; ++t) {
                     if (mask & (1u << t)) continue;
-                    const float* row = adjm + (((size_t)g * T + t) * v + ii) * v;
+                    const float* row = adjm + (((size_t)gi * T + t) * v + ii) * v;
                     for (int j = 0; j < v; ++j) if (row[j] != 0.0f) { mask |= 1u << t; break; }
                 }
             }
         }
         h_mask[i] = mask;
     }
-    rc = upload_graph(e, off, (cudaStream_t)stream);
-    if (rc) return rc;
-    rc = reserve_states(e);
-    if (rc) return rc;
-    e->graph_set = true;
+    g->valid = true;
     return GGNN_OK;
+}
+
+// Host half of ggnn_set_graph_dense: a 0/1 adjacency is scanned to edge lists for the sparse builder; a weighted matrix (and any matrix
+// under GGNN_DENSE_KEEP_MATRIX) goes to the matrix builder when `matrix_ok`, else it is refused with GGNN_EUNSUPPORTED.
+static int build_dense_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const float* adjm, bool matrix_ok) {
+    g->valid = false;
+    if (b < 0 || v <= 0 || (!adjm && b > 0)) return g->fail(GGNN_EINVAL, "null/negative argument");
+    if (g->shape.use_att) return g->fail(GGNN_EUNSUPPORTED, "propagation attention exists only in the sparse model (sparse:170-196)");
+    const int T = g->shape.T;
+    if ((int64_t)b * v > 0x7fffffff / std::max(T, 1)) return g->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
+    std::vector<std::vector<int32_t>> lists;
+    std::vector<float> indeg;
+    if (getenv("GGNN_DENSE_KEEP_MATRIX") || !scan_binary_dense(T, b, v, adjm, lists, indeg)) {
+        if (matrix_ok) return build_matrix_image(g, b, v, adjm);
+        return g->fail(GGNN_EUNSUPPORTED, "the adjacency matrix is not 0/1: a weighted matrix is fed through ggnn_set_graph_dense (matrix walk)");
+    }
+    std::vector<const int32_t*> ptrs(T);
+    std::vector<int32_t> counts(T);
+    for (int t = 0; t < T; ++t) { ptrs[t] = lists[t].data(); counts[t] = (int32_t)(lists[t].size() / 2); }
+    int rc = build_sparse_image(g, b * v, ptrs.data(), counts.data(), indeg.data());
+    if (rc) return rc;
+    g->plan.dense_v = v;
+    g->plan.plan_text += " [binary dense adjacency -> CSR]";
+    return GGNN_OK;
+}
+
+int ggnn_prepare_graph_dense(const ggnn_engine* e, int32_t save_for_backward, int32_t b, int32_t v, const float* adjm, ggnn_prepared_graph** inout) {
+    if (int rc = begin_prepare<ggnn_config>(inout, e, nullptr, 0, save_for_backward, __func__)) return rc;
+    return build_dense_image(*inout, b, v, adjm, false);
+}
+
+int ggnn_host_prepare_graph_dense(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t b, int32_t v, const float* adjm,
+                                  ggnn_prepared_graph** inout) {
+    if (int rc = begin_prepare(inout, nullptr, cfg, num_sms, save_for_backward, __func__)) return rc;
+    return build_dense_image(*inout, b, v, adjm, false);
+}
+
+int ggnn_set_graph_dense(ggnn_engine* e, int32_t b, int32_t v, const float* adjm, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
+    return set_graph_from_own_prep(e, stream, [&](ggnn_prepared_graph** g) {
+        if (int rc = begin_prepare<ggnn_config>(g, e, nullptr, 0, -1, "ggnn_set_graph_dense")) return rc;
+        return build_dense_image(*g, b, v, adjm, true);
+    });
 }
 
 static void fill_params(ggnn_engine* e, FwdParams& p, const float* h0, float* h_out) {
@@ -1983,34 +1948,17 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
 }
 
 // ------------------------------------------------------------------------------------------ sparse GCN (chem_tensorflow_gcn.py:42-82)
-// The model shape of a ggnn_gcn_config: one edge type, one "timestep" per layer (the dropout's global step is the layer index).
-static int init_gcn_shape(ggnn_engine* e, const ggnn_gcn_config* cfg, std::string& err) {
-    if (cfg->hidden_size <= 0 || cfg->hidden_size % 4 != 0) { err = "hidden_size must be a positive multiple of 4"; return GGNN_EINVAL; }
-    if (cfg->hidden_size > 256) { err = "hidden_size > 256 is not supported by this build"; return GGNN_EUNSUPPORTED; }
-    if (cfg->num_layers <= 0 || cfg->num_layers > MAX_LAYERS) { err = "num_layers must be in 1..16"; return GGNN_EINVAL; }
-    if (cfg->precision != GGNN_PREC_FP32 && cfg->precision != GGNN_PREC_BF16X3 && cfg->precision != GGNN_PREC_BF16) { err = "unknown precision"; return GGNN_EINVAL; }
-    e->model = MODEL_GCN;
-    e->D = cfg->hidden_size; e->T = 1; e->L = cfg->num_layers;
-    e->use_bias = cfg->use_bias != 0; e->precision = cfg->precision; e->device = cfg->device;
-    e->cell = CELL_RNN; e->act = ACT_RELU;
-    for (int l = 0; l < e->L; ++l) { e->steps[l] = 1; e->step_base[l] = l; e->nres[l] = 0; }
-    e->total_steps = e->L;
-    e->DP = (e->D + 15) / 16 * 16;
-    return GGNN_OK;
-}
-
 // Host half of a GCN batch: validate the int64 (row i = output, column j = input) list, feed it to the GGNN builder as one edge type
 // (source j -> target i, list order kept), then add the per-slot weights in target-CSR and source-CSR order.
 static int build_gcn_image(ggnn_prepared_graph* g, int32_t V, int64_t nnz, const int64_t* list, const float* w) {
-    ggnn_engine* e = &g->plan;
     g->valid = false;
-    if (V < 0 || nnz < 0 || (nnz > 0 && (!list || !w))) return e->fail(GGNN_EINVAL, "null/negative argument");
-    if (nnz > 0x7fffffff) return e->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
+    if (V < 0 || nnz < 0 || (nnz > 0 && (!list || !w))) return g->fail(GGNN_EINVAL, "null/negative argument");
+    if (nnz > 0x7fffffff) return g->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
     std::vector<int32_t> pairs((size_t)nnz * 2);
     for (int64_t k = 0; k < nnz; ++k) {
         const int64_t i = list[2 * k], j = list[2 * k + 1];
         if (i < 0 || i >= V || j < 0 || j >= V)
-            return e->fail(GGNN_ERANGE, "adjacency_list[%lld] = (%lld, %lld) is out of range for %d nodes", (long long)k, (long long)i, (long long)j, V);
+            return g->fail(GGNN_ERANGE, "adjacency_list[%lld] = (%lld, %lld) is out of range for %d nodes", (long long)k, (long long)i, (long long)j, V);
         pairs[2 * k] = (int32_t)j;
         pairs[2 * k + 1] = (int32_t)i;
     }
@@ -2019,13 +1967,14 @@ static int build_gcn_image(ggnn_prepared_graph* g, int32_t V, int64_t nnz, const
     const int32_t counts[1] = {(int32_t)nnz};
     int rc = build_sparse_image(g, V, lists, counts, indeg.data());
     if (rc) return rc;
-    char* base = g->image;
-    const int* csr_msg = (const int*)(base + e->off_msg);
-    float* tw = (float*)(base + e->off_slotw);
+    const BatchPlan& p = g->plan;
+    char* base = g->image.ptr;
+    const int* csr_msg = (const int*)(base + p.off_msg);
+    float* tw = (float*)(base + p.off_slotw);
     for (int64_t k = 0; k < nnz; ++k) tw[k] = w[csr_msg[k]];
-    if (e->has_transpose) {   // the source-keyed CSR lists the entries of every input column j in list order (build_sparse_image)
-        const int* trow = (const int*)(base + e->off_trow);
-        float* sw = (float*)(base + e->off_tslotw);
+    if (p.has_transpose) {   // the source-keyed CSR lists the entries of every input column j in list order (build_sparse_image)
+        const int* trow = (const int*)(base + p.off_trow);
+        float* sw = (float*)(base + p.off_tslotw);
         std::vector<int> cur(trow, trow + V);
         for (int64_t k = 0; k < nnz; ++k) sw[cur[pairs[2 * k]]++] = w[k];
     }
@@ -2036,7 +1985,7 @@ int ggnn_gcn_create(const ggnn_gcn_config* cfg, ggnn_engine** out) {
     if (!cfg || !out) { g_create_error = "null argument"; return GGNN_EINVAL; }
     *out = nullptr;
     ggnn_engine* e = new ggnn_engine();
-    if (int rc = init_gcn_shape(e, cfg, g_create_error)) { delete e; return rc; }
+    if (int rc = init_gcn_shape(*e, cfg, g_create_error)) { delete e; return rc; }
     return attach_device(e, out);
 }
 
@@ -2058,45 +2007,28 @@ int ggnn_gcn_set_weights(ggnn_engine* e, const ggnn_gcn_layer_weights* layers, i
 
 int ggnn_prepare_graph_gcn(const ggnn_engine* e, int32_t save_for_backward, int32_t V, int64_t nnz, const int64_t* list, const float* w,
                            ggnn_prepared_graph** inout) {
-    if (!e || !inout) return GGNN_EINVAL;
-    ggnn_prepared_graph* g = *inout;
-    if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
-    g->use_cuda = true;
-    copy_model_shape(&g->plan, e);
-    GGNN_REQUIRE_MODEL(&g->plan, MODEL_GCN);
-    if (save_for_backward >= 0) g->plan.save = save_for_backward != 0;
-    if (cudaSetDevice(e->device) != cudaSuccess) return g->plan.fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);
-    return build_gcn_image(g, V, nnz, list, w);
+    if (int rc = begin_prepare<ggnn_gcn_config>(inout, e, nullptr, 0, save_for_backward, __func__)) return rc;
+    return build_gcn_image(*inout, V, nnz, list, w);
 }
 
 int ggnn_host_prepare_graph_gcn(const ggnn_gcn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t V, int64_t nnz,
                                 const int64_t* list, const float* w, ggnn_prepared_graph** inout) {
-    if (!cfg || !inout || num_sms <= 0) return GGNN_EINVAL;
-    ggnn_prepared_graph* g = *inout;
-    if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
-    g->use_cuda = false;
-    g->valid = false;
-    if (int rc = init_gcn_shape(&g->plan, cfg, g->plan.err)) return rc;
-    g->plan.num_sms = num_sms; g->plan.max_smem = 227 * 1024;
-    g->plan.save = save_for_backward != 0;
-    return build_gcn_image(g, V, nnz, list, w);
+    if (int rc = begin_prepare(inout, nullptr, cfg, num_sms, save_for_backward, __func__)) return rc;
+    return build_gcn_image(*inout, V, nnz, list, w);
 }
 
 int ggnn_set_graph_gcn(ggnn_engine* e, int32_t V, int64_t nnz, const int64_t* list, const float* w, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
     GGNN_REQUIRE_MODEL(e, MODEL_GCN);
-    e->graph_set = false; e->saved_valid = false;
-    int rc = ggnn_prepare_graph_gcn(e, -1, V, nnz, list, w, &e->own_prep);
-    if (rc) { if (e->own_prep) e->err = e->own_prep->plan.err; return rc; }
-    return ggnn_set_graph_prepared(e, e->own_prep, stream);
+    return set_graph_from_own_prep(e, stream, [&](ggnn_prepared_graph** g) { return ggnn_prepare_graph_gcn(e, -1, V, nnz, list, w, g); });
 }
 
 int ggnn_prepared_graph_slot_weights(const ggnn_prepared_graph* g, float* target_csr_w, float* source_csr_w) {
-    if (!g || !g->valid || g->plan.model != MODEL_GCN) return GGNN_ESTATE;
-    const ggnn_engine& q = g->plan;
+    if (!g || !g->valid || g->shape.model != MODEL_GCN) return GGNN_ESTATE;
+    const BatchPlan& q = g->plan;
     if (source_csr_w && !q.has_transpose) return GGNN_ESTATE;
-    if (target_csr_w && q.M) memcpy(target_csr_w, g->image + q.off_slotw, sizeof(float) * (size_t)q.M);
-    if (source_csr_w && q.M) memcpy(source_csr_w, g->image + q.off_tslotw, sizeof(float) * (size_t)q.M);
+    if (target_csr_w && q.M) memcpy(target_csr_w, g->image.ptr + q.off_slotw, sizeof(float) * (size_t)q.M);
+    if (source_csr_w && q.M) memcpy(source_csr_w, g->image.ptr + q.off_tslotw, sizeof(float) * (size_t)q.M);
     return GGNN_OK;
 }
 
@@ -2392,10 +2324,9 @@ int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* gr
     e->ro_off_mask = off;     off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
     e->ro_off_val = off;      // device-only scratch: per-node gated value
     const size_t dev_bytes = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
-    if (e->ro_stage_done) CU_TRY(e, cudaEventSynchronize(e->ro_stage_done));
-    CU_TRY(e, e->ro_stage.reserve(off));
+    CU_TRY(e, e->ro_stage.begin(off));
     CU_TRY(e, e->ro_buf.reserve(dev_bytes));
-    char* base = (char*)e->ro_stage.ptr;
+    char* base = e->ro_stage.ptr;
     int* graph_of = (int*)(base + e->ro_off_graph_of);
     int* start = (int*)(base + e->ro_off_start);
     bool grouped = true;
@@ -2413,10 +2344,7 @@ int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* gr
         }
     }
     if (node_mask) memcpy(base + e->ro_off_mask, node_mask, sizeof(float) * (size_t)V);
-    cudaStream_t st = (cudaStream_t)stream;
-    CU_TRY(e, cudaMemcpyAsync(e->ro_buf.ptr, base, off, cudaMemcpyHostToDevice, st));
-    if (!e->ro_stage_done) CU_TRY(e, cudaEventCreateWithFlags(&e->ro_stage_done, cudaEventDisableTiming));
-    CU_TRY(e, cudaEventRecord(e->ro_stage_done, st));
+    CU_TRY(e, e->ro_stage.upload(e->ro_buf.ptr, off, (cudaStream_t)stream));
     e->ro_V = V; e->ro_G = G; e->ro_grouped = grouped; e->ro_has_mask = node_mask != nullptr;
     return GGNN_OK;
 }

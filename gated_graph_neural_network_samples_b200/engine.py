@@ -113,15 +113,8 @@ class PreparedGraph:
         indeg = np.ascontiguousarray(np.asarray(num_incoming_edges_per_type, dtype=np.float32))
         ptrs = (C.c_void_p * T)(*[a.ctypes.data for a in adjs])
         counts = (C.c_int32 * T)(*[a.shape[0] for a in adjs])
-        h = C.c_void_p(g._h.value)
-        rc = g.lib.ggnn_host_prepare_graph_sparse(C.byref(cfg), int(num_sms), int(bool(save_for_backward)), indeg.shape[0], ptrs, counts,
-                                                  indeg.ctypes.data, C.byref(h))
-        g._h = h
-        if rc != 0:
-            raise GgnnError(g.lib.ggnn_prepared_graph_error(g._h).decode())
-        g.V = indeg.shape[0]
-        g.T = T
-        return g
+        return g._fill(g.lib.ggnn_host_prepare_graph_sparse, indeg.shape[0], T, C.byref(cfg), int(num_sms), int(bool(save_for_backward)),
+                       indeg.shape[0], ptrs, counts, indeg.ctypes.data)
 
     @classmethod
     def host_only_dense(cls, params: dict, num_edge_types: int, adjacency_matrix, precision: str = "fp32", num_sms: int = 132,
@@ -130,15 +123,8 @@ class PreparedGraph:
         g = reuse if reuse is not None else cls()
         cfg, keep = make_config(params, num_edge_types, 0, precision)
         a = np.ascontiguousarray(np.asarray(adjacency_matrix, dtype=np.float32))
-        h = C.c_void_p(g._h.value)
-        rc = g.lib.ggnn_host_prepare_graph_dense(C.byref(cfg), int(num_sms), int(bool(save_for_backward)), a.shape[0], a.shape[2], a.ctypes.data,
-                                                 C.byref(h))
-        g._h = h
-        if rc != 0:
-            raise GgnnError(g.lib.ggnn_prepared_graph_error(g._h).decode())
-        g.V = a.shape[0] * a.shape[2]
-        g.T = int(num_edge_types)
-        return g
+        return g._fill(g.lib.ggnn_host_prepare_graph_dense, a.shape[0] * a.shape[2], int(num_edge_types), C.byref(cfg), int(num_sms),
+                       int(bool(save_for_backward)), a.shape[0], a.shape[2], a.ctypes.data)
 
     @classmethod
     def host_only_gcn(cls, hidden_size: int, num_layers: int, num_nodes: int, adjacency_list, adjacency_weights, use_bias: bool = False,
@@ -149,15 +135,18 @@ class PreparedGraph:
         g = reuse if reuse is not None else cls()
         cfg = _lib.GcnConfig(int(hidden_size), int(num_layers), int(bool(use_bias)), PRECISIONS[precision], 0)
         lst, w = _gcn_arrays(adjacency_list, adjacency_weights)
-        h = C.c_void_p(g._h.value)
-        rc = g.lib.ggnn_host_prepare_graph_gcn(C.byref(cfg), int(num_sms), int(bool(save_for_backward)), int(num_nodes), lst.shape[0],
-                                               lst.ctypes.data, w.ctypes.data, C.byref(h))
-        g._h = h
+        return g._fill(g.lib.ggnn_host_prepare_graph_gcn, int(num_nodes), 1, C.byref(cfg), int(num_sms), int(bool(save_for_backward)),
+                       int(num_nodes), lst.shape[0], lst.ctypes.data, w.ctypes.data)
+
+    def _fill(self, prepare, V: int, T: int, *args) -> "PreparedGraph":
+        """Runs the C prepare call ``prepare(*args, &handle)`` into this handle (the call allocates it when empty)."""
+        h = C.c_void_p(self._h.value)
+        rc = prepare(*args, C.byref(h))
+        self._h = h
         if rc != 0:
-            raise GgnnError(g.lib.ggnn_prepared_graph_error(g._h).decode())
-        g.V = int(num_nodes)
-        g.T = 1
-        return g
+            raise GgnnError(self.lib.ggnn_prepared_graph_error(self._h).decode())
+        self.V, self.T = V, T
+        return self
 
     def slot_weights(self, source_order: bool = False) -> np.ndarray:
         """A GCN graph's per-slot adjacency weights in target-CSR order (``source_order``: in source-CSR order, backward graphs only)."""
@@ -302,14 +291,8 @@ class PropagationEngine:
         call waits for its previous upload first)."""
         adjs, indeg, ptrs, counts = marshalled if marshalled is not None else self._sparse_args(adjacency_lists, num_incoming_edges_per_type)
         g = reuse if reuse is not None else PreparedGraph(self.lib)
-        h = C.c_void_p(g._h.value)
-        rc = self.lib.ggnn_prepare_graph_sparse(self._h, -1 if save_for_backward is None else int(bool(save_for_backward)), indeg.shape[0], ptrs,
-                                                counts, indeg.ctypes.data, C.byref(h))
-        g._h = h
-        if rc != 0:
-            raise GgnnError(self.lib.ggnn_prepared_graph_error(g._h).decode())
-        g.V = indeg.shape[0]
-        return g
+        return g._fill(self.lib.ggnn_prepare_graph_sparse, indeg.shape[0], self.T, self._h,
+                       -1 if save_for_backward is None else int(bool(save_for_backward)), indeg.shape[0], ptrs, counts, indeg.ctypes.data)
 
     def prepare_graph_dense(self, adjacency_matrix, save_for_backward: Optional[bool] = None,
                             reuse: Optional["PreparedGraph"] = None) -> "PreparedGraph":
@@ -319,14 +302,8 @@ class PropagationEngine:
         if a.ndim != 4 or a.shape[1] != self.T or a.shape[2] != a.shape[3]:
             raise GgnnError("adjacency_matrix must be [b, %d, v, v]" % self.T)
         g = reuse if reuse is not None else PreparedGraph(self.lib)
-        h = C.c_void_p(g._h.value)
-        rc = self.lib.ggnn_prepare_graph_dense(self._h, -1 if save_for_backward is None else int(bool(save_for_backward)), a.shape[0], a.shape[2],
-                                               a.ctypes.data, C.byref(h))
-        g._h = h
-        if rc != 0:
-            raise GgnnError(self.lib.ggnn_prepared_graph_error(g._h).decode())
-        g.V = a.shape[0] * a.shape[2]
-        return g
+        return g._fill(self.lib.ggnn_prepare_graph_dense, a.shape[0] * a.shape[2], self.T, self._h,
+                       -1 if save_for_backward is None else int(bool(save_for_backward)), a.shape[0], a.shape[2], a.ctypes.data)
 
     def set_graph_prepared(self, g: "PreparedGraph"):
         """The DEVICE half: adopt the plan, enqueue the one H2D copy of the image.  Keep ``g`` alive until the stream has passed it."""
@@ -576,15 +553,8 @@ class GCNEngine(PropagationEngine):
         """The HOST half of ``set_graph_gcn`` (may run in a producer thread); adopt the result with ``set_graph_prepared``."""
         lst, w = _gcn_arrays(adjacency_list, adjacency_weights)
         g = reuse if reuse is not None else PreparedGraph(self.lib)
-        h = C.c_void_p(g._h.value)
-        rc = self.lib.ggnn_prepare_graph_gcn(self._h, -1 if save_for_backward is None else int(bool(save_for_backward)), int(num_nodes),
-                                             lst.shape[0], lst.ctypes.data, w.ctypes.data, C.byref(h))
-        g._h = h
-        if rc != 0:
-            raise GgnnError(self.lib.ggnn_prepared_graph_error(g._h).decode())
-        g.V = int(num_nodes)
-        g.T = 1
-        return g
+        return g._fill(self.lib.ggnn_prepare_graph_gcn, int(num_nodes), 1, self._h, -1 if save_for_backward is None else int(bool(save_for_backward)),
+                       int(num_nodes), lst.shape[0], lst.ctypes.data, w.ctypes.data)
 
     def backward(self, d_out, grads: Sequence[dict], d_h0=None):
         """``grads[l]``: dict with optional ``kernel`` [D, D] / ``bias`` [D] fp32 CUDA tensors, accumulated into."""
