@@ -89,8 +89,6 @@ SYMBOLS = {
     "ggnn_host_target_csr": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(C.c_void_p), c_i32p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ggnn_host_stream_tables": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(C.c_void_p), c_i32p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
                                           C.c_void_p, C.POINTER(C.c_int32)]),
-    "ggnn_debug_trace": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
-    "ggnn_debug_timestamps": (C.c_int, [C.c_void_p, C.c_void_p]),
     "ggnn_plan_description": (C.c_char_p, [C.c_void_p]),
     "ggnn_gcn_create": (C.c_int, [C.POINTER(GcnConfig), C.POINTER(C.c_void_p)]),
     "ggnn_gcn_set_weights": (C.c_int, [C.c_void_p, C.POINTER(GcnLayerWeights), C.c_int32]),

@@ -185,7 +185,6 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     DevBuf tc_weights;  // pre-split, pre-tiled bf16 copies of the weights (tensor-core path)
     DevBuf tc_respre;   // residual pre-products [ntiles][128][3*DP]
     DevBuf err_flag;    // device int written by kernels on a barrier timeout
-    DevBuf dbg_buf;     // optional phase timestamps of the streaming kernels (GGNN_TS_DEBUG=1)
     bool weights_dirty = true;
     size_t tc_off_edge[MAX_LAYERS] = {0}, tc_off_gate[MAX_LAYERS] = {0}, tc_off_cand[MAX_LAYERS] = {0};
     const float* last_h0 = nullptr;
@@ -370,17 +369,12 @@ int build_plan(const ModelShape& s, int V, int gather_mode, const std::vector<in
             p.variant = 2;
             p.local = max_span <= tc::TILE_M && !force_global;
             int budget = tc::TILE_M;
-            if (p.local) {
-                const char* tr = getenv("GGNN_TC_TILE_ROWS");
-                if (tr && atoi(tr) >= max_span && atoi(tr) <= tc::TILE_M) { budget = atoi(tr); pack_components(cuts, V, budget, tile_start); }
-                else budget = pack_to_fill_chip(cuts, V, max_span, s.num_sms, tile_start);
-            } else {
-                fixed_tiles(V, tc::TILE_M, tile_start);
-            }
+            if (p.local) budget = pack_to_fill_chip(cuts, V, max_span, s.num_sms, tile_start);
+            else fixed_tiles(V, tc::TILE_M, tile_start);
             p.ntiles = (int)tile_start.size() - 1;
             p.tc_row_budget = budget;
             // compact operand tiles when no tile exceeds 64 rows (k-group stride 1024 instead of 2048): half the operand bytes, a ~3x deeper ring
-            p.tc_kgs = (p.tc_row_budget <= 64 && !getenv("GGNN_TC_NO_COMPACT")) ? 1024 : 2048;
+            p.tc_kgs = p.tc_row_budget <= 64 ? 1024 : 2048;
             snprintf(buf, sizeof buf, "wgmma-%s %s tiles=%d rows/tile<=%d%s DP=%d max_component=%d", prec,
                      p.local ? "LOCAL(all layers+steps fused, 1 launch)" : "GLOBAL(1 launch per step)", p.ntiles, budget,
                      p.tc_kgs == 1024 ? " (compact 64-row operand tiles)" : "", s.DP, max_span);
@@ -740,7 +734,7 @@ int ggnn_destroy(ggnn_engine* e) {
     if (!e) return GGNN_OK;
     cudaSetDevice(e->device);
     e->graph_buf.release(); e->state_buf.release(); e->save_bufs.release(); e->io_buf.release(); e->bwd_buf.release();
-    e->tc_weights.release(); e->tc_respre.release(); e->ts_weights.release(); e->ts_images.release(); e->ts_u.release(); e->ts_virt.release(); e->err_flag.release(); e->dbg_buf.release();
+    e->tc_weights.release(); e->tc_respre.release(); e->ts_weights.release(); e->ts_images.release(); e->ts_u.release(); e->ts_virt.release(); e->err_flag.release();
     if (e->own_prep) { ggnn_free_prepared_graph(e->own_prep); e->own_prep = nullptr; }
     e->ro_buf.release(); e->ro_stage.release(); e->att_buf.release();
     delete e;
@@ -1684,7 +1678,6 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
     if (avail < 3 * opb + bias_b + stage) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the tensor-core tile (DP=%d)", DP);
     const size_t ops = 3 * opb;   // h, agg and the gather / r*h operand tiles
     p.nstages = (int)std::min<size_t>(tc::MAX_STAGES, (avail - ops - bias_b) / stage);
-    if (const char* ns = getenv("GGNN_TC_STAGES")) p.nstages = std::max(1, std::min(p.nstages, atoi(ns)));
     if (p.nstages < 1) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the weight ring (DP=%d)", DP);
     const size_t smem = ops + bias_b + (size_t)p.nstages * stage;
     char* g = (char*)e->graph_buf.ptr;
@@ -1828,7 +1821,8 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     if (env_ks) KS = atoi(env_ks) >= 4 ? 4 : (atoi(env_ks) >= 2 ? 2 : 1);
     while (NKS % KS) KS /= 2;
     auto stage_bytes = [&](int NC) { return (size_t)KS * ((size_t)ts::A_STAGE_B + 64 * (size_t)NC); };
-    auto stages_for = [&](int NC, size_t budget) { return (int)std::min<size_t>(env_ns ? (size_t)atoi(env_ns) : (size_t)ts::MAX_NS, budget / stage_bytes(NC)); };
+    const int max_ns = env_ns ? std::max(0, std::min(atoi(env_ns), ts::MAX_NS)) : ts::MAX_NS;   // the kernel has MAX_NS stage barriers
+    auto stages_for = [&](int NC, size_t budget) { return (int)std::min<size_t>((size_t)max_ns, budget / stage_bytes(NC)); };
     ts::StreamParams base;
     memset(&base, 0, sizeof base);
     base.V = V; base.D = D; base.DP = DP; base.T = T;
@@ -1838,44 +1832,27 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     base.pair_src = (const int*)(g + e->off_pair); base.vrow_ptr = (const int*)(g + e->off_vptr);
     base.vsrc = (const int*)(g + e->off_vsrc); base.tile_vptr = (const int*)(g + e->off_tvp);
     base.vinfo = (const int4*)(g + e->off_vinfo);
-    base.virt_img = (uint8_t*)e->ts_virt.ptr;
-    // pairs with several messages are pre-summed into virtual rows by the prologue of every gather launch (GGNN_TS_VIRT=0: summed inside
-    // the gather loop instead)
-    base.virt_rows = 1;
-    if (const char* vr = getenv("GGNN_TS_VIRT")) base.virt_rows = vr[0] == '1';
+    base.virt_img = (uint8_t*)e->ts_virt.ptr;   // pairs with several messages, pre-summed by the prologue of every gather launch
     base.indeg = (const float*)(g + e->off_indeg); base.denom = (const float*)(g + e->off_denom);
     base.drop_keep = e->drop_keep; base.drop_seed = e->drop_seed;
     base.error_flag = (int*)e->err_flag.ptr;
-    // optional per-CTA phase stamps, one slice per launch (read back with ggnn_debug_trace)
-    long long* dbg = nullptr;
-    const size_t dbg_slice = (size_t)ntiles * std::max(e->ts_nblk[0], e->ts_nblk[1]) * 16;
-    if (getenv("GGNN_TS_DEBUG")) {
-        const size_t n = (dbg_slice + 2048) * (size_t)(3 * std::max(e->total_steps, 1));
-        CU_TRY(e, e->dbg_buf.reserve(n * sizeof(long long)));
-        CU_TRY(e, cudaMemsetAsync(e->dbg_buf.ptr, 0, n * sizeof(long long), st));
-        dbg = (long long*)e->dbg_buf.ptr;
-    }
-    int dbg_launch = 0;
-    long long* dbg2_cur = nullptr;   // per launch: [grid][16] phase stamps, then [256][8] K-step timeline of CTA (0,0)
-    auto next_dbg = [&]() -> long long* {
-        if (!dbg) return nullptr;
-        long long* q = dbg + (dbg_slice + 2048) * (size_t)(dbg_launch++);
-        dbg2_cur = q + dbg_slice;
-        return q;
-    };
     const int nc0 = e->ts_nc[0], nb0 = e->ts_nblk[0], nc1 = e->ts_nc[1], nb1 = e->ts_nblk[1];
     // one CTA per SM for all three kernels: the whole shared memory is the ring
     const int ns_edge = stages_for(nc0, avail > csr_b ? avail - csr_b : 0);
     const int ns_gate = stages_for(nc1, avail), ns_cand = stages_for(nc0, avail);
-    if (ns_edge < 2 || ns_gate < 2 || ns_cand < 2) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the streaming ring (DP=%d)", DP);
+    // the kernel's parity waits are only sound if every ring has at least as many stages as there are gather groups (ts::MIN_NS)
+    const int ns_min = std::min({ns_edge, ns_gate, ns_cand});
+    if (ns_min < ts::MIN_NS)
+        return e->fail(GGNN_EUNSUPPORTED, "streaming ring of %d stages (DP=%d): it needs at least %d, one per gather group", ns_min, DP,
+                       ts::MIN_NS);
     auto smem_of = [&](int NC, int ns, bool gather) { return (size_t)1024 + ts::ring_bytes(ns, stage_bytes(NC)) + (gather ? csr_b : 0); };
     const bool x3 = e->precision == GGNN_PREC_BF16X3;
     void (*k_edge)(ts::StreamParams) = nullptr;
     void (*k_fed)(ts::StreamParams) = nullptr;
-#define GGNN_TS_PICK(X, K)                                                         \
-    if (x3 == X && KS == K) {                                                      \
-        k_edge = ts::ggnn_stream_kernel<ts::NWORK_DEFAULT, true, X, K>;            \
-        k_fed = ts::ggnn_stream_kernel<ts::NWORK_DEFAULT, false, X, K>;            \
+#define GGNN_TS_PICK(X, K)                              \
+    if (x3 == X && KS == K) {                           \
+        k_edge = ts::ggnn_stream_kernel<true, X, K>;    \
+        k_fed = ts::ggnn_stream_kernel<false, X, K>;    \
     }
     GGNN_TS_PICK(true, 4) GGNN_TS_PICK(true, 2) GGNN_TS_PICK(true, 1) GGNN_TS_PICK(false, 4) GGNN_TS_PICK(false, 2) GGNN_TS_PICK(false, 1)
 #undef GGNN_TS_PICK
@@ -1912,7 +1889,7 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
             p.epi = ts::EPI_AGG; p.NC = nc0; p.nstages = ns_edge;
             p.g_img = img_in; p.w = wb + e->ts_off_edge[l]; p.kt_all = T * NKS;
             p.bias = e->use_bias ? e->w[l].edge_biases : nullptr;
-            p.img_out = img_agg; p.sv_agg = e->save ? sv + per + so : nullptr; p.gstep = gs; p.dbg = next_dbg(); p.dbg2 = dbg2_cur;
+            p.img_out = img_agg; p.sv_agg = e->save ? sv + per + so : nullptr; p.gstep = gs;
             k_edge<<<dim3(ntiles, nb0), ts::NTHREADS, sm_edge, st>>>(p);
             ++e->last_launches;
             auto set_segs = [&](ts::StreamParams& q, const uint8_t* last_img) {
@@ -1927,7 +1904,7 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
                 set_segs(q, img_in);
                 q.w = wb + e->ts_off_gate[l]; q.bias = e->w[l].gate_bias; q.h_chk = chk_in; q.u_buf = u_chk; q.img_out = img_rh;
                 if (e->save) { q.sv_r = sv + 2 * per + so; q.sv_h = sv + so; q.sv_u = sv + 3 * per + so; }
-                q.gstep = gs; q.dbg = next_dbg(); q.dbg2 = dbg2_cur;
+                q.gstep = gs;
                 k_fed<<<dim3(ntiles, nb1), ts::NTHREADS, smem_of(nc1, ns_gate, false), st>>>(q);
                 ++e->last_launches;
             }
@@ -1936,7 +1913,7 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
             set_segs(c, gru ? img_rh : img_in);
             c.w = wb + e->ts_off_cand[l]; c.bias = e->w[l].cand_bias; c.h_chk = chk_in; c.u_buf = u_chk; c.h_chk_out = chk_out; c.h_out = out; c.img_out = img_out;
             if (e->save) { if (gru) c.sv_c = sv + 4 * per + so; else c.sv_h = sv + so; }
-            c.gstep = gs; c.dbg = next_dbg(); c.dbg2 = dbg2_cur;
+            c.gstep = gs;
             k_fed<<<dim3(ntiles, nb0), ts::NTHREADS, smem_of(nc0, ns_cand, false), st>>>(c);
             ++e->last_launches;
             img_in = img_out; chk_in = chk_out;
@@ -2457,24 +2434,6 @@ int ggnn_sync_check(ggnn_engine* e, ggnn_stream_t stream) {
         cudaMemset(e->err_flag.ptr, 0, sizeof(int));
         return e->fail(GGNN_ECUDA, "propagation kernel reported a barrier timeout (role code %d)", flag);
     }
-    return GGNN_OK;
-}
-
-int ggnn_debug_timestamps(ggnn_engine* e, int64_t* out64) {
-    if (!e || !out64) return GGNN_EINVAL;
-    if (!e->dbg_buf.ptr) return e->fail(GGNN_ESTATE, "no debug timestamps recorded (set GGNN_TS_DEBUG=1)");
-    CU_TRY(e, cudaSetDevice(e->device));
-    CU_TRY(e, cudaDeviceSynchronize());
-    CU_TRY(e, cudaMemcpy(out64, e->dbg_buf.ptr, 64 * sizeof(long long), cudaMemcpyDeviceToHost));   // the phase stamps; ggnn_debug_trace returns everything
-    return GGNN_OK;
-}
-
-int ggnn_debug_trace(ggnn_engine* e, int64_t* out, int32_t capacity) {
-    if (!e || !out || capacity <= 0) return GGNN_EINVAL;
-    if (!e->dbg_buf.ptr) return e->fail(GGNN_ESTATE, "no debug trace recorded (set GGNN_TS_DEBUG=1)");
-    CU_TRY(e, cudaSetDevice(e->device));
-    CU_TRY(e, cudaDeviceSynchronize());
-    CU_TRY(e, cudaMemcpy(out, e->dbg_buf.ptr, sizeof(long long) * std::min((size_t)capacity, e->dbg_buf.cap / sizeof(long long)), cudaMemcpyDeviceToHost));
     return GGNN_OK;
 }
 

@@ -45,9 +45,16 @@ constexpr int MAX_NS = 8;            // ring stages
 constexpr int A_STAGE_B = 8192;      // one K-step of a 128-row A operand: 2 parts x 2 k-groups x 128 rows x 16 B
 constexpr int MMA_N = 128;           // output columns per CTA (the wgmma N): 64 fp32 accumulator registers per MMA thread
 constexpr int ACC_LD = MMA_N + 4;    // row stride (floats) of the accumulator parked in shared memory: conflict-free float4 rows
-constexpr int NWORK_DEFAULT = 8;     // worker warps: two gather groups of 128 rows, two epilogue column groups (17 warps in all:
+constexpr int NWORK = 8;             // worker warps: two gather groups of 128 rows, two epilogue column groups (17 warps in all:
                                      // five per SM sub-partition leave 96 registers per thread)
-constexpr int NTHREADS = (NWORK_DEFAULT + 9) * 32;
+constexpr int NGATHER = NWORK / 4;   // gather groups (4 warps = 128 rows each)
+constexpr int NTHREADS = (NWORK + 9) * 32;
+// The shallowest ring the kernel accepts.  The MMA warpgroups keep one stage's MMAs in flight while they await the next, so a ring needs
+// two stages.  And a parity wait is only sound if the waiter cannot be two phases ahead of the barrier: a gather group waiting for round r
+// of a stage has (through its previous stage, NGATHER stages back) only seen round r-2 complete when the ring has at least as many stages
+// as there are gather groups.
+constexpr int MIN_NS = 2;
+static_assert(NGATHER <= MIN_NS && MIN_NS <= MAX_NS, "every gather group needs a ring stage of its own");
 // shared memory of the ring: the stages, and at least the parked accumulator
 __host__ __device__ inline size_t ring_bytes(size_t nstages, size_t stage_b) {
     const size_t acc_b = (size_t)TILE_M * ACC_LD * sizeof(float);
@@ -74,7 +81,6 @@ struct StreamParams {
     const int4* vinfo;           // [NV][2]: {count, src0, src1, src2 | src3 .. src6}: the first sources inline, one 32-byte load per virtual row
     const int* tile_vptr;        // [ntiles+1] vid range of each tile
     uint8_t* virt_img;           // image rows of the virtual rows (written in the prologue of every launch, row index = vid)
-    int virt_rows;               // 1: pairs with several messages are pre-summed into virtual rows (molecule batches); 0: summed in the gather loop
     // ---- B operand
     const uint8_t* w;            // [nblk][kt_all] stages of 64*NC bytes: [hi: 2 k-groups x NC x 16 B | lo: same]
     int kt_all;                  // K-steps per N block in `w`
@@ -91,8 +97,6 @@ struct StreamParams {
     float* sv_h; float* sv_agg; float* sv_r; float* sv_c;   // this step's save-for-backward slots or null
     float drop_keep; unsigned long long drop_seed; int gstep;
     int* error_flag;
-    long long* dbg;   // optional per-CTA phase stamps [grid.y][grid.x][16] (GGNN_TS_DEBUG=1), or nullptr
-    long long* dbg2;  // optional per-K-step timeline of CTA (0,0): [256][8] clocks (issuer: B landed, A landed, issued | gather: start, stage free, issued | producer: stage free, issued)
 };
 
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
@@ -161,14 +165,13 @@ __device__ __forceinline__ void sum_pair_sources(const uint8_t* __restrict__ g_i
 }
 
 // KS = K-steps (16 columns) per ring stage, a divisor of DP / 16; X3 = three MMAs per product (bf16x3) instead of one
-template <int NWORK, bool GATHER, bool X3, int KS>
-__global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const __grid_constant__ StreamParams p) {
+template <bool GATHER, bool X3, int KS>
+__global__ void __launch_bounds__(NTHREADS, 1) ggnn_stream_kernel(const __grid_constant__ StreamParams p) {
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t bar_full[MAX_NS];    // B (and TMA-fed A) bytes landed
     __shared__ __align__(8) uint64_t bar_afull[MAX_NS];   // gathered A written (GATHER)
     __shared__ __align__(8) uint64_t bar_empty[MAX_NS];   // the MMAs that read the stage are complete
     __shared__ __align__(8) uint64_t bar_acc;             // the accumulator is parked in shared memory
-    __shared__ __align__(8) uint64_t bar_virt[16];        // GATHER: the virtual rows of K group j are written (by the gather groups that have no ring slot)
     __shared__ int s_abort;
     __shared__ int s_types[32];
     __shared__ int s_ntypes;
@@ -191,10 +194,6 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
         s_abort = 0;
         for (int i = 0; i < MAX_NS; ++i) { tc::mbar_init(&bar_full[i], 1); tc::mbar_init(&bar_afull[i], TILE_M); tc::mbar_init(&bar_empty[i], 8); }
         tc::mbar_init(&bar_acc, 256);
-        {   // gather groups beyond the ring depth have no stage to fill: they pre-sum the virtual rows of K groups 1.. while the others gather
-            const int idle_warps = (NWORK / 4 - min(NWORK / 4, NS)) * 4;
-            for (int i = 0; i < 16; ++i) tc::mbar_init(&bar_virt[i], idle_warps > 0 ? idle_warps : 1);
-        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         int n = 0;
         if (GATHER) {
@@ -215,18 +214,11 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
         // those K-steps is ONE contiguous piece of the image, their B operand ONE contiguous piece of the pre-tiled weights.
         if (lane == 0) {
             bool ok = true;
-            long long waited = 0;
             int s = 0, round = 0;
             const uint8_t* wb = p.w + (size_t)nb0 * p.kt_all * B_STEP_B;
             int sg = 0, j = 0;
             for (int g = 0; g < ng && ok; ++g) {
-                if (round > 0) {
-                    const long long w0 = p.dbg ? clock64() : 0;
-                    if (!tc::mbar_wait(&bar_empty[s], (uint32_t)(round - 1) & 1u, abortp)) { ok = false; break; }
-                    if (p.dbg) waited += clock64() - w0;
-                }
-                long long* d2 = (p.dbg2 && tile == 0 && nb0 == 0 && g < 256) ? p.dbg2 + g * 8 : nullptr;
-                if (d2) d2[6] = clock64();
+                if (round > 0 && !tc::mbar_wait(&bar_empty[s], (uint32_t)(round - 1) & 1u, abortp)) { ok = false; break; }
                 const int ks0 = j * KS, nks = KS;
                 uint8_t* st = smem + (size_t)s * STAGE_B;
                 const int seg_k0 = (GATHER ? s_types[sg] : sg) * NKS + ks0;   // first K-step of the stage in the weight stream
@@ -237,15 +229,12 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
                     tc::bulk_copy_g2s(st, p.seg[sg] + ((size_t)tile * NKS + ks0) * A_STAGE_B, (uint32_t)nks * A_STAGE_B, &bar_full[s]);
                 }
                 tc::bulk_copy_g2s(st + A_REGION_B, wb + (size_t)seg_k0 * B_STEP_B, (uint32_t)nks * B_STEP_B, &bar_full[s]);
-                if (d2) d2[7] = clock64();
-                // K order: TMA-fed kernels walk segment by segment; the gather GEMM walks K group by K group over all edge types (the virtual
-                // rows of K group 0 are then enough to start, the rest are pre-summed while the ring already turns)
+                // K order: TMA-fed kernels walk segment by segment; the gather GEMM walks K group by K group over all edge types
                 if (GATHER) { if (++sg == nsegs) { sg = 0; ++j; } }
                 else if (++j == GPS) { j = 0; ++sg; }
                 if (++s == NS) { s = 0; ++round; }
             }
             if (!ok) atomicExch(p.error_flag, 13);
-            if (p.dbg) p.dbg[((size_t)blockIdx.y * gridDim.x + tile) * 16 + 4] = waited;
         }
     } else if (warp >= NWORK) {
         // =============================================================================== MMA WARPGROUPS
@@ -260,18 +249,12 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
         const uint32_t smem_a = smem_u32(smem) + (uint32_t)m * 1024u;   // this half's first row inside an A stage
         const uint32_t smem_b = smem_u32(smem);
         const uint32_t lbo_b = 16u * (uint32_t)MMA_N;
-        long long waited_b = 0, waited_a = 0;
         int s = 0, prev = -1;
         uint32_t par = 0;
         for (int g = 0; g < ng; ++g) {
-            const long long w0 = p.dbg ? clock64() : 0;
             if (poller && !*abortp && !tc::mbar_wait(&bar_full[s], par, abortp)) *abortp = 1;
-            const long long w1 = p.dbg ? clock64() : 0;
             if (GATHER && poller && !*abortp && !tc::mbar_wait(&bar_afull[s], par, abortp)) *abortp = 1;
-            if (p.dbg) { waited_b += w1 - w0; waited_a += clock64() - w1; }
             asm volatile("bar.sync %0, 128;" ::"r"(6 + m) : "memory");
-            long long* d2 = (p.dbg2 && tile == 0 && nb0 == 0 && g < 256 && tid == NWORK * 32) ? p.dbg2 + g * 8 : nullptr;
-            if (d2) { d2[0] = w1; d2[1] = clock64(); }
             if (GATHER) tc::fence_async_smem();   // the gathered A stage was written through the generic proxy (cp.async / st.shared)
             const uint32_t a0 = smem_a + (uint32_t)s * STAGE_B, b0 = smem_b + (uint32_t)s * STAGE_B + A_REGION_B;
             wg::fence();
@@ -289,7 +272,6 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
             wg::wait<1>();
             if (prev >= 0) { __syncwarp(); if (lane == 0) tc::mbar_arrive(&bar_empty[prev]); }
             prev = s;
-            if (d2) d2[2] = clock64();
             if (++s == NS) { s = 0; par ^= 1u; }
         }
         wg::wait_all();
@@ -306,7 +288,6 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
             }
             tc::mbar_arrive(&bar_acc);
         }
-        if (p.dbg && tid == NWORK * 32) { long long* d = p.dbg + ((size_t)blockIdx.y * gridDim.x + tile) * 16; d[5] = waited_b; d[6] = waited_a; }
     } else {
         // =============================================================================== WORKERS
         const int wi = warp;
@@ -318,28 +299,18 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
         const int cgp = wi >> 2;
         const int nchunks = NC >> 3;
         bool ok = true;
-        const bool stamp = p.dbg && wi == 0 && lane == 0;
-        long long t0 = 0, t_gather = 0, t_acc = 0, g_load = 0, g_wait = 0, g_tail = 0, t_setup = 0;
-        if (stamp) t0 = clock64();
         const int NKC = DP >> 3;
         if (GATHER) {
-            constexpr int NG = NWORK / 4;             // gather groups (4 warps = 128 rows each)
             const int grp = wi >> 2;
             const int gi = (wi & 3) * 32 + lane;      // the tile row this thread gathers
-            const int wt = tid;
             // ---- the tile's (target, type) -> source table
-            for (int i = wt; i < TILE_M * T; i += NWORK * 32) sPair[i] = p.pair_src[(size_t)row0 * T + i];
-            const long long t_pair = stamp ? clock64() : 0;
-            // ---- virtual rows: the pairs of this tile with several messages, summed in message order (fp32), re-split, stored as image rows.
-            // The K loop of the gather GEMM is K-group major, so only the virtual rows of K group 0 must exist before the first stage:
-            // all workers pre-sum those; the groups beyond the ring depth (no stage to fill, see below) then pre-sum K groups 1.. and signal
-            // each one on bar_virt[j] while the other groups already gather.  Without surplus groups everything is pre-summed up front.
-            // (p.virt_rows == 0: pairs with several messages are summed inside the gather loop instead.)
-            const int NGE = min(NG, NS);
-            const int v0 = p.tile_vptr[tile], nv = p.virt_rows ? p.tile_vptr[tile + 1] - v0 : 0;
-            auto presum = [&](int jg, int first, int nthreads_) {   // virtual rows of K group jg, tasks dealt to `nthreads_` threads
+            for (int i = tid; i < TILE_M * T; i += NWORK * 32) sPair[i] = p.pair_src[(size_t)row0 * T + i];
+            // ---- virtual rows: the pairs of this tile with several messages, summed in message order (fp32), re-split, stored as image rows,
+            // for every K group before the first stage is gathered
+            const int v0 = p.tile_vptr[tile], nv = p.tile_vptr[tile + 1] - v0;
+            for (int jg = 0; jg < GPS; ++jg) {
                 const int ks0 = jg * KS, nks = min(KS, NKS - ks0);
-                for (int task = first; task < nv * nks; task += nthreads_) {
+                for (int task = tid; task < nv * nks; task += NWORK * 32) {
                     const int vl = task / nks, vid = v0 + vl, ks = ks0 + (task - vl * nks);
                     const int4 i0 = __ldg(p.vinfo + 2 * (size_t)vid), i1 = __ldg(p.vinfo + 2 * (size_t)vid + 1);
                     uint4 h0, l0, h1, l1;
@@ -350,55 +321,23 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
                     *reinterpret_cast<uint4*>(vp + 4096) = l0;
                     *reinterpret_cast<uint4*>(vp + 6144) = l1;
                 }
-            };
-            // worth it only if the surplus groups can finish a K group's virtual rows before the ring gets there: one round of tasks per
-            // 16 K-steps (a heuristic: molecule batches have a few dozen virtual rows per tile, dense graphs hundreds)
-            const int nidle_thr = (NG - NGE) * 128;
-            const bool overlap = NGE < NG && ((nv * KS + nidle_thr - 1) / max(nidle_thr, 1)) * 16 <= nsegs * KS;
-            if (p.virt_rows) {
-                for (int jg = 0; jg < (overlap ? 1 : GPS); ++jg) presum(jg, wt, NWORK * 32);
-                const long long t_virt = stamp ? clock64() : 0;
-                __threadfence();   // the copies below read these rows back through L2 (cp.async.cg)
-                if (stamp) { long long* d = p.dbg + ((size_t)blockIdx.y * gridDim.x + tile) * 16; d[12] = t_pair - t0; d[13] = t_virt - t0; d[14] = clock64() - t0; d[15] = nv; }
             }
+            __threadfence();   // the copies below read these rows back through L2 (cp.async.cg)
             asm volatile("bar.sync 1, %0;" ::"n"(NWORK * 32) : "memory");
-            if (stamp) t_setup = clock64();
-            if (overlap && grp >= NGE && p.virt_rows) {
-                const int nidle = (NG - NGE) * 128, me = (grp - NGE) * 128 + gi;
-                for (int jg = 1; jg < GPS; ++jg) {
-                    presum(jg, me, nidle);
-                    __threadfence();
-                    __syncwarp();
-                    if (lane == 0) tc::mbar_arrive(&bar_virt[jg]);
-                }
-            }
-            // group `grp` fills stages grp, grp + NGE, ...: every row is an asynchronous 64-byte copy per K-step (or zeros).
-            // No more groups than ring stages: a parity wait on a stage's barrier is only sound if the waiter cannot be two phases ahead
-            // of it, and group X waiting for round r of a stage has (through its previous stage, NGE K-groups back) only seen round r-2
-            // complete when NS >= NGE.  Surplus groups pre-sum virtual rows instead (above).
-            int j_seen = 0;
-            for (int g = grp < NGE ? grp : ng; g < ng && ok; g += NGE) {
+            // group `grp` fills stages grp, grp + NGATHER, ...: every row is an asynchronous 64-byte copy per K-step (or zeros).
+            // The ring has at least NGATHER stages (MIN_NS), so the parity waits below are sound.
+            for (int g = grp; g < ng && ok; g += NGATHER) {
                 const int j = g / nsegs, sg = g - j * nsegs;   // K group major: stage g = (K group j, present edge type sg)
-                const long long c0 = stamp ? clock64() : 0;
                 const int s = g % NS, round = g / NS;
-                long long* d2 = (p.dbg2 && tile == 0 && nb0 == 0 && g < 256 && gi == 0) ? p.dbg2 + g * 8 : nullptr;
-                if (d2) d2[3] = clock64();
                 const int ks0 = j * KS, nks = min(KS, NKS - ks0);
                 const int ps = sPair[gi * T + s_types[sg]];
-                if (ps < -1 && overlap && p.virt_rows && j > j_seen) {   // this K group's virtual rows come from the surplus groups
-                    if (!tc::mbar_wait(&bar_virt[j], 0, abortp)) *abortp = 1;
-                    j_seen = j;
-                }
                 const uint8_t* sp = nullptr;
                 if (ps >= 0) sp = p.g_img + ((size_t)(ps >> 7) * NKS + ks0) * A_STAGE_B + (size_t)(ps & 127) * 16;
-                else if (ps < -1 && p.virt_rows) { const int vid = -(ps + 2); sp = p.virt_img + ((size_t)(vid >> 7) * NKS + ks0) * A_STAGE_B + (size_t)(vid & 127) * 16; }
-                const long long c1 = stamp ? clock64() : 0;
+                else if (ps < -1) { const int vid = -(ps + 2); sp = p.virt_img + ((size_t)(vid >> 7) * NKS + ks0) * A_STAGE_B + (size_t)(vid & 127) * 16; }
                 // one warp of the group polls the stage's barrier, the other three block on a hardware barrier (polling warps cost issue slots)
                 if (round > 0 && (wi & 3) == 0 && !tc::mbar_wait(&bar_empty[s], (uint32_t)(round - 1) & 1u, abortp)) *abortp = 1;
                 asm volatile("bar.sync %0, 128;" ::"r"(2 + grp) : "memory");
                 if (*abortp) { ok = false; break; }
-                const long long c2 = stamp ? clock64() : 0;
-                if (d2) d2[4] = clock64();
                 uint8_t* ap = smem + (size_t)s * STAGE_B + (size_t)gi * 16;
                 const uint32_t bar = smem_u32(&bar_afull[s]);
                 if (sp) {
@@ -411,19 +350,6 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
                     }
                     // one arrival on the stage's barrier when this thread's copies have landed (the barrier counts 128 threads)
                     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];\n" ::"r"(bar) : "memory");
-                } else if (ps < -1) {   // several messages, summed here (dense graphs): loads -> registers -> stage
-                    const int vid = -(ps + 2);
-                    const int4 i0 = __ldg(p.vinfo + 2 * (size_t)vid), i1 = __ldg(p.vinfo + 2 * (size_t)vid + 1);
-                    const int* tail = p.vsrc + p.vrow_ptr[i0.x > 7 ? vid : 0];
-                    for (int i = 0; i < nks; ++i, ap += A_STAGE_B) {
-                        uint4 h0, l0, h1, l1;
-                        sum_pair_sources(p.g_img, NKS, ks0 + i, i0, i1, tail, h0, h1, l0, l1);
-                        *reinterpret_cast<uint4*>(ap) = h0;
-                        *reinterpret_cast<uint4*>(ap + 2048) = h1;
-                        *reinterpret_cast<uint4*>(ap + 4096) = l0;
-                        *reinterpret_cast<uint4*>(ap + 6144) = l1;
-                    }
-                    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
                 } else {
                     const uint4 z = make_uint4(0u, 0u, 0u, 0u);
                     for (int i = 0; i < nks; ++i, ap += A_STAGE_B) {
@@ -434,10 +360,7 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
                     }
                     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
                 }
-                if (d2) d2[5] = clock64();
-                if (stamp) { const long long c3 = clock64(); g_load += c1 - c0; g_wait += c2 - c1; g_tail += c3 - c2; }
             }
-            if (stamp) t_gather = clock64();
         }
         // ---- epilogue: parked accumulator -> registers -> outputs.  The global operands of the first chunk are requested BEFORE the wait for the
         // accumulator, those of chunk c+1 before the math of chunk c (the loads are L2 hits after the prefetch above).
@@ -467,7 +390,6 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
             asm volatile("bar.sync 1, %0;" ::"n"(NWORK * 32) : "memory");
             if (*abortp) ok = false;
         }
-        if (stamp) t_acc = clock64();
         if (ok) {
             if (p.epi == EPI_AGG) {
                 // sparse:207-209 divides by (sum of in-degrees + 1e-7); one IEEE reciprocal per row, then a multiply per element (differs from
@@ -565,11 +487,6 @@ __global__ void __launch_bounds__((NWORK + 9) * 32, 1) ggnn_stream_kernel(const 
             }
         }
         if (!ok && lane == 0) atomicExch(p.error_flag, 11);
-        if (stamp) {
-            long long* d = p.dbg + ((size_t)blockIdx.y * gridDim.x + tile) * 16;
-            d[0] = t0; d[1] = t_gather - t0; d[2] = t_acc - t0; d[3] = clock64() - t0; d[7] = nk;
-            d[8] = g_load; d[9] = g_wait; d[10] = g_tail; d[11] = t_setup - t0;
-        }
     }
     __syncthreads();
 }

@@ -201,6 +201,101 @@ __device__ __forceinline__ void lds8(const float* s, float (&v)[8]) {
 __device__ __forceinline__ float2 ld2_cg(const float* p) { return __ldcg(reinterpret_cast<const float2*>(p)); }
 __device__ __forceinline__ void st2(float* p, float a, float b) { *reinterpret_cast<float2*>(p) = make_float2(a, b); }
 
+// ------------------------------------------------------------------------------------------------ the weight ring of the tile kernels
+// (this file's kernel and gcn::gcn_wgmma_kernel).  One producer thread streams pre-tiled weights into `nslots` slots of two K-step stages
+// (2 x stage_b bytes, one bulk copy); every worker warp takes every slot in push order and releases it once its MMAs are complete.
+
+// tid 0, before the CTA's first __syncthreads: the barriers of all `nslots` slots the kernel declares
+__device__ __forceinline__ void ring_init(uint64_t* full, uint64_t* empty, int nslots) {
+    for (int i = 0; i < nslots; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], NUM_WORKERS / 32); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+
+// All-worker rendezvous on hardware named barrier 1; the abort flag is OR-reduced over the barrier so that every worker sees the same
+// verdict (ok = false) and all leave together.
+__device__ __forceinline__ void workers_sync(volatile int* abortp, bool& ok) {
+    uint32_t any;
+    asm volatile("{\n\t.reg .pred pa, pb;\n\tsetp.ne.u32 pa, %1, 0;\n\tbar.red.or.pred pb, 1, %2, pa;\n\tselp.u32 %0, 1, 0, pb;\n\t}\n"
+                 : "=r"(any) : "r"((uint32_t)(*abortp != 0)), "n"(NUM_WORKERS) : "memory");
+    if (any) ok = false;
+}
+
+// The consumer side, one per worker thread.
+struct RingReader {
+    uint64_t* full;           // [nslots] the slot's bytes have landed
+    uint64_t* empty;          // [nslots] every worker warp is done with the slot
+    volatile int* abortp;
+    uint32_t base;            // shared address of slot 0
+    uint32_t nslots;
+    uint32_t slot = 0, fpar = 0;   // the next slot / bit s: the parity to wait for on full[s]
+    // the next slot, its bytes landed (a timeout raises the abort flag and returns the slot anyway: the caller still releases it)
+    __device__ __forceinline__ uint32_t take() {
+        const uint32_t sl = slot;
+        slot = (slot + 1 == nslots) ? 0u : slot + 1;
+        if (!*abortp && !mbar_wait(&full[sl], (fpar >> sl) & 1u, abortp)) *abortp = 1;
+        fpar ^= 1u << sl;
+        return sl;
+    }
+    __device__ __forceinline__ void release(uint32_t sl, int lane) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[sl]); }
+};
+
+// The producer side, one thread, strictly in the order the workers consume.  A slot is refilled once every worker warp has released it,
+// so no waiter can be two phases behind a barrier.
+struct RingWriter {
+    uint64_t* full;
+    uint64_t* empty;
+    volatile int* abortp;
+    uint8_t* base;            // slot 0
+    uint32_t nslots, stage_b;
+    uint32_t cur = 0, used = 0, epar = 0;   // the next slot / bit s: slot s has been filled before / parity to wait for on empty[s]
+    bool ok = true;                         // false after a timeout: nothing more is pushed
+    // stream `n` consecutive stage_b-byte stages of a pre-tiled matrix, two per slot
+    __device__ __forceinline__ void push(const uint8_t* src, int n) {
+        for (int i = 0; i < n && ok; i += 2) {
+            const uint32_t bytes = (i + 1 < n) ? 2u * stage_b : stage_b;
+            const uint32_t sl = cur;
+            cur = (cur + 1 == nslots) ? 0u : cur + 1;
+            if ((used >> sl) & 1u) {
+                if (!mbar_wait(&empty[sl], (epar >> sl) & 1u, abortp)) { ok = false; break; }
+                epar ^= 1u << sl;
+            }
+            used |= 1u << sl;
+            mbar_arrive_expect_tx(&full[sl], bytes);
+            bulk_copy_g2s(base + sl * 2u * stage_b, src + (size_t)i * stage_b, bytes, &full[sl]);
+        }
+    }
+};
+
+// acc += A(op) . B(one DP x DP weight block: ceil(NKS/2) slots of two K-steps, each stage = [hi | lo]) for one worker warpgroup: A rows from
+// byte a_row on (k-group stride KGS, lo part PART_B after hi), B columns NH*nh .. +NH.  x3: three MMAs per product.  A warpgroup without rows
+// (mma_rows false) skips the MMAs but still takes and releases every slot.
+template <int NH>
+__device__ __forceinline__ void gemm_narrow(RingReader& ring, float (&acc)[NH / 2], const uint8_t* op, int NKS, int DP, uint32_t KGS, uint32_t PART_B,
+                                            uint32_t STAGE_B, uint32_t a_row, int nh, bool mma_rows, bool x3, int lane) {
+    const int nslots = (NKS + 1) / 2;
+    for (int i = 0; i < nslots; ++i) {
+        const uint32_t sl = ring.take();
+        if (mma_rows) {
+            const uint32_t b0 = ring.base + sl * 2u * STAGE_B + (uint32_t)nh * NH * 16u;
+            const int nk = (2 * i + 1 < NKS) ? 2 : 1;
+            wg::fence();
+            for (int h = 0; h < nk; ++h) {
+                const uint32_t a = smem_u32(op) + (uint32_t)(2 * i + h) * 2u * KGS + a_row;
+                const uint32_t b = b0 + (uint32_t)h * STAGE_B;
+                const uint64_t ad = wg::make_desc(a, KGS, 128), bd = wg::make_desc(b, 16u * DP, 128);
+                wg::Mma<NH>::run(acc, ad, bd);
+                if (x3) {
+                    wg::Mma<NH>::run(acc, ad, wg::make_desc(b + 32u * DP, 16u * DP, 128));
+                    wg::Mma<NH>::run(acc, wg::make_desc(a + PART_B, KGS, 128), bd);
+                }
+            }
+            wg::commit();
+            wg::wait_all();
+        }
+        ring.release(sl, lane);
+    }
+}
+
 template <bool LOCAL, int NH>
 __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_constant__ TcParams p) {
     constexpr int NF = NH / 2;   // accumulator floats per thread and quantity (m64 x NH fragment)
@@ -235,8 +330,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
 
     if (tid == 0) {
         s_abort = 0;
-        for (int i = 0; i < MAX_STAGES; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], NUM_WORKERS / 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        ring_init(bar_full, bar_empty, MAX_STAGES);
     }
     __syncthreads();
     volatile int* abortp = &s_abort;
@@ -258,58 +352,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
         const bool mma_rows = mh * 64 < rows;                       // warpgroup-uniform: the warpgroup has rows at all
         const bool x3 = p.nparts == 3;
         bool ok = true;
-        // All-worker rendezvous on hardware named barrier 1; the abort flag is OR-reduced over the barrier so that every worker
-        // sees the same verdict and all leave together.
-        auto workers_sync = [&]() {
-            uint32_t any;
-            asm volatile("{\n\t.reg .pred pa, pb;\n\tsetp.ne.u32 pa, %1, 0;\n\tbar.red.or.pred pb, 1, %2, pa;\n\tselp.u32 %0, 1, 0, pb;\n\t}\n"
-                         : "=r"(any) : "r"((uint32_t)(*abortp != 0)), "n"(NUM_WORKERS) : "memory");
-            if (any) ok = false;
-        };
+        auto workers_sync = [&]() { tc::workers_sync(abortp, ok); };
         auto publish_sync = [&]() { fence_async_smem(); workers_sync(); };   // operand tiles written -> visible to wgmma
-        // ---- weight ring: every worker warp walks every slot in push order
-        uint32_t slot = 0, fpar = 0;
-        const uint32_t ring_a = smem_u32(ring);
-        auto take_slot = [&]() -> uint32_t {
-            const uint32_t sl = slot;
-            slot = (slot + 1 == (uint32_t)nst) ? 0u : slot + 1;
-            if (!*abortp && !mbar_wait(&bar_full[sl], (fpar >> sl) & 1u, abortp)) *abortp = 1;
-            fpar ^= 1u << sl;
-            return sl;
-        };
-        auto release_slot = [&](uint32_t sl) { __syncwarp(); if (lane == 0) mbar_arrive(&bar_empty[sl]); };
+        RingReader rd{bar_full, bar_empty, abortp, smem_u32(ring), (uint32_t)nst};
         const uint32_t a_row = (uint32_t)mh * 64u * 16u;   // this warpgroup's first row inside an A operand
-        // acc += A(op) . B(one DP x DP block: ceil(NKS/2) slots of two K-steps, each stage = [hi | lo]), this warpgroup's columns
         auto gemm_narrow = [&](float (&acc)[NF], const uint8_t* op) {
-            const int nslots = (NKS + 1) / 2;
-            for (int i = 0; i < nslots; ++i) {
-                const uint32_t sl = take_slot();
-                if (mma_rows) {
-                    const uint32_t b0 = ring_a + sl * 2u * STAGE_B + (uint32_t)nh * NH * 16u;
-                    const int nk = (2 * i + 1 < NKS) ? 2 : 1;
-                    wg::fence();
-                    for (int h = 0; h < nk; ++h) {
-                        const uint32_t a = smem_u32(op) + (uint32_t)(2 * i + h) * 2u * KGS + a_row;
-                        const uint32_t b = b0 + (uint32_t)h * STAGE_B;
-                        const uint64_t ad = wg::make_desc(a, KGS, 128), bd = wg::make_desc(b, 16u * DP, 128);
-                        wg::Mma<NH>::run(acc, ad, bd);
-                        if (x3) {
-                            wg::Mma<NH>::run(acc, ad, wg::make_desc(b + 32u * DP, 16u * DP, 128));
-                            wg::Mma<NH>::run(acc, wg::make_desc(a + PART_B, KGS, 128), bd);
-                        }
-                    }
-                    wg::commit();
-                    wg::wait_all();
-                }
-                release_slot(sl);
-            }
+            tc::gemm_narrow<NH>(rd, acc, op, NKS, DP, KGS, PART_B, STAGE_B, a_row, nh, mma_rows, x3, lane);
         };
         // [r | u] += A(op) . B(one segment of the N = 2*DP gate block: NKS slots, stage 0 = hi, stage 1 = lo); columns of r and of u
         auto gemm_wide = [&](float (&ar)[NF], float (&au)[NF], const uint8_t* op) {
             for (int i = 0; i < NKS; ++i) {
-                const uint32_t sl = take_slot();
+                const uint32_t sl = rd.take();
                 if (mma_rows) {
-                    const uint32_t bh = ring_a + sl * 2u * STAGE_B, bl = bh + STAGE_B;
+                    const uint32_t bh = rd.base + sl * 2u * STAGE_B, bl = bh + STAGE_B;
                     const uint32_t cr = (uint32_t)nh * NH * 16u, cu = (uint32_t)(DP + nh * NH) * 16u, lbo = 32u * DP;
                     const uint32_t a = smem_u32(op) + (uint32_t)i * 2u * KGS + a_row;
                     const uint64_t ad = wg::make_desc(a, KGS, 128);
@@ -326,7 +381,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
                     wg::commit();
                     wg::wait_all();
                 }
-                release_slot(sl);
+                rd.release(sl, lane);
             }
         };
         auto zero = [](float (&a)[NF]) {
@@ -607,50 +662,31 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
         if (!ok && tid == 0) atomicExch(p.error_flag, 1);
     } else if (lane == 0) {
         // =============================================================================== WEIGHT PRODUCER
-        // One thread, strictly in the order the workers consume: a push moves a whole slot = two stages (2 x 64*DP bytes, contiguous in
-        // the pre-tiled weights) with one bulk copy.  A slot is refilled once all 16 worker warps have released it, so no waiter can be
-        // two phases behind a barrier.
-        const uint32_t nstg = (uint32_t)nst;
-        uint32_t cur = 0, used = 0, epar = 0;   // bit s: slot s has been filled before / parity to wait for on bar_empty[s]
-        bool ok = true;
-        // stream `nstages` consecutive 64*DP-byte stages of a pre-tiled matrix, two per slot
-        auto push = [&](const uint8_t* src, int nstages) {
-            for (int i = 0; i < nstages && ok; i += 2) {
-                const uint32_t bytes = (i + 1 < nstages) ? 2u * STAGE_B : STAGE_B;
-                const uint32_t sl = cur;
-                cur = (cur + 1 == nstg) ? 0u : cur + 1;
-                if ((used >> sl) & 1u) {
-                    if (!mbar_wait(&bar_empty[sl], (epar >> sl) & 1u, abortp)) { ok = false; break; }
-                    epar ^= 1u << sl;
-                }
-                used |= 1u << sl;
-                mbar_arrive_expect_tx(&bar_full[sl], bytes);
-                bulk_copy_g2s(ring + sl * 2u * STAGE_B, src + (size_t)i * STAGE_B, bytes, &bar_full[sl]);
-            }
-        };
-        for (int l = l_begin; l < l_end && ok; ++l) {
+        // the weights of every layer and step, in the order the workers' GEMMs consume them
+        RingWriter wr{bar_full, bar_empty, abortp, ring, (uint32_t)nst, STAGE_B};
+        for (int l = l_begin; l < l_end && wr.ok; ++l) {
             const TcLayer& ly = p.layer[l];
             const int s_begin = LOCAL ? 0 : p.g_step;
             const int s_end = LOCAL ? ly.steps : p.g_step + 1;
             const bool gru = p.cell == CELL_GRU;
             const size_t blk = (size_t)NKS * STAGE_B;   // one DP x DP block; a gate block is two of these per K segment
             if (ly.nres > 0 && s_end > s_begin) {
-                for (int i = 0; i < ly.nres && ok; ++i) {
-                    if (gru) push(ly.w_gate + (size_t)i * 2 * blk, 2 * NKS);
-                    push(ly.w_cand + (size_t)i * blk, NKS);
+                for (int i = 0; i < ly.nres && wr.ok; ++i) {
+                    if (gru) wr.push(ly.w_gate + (size_t)i * 2 * blk, 2 * NKS);
+                    wr.push(ly.w_cand + (size_t)i * blk, NKS);
                 }
             }
             const size_t kx = (size_t)ly.nres, kh = (size_t)ly.nres + 1;
-            for (int s = s_begin; s < s_end && ok; ++s) {
-                for (int t = 0; t < T && ok; ++t) {
+            for (int s = s_begin; s < s_end && wr.ok; ++s) {
+                for (int t = 0; t < T && wr.ok; ++t) {
                     if (!((tmask >> t) & 1u)) continue;
-                    push(ly.w_edge + (size_t)t * blk, NKS);
+                    wr.push(ly.w_edge + (size_t)t * blk, NKS);
                 }
-                if (gru) { push(ly.w_gate + kx * 2 * blk, 2 * NKS); push(ly.w_gate + kh * 2 * blk, 2 * NKS); }
-                push(ly.w_cand + kx * blk, NKS); push(ly.w_cand + kh * blk, NKS);
+                if (gru) { wr.push(ly.w_gate + kx * 2 * blk, 2 * NKS); wr.push(ly.w_gate + kh * 2 * blk, 2 * NKS); }
+                wr.push(ly.w_cand + kx * blk, NKS); wr.push(ly.w_cand + kh * blk, NKS);
             }
         }
-        if (!ok) atomicExch(p.error_flag, 3);
+        if (!wr.ok) atomicExch(p.error_flag, 3);
     }
     __syncthreads();
 }

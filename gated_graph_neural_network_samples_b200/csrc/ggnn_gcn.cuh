@@ -8,9 +8,9 @@
 //                     connected components, all layers run in one launch and H stays in shared memory between layers.  GLOBAL: one launch
 //                     per layer, the gather reads the previous layer's fp32 state from global memory (a component larger than a tile).
 //                     Warp roles and operand layouts follow ggnn_fwd_tc.cuh: four worker warpgroups, warpgroup w owns rows 64*(w%2) .. +64 and
-//                     columns NH*(w/2) .. +NH (NH = DP/2) of S . W; S is split into bf16 hi/lo in the canonical no-swizzle K-major layout; one
-//                     producer thread streams the pre-split, pre-tiled W_l (tc::ggnn_tile_weights_kernel) through a cp.async.bulk / mbarrier
-//                     ring; every wait is bounded and a timeout sets the engine's error flag (ggnn_sync_check).
+//                     columns NH*(w/2) .. +NH (NH = DP/2) of S . W; S is split into bf16 hi/lo in the canonical no-swizzle K-major layout.
+//                     The pre-split, pre-tiled W_l (tc::ggnn_tile_weights_kernel) streams through the tile kernels' weight ring
+//                     (tc::RingWriter / tc::RingReader, tc::gemm_narrow); a timeout sets the engine's error flag (ggnn_sync_check).
 //   gcn_fp32_kernel   fp32 precision and hidden sizes in (128, 256]: per layer, 32 rows per CTA, weighted CSR gather into shared memory,
 //                     FFMA GEMM with W_l from L1/L2, same epilogue.
 // The backward pass (ggnn_engine.cu) reuses ggnn_bwd.cuh; only the relu / dropout gradient below is GCN-specific.
@@ -83,8 +83,7 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid
     const int nst = p.nstages;
     if (tid == 0) {
         s_abort = 0;
-        for (int i = 0; i < MAX_STAGES; ++i) { mbar_init(&bar_full[i], 1); mbar_init(&bar_empty[i], NUM_WORKERS / 32); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        ring_init(bar_full, bar_empty, MAX_STAGES);
     }
     __syncthreads();
     volatile int* abortp = &s_abort;
@@ -101,22 +100,7 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid
         const bool mma_rows = mh * 64 < rows;
         const bool x3 = p.nparts == 3;
         bool ok = true;
-        auto workers_sync = [&]() {
-            uint32_t any;
-            asm volatile("{\n\t.reg .pred pa, pb;\n\tsetp.ne.u32 pa, %1, 0;\n\tbar.red.or.pred pb, 1, %2, pa;\n\tselp.u32 %0, 1, 0, pb;\n\t}\n"
-                         : "=r"(any) : "r"((uint32_t)(*abortp != 0)), "n"(NUM_WORKERS) : "memory");
-            if (any) ok = false;
-        };
-        uint32_t slot = 0, fpar = 0;
-        const uint32_t ring_a = smem_u32(ring);
-        auto take_slot = [&]() -> uint32_t {
-            const uint32_t sl = slot;
-            slot = (slot + 1 == (uint32_t)nst) ? 0u : slot + 1;
-            if (!*abortp && !mbar_wait(&bar_full[sl], (fpar >> sl) & 1u, abortp)) *abortp = 1;
-            fpar ^= 1u << sl;
-            return sl;
-        };
-        auto release_slot = [&](uint32_t sl) { __syncwarp(); if (lane == 0) mbar_arrive(&bar_empty[sl]); };
+        RingReader rd{bar_full, bar_empty, abortp, smem_u32(ring), (uint32_t)nst};
         const uint32_t a_row = (uint32_t)mh * 64u * 16u;
 
         if (LOCAL) {   // the tile's input states -> shared memory (padding columns zero)
@@ -128,7 +112,7 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid
                 *reinterpret_cast<float4*>(d) = make_float4(v[0], v[1], v[2], v[3]);
                 *reinterpret_cast<float4*>(d + 4) = make_float4(v[4], v[5], v[6], v[7]);
             }
-            workers_sync();
+            workers_sync(abortp, ok);
         }
         for (int l = l_begin; l < l_end && ok; ++l) {
             // ---- S = A . H for the tile's rows -> operand tile (hi / lo); rows beyond the tile are zero
@@ -151,33 +135,12 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid
                 }
             }
             fence_async_smem();
-            workers_sync();
+            workers_sync(abortp, ok);
             // ---- S . W_l on wgmma
             float acc[NF];
 #pragma unroll
             for (int i = 0; i < NF; ++i) acc[i] = 0.f;
-            const int nslots = (NKS + 1) / 2;
-            for (int i = 0; i < nslots; ++i) {
-                const uint32_t sl = take_slot();
-                if (mma_rows) {
-                    const uint32_t b0 = ring_a + sl * 2u * STAGE_B + (uint32_t)nh * NH * 16u;
-                    const int nk = (2 * i + 1 < NKS) ? 2 : 1;
-                    wg::fence();
-                    for (int h = 0; h < nk; ++h) {
-                        const uint32_t a = smem_u32(opS) + (uint32_t)(2 * i + h) * 2u * KGS + a_row;
-                        const uint32_t b = b0 + (uint32_t)h * STAGE_B;
-                        const uint64_t ad = wg::make_desc(a, KGS, 128), bd = wg::make_desc(b, 16u * DP, 128);
-                        wg::Mma<NH>::run(acc, ad, bd);
-                        if (x3) {
-                            wg::Mma<NH>::run(acc, ad, wg::make_desc(b + 32u * DP, 16u * DP, 128));
-                            wg::Mma<NH>::run(acc, wg::make_desc(a + PART_B, KGS, 128), bd);
-                        }
-                    }
-                    wg::commit();
-                    wg::wait_all();
-                }
-                release_slot(sl);
-            }
+            gemm_narrow<NH>(rd, acc, opS, NKS, DP, KGS, PART_B, STAGE_B, a_row, nh, mma_rows, x3, lane);
             // ---- epilogue: bias, relu, dropout; the state goes back to the tile (LOCAL) and to global memory
             const bool to_smem = LOCAL && l + 1 < l_end;
             const bool to_global = !LOCAL || l + 1 == l_end || p.save;
@@ -196,30 +159,14 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid
                     }
                     if (to_smem) st2(sH + (size_t)r * DP + c, v0, v1);
                 }
-            workers_sync();   // the next layer's gather reads the new states and overwrites the operand tile
+            workers_sync(abortp, ok);   // the next layer's gather reads the new states and overwrites the operand tile
         }
         if (!ok && tid == 0) atomicExch(p.error_flag, 1);
     } else if (lane == 0) {
-        // ============================================================ WEIGHT PRODUCER: W_l of every layer, two K-step stages per slot
-        const uint32_t nstg = (uint32_t)nst;
-        uint32_t cur = 0, used = 0, epar = 0;
-        bool ok = true;
-        for (int l = l_begin; l < l_end && ok; ++l) {
-            const uint8_t* src = p.w_tiled[l];
-            for (int i = 0; i < NKS && ok; i += 2) {
-                const uint32_t bytes = (i + 1 < NKS) ? 2u * STAGE_B : STAGE_B;
-                const uint32_t sl = cur;
-                cur = (cur + 1 == nstg) ? 0u : cur + 1;
-                if ((used >> sl) & 1u) {
-                    if (!mbar_wait(&bar_empty[sl], (epar >> sl) & 1u, abortp)) { ok = false; break; }
-                    epar ^= 1u << sl;
-                }
-                used |= 1u << sl;
-                mbar_arrive_expect_tx(&bar_full[sl], bytes);
-                bulk_copy_g2s(ring + sl * 2u * STAGE_B, src + (size_t)i * STAGE_B, bytes, &bar_full[sl]);
-            }
-        }
-        if (!ok) atomicExch(p.error_flag, 3);
+        // ============================================================ WEIGHT PRODUCER: W_l of every layer
+        RingWriter wr{bar_full, bar_empty, abortp, ring, (uint32_t)nst, STAGE_B};
+        for (int l = l_begin; l < l_end && wr.ok; ++l) wr.push(p.w_tiled[l], NKS);
+        if (!wr.ok) atomicExch(p.error_flag, 3);
     }
     __syncthreads();
 }

@@ -306,11 +306,6 @@ int ggnn_copy_layer_state(ggnn_engine* e, int32_t layer, float* dst, ggnn_stream
 /* Kernel launches issued by the last forward / backward call, and plan description text. */
 int ggnn_last_launch_count(const ggnn_engine* e);
 const char* ggnn_plan_description(const ggnn_engine* e);
-/* Profiling aid: with GGNN_TS_DEBUG=1 the streaming tensor-core kernels record per-CTA clock64() phase stamps; this copies the
- * first 64 entries of the buffer to out64[64]. */
-int ggnn_debug_timestamps(ggnn_engine* e, int64_t* out64);
-/* ... and the whole buffer (up to `capacity` entries): per launch, [grid][16] phase stamps, then a [256][8] K-step timeline of CTA (0,0). */
-int ggnn_debug_trace(ggnn_engine* e, int64_t* out, int32_t capacity);
 
 #ifdef __cplusplus
 }

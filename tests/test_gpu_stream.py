@@ -223,9 +223,9 @@ def test_hub_nodes_with_many_messages_per_type():
 
 @pytest.mark.parametrize("ksteps,stages", [("1", "8"), ("1", "2"), ("2", "3"), ("4", "2"), ("4", "3"), ("3", "5")])
 def test_ring_geometry_does_not_change_the_result(monkeypatch, ksteps, stages):
-    """K-steps per stage and ring depth (incl. fewer stages than gather groups, partial last stages of a K segment) only change the
-    schedule and -- because the gather GEMM walks K group by K group -- the fp32 summation order: the result stays within rounding of the
-    default geometry and is bit-identical from run to run for a fixed geometry."""
+    """K-steps per stage and ring depth (incl. the shallowest ring, one stage per gather group, and partial last stages of a K segment)
+    only change the schedule and -- because the gather GEMM walks K group by K group -- the fp32 summation order: the result stays within
+    rounding of the default geometry and is bit-identical from run to run for a fixed geometry."""
     _, b = U.molecule_batch(40, 256, T=8, seed=21)
     w = O.init_sparse_weights(CFG4, 8, np.random.default_rng(1))
     args = (CFG4, 8, w, b["adjacency_lists"], b["num_incoming_edges_per_type"], b["initial_node_representation"])
