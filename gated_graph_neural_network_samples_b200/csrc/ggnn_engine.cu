@@ -1712,10 +1712,16 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
     p.res_pre = (float*)e->tc_respre.ptr;
     p.error_flag = (int*)e->err_flag.ptr;
     const size_t vd_bytes = (size_t)e->V * e->D * sizeof(float);
-    // the wgmma N of a warpgroup's column half (DP / 2) is an instruction immediate: one kernel per padded hidden size
+    // the wgmma N of a warpgroup's columns is an instruction immediate: one kernel per padded hidden size and layout (compact tiles
+    // split the columns four ways, 128-row tiles two ways)
     void (*kern)(tc::TcParams) = nullptr;
+    const bool compact = e->tc_kgs == 1024;
     switch (DP / 2) {
-#define GGNN_TC_CASE(nh) case nh: kern = e->local ? tc::ggnn_fwd_tc_kernel<true, nh> : tc::ggnn_fwd_tc_kernel<false, nh>; break;
+#define GGNN_TC_CASE(nh)                                                                                                              \
+    case nh:                                                                                                                          \
+        kern = !e->local ? tc::ggnn_fwd_tc_kernel<false, nh, false>                                                                   \
+                         : (compact ? tc::ggnn_fwd_tc_kernel<true, nh, true> : tc::ggnn_fwd_tc_kernel<true, nh, false>);            \
+        break;
         GGNN_TC_CASE(8) GGNN_TC_CASE(16) GGNN_TC_CASE(24) GGNN_TC_CASE(32) GGNN_TC_CASE(40) GGNN_TC_CASE(48) GGNN_TC_CASE(56) GGNN_TC_CASE(64)
 #undef GGNN_TC_CASE
         default: return e->fail(GGNN_EUNSUPPORTED, "no tile-local tensor-core kernel for DP=%d", DP);

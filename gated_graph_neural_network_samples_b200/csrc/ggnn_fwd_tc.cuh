@@ -13,8 +13,9 @@
 // Warp roles: warps 0-15 = four worker warpgroups, warp 16 = weight producer.  Worker warpgroup w owns rows 64*(w%2) .. +64 and
 // columns NH*(w/2) .. +NH (NH = DP/2) of every GEMM output -- for the gate GEMM those columns of r AND of u -- so that the node state,
 // the gates, the candidate and their epilogues line up element for element in each thread's wgmma accumulator fragment, and the fp32
-// master copy of the node states stays in registers for the whole launch (LOCAL mode: the recurrence never leaves the SM).  The gathers
-// are row-per-thread over all 16 worker warps.
+// master copy of the node states stays in registers for the whole launch (LOCAL mode: the recurrence never leaves the SM).  On compact
+// tiles (<= 64 rows) all four warpgroups work on rows 0..63 and split the columns four ways instead (COMPACT_WIDTH), so none of them
+// idles on rows that do not exist.  The gathers are row-per-thread over all 16 worker warps.
 //
 // Shared memory: three A-operand tiles (h, agg, A_t / r*h), each hi+lo in the canonical K-major no-swizzle layout
 //   byte(row, k) = part*PART_B + (k/8)*KGS + row*16 + (k%8)*2     (KGS = 16 * allocated rows: 2048, or 1024 for compact <= 64-row tiles)
@@ -267,16 +268,16 @@ struct RingWriter {
 };
 
 // acc += A(op) . B(one DP x DP weight block: ceil(NKS/2) slots of two K-steps, each stage = [hi | lo]) for one worker warpgroup: A rows from
-// byte a_row on (k-group stride KGS, lo part PART_B after hi), B columns NH*nh .. +NH.  x3: three MMAs per product.  A warpgroup without rows
+// byte a_row on (k-group stride KGS, lo part PART_B after hi), B columns col0 .. +NH.  x3: three MMAs per product.  A warpgroup without rows
 // (mma_rows false) skips the MMAs but still takes and releases every slot.
 template <int NH>
 __device__ __forceinline__ void gemm_narrow(RingReader& ring, float (&acc)[NH / 2], const uint8_t* op, int NKS, int DP, uint32_t KGS, uint32_t PART_B,
-                                            uint32_t STAGE_B, uint32_t a_row, int nh, bool mma_rows, bool x3, int lane) {
+                                            uint32_t STAGE_B, uint32_t a_row, int col0, bool mma_rows, bool x3, int lane) {
     const int nslots = (NKS + 1) / 2;
     for (int i = 0; i < nslots; ++i) {
         const uint32_t sl = ring.take();
         if (mma_rows) {
-            const uint32_t b0 = ring.base + sl * 2u * STAGE_B + (uint32_t)nh * NH * 16u;
+            const uint32_t b0 = ring.base + sl * 2u * STAGE_B + (uint32_t)col0 * 16u;
             const int nk = (2 * i + 1 < NKS) ? 2 : 1;
             wg::fence();
             for (int h = 0; h < nk; ++h) {
@@ -296,10 +297,21 @@ __device__ __forceinline__ void gemm_narrow(RingReader& ring, float (&acc)[NH / 
     }
 }
 
-template <bool LOCAL, int NH>
+// Column split of the compact layout (tiles of <= 64 rows): all four worker warpgroups on MMA rows 0..63, each with about a quarter of the
+// DP = 2*NH output columns.  Every warpgroup computes the same width WC, DP/4 rounded up to a multiple of 8 (the wgmma N), so one body
+// serves them all: warpgroup w computes columns min(w*WC, DP-WC) .. +WC and owns -- stores -- those from w*WC on.  DP = 16k, k odd: 4k+4
+// columns, the last warpgroup recomputing 8 of its neighbour's (DP = 112: owned 32/32/32/16); at DP = 16 and 48 the last warpgroup owns
+// no columns.  The slowest warpgroup's MMA chain is as long as with unequal widths (4k+4, 4k+4, 4k-4, 4k-4).
+template <int NH>
+constexpr int COMPACT_WIDTH = (NH / 2) % 8 == 0 ? NH / 2 : NH / 2 + 4;
+
+// COMPACT: every tile has <= 64 rows (k-group stride 1024) and the four warpgroups split the columns (COMPACT_WIDTH); otherwise
+// warpgroup w owns MMA rows 64*(w%2) .. +64 and columns NH*(w/2) .. +NH.
+template <bool LOCAL, int NH, bool COMPACT>
 __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_constant__ TcParams p) {
-    constexpr int NF = NH / 2;   // accumulator floats per thread and quantity (m64 x NH fragment)
-    constexpr int NJ = NH / 8;   // 8-column blocks of a fragment
+    constexpr int WN = COMPACT ? COMPACT_WIDTH<NH> : NH;   // the columns of one warpgroup (wgmma N, an instruction immediate)
+    constexpr int NF = WN / 2;   // accumulator floats per thread and quantity (m64 x WN fragment)
+    constexpr int NJ = WN / 8;   // 8-column blocks of a fragment
     extern __shared__ __align__(1024) uint8_t smem[];
     __shared__ __align__(8) uint64_t bar_full[MAX_STAGES];    // weight slot landed
     __shared__ __align__(8) uint64_t bar_empty[MAX_STAGES];   // every worker warp is done with the slot
@@ -308,7 +320,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
     const int D = p.D, DP = p.DP, T = p.T;
     const int NKC = DP >> 3;   // 8-column chunks per DP
     const int NKS = DP >> 4;   // K-steps (16) per DP-wide operand
-    const uint32_t KGS = (uint32_t)p.kgs;
+    const uint32_t KGS = COMPACT ? 1024u : (uint32_t)p.kgs;
     const uint32_t PART_B = (uint32_t)DP * KGS / 8u;   // bytes per part (hi or lo)
     const uint32_t OPB = 2u * PART_B;                  // bytes per A operand (hi + lo)
     const uint32_t STAGE_B = (uint32_t)DP * 64u;       // bytes per weight stage (K = 16 x N = DP, hi + lo)
@@ -345,19 +357,22 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
         const int nkc_tile = NKC;
         constexpr int NCG = NUM_WORKERS / 128;
         const int row = q * 32 + lane;
-        // ---- fragment view (GEMMs and epilogues): warpgroup wgi owns rows 64*mh .. +64, columns NH*nh .. +NH
-        const int wgi = warp >> 2, mh = wgi & 1, nh = wgi >> 1;
-        const int fr0 = mh * 64 + (warp & 3) * 16 + (lane >> 2);    // fragment rows fr0, fr0 + 8
-        const int fc0 = nh * NH + (lane & 3) * 2;                   // fragment columns fc0 + 8j, fc0 + 8j + 1
-        const bool mma_rows = mh * 64 < rows;                       // warpgroup-uniform: the warpgroup has rows at all
+        // ---- fragment view (GEMMs and epilogues): warpgroup wgi computes rows m0 .. +64, columns col0 .. +WN, and owns those from own0 on
+        const int wgi = warp >> 2;
+        const int m0 = COMPACT ? 0 : 64 * (wgi & 1);
+        const int own0 = COMPACT ? WN * wgi : NH * (wgi >> 1);
+        const int col0 = COMPACT ? min(own0, DP - WN) : own0;
+        const int fr0 = m0 + (warp & 3) * 16 + (lane >> 2);         // fragment rows fr0, fr0 + 8
+        const int fc0 = col0 + (lane & 3) * 2;                      // fragment columns fc0 + 8j, fc0 + 8j + 1
+        const bool mma_rows = m0 < rows;                            // warpgroup-uniform: the warpgroup has rows at all
         const bool x3 = p.nparts == 3;
         bool ok = true;
         auto workers_sync = [&]() { tc::workers_sync(abortp, ok); };
         auto publish_sync = [&]() { fence_async_smem(); workers_sync(); };   // operand tiles written -> visible to wgmma
         RingReader rd{bar_full, bar_empty, abortp, smem_u32(ring), (uint32_t)nst};
-        const uint32_t a_row = (uint32_t)mh * 64u * 16u;   // this warpgroup's first row inside an A operand
+        const uint32_t a_row = (uint32_t)m0 * 16u;   // this warpgroup's first row inside an A operand
         auto gemm_narrow = [&](float (&acc)[NF], const uint8_t* op) {
-            tc::gemm_narrow<NH>(rd, acc, op, NKS, DP, KGS, PART_B, STAGE_B, a_row, nh, mma_rows, x3, lane);
+            tc::gemm_narrow<WN>(rd, acc, op, NKS, DP, KGS, PART_B, STAGE_B, a_row, col0, mma_rows, x3, lane);
         };
         // [r | u] += A(op) . B(one segment of the N = 2*DP gate block: NKS slots, stage 0 = hi, stage 1 = lo); columns of r and of u
         auto gemm_wide = [&](float (&ar)[NF], float (&au)[NF], const uint8_t* op) {
@@ -365,18 +380,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
                 const uint32_t sl = rd.take();
                 if (mma_rows) {
                     const uint32_t bh = rd.base + sl * 2u * STAGE_B, bl = bh + STAGE_B;
-                    const uint32_t cr = (uint32_t)nh * NH * 16u, cu = (uint32_t)(DP + nh * NH) * 16u, lbo = 32u * DP;
+                    const uint32_t cr = (uint32_t)col0 * 16u, cu = (uint32_t)(DP + col0) * 16u, lbo = 32u * DP;
                     const uint32_t a = smem_u32(op) + (uint32_t)i * 2u * KGS + a_row;
                     const uint64_t ad = wg::make_desc(a, KGS, 128);
                     wg::fence();
-                    wg::Mma<NH>::run(ar, ad, wg::make_desc(bh + cr, lbo, 128));
-                    wg::Mma<NH>::run(au, ad, wg::make_desc(bh + cu, lbo, 128));
+                    wg::Mma<WN>::run(ar, ad, wg::make_desc(bh + cr, lbo, 128));
+                    wg::Mma<WN>::run(au, ad, wg::make_desc(bh + cu, lbo, 128));
                     if (x3) {
                         const uint64_t al = wg::make_desc(a + PART_B, KGS, 128);
-                        wg::Mma<NH>::run(ar, ad, wg::make_desc(bl + cr, lbo, 128));
-                        wg::Mma<NH>::run(au, ad, wg::make_desc(bl + cu, lbo, 128));
-                        wg::Mma<NH>::run(ar, al, wg::make_desc(bh + cr, lbo, 128));
-                        wg::Mma<NH>::run(au, al, wg::make_desc(bh + cu, lbo, 128));
+                        wg::Mma<WN>::run(ar, ad, wg::make_desc(bl + cr, lbo, 128));
+                        wg::Mma<WN>::run(au, ad, wg::make_desc(bl + cu, lbo, 128));
+                        wg::Mma<WN>::run(ar, al, wg::make_desc(bh + cr, lbo, 128));
+                        wg::Mma<WN>::run(au, al, wg::make_desc(bh + cu, lbo, 128));
                     }
                     wg::commit();
                     wg::wait_all();
@@ -388,7 +403,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
 #pragma unroll
             for (int i = 0; i < NF; ++i) a[i] = 0.0f;
         };
-        // fragment element (j, half, e) = acc[4j + 2*half + e]: row fr0 + 8*half, column fc0 + 8j + e
+        // fragment element (j, half, e) = acc[4j + 2*half + e]: row fr0 + 8*half, column fc0 + 8j + e.  The epilogues visit the elements
+        // of the columns the warpgroup owns only (the others are stored by their owner and never read back by this warpgroup).
 #define GGNN_FRAG_PAIRS(...)                                                    \
     _Pragma("unroll") for (int j = 0; j < NJ; ++j)                              \
     _Pragma("unroll") for (int hf = 0; hf < 2; ++hf) {                          \
@@ -397,11 +413,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
         const bool fok = fr < rows && fc < D;                                   \
         const int fg = row0 + (fr < rows ? fr : 0);                             \
         (void)fi; (void)fok; (void)fg;                                          \
-        __VA_ARGS__                                                             \
+        if (!COMPACT || fc >= own0) { __VA_ARGS__ }                             \
     }
 
         // ---- initial state: global fp32 -> registers (fp32 master) + opH (bf16 hi/lo)
         float hs[NF];
+        if (COMPACT) zero(hs);   // (the elements of columns the warpgroup does not own are never loaded)
         {
             const float* hin = LOCAL ? p.state[0] : p.g_in;
             GGNN_FRAG_PAIRS({

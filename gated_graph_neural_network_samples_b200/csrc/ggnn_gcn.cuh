@@ -140,7 +140,7 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid
             float acc[NF];
 #pragma unroll
             for (int i = 0; i < NF; ++i) acc[i] = 0.f;
-            gemm_narrow<NH>(rd, acc, opS, NKS, DP, KGS, PART_B, STAGE_B, a_row, nh, mma_rows, x3, lane);
+            gemm_narrow<NH>(rd, acc, opS, NKS, DP, KGS, PART_B, STAGE_B, a_row, nh * NH, mma_rows, x3, lane);
             // ---- epilogue: bias, relu, dropout; the state goes back to the tile (LOCAL) and to global memory
             const bool to_smem = LOCAL && l + 1 < l_end;
             const bool to_global = !LOCAL || l + 1 == l_end || p.save;
