@@ -66,11 +66,7 @@ class DenseGGNNChemModel(ChemModel):
         adj = np.asarray(feed[self.placeholders['adjacency_matrix']], dtype=np.float32)          # [b, e, v, v]
         b, v = adj.shape[0], adj.shape[2]
         self.engine.set_save_for_backward(torch.is_grad_enabled())
-        prepared = feed.get('_prepared_graph')
-        if prepared is not None and prepared.for_training == torch.is_grad_enabled():
-            self.engine.set_graph_prepared(prepared)     # built by the batch producer thread: only the upload is left
-            self._prepared_pool.append(prepared)
-        else:
+        if not self._adopt_prepared_graph(feed):     # a graph built by the batch producer thread leaves only the upload
             self.engine.set_graph_dense(adj)
         keep = float(feed.get(self.placeholders['edge_weight_dropout_keep_prob'], 1.0))
         edge_weights = self.weights['edge_weights']
@@ -158,8 +154,6 @@ class DenseGGNNChemModel(ChemModel):
             # half of the batch (0/1 adjacency -> edge lists -> CSR, tile plan, one pinned image) is built here, next to the packing
             eng = getattr(self, 'engine', None)
             if getattr(self, 'prepare_graphs_in_producer', True) and hasattr(eng, 'prepare_graph_dense'):
-                pool = self.__dict__.setdefault('_prepared_pool', [])
-                g = eng.prepare_graph_dense(feed['adjacency_matrix'], save_for_backward=is_training, reuse=pool.pop() if pool else None)
-                g.for_training = bool(is_training)
-                feed['_prepared_graph'] = g
+                feed['_prepared_graph'] = self._prepare_from_pool(
+                    lambda reuse: eng.prepare_graph_dense(feed['adjacency_matrix'], save_for_backward=is_training, reuse=reuse), is_training)
             yield feed

@@ -242,6 +242,41 @@ class ChemModel(object):
         import torch
         return torch.as_tensor(np.asarray(self.feed[self.placeholders['initial_node_representation']], dtype=np.float32), device=self.device)
 
+    # ------------------------------------------------------------------ batch plumbing the plug-ins share
+    def _flat_view(self, data, flatten):
+        """(``flatten(data)``, the flat ids of ``data``'s graphs in the list's current order).  The flattened graphs are built once per list
+        object and kept while the list keeps its graphs (it is shuffled in place every epoch); graphs are identified by object identity, so
+        copies of the list or a changed membership simply rebuild."""
+        cache = self.__dict__.setdefault('_flat_cache', [])
+        for ref, flat, pos in cache:
+            if ref is data and flat.num_graphs == len(data):
+                try:
+                    return flat, np.fromiter((pos[id(g)] for g in data), dtype=np.int64, count=len(data))
+                except KeyError:
+                    break
+        flat = flatten(data)
+        cache[:] = [c for c in cache if c[0] is not data][-3:] + [(data, flat, {id(g): i for i, g in enumerate(data)})]
+        return flat, np.arange(len(data), dtype=np.int64)
+
+    def _prepare_from_pool(self, prepare, is_training: bool):
+        """Runs in the batch producer thread: ``prepare(reuse)`` builds the host half of one batch's graph (into a prepared graph taken back
+        from the pool when there is one), tagged with whether it was built for training."""
+        pool = self.__dict__.setdefault('_prepared_pool', [])
+        g = prepare(pool.pop() if pool else None)
+        g.for_training = bool(is_training)
+        return g
+
+    def _adopt_prepared_graph(self, feed) -> bool:
+        """Hook 2's half of the above: uploads the feed's prepared graph when it was built for this kind of step (training or not) and
+        returns True; False means the caller sets the graph from the feed itself."""
+        import torch
+        prepared = feed.get('_prepared_graph')
+        if prepared is None or prepared.for_training != torch.is_grad_enabled():
+            return False
+        self.engine.set_graph_prepared(prepared)
+        self.__dict__.setdefault('_prepared_pool', []).append(prepared)   # rebuilt in place for a later batch; a rebuild first waits for this upload
+        return True
+
     # ------------------------------------------------------------------ epoch loop (chem_tensorflow.py:214-253)
     # per-task "chemical accuracy" thresholds of QM9 the reference reports error ratios against (chem_tensorflow.py:215-217)
     CHEMICAL_ACCURACIES = np.array([0.066513725, 0.012235489, 0.071939046, 0.033730778, 0.033486113, 0.004278493, 0.001330901,

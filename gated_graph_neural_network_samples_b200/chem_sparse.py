@@ -159,12 +159,8 @@ class SparseGGNNChemModel(ChemModel):
         T, D = self.num_edge_types, self.params['hidden_size']
         adjacency_lists = [feed[k] for k in self.placeholders['adjacency_lists']]
         self.engine.set_save_for_backward(torch.is_grad_enabled())   # before set_graph: the source-keyed CSR is built there
-        prepared = feed.get('_prepared_graph')
-        if prepared is not None and prepared.for_training == torch.is_grad_enabled():
-            # the host half (CSR, tile plan, pinned image) was built by the batch producer thread: only the upload is left
-            self.engine.set_graph_prepared(prepared)
-            self._prepared_pool.append(prepared)    # rebuilt in place for a later batch; a rebuild first waits for this upload
-        else:
+        # the host half (CSR, tile plan, pinned image) was built by the batch producer thread when the feed carries it: only the upload is left
+        if not self._adopt_prepared_graph(feed):
             self.engine.set_graph_sparse(adjacency_lists, feed[self.placeholders['num_incoming_edges_per_type']])
         state_keep = float(feed.get(self.placeholders['graph_state_keep_prob'], 1.0))
         # DropoutWrapper(state_keep_prob), sparse:113-114: done inside the kernels; a fresh mask seed per run, drawn from
@@ -253,21 +249,6 @@ class SparseGGNNChemModel(ChemModel):
                         processed[ex_id]['labels'][task_id] = None
         return processed
 
-    def _flat_view(self, data):
-        """(FlatSparseGraphs of the graphs in ``data``, their flat ids in the list's current order).  Built once per list object and kept
-        while the list keeps its graphs (it is shuffled in place every epoch, sparse:281-282); graphs are identified by object
-        identity, so copies of the list or a changed membership simply rebuild."""
-        cache = self.__dict__.setdefault('_flat_cache', [])
-        for ref, flat, pos in cache:
-            if ref is data and flat.num_graphs == len(data):
-                try:
-                    return flat, np.fromiter((pos[id(g)] for g in data), dtype=np.int64, count=len(data))
-                except KeyError:
-                    break
-        flat = packing.FlatSparseGraphs(data, self.num_edge_types)
-        cache[:] = [c for c in cache if c[0] is not data][-3:] + [(data, flat, {id(g): i for i, g in enumerate(data)})]
-        return flat, np.arange(len(data), dtype=np.int64)
-
     def make_minibatch_iterator(self, data: Any, is_training: bool):
         if is_training:
             np.random.shuffle(data)                                                              # sparse:281-282
@@ -275,7 +256,7 @@ class SparseGGNNChemModel(ChemModel):
         edge_keep = self.params['edge_weight_dropout_keep_prob'] if is_training else 1.
         # the processed graphs are flattened once per dataset (packing.FlatSparseGraphs); every batch is then a handful of NumPy gathers
         # instead of the per-graph loop of sparse:288-350 -- same arrays, bit for bit (tests/test_packing.py)
-        flat, order = self._flat_view(data)
+        flat, order = self._flat_view(data, lambda d: packing.FlatSparseGraphs(d, self.num_edge_types))   # kept across epochs (sparse:281-282)
         for b in flat.iter_minibatches(order, self.params['batch_size'], self.params['hidden_size']):
             feed = {k: b[k] for k in ('initial_node_representation', 'num_incoming_edges_per_type', 'graph_nodes_list',
                                       'target_values', 'target_mask', 'num_graphs')}
@@ -287,10 +268,7 @@ class SparseGGNNChemModel(ChemModel):
             # validation, stable target-sorted CSR, tile plan, one pinned image -- is done HERE, next to the packing it follows in the
             # reference (sparse:288-350), so the consumer thread only enqueues the upload and the kernels (SURVEY 8 f3)
             if getattr(self, 'prepare_graphs_in_producer', True) and hasattr(getattr(self, 'engine', None), 'prepare_graph_sparse'):
-                pool = self.__dict__.setdefault('_prepared_pool', [])
-                reuse = pool.pop() if pool else None
-                g = self.engine.prepare_graph_sparse(b['adjacency_lists'], b['num_incoming_edges_per_type'], save_for_backward=is_training,
-                                                     reuse=reuse)
-                g.for_training = bool(is_training)
-                feed['_prepared_graph'] = g
+                feed['_prepared_graph'] = self._prepare_from_pool(
+                    lambda reuse: self.engine.prepare_graph_sparse(b['adjacency_lists'], b['num_incoming_edges_per_type'],
+                                                                   save_for_backward=is_training, reuse=reuse), is_training)
             yield feed

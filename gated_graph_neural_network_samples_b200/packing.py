@@ -106,7 +106,34 @@ def iter_sparse_minibatches(data: Sequence[dict], batch_size_nodes: int, hidden_
         yield pack_sparse_batch(data[start:i], hidden_size, num_edge_types)
 
 
-class FlatSparseGraphs:
+class _FlatGraphs:
+    """What the flattened graph sets share: ``n_nodes`` per graph, ``pack(idx, hidden_size)`` for one batch, and the node-budget batching."""
+
+    @staticmethod
+    def _ranges(starts: np.ndarray, lengths: np.ndarray) -> np.ndarray:
+        """Concatenation of arange(starts[i], starts[i] + lengths[i])."""
+        total = int(lengths.sum())
+        if total == 0:
+            return np.zeros(0, np.int64)
+        out_off = np.cumsum(lengths) - lengths
+        return np.arange(total, dtype=np.int64) + np.repeat(starts - out_off, lengths)
+
+    def iter_minibatches(self, order, batch_size_nodes: int, hidden_size: int):
+        """The greedy node-budget batching of sparse:286-297 / gcn:150-162 over the graphs in ``order`` (flat ids)."""
+        order = np.asarray(order, dtype=np.int64)
+        csum = np.cumsum(self.n_nodes[order])
+        start, N = 0, order.shape[0]
+        while start < N:
+            base = int(csum[start - 1]) if start else 0
+            end = int(np.searchsorted(csum, base + batch_size_nodes, side="left"))   # graphs whose running node count stays < budget
+            if end == start:
+                raise Exception("graph %d has %d nodes and does not fit batch_size=%d"
+                                % (start, int(self.n_nodes[order[start]]), batch_size_nodes))
+            yield self.pack(order[start:end], hidden_size)
+            start = end
+
+
+class FlatSparseGraphs(_FlatGraphs):
     """Processed graphs (``process_raw_graphs_sparse``) flattened ONCE into a few contiguous arrays, so that assembling a batch
     is a constant number of NumPy gathers instead of the per-graph Python loop of sparse:288-350 (SURVEY 8f-3: at a 100 k-node
     batch the loop costs ~0.26 s against a 9 ms training step).  ``pack(idx)`` returns exactly what
@@ -146,15 +173,6 @@ class FlatSparseGraphs:
                     self.labels[i, k] = v
                     self.mask[i, k] = 1.0
 
-    @staticmethod
-    def _ranges(starts: np.ndarray, lengths: np.ndarray) -> np.ndarray:
-        """Concatenation of arange(starts[i], starts[i] + lengths[i])."""
-        total = int(lengths.sum())
-        if total == 0:
-            return np.zeros(0, np.int64)
-        out_off = np.cumsum(lengths) - lengths
-        return np.arange(total, dtype=np.int64) + np.repeat(starts - out_off, lengths)
-
     def pack(self, idx, hidden_size: int) -> dict:
         idx = np.asarray(idx, dtype=np.int64)
         G, T = idx.shape[0], self.num_edge_types
@@ -179,20 +197,6 @@ class FlatSparseGraphs:
             "target_mask": np.ascontiguousarray(self.mask[idx].T).reshape(-1, G),
             "num_graphs": G,
         }
-
-    def iter_minibatches(self, order, batch_size_nodes: int, hidden_size: int):
-        """The greedy node-budget batching of sparse:286-297 over the graphs in ``order`` (flat ids)."""
-        order = np.asarray(order, dtype=np.int64)
-        csum = np.cumsum(self.n_nodes[order])
-        start, N = 0, order.shape[0]
-        while start < N:
-            base = int(csum[start - 1]) if start else 0
-            end = int(np.searchsorted(csum, base + batch_size_nodes, side="left"))   # graphs whose running node count stays < budget
-            if end == start:
-                raise Exception("graph %d has %d nodes and does not fit batch_size=%d"
-                                % (start, int(self.n_nodes[order[start]]), batch_size_nodes))
-            yield self.pack(order[start:end], hidden_size)
-            start = end
 
 
 # ------------------------------------------------------------------------------------------- dense
@@ -317,3 +321,54 @@ def iter_gcn_minibatches(data: Sequence[dict], batch_size_nodes: int, hidden_siz
             raise Exception("graph %d has %d nodes and does not fit batch_size=%d"
                             % (i, len(data[i]["init"]), batch_size_nodes))  # the reference loops forever here
         yield pack_gcn_batch(data[start:i], hidden_size)
+
+
+class FlatGCNGraphs(_FlatGraphs):
+    """Processed GCN graphs (``process_raw_graphs_gcn``) flattened ONCE -- features, graph-local adjacency lists, float64 weights, labels,
+    node and entry offsets -- so that a batch is a few NumPy gathers instead of the per-graph loop of gcn:150-197 (at the default
+    100 000-node budget that loop is the producer thread's whole cost).  ``pack(idx)`` returns exactly what
+    ``pack_gcn_batch([graphs[i] for i in idx])`` returns: same keys, dtypes and values."""
+
+    def __init__(self, graphs: Sequence[dict]):
+        N = len(graphs)
+        self.num_graphs = N
+        self.n_nodes = np.fromiter((len(g["init"]) for g in graphs), dtype=np.int64, count=N)
+        self.node_off = np.concatenate([[0], np.cumsum(self.n_nodes)])
+        lists = [np.asarray(g["adjacency_list"], np.int64).reshape(-1, 2) for g in graphs]
+        self.entry_off = np.concatenate([[0], np.cumsum([l.shape[0] for l in lists])]).astype(np.int64)
+        self.lists = np.concatenate(lists, axis=0) if N else np.zeros((0, 2), np.int64)
+        self.weights = (np.concatenate([np.asarray(g["adjacency_weights"], np.float64).reshape(-1) for g in graphs]) if N
+                        else np.zeros(0, np.float64))
+        self.ann = max((np.asarray(g["init"]).shape[1] for g in graphs), default=0)
+        self.feat = np.zeros((int(self.node_off[-1]), self.ann), np.float32)
+        ntasks = len(graphs[0]["labels"]) if N else 0
+        self.labels = np.zeros((N, ntasks), np.float32)
+        self.mask = np.zeros((N, ntasks), np.float32)
+        for i, g in enumerate(graphs):
+            init = np.asarray(g["init"], np.float32)
+            o = int(self.node_off[i])
+            self.feat[o:o + init.shape[0], :init.shape[1]] = init
+            for k, v in enumerate(g["labels"]):
+                if v is not None:
+                    self.labels[i, k] = v
+                    self.mask[i, k] = 1.0
+
+    def pack(self, idx, hidden_size: int) -> dict:
+        idx = np.asarray(idx, dtype=np.int64)
+        G = idx.shape[0]
+        n = self.n_nodes[idx]
+        batch_off = np.cumsum(n) - n                                            # node offset of each graph in the batch (gcn:170)
+        nodes = self._ranges(self.node_off[idx], n)
+        feats = np.zeros((nodes.shape[0], hidden_size), np.float32)             # gcn:165-167
+        feats[:, :self.ann] = self.feat[nodes]
+        m = self.entry_off[idx + 1] - self.entry_off[idx]
+        rows = self._ranges(self.entry_off[idx], m)
+        return {
+            "initial_node_representation": feats,
+            "adjacency_list": self.lists[rows] + np.repeat(batch_off, m)[:, None],
+            "adjacency_weights": self.weights[rows],
+            "graph_nodes_list": np.repeat(np.arange(G, dtype=np.int32), n),     # gcn:169
+            "target_values": np.ascontiguousarray(self.labels[idx].T).reshape(-1, G),
+            "target_mask": np.ascontiguousarray(self.mask[idx].T).reshape(-1, G),
+            "num_graphs": G,
+        }
