@@ -97,9 +97,10 @@ class DenseGGNNChemModel(ChemModel):
         import torch
         D = self.params['hidden_size']
         h0 = self.initial_node_representation_tensor()
-        ag = regression_gate.affine() if hasattr(regression_gate, 'affine') else None
-        at = regression_transform.affine() if hasattr(regression_transform, 'affine') else None
-        if ag is not None and at is not None and last_h.is_cuda and getattr(self, '_padded_hidden', D) == D:   # fused kernel (SURVEY 8f-1): masked per-graph sum included
+        fused = last_h.is_cuda and getattr(self, '_padded_hidden', D) == D   # affine() draws the weight-dropout mask: only when it is used
+        ag = regression_gate.affine() if fused and hasattr(regression_gate, 'affine') else None
+        at = regression_transform.affine() if fused and hasattr(regression_transform, 'affine') else None
+        if ag is not None and at is not None:   # fused kernel (SURVEY 8f-1): masked per-graph sum included
             b, v = last_h.shape[0], last_h.shape[1]
             self.engine.readout_set_graphs(b, nodes_per_graph=v, node_mask=self.feed[self.placeholders['node_mask']])
             self.output = self._readout.apply(self.engine, last_h.reshape(b * v, D), h0.reshape(b * v, D), ag[0], ag[1], at[0], at[1])

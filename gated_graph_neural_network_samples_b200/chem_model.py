@@ -14,6 +14,7 @@ runs in libggnn_b200.so.
 from __future__ import annotations
 
 import json
+import math
 import os
 import pickle
 import random
@@ -188,7 +189,21 @@ class ChemModel(object):
                     print("Freezing weights of variable %s." % n)
             named = [(n, v) for n, v in named if id(v) not in frozen]
         self._train_vars = named
-        self.optimizer = torch.optim.Adam([v for _, v in named], lr=self.params['learning_rate'], eps=1e-8)   # tf.train.AdamOptimizer defaults
+        # tf.train.AdamOptimizer defaults (beta1 0.9, beta2 0.999, epsilon 1e-8); _set_tf_adam_epsilon turns torch's update into TF's
+        self.optimizer = torch.optim.Adam([v for _, v in named], lr=self.params['learning_rate'], eps=self.ADAM_EPSILON)
+
+    ADAM_EPSILON = 1e-8
+
+    def _set_tf_adam_epsilon(self):
+        """TF 1.3's ApplyAdam updates  var -= lr * sqrt(1 - b2^t) / (1 - b1^t) * m / (sqrt(v) + eps);  torch's Adam updates
+        var -= lr / (1 - b1^t) * m / (sqrt(v) / sqrt(1 - b2^t) + eps).  The two agree when torch's eps is eps / sqrt(1 - b2^t) for the
+        step t about to be taken; left as it is, torch's effective epsilon is 3e-10 at t = 1 and small gradients (biases, rare edge
+        types) take steps several times TF's.  All trainables step together, so one counter serves the group."""
+        opt = self.optimizer
+        for group in opt.param_groups:
+            st = next((opt.state[p] for p in group['params'] if opt.state.get(p)), None)
+            t = (int(st['step']) if st else 0) + 1
+            group['eps'] = self.ADAM_EPSILON / math.sqrt(1.0 - group['betas'][1] ** t)
 
     def train_step(self, loss):
         """Adam step with per-variable clip_by_norm (chem_tensorflow.py:183-191).  Under torch.distributed the gradient is the one of
@@ -211,6 +226,7 @@ class ChemModel(object):
                 n = v.grad.norm()
                 if n > clamp:
                     v.grad.mul_(clamp / n)
+        self._set_tf_adam_epsilon()
         self.optimizer.step()
         self.after_weight_update()
         return active

@@ -221,9 +221,11 @@ class SparseGGNNChemModel(ChemModel):
     def gated_regression(self, last_h, regression_gate, regression_transform):
         import torch
         h0 = self.initial_node_representation_tensor()
-        ag = regression_gate.affine() if hasattr(regression_gate, 'affine') else None
-        at = regression_transform.affine() if hasattr(regression_transform, 'affine') else None
-        if ag is not None and at is not None and last_h.is_cuda and getattr(self, '_padded_hidden', last_h.shape[-1]) == last_h.shape[-1]:
+        # affine() draws the out-layer weight-dropout mask: asked only when the fused kernel will use it, so each weight gets one mask
+        fused = last_h.is_cuda and getattr(self, '_padded_hidden', last_h.shape[-1]) == last_h.shape[-1]
+        ag = regression_gate.affine() if fused and hasattr(regression_gate, 'affine') else None
+        at = regression_transform.affine() if fused and hasattr(regression_transform, 'affine') else None
+        if ag is not None and at is not None:
             # the fused kernel: both dot products, sigmoid, product and the per-graph segment sum in one launch
             self.engine.readout_set_graphs(int(self.feed[self.placeholders['num_graphs']]),
                                            graph_nodes_list=self.feed[self.placeholders['graph_nodes_list']])

@@ -360,11 +360,24 @@ def state_dropout_mask(seed, global_step, V, D, keep):
     return u < np.float32(keep)
 
 
+def _apply_state_dropout(h, state_dropout, global_step, mask_width):
+    """DropoutWrapper on the new state with the engine's mask (state_dropout_mask).  An engine running a hidden size zero-padded to a
+    multiple of 4 draws its mask at the padded width: ``mask_width`` is that width, and the first D columns of its mask apply."""
+    import torch
+    if state_dropout is None or state_dropout[0] >= 1.0:
+        return h
+    keep, seed = state_dropout
+    V, D = h.shape
+    mask = torch.from_numpy(state_dropout_mask(seed, global_step, V, mask_width or D, keep)[:, :D])
+    return torch.where(mask, h / float(np.float32(keep)), torch.zeros((), dtype=h.dtype))
+
+
 def sparse_propagation_torch(h0, adjacency_lists, num_incoming_edges_per_type, weights, params,
-                             return_all_layers=False, dtype=None, state_dropout=None):
+                             return_all_layers=False, dtype=None, state_dropout=None, mask_width=None):
     """Same ops and materialisations as sparse:159-216 with torch CPU fp32 kernels:
     index_select (embedding_lookup) -> matmul -> cat -> index_add_ (unsorted_segment_sum) -> matmul bias
-    -> divide -> cat -> explicit GRUCell/BasicRNNCell arithmetic.  Inputs may be NumPy or torch."""
+    -> divide -> cat -> explicit GRUCell/BasicRNNCell arithmetic.  Inputs may be NumPy or torch.
+    ``state_dropout`` = (keep, seed) and ``mask_width``: see _apply_state_dropout."""
     import torch
     dtype = dtype or torch.float32   # float64 + requires_grad tensors give the autograd reference for the backward tests
     t = lambda a: a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
@@ -417,16 +430,14 @@ def sparse_propagation_torch(h0, adjacency_lists, num_incoming_edges_per_type, w
                 states[-1] = u * h + (1 - u) * c
             else:
                 states[-1] = act(torch.matmul(torch.cat([x, h], -1), w["rnn_kernel"]) + w["rnn_bias"])
-            if state_dropout is not None and state_dropout[0] < 1.0:
-                keep, seed = state_dropout
-                mask = torch.from_numpy(state_dropout_mask(seed, global_step, V, D, keep))
-                states[-1] = torch.where(mask, states[-1] / float(np.float32(keep)), torch.zeros((), dtype=dtype))
+            states[-1] = _apply_state_dropout(states[-1], state_dropout, global_step, mask_width)
             global_step += 1
     return states if return_all_layers else states[-1]
 
 
-def dense_propagation_torch(h0, adjacency_matrix, weights, params, dtype=None):
-    """dense:100-115 with torch CPU fp32 kernels (matmul / batched matmul / GRUCell arithmetic)."""
+def dense_propagation_torch(h0, adjacency_matrix, weights, params, dtype=None, state_dropout=None, mask_width=None):
+    """dense:100-115 with torch CPU fp32 kernels (matmul / batched matmul / GRUCell arithmetic).  ``state_dropout`` (DropoutWrapper,
+    dense:89) as in sparse_propagation_torch, over the [b*v, D] state rows, one global step per timestep."""
     import torch
     dtype = dtype or torch.float32
     t = lambda a: a if isinstance(a, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(a))
@@ -436,7 +447,7 @@ def dense_propagation_torch(h0, adjacency_matrix, weights, params, dtype=None):
     b, v, D = h0.shape
     T = A.shape[0]
     h = h0.reshape(-1, D)
-    for _ in range(int(params["num_timesteps"])):
+    for step in range(int(params["num_timesteps"])):
         acts = None
         for e in range(T):
             m = torch.matmul(h, w["edge_weights"][e]).reshape(b, v, D)
@@ -448,7 +459,7 @@ def dense_propagation_torch(h0, adjacency_matrix, weights, params, dtype=None):
         ru = torch.sigmoid(torch.matmul(torch.cat([acts, h], -1), w["gate_kernel"]) + w["gate_bias"])
         r, u = ru[:, :D], ru[:, D:]
         c = torch.tanh(torch.matmul(torch.cat([acts, r * h], -1), w["cand_kernel"]) + w["cand_bias"])
-        h = u * h + (1 - u) * c
+        h = _apply_state_dropout(u * h + (1 - u) * c, state_dropout, step, mask_width)
     return h.reshape(b, v, D)
 
 
