@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <array>
 #include <chrono>
 #ifdef _OPENMP
 #include <omp.h>
@@ -164,16 +165,51 @@ struct BatchPlan {
     int64_t edges_of_type[32] = {0};
 };
 
+// Typed device pointers into the uploaded graph image of the current batch, made once per upload by ggnn_set_graph_prepared.  An array
+// the plan does not carry points at the start of the image.
+struct GraphDev {
+    const int *row_ptr, *csr_src, *csr_msg;
+    const float *indeg, *denom;
+    const int* tile_start;
+    const unsigned* tile_mask;
+    const float* dense_adj;
+    const int *trow, *ttgt, *tslot;                      // source-keyed CSR (save_for_backward)
+    const int *pair_src, *vrow_ptr, *vsrc, *tile_vptr;   // streaming plan
+    const int4* vinfo;
+    const float *slot_w, *tslot_w;                       // GCN: per-slot adjacency weights
+};
+
+// The weights in the pre-split, pre-tiled bf16 layout of one tensor-core kernel family, with each layer's offsets.  The tiles are rebuilt
+// when the weights changed since they were made (ggnn_set_weights / ggnn_gcn_set_weights bump the engine's weights generation) or when
+// the layout changed, and at no other time.
+struct WeightTiles {
+    DevBuf buf;
+    size_t off_edge[MAX_LAYERS] = {0}, off_gate[MAX_LAYERS] = {0}, off_cand[MAX_LAYERS] = {0};
+    uint64_t gen = 0;     // the weights generation the tiles were made from (0: none)
+    size_t bytes = 0;     // the layout they were made for: its size and, for the streaming layout, its N-block widths
+    int nc[2] = {0, 0};
+
+    // Makes room for a layout of `size` bytes and N-block widths n0 / n1.  `retile` says whether the tiles are not those of weights
+    // generation `want` in that layout; the caller then makes them and sets `gen`.
+    cudaError_t reserve(size_t size, int n0, int n1, uint64_t want, bool& retile) {
+        retile = gen != want || bytes != size || nc[0] != n0 || nc[1] != n1;
+        if (retile) { gen = 0; bytes = size; nc[0] = n0; nc[1] = n1; }
+        return buf.reserve(size);
+    }
+};
+
 }  // namespace
 
 struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     bool weights_set = false;
+    uint64_t weights_gen = 0;   // bumped by every successful ggnn_set_weights / ggnn_gcn_set_weights
     ggnn_layer_weights w[MAX_LAYERS];
     ggnn_gcn_layer_weights gcn_w[MAX_LAYERS] = {};
     bool graph_set = false;
 
     // device memory
     DevBuf graph_buf;   // the graph image of the current batch
+    GraphDev gd;        // ... and the view of it every driver reads
     // readout (gated_regression): node -> graph map of the current batch
     DevBuf ro_buf; StagedImage ro_stage;
     int ro_V = -1, ro_G = 0; bool ro_grouped = false, ro_has_mask = false;
@@ -182,18 +218,15 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     DevBuf save_bufs;   // 5 (CudnnCompatibleGRUCell: 6) x total_steps x [V][D]
     DevBuf io_buf;      // h0 / h_out staging for ggnn_forward_host
     DevBuf bwd_buf;     // backward scratch
-    DevBuf tc_weights;  // pre-split, pre-tiled bf16 copies of the weights (tensor-core path)
+    WeightTiles tc_tiles;   // the weights tiled for the tile-local wgmma kernel (GGNN) or the GCN wgmma kernel
+    WeightTiles ts_tiles;   // ... and for the streaming kernel
     DevBuf tc_respre;   // residual pre-products [ntiles][128][3*DP]
     DevBuf err_flag;    // device int written by kernels on a barrier timeout
-    bool weights_dirty = true;
-    size_t tc_off_edge[MAX_LAYERS] = {0}, tc_off_gate[MAX_LAYERS] = {0}, tc_off_cand[MAX_LAYERS] = {0};
     const float* last_h0 = nullptr;
     float* last_out = nullptr;
     bool save = false;
     bool saved_valid = false;
-    DevBuf ts_weights, ts_images, ts_u;
-    size_t ts_off_edge[MAX_LAYERS] = {0}, ts_off_gate[MAX_LAYERS] = {0}, ts_off_cand[MAX_LAYERS] = {0};
-    int ts_tiled_nc[2] = {-1, -1};                   // the N-block widths the tiled weights were made for
+    DevBuf ts_images;                                // the streaming plan's operand images and chunk-major states
     DevBuf ts_virt;                                  // the operand image of the streaming plan's virtual rows
     DevBuf att_buf;                  // attention probabilities per target-CSR slot ([steps][M] when saving for backward, else [M])
     float drop_keep = 1.0f; unsigned long long drop_seed = 0;          // state dropout for the next forward
@@ -222,8 +255,132 @@ struct ggnn_prepared_graph : ErrorText {
         if (_st != cudaSuccess) return (e)->fail(GGNN_ECUDA, "%s failed: %s", #call, cudaGetErrorString(_st)); \
     } while (0)
 
-static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers,
-                              float* d_h0, ggnn_stream_t stream);
+// ------------------------------------------------------------------------------------------ the engine's device buffers of a batch
+// Elements of one [V][D] state array (at least one row).
+static size_t state_elems(const ggnn_engine* e) { return (size_t)std::max(e->V, 1) * e->D; }
+
+// node_states_per_layer of the forward that read h0 and wrote h_out: [0] is h0 (only ever read), [L] is h_out, the layers between live at
+// the front of state_buf.
+static float* layer_state(const ggnn_engine* e, int l, const float* h0, float* h_out) {
+    if (l == 0) return const_cast<float*>(h0);
+    if (l == e->L) return h_out;
+    return (float*)e->state_buf.ptr + (size_t)(l - 1) * state_elems(e);
+}
+
+// The state pointers of a kernel's parameters (FwdParams, TcParams, GcnParams): read side [0..L], write side [1..L].
+template <class Params>
+static void set_layer_states(const ggnn_engine* e, Params& p, const float* h0, float* h_out) {
+    p.state[0] = h0;
+    for (int l = 1; l <= e->L; ++l) p.state[l] = p.state_w[l] = layer_state(e, l, h0, h_out);
+}
+
+// The GLOBAL plans' ping-pong temporaries (i = 0, 1) of a layer's inner timesteps: the two [V][D] slots of state_buf behind the layers.
+static float* step_temp(const ggnn_engine* e, int i) { return (float*)e->state_buf.ptr + (size_t)(e->L - 1 + i) * state_elems(e); }
+
+// The activations global step `gs` saves for the backward pass, each [V][D]: save_bufs holds 5 (CudnnCompatibleGRUCell: 6) arrays of
+// total_steps steps.  All null when save_for_backward is off.
+static SaveDev saved_step(const ggnn_engine* e, int gs) {
+    SaveDev s;
+    memset(&s, 0, sizeof s);
+    if (!e->save) return s;
+    const size_t per = state_elems(e) * (size_t)std::max(e->total_steps, 1);
+    float* b = (float*)e->save_bufs.ptr + (size_t)gs * state_elems(e);
+    s.h_in = b; s.agg = b + per; s.r = b + 2 * per; s.u = b + 3 * per; s.c = b + 4 * per;
+    s.q = e->cell == CELL_CUDNN_GRU ? b + 5 * per : nullptr;
+    return s;
+}
+
+// The fields the parameters of the fp32 and the tile-local wgmma kernels share (FwdParams, tc::TcParams); the rest is zero.
+template <class Params>
+static void fill_common_params(const ggnn_engine* e, Params& p, const float* h0, float* h_out) {
+    memset(&p, 0, sizeof p);
+    p.V = e->V; p.D = e->D; p.T = e->T; p.L = e->L;
+    p.use_bias = e->use_bias; p.use_avg = e->use_avg; p.cell = e->cell; p.act = e->act;
+    p.gather_mode = e->gather_mode; p.dense_v = e->dense_v; p.save = e->save ? 1 : 0;
+    p.drop_keep = e->drop_keep; p.drop_seed = e->drop_seed;
+    const GraphDev& gd = e->gd;
+    p.tile_start = gd.tile_start; p.tile_mask = gd.tile_mask; p.row_ptr = gd.row_ptr; p.csr_src = gd.csr_src;
+    p.dense_adj = gd.dense_adj; p.indeg = gd.indeg; p.denom = gd.denom;
+    set_layer_states(e, p, h0, h_out);
+    p.save_buf = saved_step(e, 0);   // the kernels index it by global step
+    for (int l = 0; l < e->L; ++l) {
+        p.layer[l].steps = e->steps[l]; p.layer[l].nres = e->nres[l];
+        for (int i = 0; i < MAX_RES; ++i) p.layer[l].res[i] = e->res[l][i];
+        p.step_base[l] = e->step_base[l];
+    }
+}
+
+// Runs a forward kernel of the fp32 or the tile-local wgmma family: `launch(p)` launches it once.  A LOCAL plan runs every layer and
+// timestep in one launch.  A GLOBAL plan launches once per timestep: a layer's inner timesteps ping-pong between the two step temporaries
+// and its last one writes the layer's state; a layer without timesteps aliases its input (sparse:152).
+template <class Params, class Launch>
+static int launch_steps(ggnn_engine* e, Params& p, cudaStream_t st, Launch launch) {
+    if (e->local) {
+        launch(p);
+        ++e->last_launches;
+        return GGNN_OK;
+    }
+    const size_t vd_bytes = (size_t)e->V * e->D * sizeof(float);
+    for (int l = 0; l < e->L; ++l) {
+        const float* in = p.state[l];
+        if (e->steps[l] == 0) {
+            CU_TRY(e, cudaMemcpyAsync(p.state_w[l + 1], in, vd_bytes, cudaMemcpyDeviceToDevice, st));
+            continue;
+        }
+        for (int s = 0; s < e->steps[l]; ++s) {
+            float* out = (s == e->steps[l] - 1) ? p.state_w[l + 1] : step_temp(e, s & 1);
+            p.g_layer = l; p.g_step = s; p.g_in = in; p.g_out = out;
+            launch(p);
+            ++e->last_launches;
+            in = out;
+        }
+    }
+    return GGNN_OK;
+}
+
+static int no_graph(ggnn_engine* e) {
+    return e->fail(GGNN_ESTATE, "no graph set (%s)", e->model == MODEL_GCN ? "ggnn_set_graph_gcn / ggnn_set_graph_prepared" : "ggnn_set_graph_sparse/dense");
+}
+
+// The gradient pointers of a layer; the weight-gradient kernels update them with 16-byte vector atomics.
+static std::array<const void*, 8> grad_pointers(const ggnn_layer_grads& g) {
+    return {g.edge_weights, g.edge_biases, g.gate_kernel, g.gate_bias, g.cand_kernel, g.cand_bias, g.edge_type_attention_weights, g.cand_hidden_bias};
+}
+static std::array<const void*, 8> grad_pointers(const ggnn_gcn_layer_grads& g) { return {g.kernel, g.bias}; }
+
+// The checks both backward calls start with.  `fn` names the call, `graph_call` the call that builds the source-keyed CSR.
+template <class Grads>
+static int begin_backward(ggnn_engine* e, const char* fn, const char* graph_call, const float* d_h_out, const Grads* grads, int num_layers,
+                          const float* d_h0) {
+    if (!e->graph_set || !e->weights_set) return e->fail(GGNN_ESTATE, "no graph / weights set");
+    if (!e->saved_valid) return e->fail(GGNN_ESTATE, "%s needs a preceding ggnn_forward with save_for_backward enabled", fn);
+    if (!e->has_transpose) return e->fail(GGNN_ESTATE, "enable save_for_backward BEFORE %s (the source-keyed CSR is built there)", graph_call);
+    if (!grads || num_layers != e->L || (!d_h_out && e->V > 0)) return e->fail(GGNN_EINVAL, "bad backward arguments");
+    for (int l = 0; l < e->L; ++l)
+        for (const void* q : grad_pointers(grads[l]))
+            if ((uintptr_t)q & 15) return e->fail(GGNN_EINVAL, "layer %d: gradient pointers must be 16-byte aligned", l);
+    if (((uintptr_t)d_h_out & 15) || ((uintptr_t)d_h0 & 15)) return e->fail(GGNN_EINVAL, "d_h_out / d_h0 must be 16-byte aligned");
+    CU_TRY(e, cudaSetDevice(e->device));
+    e->last_launches = 0;
+    return GGNN_OK;
+}
+
+// The device side of the host-buffer calls: h0 and h_out in two 256-byte-aligned slots at the front of io_buf, `scratch_bytes` more
+// behind them.  Enqueues the upload of the `bytes` of h0.
+struct IoSlots {
+    float* in;
+    float* out;
+    char* scratch;
+};
+static int stage_io(ggnn_engine* e, const float* h0_host, size_t bytes, size_t scratch_bytes, cudaStream_t st, IoSlots& io) {
+    CU_TRY(e, cudaSetDevice(e->device));
+    const size_t slot = align_up(std::max<size_t>(bytes, 16), 256);
+    CU_TRY(e, e->io_buf.reserve(2 * slot + scratch_bytes));
+    char* b = (char*)e->io_buf.ptr;
+    io = IoSlots{(float*)b, (float*)(b + slot), b + 2 * slot};
+    if (bytes) CU_TRY(e, cudaMemcpyAsync(io.in, h0_host, bytes, cudaMemcpyHostToDevice, st));
+    return GGNN_OK;
+}
 
 // The calls of the other model refuse a GGNN / GCN engine.
 static int wrong_model(ErrorText* t, const char* fn, int have, int want) {
@@ -435,20 +592,8 @@ void find_cuts(const int* reach, int V, std::vector<int>& cuts) {
 static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers,
                               float* d_h0, ggnn_stream_t stream) {
     using namespace ggnn::bwd;
-    if (!e->graph_set || !e->weights_set) return e->fail(GGNN_ESTATE, "no graph / weights set");
-    if (!e->saved_valid) return e->fail(GGNN_ESTATE, "ggnn_backward needs a preceding ggnn_forward with save_for_backward enabled");
-    if (!e->has_transpose) return e->fail(GGNN_ESTATE, "enable save_for_backward BEFORE ggnn_set_graph_sparse (the source-keyed CSR is built there)");
-    if (!grads || num_layers != e->L || (!d_h_out && e->V > 0)) return e->fail(GGNN_EINVAL, "bad backward arguments");
-    for (int l = 0; l < e->L; ++l) {   // the weight-gradient kernels use 16-byte vector atomics
-        const void* ps[8] = {grads[l].edge_weights, grads[l].edge_biases, grads[l].gate_kernel, grads[l].gate_bias, grads[l].cand_kernel, grads[l].cand_bias,
-                             grads[l].edge_type_attention_weights, grads[l].cand_hidden_bias};
-        for (const void* q : ps)
-            if (q && ((uintptr_t)q & 15)) return e->fail(GGNN_EINVAL, "layer %d: gradient pointers must be 16-byte aligned", l);
-    }
-    if (((uintptr_t)d_h_out & 15) || ((uintptr_t)d_h0 & 15)) return e->fail(GGNN_EINVAL, "d_h_out / d_h0 must be 16-byte aligned");
-    CU_TRY(e, cudaSetDevice(e->device));
+    if (int rc = begin_backward(e, "ggnn_backward", "ggnn_set_graph_sparse", d_h_out, grads, num_layers, d_h0)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    e->last_launches = 0;
     const int V = e->V, D = e->D, T = e->T, L = e->L;
     if (V == 0) return GGNN_OK;
     const size_t vd = (size_t)V * D;
@@ -473,20 +618,8 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
     CU_TRY(e, cudaMemcpyAsync(dstate + vd * L, d_h_out, vd * sizeof(float), cudaMemcpyDeviceToDevice, st));
     // forward values of node_states_per_layer
     std::vector<const float*> fstate(L + 1);
-    fstate[0] = e->last_h0; fstate[L] = e->last_out;
-    for (int l = 1; l < L; ++l) fstate[l] = (const float*)e->state_buf.ptr + (size_t)(l - 1) * vd;
-    const float* sv = (const float*)e->save_bufs.ptr;
-    const size_t per = vd * (size_t)std::max(e->total_steps, 1);
-    const float *sv_h = sv, *sv_x = sv + per, *sv_r = sv + 2 * per, *sv_u = sv + 3 * per, *sv_c = sv + 4 * per, *sv_q = sv + 5 * per;
-    char* g = (char*)e->graph_buf.ptr;
-    const int* row_ptr = (const int*)(g + e->off_row_ptr);
-    const int* csr_src = (const int*)(g + e->off_src);
-    const int* trow = (const int*)(g + e->off_trow);
-    const int* ttgt = (const int*)(g + e->off_ttgt);
-    const int* tslot = (const int*)(g + e->off_tslot);
-    const float* dadj = (const float*)(g + e->off_adj);
-    const float* indeg = (const float*)(g + e->off_indeg);
-    const float* denom = (const float*)(g + e->off_denom);
+    for (int l = 0; l <= L; ++l) fstate[l] = layer_state(e, l, e->last_h0, e->last_out);
+    const GraphDev& gd = e->gd;
     const long long n = (long long)vd;
     const int eb = (int)std::min<long long>((n + 255) / 256, 4096);
     auto gemm_nt = [&](bool acc, const float* A, int lda, int a_stride, const float* B, int ldb, int b_stride, int nseg, float* C, int ldc,
@@ -530,8 +663,8 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
         float* dhn = dstate + (size_t)(l + 1) * vd;   // gradient wrt the state leaving the current step
         float* dh_new = dha;
         for (int s = e->steps[l] - 1; s >= 0; --s) {
-            const size_t so = (size_t)(e->step_base[l] + s) * vd;
-            const float *h = sv_h + so, *x = sv_x + so;
+            const SaveDev sv = saved_step(e, e->step_base[l] + s);
+            const float *h = sv.h_in, *x = sv.agg;
             if (e->saved_drop_keep < 1.0f) {
                 dropout_grad_kernel<<<eb, 256, 0, st>>>(dhn, e->saved_drop_seed, e->step_base[l] + s, V, D, e->saved_drop_keep, n);
                 ++e->last_launches;
@@ -546,18 +679,18 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
                 return sl;
             };
             if (e->cell == CELL_GRU) {
-                const float *r = sv_r + so, *u = sv_u + so, *c = sv_c + so;
+                const float *r = sv.r, *u = sv.u, *c = sv.c;
                 gru_bwd1_kernel<<<eb, 256, 0, st>>>(dhn, h, r, u, c, dpc, dpg, dh_new, rh, n, D, e->act); ++e->last_launches;
                 gemm_nt(false, dpc, D, 0, w.cand_kernel, D, 0, 1, dxc, ldx, V, ldx, D);
                 gemm_tn(cell_segs(rh), R + 2, true, dpc, D, gw.cand_kernel, D, (size_t)D * D, gw.cand_bias, V, D, D);
                 gru_bwd2_kernel<<<eb, 256, 0, st>>>(dxc, ldx, (R + 1) * D, h, r, dpg, dh_new, n, D); ++e->last_launches;
                 gemm_nt(false, dpg, 2 * D, 0, w.gate_kernel, 2 * D, 0, 1, dxg, ldx, V, ldx, 2 * D);
                 gemm_tn(cell_segs(h), R + 2, true, dpg, 2 * D, gw.gate_kernel, 2 * D, (size_t)D * 2 * D, gw.gate_bias, V, 2 * D, D);
-                split_input_grad_kernel<<<eb, 256, 0, st>>>(dxc, dxg, ldx, R, d_ptrs, dxp, e->use_avg ? denom : nullptr, dh_new, 0, 1, 1, n, D);
+                split_input_grad_kernel<<<eb, 256, 0, st>>>(dxc, dxg, ldx, R, d_ptrs, dxp, e->use_avg ? gd.denom : nullptr, dh_new, 0, 1, 1, n, D);
                 ++e->last_launches;
             } else if (e->cell == CELL_CUDNN_GRU) {
                 // c = act(x.K_in + b_in + r*q), q = h.K_hid + b_hid: the candidate kernel's first din rows see [res.., x], its last D rows see h
-                const float *r = sv_r + so, *u = sv_u + so, *c = sv_c + so, *q = sv_q + so;
+                const float *r = sv.r, *u = sv.u, *c = sv.c, *q = sv.q;
                 float* dq = rh;   // the r*h scratch of the GRU branch is free here
                 cudnn_gru_bwd1_kernel<<<eb, 256, 0, st>>>(dhn, h, r, u, c, q, dpc, dq, dpg, dh_new, n, D, e->act); ++e->last_launches;
                 gemm_nt(false, dpc, D, 0, w.cand_kernel, D, 0, 1, dxc, ldx, V, din, D);                                  // d[res.., x] = dpc . K_in^T
@@ -572,14 +705,14 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
                 gemm_nt(false, dpg, 2 * D, 0, w.gate_kernel, 2 * D, 0, 1, dxg, ldx, V, ldx, 2 * D);
                 gemm_tn(cell_segs(h), R + 2, true, dpg, 2 * D, gw.gate_kernel, 2 * D, (size_t)D * 2 * D, gw.gate_bias, V, 2 * D, D);
                 // dxc holds only the din input columns: the recurrent gradient of the candidate went into dh_new through dq above
-                split_input_grad_kernel<<<eb, 256, 0, st>>>(dxc, dxg, ldx, R, d_ptrs, dxp, e->use_avg ? denom : nullptr, dh_new, 0, 1, 1, n, D);
+                split_input_grad_kernel<<<eb, 256, 0, st>>>(dxc, dxg, ldx, R, d_ptrs, dxp, e->use_avg ? gd.denom : nullptr, dh_new, 0, 1, 1, n, D);
                 ++e->last_launches;
             } else {
-                const float* hnew = (s == e->steps[l] - 1) ? fstate[l + 1] : sv_h + so + vd;
+                const float* hnew = (s == e->steps[l] - 1) ? fstate[l + 1] : saved_step(e, e->step_base[l] + s + 1).h_in;
                 rnn_bwd1_kernel<<<eb, 256, 0, st>>>(dhn, hnew, dpc, n, e->act, e->saved_drop_keep < 1.0f ? e->saved_drop_keep : 1.0f); ++e->last_launches;
                 gemm_nt(false, dpc, D, 0, w.cand_kernel, D, 0, 1, dxc, ldx, V, ldx, D);
                 gemm_tn(cell_segs(h), R + 2, true, dpc, D, gw.cand_kernel, D, (size_t)D * D, gw.cand_bias, V, D, D);
-                split_input_grad_kernel<<<eb, 256, 0, st>>>(dxc, nullptr, ldx, R, d_ptrs, dxp, e->use_avg ? denom : nullptr, dh_new, 1, 0, 0, n, D);
+                split_input_grad_kernel<<<eb, 256, 0, st>>>(dxc, nullptr, ldx, R, d_ptrs, dxp, e->use_avg ? gd.denom : nullptr, dh_new, 1, 0, 0, n, D);
                 ++e->last_launches;
             }
             // ---- messages: all edge types at once.  At[v, t*D..] = sum of h over the type-t sources of v, Gt[s, t*D..] = sum of dx' over
@@ -589,25 +722,25 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
                 if (e->use_att) {   // softmax backward first (it adds to dh_new), then the gathers are weighted by the probabilities
                     alpha = (const float*)e->att_buf.ptr + (size_t)(e->step_base[l] + s) * (size_t)std::max<int64_t>(e->M, 1);
                     gemm_nt(false, dxp, D, 0, w.edge_weights, D, 0, 1, Pall, TD, V, TD, D);   // P[v, t*D+k] = <dx'[v], W_t[k, :]>
-                    attention_bwd_target_kernel<<<nodes_blocks, 256, 0, st>>>(row_ptr, csr_src, h, Pall, alpha, w.edge_type_attention_weights, dsa,
-                                                                              dh_new, gw.edge_type_attention_weights, V, D, T);
-                    attention_bwd_source_kernel<<<nodes_blocks, 256, 0, st>>>(trow, ttgt, tslot, h, dsa, dh_new, V, D, T);
+                    attention_bwd_target_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, Pall, alpha, w.edge_type_attention_weights,
+                                                                              dsa, dh_new, gw.edge_type_attention_weights, V, D, T);
+                    attention_bwd_source_kernel<<<nodes_blocks, 256, 0, st>>>(gd.trow, gd.ttgt, gd.tslot, h, dsa, dh_new, V, D, T);
                     e->last_launches += 2;
                 }
-                GatherJob j0{row_ptr, csr_src, h, At, alpha, nullptr}, j1{trow, ttgt, dxp, Gt, alpha, alpha ? tslot : nullptr};
+                GatherJob j0{gd.row_ptr, gd.csr_src, h, At, alpha, nullptr}, j1{gd.trow, gd.ttgt, dxp, Gt, alpha, alpha ? gd.tslot : nullptr};
                 csr_gather_all_kernel<<<dim3(nodes_blocks, 2), 256, 0, st>>>(j0, j1, V, D, T);
                 ++e->last_launches;
             } else {
                 for (int t = 0; t < T; ++t) {
-                    dense_gather_sum_kernel<<<nodes_blocks, 256, 0, st>>>(dadj, h, At + (size_t)t * D, TD, V, D, T, t, e->dense_v, 0);
-                    dense_gather_sum_kernel<<<nodes_blocks, 256, 0, st>>>(dadj, dxp, Gt + (size_t)t * D, TD, V, D, T, t, e->dense_v, 1);
+                    dense_gather_sum_kernel<<<nodes_blocks, 256, 0, st>>>(gd.dense_adj, h, At + (size_t)t * D, TD, V, D, T, t, e->dense_v, 0);
+                    dense_gather_sum_kernel<<<nodes_blocks, 256, 0, st>>>(gd.dense_adj, dxp, Gt + (size_t)t * D, TD, V, D, T, t, e->dense_v, 1);
                     e->last_launches += 2;
                 }
             }
             if (e->use_bias && gw.edge_biases) {   // dB[t,:] += sum_v indeg[v,t] dx'[v,:]  =  indeg^T . dx'
                 SegList sl;
                 memset(&sl, 0, sizeof sl);
-                sl.p[0] = indeg; sl.ld[0] = T;
+                sl.p[0] = gd.indeg; sl.ld[0] = T;
                 gemm_tn(sl, 1, false, dxp, D, gw.edge_biases, D, 0, nullptr, V, D, T);
             }
             if (gw.edge_weights) {
@@ -734,7 +867,7 @@ int ggnn_destroy(ggnn_engine* e) {
     if (!e) return GGNN_OK;
     cudaSetDevice(e->device);
     e->graph_buf.release(); e->state_buf.release(); e->save_bufs.release(); e->io_buf.release(); e->bwd_buf.release();
-    e->tc_weights.release(); e->tc_respre.release(); e->ts_weights.release(); e->ts_images.release(); e->ts_u.release(); e->ts_virt.release(); e->err_flag.release();
+    e->tc_tiles.buf.release(); e->tc_respre.release(); e->ts_tiles.buf.release(); e->ts_images.release(); e->ts_virt.release(); e->err_flag.release();
     if (e->own_prep) { ggnn_free_prepared_graph(e->own_prep); e->own_prep = nullptr; }
     e->ro_buf.release(); e->ro_stage.release(); e->att_buf.release();
     delete e;
@@ -758,7 +891,7 @@ int ggnn_set_weights(ggnn_engine* e, const ggnn_layer_weights* layers, int32_t n
         e->w[l] = w;
     }
     e->weights_set = true;
-    e->weights_dirty = true;   // the tensor-core path re-tiles its bf16 copies at the next forward
+    ++e->weights_gen;   // the tensor-core paths re-tile their bf16 copies at their next forward
     return GGNN_OK;
 }
 
@@ -1372,6 +1505,16 @@ int ggnn_set_graph_prepared(ggnn_engine* e, ggnn_prepared_graph* g, ggnn_stream_
     static_cast<BatchPlan&>(*e) = g->plan;
     CU_TRY(e, e->graph_buf.reserve(g->bytes));
     CU_TRY(e, g->image.upload(e->graph_buf.ptr, g->bytes, (cudaStream_t)stream));
+    const char* b = (const char*)e->graph_buf.ptr;
+    GraphDev& d = e->gd;
+    d.row_ptr = (const int*)(b + e->off_row_ptr); d.csr_src = (const int*)(b + e->off_src); d.csr_msg = (const int*)(b + e->off_msg);
+    d.indeg = (const float*)(b + e->off_indeg); d.denom = (const float*)(b + e->off_denom);
+    d.tile_start = (const int*)(b + e->off_tiles); d.tile_mask = (const unsigned*)(b + e->off_mask);
+    d.dense_adj = (const float*)(b + e->off_adj);
+    d.trow = (const int*)(b + e->off_trow); d.ttgt = (const int*)(b + e->off_ttgt); d.tslot = (const int*)(b + e->off_tslot);
+    d.pair_src = (const int*)(b + e->off_pair); d.vrow_ptr = (const int*)(b + e->off_vptr); d.vsrc = (const int*)(b + e->off_vsrc);
+    d.tile_vptr = (const int*)(b + e->off_tvp); d.vinfo = (const int4*)(b + e->off_vinfo);
+    d.slot_w = (const float*)(b + e->off_slotw); d.tslot_w = (const float*)(b + e->off_tslotw);
     int rc = reserve_states(e);
     if (rc) return rc;
     e->graph_set = true;
@@ -1576,28 +1719,16 @@ int ggnn_set_graph_dense(ggnn_engine* e, int32_t b, int32_t v, const float* adjm
     });
 }
 
-static void fill_params(ggnn_engine* e, FwdParams& p, const float* h0, float* h_out) {
-    memset(&p, 0, sizeof p);
-    p.V = e->V; p.D = e->D; p.T = e->T; p.L = e->L;
-    p.use_bias = e->use_bias; p.use_avg = e->use_avg; p.cell = e->cell; p.act = e->act;
-    p.gather_mode = e->gather_mode; p.dense_v = e->dense_v; p.save = e->save ? 1 : 0;
-    p.drop_keep = e->drop_keep; p.drop_seed = e->drop_seed;
-    p.use_att = e->use_att; p.att = (float*)e->att_buf.ptr; p.att_stride = e->save ? (size_t)std::max<int64_t>(e->M, 1) : 0;
-    char* g = (char*)e->graph_buf.ptr;
-    p.tile_start = (const int*)(g + e->off_tiles);
-    p.tile_mask = (const unsigned*)(g + e->off_mask);
-    p.row_ptr = (const int*)(g + e->off_row_ptr);
-    p.csr_src = (const int*)(g + e->off_src);
-    p.dense_adj = (const float*)(g + e->off_adj);
-    p.indeg = (const float*)(g + e->off_indeg);
-    p.denom = (const float*)(g + e->off_denom);
-    const size_t vd = (size_t)std::max(e->V, 1) * e->D;
-    float* sb = (float*)e->state_buf.ptr;
-    p.state[0] = h0; p.state_w[0] = nullptr;
-    for (int l = 1; l <= e->L; ++l) {
-        float* ptr = (l == e->L) ? h_out : sb + (size_t)(l - 1) * vd;
-        p.state[l] = ptr; p.state_w[l] = ptr;
+// ------------------------------------------------------------------------------------------ forward drivers (host)
+// fp32 CUDA-core path (ggnn_fwd_ffma.cuh); the only one with propagation attention and CudnnCompatibleGRUCell.
+static int forward_ffma(ggnn_engine* e, const float* h0, float* h_out, cudaStream_t st) {
+    if (e->use_att) {
+        if (e->gather_mode != GATHER_SPARSE) return e->fail(GGNN_EUNSUPPORTED, "propagation attention needs the sparse graph format");
+        CU_TRY(e, e->att_buf.reserve(sizeof(float) * (size_t)std::max<int64_t>(e->M, 1) * (size_t)(e->save ? std::max(e->total_steps, 1) : 1)));
     }
+    FwdParams p;
+    fill_common_params(e, p, h0, h_out);
+    p.use_att = e->use_att; p.att = (float*)e->att_buf.ptr; p.att_stride = e->save ? (size_t)std::max<int64_t>(e->M, 1) : 0;
     for (int l = 0; l < e->L; ++l) {
         LayerDev& ld = p.layer[l];
         ld.edge_w = e->w[l].edge_weights; ld.edge_b = e->w[l].edge_biases;
@@ -1605,47 +1736,47 @@ static void fill_params(ggnn_engine* e, FwdParams& p, const float* h0, float* h_
         ld.cand_k = e->w[l].cand_kernel; ld.cand_b = e->w[l].cand_bias;
         ld.att_w = e->use_att ? e->w[l].edge_type_attention_weights : nullptr;
         ld.cand_hb = e->cell == CELL_CUDNN_GRU ? e->w[l].cand_hidden_bias : nullptr;
-        ld.steps = e->steps[l]; ld.nres = e->nres[l];
-        for (int i = 0; i < MAX_RES; ++i) ld.res[i] = e->res[l][i];
-        p.step_base[l] = e->step_base[l];
     }
-    if (e->save) {
-        float* s = (float*)e->save_bufs.ptr;
-        const size_t per = vd * (size_t)std::max(e->total_steps, 1);
-        p.save_buf.h_in = s; p.save_buf.agg = s + per; p.save_buf.r = s + 2 * per; p.save_buf.u = s + 3 * per; p.save_buf.c = s + 4 * per;
-        p.save_buf.q = e->cell == CELL_CUDNN_GRU ? s + 5 * per : nullptr;
-    }
+    FwdKernel k = pick_fwd_kernel(e->variant, e->nb1, e->local);
+    if (!k) return e->fail(GGNN_EUNSUPPORTED, "no kernel for variant=%d nb1=%d", e->variant, e->nb1);
+    const size_t smem = fwd_smem_bytes(e->variant, e->nb1, e->D, e->T);
+    CU_TRY(e, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    return launch_steps(e, p, st, [&](const FwdParams& q) { k<<<e->ntiles, 256, smem, st>>>(q); });
 }
 
-
-// ------------------------------------------------------------------------------------------ tensor-core path (host)
+// The tile-local wgmma layout (ggnn_fwd_tc.cuh): per layer the T edge blocks, then the gate and the candidate kernel in nres + 2 input
+// segments.  A GCN layer is one edge block.
 static int tc_prepare_weights(ggnn_engine* e, cudaStream_t st) {
+    const bool gcn = e->model == MODEL_GCN;
     const int D = e->D, DP = e->DP, T = e->T, NKS = DP / 16;
+    WeightTiles& c = e->tc_tiles;
     size_t off = 0;
     for (int l = 0; l < e->L; ++l) {
         const int nseg = e->nres[l] + 2;
-        e->tc_off_edge[l] = off; off += (size_t)T * NKS * 64 * DP;
-        e->tc_off_gate[l] = off; off += (size_t)nseg * NKS * 128 * DP;
-        e->tc_off_cand[l] = off; off += (size_t)nseg * NKS * 64 * DP;
+        c.off_edge[l] = off; off += (size_t)T * NKS * 64 * DP;
+        if (gcn) continue;
+        c.off_gate[l] = off; off += (size_t)nseg * NKS * 128 * DP;
+        c.off_cand[l] = off; off += (size_t)nseg * NKS * 64 * DP;
     }
-    if (off > e->tc_weights.cap) e->weights_dirty = true;
-    CU_TRY(e, e->tc_weights.reserve(off));
-    if (!e->weights_dirty) return GGNN_OK;
-    uint8_t* base = (uint8_t*)e->tc_weights.ptr;
+    bool retile = false;
+    CU_TRY(e, c.reserve(off, 0, 0, e->weights_gen, retile));
+    if (!retile) return GGNN_OK;
+    uint8_t* base = (uint8_t*)c.buf.ptr;
+    auto launch = [&](const float* W, size_t out, int segs, int blks, int src_ld) {
+        const long long total = (long long)segs * NKS * 2 * blks * DP;
+        const int blocks = (int)std::min<long long>((total + 255) / 256, 1024);
+        tc::ggnn_tile_weights_kernel<<<blocks, 256, 0, st>>>(W, base + out, D, DP, segs, blks, src_ld, 0);
+        ++e->last_launches;
+    };
     for (int l = 0; l < e->L; ++l) {
         const int nseg = e->nres[l] + 2;
-        auto launch = [&](const float* W, uint8_t* out, int segs, int blks, int src_ld, int col0) {
-            const long long total = (long long)segs * NKS * 2 * blks * DP;
-            const int blocks = (int)std::min<long long>((total + 255) / 256, 1024);
-            tc::ggnn_tile_weights_kernel<<<blocks, 256, 0, st>>>(W, out, D, DP, segs, blks, src_ld, col0);
-            ++e->last_launches;
-        };
-        launch(e->w[l].edge_weights, base + e->tc_off_edge[l], T, 1, D, 0);
-        if (e->cell == CELL_GRU) launch(e->w[l].gate_kernel, base + e->tc_off_gate[l], nseg, 2, 2 * D, 0);
-        launch(e->w[l].cand_kernel, base + e->tc_off_cand[l], nseg, 1, D, 0);
+        if (gcn) { launch(e->gcn_w[l].kernel, c.off_edge[l], 1, 1, D); continue; }
+        launch(e->w[l].edge_weights, c.off_edge[l], T, 1, D);
+        if (e->cell == CELL_GRU) launch(e->w[l].gate_kernel, c.off_gate[l], nseg, 2, 2 * D);
+        launch(e->w[l].cand_kernel, c.off_cand[l], nseg, 1, D);
     }
     CU_TRY(e, cudaGetLastError());
-    e->weights_dirty = false;
+    c.gen = e->weights_gen;
     return GGNN_OK;
 }
 
@@ -1657,16 +1788,12 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
     for (int l = 0; l < e->L; ++l) any_res |= e->nres[l] > 0;
     if (any_res) CU_TRY(e, e->tc_respre.reserve((size_t)e->ntiles * tc::TILE_M * 3 * DP * sizeof(float)));
     tc::TcParams p;
-    memset(&p, 0, sizeof p);
-    p.V = e->V; p.D = e->D; p.DP = DP; p.T = e->T; p.L = e->L;
-    p.use_bias = e->use_bias; p.use_avg = e->use_avg; p.cell = e->cell; p.act = e->act;
-    p.gather_mode = e->gather_mode; p.dense_v = e->dense_v; p.save = e->save ? 1 : 0;
+    fill_common_params(e, p, h0, h_out);
+    p.DP = DP;
     p.nparts = e->precision == GGNN_PREC_BF16X3 ? 3 : 1;
-    p.drop_keep = e->drop_keep; p.drop_seed = e->drop_seed;
     p.kgs = e->tc_kgs;
     const size_t opb = (size_t)DP * (size_t)p.kgs / 4, stage = (size_t)DP * 128;   // a ring slot = two 64*DP-byte K-step stages
     // tile-local sparse graphs: stage the tile's CSR slice in shared memory when it is small enough
-    p.csr_cache = 0; p.csr_cap_msgs = 0;
     size_t csr_b = 0;
     if (e->local && e->gather_mode == GATHER_SPARSE && e->T <= 16 && e->max_tile_msgs <= 4096) {
         p.csr_cache = 1;
@@ -1680,38 +1807,15 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
     p.nstages = (int)std::min<size_t>(tc::MAX_STAGES, (avail - ops - bias_b) / stage);
     if (p.nstages < 1) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the weight ring (DP=%d)", DP);
     const size_t smem = ops + bias_b + (size_t)p.nstages * stage;
-    char* g = (char*)e->graph_buf.ptr;
-    p.tile_start = (const int*)(g + e->off_tiles);
-    p.tile_mask = (const unsigned*)(g + e->off_mask);
-    p.row_ptr = (const int*)(g + e->off_row_ptr);
-    p.csr_src = (const int*)(g + e->off_src);
-    p.dense_adj = (const float*)(g + e->off_adj);
-    p.indeg = (const float*)(g + e->off_indeg);
-    p.denom = (const float*)(g + e->off_denom);
-    const size_t vd = (size_t)std::max(e->V, 1) * e->D;
-    float* sb = (float*)e->state_buf.ptr;
-    p.state[0] = h0;
-    for (int l = 1; l <= e->L; ++l) {
-        float* ptr = (l == e->L) ? h_out : sb + (size_t)(l - 1) * vd;
-        p.state[l] = ptr; p.state_w[l] = ptr;
-    }
-    uint8_t* wb = (uint8_t*)e->tc_weights.ptr;
+    const WeightTiles& wt = e->tc_tiles;
+    const uint8_t* wb = (const uint8_t*)wt.buf.ptr;
     for (int l = 0; l < e->L; ++l) {
         tc::TcLayer& ld = p.layer[l];
-        ld.w_edge = wb + e->tc_off_edge[l]; ld.w_gate = wb + e->tc_off_gate[l]; ld.w_cand = wb + e->tc_off_cand[l];
+        ld.w_edge = wb + wt.off_edge[l]; ld.w_gate = wb + wt.off_gate[l]; ld.w_cand = wb + wt.off_cand[l];
         ld.edge_b = e->w[l].edge_biases; ld.gate_b = e->w[l].gate_bias; ld.cand_b = e->w[l].cand_bias;
-        ld.steps = e->steps[l]; ld.nres = e->nres[l];
-        for (int i = 0; i < MAX_RES; ++i) ld.res[i] = e->res[l][i];
-        p.step_base[l] = e->step_base[l];
-    }
-    if (e->save) {
-        float* s = (float*)e->save_bufs.ptr;
-        const size_t per = vd * (size_t)std::max(e->total_steps, 1);
-        p.save_buf.h_in = s; p.save_buf.agg = s + per; p.save_buf.r = s + 2 * per; p.save_buf.u = s + 3 * per; p.save_buf.c = s + 4 * per;
     }
     p.res_pre = (float*)e->tc_respre.ptr;
     p.error_flag = (int*)e->err_flag.ptr;
-    const size_t vd_bytes = (size_t)e->V * e->D * sizeof(float);
     // the wgmma N of a warpgroup's columns is an instruction immediate: one kernel per padded hidden size and layout (compact tiles
     // split the columns four ways, 128-row tiles two ways)
     void (*kern)(tc::TcParams) = nullptr;
@@ -1727,47 +1831,26 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
         default: return e->fail(GGNN_EUNSUPPORTED, "no tile-local tensor-core kernel for DP=%d", DP);
     }
     CU_TRY(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (e->local) {
-        kern<<<e->ntiles, tc::NTHREADS, smem, st>>>(p);
-        ++e->last_launches;
-    } else {
-        float* tmp0 = sb + (size_t)(e->L - 1 > 0 ? e->L - 1 : 0) * vd;
-        float* tmp1 = tmp0 + vd;
-        for (int l = 0; l < e->L; ++l) {
-            const float* in = p.state[l];
-            if (e->steps[l] == 0) {
-                CU_TRY(e, cudaMemcpyAsync(p.state_w[l + 1], in, vd_bytes, cudaMemcpyDeviceToDevice, st));
-                continue;
-            }
-            for (int s = 0; s < e->steps[l]; ++s) {
-                float* out = (s == e->steps[l] - 1) ? p.state_w[l + 1] : ((s & 1) ? tmp1 : tmp0);
-                p.g_layer = l; p.g_step = s; p.g_in = in; p.g_out = out;
-                kern<<<e->ntiles, tc::NTHREADS, smem, st>>>(p);
-                ++e->last_launches;
-                in = out;
-            }
-        }
-    }
-    CU_TRY(e, cudaGetLastError());
-    if (e->save) { e->saved_valid = true; e->saved_drop_keep = e->drop_keep; e->saved_drop_seed = e->drop_seed; }
-    return GGNN_OK;
+    return launch_steps(e, p, st, [&](const tc::TcParams& q) { kern<<<e->ntiles, tc::NTHREADS, smem, st>>>(q); });
 }
 
 // ------------------------------------------------------------------------------------------ streaming tensor-core path (host)
+// The streaming layout (ggnn_fwd_stream.cuh): per layer, in N blocks of ts_nc columns, the T edge blocks, the gate and the candidate kernel.
 static int ts_prepare_weights(ggnn_engine* e, cudaStream_t st) {
     const int D = e->D, DP = e->DP, T = e->T, NKS = DP / 16;
     const int nc0 = e->ts_nc[0], nb0 = e->ts_nblk[0], nc1 = e->ts_nc[1], nb1 = e->ts_nblk[1];
+    WeightTiles& c = e->ts_tiles;
     size_t off = 0;
     for (int l = 0; l < e->L; ++l) {
         const int nseg = e->nres[l] + 2;
-        e->ts_off_edge[l] = off; off += (size_t)nb0 * T * NKS * 64 * nc0;
-        e->ts_off_gate[l] = off; off += (size_t)nb1 * nseg * NKS * 64 * nc1;
-        e->ts_off_cand[l] = off; off += (size_t)nb0 * nseg * NKS * 64 * nc0;
+        c.off_edge[l] = off; off += (size_t)nb0 * T * NKS * 64 * nc0;
+        c.off_gate[l] = off; off += (size_t)nb1 * nseg * NKS * 64 * nc1;
+        c.off_cand[l] = off; off += (size_t)nb0 * nseg * NKS * 64 * nc0;
     }
-    if (off > e->ts_weights.cap || e->ts_tiled_nc[0] != nc0 || e->ts_tiled_nc[1] != nc1) e->weights_dirty = true;
-    CU_TRY(e, e->ts_weights.reserve(off));
-    if (!e->weights_dirty) return GGNN_OK;
-    uint8_t* base = (uint8_t*)e->ts_weights.ptr;
+    bool retile = false;
+    CU_TRY(e, c.reserve(off, nc0, nc1, e->weights_gen, retile));
+    if (!retile) return GGNN_OK;
+    uint8_t* base = (uint8_t*)c.buf.ptr;
     for (int l = 0; l < e->L; ++l) {
         const int nseg = e->nres[l] + 2;
         auto launch = [&](const float* W, uint8_t* out, int segs, int ncolblk, int src_ld, int NC, int nblk) {
@@ -1776,13 +1859,12 @@ static int ts_prepare_weights(ggnn_engine* e, cudaStream_t st) {
             ts::ggnn_tile_weights_stream_kernel<<<blocks, 256, 0, st>>>(W, out, D, DP, segs, ncolblk, src_ld, NC, nblk);
             ++e->last_launches;
         };
-        launch(e->w[l].edge_weights, base + e->ts_off_edge[l], T, 1, D, nc0, nb0);
-        if (e->cell == CELL_GRU) launch(e->w[l].gate_kernel, base + e->ts_off_gate[l], nseg, 2, 2 * D, nc1, nb1);
-        launch(e->w[l].cand_kernel, base + e->ts_off_cand[l], nseg, 1, D, nc0, nb0);
+        launch(e->w[l].edge_weights, base + c.off_edge[l], T, 1, D, nc0, nb0);
+        if (e->cell == CELL_GRU) launch(e->w[l].gate_kernel, base + c.off_gate[l], nseg, 2, 2 * D, nc1, nb1);
+        launch(e->w[l].cand_kernel, base + c.off_cand[l], nseg, 1, D, nc0, nb0);
     }
     CU_TRY(e, cudaGetLastError());
-    e->weights_dirty = false;
-    e->ts_tiled_nc[0] = nc0; e->ts_tiled_nc[1] = nc1;
+    c.gen = e->weights_gen;
     return GGNN_OK;
 }
 
@@ -1804,16 +1886,9 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     auto chk_state = [&](int l) { return (float*)(cb + (size_t)l * img_b); };
     float* chk_tmp[2] = {(float*)(cb + (size_t)(L + 1) * img_b), (float*)(cb + (size_t)(L + 2) * img_b)};
     float* u_chk = (float*)(cb + (size_t)(L + 3) * img_b);
-    const size_t vd = (size_t)std::max(V, 1) * D;
     const size_t vd_bytes = (size_t)V * D * sizeof(float);
-    float* sb = (float*)e->state_buf.ptr;
-    std::vector<float*> state(L + 1);
-    state[0] = const_cast<float*>(h0);
-    for (int l = 1; l <= L; ++l) state[l] = (l == L) ? h_out : sb + (size_t)(l - 1) * vd;
     const bool gru = e->cell == CELL_GRU;
-    float* sv = (float*)e->save_bufs.ptr;
-    const size_t per = vd * (size_t)std::max(e->total_steps, 1);
-    char* g = (char*)e->graph_buf.ptr;
+    const GraphDev& gd = e->gd;
 
     // shared-memory budgets
     const size_t avail = (e->max_smem > 2048 ? e->max_smem - 2048 : 0);
@@ -1834,12 +1909,10 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     base.V = V; base.D = D; base.DP = DP; base.T = T;
     base.nparts = e->precision == GGNN_PREC_BF16X3 ? 3 : 1;
     base.cell = e->cell; base.act = e->act; base.use_bias = e->use_bias; base.use_avg = e->use_avg;
-    base.tile_mask = (const unsigned*)(g + e->off_mask);
-    base.pair_src = (const int*)(g + e->off_pair); base.vrow_ptr = (const int*)(g + e->off_vptr);
-    base.vsrc = (const int*)(g + e->off_vsrc); base.tile_vptr = (const int*)(g + e->off_tvp);
-    base.vinfo = (const int4*)(g + e->off_vinfo);
+    base.tile_mask = gd.tile_mask;
+    base.pair_src = gd.pair_src; base.vrow_ptr = gd.vrow_ptr; base.vsrc = gd.vsrc; base.tile_vptr = gd.tile_vptr; base.vinfo = gd.vinfo;
     base.virt_img = (uint8_t*)e->ts_virt.ptr;   // pairs with several messages, pre-summed by the prologue of every gather launch
-    base.indeg = (const float*)(g + e->off_indeg); base.denom = (const float*)(g + e->off_denom);
+    base.indeg = gd.indeg; base.denom = gd.denom;
     base.drop_keep = e->drop_keep; base.drop_seed = e->drop_seed;
     base.error_flag = (int*)e->err_flag.ptr;
     const int nc0 = e->ts_nc[0], nb0 = e->ts_nblk[0], nc1 = e->ts_nc[1], nb1 = e->ts_nblk[1];
@@ -1872,12 +1945,13 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
         ts::ggnn_image_kernel<<<(int)std::min<long long>((total + 255) / 256, 4096), 256, 0, st>>>(h0, img_state(0), chk_state(0), V, D, DP, ntiles);
         ++e->last_launches;
     }
-    const uint8_t* wb = (const uint8_t*)e->ts_weights.ptr;
+    const WeightTiles& wt = e->ts_tiles;
+    const uint8_t* wb = (const uint8_t*)wt.buf.ptr;
     for (int l = 0; l < L; ++l) {
         const uint8_t* img_in = img_state(l);
         const float* chk_in = chk_state(l);
         if (e->steps[l] == 0) {   // a layer without timesteps aliases the previous state (sparse:152)
-            CU_TRY(e, cudaMemcpyAsync(state[l + 1], state[l], vd_bytes, cudaMemcpyDeviceToDevice, st));
+            CU_TRY(e, cudaMemcpyAsync(layer_state(e, l + 1, h0, h_out), layer_state(e, l, h0, h_out), vd_bytes, cudaMemcpyDeviceToDevice, st));
             CU_TRY(e, cudaMemcpyAsync(img_state(l + 1), img_in, img_b, cudaMemcpyDeviceToDevice, st));
             CU_TRY(e, cudaMemcpyAsync(chk_state(l + 1), chk_in, img_b, cudaMemcpyDeviceToDevice, st));
             continue;
@@ -1885,17 +1959,17 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
         const int R = e->nres[l], nseg = R + 2;
         for (int s = 0; s < e->steps[l]; ++s) {
             const bool last = s == e->steps[l] - 1;
-            float* out = last ? state[l + 1] : nullptr;   // the row-major copy exists only for node_states_per_layer entries
+            float* out = last ? layer_state(e, l + 1, h0, h_out) : nullptr;   // the row-major copy exists only for node_states_per_layer entries
             uint8_t* img_out = last ? img_state(l + 1) : img_tmp[s & 1];
             float* chk_out = last ? chk_state(l + 1) : chk_tmp[s & 1];
             const int gs = e->step_base[l] + s;
-            const size_t so = (size_t)gs * vd;
+            const SaveDev sv = saved_step(e, gs);
             // ---- aggregated messages
             ts::StreamParams p = base;
             p.epi = ts::EPI_AGG; p.NC = nc0; p.nstages = ns_edge;
-            p.g_img = img_in; p.w = wb + e->ts_off_edge[l]; p.kt_all = T * NKS;
+            p.g_img = img_in; p.w = wb + wt.off_edge[l]; p.kt_all = T * NKS;
             p.bias = e->use_bias ? e->w[l].edge_biases : nullptr;
-            p.img_out = img_agg; p.sv_agg = e->save ? sv + per + so : nullptr; p.gstep = gs;
+            p.img_out = img_agg; p.sv_agg = sv.agg; p.gstep = gs;
             k_edge<<<dim3(ntiles, nb0), ts::NTHREADS, sm_edge, st>>>(p);
             ++e->last_launches;
             auto set_segs = [&](ts::StreamParams& q, const uint8_t* last_img) {
@@ -1908,8 +1982,8 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
                 ts::StreamParams q = base;
                 q.epi = ts::EPI_GATE; q.NC = nc1; q.nstages = ns_gate;
                 set_segs(q, img_in);
-                q.w = wb + e->ts_off_gate[l]; q.bias = e->w[l].gate_bias; q.h_chk = chk_in; q.u_buf = u_chk; q.img_out = img_rh;
-                if (e->save) { q.sv_r = sv + 2 * per + so; q.sv_h = sv + so; q.sv_u = sv + 3 * per + so; }
+                q.w = wb + wt.off_gate[l]; q.bias = e->w[l].gate_bias; q.h_chk = chk_in; q.u_buf = u_chk; q.img_out = img_rh;
+                q.sv_r = sv.r; q.sv_h = sv.h_in; q.sv_u = sv.u;
                 q.gstep = gs;
                 k_fed<<<dim3(ntiles, nb1), ts::NTHREADS, smem_of(nc1, ns_gate, false), st>>>(q);
                 ++e->last_launches;
@@ -1917,16 +1991,14 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
             ts::StreamParams c = base;
             c.epi = ts::EPI_CAND; c.NC = nc0; c.nstages = ns_cand;
             set_segs(c, gru ? img_rh : img_in);
-            c.w = wb + e->ts_off_cand[l]; c.bias = e->w[l].cand_bias; c.h_chk = chk_in; c.u_buf = u_chk; c.h_chk_out = chk_out; c.h_out = out; c.img_out = img_out;
-            if (e->save) { if (gru) c.sv_c = sv + 4 * per + so; else c.sv_h = sv + so; }
+            c.w = wb + wt.off_cand[l]; c.bias = e->w[l].cand_bias; c.h_chk = chk_in; c.u_buf = u_chk; c.h_chk_out = chk_out; c.h_out = out; c.img_out = img_out;
+            if (gru) c.sv_c = sv.c; else c.sv_h = sv.h_in;
             c.gstep = gs;
             k_fed<<<dim3(ntiles, nb0), ts::NTHREADS, smem_of(nc0, ns_cand, false), st>>>(c);
             ++e->last_launches;
             img_in = img_out; chk_in = chk_out;
         }
     }
-    CU_TRY(e, cudaGetLastError());
-    if (e->save) { e->saved_valid = true; e->saved_drop_keep = e->drop_keep; e->saved_drop_seed = e->drop_seed; }
     return GGNN_OK;
 }
 
@@ -1984,7 +2056,7 @@ int ggnn_gcn_set_weights(ggnn_engine* e, const ggnn_gcn_layer_weights* layers, i
     }
     for (int l = 0; l < e->L; ++l) { e->gcn_w[l] = layers[l]; if (!e->use_bias) e->gcn_w[l].bias = nullptr; }
     e->weights_set = true;
-    e->weights_dirty = true;
+    ++e->weights_gen;
     return GGNN_OK;
 }
 
@@ -2023,37 +2095,16 @@ static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream
     p.V = V; p.D = D; p.DP = DP; p.L = L;
     p.nparts = e->precision == GGNN_PREC_BF16X3 ? 3 : 1;
     p.save = e->save ? 1 : 0;
-    char* g = (char*)e->graph_buf.ptr;
-    p.tile_start = (const int*)(g + e->off_tiles);
-    p.row_ptr = (const int*)(g + e->off_row_ptr);
-    p.csr_src = (const int*)(g + e->off_src);
-    p.slot_w = (const float*)(g + e->off_slotw);
-    const size_t vd = (size_t)std::max(V, 1) * D;
-    float* sb = (float*)e->state_buf.ptr;
-    p.state[0] = h0;
-    for (int l = 1; l <= L; ++l) {
-        float* ptr = (l == L) ? h_out : sb + (size_t)(l - 1) * vd;
-        p.state[l] = ptr; p.state_w[l] = ptr;
-    }
+    p.tile_start = e->gd.tile_start; p.row_ptr = e->gd.row_ptr; p.csr_src = e->gd.csr_src; p.slot_w = e->gd.slot_w;
+    set_layer_states(e, p, h0, h_out);
     for (int l = 0; l < L; ++l) { p.kernel[l] = e->gcn_w[l].kernel; p.bias[l] = e->gcn_w[l].bias; }
     p.drop_keep = e->drop_keep; p.drop_seed = e->drop_seed;
     p.error_flag = (int*)e->err_flag.ptr;
     if (tcore) {
-        const int NKS = DP / 16;
-        const size_t per_layer = (size_t)NKS * 64 * DP;   // one DP x DP block, pre-split and pre-tiled
-        if ((size_t)L * per_layer > e->tc_weights.cap) e->weights_dirty = true;
-        CU_TRY(e, e->tc_weights.reserve((size_t)L * per_layer));
-        uint8_t* wb = (uint8_t*)e->tc_weights.ptr;
-        if (e->weights_dirty) {
-            const long long total = (long long)NKS * 2 * DP;
-            for (int l = 0; l < L; ++l) {
-                tc::ggnn_tile_weights_kernel<<<(int)std::min<long long>((total + 255) / 256, 1024), 256, 0, st>>>(e->gcn_w[l].kernel, wb + l * per_layer, D,
-                                                                                                                 DP, 1, 1, D, 0);
-                ++e->last_launches;
-            }
-            e->weights_dirty = false;
-        }
-        for (int l = 0; l < L; ++l) p.w_tiled[l] = wb + l * per_layer;
+        int rc = tc_prepare_weights(e, st);
+        if (rc) return rc;
+        const WeightTiles& wt = e->tc_tiles;
+        for (int l = 0; l < L; ++l) p.w_tiled[l] = (const uint8_t*)wt.buf.ptr + wt.off_edge[l];
         const size_t opb = (size_t)DP * gcn::KGS / 4, slot_b = (size_t)DP * 128, sh_b = e->local ? (size_t)tc::TILE_M * DP * sizeof(float) : 0;
         const size_t avail = e->max_smem > 1024 ? e->max_smem - 1024 : 0;
         p.nstages = (int)std::min<size_t>(gcn::MAX_STAGES, avail > opb + sh_b ? (avail - opb - sh_b) / slot_b : 0);
@@ -2081,8 +2132,6 @@ static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream
             ++e->last_launches;
         }
     }
-    CU_TRY(e, cudaGetLastError());
-    if (e->save) { e->saved_valid = true; e->saved_drop_keep = e->drop_keep; e->saved_drop_seed = e->drop_seed; }
     return GGNN_OK;
 }
 
@@ -2096,17 +2145,8 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
     using namespace ggnn::bwd;
     if (!e) return GGNN_EINVAL;
     GGNN_REQUIRE_MODEL(e, MODEL_GCN);
-    if (!e->graph_set || !e->weights_set) return e->fail(GGNN_ESTATE, "no graph / weights set");
-    if (!e->saved_valid) return e->fail(GGNN_ESTATE, "ggnn_gcn_backward needs a preceding ggnn_forward with save_for_backward enabled");
-    if (!e->has_transpose) return e->fail(GGNN_ESTATE, "enable save_for_backward BEFORE setting the graph (the source-keyed CSR is built there)");
-    if (!grads || num_layers != e->L || (!d_h_out && e->V > 0)) return e->fail(GGNN_EINVAL, "bad backward arguments");
-    for (int l = 0; l < e->L; ++l)
-        if (((uintptr_t)grads[l].kernel & 15) || ((uintptr_t)grads[l].bias & 15))
-            return e->fail(GGNN_EINVAL, "layer %d: gradient pointers must be 16-byte aligned", l);
-    if (((uintptr_t)d_h_out & 15) || ((uintptr_t)d_h0 & 15)) return e->fail(GGNN_EINVAL, "d_h_out / d_h0 must be 16-byte aligned");
-    CU_TRY(e, cudaSetDevice(e->device));
+    if (int rc = begin_backward(e, "ggnn_gcn_backward", "setting the graph", d_h_out, grads, num_layers, d_h0)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    e->last_launches = 0;
     const int V = e->V, D = e->D, L = e->L;
     if (V == 0) return GGNN_OK;
     const size_t vd = (size_t)V * D;
@@ -2114,16 +2154,9 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
     CU_TRY(e, e->bwd_buf.reserve(4 * slab));
     char* bb = (char*)e->bwd_buf.ptr;
     float *dH = (float*)bb, *dP = (float*)(bb + slab), *S = (float*)(bb + 2 * slab), *dS = (float*)(bb + 3 * slab);
-    char* g = (char*)e->graph_buf.ptr;
-    const int* row_ptr = (const int*)(g + e->off_row_ptr);
-    const int* csr_src = (const int*)(g + e->off_src);
-    const float* slotw = (const float*)(g + e->off_slotw);
-    const int* trow = (const int*)(g + e->off_trow);
-    const int* ttgt = (const int*)(g + e->off_ttgt);
-    const float* tslotw = (const float*)(g + e->off_tslotw);
+    const GraphDev& gd = e->gd;
     std::vector<const float*> fstate(L + 1);
-    fstate[0] = e->last_h0; fstate[L] = e->last_out;
-    for (int l = 1; l < L; ++l) fstate[l] = (const float*)e->state_buf.ptr + (size_t)(l - 1) * vd;
+    for (int l = 0; l <= L; ++l) fstate[l] = layer_state(e, l, e->last_h0, e->last_out);
     const long long n = (long long)vd;
     const int eb = (int)std::min<long long>((n + 255) / 256, 4096);
     const dim3 gather_grid((V + 7) / 8, 1);
@@ -2138,7 +2171,7 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
         }
         const ggnn_gcn_layer_grads& gw = grads[l];
         if (gw.kernel) {
-            GatherJob j{row_ptr, csr_src, fstate[l], S, slotw, nullptr};
+            GatherJob j{gd.row_ptr, gd.csr_src, fstate[l], S, gd.slot_w, nullptr};
             csr_gather_all_kernel<<<gather_grid, 256, 0, st>>>(j, j, V, D, 1);
             SegList sl;
             memset(&sl, 0, sizeof sl);
@@ -2158,7 +2191,7 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
         gemm_nt_kernel<false><<<dim3((D + NT_BN - 1) / NT_BN, (V + NT_BM - 1) / NT_BM), 128, 0, st>>>(dpre, D, 0, e->gcn_w[l].kernel, D, 0, 1, dS, D, V,
                                                                                                       D, D);
         float* dst = l == 0 ? d_h0 : dH;
-        GatherJob j{trow, ttgt, dS, dst, tslotw, nullptr};
+        GatherJob j{gd.trow, gd.ttgt, dS, dst, gd.tslot_w, nullptr};
         csr_gather_all_kernel<<<gather_grid, 256, 0, st>>>(j, j, V, D, 1);
         e->last_launches += 2;
         dout = dst;
@@ -2171,7 +2204,7 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
     if (!e) return GGNN_EINVAL;
     const bool gcn = e->model == MODEL_GCN;
     if (!e->weights_set) return e->fail(GGNN_ESTATE, "%s has not been called", gcn ? "ggnn_gcn_set_weights" : "ggnn_set_weights");
-    if (!e->graph_set) return e->fail(GGNN_ESTATE, "no graph set (%s)", gcn ? "ggnn_set_graph_gcn / ggnn_set_graph_prepared" : "ggnn_set_graph_sparse/dense");
+    if (!e->graph_set) return no_graph(e);
     if ((!h0 || !h_out) && e->V > 0) return e->fail(GGNN_EINVAL, "null state pointer");
     if (((uintptr_t)h0 & 15) || ((uintptr_t)h_out & 15)) return e->fail(GGNN_EINVAL, "state pointers must be 16-byte aligned");
     CU_TRY(e, cudaSetDevice(e->device));
@@ -2180,47 +2213,15 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
     e->last_h0 = h0; e->last_out = h_out; e->saved_valid = false;
     if (e->V == 0) return GGNN_OK;
     if (e->save) { int rc = reserve_states(e); if (rc) return rc; }
-    if (e->model == MODEL_GCN) return forward_gcn(e, h0, h_out, st);
-    const size_t vd_bytes = (size_t)e->V * e->D * sizeof(float);
-    if (e->total_steps == 0) {  // no propagation at all: result is the input (sparse:152 with empty loops)
-        if (h_out != h0) CU_TRY(e, cudaMemcpyAsync(h_out, h0, vd_bytes, cudaMemcpyDeviceToDevice, st));
+    if (!gcn && e->total_steps == 0) {  // no propagation at all: result is the input (sparse:152 with empty loops)
+        if (h_out != h0) CU_TRY(e, cudaMemcpyAsync(h_out, h0, (size_t)e->V * e->D * sizeof(float), cudaMemcpyDeviceToDevice, st));
         return GGNN_OK;
     }
-    if (e->precision != GGNN_PREC_FP32) return e->stream ? forward_stream(e, h0, h_out, st) : forward_tc(e, h0, h_out, st);
-    if (e->use_att) {
-        if (e->gather_mode != GATHER_SPARSE) return e->fail(GGNN_EUNSUPPORTED, "propagation attention needs the sparse graph format");
-        CU_TRY(e, e->att_buf.reserve(sizeof(float) * (size_t)std::max<int64_t>(e->M, 1) * (size_t)(e->save ? std::max(e->total_steps, 1) : 1)));
-    }
-    FwdParams p;
-    fill_params(e, p, h0, h_out);
-    FwdKernel k = pick_fwd_kernel(e->variant, e->nb1, e->local);
-    if (!k) return e->fail(GGNN_EUNSUPPORTED, "no kernel for variant=%d nb1=%d", e->variant, e->nb1);
-    const size_t smem = fwd_smem_bytes(e->variant, e->nb1, e->D, e->T);
-    CU_TRY(e, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int threads = 256;
-    if (e->local) {
-        // layers with zero timesteps just alias the previous state (sparse:152): copy afterwards
-        k<<<e->ntiles, threads, smem, st>>>(p);
-        ++e->last_launches;
-    } else {
-        const size_t vd = (size_t)e->V * e->D;
-        float* tmp0 = (float*)e->state_buf.ptr + (size_t)(e->L - 1 > 0 ? e->L - 1 : 0) * vd;
-        float* tmp1 = tmp0 + vd;
-        for (int l = 0; l < e->L; ++l) {
-            const float* in = p.state[l];
-            if (e->steps[l] == 0) {
-                CU_TRY(e, cudaMemcpyAsync(p.state_w[l + 1], in, vd_bytes, cudaMemcpyDeviceToDevice, st));
-                continue;
-            }
-            for (int s = 0; s < e->steps[l]; ++s) {
-                float* out = (s == e->steps[l] - 1) ? p.state_w[l + 1] : ((s & 1) ? tmp1 : tmp0);
-                p.g_layer = l; p.g_step = s; p.g_in = in; p.g_out = out;
-                k<<<e->ntiles, threads, smem, st>>>(p);
-                ++e->last_launches;
-                in = out;
-            }
-        }
-    }
+    int rc;
+    if (gcn) rc = forward_gcn(e, h0, h_out, st);
+    else if (e->precision == GGNN_PREC_FP32) rc = forward_ffma(e, h0, h_out, st);
+    else rc = e->stream ? forward_stream(e, h0, h_out, st) : forward_tc(e, h0, h_out, st);
+    if (rc) return rc;
     CU_TRY(e, cudaGetLastError());
     if (e->save) { e->saved_valid = true; e->saved_drop_keep = e->drop_keep; e->saved_drop_seed = e->drop_seed; }
     return GGNN_OK;
@@ -2228,20 +2229,14 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
 
 int ggnn_forward_host_async(ggnn_engine* e, const float* h0_host, float* h_out_host, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
-    if (!e->graph_set)
-        return e->fail(GGNN_ESTATE, "no graph set (%s)", e->model == MODEL_GCN ? "ggnn_set_graph_gcn / ggnn_set_graph_prepared" : "ggnn_set_graph_sparse/dense");
+    if (!e->graph_set) return no_graph(e);
     if ((!h0_host || !h_out_host) && e->V > 0) return e->fail(GGNN_EINVAL, "null host pointer");
-    CU_TRY(e, cudaSetDevice(e->device));
-    cudaStream_t st = (cudaStream_t)stream;
     const size_t bytes = (size_t)e->V * e->D * sizeof(float);
-    const size_t slot = align_up(std::max<size_t>(bytes, 16), 256);
-    CU_TRY(e, e->io_buf.reserve(2 * slot));
-    float* d_in = (float*)e->io_buf.ptr;
-    float* d_out = (float*)((char*)e->io_buf.ptr + slot);
-    if (bytes) CU_TRY(e, cudaMemcpyAsync(d_in, h0_host, bytes, cudaMemcpyHostToDevice, st));
-    int rc = ggnn_forward(e, d_in, d_out, stream);
+    IoSlots io;
+    if (int rc = stage_io(e, h0_host, bytes, 0, (cudaStream_t)stream, io)) return rc;
+    int rc = ggnn_forward(e, io.in, io.out, stream);
     if (rc) return rc;
-    if (bytes) CU_TRY(e, cudaMemcpyAsync(h_out_host, d_out, bytes, cudaMemcpyDeviceToHost, st));
+    if (bytes) CU_TRY(e, cudaMemcpyAsync(h_out_host, io.out, bytes, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
     return GGNN_OK;
 }
 
@@ -2260,19 +2255,16 @@ template <class SetGraph>
 static int run_host(ggnn_engine* e, int64_t V, const float* h0_host, float* h_out_host, cudaStream_t st, SetGraph set_graph) {
     if (!e) return GGNN_EINVAL;
     if (V < 0 || ((!h0_host || !h_out_host) && V > 0)) return e->fail(GGNN_EINVAL, "null host pointer / negative size");
-    CU_TRY(e, cudaSetDevice(e->device));
     const size_t bytes = (size_t)V * e->D * sizeof(float);
-    const size_t slot = align_up(std::max<size_t>(bytes, 16), 256);
-    CU_TRY(e, e->io_buf.reserve(2 * slot));
-    float* d_in = (float*)e->io_buf.ptr;
-    float* d_out = (float*)((char*)e->io_buf.ptr + slot);
-    if (bytes) CU_TRY(e, cudaMemcpyAsync(d_in, h0_host, bytes, cudaMemcpyHostToDevice, st));
-    int rc = set_graph();
+    IoSlots io;
+    int rc = stage_io(e, h0_host, bytes, 0, st, io);
+    if (rc) return rc;
+    rc = set_graph();
     if (rc) return rc;
     if ((int64_t)e->V != V) return e->fail(GGNN_EINVAL, "graph has %d nodes, h0 has %lld rows", e->V, (long long)V);
-    rc = ggnn_forward(e, d_in, d_out, (ggnn_stream_t)st);
+    rc = ggnn_forward(e, io.in, io.out, (ggnn_stream_t)st);
     if (rc) return rc;
-    if (bytes) CU_TRY(e, cudaMemcpyAsync(h_out_host, d_out, bytes, cudaMemcpyDeviceToHost, st));
+    if (bytes) CU_TRY(e, cudaMemcpyAsync(h_out_host, io.out, bytes, cudaMemcpyDeviceToHost, st));
     CU_TRY(e, cudaStreamSynchronize(st));
     return GGNN_OK;
 }
@@ -2394,37 +2386,34 @@ int ggnn_run_sparse_host_readout(ggnn_engine* e, int32_t V, const int32_t* const
     if (V < 0 || G < 0 || num_tasks <= 0 || !tasks || !loss_out || !accuracy_out || (V > 0 && (!h0_host || !graph_nodes_list)) ||
         (G > 0 && (!target_values || !target_mask)))
         return e->fail(GGNN_EINVAL, "null / negative argument");
-    CU_TRY(e, cudaSetDevice(e->device));
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t bytes = (size_t)V * e->D * sizeof(float);
-    const size_t slot = align_up(std::max<size_t>(bytes, 16), 256);
     const size_t tg = (size_t)num_tasks * std::max(G, 1);
     // device scratch behind the two state slots: targets | masks | per-task readout [tasks][G] | results [2*tasks]
-    const size_t o_tv = 2 * slot, o_tm = o_tv + align_up(tg * 4, 256), o_ro = o_tm + align_up(tg * 4, 256), o_res = o_ro + align_up(tg * 4, 256);
-    CU_TRY(e, e->io_buf.reserve(o_res + align_up((size_t)2 * num_tasks * 4, 256)));
-    char* io = (char*)e->io_buf.ptr;
-    float *d_in = (float*)io, *d_out = (float*)(io + slot);
-    if (bytes) CU_TRY(e, cudaMemcpyAsync(d_in, h0_host, bytes, cudaMemcpyHostToDevice, st));        // overlaps the host-side CSR build below
+    const size_t o_tm = align_up(tg * 4, 256), o_ro = 2 * o_tm, o_res = 3 * o_tm;
+    IoSlots io;   // the h0 upload overlaps the host-side CSR build below
+    int rc = stage_io(e, h0_host, (size_t)V * e->D * sizeof(float), o_res + align_up((size_t)2 * num_tasks * 4, 256), st, io);
+    if (rc) return rc;
+    char* sc = io.scratch;
     if (G > 0) {
-        CU_TRY(e, cudaMemcpyAsync(io + o_tv, target_values, tg * 4, cudaMemcpyHostToDevice, st));
-        CU_TRY(e, cudaMemcpyAsync(io + o_tm, target_mask, tg * 4, cudaMemcpyHostToDevice, st));
+        CU_TRY(e, cudaMemcpyAsync(sc, target_values, tg * 4, cudaMemcpyHostToDevice, st));
+        CU_TRY(e, cudaMemcpyAsync(sc + o_tm, target_mask, tg * 4, cudaMemcpyHostToDevice, st));
     }
-    int rc = ggnn_set_graph_sparse(e, V, adjacency_lists, num_edges, indeg, stream);
+    rc = ggnn_set_graph_sparse(e, V, adjacency_lists, num_edges, indeg, stream);
     if (rc) return rc;
     rc = ggnn_readout_set_graphs(e, V, graph_nodes_list, G, 0, nullptr, stream);
     if (rc) return rc;
-    rc = ggnn_forward(e, d_in, d_out, stream);
+    rc = ggnn_forward(e, io.in, io.out, stream);
     if (rc) return rc;
     for (int t = 0; t < num_tasks; ++t) {
-        rc = ggnn_readout_forward(e, d_out, d_in, tasks[t].w_gate, tasks[t].b_gate, tasks[t].w_trans, tasks[t].b_trans,
-                                  (float*)(io + o_ro) + (size_t)t * G, stream);
+        rc = ggnn_readout_forward(e, io.out, io.in, tasks[t].w_gate, tasks[t].b_gate, tasks[t].w_trans, tasks[t].b_trans,
+                                  (float*)(sc + o_ro) + (size_t)t * G, stream);
         if (rc) return rc;
     }
-    readout::masked_loss_kernel<<<num_tasks, 256, 0, st>>>((const float*)(io + o_ro), (const float*)(io + o_tv), (const float*)(io + o_tm),
-                                                           (float*)(io + o_res), G, num_tasks);
+    readout::masked_loss_kernel<<<num_tasks, 256, 0, st>>>((const float*)(sc + o_ro), (const float*)sc, (const float*)(sc + o_tm),
+                                                           (float*)(sc + o_res), G, num_tasks);
     CU_TRY(e, cudaGetLastError());
     std::vector<float> res((size_t)2 * num_tasks);
-    CU_TRY(e, cudaMemcpyAsync(res.data(), io + o_res, sizeof(float) * 2 * num_tasks, cudaMemcpyDeviceToHost, st));
+    CU_TRY(e, cudaMemcpyAsync(res.data(), sc + o_res, sizeof(float) * 2 * num_tasks, cudaMemcpyDeviceToHost, st));
     CU_TRY(e, cudaStreamSynchronize(st));
     for (int t = 0; t < num_tasks; ++t) { loss_out[t] = res[t]; accuracy_out[t] = res[num_tasks + t]; }
     return GGNN_OK;
@@ -2484,10 +2473,9 @@ int ggnn_get_csr(ggnn_engine* e, int32_t* row_ptr, int32_t* src, int32_t* msg) {
     if (!e->graph_set || e->gather_mode != GATHER_SPARSE) return e->fail(GGNN_ESTATE, "no sparse graph set");
     CU_TRY(e, cudaSetDevice(e->device));
     CU_TRY(e, cudaDeviceSynchronize());
-    char* g = (char*)e->graph_buf.ptr;
-    if (row_ptr) CU_TRY(e, cudaMemcpy(row_ptr, g + e->off_row_ptr, sizeof(int) * ((size_t)e->V * e->T + 1), cudaMemcpyDeviceToHost));
-    if (src && e->M) CU_TRY(e, cudaMemcpy(src, g + e->off_src, sizeof(int) * (size_t)e->M, cudaMemcpyDeviceToHost));
-    if (msg && e->M) CU_TRY(e, cudaMemcpy(msg, g + e->off_msg, sizeof(int) * (size_t)e->M, cudaMemcpyDeviceToHost));
+    if (row_ptr) CU_TRY(e, cudaMemcpy(row_ptr, e->gd.row_ptr, sizeof(int) * ((size_t)e->V * e->T + 1), cudaMemcpyDeviceToHost));
+    if (src && e->M) CU_TRY(e, cudaMemcpy(src, e->gd.csr_src, sizeof(int) * (size_t)e->M, cudaMemcpyDeviceToHost));
+    if (msg && e->M) CU_TRY(e, cudaMemcpy(msg, e->gd.csr_msg, sizeof(int) * (size_t)e->M, cudaMemcpyDeviceToHost));
     return GGNN_OK;
 }
 
@@ -2495,10 +2483,7 @@ int ggnn_layer_state(ggnn_engine* e, int32_t layer, const float** dev_ptr) {
     if (!e || !dev_ptr) return GGNN_EINVAL;
     if (layer < 0 || layer > e->L) return e->fail(GGNN_EINVAL, "layer index %d out of range", layer);
     if (!e->last_out) return e->fail(GGNN_ESTATE, "no forward has run");
-    const size_t vd = (size_t)std::max(e->V, 1) * e->D;
-    if (layer == 0) *dev_ptr = e->last_h0;
-    else if (layer == e->L) *dev_ptr = e->last_out;
-    else *dev_ptr = (const float*)e->state_buf.ptr + (size_t)(layer - 1) * vd;
+    *dev_ptr = layer_state(e, layer, e->last_h0, e->last_out);
     return GGNN_OK;
 }
 

@@ -237,6 +237,34 @@ def test_ring_geometry_does_not_change_the_result(monkeypatch, ksteps, stages):
     np.testing.assert_array_equal(got, U.engine_sparse(*args, precision=PREC))
 
 
+@pytest.mark.parametrize("first", ["1", "0"])
+def test_set_weights_once_reaches_both_plans_of_one_engine(monkeypatch, first):
+    """One engine, weights set once per update, batches alternating between the streaming and the tile-local plan: each plan keeps its
+    own tiled copy of the weights, and a forward after set_weights must run on the new weights whichever plan tiled them last."""
+    import torch
+    from gated_graph_neural_network_samples_b200.engine import PropagationEngine
+    _, b = U.molecule_batch(40, 100, T=4, seed=13)
+    h0, adj, indeg = b["initial_node_representation"], b["adjacency_lists"], b["num_incoming_edges_per_type"]
+    w1, w2 = (O.init_sparse_weights(CFG2, 4, np.random.default_rng(s)) for s in (1, 2))
+    eng = PropagationEngine(CFG2, 4, precision=PREC)
+    h0_dev = torch.from_numpy(h0).cuda()
+
+    def forward(stream):
+        monkeypatch.setenv("GGNN_TC_STREAM", stream)   # read when the batch is prepared
+        eng.set_graph_sparse(adj, indeg)
+        assert ("STREAM" in eng.plan) == (stream == "1"), eng.plan
+        out = eng.forward(h0_dev).cpu().numpy()
+        eng.sync_check()
+        return out
+
+    other = "0" if first == "1" else "1"
+    eng.set_weights(U.to_cuda_weights(w1))
+    forward(first)
+    eng.set_weights(U.to_cuda_weights(w2))
+    forward(other)
+    _check(forward(first), O.sparse_propagation_np(h0, adj, indeg, w2, CFG2, dtype=np.float64), "plan %s after the other plan re-tiled" % first)
+
+
 def test_twelve_edge_types_and_hidden_100_padding(monkeypatch):
     """More edge types than any BASELINE configuration (tile masks, K segments) on the forced streaming plan at a hidden size that is
     not a multiple of 16 (DP = 112: seven K-steps per segment, a partial last stage)."""
