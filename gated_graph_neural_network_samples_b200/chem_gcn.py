@@ -36,6 +36,7 @@ def _propagation_function():
             engine.set_weights(kernels, biases)
             engine.set_save_for_backward(need)
             out = engine.forward(h0.detach().contiguous())
+            ctx.serial = engine.serial   # the backward refuses once another forward, graph or weights replaced this one's
             ctx.engine, ctx.shapes = engine, [t.shape for t in weights]
             ctx.h0_needs = bool(ctx.needs_input_grad[1])
             ctx.keepalive = (h0, out, kernels, biases)   # the engine reads these buffers again in ggnn_gcn_backward
@@ -43,6 +44,7 @@ def _propagation_function():
 
         @staticmethod
         def backward(ctx, d_out):
+            ctx.engine.require_serial(ctx.serial, "the GCN propagation's backward")
             L = ctx.engine.L
             grads = [torch.zeros(s, dtype=torch.float32, device=d_out.device) for s in ctx.shapes]
             layers = [{'kernel': grads[l], 'bias': grads[L + l] if len(grads) > L else None} for l in range(L)]

@@ -34,6 +34,7 @@ def _propagation_function():
             engine.set_weights([{k: v.detach().contiguous() for k, v in lw.items()} for lw in layers])
             engine.set_save_for_backward(need)
             out = engine.forward(h0.detach().contiguous())
+            ctx.serial = engine.serial   # the backward refuses once another forward, graph or weights replaced this one's
             ctx.engine, ctx.layout, ctx.shapes = engine, layout, [t.shape for t in flat]
             ctx.h0_needs = bool(ctx.needs_input_grad[2])
             ctx.keepalive = (h0, out, flat)   # the engine reads these buffers again in ggnn_backward
@@ -41,6 +42,7 @@ def _propagation_function():
 
         @staticmethod
         def backward(ctx, d_out):
+            ctx.engine.require_serial(ctx.serial, "the propagation's backward")
             grads_flat = [torch.zeros(s, dtype=torch.float32, device=d_out.device) for s in ctx.shapes]
             grads = [{k: grads_flat[i] for k, i in lay.items()} for lay in ctx.layout]
             d_h0 = torch.zeros_like(d_out) if ctx.h0_needs else None

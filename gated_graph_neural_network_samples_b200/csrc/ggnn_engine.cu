@@ -222,10 +222,13 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     WeightTiles ts_tiles;   // ... and for the streaming kernel
     DevBuf tc_respre;   // residual pre-products [ntiles][128][3*DP]
     DevBuf err_flag;    // device int written by kernels on a barrier timeout
+    // the state buffers of the last forward on the current graph; fwd_valid is cleared by every graph upload.  Without save_for_backward
+    // the fused GCN kernel keeps the layers between h0 and h_out on chip: layers_written says whether state_buf holds them.
     const float* last_h0 = nullptr;
     float* last_out = nullptr;
+    bool fwd_valid = false, layers_written = false;
     bool save = false;
-    bool saved_valid = false;
+    bool saved_valid = false;   // the saved activations are those of the last forward, with the current weights
     DevBuf ts_images;                                // the streaming plan's operand images and chunk-major states
     DevBuf ts_virt;                                  // the operand image of the streaming plan's virtual rows
     DevBuf att_buf;                  // attention probabilities per target-CSR slot ([steps][M] when saving for backward, else [M])
@@ -336,6 +339,14 @@ static int launch_steps(ggnn_engine* e, Params& p, cudaStream_t st, Launch launc
         }
     }
     return GGNN_OK;
+}
+
+// Everything the engine knows about the previous batch beyond its buffers: the graph, the last forward and its saved activations, and the
+// readout's node -> graph map.  Called first by every graph upload, so a failed upload leaves no batch behind either.
+static void forget_batch(ggnn_engine* e) {
+    e->graph_set = false; e->saved_valid = false;
+    e->last_h0 = nullptr; e->last_out = nullptr; e->fwd_valid = false; e->layers_written = false;
+    e->ro_V = -1;
 }
 
 static int no_graph(ggnn_engine* e) {
@@ -888,10 +899,11 @@ int ggnn_set_weights(ggnn_engine* e, const ggnn_layer_weights* layers, int32_t n
         const void* ps[7] = {w.edge_weights, w.edge_biases, w.gate_kernel, w.gate_bias, w.cand_kernel, w.cand_bias, w.cand_hidden_bias};
         for (const void* q : ps)
             if (q && ((uintptr_t)q & 15)) return e->fail(GGNN_EINVAL, "layer %d: weight pointers must be 16-byte aligned", l);
-        e->w[l] = w;
     }
+    for (int l = 0; l < e->L; ++l) e->w[l] = layers[l];   // all or nothing: a refused call leaves the previous weights bound
     e->weights_set = true;
-    ++e->weights_gen;   // the tensor-core paths re-tile their bf16 copies at their next forward
+    ++e->weights_gen;       // the tensor-core paths re-tile their bf16 copies at their next forward
+    e->saved_valid = false;   // a backward combines the saved activations with the bound weights: both must be the last forward's
     return GGNN_OK;
 }
 
@@ -1435,7 +1447,7 @@ static int begin_prepare(ggnn_prepared_graph** inout, const ggnn_engine* e, cons
 // halves a caller can run on two threads), then the engine uploads it.
 template <class Build>
 static int set_graph_from_own_prep(ggnn_engine* e, ggnn_stream_t stream, Build build) {
-    e->graph_set = false; e->saved_valid = false;
+    forget_batch(e);
     int rc = build(&e->own_prep);
     if (rc) { if (e->own_prep) e->err = e->own_prep->err; return rc; }
     return ggnn_set_graph_prepared(e, e->own_prep, stream);
@@ -1491,7 +1503,7 @@ int ggnn_prepare_graph_sparse(const ggnn_engine* e, int32_t save_for_backward, i
 
 int ggnn_set_graph_prepared(ggnn_engine* e, ggnn_prepared_graph* g, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
-    e->graph_set = false; e->saved_valid = false;
+    forget_batch(e);
     if (!g || !g->valid) return e->fail(GGNN_ESTATE, "the prepared graph is empty (its build failed or never ran)");
     const ModelShape& q = g->shape;
     if (q.model != e->model)
@@ -2057,6 +2069,7 @@ int ggnn_gcn_set_weights(ggnn_engine* e, const ggnn_gcn_layer_weights* layers, i
     for (int l = 0; l < e->L; ++l) { e->gcn_w[l] = layers[l]; if (!e->use_bias) e->gcn_w[l].bias = nullptr; }
     e->weights_set = true;
     ++e->weights_gen;
+    e->saved_valid = false;   // as in ggnn_set_weights
     return GGNN_OK;
 }
 
@@ -2087,9 +2100,12 @@ int ggnn_prepared_graph_slot_weights(const ggnn_prepared_graph* g, float* target
     return GGNN_OK;
 }
 
+// Whether the GCN runs on its wgmma kernel (else on the fp32 kernel, one launch per layer).
+static bool gcn_on_tensor_cores(const ggnn_engine* e) { return e->precision != GGNN_PREC_FP32 && e->DP <= 128; }
+
 static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream_t st) {
     const int D = e->D, DP = e->DP, L = e->L, V = e->V;
-    const bool tcore = e->precision != GGNN_PREC_FP32 && DP <= 128;
+    const bool tcore = gcn_on_tensor_cores(e);
     gcn::GcnParams p;
     memset(&p, 0, sizeof p);
     p.V = V; p.D = D; p.DP = DP; p.L = L;
@@ -2210,12 +2226,17 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
     CU_TRY(e, cudaSetDevice(e->device));
     cudaStream_t st = (cudaStream_t)stream;
     e->last_launches = 0;
-    e->last_h0 = h0; e->last_out = h_out; e->saved_valid = false;
-    if (e->V == 0) return GGNN_OK;
+    e->fwd_valid = false; e->layers_written = false; e->saved_valid = false;
+    const auto done = [&](bool layers_written, bool saved) {
+        e->last_h0 = h0; e->last_out = h_out; e->fwd_valid = true; e->layers_written = layers_written;
+        if (saved) { e->saved_valid = true; e->saved_drop_keep = e->drop_keep; e->saved_drop_seed = e->drop_seed; }
+        return GGNN_OK;
+    };
+    if (e->V == 0) return done(true, e->save);   // the backward of an empty batch has nothing to compute either
     if (e->save) { int rc = reserve_states(e); if (rc) return rc; }
     if (!gcn && e->total_steps == 0) {  // no propagation at all: result is the input (sparse:152 with empty loops)
         if (h_out != h0) CU_TRY(e, cudaMemcpyAsync(h_out, h0, (size_t)e->V * e->D * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        return GGNN_OK;
+        return done(false, false);
     }
     int rc;
     if (gcn) rc = forward_gcn(e, h0, h_out, st);
@@ -2223,8 +2244,7 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
     else rc = e->stream ? forward_stream(e, h0, h_out, st) : forward_tc(e, h0, h_out, st);
     if (rc) return rc;
     CU_TRY(e, cudaGetLastError());
-    if (e->save) { e->saved_valid = true; e->saved_drop_keep = e->drop_keep; e->saved_drop_seed = e->drop_seed; }
-    return GGNN_OK;
+    return done(!(gcn && e->local && gcn_on_tensor_cores(e) && !e->save), e->save);
 }
 
 int ggnn_forward_host_async(ggnn_engine* e, const float* h0_host, float* h_out_host, ggnn_stream_t stream) {
@@ -2482,7 +2502,9 @@ int ggnn_get_csr(ggnn_engine* e, int32_t* row_ptr, int32_t* src, int32_t* msg) {
 int ggnn_layer_state(ggnn_engine* e, int32_t layer, const float** dev_ptr) {
     if (!e || !dev_ptr) return GGNN_EINVAL;
     if (layer < 0 || layer > e->L) return e->fail(GGNN_EINVAL, "layer index %d out of range", layer);
-    if (!e->last_out) return e->fail(GGNN_ESTATE, "no forward has run");
+    if (!e->graph_set || !e->fwd_valid) return e->fail(GGNN_ESTATE, "no forward has run on the current graph");
+    if (layer > 0 && layer < e->L && !e->layers_written)
+        return e->fail(GGNN_ESTATE, "layer %d: the last forward did not write the layers between h0 and the result (enable save_for_backward)", layer);
     *dev_ptr = layer_state(e, layer, e->last_h0, e->last_out);
     return GGNN_OK;
 }

@@ -212,6 +212,7 @@ class PropagationEngine:
             raise GgnnError(self.lib.ggnn_last_error(None).decode())
         self.device = int(device)
         self.V = 0
+        self.serial = 0   # bumped by every forward, graph upload and weight binding: see require_serial
         self._weights_keepalive = None
         self._graph_keepalive = None
 
@@ -254,6 +255,7 @@ class PropagationEngine:
                     raise GgnnError("layer %d %s has shape %s, expected %s" % (l, f, tuple(t.shape), shapes[f]))
                 setattr(arr[l], f, t.data_ptr())
                 keep.append(t)
+        self.serial += 1
         self._check(self.lib.ggnn_set_weights(self._h, arr, len(layers)))
         self._weights_keepalive = keep
 
@@ -274,6 +276,7 @@ class PropagationEngine:
         ``[V, T]`` in-degree table.  HOST arrays; index validation, CSR build and upload happen in the library."""
         adjs, indeg, ptrs, counts = self._sparse_args(adjacency_lists, num_incoming_edges_per_type)
         V = indeg.shape[0]
+        self.serial += 1
         self._check(self.lib.ggnn_set_graph_sparse(self._h, V, ptrs, counts, indeg.ctypes.data, self._stream()))
         self.V = V
         self._graph_keepalive = (adjs, indeg)
@@ -307,6 +310,7 @@ class PropagationEngine:
 
     def set_graph_prepared(self, g: "PreparedGraph"):
         """The DEVICE half: adopt the plan, enqueue the one H2D copy of the image.  Keep ``g`` alive until the stream has passed it."""
+        self.serial += 1
         self._check(self.lib.ggnn_set_graph_prepared(self._h, g._h, self._stream()))
         self.V = g.V
         self._graph_keepalive = (g,)
@@ -321,6 +325,7 @@ class PropagationEngine:
             raise GgnnError("h0 has %d elements, the graph has %d nodes x %d" % (h0.size, V, self.D))
         if out is None:
             out = np.empty_like(h0)
+        self.serial += 1
         self._check(self.lib.ggnn_run_sparse_host(self._h, V, ptrs, counts, indeg.ctypes.data, h0.ctypes.data, out.ctypes.data, self._stream()))
         self.V = V
         self._graph_keepalive = (adjs, indeg)
@@ -344,6 +349,7 @@ class PropagationEngine:
             arr[i].w_gate, arr[i].b_gate = self._f32(wg, 2 * self.D, "w_gate"), self._f32(bg, 1, "b_gate")
             arr[i].w_trans, arr[i].b_trans = self._f32(wt, self.D, "w_trans"), self._f32(bt, 1, "b_trans")
         loss, acc = np.empty(nt, np.float32), np.empty(nt, np.float32)
+        self.serial += 1
         self._check(self.lib.ggnn_run_sparse_host_readout(self._h, V, ptrs, counts, indeg.ctypes.data, h0.ctypes.data, gnl.ctypes.data, G, nt, arr,
                                                           tv.ctypes.data, tm.ctypes.data, loss.ctypes.data, acc.ctypes.data, self._stream()))
         self.V = V
@@ -360,6 +366,7 @@ class PropagationEngine:
             raise GgnnError("h0 has %d elements, the graph has %d nodes x %d" % (h0.size, V, self.D))
         if out is None:
             out = np.empty_like(h0)
+        self.serial += 1
         self._check(self.lib.ggnn_run_dense_host(self._h, a.shape[0], a.shape[2], a.ctypes.data, h0.ctypes.data, out.ctypes.data, self._stream()))
         self.V = V
         self._graph_keepalive = (a,)
@@ -370,6 +377,7 @@ class PropagationEngine:
         a = np.ascontiguousarray(np.asarray(adjacency_matrix, dtype=np.float32))
         if a.ndim != 4 or a.shape[1] != self.T or a.shape[2] != a.shape[3]:
             raise GgnnError("adjacency_matrix must be [b, %d, v, v]" % self.T)
+        self.serial += 1
         self._check(self.lib.ggnn_set_graph_dense(self._h, a.shape[0], a.shape[2], a.ctypes.data, self._stream()))
         self.V = a.shape[0] * a.shape[2]
         self._graph_keepalive = (a,)
@@ -384,6 +392,7 @@ class PropagationEngine:
             raise GgnnError("h0 has %d elements, the graph has %d nodes x %d" % (h0.numel(), self.V, self.D))
         if out is None:
             out = torch.empty_like(h0)
+        self.serial += 1
         self._check(self.lib.ggnn_forward(self._h, h0.data_ptr(), out.data_ptr(), self._stream()))
         return out
 
@@ -396,8 +405,17 @@ class PropagationEngine:
         if out is None:
             out = np.empty_like(h0)
         fn = self.lib.ggnn_forward_host if sync else self.lib.ggnn_forward_host_async
+        self.serial += 1
         self._check(fn(self._h, h0.ctypes.data, out.ctypes.data, self._stream()))
         return out
+
+    def require_serial(self, serial: int, what: str = "this backward"):
+        """Raises ``GgnnError`` unless the engine's serial is still ``serial``.  An autograd node records the serial after its forward:
+        ``backward`` reads the engine's saved activations, states and weights, which any later forward, graph upload or weight binding
+        replaces.  Repeated backward calls of one forward keep the serial."""
+        if self.serial != serial:
+            raise GgnnError("%s belongs to an earlier forward: the engine has run %d forward / graph / weight call(s) since, so its saved "
+                            "activations are not this forward's" % (what, self.serial - serial))
 
     def sync_check(self):
         """Synchronise the stream and raise if a kernel reported an (always bounded) barrier timeout."""
@@ -492,6 +510,9 @@ class PropagationEngine:
         """Copy of node_states_per_layer[layer] (0 = h0, L = result) of the last forward, as a CUDA tensor."""
         import torch
         out = torch.empty(self.V, self.D, dtype=torch.float32, device="cuda:%d" % self.device)
+        if self.V == 0:   # nothing to copy (an empty tensor has no storage); the engine still says whether the state exists
+            self._check(self.lib.ggnn_layer_state(self._h, int(layer), C.byref(C.c_void_p())))
+            return out
         self._check(self.lib.ggnn_copy_layer_state(self._h, int(layer), out.data_ptr(), self._stream()))
         return out
 
@@ -522,6 +543,7 @@ class GCNEngine(PropagationEngine):
             raise GgnnError(self.lib.ggnn_last_error(None).decode())
         self.device = int(device)
         self.V = 0
+        self.serial = 0   # bumped by every forward, graph upload and weight binding: see require_serial
         self._weights_keepalive = None
         self._graph_keepalive = None
 
@@ -537,6 +559,7 @@ class GCNEngine(PropagationEngine):
                     raise GgnnError("the engine uses biases: pass biases")
                 arr[l].bias = self._f32(biases[l], self.D, "layer %d bias" % l)
                 keep.append(biases[l])
+        self.serial += 1
         self._check(self.lib.ggnn_gcn_set_weights(self._h, arr, len(kernels)))
         self._weights_keepalive = keep
 
@@ -544,6 +567,7 @@ class GCNEngine(PropagationEngine):
         """The reference's feed (chem_tensorflow_gcn.py:44-47): ``[nnz, 2]`` (row i = output, column j = input) and ``[nnz]`` weights, HOST
         arrays; validation, stable CSR build, tile plan and upload happen in the library."""
         lst, w = _gcn_arrays(adjacency_list, adjacency_weights)
+        self.serial += 1
         self._check(self.lib.ggnn_set_graph_gcn(self._h, int(num_nodes), lst.shape[0], lst.ctypes.data, w.ctypes.data, self._stream()))
         self.V = int(num_nodes)
         self._graph_keepalive = (lst, w)

@@ -97,7 +97,9 @@ int ggnn_create(const ggnn_config* cfg, ggnn_engine** out);
 int ggnn_destroy(ggnn_engine* e);
 const char* ggnn_last_error(const ggnn_engine* e); /* e may be NULL: error of the last failed ggnn_create */
 
-/* Bind the trainables (device pointers, one entry per layer); pointers are read at every forward. */
+/* Bind the trainables (device pointers, one entry per layer); pointers are read at every forward.  A refused call binds nothing.  The
+ * saved activations of the last forward are dropped: ggnn_backward then returns GGNN_ESTATE until the next forward with save_for_backward,
+ * so a backward never combines one forward's activations with other weights. */
 int ggnn_set_weights(ggnn_engine* e, const ggnn_layer_weights* layers, int32_t num_layers);
 
 /* Feed one batch's graph structure in the reference wire format (sparse:331-348), HOST pointers:
@@ -120,6 +122,8 @@ int ggnn_set_graph_sparse(ggnn_engine* e, int32_t num_nodes, const int32_t* cons
  *                               previous upload).
  *   ggnn_set_graph_prepared     engine thread: adopts the plan and enqueues the single H2D copy of the image on `stream`.  The prepared
  *                               graph must stay alive (and must not be rebuilt from a thread that skips the wait above) until that copy ran.
+ * Every graph upload, failed ones included, first forgets the previous batch: its forward (ggnn_layer_state), its saved activations
+ * (ggnn_backward) and its readout map (ggnn_readout_set_graphs must follow the upload).
  * ggnn_set_graph_sparse is exactly these two calls on an engine-owned prepared graph.  On failure the text is in
  * ggnn_prepared_graph_error (prepare) / ggnn_last_error (set). */
 typedef struct ggnn_prepared_graph ggnn_prepared_graph;
@@ -183,7 +187,8 @@ int ggnn_forward_host_async(ggnn_engine* e, const float* h0_host, float* h_out_h
  *   dense : graph_nodes_list NULL, nodes_per_graph = num_vertices (graph = row / num_vertices), node_mask [b*v] float32 (dense:126)
  * Nodes grouped by graph (what the packers produce) are summed in node order, deterministically, like TF's CPU
  * unsorted_segment_sum; an ungrouped list falls back to float atomics.  All other pointers are DEVICE fp32; `out` is [num_graphs].
- * ggnn_readout_backward writes d_h_last [V,D] and ACCUMULATES into the weight gradients (caller zeroes; any may be NULL). */
+ * ggnn_readout_backward writes d_h_last [V,D] and ACCUMULATES into the weight gradients (caller zeroes; any may be NULL).  The map belongs
+ * to the current batch: a graph upload drops it, and the readout calls return GGNN_ESTATE until ggnn_readout_set_graphs runs again. */
 int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* graph_nodes_list, int32_t num_graphs,
                             int32_t nodes_per_graph, const float* node_mask, ggnn_stream_t stream);
 int ggnn_readout_forward(ggnn_engine* e, const float* h_last, const float* h0, const float* w_gate, const float* b_gate,
@@ -299,7 +304,9 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
 int ggnn_num_messages(const ggnn_engine* e, int64_t* out);
 /* Copies the engine's device CSR back: row_ptr [V*T+1] (rows keyed target*T+type), src [M], msg [M]. */
 int ggnn_get_csr(ggnn_engine* e, int32_t* row_ptr, int32_t* src, int32_t* msg);
-/* Pointer to node_states_per_layer[layer] (layer 0 = h0, num_layers = final), valid after forward. */
+/* Pointer to node_states_per_layer[layer] (layer 0 = h0, num_layers = final) of the last forward.  GGNN_ESTATE until a forward has run on
+ * the current graph (every graph upload clears it), and for 0 < layer < num_layers when the last forward did not write those layers: the
+ * GCN wgmma kernel's LOCAL plan without save_for_backward, and a model without timesteps. */
 int ggnn_layer_state(ggnn_engine* e, int32_t layer, const float** dev_ptr);
 /* Device-to-device copy of that state into dst [V, D] on `stream`. */
 int ggnn_copy_layer_state(ggnn_engine* e, int32_t layer, float* dst, ggnn_stream_t stream);
