@@ -1805,19 +1805,24 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
     p.nparts = e->precision == GGNN_PREC_BF16X3 ? 3 : 1;
     p.kgs = e->tc_kgs;
     const size_t opb = (size_t)DP * (size_t)p.kgs / 4, stage = (size_t)DP * 128;   // a ring slot = two 64*DP-byte K-step stages
-    // tile-local sparse graphs: stage the tile's CSR slice in shared memory when it is small enough
+    const size_t ops = 3 * opb;   // h, agg and the gather / r*h operand tiles
+    const size_t avail = e->max_smem > 1024 ? e->max_smem - 1024 : 0;
+    // tile-local sparse graphs: stage the tile's CSR slice in shared memory when it is small enough and leaves the weight ring the two
+    // slots a worker holds at once (one slot's MMAs in flight while the next slot's are issued; DP 128 with 128-row tiles has room for
+    // two slots only without the cache)
     size_t csr_b = 0;
     if (e->local && e->gather_mode == GATHER_SPARSE && e->T <= 16 && e->max_tile_msgs <= 4096) {
-        p.csr_cache = 1;
-        p.csr_cap_msgs = (e->max_tile_msgs + 15) / 16 * 16;
-        csr_b = (size_t)((tc::TILE_M * e->T + 1 + 7) & ~7) * 2 + (size_t)p.csr_cap_msgs;
+        const int cap = (e->max_tile_msgs + 15) / 16 * 16;
+        const size_t b = (size_t)((tc::TILE_M * e->T + 1 + 7) & ~7) * 2 + (size_t)cap;
+        if (avail >= ops + (size_t)3 * DP * sizeof(float) + b + 64 + 2 * stage) {
+            p.csr_cache = 1;
+            p.csr_cap_msgs = cap;
+            csr_b = b;
+        }
     }
     const size_t bias_b = (size_t)3 * DP * sizeof(float) + csr_b + 64;
-    const size_t avail = e->max_smem > 1024 ? e->max_smem - 1024 : 0;
-    if (avail < 3 * opb + bias_b + stage) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the tensor-core tile (DP=%d)", DP);
-    const size_t ops = 3 * opb;   // h, agg and the gather / r*h operand tiles
+    if (avail < ops + bias_b + 2 * stage) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the tensor-core tile (DP=%d)", DP);
     p.nstages = (int)std::min<size_t>(tc::MAX_STAGES, (avail - ops - bias_b) / stage);
-    if (p.nstages < 1) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the weight ring (DP=%d)", DP);
     const size_t smem = ops + bias_b + (size_t)p.nstages * stage;
     const WeightTiles& wt = e->tc_tiles;
     const uint8_t* wb = (const uint8_t*)wt.buf.ptr;
@@ -1828,22 +1833,26 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
     }
     p.res_pre = (float*)e->tc_respre.ptr;
     p.error_flag = (int*)e->err_flag.ptr;
-    // the wgmma N of a warpgroup's columns is an instruction immediate: one kernel per padded hidden size and layout (compact tiles
-    // split the columns four ways, 128-row tiles two ways)
+    // the wgmma N of a warpgroup's columns is an instruction immediate: one kernel per padded hidden size, layout (compact tiles
+    // split the columns four ways, 128-row tiles two ways) and precision (bf16x3 / bf16: the MMA path is straight-line code)
     void (*kern)(tc::TcParams) = nullptr;
-    const bool compact = e->tc_kgs == 1024;
+    const bool compact = e->tc_kgs == 1024, x3 = p.nparts == 3;
     switch (DP / 2) {
+#define GGNN_TC_LAYOUTS(nh, x3)                                                                                                       \
+    (!e->local ? tc::ggnn_fwd_tc_kernel<false, nh, false, x3>                                                                         \
+               : (compact ? tc::ggnn_fwd_tc_kernel<true, nh, true, x3> : tc::ggnn_fwd_tc_kernel<true, nh, false, x3>))
 #define GGNN_TC_CASE(nh)                                                                                                              \
     case nh:                                                                                                                          \
-        kern = !e->local ? tc::ggnn_fwd_tc_kernel<false, nh, false>                                                                   \
-                         : (compact ? tc::ggnn_fwd_tc_kernel<true, nh, true> : tc::ggnn_fwd_tc_kernel<true, nh, false>);            \
+        kern = x3 ? GGNN_TC_LAYOUTS(nh, true) : GGNN_TC_LAYOUTS(nh, false);                                                           \
         break;
         GGNN_TC_CASE(8) GGNN_TC_CASE(16) GGNN_TC_CASE(24) GGNN_TC_CASE(32) GGNN_TC_CASE(40) GGNN_TC_CASE(48) GGNN_TC_CASE(56) GGNN_TC_CASE(64)
 #undef GGNN_TC_CASE
+#undef GGNN_TC_LAYOUTS
         default: return e->fail(GGNN_EUNSUPPORTED, "no tile-local tensor-core kernel for DP=%d", DP);
     }
     CU_TRY(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    return launch_steps(e, p, st, [&](const tc::TcParams& q) { kern<<<e->ntiles, tc::NTHREADS, smem, st>>>(q); });
+    const int nthreads = e->local && compact ? tc::NTHREADS<true> : tc::NTHREADS<false>;
+    return launch_steps(e, p, st, [&](const tc::TcParams& q) { kern<<<e->ntiles, nthreads, smem, st>>>(q); });
 }
 
 // ------------------------------------------------------------------------------------------ streaming tensor-core path (host)
@@ -2128,7 +2137,11 @@ static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream
         const size_t smem = opb + (size_t)p.nstages * slot_b + sh_b;
         void (*kern)(gcn::GcnParams) = nullptr;
         switch (DP / 2) {
-#define GGNN_GCN_CASE(nh) case nh: kern = e->local ? gcn::gcn_wgmma_kernel<true, nh> : gcn::gcn_wgmma_kernel<false, nh>; break;
+#define GGNN_GCN_CASE(nh)                                                                                                    \
+    case nh:                                                                                                                 \
+        kern = e->local ? (p.nparts == 3 ? gcn::gcn_wgmma_kernel<true, nh, true> : gcn::gcn_wgmma_kernel<true, nh, false>)   \
+                        : (p.nparts == 3 ? gcn::gcn_wgmma_kernel<false, nh, true> : gcn::gcn_wgmma_kernel<false, nh, false>); \
+        break;
             GGNN_GCN_CASE(8) GGNN_GCN_CASE(16) GGNN_GCN_CASE(24) GGNN_GCN_CASE(32) GGNN_GCN_CASE(40) GGNN_GCN_CASE(48) GGNN_GCN_CASE(56) GGNN_GCN_CASE(64)
 #undef GGNN_GCN_CASE
             default: return e->fail(GGNN_EUNSUPPORTED, "no GCN tensor-core kernel for DP=%d", DP);
@@ -2136,7 +2149,7 @@ static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream
         CU_TRY(e, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         for (int l = 0; l < (e->local ? 1 : L); ++l) {
             p.g_layer = l;
-            kern<<<e->ntiles, tc::NTHREADS, smem, st>>>(p);
+            kern<<<e->ntiles, gcn::NTHREADS, smem, st>>>(p);
             ++e->last_launches;
         }
     } else {

@@ -10,7 +10,8 @@
 // product is issued as 3 MMAs  Ah.Bh + Ah.Bl + Al.Bh  (the dropped Al.Bl term is 2^-16 relative); "fast" mode
 // issues Ah.Bh only.
 //
-// Warp roles: warps 0-15 = four worker warpgroups, warp 16 = weight producer.  Worker warpgroup w owns rows 64*(w%2) .. +64 and
+// Warp roles: warps 0-15 = four worker warpgroups, warp 16 = weight producer (on compact tiles warps 16-19, a warpgroup whose registers
+// go to the workers: NTHREADS).  Worker warpgroup w owns rows 64*(w%2) .. +64 and
 // columns NH*(w/2) .. +NH (NH = DP/2) of every GEMM output -- for the gate GEMM those columns of r AND of u -- so that the node state,
 // the gates, the candidate and their epilogues line up element for element in each thread's wgmma accumulator fragment, and the fp32
 // master copy of the node states stays in registers for the whole launch (LOCAL mode: the recurrence never leaves the SM).  On compact
@@ -34,7 +35,15 @@ namespace tc {
 constexpr int TILE_M = 128;
 constexpr int NUM_WORKERS = 512;          // 16 worker warps = 4 warpgroups
 constexpr int WARP_PROD = NUM_WORKERS / 32;
-constexpr int NTHREADS = NUM_WORKERS + 32;
+// Threads of ggnn_fwd_tc_kernel.  128-row tiles: the workers + one producer warp (17 warps, 96 registers per thread: 5 warps on one SM
+// sub-partition).  Compact tiles: the workers + a producer warpgroup (20 warps, also 96 at launch) that hands all but PRODUCER_REGS of
+// its registers to the workers (setmaxnreg): 512 * 112 + 128 * 32 = 640 * 96.  The 128-row instances, whose accumulator fragments are
+// twice as wide, do not keep a wgmma pipeline even at 112 registers; they issue one weight slot at a time (gemm_narrow_serial).
+template <bool COMPACT>
+constexpr int NTHREADS = NUM_WORKERS + (COMPACT ? 128 : 32);
+constexpr int WORKER_REGS = 112;
+constexpr int PRODUCER_REGS = 32;
+static_assert(NUM_WORKERS * WORKER_REGS + (NTHREADS<true> - NUM_WORKERS) * PRODUCER_REGS <= NTHREADS<true> * 96, "register file");
 constexpr int MAX_STAGES = 10;            // ring slots; a slot holds TWO K-step stages (2 x 64*DP bytes, one bulk copy)
 
 struct TcLayer {
@@ -99,7 +108,7 @@ __device__ __forceinline__ bool mbar_try(uint32_t addr, uint32_t parity) {
                  : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
     return ok != 0;
 }
-__device__ __noinline__ bool mbar_wait_slow(uint32_t addr, uint32_t parity, volatile int* abort_flag) {
+__device__ __forceinline__ bool mbar_spin(uint32_t addr, uint32_t parity, volatile int* abort_flag) {
     const long long t0 = clock64();
     for (unsigned it = 1;; ++it) {
         uint32_t ok;
@@ -113,10 +122,18 @@ __device__ __noinline__ bool mbar_wait_slow(uint32_t addr, uint32_t parity, vola
         }
     }
 }
+__device__ __noinline__ bool mbar_wait_slow(uint32_t addr, uint32_t parity, volatile int* abort_flag) { return mbar_spin(addr, parity, abort_flag); }
 __device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, volatile int* abort_flag) {
     const uint32_t addr = smem_u32(bar);
     if (mbar_try(addr, parity)) return true;
     return mbar_wait_slow(addr, parity, abort_flag);
+}
+// The same wait without a function call, for the weight ring of the tile kernels: a call inside a setmaxnreg region (the compact tile
+// kernel's workers) fails register allocation.
+__device__ __forceinline__ bool mbar_wait_inline(uint64_t* bar, uint32_t parity, volatile int* abort_flag) {
+    const uint32_t addr = smem_u32(bar);
+    if (mbar_try(addr, parity)) return true;
+    return mbar_spin(addr, parity, abort_flag);
 }
 __device__ __forceinline__ void bulk_copy_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -124,6 +141,11 @@ __device__ __forceinline__ void bulk_copy_g2s(void* dst_smem, const void* src_gm
 }
 // generic-proxy shared-memory writes (operand tiles) -> visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// per-thread register budget of the executing warpgroup from here on (every thread of the warpgroup executes it)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // x = hi + lo with hi, lo bf16 (round to nearest): 16 mantissa bits kept
 __device__ __forceinline__ void split8(const float (&x)[8], uint4& hi, uint4& lo) {
@@ -233,7 +255,7 @@ struct RingReader {
     __device__ __forceinline__ uint32_t take() {
         const uint32_t sl = slot;
         slot = (slot + 1 == nslots) ? 0u : slot + 1;
-        if (!*abortp && !mbar_wait(&full[sl], (fpar >> sl) & 1u, abortp)) *abortp = 1;
+        if (!*abortp && !mbar_wait_inline(&full[sl], (fpar >> sl) & 1u, abortp)) *abortp = 1;
         fpar ^= 1u << sl;
         return sl;
     }
@@ -257,7 +279,7 @@ struct RingWriter {
             const uint32_t sl = cur;
             cur = (cur + 1 == nslots) ? 0u : cur + 1;
             if ((used >> sl) & 1u) {
-                if (!mbar_wait(&empty[sl], (epar >> sl) & 1u, abortp)) { ok = false; break; }
+                if (!mbar_wait_inline(&empty[sl], (epar >> sl) & 1u, abortp)) { ok = false; break; }
                 epar ^= 1u << sl;
             }
             used |= 1u << sl;
@@ -267,27 +289,78 @@ struct RingWriter {
     }
 };
 
+// After the MMAs of slot i are committed: keep them in flight and release slot i-1 (`prev`) once wgmma.wait_group 1 says its group has
+// retired.  A worker warp holds two slots at a time, so the ring has at least two (forward_tc).  `first` is a constant after unrolling:
+// a wait_group on a path ptxas cannot resolve makes it serialise every MMA.
+__device__ __forceinline__ void retire_slot(RingReader& ring, uint32_t sl, uint32_t& prev, bool first, int lane) {
+    if (!first) {
+        wg::wait<1>();
+        ring.release(prev, lane);
+    }
+    prev = sl;
+}
+// the end of a GEMM: every MMA complete (the caller reads the accumulators next, or rewrites an operand tile), the last slot released
+__device__ __forceinline__ void retire_last(RingReader& ring, uint32_t prev, int lane) {
+    wg::wait_all();
+    ring.release(prev, lane);
+}
+
 // acc += A(op) . B(one DP x DP weight block: ceil(NKS/2) slots of two K-steps, each stage = [hi | lo]) for one worker warpgroup: A rows from
-// byte a_row on (k-group stride KGS, lo part PART_B after hi), B columns col0 .. +NH.  x3: three MMAs per product.  A warpgroup without rows
-// (mma_rows false) skips the MMAs but still takes and releases every slot.
-template <int NH>
-__device__ __forceinline__ void gemm_narrow(RingReader& ring, float (&acc)[NH / 2], const uint8_t* op, int NKS, int DP, uint32_t KGS, uint32_t PART_B,
-                                            uint32_t STAGE_B, uint32_t a_row, int col0, bool mma_rows, bool x3, int lane) {
-    const int nslots = (NKS + 1) / 2;
-    for (int i = 0; i < nslots; ++i) {
+// byte a_row on (k-group stride KGS, lo part DP*KGS/8 after hi), B columns col0 .. +WN.  X3: three MMAs per product.  Every trip count is a
+// template constant (an odd NKS ends in a slot of one K-step), so the MMAs of a slot are straight-line code that ptxas does not serialise.
+// Every warpgroup issues its MMAs, also on operand rows that the tile does not have: the operand tiles hold zeros there and the epilogues
+// never store those rows.
+template <int WN, int DP, bool X3, uint32_t KGS>
+__device__ __forceinline__ void gemm_narrow(RingReader& ring, float (&acc)[WN / 2], uint32_t op, uint32_t a_row, int col0, int lane) {
+    constexpr int NKS = DP / 16, NSLOTS = (NKS + 1) / 2;
+    constexpr uint32_t STAGE_B = DP * 64u, PART_B = DP * KGS / 8u;
+    uint32_t prev = 0;
+#pragma unroll
+    for (int i = 0; i < NSLOTS; ++i) {
+        const uint32_t sl = ring.take();
+        const uint32_t b0 = ring.base + sl * 2u * STAGE_B + (uint32_t)col0 * 16u;
+        wg::fence();
+#pragma unroll
+        for (int h = 0; h < ((2 * i + 1 < NKS) ? 2 : 1); ++h) {
+            const uint32_t a = op + (uint32_t)(2 * i + h) * 2u * KGS + a_row;
+            const uint32_t b = b0 + (uint32_t)h * STAGE_B;
+            const uint64_t ad = wg::make_desc(a, KGS, 128), bd = wg::make_desc(b, 16u * DP, 128);
+            wg::Mma<WN>::run(acc, ad, bd);
+            if (X3) {
+                wg::Mma<WN>::run(acc, ad, wg::make_desc(b + 32u * DP, 16u * DP, 128));
+                wg::Mma<WN>::run(acc, wg::make_desc(a + PART_B, KGS, 128), bd);
+            }
+        }
+        wg::commit();
+        retire_slot(ring, sl, prev, i == 0, lane);
+    }
+    retire_last(ring, prev, lane);
+}
+
+// The same product one slot at a time (commit, wait for every group, release), for the 128-row layout of ggnn_fwd_tc_kernel: its
+// accumulator fragments are twice as wide as the compact ones, ptxas cannot keep a wgmma pipeline under the 96-register cap of 17 warps,
+// and an unrolled pipelined body only lengthens live ranges and spills.  A warpgroup without rows (mma_rows false) skips the MMAs but
+// still takes and releases every slot.
+template <int WN, int DP, bool X3, uint32_t KGS>
+__device__ __forceinline__ void gemm_narrow_serial(RingReader& ring, float (&acc)[WN / 2], uint32_t op, uint32_t a_row, int col0, bool mma_rows,
+                                                   int lane) {
+    constexpr int NKS = DP / 16, NSLOTS = (NKS + 1) / 2;
+    constexpr uint32_t STAGE_B = DP * 64u, PART_B = DP * KGS / 8u;
+#pragma unroll 1
+    for (int i = 0; i < NSLOTS; ++i) {
         const uint32_t sl = ring.take();
         if (mma_rows) {
             const uint32_t b0 = ring.base + sl * 2u * STAGE_B + (uint32_t)col0 * 16u;
             const int nk = (2 * i + 1 < NKS) ? 2 : 1;
             wg::fence();
             for (int h = 0; h < nk; ++h) {
-                const uint32_t a = smem_u32(op) + (uint32_t)(2 * i + h) * 2u * KGS + a_row;
+                const uint32_t a = op + (uint32_t)(2 * i + h) * 2u * KGS + a_row;
                 const uint32_t b = b0 + (uint32_t)h * STAGE_B;
                 const uint64_t ad = wg::make_desc(a, KGS, 128), bd = wg::make_desc(b, 16u * DP, 128);
-                wg::Mma<NH>::run(acc, ad, bd);
-                if (x3) {
-                    wg::Mma<NH>::run(acc, ad, wg::make_desc(b + 32u * DP, 16u * DP, 128));
-                    wg::Mma<NH>::run(acc, wg::make_desc(a + PART_B, KGS, 128), bd);
+                wg::Mma<WN>::run(acc, ad, bd);
+                if (X3) {
+                    wg::Mma<WN>::run(acc, ad, wg::make_desc(b + 32u * DP, 16u * DP, 128));
+                    wg::Mma<WN>::run(acc, wg::make_desc(a + PART_B, KGS, 128), bd);
                 }
             }
             wg::commit();
@@ -306,9 +379,10 @@ template <int NH>
 constexpr int COMPACT_WIDTH = (NH / 2) % 8 == 0 ? NH / 2 : NH / 2 + 4;
 
 // COMPACT: every tile has <= 64 rows (k-group stride 1024) and the four warpgroups split the columns (COMPACT_WIDTH); otherwise
-// warpgroup w owns MMA rows 64*(w%2) .. +64 and columns NH*(w/2) .. +NH.
-template <bool LOCAL, int NH, bool COMPACT>
-__global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_constant__ TcParams p) {
+// warpgroup w owns MMA rows 64*(w%2) .. +64 and columns NH*(w/2) .. +NH.  X3: bf16x3 (p.nparts == 3), else one bf16 MMA per product.
+// DP = 2*NH and the k-group stride are template constants too, so that every MMA path is straight-line code.
+template <bool LOCAL, int NH, bool COMPACT, bool X3>
+__global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const __grid_constant__ TcParams p) {
     constexpr int WN = COMPACT ? COMPACT_WIDTH<NH> : NH;   // the columns of one warpgroup (wgmma N, an instruction immediate)
     constexpr int NF = WN / 2;   // accumulator floats per thread and quantity (m64 x WN fragment)
     constexpr int NJ = WN / 8;   // 8-column blocks of a fragment
@@ -317,13 +391,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
     __shared__ __align__(8) uint64_t bar_empty[MAX_STAGES];   // every worker warp is done with the slot
     __shared__ int s_abort;
 
-    const int D = p.D, DP = p.DP, T = p.T;
-    const int NKC = DP >> 3;   // 8-column chunks per DP
-    const int NKS = DP >> 4;   // K-steps (16) per DP-wide operand
-    const uint32_t KGS = COMPACT ? 1024u : (uint32_t)p.kgs;
-    const uint32_t PART_B = (uint32_t)DP * KGS / 8u;   // bytes per part (hi or lo)
-    const uint32_t OPB = 2u * PART_B;                  // bytes per A operand (hi + lo)
-    const uint32_t STAGE_B = (uint32_t)DP * 64u;       // bytes per weight stage (K = 16 x N = DP, hi + lo)
+    constexpr int DP = 2 * NH;
+    constexpr int NKC = DP >> 3;   // 8-column chunks per DP
+    constexpr int NKS = DP >> 4;   // K-steps (16) per DP-wide operand
+    constexpr uint32_t KGS = COMPACT ? 1024u : 2048u;   // (p.kgs)
+    constexpr uint32_t PART_B = (uint32_t)DP * KGS / 8u;   // bytes per part (hi or lo)
+    constexpr uint32_t OPB = 2u * PART_B;                  // bytes per A operand (hi + lo)
+    constexpr uint32_t STAGE_B = (uint32_t)DP * 64u;       // bytes per weight stage (K = 16 x N = DP, hi + lo)
+    const int D = p.D, T = p.T;
     uint8_t* opH = smem;
     uint8_t* opX = opH + OPB;
     uint8_t* opA = opX + OPB;
@@ -352,6 +427,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
 
     if (warp < WARP_PROD) {
         // =============================================================================== WORKERS
+        if (COMPACT) setmaxnreg_inc<WORKER_REGS>();
         // ---- row-per-thread view (gathers): row q*32 + lane, column-chunk group cg
         const int q = warp & 3, cg = warp >> 2;
         const int nkc_tile = NKC;
@@ -364,39 +440,55 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
         const int col0 = COMPACT ? min(own0, DP - WN) : own0;
         const int fr0 = m0 + (warp & 3) * 16 + (lane >> 2);         // fragment rows fr0, fr0 + 8
         const int fc0 = col0 + (lane & 3) * 2;                      // fragment columns fc0 + 8j, fc0 + 8j + 1
-        const bool mma_rows = m0 < rows;                            // warpgroup-uniform: the warpgroup has rows at all
-        const bool x3 = p.nparts == 3;
         bool ok = true;
         auto workers_sync = [&]() { tc::workers_sync(abortp, ok); };
         auto publish_sync = [&]() { fence_async_smem(); workers_sync(); };   // operand tiles written -> visible to wgmma
         RingReader rd{bar_full, bar_empty, abortp, smem_u32(ring), (uint32_t)nst};
         const uint32_t a_row = (uint32_t)m0 * 16u;   // this warpgroup's first row inside an A operand
+        const bool mma_rows = m0 < rows;             // warpgroup-uniform: the warpgroup has rows at all (always, on compact tiles)
+        // Compact tiles pipeline the MMAs (gemm_narrow); 128-row tiles issue one slot at a time (gemm_narrow_serial).
         auto gemm_narrow = [&](float (&acc)[NF], const uint8_t* op) {
-            tc::gemm_narrow<WN>(rd, acc, op, NKS, DP, KGS, PART_B, STAGE_B, a_row, col0, mma_rows, x3, lane);
+            if constexpr (COMPACT) tc::gemm_narrow<WN, DP, X3, KGS>(rd, acc, smem_u32(op), a_row, col0, lane);
+            else tc::gemm_narrow_serial<WN, DP, X3, KGS>(rd, acc, smem_u32(op), a_row, col0, mma_rows, lane);
         };
-        // [r | u] += A(op) . B(one segment of the N = 2*DP gate block: NKS slots, stage 0 = hi, stage 1 = lo); columns of r and of u
+        // [r | u] += A(op) . B(one segment of the N = 2*DP gate block: NKS slots, stage 0 = hi, stage 1 = lo); columns of r and of u.
+        // One K-step per slot; slot i's MMAs stay in flight while slot i+1's are issued (compact), or one slot at a time (128-row).
+        auto wide_mmas = [&](float (&ar)[NF], float (&au)[NF], uint32_t sl, uint32_t a) {
+            const uint32_t bh = rd.base + sl * 2u * STAGE_B, bl = bh + STAGE_B;
+            const uint32_t cr = (uint32_t)col0 * 16u, cu = (uint32_t)(DP + col0) * 16u, lbo = 32u * DP;
+            const uint64_t ad = wg::make_desc(a, KGS, 128);
+            wg::fence();
+            wg::Mma<WN>::run(ar, ad, wg::make_desc(bh + cr, lbo, 128));
+            wg::Mma<WN>::run(au, ad, wg::make_desc(bh + cu, lbo, 128));
+            if (X3) {
+                const uint64_t al = wg::make_desc(a + PART_B, KGS, 128);
+                wg::Mma<WN>::run(ar, ad, wg::make_desc(bl + cr, lbo, 128));
+                wg::Mma<WN>::run(au, ad, wg::make_desc(bl + cu, lbo, 128));
+                wg::Mma<WN>::run(ar, al, wg::make_desc(bh + cr, lbo, 128));
+                wg::Mma<WN>::run(au, al, wg::make_desc(bh + cu, lbo, 128));
+            }
+            wg::commit();
+        };
         auto gemm_wide = [&](float (&ar)[NF], float (&au)[NF], const uint8_t* op) {
-            for (int i = 0; i < NKS; ++i) {
-                const uint32_t sl = rd.take();
-                if (mma_rows) {
-                    const uint32_t bh = rd.base + sl * 2u * STAGE_B, bl = bh + STAGE_B;
-                    const uint32_t cr = (uint32_t)col0 * 16u, cu = (uint32_t)(DP + col0) * 16u, lbo = 32u * DP;
-                    const uint32_t a = smem_u32(op) + (uint32_t)i * 2u * KGS + a_row;
-                    const uint64_t ad = wg::make_desc(a, KGS, 128);
-                    wg::fence();
-                    wg::Mma<WN>::run(ar, ad, wg::make_desc(bh + cr, lbo, 128));
-                    wg::Mma<WN>::run(au, ad, wg::make_desc(bh + cu, lbo, 128));
-                    if (x3) {
-                        const uint64_t al = wg::make_desc(a + PART_B, KGS, 128);
-                        wg::Mma<WN>::run(ar, ad, wg::make_desc(bl + cr, lbo, 128));
-                        wg::Mma<WN>::run(au, ad, wg::make_desc(bl + cu, lbo, 128));
-                        wg::Mma<WN>::run(ar, al, wg::make_desc(bh + cr, lbo, 128));
-                        wg::Mma<WN>::run(au, al, wg::make_desc(bh + cu, lbo, 128));
-                    }
-                    wg::commit();
-                    wg::wait_all();
+            if constexpr (COMPACT) {
+                uint32_t prev = 0;
+#pragma unroll
+                for (int i = 0; i < NKS; ++i) {
+                    const uint32_t sl = rd.take();
+                    wide_mmas(ar, au, sl, smem_u32(op) + (uint32_t)i * 2u * KGS + a_row);
+                    retire_slot(rd, sl, prev, i == 0, lane);
                 }
-                rd.release(sl, lane);
+                retire_last(rd, prev, lane);
+            } else {
+#pragma unroll 1
+                for (int i = 0; i < NKS; ++i) {
+                    const uint32_t sl = rd.take();
+                    if (mma_rows) {
+                        wide_mmas(ar, au, sl, smem_u32(op) + (uint32_t)i * 2u * KGS + a_row);
+                        wg::wait_all();
+                    }
+                    rd.release(sl, lane);
+                }
             }
         };
         auto zero = [](float (&a)[NF]) {
@@ -509,7 +601,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
                             const uint8_t* colbase = opH + (size_t)kc * KGS;
                             const uint32_t lo_off = PART_B;
                             int m = beg;
-                            if (p.nparts == 3) {
+                            if (X3) {
                                 for (; m + 1 < end; m += 2) {
                                     const uint8_t* s0 = colbase + (size_t)sSrc[m] * 16;
                                     const uint8_t* s1 = colbase + (size_t)sSrc[m + 1] * 16;
@@ -532,7 +624,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
                                     const int sl = csr_smem ? (int)sSrc[m] : (p.csr_src[m] - row0);
                                     const uint8_t* sp = opH + (size_t)kc * KGS + (size_t)sl * 16;
                                     unpack8_add(*reinterpret_cast<const uint4*>(sp), a8, 1.0f);
-                                    if (p.nparts == 3) unpack8_add(*reinterpret_cast<const uint4*>(sp + PART_B), a8, 1.0f);
+                                    if (X3) unpack8_add(*reinterpret_cast<const uint4*>(sp + PART_B), a8, 1.0f);
                                 } else {
                                     // GLOBAL mode: source rows come from the previous step's fp32 state in L2; keep 4 rows in flight
                                     float hv[4][8];
@@ -559,7 +651,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
                                     if (LOCAL) {
                                         const uint8_t* sp = opH + (size_t)kc * KGS + (size_t)(src - row0) * 16;
                                         unpack8_add(*reinterpret_cast<const uint4*>(sp), a8, a);
-                                        if (p.nparts == 3) unpack8_add(*reinterpret_cast<const uint4*>(sp + PART_B), a8, a);
+                                        if (X3) unpack8_add(*reinterpret_cast<const uint4*>(sp + PART_B), a8, a);
                                     } else {
                                         float hv[8];
                                         load8_guarded_cg(p.g_in + (size_t)src * D, kc * 8, D, hv);
@@ -596,65 +688,119 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
                 publish_sync();
                 if (!ok) break;
                 float* outp = LOCAL ? ((s == ly.steps - 1) ? p.state_w[l + 1] : nullptr) : p.g_out;
-                if (gru) {
-                    // -------------------------------------------------------- gates: r*h -> opA, u stays in registers
-                    float gr[NF], gu[NF];
-                    zero(gr); zero(gu);
-                    gemm_wide(gr, gu, opX);
-                    gemm_wide(gr, gu, opH);
-                    GGNN_FRAG_PAIRS({
-                        float br0 = sBias[fc], br1 = sBias[fc + 1], bu0 = sBias[DP + fc], bu1 = sBias[DP + fc + 1];
-                        if (ly.nres > 0) {
-                            const float* rp = res_pre + (size_t)fr * 3 * DP + fc;
-                            br0 += rp[0]; br1 += rp[1]; bu0 += rp[DP]; bu1 += rp[DP + 1];
-                        }
-                        const float r0 = sigmoid_fast(gr[fi] + br0), r1 = sigmoid_fast(gr[fi + 1] + br1);
-                        gu[fi] = sigmoid_fast(gu[fi] + bu0); gu[fi + 1] = sigmoid_fast(gu[fi + 1] + bu1);
-                        if (p.save && fok) {
-                            const size_t o = save_base + (size_t)fg * D + fc;
-                            st2(p.save_buf.r + o, r0, r1);
-                            st2(p.save_buf.h_in + o, hs[fi], hs[fi + 1]);
-                            st2(p.save_buf.u + o, gu[fi], gu[fi + 1]);
-                        }
-                        store_operand_pair(opA, KGS, PART_B, fr, fc, r0 * hs[fi], r1 * hs[fi + 1]);
-                    })
-                    publish_sync();
-                    if (!ok) break;
-                    // -------------------------------------------------------- candidate, new state
+                if constexpr (COMPACT) {
+                    // one candidate GEMM for both cells: a second copy under a runtime branch keeps ptxas from pipelining the MMAs
+                    float gu[NF];   // GRU: the update gate u
+                    if (gru) {
+                        // -------------------------------------------------------- gates: r*h -> opA, u stays in registers
+                        float gr[NF];
+                        zero(gr); zero(gu);
+                        gemm_wide(gr, gu, opX);
+                        gemm_wide(gr, gu, opH);
+                        GGNN_FRAG_PAIRS({
+                            float br0 = sBias[fc], br1 = sBias[fc + 1], bu0 = sBias[DP + fc], bu1 = sBias[DP + fc + 1];
+                            if (ly.nres > 0) {
+                                const float* rp = res_pre + (size_t)fr * 3 * DP + fc;
+                                br0 += rp[0]; br1 += rp[1]; bu0 += rp[DP]; bu1 += rp[DP + 1];
+                            }
+                            const float r0 = sigmoid_fast(gr[fi] + br0), r1 = sigmoid_fast(gr[fi + 1] + br1);
+                            gu[fi] = sigmoid_fast(gu[fi] + bu0); gu[fi + 1] = sigmoid_fast(gu[fi + 1] + bu1);
+                            if (p.save && fok) {
+                                const size_t o = save_base + (size_t)fg * D + fc;
+                                st2(p.save_buf.r + o, r0, r1);
+                                st2(p.save_buf.h_in + o, hs[fi], hs[fi + 1]);
+                                st2(p.save_buf.u + o, gu[fi], gu[fi + 1]);
+                            }
+                            store_operand_pair(opA, KGS, PART_B, fr, fc, r0 * hs[fi], r1 * hs[fi + 1]);
+                        })
+                        publish_sync();
+                        if (!ok) break;
+                    }
+                    // ------------------------------------------------------------ candidate [agg | r*h] . K_c (GRU), [agg | h] . K_c (RNN); new state
                     float gc[NF];
                     zero(gc);
                     gemm_narrow(gc, opX);
-                    gemm_narrow(gc, opA);
+                    gemm_narrow(gc, gru ? opA : opH);
                     GGNN_FRAG_PAIRS({
                         float bc0 = sBias[2 * DP + fc], bc1 = sBias[2 * DP + fc + 1];
                         if (ly.nres > 0) {
                             const float* rp = res_pre + (size_t)fr * 3 * DP + 2 * DP + fc;
                             bc0 += rp[0]; bc1 += rp[1];
                         }
-                        const float c0 = act_fast(gc[fi] + bc0, p.act), c1 = act_fast(gc[fi + 1] + bc1, p.act);
-                        if (p.save && fok) st2(p.save_buf.c + save_base + (size_t)fg * D + fc, c0, c1);
-                        gc[fi] = fmaf(gu[fi], hs[fi] - c0, c0);            // u*h + (1-u)*c
-                        gc[fi + 1] = fmaf(gu[fi + 1], hs[fi + 1] - c1, c1);
+                        if (gru) {
+                            const float c0 = act_fast(gc[fi] + bc0, p.act), c1 = act_fast(gc[fi + 1] + bc1, p.act);
+                            if (p.save && fok) st2(p.save_buf.c + save_base + (size_t)fg * D + fc, c0, c1);
+                            gc[fi] = fmaf(gu[fi], hs[fi] - c0, c0);            // u*h + (1-u)*c
+                            gc[fi + 1] = fmaf(gu[fi + 1], hs[fi + 1] - c1, c1);
+                        } else {
+                            if (p.save && fok) st2(p.save_buf.h_in + save_base + (size_t)fg * D + fc, hs[fi], hs[fi + 1]);
+                            gc[fi] = act_fast(gc[fi] + bc0, p.act);
+                            gc[fi + 1] = act_fast(gc[fi + 1] + bc1, p.act);
+                        }
                     })
 #pragma unroll
                     for (int i = 0; i < NF; ++i) hs[i] = gc[i];
                 } else {
-                    float gc[NF];
-                    zero(gc);
-                    gemm_narrow(gc, opX);
-                    gemm_narrow(gc, opH);
-                    GGNN_FRAG_PAIRS({
-                        float bc0 = sBias[2 * DP + fc], bc1 = sBias[2 * DP + fc + 1];
-                        if (ly.nres > 0) {
-                            const float* rp = res_pre + (size_t)fr * 3 * DP + 2 * DP + fc;
-                            bc0 += rp[0]; bc1 += rp[1];
-                        }
-                        if (p.save && fok) st2(p.save_buf.h_in + save_base + (size_t)fg * D + fc, hs[fi], hs[fi + 1]);
-                        gc[fi] = act_fast(gc[fi] + bc0, p.act);
-                        gc[fi + 1] = act_fast(gc[fi + 1] + bc1, p.act);
-                    })
+                    if (gru) {
+                        // -------------------------------------------------------- gates: r*h -> opA, u stays in registers
+                        float gr[NF], gu[NF];
+                        zero(gr); zero(gu);
+                        gemm_wide(gr, gu, opX);
+                        gemm_wide(gr, gu, opH);
+                        GGNN_FRAG_PAIRS({
+                            float br0 = sBias[fc], br1 = sBias[fc + 1], bu0 = sBias[DP + fc], bu1 = sBias[DP + fc + 1];
+                            if (ly.nres > 0) {
+                                const float* rp = res_pre + (size_t)fr * 3 * DP + fc;
+                                br0 += rp[0]; br1 += rp[1]; bu0 += rp[DP]; bu1 += rp[DP + 1];
+                            }
+                            const float r0 = sigmoid_fast(gr[fi] + br0), r1 = sigmoid_fast(gr[fi + 1] + br1);
+                            gu[fi] = sigmoid_fast(gu[fi] + bu0); gu[fi + 1] = sigmoid_fast(gu[fi + 1] + bu1);
+                            if (p.save && fok) {
+                                const size_t o = save_base + (size_t)fg * D + fc;
+                                st2(p.save_buf.r + o, r0, r1);
+                                st2(p.save_buf.h_in + o, hs[fi], hs[fi + 1]);
+                                st2(p.save_buf.u + o, gu[fi], gu[fi + 1]);
+                            }
+                            store_operand_pair(opA, KGS, PART_B, fr, fc, r0 * hs[fi], r1 * hs[fi + 1]);
+                        })
+                        publish_sync();
+                        if (!ok) break;
+                        // -------------------------------------------------------- candidate, new state
+                        float gc[NF];
+                        zero(gc);
+                        gemm_narrow(gc, opX);
+                        gemm_narrow(gc, opA);
+                        GGNN_FRAG_PAIRS({
+                            float bc0 = sBias[2 * DP + fc], bc1 = sBias[2 * DP + fc + 1];
+                            if (ly.nres > 0) {
+                                const float* rp = res_pre + (size_t)fr * 3 * DP + 2 * DP + fc;
+                                bc0 += rp[0]; bc1 += rp[1];
+                            }
+                            const float c0 = act_fast(gc[fi] + bc0, p.act), c1 = act_fast(gc[fi + 1] + bc1, p.act);
+                            if (p.save && fok) st2(p.save_buf.c + save_base + (size_t)fg * D + fc, c0, c1);
+                            gc[fi] = fmaf(gu[fi], hs[fi] - c0, c0);            // u*h + (1-u)*c
+                            gc[fi + 1] = fmaf(gu[fi + 1], hs[fi + 1] - c1, c1);
+                        })
 #pragma unroll
-                    for (int i = 0; i < NF; ++i) hs[i] = gc[i];
+                        for (int i = 0; i < NF; ++i) hs[i] = gc[i];
+                    } else {
+                        float gc[NF];
+                        zero(gc);
+                        gemm_narrow(gc, opX);
+                        gemm_narrow(gc, opH);
+                        GGNN_FRAG_PAIRS({
+                            float bc0 = sBias[2 * DP + fc], bc1 = sBias[2 * DP + fc + 1];
+                            if (ly.nres > 0) {
+                                const float* rp = res_pre + (size_t)fr * 3 * DP + 2 * DP + fc;
+                                bc0 += rp[0]; bc1 += rp[1];
+                            }
+                            if (p.save && fok) st2(p.save_buf.h_in + save_base + (size_t)fg * D + fc, hs[fi], hs[fi + 1]);
+                            gc[fi] = act_fast(gc[fi] + bc0, p.act);
+                            gc[fi + 1] = act_fast(gc[fi + 1] + bc1, p.act);
+                        })
+#pragma unroll
+                        for (int i = 0; i < NF; ++i) hs[i] = gc[i];
+                    }
                 }
                 workers_sync();   // every MMA that reads opH is complete before the state update rewrites it
                 if (!ok) break;
@@ -677,7 +823,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_fwd_tc_kernel(const __grid_c
         }  // layers
 #undef GGNN_FRAG_PAIRS
         if (!ok && tid == 0) atomicExch(p.error_flag, 1);
-    } else if (lane == 0) {
+    } else if (COMPACT) {
+        setmaxnreg_dec<PRODUCER_REGS>();
+    }
+    if (warp == WARP_PROD && lane == 0) {
         // =============================================================================== WEIGHT PRODUCER
         // the weights of every layer and step, in the order the workers' GEMMs consume them
         RingWriter wr{bar_full, bar_empty, abortp, ring, (uint32_t)nst, STAGE_B};

@@ -22,6 +22,7 @@
 namespace ggnn {
 namespace gcn {
 
+constexpr int NTHREADS = tc::NUM_WORKERS + 32;   // the tile kernels' four worker warpgroups + one producer warp (no spills at 96 registers)
 constexpr int MAX_STAGES = 8;
 constexpr int KGS = 2048;              // A-operand k-group stride: 128 rows x 16 bytes
 constexpr int F32_ROWS = 32;           // rows per CTA of the fp32 kernel
@@ -58,8 +59,9 @@ __device__ __forceinline__ float epilogue(float v, const GcnParams& p, int l, in
 }
 
 // ------------------------------------------------------------------------------------------------ tensor cores
-template <bool LOCAL, int NH>
-__global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid_constant__ GcnParams p) {
+// X3: bf16x3 (p.nparts == 3), else one bf16 MMA per product; DP = 2*NH
+template <bool LOCAL, int NH, bool X3>
+__global__ void __launch_bounds__(NTHREADS, 1) gcn_wgmma_kernel(const __grid_constant__ GcnParams p) {
     using namespace tc;
     constexpr int NF = NH / 2;   // accumulator floats per thread (m64 x NH fragment)
     constexpr int NJ = NH / 8;   // 8-column blocks of a fragment
@@ -68,11 +70,12 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid
     __shared__ __align__(8) uint64_t bar_empty[MAX_STAGES];
     __shared__ int s_abort;
 
-    const int D = p.D, DP = p.DP;
-    const int NKC = DP >> 3, NKS = DP >> 4;
-    const uint32_t PART_B = (uint32_t)DP * KGS / 8u;
-    const uint32_t OPB = 2u * PART_B;
-    const uint32_t STAGE_B = (uint32_t)DP * 64u;
+    constexpr int DP = 2 * NH;
+    constexpr int NKC = DP >> 3, NKS = DP >> 4;
+    constexpr uint32_t PART_B = (uint32_t)DP * KGS / 8u;
+    constexpr uint32_t OPB = 2u * PART_B;
+    constexpr uint32_t STAGE_B = (uint32_t)DP * 64u;
+    const int D = p.D;
     uint8_t* opS = smem;
     uint8_t* ring = opS + OPB;
     float* sH = reinterpret_cast<float*>(ring + (size_t)p.nstages * 2 * STAGE_B);   // LOCAL: [128][DP] fp32 node states of the tile
@@ -97,8 +100,6 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid
         const int wgi = warp >> 2, mh = wgi & 1, nh = wgi >> 1;   // fragment view
         const int fr0 = mh * 64 + (warp & 3) * 16 + (lane >> 2);
         const int fc0 = nh * NH + (lane & 3) * 2;
-        const bool mma_rows = mh * 64 < rows;
-        const bool x3 = p.nparts == 3;
         bool ok = true;
         RingReader rd{bar_full, bar_empty, abortp, smem_u32(ring), (uint32_t)nst};
         const uint32_t a_row = (uint32_t)mh * 64u * 16u;
@@ -140,7 +141,7 @@ __global__ void __launch_bounds__(tc::NTHREADS, 1) gcn_wgmma_kernel(const __grid
             float acc[NF];
 #pragma unroll
             for (int i = 0; i < NF; ++i) acc[i] = 0.f;
-            gemm_narrow<NH>(rd, acc, opS, NKS, DP, KGS, PART_B, STAGE_B, a_row, nh * NH, mma_rows, x3, lane);
+            gemm_narrow<NH, DP, X3, (uint32_t)KGS>(rd, acc, smem_u32(opS), a_row, nh * NH, lane);
             // ---- epilogue: bias, relu, dropout; the state goes back to the tile (LOCAL) and to global memory
             const bool to_smem = LOCAL && l + 1 < l_end;
             const bool to_global = !LOCAL || l + 1 == l_end || p.save;
