@@ -141,6 +141,7 @@ struct ModelShape {
 // What build_plan and the image builders derive from one batch: the tile plan and the layout of the graph image.
 struct BatchPlan {
     int gather_mode = GATHER_SPARSE;
+    bool weighted = false;   // every message has a weight (GCN): the image carries the slot weights
     int V = 0, dense_v = 0;
     int64_t M = 0;
     int variant = 0;  // 0: RG=8,CS=1 (64-row tiles)   1: RG=4,CS=2 (32-row tiles)
@@ -161,8 +162,7 @@ struct BatchPlan {
     bool has_transpose = false;
     size_t off_tslot = 0;            // source-keyed CSR entry -> target-CSR slot (attention backward)
     size_t off_pair = 0, off_vptr = 0, off_vsrc = 0, off_tvp = 0, off_vinfo = 0;   // streaming plan: (target,type) -> source table, virtual rows (pairs with several messages)
-    size_t off_slotw = 0, off_tslotw = 0;   // GCN: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
-    int64_t edges_of_type[32] = {0};
+    size_t off_slotw = 0, off_tslotw = 0;   // weighted: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
 };
 
 // Typed device pointers into the uploaded graph image of the current batch, made once per upload by ggnn_set_graph_prepared.  An array
@@ -1072,8 +1072,11 @@ static bool host_team_is_fast(int team) {
 #endif
 
 // ---- the host half of ggnn_set_graph_sparse: validation, tile plan, stable target-sorted CSR, streaming tables -> g->image.
+// `weighted`: the batch has one weight per message, `w`, in the type-major message order (required when there are messages); the image
+// then carries them in target-CSR order and, with the source-keyed CSR, in source-CSR order.
 // Nothing here touches the device except the pinned allocation of the image and the wait for the previous upload out of it.
-static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* const* adj, const int32_t* num_edges, const float* indeg) {
+static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* const* adj, const int32_t* num_edges, const float* indeg,
+                              bool weighted, const float* w) {
     const ModelShape& shape = g->shape;
     BatchPlan& p = g->plan;
     g->valid = false;
@@ -1094,6 +1097,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
         M += num_edges[t];
     }
     if (M > 0x7fffffff || (int64_t)V * T + 1 > 0x7fffffff) return g->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
+    if (weighted && M > 0 && !w) return g->fail(GGNN_EINVAL, "null message weights");
 
     // ---- host threads.  Every pass below is split over `nth` threads by TARGET ranges (pass 1: equal node ranges; later passes: equal
     // tile ranges): each thread scans the whole edge list (sequential reads) and performs only the scattered writes of its own rows, in the
@@ -1195,6 +1199,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     int rc = build_plan(shape, V, GATHER_SPARSE, cuts, p, tile_start, g->err);
     if (rc) return rc;
     p.M = M;
+    p.weighted = weighted;
     const int ntiles = p.ntiles;
     lap("tile plan", t_lap);
     nth = std::max(1, std::min(nth, ntiles));
@@ -1249,12 +1254,11 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
         p.off_tvp = off;  off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
         p.off_vinfo = off; off = align_up(off + sizeof(int) * 8 * (size_t)std::max(nv, 1), 16);
     }
-    if (shape.model == MODEL_GCN) {   // per-slot adjacency weights, filled by build_gcn_image
+    if (p.weighted) {   // per-slot adjacency weights
         p.off_slotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16);
         if (p.has_transpose) { p.off_tslotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16); }
     }
     p.ts_nv = nv;
-    for (int t = 0; t < T; ++t) p.edges_of_type[t] = num_edges[t];
     CU_TRY(g, g->image.begin(off));
     g->bytes = off;
     char* base = g->image.ptr;
@@ -1358,6 +1362,10 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
             }
             if (k == nth - 1) tvp[ntiles] = vid;
         }
+        if (weighted) {   // the weights of this range's slots, in target-CSR order
+            float* slotw = (float*)(base + p.off_slotw);
+            for (int64_t m = part_msgs[k]; m < part_msgs[k + 1]; ++m) slotw[m] = w[csr_msg[m]];
+        }
         if (v1 > v0) memcpy(h_indeg + (size_t)v0 * T, indeg + (size_t)v0 * T, sizeof(float) * (size_t)(v1 - v0) * T);
         for (int v = v0; v < v1; ++v) {
             const float* row = indeg + (size_t)v * T;
@@ -1382,6 +1390,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
         for (size_t k = 0; k < (size_t)V * T; ++k) cnt[k] = trow[k];
         std::vector<int> slot_of_msg;
         int* tslot = shape.use_att ? (int*)(base + p.off_tslot) : nullptr;
+        float* tslotw = weighted ? (float*)(base + p.off_tslotw) : nullptr;
         if (tslot) {
             slot_of_msg.resize((size_t)std::max<int64_t>(M, 1));
             for (int64_t k = 0; k < M; ++k) slot_of_msg[csr_msg[k]] = (int)k;
@@ -1392,6 +1401,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
                 const int j = cnt[(size_t)adj[t][2 * i] * T + t]++;
                 ttgt[j] = adj[t][2 * i + 1];
                 if (tslot) tslot[j] = slot_of_msg[m];
+                if (tslotw) tslotw[j] = w[m];
             }
     }
     lap("denom+masks+extra", t_lap);
@@ -1458,7 +1468,7 @@ extern "C" {
 int ggnn_host_prepare_graph_sparse(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t V, const int32_t* const* adj,
                                    const int32_t* num_edges, const float* indeg, ggnn_prepared_graph** inout) {
     if (int rc = begin_prepare(inout, nullptr, cfg, num_sms, save_for_backward, __func__)) return rc;
-    return build_sparse_image(*inout, V, adj, num_edges, indeg);
+    return build_sparse_image(*inout, V, adj, num_edges, indeg, false, nullptr);
 }
 
 int ggnn_prepared_graph_info(const ggnn_prepared_graph* g, int32_t* num_nodes, int64_t* num_messages, int32_t* num_tiles, int64_t* image_bytes,
@@ -1498,7 +1508,7 @@ int ggnn_prepared_graph_image(const ggnn_prepared_graph* g, void* dst, int64_t c
 int ggnn_prepare_graph_sparse(const ggnn_engine* e, int32_t save_for_backward, int32_t V, const int32_t* const* adj, const int32_t* num_edges,
                               const float* indeg, ggnn_prepared_graph** inout) {
     if (int rc = begin_prepare<ggnn_config>(inout, e, nullptr, 0, save_for_backward, __func__)) return rc;
-    return build_sparse_image(*inout, V, adj, num_edges, indeg);
+    return build_sparse_image(*inout, V, adj, num_edges, indeg, false, nullptr);
 }
 
 int ggnn_set_graph_prepared(ggnn_engine* e, ggnn_prepared_graph* g, ggnn_stream_t stream) {
@@ -1630,7 +1640,6 @@ static int build_matrix_image(ggnn_prepared_graph* g, int32_t b, int32_t v, cons
     if (rc) return rc;
     p.dense_v = v;
     p.has_transpose = true;   // the dense adjacency is its own transpose source
-    for (int t = 0; t < T; ++t) p.edges_of_type[t] = 1;
     const int ntiles = p.ntiles;
     const size_t adj_elems = (size_t)b * T * v * v;
     size_t off = 0;
@@ -1704,7 +1713,7 @@ static int build_dense_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const
     std::vector<const int32_t*> ptrs(T);
     std::vector<int32_t> counts(T);
     for (int t = 0; t < T; ++t) { ptrs[t] = lists[t].data(); counts[t] = (int32_t)(lists[t].size() / 2); }
-    int rc = build_sparse_image(g, b * v, ptrs.data(), counts.data(), indeg.data());
+    int rc = build_sparse_image(g, b * v, ptrs.data(), counts.data(), indeg.data(), false, nullptr);
     if (rc) return rc;
     g->plan.dense_v = v;
     g->plan.plan_text += " [binary dense adjacency -> CSR]";
@@ -2025,7 +2034,7 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
 
 // ------------------------------------------------------------------------------------------ sparse GCN (chem_tensorflow_gcn.py:42-82)
 // Host half of a GCN batch: validate the int64 (row i = output, column j = input) list, feed it to the GGNN builder as one edge type
-// (source j -> target i, list order kept), then add the per-slot weights in target-CSR and source-CSR order.
+// (source j -> target i, list order kept) with the weights as per-message weights.
 static int build_gcn_image(ggnn_prepared_graph* g, int32_t V, int64_t nnz, const int64_t* list, const float* w) {
     g->valid = false;
     if (V < 0 || nnz < 0 || (nnz > 0 && (!list || !w))) return g->fail(GGNN_EINVAL, "null/negative argument");
@@ -2041,20 +2050,7 @@ static int build_gcn_image(ggnn_prepared_graph* g, int32_t V, int64_t nnz, const
     const std::vector<float> indeg((size_t)std::max(V, 1), 0.0f);
     const int32_t* lists[1] = {pairs.data()};
     const int32_t counts[1] = {(int32_t)nnz};
-    int rc = build_sparse_image(g, V, lists, counts, indeg.data());
-    if (rc) return rc;
-    const BatchPlan& p = g->plan;
-    char* base = g->image.ptr;
-    const int* csr_msg = (const int*)(base + p.off_msg);
-    float* tw = (float*)(base + p.off_slotw);
-    for (int64_t k = 0; k < nnz; ++k) tw[k] = w[csr_msg[k]];
-    if (p.has_transpose) {   // the source-keyed CSR lists the entries of every input column j in list order (build_sparse_image)
-        const int* trow = (const int*)(base + p.off_trow);
-        float* sw = (float*)(base + p.off_tslotw);
-        std::vector<int> cur(trow, trow + V);
-        for (int64_t k = 0; k < nnz; ++k) sw[cur[pairs[2 * k]]++] = w[k];
-    }
-    return GGNN_OK;
+    return build_sparse_image(g, V, lists, counts, indeg.data(), true, w);
 }
 
 int ggnn_gcn_create(const ggnn_gcn_config* cfg, ggnn_engine** out) {
@@ -2101,7 +2097,7 @@ int ggnn_set_graph_gcn(ggnn_engine* e, int32_t V, int64_t nnz, const int64_t* li
 }
 
 int ggnn_prepared_graph_slot_weights(const ggnn_prepared_graph* g, float* target_csr_w, float* source_csr_w) {
-    if (!g || !g->valid || g->shape.model != MODEL_GCN) return GGNN_ESTATE;
+    if (!g || !g->valid || !g->plan.weighted) return GGNN_ESTATE;
     const BatchPlan& q = g->plan;
     if (source_csr_w && !q.has_transpose) return GGNN_ESTATE;
     if (target_csr_w && q.M) memcpy(target_csr_w, g->image.ptr + q.off_slotw, sizeof(float) * (size_t)q.M);
