@@ -34,6 +34,7 @@ def _propagation_function():
             kernels = [k.detach().contiguous() for k in weights[:L]]
             biases = [b.detach().contiguous() for b in weights[L:]] or None
             engine.set_weights(kernels, biases)
+            engine.set_deterministic(torch.are_deterministic_algorithms_enabled())
             engine.set_save_for_backward(need)
             out = engine.forward(h0.detach().contiguous())
             ctx.serial = engine.serial   # the backward refuses once another forward, graph or weights replaced this one's
@@ -49,6 +50,7 @@ def _propagation_function():
             grads = [torch.zeros(s, dtype=torch.float32, device=d_out.device) for s in ctx.shapes]
             layers = [{'kernel': grads[l], 'bias': grads[L + l] if len(grads) > L else None} for l in range(L)]
             d_h0 = torch.zeros_like(d_out) if ctx.h0_needs else None
+            ctx.engine.set_deterministic(torch.are_deterministic_algorithms_enabled())
             ctx.engine.backward(d_out.contiguous(), layers, d_h0)
             return (None, d_h0) + tuple(grads)
 

@@ -32,6 +32,7 @@ def _propagation_function():
             # ctx.needs_input_grad is all False under torch.no_grad() (validation epochs): no activations are saved there
             need = any(ctx.needs_input_grad[2:])
             engine.set_weights([{k: v.detach().contiguous() for k, v in lw.items()} for lw in layers])
+            engine.set_deterministic(torch.are_deterministic_algorithms_enabled())
             engine.set_save_for_backward(need)
             out = engine.forward(h0.detach().contiguous())
             ctx.serial = engine.serial   # the backward refuses once another forward, graph or weights replaced this one's
@@ -46,6 +47,7 @@ def _propagation_function():
             grads_flat = [torch.zeros(s, dtype=torch.float32, device=d_out.device) for s in ctx.shapes]
             grads = [{k: grads_flat[i] for k, i in lay.items()} for lay in ctx.layout]
             d_h0 = torch.zeros_like(d_out) if ctx.h0_needs else None
+            ctx.engine.set_deterministic(torch.are_deterministic_algorithms_enabled())
             ctx.engine.backward(d_out.contiguous(), grads, d_h0)
             return (None, None, d_h0) + tuple(grads_flat)
 

@@ -14,8 +14,9 @@
 //          dh   += G_t . W_t^T   (G_t[s] = sum of dx'[target] over the type-t messages LEAVING s: source CSR)
 //
 // Kernels: elementwise cell gradients, one CSR gather for all edge types, a 64x64-tile FFMA GEMM  C (+)= sum_s A_s . B_s^T
-// for the data gradients and a split-row  C_s += A_s^T . B  with fp32 atomics for the weight (+ bias) gradients; the
-// segment lists keep it at ~12 launches per timestep whatever the number of edge types and residual inputs.
+// for the data gradients and a split-row  C_s += A_s^T . B  with fp32 atomics for the weight (+ bias) gradients (or, in deterministic mode,
+// per-split partials added in split order by a second kernel); the segment lists keep it at ~12 launches per timestep whatever the number
+// of edge types and residual inputs.
 #pragma once
 #include "ggnn_common.cuh"
 
@@ -117,9 +118,11 @@ struct SegList {
     const float* p[MAX_SEGS];
     int ld[MAX_SEGS];
 };
-__global__ void __launch_bounds__(64) gemm_tn_atomic_kernel(SegList segs, int kblocks, int a_vec, const float* __restrict__ B, int ldb,
-                                                            float* __restrict__ C, int ldc, size_t c_stride, float* __restrict__ bias_out, int M,
-                                                            int N, int K, int rows_per_split) {
+// SPLIT = false adds the tile into C with vector atomics (the row splits of one output tile race); SPLIT = true stores it with plain
+// stores into its split's own partial (C, bias_out are then the split's slab: gemm_tn_split_kernel).
+template <bool SPLIT>
+__device__ __forceinline__ void gemm_tn_tile(const SegList& segs, int kblocks, int a_vec, const float* __restrict__ B, int ldb, float* __restrict__ C,
+                                             int ldc, size_t c_stride, float* __restrict__ bias_out, int M, int N, int K, int rows_per_split) {
     __shared__ __align__(16) float As[2][GEMM_BK][64 + 4];
     __shared__ __align__(16) float Bs[2][GEMM_BK][64 + 4];
     const int tid = threadIdx.x, tx = tid & 7, ty = tid >> 3;
@@ -199,10 +202,84 @@ __global__ void __launch_bounds__(64) gemm_tn_atomic_kernel(SegList segs, int kb
         for (int jq = 0; jq < 2; ++jq) {
             const int n = n0 + tx * 4 + jq * 32;
             if (n >= N) continue;
-            atomicAdd(reinterpret_cast<float4*>(Cs + (size_t)k * ldc + n), make_float4(acc[i][jq * 4], acc[i][jq * 4 + 1], acc[i][jq * 4 + 2], acc[i][jq * 4 + 3]));
+            const float4 v = make_float4(acc[i][jq * 4], acc[i][jq * 4 + 1], acc[i][jq * 4 + 2], acc[i][jq * 4 + 3]);
+            if (SPLIT) *reinterpret_cast<float4*>(Cs + (size_t)k * ldc + n) = v;
+            else atomicAdd(reinterpret_cast<float4*>(Cs + (size_t)k * ldc + n), v);
         }
     }
-    if (do_bias && n0 + tid < N) atomicAdd(bias_out + n0 + tid, bsum);
+    if (do_bias && n0 + tid < N) {
+        if (SPLIT) bias_out[n0 + tid] = bsum;
+        else atomicAdd(bias_out + n0 + tid, bsum);
+    }
+}
+__global__ void __launch_bounds__(64) gemm_tn_atomic_kernel(SegList segs, int kblocks, int a_vec, const float* __restrict__ B, int ldb,
+                                                            float* __restrict__ C, int ldc, size_t c_stride, float* __restrict__ bias_out, int M,
+                                                            int N, int K, int rows_per_split) {
+    gemm_tn_tile<false>(segs, kblocks, a_vec, B, ldb, C, ldc, c_stride, bias_out, M, N, K, rows_per_split);
+}
+
+// ---------------------------------------------------------------- weight gradients in a fixed order (ggnn_set_deterministic)
+// Split z (blockIdx.z) of the same tiles stores its partial sums, without atomics, to part[z][s][K][N] (every segment s of the launch) and
+// its bias partial to bias_part[z][N]; split_reduce_kernel then adds the splits in split order and adds the result into C once.
+__global__ void __launch_bounds__(64) gemm_tn_split_kernel(SegList segs, int kblocks, int a_vec, const float* __restrict__ B, int ldb,
+                                                           float* __restrict__ part, float* __restrict__ bias_part, int M, int N, int K,
+                                                           int rows_per_split) {
+    const size_t per = (size_t)K * N;
+    gemm_tn_tile<true>(segs, kblocks, a_vec, B, ldb, part + (size_t)blockIdx.z * (gridDim.y / kblocks) * per, N, per,
+                       bias_part ? bias_part + (size_t)blockIdx.z * N : nullptr, M, N, K, rows_per_split);
+}
+// Bias-only requests: split z (blockIdx.y) stores the column sums of rows [z*rows_per_split, ..) of src, in row order, to bias_part[z][N].
+__global__ void __launch_bounds__(256) colsum_split_kernel(const float* __restrict__ src, int ld, float* __restrict__ bias_part, int M, int N,
+                                                           int rows_per_split) {
+    const int n = blockIdx.x * 256 + threadIdx.x;
+    if (n >= N) return;
+    const int mb = blockIdx.y * rows_per_split, me = min(M, mb + rows_per_split);
+    float s = 0.f;
+    for (int m = mb; m < me; ++m) s += src[(size_t)m * ld + n];
+    bias_part[(size_t)blockIdx.y * N + n] = s;
+}
+// C[s*c_stride + k*ldc + n] += sum_{z < splits} part[z][s][k][n]   and   bias_out[n] += sum_z bias_part[z][n], each sum in split order.
+// One thread per 4 consecutive outputs (N is a multiple of 4), then one per bias entry; C == nullptr: the bias only.
+__global__ void __launch_bounds__(256) split_reduce_kernel(const float* __restrict__ part, const float* __restrict__ bias_part, int splits, int nseg,
+                                                           int K, int N, float* __restrict__ C, int ldc, size_t c_stride, float* __restrict__ bias_out) {
+    const int per = K * N, quads = C ? nseg * per / 4 : 0, total = quads + (bias_out ? N : 0);   // K*N <= 256*512, nseg <= 16
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+        if (i < quads) {
+            const int e = i * 4, s = e / per, r = e - s * per, k = r / N, n = r - k * N;
+            float4 a = *reinterpret_cast<const float4*>(part + e);
+            for (int z = 1; z < splits; ++z) {
+                const float4 b = *reinterpret_cast<const float4*>(part + (size_t)z * nseg * per + e);
+                a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+            }
+            float4* c = reinterpret_cast<float4*>(C + s * c_stride + (size_t)k * ldc + n);
+            float4 o = *c;
+            o.x += a.x; o.y += a.y; o.z += a.z; o.w += a.w;
+            *c = o;
+        } else {
+            const int n = i - quads;
+            float a = bias_part[n];
+            for (int z = 1; z < splits; ++z) a += bias_part[(size_t)z * N + n];
+            bias_out[n] += a;
+        }
+    }
+}
+// dst[c] += sum over rows r of part[r * ld + c], for every column c (one block each): each thread adds rows tid, tid+256, .. in order, then a
+// fixed tree adds the 256 threads' sums -- the same order on every launch.
+__device__ __forceinline__ float ordered_column_sum(const float* __restrict__ part, int rows, int ld, int c, float* s_red) {
+    float a = 0.f;
+    for (int r = threadIdx.x; r < rows; r += 256) a += part[(size_t)r * ld + c];
+    s_red[threadIdx.x] = a;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (threadIdx.x < o) s_red[threadIdx.x] += s_red[threadIdx.x + o];
+        __syncthreads();
+    }
+    return s_red[0];
+}
+__global__ void __launch_bounds__(256) ordered_colsum_kernel(const float* __restrict__ part, int rows, int ld, float* __restrict__ dst) {
+    __shared__ float s_red[256];
+    const float a = ordered_column_sum(part, rows, ld, blockIdx.x, s_red);
+    if (threadIdx.x == 0) dst[blockIdx.x] += a;
 }
 
 // ---------------------------------------------------------------- column sums: dst[n] += sum_m src[m, n]  (optionally weighted by w[m*wstride])
@@ -334,13 +411,14 @@ __global__ void __launch_bounds__(256) csr_gather_all_kernel(GatherJob j0, Gathe
 //   d s_m = alpha_m (d alpha_m - sum_k alpha_k d alpha_k),   d a_t += d s_m <h[src], h[v]>,
 //   d h[v] += sum_m d s_m a_t h[src_m]   (this kernel, one warp per target),   d h[src] += d s_m a_t h[v]  (source kernel below).
 // dsa[slot] = d s_m a_t is left for the source kernel; scratch[slot] holds d alpha in between.
-__global__ void __launch_bounds__(256) attention_bwd_target_kernel(const int* __restrict__ row_ptr, const int* __restrict__ csr_src,
-                                                                   const float* __restrict__ h, const float* __restrict__ P,
-                                                                   const float* __restrict__ alpha, const float* __restrict__ att_w,
-                                                                   float* __restrict__ dsa, float* __restrict__ dh, float* __restrict__ d_att_w,
-                                                                   int V, int D, int T) {
-    __shared__ float s_daw[16];
-    if (threadIdx.x < 16) s_daw[threadIdx.x] = 0.f;
+// ORDERED = false adds d a_t with shared then global atomics.  ORDERED = true (ggnn_set_deterministic): every warp's d a_t goes to its own
+// shared slot, the block adds the slots in warp order and stores its partial to d_att_w[blockIdx.x * T + t] (then ordered_colsum_kernel).
+template <bool ORDERED>
+__device__ __forceinline__ void attention_bwd_target(const int* __restrict__ row_ptr, const int* __restrict__ csr_src, const float* __restrict__ h,
+                                                     const float* __restrict__ P, const float* __restrict__ alpha, const float* __restrict__ att_w,
+                                                     float* __restrict__ dsa, float* __restrict__ dh, float* __restrict__ d_att_w, int V, int D, int T) {
+    __shared__ float s_daw[ORDERED ? 8 * 16 : 16];
+    if (threadIdx.x < (ORDERED ? 8 * 16 : 16)) s_daw[threadIdx.x] = 0.f;
     __syncthreads();
     const int v = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (v < V) {
@@ -380,7 +458,8 @@ __global__ void __launch_bounds__(256) attention_bwd_target_kernel(const int* __
                 __syncwarp();
                 if (lane == 0) dsa[m] = ds * aw;
             }
-            if (lane == 0 && d_att_w && daw != 0.f) atomicAdd(&s_daw[t], daw);
+            if (ORDERED) { if (lane == 0) s_daw[(threadIdx.x >> 5) * 16 + t] = daw; }
+            else if (lane == 0 && d_att_w && daw != 0.f) atomicAdd(&s_daw[t], daw);
         }
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -389,7 +468,28 @@ __global__ void __launch_bounds__(256) attention_bwd_target_kernel(const int* __
         }
     }
     __syncthreads();
-    if (d_att_w && threadIdx.x < T && s_daw[threadIdx.x] != 0.f) atomicAdd(d_att_w + threadIdx.x, s_daw[threadIdx.x]);
+    if (ORDERED) {
+        if (threadIdx.x < T) {
+            float a = s_daw[threadIdx.x];
+            for (int w = 1; w < 8; ++w) a += s_daw[w * 16 + threadIdx.x];
+            d_att_w[(size_t)blockIdx.x * T + threadIdx.x] = a;
+        }
+    } else if (d_att_w && threadIdx.x < T && s_daw[threadIdx.x] != 0.f) atomicAdd(d_att_w + threadIdx.x, s_daw[threadIdx.x]);
+}
+__global__ void __launch_bounds__(256) attention_bwd_target_kernel(const int* __restrict__ row_ptr, const int* __restrict__ csr_src,
+                                                                   const float* __restrict__ h, const float* __restrict__ P,
+                                                                   const float* __restrict__ alpha, const float* __restrict__ att_w,
+                                                                   float* __restrict__ dsa, float* __restrict__ dh, float* __restrict__ d_att_w,
+                                                                   int V, int D, int T) {
+    attention_bwd_target<false>(row_ptr, csr_src, h, P, alpha, att_w, dsa, dh, d_att_w, V, D, T);
+}
+// d_att_part: [gridDim.x][T] block partials of d a_t, reduced by ordered_colsum_kernel
+__global__ void __launch_bounds__(256) attention_bwd_target_ordered_kernel(const int* __restrict__ row_ptr, const int* __restrict__ csr_src,
+                                                                           const float* __restrict__ h, const float* __restrict__ P,
+                                                                           const float* __restrict__ alpha, const float* __restrict__ att_w,
+                                                                           float* __restrict__ dsa, float* __restrict__ dh,
+                                                                           float* __restrict__ d_att_part, int V, int D, int T) {
+    attention_bwd_target<true>(row_ptr, csr_src, h, P, alpha, att_w, dsa, dh, d_att_part, V, D, T);
 }
 // d h[s] += sum over the messages LEAVING s of dsa[target-CSR slot] * h[target]     (source-keyed CSR, one warp per source)
 __global__ void __launch_bounds__(256) attention_bwd_source_kernel(const int* __restrict__ trow, const int* __restrict__ ttgt,

@@ -214,6 +214,8 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     DevBuf ro_buf; StagedImage ro_stage;
     int ro_V = -1, ro_G = 0; bool ro_grouped = false, ro_has_mask = false;
     size_t ro_off_graph_of = 0, ro_off_start = 0, ro_off_mask = 0, ro_off_val = 0;
+    size_t ro_off_perm = 0;   // ungrouped lists: the stable by-graph node permutation (graph g owns perm[start[g] .. start[g+1]))
+    DevBuf ro_ws;             // deterministic readout backward: per-block partials of the weight gradients
     DevBuf state_buf;   // intermediate layer states (L-1) + 2 ping-pong step buffers, each [V][D]
     DevBuf save_bufs;   // 5 (CudnnCompatibleGRUCell: 6) x total_steps x [V][D]
     DevBuf io_buf;      // h0 / h_out staging for ggnn_forward_host
@@ -229,6 +231,7 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     bool fwd_valid = false, layers_written = false;
     bool save = false;
     bool saved_valid = false;   // the saved activations are those of the last forward, with the current weights
+    bool det = false;           // ggnn_set_deterministic: fixed-order weight-gradient and readout sums
     DevBuf ts_images;                                // the streaming plan's operand images and chunk-major states
     DevBuf ts_virt;                                  // the operand image of the streaming plan's virtual rows
     DevBuf att_buf;                  // attention probabilities per target-CSR slot ([steps][M] when saving for backward, else [M])
@@ -600,6 +603,86 @@ void find_cuts(const int* reach, int V, std::vector<int>& cuts) {
 }  // namespace
 
 // ------------------------------------------------------------------------------------------ backward (host orchestration)
+// The weight-gradient launch  C_s[K,N] += A_s^T . B  for every segment s (C_s = C + s*c_stride), bias[n] += sum_m B[m,n], shared by the
+// GGNN and the GCN backward.  Where the split policy lives:
+//  - atomic (the default): ~4 CTAs of 64 threads per SM, >= 64 rows per split (every split costs K*N atomics per segment), the splits add
+//    into C with float atomics; a bias-only request sums 512-row blocks with atomics.
+//  - deterministic (ggnn_set_deterministic): the split count and boundaries depend on (M, N, K, nseg) only -- the same target of
+//    DET_TARGET_CTAS CTAs whatever the GPU -- and every split stores its partial into `ws`; split_reduce_kernel adds them in split order and
+//    adds the sum into C (and bias) once.  A bias-only request: 512-row splits, the same reduction.
+struct TnSplit {
+    int splits = 1, rows = 0;   // number of row splits, rows per split (a multiple of GEMM_BK)
+    size_t ws_floats = 0;       // deterministic: floats of the partials, [splits][nseg][K][N] + [splits][N]
+};
+constexpr int DET_TARGET_CTAS = 512;
+constexpr int COLSUM_ROWS = 512;
+static TnSplit tn_split(int target_ctas, bool has_C, bool has_bias, int M, int N, int K, int nseg) {
+    TnSplit p;
+    if (has_C) {
+        const int kblocks = (K + 63) / 64;
+        const int tiles = ((N + 63) / 64) * nseg * kblocks;
+        const int want = std::max(1, (target_ctas + tiles - 1) / tiles);
+        const int splits = std::max(1, std::min(want, (M + 63) / 64));
+        p.rows = ((M + splits - 1) / splits + ggnn::bwd::GEMM_BK - 1) / ggnn::bwd::GEMM_BK * ggnn::bwd::GEMM_BK;
+        p.splits = (M + p.rows - 1) / p.rows;
+        p.ws_floats = (size_t)p.splits * nseg * K * N;
+    } else {
+        p.rows = COLSUM_ROWS;
+        p.splits = (M + COLSUM_ROWS - 1) / COLSUM_ROWS;
+    }
+    if (has_bias) p.ws_floats += (size_t)p.splits * N;
+    return p;
+}
+// Floats of deterministic workspace a gemm_tn call of this shape needs (0 when the engine is not in deterministic mode).
+static size_t gemm_tn_workspace(const ggnn_engine* e, bool has_C, bool has_bias, int M, int N, int K, int nseg) {
+    return e->det && (has_C || has_bias) ? tn_split(DET_TARGET_CTAS, has_C, has_bias, M, N, K, nseg).ws_floats : 0;
+}
+// `ws` holds `ws_cap` floats; a deterministic call whose partials would not fit launches nothing and fails (the caller sizes the workspace
+// from every shape it launches, gemm_tn_workspace, so this is a guard against a sizing mistake, never a silent overflow).
+static int gemm_tn(ggnn_engine* e, cudaStream_t st, float* ws, size_t ws_cap, const ggnn::bwd::SegList& segs, int nseg, bool a_vec, const float* B,
+                   int ldb, float* C, int ldc, size_t c_stride, float* bias, int M, int N, int K) {
+    using namespace ggnn::bwd;
+    if (!C && !bias) return GGNN_OK;
+    const int kblocks = (K + 63) / 64;
+    if (!e->det) {
+        if (C) {
+            const TnSplit p = tn_split(4 * e->num_sms, true, false, M, N, K, nseg);
+            gemm_tn_atomic_kernel<<<dim3((N + 63) / 64, nseg * kblocks, p.splits), 64, 0, st>>>(segs, kblocks, a_vec ? 1 : 0, B, ldb, C, ldc,
+                                                                                                c_stride, bias, M, N, K, p.rows);
+        } else {
+            colsum_atomic_kernel<<<dim3((N + 255) / 256, (M + COLSUM_ROWS - 1) / COLSUM_ROWS), 256, 0, st>>>(B, ldb, nullptr, 0, bias, M, N,
+                                                                                                              COLSUM_ROWS);
+        }
+        ++e->last_launches;
+        return GGNN_OK;
+    }
+    const TnSplit p = tn_split(DET_TARGET_CTAS, C != nullptr, bias != nullptr, M, N, K, nseg);
+    if (p.ws_floats > ws_cap)
+        return e->fail(GGNN_ESTATE, "internal: the deterministic workspace holds %zu floats, a weight-gradient launch (M %d, N %d, K %d, %d segments) "
+                                    "needs %zu", ws_cap, M, N, K, nseg, p.ws_floats);
+    float* bias_part = bias ? ws + (C ? (size_t)p.splits * nseg * K * N : 0) : nullptr;
+    if (C) gemm_tn_split_kernel<<<dim3((N + 63) / 64, nseg * kblocks, p.splits), 64, 0, st>>>(segs, kblocks, a_vec ? 1 : 0, B, ldb, ws, bias_part,
+                                                                                               M, N, K, p.rows);
+    else colsum_split_kernel<<<dim3((N + 255) / 256, p.splits), 256, 0, st>>>(B, ldb, bias_part, M, N, p.rows);
+    const size_t work = (C ? (size_t)nseg * K * N / 4 : 0) + (bias ? N : 0);
+    split_reduce_kernel<<<(int)std::min<size_t>((work + 255) / 256, 4096), 256, 0, st>>>(ws, bias_part, p.splits, nseg, K, N, C, ldc, c_stride, bias);
+    e->last_launches += 2;
+    return GGNN_OK;
+}
+
+// The gradient fields of layer l the model has, with their sizes in floats, in ggnn_layer_grads order (a field the model lacks: size 0).
+static std::array<size_t, 8> layer_grad_floats(const ggnn_engine* e, int l) {
+    const size_t D = e->D, T = e->T, rows = D * (2 + e->nres[l]);   // [res.. | x | h] rows of the cell kernels
+    const bool gates = e->cell != CELL_RNN;
+    return {T * D * D, e->use_bias ? T * D : 0, gates ? rows * 2 * D : 0, gates ? 2 * D : 0, rows * D, D, e->use_att ? T : 0,
+            e->cell == CELL_CUDNN_GRU ? D : 0};
+}
+static float** grad_field(ggnn_layer_grads& g, int i) {
+    float** f[8] = {&g.edge_weights, &g.edge_biases, &g.gate_kernel, &g.gate_bias, &g.cand_kernel, &g.cand_bias, &g.edge_type_attention_weights,
+                    &g.cand_hidden_bias};
+    return f[i];
+}
+
 static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers,
                               float* d_h0, ggnn_stream_t stream) {
     using namespace ggnn::bwd;
@@ -617,6 +700,34 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
     const size_t o_dstate = take(vd * (L + 1)), o_dha = take(vd), o_dhb = take(vd), o_dpc = take(vd), o_dpg = take(2 * vd);
     const size_t o_dxc = take((size_t)V * ldx_max), o_dxg = take((size_t)V * ldx_max), o_rh = take(vd), o_dxp = take(vd), o_at = take(vd * T), o_gt = take(vd * T);
     const size_t o_pall = take(e->use_att ? vd * T : 0), o_dsa = take(e->use_att ? (size_t)std::max<int64_t>(e->M, 1) : 0);
+    // deterministic mode: room for the partials of every weight-gradient launch below (the need is not monotone in the segment count --
+    // fewer segments get more splits -- so every launched shape is sized), and the attention's per-block d a_t
+    const int nodes_blocks = (V + 7) / 8;
+    size_t ws_floats = 0;
+    if (e->det) {
+        auto need = [&](bool has_C, int N, int K, int nseg) { ws_floats = std::max(ws_floats, gemm_tn_workspace(e, has_C, true, V, N, K, nseg)); };
+        for (int l = 0; l < L; ++l) {
+            const int R = e->nres[l];
+            need(true, D, D, R + 2);         // candidate kernel (GRU, RNN), [res.. | x | r*h or h]
+            need(true, 2 * D, D, R + 2);     // gate kernel
+            if (e->cell == CELL_CUDNN_GRU) { need(true, D, D, R + 1); need(true, D, D, 1); }   // input and hidden projections
+        }
+        need(true, D, T, 1);                 // edge biases (indeg^T . dx'), no bias partial: sized with one, which is larger
+        for (int t0 = 0; t0 < T; t0 += MAX_SEGS) need(true, D, D, std::min(MAX_SEGS, T - t0));   // edge-weight chunks
+        need(false, D, D, 1);                // bias-only requests
+        need(false, 2 * D, D, 1);
+        if (e->use_att) ws_floats = std::max(ws_floats, (size_t)nodes_blocks * T);
+    }
+    const size_t o_ws = take(ws_floats);
+    // deterministic mode: a layer's weight gradients are summed over its timesteps in zeroed buffers, then added to the caller's once
+    size_t gsum_floats = 0;
+    if (e->det)
+        for (int l = 0; l < L; ++l) {
+            size_t f = 0;
+            for (size_t x : layer_grad_floats(e, l)) f += align_up(x, 64);
+            gsum_floats = std::max(gsum_floats, f);
+        }
+    const size_t o_gsum = take(gsum_floats);
     const size_t o_ptrs = off; off += 256;
     CU_TRY(e, e->bwd_buf.reserve(off));
     char* bb = (char*)e->bwd_buf.ptr;
@@ -625,6 +736,7 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
     float *dxc = (float*)(bb + o_dxc), *dxg = (float*)(bb + o_dxg), *rh = (float*)(bb + o_rh), *dxp = (float*)(bb + o_dxp);
     float *At = (float*)(bb + o_at), *Gt = (float*)(bb + o_gt), *Pall = (float*)(bb + o_pall), *dsa = (float*)(bb + o_dsa);
     float** d_ptrs = (float**)(bb + o_ptrs);
+    float* ws = (float*)(bb + o_ws);
     CU_TRY(e, cudaMemsetAsync(dstate, 0, vd * L * sizeof(float), st));
     CU_TRY(e, cudaMemcpyAsync(dstate + vd * L, d_h_out, vd * sizeof(float), cudaMemcpyDeviceToDevice, st));
     // forward values of node_states_per_layer
@@ -641,31 +753,27 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
         ++e->last_launches;
     };
     // C_s[K,N] += A_s^T . B for every segment (C_s = C + s*c_stride), bias[n] += sum_m B[m,n]
+    int ws_rc = GGNN_OK;   // the first failure of a weight-gradient launch (none launches after it)
     auto gemm_tn = [&](const SegList& segs, int nseg, bool a_vec, const float* B, int ldb, float* C, int ldc, size_t c_stride, float* bias, int M,
                        int N, int K) {
-        if (!C && !bias) return;
-        if (C) {
-            const int kblocks = (K + 63) / 64;
-            const int tiles = ((N + 63) / 64) * nseg * kblocks;
-            // ~4 CTAs of 64 threads per SM; every split costs K*N atomics per segment, so keep >= 64 rows per split
-            const int want = std::max(1, (4 * e->num_sms + tiles - 1) / tiles);
-            const int splits = std::max(1, std::min(want, (M + 63) / 64));
-            const int rps = ((M + splits - 1) / splits + GEMM_BK - 1) / GEMM_BK * GEMM_BK;
-            dim3 grid((N + 63) / 64, nseg * kblocks, (M + rps - 1) / rps);
-            gemm_tn_atomic_kernel<<<grid, 64, 0, st>>>(segs, kblocks, a_vec ? 1 : 0, B, ldb, C, ldc, c_stride, bias, M, N, K, rps);
-        } else {   // bias gradient only
-            const int rpb = 512;
-            dim3 grid((N + 255) / 256, (M + rpb - 1) / rpb);
-            colsum_atomic_kernel<<<grid, 256, 0, st>>>(B, ldb, nullptr, 0, bias, M, N, rpb);
-        }
-        ++e->last_launches;
+        if (ws_rc == GGNN_OK) ws_rc = ::gemm_tn(e, st, ws, ws_floats, segs, nseg, a_vec, B, ldb, C, ldc, c_stride, bias, M, N, K);
     };
-    const int nodes_blocks = (V + 7) / 8;
     const int TD = T * D;
     for (int l = L - 1; l >= 0; --l) {
         const int R = e->nres[l], din = D * (1 + R), ldx = din + D;
         const ggnn_layer_weights& w = e->w[l];
-        const ggnn_layer_grads& gw = grads[l];
+        ggnn_layer_grads gw = grads[l];
+        const std::array<size_t, 8> gfloats = layer_grad_floats(e, l);
+        if (e->det) {
+            float* p = (float*)(bb + o_gsum);
+            for (int i = 0; i < 8; ++i) {
+                float** f = grad_field(gw, i);
+                if (!*f) continue;
+                *f = gfloats[i] ? p : nullptr;
+                p += align_up(gfloats[i], 64);
+            }
+            CU_TRY(e, cudaMemsetAsync(bb + o_gsum, 0, (char*)p - (bb + o_gsum), st));
+        }
         if (R > 0) {
             float* hp[MAX_RES];
             for (int i = 0; i < R; ++i) hp[i] = dstate + (size_t)e->res[l][i] * vd;
@@ -733,8 +841,15 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
                 if (e->use_att) {   // softmax backward first (it adds to dh_new), then the gathers are weighted by the probabilities
                     alpha = (const float*)e->att_buf.ptr + (size_t)(e->step_base[l] + s) * (size_t)std::max<int64_t>(e->M, 1);
                     gemm_nt(false, dxp, D, 0, w.edge_weights, D, 0, 1, Pall, TD, V, TD, D);   // P[v, t*D+k] = <dx'[v], W_t[k, :]>
-                    attention_bwd_target_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, Pall, alpha, w.edge_type_attention_weights,
-                                                                              dsa, dh_new, gw.edge_type_attention_weights, V, D, T);
+                    if (e->det && gw.edge_type_attention_weights) {   // per-block d a_t into ws, then added over the blocks in a fixed order
+                        attention_bwd_target_ordered_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, Pall, alpha,
+                                                                                          w.edge_type_attention_weights, dsa, dh_new, ws, V, D, T);
+                        ordered_colsum_kernel<<<T, 256, 0, st>>>(ws, nodes_blocks, T, gw.edge_type_attention_weights);
+                        ++e->last_launches;
+                    } else {
+                        attention_bwd_target_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, Pall, alpha, w.edge_type_attention_weights,
+                                                                                  dsa, dh_new, gw.edge_type_attention_weights, V, D, T);
+                    }
                     attention_bwd_source_kernel<<<nodes_blocks, 256, 0, st>>>(gd.trow, gd.ttgt, gd.tslot, h, dsa, dh_new, V, D, T);
                     e->last_launches += 2;
                 }
@@ -767,9 +882,19 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
             dhn = dh_new;
             dh_new = (dh_new == dha) ? dhb : dha;
         }
+        if (e->det) {
+            ggnn_layer_grads out = grads[l];
+            for (int i = 0; i < 8; ++i) {
+                float *dst = *grad_field(out, i), *src = *grad_field(gw, i);
+                if (!dst || !src) continue;
+                add_inplace_kernel<<<(int)std::min<size_t>((gfloats[i] + 255) / 256, 4096), 256, 0, st>>>(dst, src, (long long)gfloats[i]);
+                ++e->last_launches;
+            }
+        }
         if (e->steps[l] > 0) { add_inplace_kernel<<<eb, 256, 0, st>>>(dstate + (size_t)l * vd, dhn, n); ++e->last_launches; }
         else { add_inplace_kernel<<<eb, 256, 0, st>>>(dstate + (size_t)l * vd, dstate + (size_t)(l + 1) * vd, n); ++e->last_launches; }
     }
+    if (ws_rc != GGNN_OK) return ws_rc;
     if (d_h0) CU_TRY(e, cudaMemcpyAsync(d_h0, dstate, vd * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CU_TRY(e, cudaGetLastError());
     return GGNN_OK;
@@ -880,7 +1005,7 @@ int ggnn_destroy(ggnn_engine* e) {
     e->graph_buf.release(); e->state_buf.release(); e->save_bufs.release(); e->io_buf.release(); e->bwd_buf.release();
     e->tc_tiles.buf.release(); e->tc_respre.release(); e->ts_tiles.buf.release(); e->ts_images.release(); e->ts_virt.release(); e->err_flag.release();
     if (e->own_prep) { ggnn_free_prepared_graph(e->own_prep); e->own_prep = nullptr; }
-    e->ro_buf.release(); e->ro_stage.release(); e->att_buf.release();
+    e->ro_buf.release(); e->ro_stage.release(); e->att_buf.release(); e->ro_ws.release();
     delete e;
     return GGNN_OK;
 }
@@ -2163,7 +2288,7 @@ static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream
 // Backward of the GCN layers, fp32 on CUDA cores, per layer in reverse:
 //   dPre = dOut (last layer) or dOut * relu'(y) * mask / keep (gcn_relu_dropout_grad_kernel, from the saved output y)
 //   S    = A . H_l (recomputed from the saved layer input: one gather instead of L saved [V, D] arrays)
-//   dW  += S^T . dPre,  db += sum dPre            (gemm_tn_atomic_kernel, the bias rides along)
+//   dW  += S^T . dPre,  db += sum dPre            (gemm_tn: atomic or fixed-order split sums, the bias rides along)
 //   dS   = dPre . W^T                             (gemm_nt_kernel)
 //   dH_l = A^T . dS                               (csr_gather_all_kernel over the source-keyed CSR with its per-slot weights: no float atomics)
 int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0, ggnn_stream_t stream) {
@@ -2176,9 +2301,10 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
     if (V == 0) return GGNN_OK;
     const size_t vd = (size_t)V * D;
     const size_t slab = align_up(vd * sizeof(float), 256);
-    CU_TRY(e, e->bwd_buf.reserve(4 * slab));
+    const size_t ws_floats = std::max(gemm_tn_workspace(e, true, e->use_bias, V, D, D, 1), gemm_tn_workspace(e, false, e->use_bias, V, D, D, 1));
+    CU_TRY(e, e->bwd_buf.reserve(4 * slab + ws_floats * sizeof(float)));
     char* bb = (char*)e->bwd_buf.ptr;
-    float *dH = (float*)bb, *dP = (float*)(bb + slab), *S = (float*)(bb + 2 * slab), *dS = (float*)(bb + 3 * slab);
+    float *dH = (float*)bb, *dP = (float*)(bb + slab), *S = (float*)(bb + 2 * slab), *dS = (float*)(bb + 3 * slab), *ws = (float*)(bb + 4 * slab);
     const GraphDev& gd = e->gd;
     std::vector<const float*> fstate(L + 1);
     for (int l = 0; l <= L; ++l) fstate[l] = layer_state(e, l, e->last_h0, e->last_out);
@@ -2198,19 +2324,15 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
         if (gw.kernel) {
             GatherJob j{gd.row_ptr, gd.csr_src, fstate[l], S, gd.slot_w, nullptr};
             csr_gather_all_kernel<<<gather_grid, 256, 0, st>>>(j, j, V, D, 1);
+            ++e->last_launches;
             SegList sl;
             memset(&sl, 0, sizeof sl);
             sl.p[0] = S; sl.ld[0] = D;
-            const int kblocks = (D + 63) / 64, tiles = ((D + 63) / 64) * kblocks;
-            const int want = std::max(1, (4 * e->num_sms + tiles - 1) / tiles);
-            const int splits = std::max(1, std::min(want, (V + 63) / 64));
-            const int rps = ((V + splits - 1) / splits + GEMM_BK - 1) / GEMM_BK * GEMM_BK;
-            gemm_tn_atomic_kernel<<<dim3((D + 63) / 64, kblocks, (V + rps - 1) / rps), 64, 0, st>>>(sl, kblocks, 1, dpre, D, gw.kernel, D, 0,
-                                                                                                   e->use_bias ? gw.bias : nullptr, V, D, D, rps);
-            e->last_launches += 2;
+            if (int rc = gemm_tn(e, st, ws, ws_floats, sl, 1, true, dpre, D, gw.kernel, D, 0, e->use_bias ? gw.bias : nullptr, V, D, D)) return rc;
         } else if (e->use_bias && gw.bias) {
-            colsum_atomic_kernel<<<dim3((D + 255) / 256, (V + 511) / 512), 256, 0, st>>>(dpre, D, nullptr, 0, gw.bias, V, D, 512);
-            ++e->last_launches;
+            SegList none;
+            memset(&none, 0, sizeof none);
+            if (int rc = gemm_tn(e, st, ws, ws_floats, none, 1, true, dpre, D, nullptr, D, 0, gw.bias, V, D, D)) return rc;
         }
         if (l == 0 && !d_h0) break;
         gemm_nt_kernel<false><<<dim3((D + NT_BN - 1) / NT_BN, (V + NT_BM - 1) / NT_BM), 128, 0, st>>>(dpre, D, 0, e->gcn_w[l].kernel, D, 0, 1, dS, D, V,
@@ -2326,6 +2448,7 @@ int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* gr
     e->ro_off_graph_of = off; off = align_up(off + sizeof(int) * (size_t)std::max(V, 1), 16);
     e->ro_off_start = off;    off = align_up(off + sizeof(int) * (size_t)(G + 1), 16);
     e->ro_off_mask = off;     off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
+    e->ro_off_perm = off;     off = align_up(off + sizeof(int) * (size_t)std::max(V, 1), 16);   // uploaded for ungrouped lists only
     e->ro_off_val = off;      // device-only scratch: per-node gated value
     const size_t dev_bytes = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
     CU_TRY(e, e->ro_stage.begin(off));
@@ -2346,9 +2469,16 @@ int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* gr
             while (v < V && graph_of[v] < g) ++v;
             start[g] = v;
         }
+    } else {   // the stable counting sort by graph: graph g owns perm[start[g] .. start[g+1]), its nodes in index order (deterministic mode)
+        int* perm = (int*)(base + e->ro_off_perm);
+        std::fill(start, start + G + 1, 0);
+        for (int v = 0; v < V; ++v) ++start[graph_of[v] + 1];
+        for (int g = 0; g < G; ++g) start[g + 1] += start[g];
+        std::vector<int> cursor(start, start + G);
+        for (int v = 0; v < V; ++v) perm[cursor[graph_of[v]]++] = v;
     }
     if (node_mask) memcpy(base + e->ro_off_mask, node_mask, sizeof(float) * (size_t)V);
-    CU_TRY(e, e->ro_stage.upload(e->ro_buf.ptr, off, (cudaStream_t)stream));
+    CU_TRY(e, e->ro_stage.upload(e->ro_buf.ptr, grouped ? e->ro_off_perm : off, (cudaStream_t)stream));
     e->ro_V = V; e->ro_G = G; e->ro_grouped = grouped; e->ro_has_mask = node_mask != nullptr;
     return GGNN_OK;
 }
@@ -2380,6 +2510,9 @@ int ggnn_readout_forward(ggnn_engine* e, const float* h_last, const float* h0, c
     if (V > 0) readout::readout_node_kernel<<<(V + 7) / 8, 256, 0, st>>>(h_last, h0, w, mask, val, V, e->D);
     if (e->ro_grouped || V == 0) {
         readout::readout_sum_grouped_kernel<<<(G + 127) / 128, 128, 0, st>>>(val, (const int*)(g + e->ro_off_start), out, G);
+    } else if (e->det) {
+        readout::readout_sum_permuted_kernel<<<(G + 127) / 128, 128, 0, st>>>(val, (const int*)(g + e->ro_off_start), (const int*)(g + e->ro_off_perm),
+                                                                            out, G);
     } else {
         CU_TRY(e, cudaMemsetAsync(out, 0, sizeof(float) * (size_t)G, st));
         readout::readout_sum_atomic_kernel<<<(V + 255) / 256, 256, 0, st>>>(val, (const int*)(g + e->ro_off_graph_of), out, V);
@@ -2400,6 +2533,16 @@ int ggnn_readout_backward(ggnn_engine* e, const float* h_last, const float* h0, 
     char* g = (char*)e->ro_buf.ptr;
     const float* mask = e->ro_has_mask ? (const float*)(g + e->ro_off_mask) : nullptr;
     readout::Weights w{w_gate, b_gate, w_trans, b_trans};
+    if (e->det) {   // a grid fixed by V alone, per-block partials, then every gradient entry summed over the blocks in a fixed order
+        const int blocks = std::max(1, std::min((V + 7) / 8, readout::RO_ORDERED_BLOCKS)), cols = 3 * e->D + 2;
+        CU_TRY(e, e->ro_ws.reserve(sizeof(float) * (size_t)blocks * cols));
+        float* part = (float*)e->ro_ws.ptr;
+        readout::readout_bwd_ordered_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(h_last, h0, w, (const int*)(g + e->ro_off_graph_of), mask, d_out,
+                                                                                     d_h_last, part, V, e->D);
+        readout::readout_bwd_reduce_kernel<<<cols, 256, 0, (cudaStream_t)stream>>>(part, blocks, e->D, d_w_gate, d_b_gate, d_w_trans, d_b_trans);
+        CU_TRY(e, cudaGetLastError());
+        return GGNN_OK;
+    }
     const int blocks = std::max(1, std::min((V + 7) / 8, 4 * e->num_sms));
     readout::readout_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(h_last, h0, w, (const int*)(g + e->ro_off_graph_of), mask, d_out, d_h_last,
                                                                          d_w_gate, d_b_gate, d_w_trans, d_b_trans, V, e->D);
@@ -2465,6 +2608,12 @@ int ggnn_set_save_for_backward(ggnn_engine* e, int32_t enable) {
     if (!e) return GGNN_EINVAL;
     e->save = enable != 0;
     e->saved_valid = false;
+    return GGNN_OK;
+}
+
+int ggnn_set_deterministic(ggnn_engine* e, int32_t enable) {
+    if (!e) return GGNN_EINVAL;
+    e->det = enable != 0;
     return GGNN_OK;
 }
 

@@ -3,10 +3,12 @@
 //   out[g]  = sum of val over the nodes of graph g          (tf.unsorted_segment_sum / masked reduce_sum)
 // The reference's readout MLPs have no hidden layers (chem_tensorflow.py:153-157), so each is one affine map to a scalar.
 // Forward: one warp per node computes val[v] (every node row read once, float4), then one thread per graph adds its nodes in
-// order (the serial order of TF's CPU segment sum, deterministic); node lists not grouped by graph take an atomicAdd stage.  Backward: one warp per node
-// recomputes the two dot products, writes d h_T, accumulates the weight gradients in registers and reduces them per block.
+// order (the serial order of TF's CPU segment sum, deterministic); node lists not grouped by graph take an atomicAdd stage (in deterministic
+// mode, the same per-graph order through a by-graph permutation).  Backward: one warp per node recomputes the two dot products, writes d h_T,
+// accumulates the weight gradients in registers and reduces them per block.
 #pragma once
 #include "ggnn_common.cuh"
+#include "ggnn_bwd.cuh"
 
 namespace ggnn {
 namespace readout {
@@ -78,16 +80,35 @@ __global__ void __launch_bounds__(256) readout_sum_atomic_kernel(const float* __
     if (v < V) atomicAdd(out + graph_of[v], val[v]);
 }
 
-// d_out[G] -> d_h_last[V,D] (written), d_w_gate[2D] / d_b_gate[1] / d_w_trans[D] / d_b_trans[1] (accumulated, atomics per block)
-__global__ void __launch_bounds__(256) readout_bwd_kernel(const float* __restrict__ h_last, const float* __restrict__ h0, Weights w,
-                                                          const int* __restrict__ graph_of, const float* __restrict__ mask,
-                                                          const float* __restrict__ d_out, float* __restrict__ d_h_last,
-                                                          float* __restrict__ d_w_gate, float* __restrict__ d_b_gate,
-                                                          float* __restrict__ d_w_trans, float* __restrict__ d_b_trans, int V, int D) {
-    __shared__ float red[3 * 256 + 2];   // [d_w_gate(h_T part) | d_w_gate(h_0 part) | d_w_trans] for d < 256, then the two biases
+// stage 2 of an ungrouped graph_of[v] in deterministic mode: graph g owns positions [graph_start[g], graph_start[g+1]) of the stable by-graph
+// permutation `perm` (node index order inside a graph), summed in that order -- the grouped kernel's order, through one indirection
+__global__ void __launch_bounds__(128) readout_sum_permuted_kernel(const float* __restrict__ val, const int* __restrict__ graph_start,
+                                                                   const int* __restrict__ perm, float* __restrict__ out, int G) {
+    const int g = blockIdx.x * 128 + threadIdx.x;
+    if (g >= G) return;
+    float acc = 0.f;
+    for (int i = graph_start[g]; i < graph_start[g + 1]; ++i) acc += val[perm[i]];
+    out[g] = acc;
+}
+
+// d_out[G] -> d_h_last[V,D] (written), d_w_gate[2D] / d_b_gate[1] / d_w_trans[D] / d_b_trans[1].
+// ORDERED = false accumulates them with shared, then global atomics per block.  ORDERED = true (ggnn_set_deterministic): each warp stores its
+// sums to its own shared row, the block adds the rows in warp order and stores its partial [d_w_gate | d_w_trans | d_b_gate | d_b_trans]
+// ([3D+2]) to part[blockIdx.x]; readout_bwd_reduce_kernel adds the blocks.  The grid must then not depend on the GPU (the grid-stride loop
+// gives every warp its nodes by gridDim).
+constexpr int RO_ROW = 3 * 256 + 2;   // [d_w_gate(h_T part) | d_w_gate(h_0 part) | d_w_trans] for d < 256, then the two biases
+constexpr int RO_ORDERED_BLOCKS = 512;
+template <bool ORDERED>
+__device__ __forceinline__ void readout_bwd(const float* __restrict__ h_last, const float* __restrict__ h0, const Weights& w,
+                                            const int* __restrict__ graph_of, const float* __restrict__ mask, const float* __restrict__ d_out,
+                                            float* __restrict__ d_h_last, float* __restrict__ d_w_gate, float* __restrict__ d_b_gate,
+                                            float* __restrict__ d_w_trans, float* __restrict__ d_b_trans, float* __restrict__ part, int V, int D) {
+    __shared__ float red[ORDERED ? 8 * RO_ROW : RO_ROW];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int i = threadIdx.x; i < 3 * 256 + 2; i += 256) red[i] = 0.f;
-    __syncthreads();
+    if (!ORDERED) {
+        for (int i = threadIdx.x; i < 3 * 256 + 2; i += 256) red[i] = 0.f;
+        __syncthreads();
+    }
     float gw_a[MAX_D_PER_LANE], gw_b[MAX_D_PER_LANE], tw[MAX_D_PER_LANE];
 #pragma unroll
     for (int j = 0; j < MAX_D_PER_LANE; ++j) gw_a[j] = gw_b[j] = tw[j] = 0.f;
@@ -114,6 +135,25 @@ __global__ void __launch_bounds__(256) readout_bwd_kernel(const float* __restric
         }
         gb += dgp; tb += dt;
     }
+    if (ORDERED) {
+        float* row = red + warp * RO_ROW;
+#pragma unroll
+        for (int j = 0; j < MAX_D_PER_LANE; ++j) {
+            const int d = lane + 32 * j;
+            if (d < D) { row[d] = gw_a[j]; row[256 + d] = gw_b[j]; row[512 + d] = tw[j]; }
+        }
+        if (lane == 0) { row[768] = gb; row[769] = tb; }
+        __syncthreads();
+        float* out = part + (size_t)blockIdx.x * (3 * D + 2);
+        for (int c = threadIdx.x; c < 3 * D + 2; c += 256) {
+            // column c of the partial: [0, 2D) d_w_gate, [2D, 3D) d_w_trans, 3D d_b_gate, 3D+1 d_b_trans
+            const int src = c < D ? c : c < 2 * D ? 256 + c - D : c < 3 * D ? 512 + c - 2 * D : 768 + c - 3 * D;
+            float a = red[src];
+            for (int q = 1; q < 8; ++q) a += red[q * RO_ROW + src];
+            out[c] = a;
+        }
+        return;
+    }
 #pragma unroll
     for (int j = 0; j < MAX_D_PER_LANE; ++j) {
         const int d = lane + 32 * j;
@@ -129,6 +169,33 @@ __global__ void __launch_bounds__(256) readout_bwd_kernel(const float* __restric
         if (d_b_gate) atomicAdd(d_b_gate, red[768]);
         if (d_b_trans) atomicAdd(d_b_trans, red[769]);
     }
+}
+__global__ void __launch_bounds__(256) readout_bwd_kernel(const float* __restrict__ h_last, const float* __restrict__ h0, Weights w,
+                                                          const int* __restrict__ graph_of, const float* __restrict__ mask,
+                                                          const float* __restrict__ d_out, float* __restrict__ d_h_last,
+                                                          float* __restrict__ d_w_gate, float* __restrict__ d_b_gate,
+                                                          float* __restrict__ d_w_trans, float* __restrict__ d_b_trans, int V, int D) {
+    readout_bwd<false>(h_last, h0, w, graph_of, mask, d_out, d_h_last, d_w_gate, d_b_gate, d_w_trans, d_b_trans, nullptr, V, D);
+}
+// part: [gridDim.x][3D+2] block partials, reduced by readout_bwd_reduce_kernel
+__global__ void __launch_bounds__(256) readout_bwd_ordered_kernel(const float* __restrict__ h_last, const float* __restrict__ h0, Weights w,
+                                                                  const int* __restrict__ graph_of, const float* __restrict__ mask,
+                                                                  const float* __restrict__ d_out, float* __restrict__ d_h_last,
+                                                                  float* __restrict__ part, int V, int D) {
+    readout_bwd<true>(h_last, h0, w, graph_of, mask, d_out, d_h_last, nullptr, nullptr, nullptr, nullptr, part, V, D);
+}
+// one block per column of the [blocks][3D+2] partials: the blocks added in a fixed order (ggnn::bwd::ordered_column_sum), then once into the
+// caller's gradient (any of the four may be NULL)
+__global__ void __launch_bounds__(256) readout_bwd_reduce_kernel(const float* __restrict__ part, int blocks, int D, float* __restrict__ d_w_gate,
+                                                                 float* __restrict__ d_b_gate, float* __restrict__ d_w_trans,
+                                                                 float* __restrict__ d_b_trans) {
+    __shared__ float s_red[256];
+    const int c = blockIdx.x;
+    float* dst = c < 2 * D ? (d_w_gate ? d_w_gate + c : nullptr) : c < 3 * D ? (d_w_trans ? d_w_trans + c - 2 * D : nullptr)
+                                                                              : c == 3 * D ? d_b_gate : d_b_trans;
+    if (!dst) return;
+    const float a = bwd::ordered_column_sum(part, blocks, 3 * D + 2, c, s_red);
+    if (threadIdx.x == 0) *dst += a;
 }
 
 // Masked regression loss of one task (chem_tensorflow.py:161-166): diff = (computed - target) * mask,

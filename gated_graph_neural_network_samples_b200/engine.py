@@ -434,6 +434,11 @@ class PropagationEngine:
     def set_save_for_backward(self, enable: bool):
         self._check(self.lib.ggnn_set_save_for_backward(self._h, int(bool(enable))))
 
+    def set_deterministic(self, enable: bool):
+        """``ggnn_set_deterministic``: fixed-order weight-gradient and readout sums from the next call on, so that the same inputs give
+        the same bits in every output and gradient (the autograd nodes set it from ``torch.are_deterministic_algorithms_enabled()``)."""
+        self._check(self.lib.ggnn_set_deterministic(self._h, int(bool(enable))))
+
     def backward(self, d_out, grads: Sequence[dict], d_h0=None):
         arr = (_lib.GgnnLayerGrads * len(grads))()
         for l, g in enumerate(grads):

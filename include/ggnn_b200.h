@@ -186,7 +186,8 @@ int ggnn_forward_host_async(ggnn_engine* e, const float* h0_host, float* h_out_h
  *   sparse: graph_nodes_list [V] int32 (sparse:337), node_mask NULL
  *   dense : graph_nodes_list NULL, nodes_per_graph = num_vertices (graph = row / num_vertices), node_mask [b*v] float32 (dense:126)
  * Nodes grouped by graph (what the packers produce) are summed in node order, deterministically, like TF's CPU
- * unsorted_segment_sum; an ungrouped list falls back to float atomics.  All other pointers are DEVICE fp32; `out` is [num_graphs].
+ * unsorted_segment_sum; an ungrouped list falls back to float atomics (with ggnn_set_deterministic on, each graph's nodes are summed in
+ * node order through a stable by-graph permutation built here).  All other pointers are DEVICE fp32; `out` is [num_graphs].
  * ggnn_readout_backward writes d_h_last [V,D] and ACCUMULATES into the weight gradients (caller zeroes; any may be NULL).  The map belongs
  * to the current batch: a graph upload drops it, and the readout calls return GGNN_ESTATE until ggnn_readout_set_graphs runs again. */
 int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* graph_nodes_list, int32_t num_graphs,
@@ -231,6 +232,14 @@ int ggnn_state_dropout_mask(int32_t V, int32_t D, int32_t global_step, float kee
  * Must follow a ggnn_forward on the same graph with save_for_backward enabled.
  * d_h_out: DEVICE [V, D]; grads: per layer, accumulated into; d_h0: DEVICE [V, D] or NULL. */
 int ggnn_set_save_for_backward(ggnn_engine* e, int32_t enable);
+/* Deterministic mode (off by default; GGNN and GCN engines; takes effect from the next call).  With it on, the same engine configuration,
+ * batch, weights, dropout seed and caller buffer contents produce identical bits in every output and every accumulated gradient buffer,
+ * from call to call, engine to engine and process to process.  It governs ggnn_backward, ggnn_gcn_backward, ggnn_readout_forward /
+ * ggnn_readout_backward and ggnn_run_sparse_host_readout: every weight and bias gradient G is summed in a fixed order over row splits that
+ * depend only on the problem's shape (not on the GPU's SM count), and then added once (C <- C + G, as with it off); an ungrouped
+ * graph_nodes_list is summed per graph in node order.  The forward and d h0 are bit-reproducible in either mode.  With it off the weight
+ * gradients and an ungrouped readout sum are added with float atomics, equal only within their ordering noise. */
+int ggnn_set_deterministic(ggnn_engine* e, int32_t enable);
 int ggnn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers,
                   float* d_h0, ggnn_stream_t stream);
 
