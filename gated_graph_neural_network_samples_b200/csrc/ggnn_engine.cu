@@ -30,6 +30,7 @@
 #include "ggnn_fwd_tc.cuh"
 #include "ggnn_fwd_stream.cuh"
 #include "ggnn_gcn.cuh"
+#include "ggnn_tc_smem.h"
 
 using namespace ggnn;
 
@@ -150,6 +151,7 @@ struct BatchPlan {
     int ntiles = 0;
     int max_span = 0;
     int max_tile_msgs = 0;   // largest number of messages whose target lies in one tile
+    int max_tile_types = 0;  // largest number of edge types present in one tile
     std::string plan_text;
     // streaming tensor-core plan (ggnn_fwd_stream.cuh): D > 128, or forced with GGNN_TC_STREAM=1
     bool stream = false;
@@ -1408,11 +1410,11 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     // table and the virtual rows of its range, numbered from the range's offset; then in-degrees / denominators of its nodes.
     std::vector<int>& cursor = g->h_cursor;   // next free slot of every (target, type) row (its own array: the counts of a range's last
     cursor.resize((size_t)V * T + 1);         // row are read by one thread while the next range's thread already writes cursors)
-    int max_tile_msgs = 0;
+    int max_tile_msgs = 0, max_tile_types = 0;
     row_ptr[0] = 0;
     if (vptr) vptr[0] = 0;
 #ifdef _OPENMP
-#pragma omp parallel for schedule(static, 1) num_threads(nth) if (nth > 1) reduction(max : max_tile_msgs)
+#pragma omp parallel for schedule(static, 1) num_threads(nth) if (nth > 1) reduction(max : max_tile_msgs, max_tile_types)
 #endif
     for (int k = 0; k < nth; ++k) {
         int run = (int)part_msgs[k];
@@ -1429,11 +1431,13 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
                 }
             h_mask[i] = mask;
             max_tile_msgs = std::max(max_tile_msgs, run - tile_first);
+            max_tile_types = std::max(max_tile_types, __builtin_popcount(mask));
             h_tiles[i] = tile_start[i];
         }
         if (k == nth - 1) h_tiles[ntiles] = tile_start[ntiles];
     }
     p.max_tile_msgs = max_tile_msgs;
+    p.max_tile_types = max_tile_types;
     lap("row sweep", t_lap);
 #ifdef _OPENMP
 #pragma omp parallel for schedule(static, 1) num_threads(nth) if (nth > 1)
@@ -1816,6 +1820,7 @@ static int build_matrix_image(ggnn_prepared_graph* g, int32_t b, int32_t v, cons
             }
         }
         h_mask[i] = mask;
+        p.max_tile_types = std::max(p.max_tile_types, __builtin_popcount(mask));
     }
     g->valid = true;
     return GGNN_OK;
@@ -1938,26 +1943,21 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
     p.DP = DP;
     p.nparts = e->precision == GGNN_PREC_BF16X3 ? 3 : 1;
     p.kgs = e->tc_kgs;
-    const size_t opb = (size_t)DP * (size_t)p.kgs / 4, stage = (size_t)DP * 128;   // a ring slot = two 64*DP-byte K-step stages
-    const size_t ops = 3 * opb;   // h, agg and the gather / r*h operand tiles
     const size_t avail = e->max_smem > 1024 ? e->max_smem - 1024 : 0;
-    // tile-local sparse graphs: stage the tile's CSR slice in shared memory when it is small enough and leaves the weight ring the two
-    // slots a worker holds at once (one slot's MMAs in flight while the next slot's are issued; DP 128 with 128-row tiles has room for
-    // two slots only without the cache)
-    size_t csr_b = 0;
-    if (e->local && e->gather_mode == GATHER_SPARSE && e->T <= 16 && e->max_tile_msgs <= 4096) {
-        const int cap = (e->max_tile_msgs + 15) / 16 * 16;
-        const size_t b = (size_t)((tc::TILE_M * e->T + 1 + 7) & ~7) * 2 + (size_t)cap;
-        if (avail >= ops + (size_t)3 * DP * sizeof(float) + b + 64 + 2 * stage) {
-            p.csr_cache = 1;
-            p.csr_cap_msgs = cap;
-            csr_b = b;
-        }
-    }
-    const size_t bias_b = (size_t)3 * DP * sizeof(float) + csr_b + 64;
-    if (avail < ops + bias_b + 2 * stage) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the tensor-core tile (DP=%d)", DP);
-    p.nstages = (int)std::min<size_t>(tc::MAX_STAGES, (avail - ops - bias_b) / stage);
-    const size_t smem = ops + bias_b + (size_t)p.nstages * stage;
+    // the shared-memory plan (ggnn_tc_smem.h): the CSR slice of tile-local graphs when it fits beside the two ring slots a worker holds
+    // at once (DP 128 with 128-row tiles has room for two slots only without it), the number of gather tiles (GGNN_TC_GATHER_TILES=<n>
+    // overrides the edge types per tile, clamped to what fits), the ring depth
+    static_assert(tc::TILE_M == 128, "ggnn_tc_smem.h sizes the CSR slice for 128-row tiles");
+    int ng_request = 0;
+    if (const char* g = getenv("GGNN_TC_GATHER_TILES")) ng_request = std::max(2, atoi(g));
+    const TcSmemPlan sp = tc_smem_plan(DP, p.kgs, e->T, e->local, e->gather_mode == GATHER_SPARSE, e->use_bias != 0, e->max_tile_msgs,
+                                       e->max_tile_types, avail, tc::MAX_STAGES, ng_request);
+    if (sp.nstages < 2) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the tensor-core tile (DP=%d)", DP);
+    p.csr_cache = sp.csr_cache;
+    p.csr_cap_msgs = sp.csr_cap_msgs;
+    p.ngather = sp.ngather;
+    p.nstages = sp.nstages;
+    const size_t smem = sp.smem;
     const WeightTiles& wt = e->tc_tiles;
     const uint8_t* wb = (const uint8_t*)wt.buf.ptr;
     for (int l = 0; l < e->L; ++l) {

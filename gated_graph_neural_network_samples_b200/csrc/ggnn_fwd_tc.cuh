@@ -18,10 +18,11 @@
 // tiles (<= 64 rows) all four warpgroups work on rows 0..63 and split the columns four ways instead (COMPACT_WIDTH), so none of them
 // idles on rows that do not exist.  The gathers are row-per-thread over all 16 worker warps.
 //
-// Shared memory: three A-operand tiles (h, agg, A_t / r*h), each hi+lo in the canonical K-major no-swizzle layout
+// Shared memory (ggnn_tc_smem.h): A-operand tiles, each hi+lo in the canonical K-major no-swizzle layout
 //   byte(row, k) = part*PART_B + (k/8)*KGS + row*16 + (k%8)*2     (KGS = 16 * allocated rows: 2048, or 1024 for compact <= 64-row tiles)
-// then a ring of weight slots that the producer thread fills with cp.async.bulk (1-D TMA) from a pre-split, pre-tiled bf16 copy of the
-// weights (every worker warp releases every slot), the biases and the tile's CSR slice.
+// -- h, and p.ngather >= 2 gather tiles (A_t of up to ngather edge types at once; tiles 0 and 1 double as the agg and r*h tiles) --, a
+// ring of weight slots that the producer thread fills with cp.async.bulk (1-D TMA) from a pre-split, pre-tiled bf16 copy of the weights
+// (every worker warp releases every slot), the biases, the tile's per-row constants (compact tiles) and the tile's CSR slice.
 // Every mbarrier wait is bounded; on timeout an error code is written and all roles drain.
 #pragma once
 #include <cuda_bf16.h>
@@ -65,6 +66,7 @@ struct TcParams {
     int gather_mode, dense_v, save;
     int nparts;   // 3: bf16x3 (fp32-accurate), 1: single bf16 MMA
     int nstages;  // weight ring depth
+    int ngather;  // gather tiles (>= 2): the A_t of up to ngather edge types are gathered in one pass, then their MMAs run back to back
     int kgs;            // A-operand k-group stride in bytes: 2048 (128-row tiles) or 1024 (compact: every tile has <= 64 rows)
     int csr_cache;      // LOCAL sparse only: the tile's CSR slice is staged in shared memory (uint16 row offsets, uint8 local sources)
     int csr_cap_msgs;   // capacity of the shared source array
@@ -399,12 +401,19 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
     constexpr uint32_t OPB = 2u * PART_B;                  // bytes per A operand (hi + lo)
     constexpr uint32_t STAGE_B = (uint32_t)DP * 64u;       // bytes per weight stage (K = 16 x N = DP, hi + lo)
     const int D = p.D, T = p.T;
+    constexpr int RA = (int)(KGS / 16u);                   // allocated rows of an A operand
     uint8_t* opH = smem;
-    uint8_t* opX = opH + OPB;
-    uint8_t* opA = opX + OPB;
-    uint8_t* ring = opA + OPB;                                                   // nstages slots of 2*STAGE_B, 1024-byte aligned
-    float* sBias = reinterpret_cast<float*>(ring + (size_t)p.nstages * 2 * STAGE_B);   // [3*DP]: gate r | gate u | cand, zero padded
-    uint16_t* sRowPtr = reinterpret_cast<uint16_t*>(sBias + 3 * DP);              // [128*T + 1] (csr_cache)
+    // compact: h | ring | ngather gather tiles (the producer's ring at a fixed offset); 128-row: h | 2 gather tiles | ring
+    const int ngather = COMPACT ? p.ngather : 2;
+    const size_t ring_b = (size_t)p.nstages * 2 * STAGE_B;
+    uint8_t* ring = opH + (COMPACT ? 1 : 3) * OPB;                               // nstages slots of 2*STAGE_B, 1024-byte aligned
+    uint8_t* opX = COMPACT ? ring + ring_b : opH + OPB;                          // gather tile 0
+    uint8_t* opA = opX + OPB;                                                    // gather tile 1
+    constexpr bool row_cache = COMPACT;                                          // the per-row constants are staged (compact tiles)
+    float* sBias = reinterpret_cast<float*>(COMPACT ? opX + (size_t)ngather * OPB : ring + ring_b);   // [3*DP]: gate r | gate u | cand
+    float* sInvDen = sBias + 3 * DP;                                             // [RA] (row_cache): 1/denominator, 1 without averaging
+    float* sIndeg = sInvDen + RA;                                                // [RA*T] (row_cache, use_bias): in-degree per type
+    uint16_t* sRowPtr = reinterpret_cast<uint16_t*>(sInvDen + (row_cache ? RA * (1 + (p.use_bias ? T : 0)) : 0));   // [128*T + 1] (csr_cache)
     uint8_t* sSrc = reinterpret_cast<uint8_t*>(sRowPtr + ((TILE_M * T + 1 + 7) & ~7)); // [csr_cap_msgs]
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -528,6 +537,12 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
             const int mt = p.row_ptr[(size_t)(row0 + rows) * T] - base;
             for (int i = tid; i < mt; i += NUM_WORKERS) sSrc[i] = (uint8_t)(p.csr_src[base + i] - row0);
         }
+        // the per-row constants of the agg epilogue, read every timestep: staged once (the same expressions as the epilogue's global reads)
+        if (row_cache) {
+            for (int i = tid; i < RA; i += NUM_WORKERS) sInvDen[i] = (p.use_avg && i < rows) ? __fdividef(1.0f, p.denom[row0 + i]) : 1.0f;
+            if (p.use_bias)
+                for (int i = tid; i < RA * T; i += NUM_WORKERS) sIndeg[i] = i < rows * T ? p.indeg[(size_t)row0 * T + i] : 0.0f;
+        }
         publish_sync();
 
         for (int l = l_begin; l < l_end && ok; ++l) {
@@ -568,11 +583,17 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
             }
             for (int s = s_begin; s < s_end && ok; ++s) {
                 const size_t save_base = (size_t)(p.step_base[l] + s) * VD;
-                // ------------------------------------------------------------ gather + G1 per present type
-                // A_t tiles alternate between opA and opX: the gather of type n+1 never overwrites what the MMAs of type n read
+                // ------------------------------------------------------------ gather + G1
+                // Compact tiles: the A_t of a group of present types are gathered into consecutive gather tiles (rotating over the ngather
+                // tiles), published with one barrier, then the group's MMAs run back to back in type order, so acc sums the same products in
+                // the same order as one type at a time.  A tile whose types fit in the gather tiles is one group; otherwise groups of
+                // ngather/2 types, so that a group never overwrites the tiles of the group before it, whose MMAs other warpgroups may still
+                // be issuing.  128-row tiles: one type at a time, A_t alternating between opA and opX (the gather of type n+1 never
+                // overwrites what the MMAs of type n read).
                 float acc[NF];
                 zero(acc);
-                int nty = 0;
+                const int gsz = __popc(tmask) <= ngather ? ngather : ngather / 2;   // (compact)
+                int nty = 0, n = 0, gt = 0, gt0 = 0;   // types gathered; of them in the open group; the next gather tile; the group's first
                 // The gather touches shared memory only, so with compact tiles -- rows 0..63 only -- all 16 worker warps share it:
                 // row group = warp & 1, eight column-chunk groups instead of four.
                 const bool gsplit = KGS == 1024u;
@@ -583,8 +604,11 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                 const int g_nkc = gsplit ? nkc_tile : (((uint32_t)(q * 32) * 16u < KGS) ? nkc_tile : 0);
                 for (int t = 0; t < T && ok; ++t) {
                     if (!((tmask >> t) & 1u)) continue;
-                    uint8_t* gdst = (nty & 1) ? opX : opA;
+                    if (n == 0) gt0 = gt;
+                    uint8_t* gdst = COMPACT ? opX + (size_t)gt * OPB : ((nty & 1) ? opX : opA);
+                    gt = gt + 1 == ngather ? 0 : gt + 1;
                     ++nty;
+                    ++n;
                     int beg = 0, end = 0, dg = 0, di = 0;
                     if (g_row_ok) {
                         if (p.gather_mode == GATHER_SPARSE) {
@@ -663,23 +687,29 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                         }
                         store_operand_chunk(gdst, KGS, PART_B, kc, g_row, a8);
                     }
+                    if (COMPACT && n < gsz && ((tmask >> t) >> 1) != 0) continue;   // the group is open and another type follows
                     publish_sync();
                     if (!ok) break;
-                    gemm_narrow(acc, gdst);
+                    if constexpr (COMPACT) {
+                        for (int k = 0, j = gt0; k < n; ++k, j = (j + 1 == ngather) ? 0 : j + 1) gemm_narrow(acc, opX + (size_t)j * OPB);
+                    } else {
+                        gemm_narrow(acc, gdst);
+                    }
+                    n = 0;
                 }
-                workers_sync();   // every G1 MMA is complete before opX / opA are rewritten
+                workers_sync();   // every G1 MMA is complete before the gather tiles (opX / opA) are rewritten
                 if (!ok) break;
                 // ------------------------------------------------------------ agg epilogue: + indeg.B, / (deg + 1e-7) -> opX
                 GGNN_FRAG_PAIRS({
                     float v0 = acc[fi], v1 = acc[fi + 1];
                     if (p.use_bias && fc < D) {
                         for (int t = 0; t < T; ++t) {
-                            const float ind = p.indeg[(size_t)fg * T + t];
+                            const float ind = row_cache ? sIndeg[fr * T + t] : p.indeg[(size_t)fg * T + t];
                             const float2 b = *reinterpret_cast<const float2*>(ly.edge_b + (size_t)t * D + fc);
                             v0 = fmaf(ind, b.x, v0); v1 = fmaf(ind, b.y, v1);
                         }
                     }
-                    const float inv_den = (p.use_avg && fr < rows) ? __fdividef(1.0f, p.denom[fg]) : 1.0f;
+                    const float inv_den = row_cache ? sInvDen[fr] : (p.use_avg && fr < rows) ? __fdividef(1.0f, p.denom[fg]) : 1.0f;
                     v0 = fr < rows ? v0 * inv_den : 0.0f;
                     v1 = fr < rows ? v1 * inv_den : 0.0f;
                     if (p.save && fok) st2(p.save_buf.agg + save_base + (size_t)fg * D + fc, v0, v1);
