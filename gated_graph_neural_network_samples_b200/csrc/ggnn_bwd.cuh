@@ -377,7 +377,7 @@ __global__ void add_inplace_kernel(float* __restrict__ dst, const float* __restr
 // ---------------------------------------------------------------- gathers, all edge types in one launch (one warp per node):
 //   out[v, t*D + :] = sum_{slots of row (v*T+t)} in[idx[slot], :]        out is [V, T*D]
 // blockIdx.y = 0: A_t from the target-keyed CSR over the states; 1: G_t from the source-keyed CSR over dx'.
-// w (optional): per-slot weight (the attention probability), looked up as w[widx ? widx[slot] : slot]
+// w (optional): per-slot weight (the attention probability, or the entry of a weighted adjacency), looked up as w[widx ? widx[slot] : slot]
 struct GatherJob { const int* row_ptr; const int* idx; const float* in; float* out; const float* w; const int* widx; };
 __global__ void __launch_bounds__(256) csr_gather_all_kernel(GatherJob j0, GatherJob j1, int V, int D, int T) {
     const GatherJob jb = blockIdx.y == 0 ? j0 : j1;
@@ -512,25 +512,5 @@ __global__ void __launch_bounds__(256) attention_bwd_source_kernel(const int* __
         *o = cur;
     }
 }
-// dense adjacency [b][T][v][v]: out[g*nv+i] = sum_j A[g,t,i,j] in[g*nv+j]   (transpose: sum_j A[g,t,j,i] in[g*nv+j])
-__global__ void __launch_bounds__(256) dense_gather_sum_kernel(const float* __restrict__ adj, const float* __restrict__ in, float* __restrict__ out,
-                                                               int ldo, int V, int D, int T, int t, int nv, int transpose) {
-    const int v = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (v >= V) return;
-    const int g = v / nv, i = v - g * nv;
-    const float* base = adj + ((size_t)g * T + t) * nv * nv;
-    for (int c4 = lane; c4 < (D >> 2); c4 += 32) {
-        float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (int j = 0; j < nv; ++j) {
-            const float a = transpose ? base[(size_t)j * nv + i] : base[(size_t)i * nv + j];
-            if (a != 0.0f) {
-                const float4 x = *reinterpret_cast<const float4*>(in + (size_t)(g * nv + j) * D + (c4 << 2));
-                s.x = fmaf(a, x.x, s.x); s.y = fmaf(a, x.y, s.y); s.z = fmaf(a, x.z, s.z); s.w = fmaf(a, x.w, s.w);
-            }
-        }
-        *reinterpret_cast<float4*>(out + (size_t)v * ldo + (c4 << 2)) = s;
-    }
-}
-
 }  // namespace bwd
 }  // namespace ggnn

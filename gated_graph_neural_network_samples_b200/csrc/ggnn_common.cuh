@@ -11,7 +11,6 @@ constexpr int KC = 16;         // K rows of a weight operand per shared-memory s
 
 enum { CELL_GRU = 0, CELL_RNN = 1, CELL_CUDNN_GRU = 2 };
 enum { ACT_TANH = 0, ACT_RELU = 1 };
-enum { GATHER_SPARSE = 0, GATHER_DENSE = 1 };
 
 struct LayerDev {
     const float* edge_w;   // [T][D][D]
@@ -40,14 +39,12 @@ struct SaveDev {
 struct FwdParams {
     int V, D, T, L;
     int use_bias, use_avg, cell, act;
-    int gather_mode;          // GATHER_SPARSE / GATHER_DENSE
-    int dense_v;              // vertices per graph (dense)
     int save;                 // keep activations for backward
     const int* tile_start;    // [ntiles+1] first node of each tile
     const unsigned* tile_mask;// [ntiles] bit t set iff some node of the tile has an incoming type-t message
     const int* row_ptr;       // [V*T+1] CSR rows keyed target*T+type (stable in message order)
     const int* csr_src;       // [M] source node of each CSR slot
-    const float* dense_adj;   // [b][T][v][v]
+    const float* slot_w;      // [M] weight of each CSR slot (weighted dense adjacency), or nullptr
     const float* indeg;       // [V][T] num_incoming_edges_per_type
     const float* denom;       // [V] fp32(sum_t indeg) + 1e-7f
     const float* state[MAX_LAYERS + 1];   // node_states_per_layer: [0]=h0 ... [L]=result (read side)

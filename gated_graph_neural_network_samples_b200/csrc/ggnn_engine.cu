@@ -141,9 +141,8 @@ struct ModelShape {
 
 // What build_plan and the image builders derive from one batch: the tile plan and the layout of the graph image.
 struct BatchPlan {
-    int gather_mode = GATHER_SPARSE;
-    bool weighted = false;   // every message has a weight (GCN): the image carries the slot weights
-    int V = 0, dense_v = 0;
+    bool weighted = false;   // every message has a weight (GCN, weighted dense adjacency): the image carries the slot weights
+    int V = 0;
     int64_t M = 0;
     int variant = 0;  // 0: RG=8,CS=1 (64-row tiles)   1: RG=4,CS=2 (32-row tiles)
     int nb1 = 0;
@@ -158,8 +157,8 @@ struct BatchPlan {
     int ts_nc[2] = {0, 0}, ts_nblk[2] = {0, 0};      // [0]: DP-wide outputs (agg, candidate)  [1]: the 2*DP-wide gate output
     int ts_nv = 0;                                   // number of virtual rows of the current batch
     int tc_row_budget = 128, tc_kgs = 2048;   // tensor-core plan: no tile has more rows than the budget; <= 64 selects compact operand tiles
-    // the graph image: row_ptr | csr_src | csr_msg | indeg | denom | tile_start | tile_mask | (dense adj) | ...
-    size_t off_row_ptr = 0, off_src = 0, off_msg = 0, off_indeg = 0, off_denom = 0, off_tiles = 0, off_mask = 0, off_adj = 0;
+    // the graph image: row_ptr | csr_src | csr_msg | indeg | denom | tile_start | tile_mask | ...
+    size_t off_row_ptr = 0, off_src = 0, off_msg = 0, off_indeg = 0, off_denom = 0, off_tiles = 0, off_mask = 0;
     size_t off_trow = 0, off_ttgt = 0;   // source-keyed CSR (rows source*T+type -> targets), built when save_for_backward is on
     bool has_transpose = false;
     size_t off_tslot = 0;            // source-keyed CSR entry -> target-CSR slot (attention backward)
@@ -174,11 +173,10 @@ struct GraphDev {
     const float *indeg, *denom;
     const int* tile_start;
     const unsigned* tile_mask;
-    const float* dense_adj;
     const int *trow, *ttgt, *tslot;                      // source-keyed CSR (save_for_backward)
     const int *pair_src, *vrow_ptr, *vsrc, *tile_vptr;   // streaming plan
     const int4* vinfo;
-    const float *slot_w, *tslot_w;                       // GCN: per-slot adjacency weights
+    const float *slot_w, *tslot_w;                       // weighted batches: per-slot adjacency weights
 };
 
 // The weights in the pre-split, pre-tiled bf16 layout of one tensor-core kernel family, with each layer's offsets.  The tiles are rebuilt
@@ -244,7 +242,7 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
 };
 
 // The host half of ggnn_set_graph_*: the model shape goes in, the batch plan and the packed image (CSR, in-degrees, tiles, streaming
-// tables, or a weighted dense matrix) come out; nothing here touches the device but the pinned image.  Built by a producer thread,
+// tables, the slot weights of a weighted batch) come out; nothing here touches the device but the pinned image.  Built by a producer thread,
 // uploaded by the engine's thread (ggnn_set_graph_prepared) -- the ThreadedIterator overlap of the reference's training loop
 // (chem_tensorflow.py:225, utils.py:16-36).
 struct ggnn_prepared_graph : ErrorText {
@@ -304,11 +302,11 @@ static void fill_common_params(const ggnn_engine* e, Params& p, const float* h0,
     memset(&p, 0, sizeof p);
     p.V = e->V; p.D = e->D; p.T = e->T; p.L = e->L;
     p.use_bias = e->use_bias; p.use_avg = e->use_avg; p.cell = e->cell; p.act = e->act;
-    p.gather_mode = e->gather_mode; p.dense_v = e->dense_v; p.save = e->save ? 1 : 0;
+    p.save = e->save ? 1 : 0;
     p.drop_keep = e->drop_keep; p.drop_seed = e->drop_seed;
     const GraphDev& gd = e->gd;
     p.tile_start = gd.tile_start; p.tile_mask = gd.tile_mask; p.row_ptr = gd.row_ptr; p.csr_src = gd.csr_src;
-    p.dense_adj = gd.dense_adj; p.indeg = gd.indeg; p.denom = gd.denom;
+    p.slot_w = e->weighted ? gd.slot_w : nullptr; p.indeg = gd.indeg; p.denom = gd.denom;
     set_layer_states(e, p, h0, h_out);
     p.save_buf = saved_step(e, 0);   // the kernels index it by global step
     for (int l = 0; l < e->L; ++l) {
@@ -484,12 +482,13 @@ int pack_to_fill_chip(const std::vector<int>& cuts, int V, int max_span, int num
 }
 
 // The tile plan of a batch of V nodes: which kernel, and the tiles.  `cuts` are the sorted node indices where the batch may be split
-// between connected components (cuts.front() == 0, cuts.back() == V).  Starts `p` afresh; the image builders fill in the rest.
-int build_plan(const ModelShape& s, int V, int gather_mode, const std::vector<int>& cuts, BatchPlan& p, std::vector<int>& tile_start,
+// between connected components (cuts.front() == 0, cuts.back() == V); `weighted`: every message has a weight.  Starts `p` afresh; the image
+// builders fill in the rest.
+int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>& cuts, BatchPlan& p, std::vector<int>& tile_start,
                std::string& err) {
     p = BatchPlan();
     p.V = V;
-    p.gather_mode = gather_mode;
+    p.weighted = weighted;
     int max_span = 0;
     for (size_t i = 1; i < cuts.size(); ++i) max_span = std::max(max_span, cuts[i] - cuts[i - 1]);
     p.max_span = max_span;
@@ -517,13 +516,14 @@ int build_plan(const ModelShape& s, int V, int gather_mode, const std::vector<in
     } else if (s.precision != GGNN_PREC_FP32) {
         const char* fs = getenv("GGNN_TC_STREAM");
         // a component larger than a tile cannot use the tile-local fused kernel: the streaming plan beats one launch per timestep of that
-        // kernel (cfg5 on an H100: 0.77 vs 0.94 ms), so it is the default there; GGNN_TC_STREAM=0/1 and GGNN_FORCE_GLOBAL=1 override
-        const bool big_component = max_span > tc::TILE_M && gather_mode == GATHER_SPARSE && !force_global && !(fs && fs[0] == '0');
-        if (s.DP > 128 || big_component || (fs && fs[0] == '1' && gather_mode == GATHER_SPARSE)) {
+        // kernel (cfg5 on an H100: 0.77 vs 0.94 ms), so it is the default there; GGNN_TC_STREAM=0/1 and GGNN_FORCE_GLOBAL=1 override.
+        // The streaming kernels sum unweighted messages only: a weighted batch stays on the tile kernel.
+        const bool big_component = max_span > tc::TILE_M && !weighted && !force_global && !(fs && fs[0] == '0');
+        if (s.DP > 128 || big_component || (fs && fs[0] == '1' && !weighted)) {
             // streaming plan: fixed 128-row tiles (the gather reads the previous state from L2, so tiles need not respect components),
             // one launch per GEMM of a timestep; N blocks sized so that small batches still spread over the chip
-            if (gather_mode != GATHER_SPARSE) {
-                err = "hidden_size > 128 on the tensor-core path needs the CSR graph format (a weighted dense adjacency runs on GGNN_PREC_FP32)";
+            if (weighted) {
+                err = "hidden_size > 128 on the tensor-core path needs unweighted messages (a weighted dense adjacency runs on GGNN_PREC_FP32)";
                 return GGNN_EUNSUPPORTED;
             }
             p.stream = true; p.variant = 3;
@@ -837,34 +837,30 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
                 ++e->last_launches;
             }
             // ---- messages: all edge types at once.  At[v, t*D..] = sum of h over the type-t sources of v, Gt[s, t*D..] = sum of dx' over
-            // the type-t targets of s
-            if (e->gather_mode == GATHER_SPARSE) {
-                const float* alpha = nullptr;
-                if (e->use_att) {   // softmax backward first (it adds to dh_new), then the gathers are weighted by the probabilities
-                    alpha = (const float*)e->att_buf.ptr + (size_t)(e->step_base[l] + s) * (size_t)std::max<int64_t>(e->M, 1);
-                    gemm_nt(false, dxp, D, 0, w.edge_weights, D, 0, 1, Pall, TD, V, TD, D);   // P[v, t*D+k] = <dx'[v], W_t[k, :]>
-                    if (e->det && gw.edge_type_attention_weights) {   // per-block d a_t into ws, then added over the blocks in a fixed order
-                        attention_bwd_target_ordered_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, Pall, alpha,
-                                                                                          w.edge_type_attention_weights, dsa, dh_new, ws, V, D, T);
-                        ordered_colsum_kernel<<<T, 256, 0, st>>>(ws, nodes_blocks, T, gw.edge_type_attention_weights);
-                        ++e->last_launches;
-                    } else {
-                        attention_bwd_target_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, Pall, alpha, w.edge_type_attention_weights,
-                                                                                  dsa, dh_new, gw.edge_type_attention_weights, V, D, T);
-                    }
-                    attention_bwd_source_kernel<<<nodes_blocks, 256, 0, st>>>(gd.trow, gd.ttgt, gd.tslot, h, dsa, dh_new, V, D, T);
-                    e->last_launches += 2;
+            // the type-t targets of s.  A weighted batch weights both by the adjacency entry of the slot.
+            GatherJob j0{gd.row_ptr, gd.csr_src, h, At, nullptr, nullptr}, j1{gd.trow, gd.ttgt, dxp, Gt, nullptr, nullptr};
+            if (e->use_att) {   // softmax backward first (it adds to dh_new), then the gathers are weighted by the probabilities
+                const float* alpha = (const float*)e->att_buf.ptr + (size_t)(e->step_base[l] + s) * (size_t)std::max<int64_t>(e->M, 1);
+                gemm_nt(false, dxp, D, 0, w.edge_weights, D, 0, 1, Pall, TD, V, TD, D);   // P[v, t*D+k] = <dx'[v], W_t[k, :]>
+                if (e->det && gw.edge_type_attention_weights) {   // per-block d a_t into ws, then added over the blocks in a fixed order
+                    attention_bwd_target_ordered_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, Pall, alpha,
+                                                                                      w.edge_type_attention_weights, dsa, dh_new, ws, V, D, T);
+                    ordered_colsum_kernel<<<T, 256, 0, st>>>(ws, nodes_blocks, T, gw.edge_type_attention_weights);
+                    ++e->last_launches;
+                } else {
+                    attention_bwd_target_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, Pall, alpha, w.edge_type_attention_weights,
+                                                                              dsa, dh_new, gw.edge_type_attention_weights, V, D, T);
                 }
-                GatherJob j0{gd.row_ptr, gd.csr_src, h, At, alpha, nullptr}, j1{gd.trow, gd.ttgt, dxp, Gt, alpha, alpha ? gd.tslot : nullptr};
-                csr_gather_all_kernel<<<dim3(nodes_blocks, 2), 256, 0, st>>>(j0, j1, V, D, T);
-                ++e->last_launches;
-            } else {
-                for (int t = 0; t < T; ++t) {
-                    dense_gather_sum_kernel<<<nodes_blocks, 256, 0, st>>>(gd.dense_adj, h, At + (size_t)t * D, TD, V, D, T, t, e->dense_v, 0);
-                    dense_gather_sum_kernel<<<nodes_blocks, 256, 0, st>>>(gd.dense_adj, dxp, Gt + (size_t)t * D, TD, V, D, T, t, e->dense_v, 1);
-                    e->last_launches += 2;
-                }
+                attention_bwd_source_kernel<<<nodes_blocks, 256, 0, st>>>(gd.trow, gd.ttgt, gd.tslot, h, dsa, dh_new, V, D, T);
+                e->last_launches += 2;
+                j0.w = j1.w = alpha;
+                j1.widx = gd.tslot;
+            } else if (e->weighted) {
+                j0.w = gd.slot_w;
+                j1.w = gd.tslot_w;
             }
+            csr_gather_all_kernel<<<dim3(nodes_blocks, 2), 256, 0, st>>>(j0, j1, V, D, T);
+            ++e->last_launches;
             if (e->use_bias && gw.edge_biases) {   // dB[t,:] += sum_v indeg[v,t] dx'[v,:]  =  indeg^T . dx'
                 SegList sl;
                 memset(&sl, 0, sizeof sl);
@@ -1107,7 +1103,7 @@ int ggnn_host_tile_plan(int32_t hidden_size, int32_t num_edge_types, int32_t pre
     BatchPlan p;
     std::string err;
     std::vector<int> ts;
-    int rc = build_plan(s, V, GATHER_SPARSE, cuts, p, ts, err);
+    int rc = build_plan(s, V, false, cuts, p, ts, err);
     if (rc) return rc;
     *num_tiles = p.ntiles;
     if ((int)ts.size() > tile_capacity) return GGNN_EINVAL;
@@ -1323,10 +1319,9 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     find_cuts(need_cuts ? reach.data() : nullptr, V, cuts);
     lap("validate+count", t_lap);
     std::vector<int> tile_start;
-    int rc = build_plan(shape, V, GATHER_SPARSE, cuts, p, tile_start, g->err);
+    int rc = build_plan(shape, V, weighted, cuts, p, tile_start, g->err);
     if (rc) return rc;
     p.M = M;
-    p.weighted = weighted;
     const int ntiles = p.ntiles;
     lap("tile plan", t_lap);
     nth = std::max(1, std::min(nth, ntiles));
@@ -1363,7 +1358,6 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     p.off_denom = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
     p.off_tiles = off;   off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
     p.off_mask = off;    off = align_up(off + sizeof(unsigned) * (size_t)std::max(ntiles, 1), 16);
-    p.off_adj = off;
     p.has_transpose = g->save;
     if (p.has_transpose) {
         p.off_trow = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
@@ -1661,7 +1655,6 @@ int ggnn_set_graph_prepared(ggnn_engine* e, ggnn_prepared_graph* g, ggnn_stream_
     d.row_ptr = (const int*)(b + e->off_row_ptr); d.csr_src = (const int*)(b + e->off_src); d.csr_msg = (const int*)(b + e->off_msg);
     d.indeg = (const float*)(b + e->off_indeg); d.denom = (const float*)(b + e->off_denom);
     d.tile_start = (const int*)(b + e->off_tiles); d.tile_mask = (const unsigned*)(b + e->off_mask);
-    d.dense_adj = (const float*)(b + e->off_adj);
     d.trow = (const int*)(b + e->off_trow); d.ttgt = (const int*)(b + e->off_ttgt); d.tslot = (const int*)(b + e->off_tslot);
     d.pair_src = (const int*)(b + e->off_pair); d.vrow_ptr = (const int*)(b + e->off_vptr); d.vsrc = (const int*)(b + e->off_vsrc);
     d.tile_vptr = (const int*)(b + e->off_tvp); d.vinfo = (const int4*)(b + e->off_vinfo);
@@ -1680,18 +1673,19 @@ int ggnn_set_graph_sparse(ggnn_engine* e, int32_t V, const int32_t* const* adj, 
 }
 
 
-// The reference only ever feeds 0/1 adjacency (dense:30-36).  A binary adjacency IS an edge list: A_t.(h W_t + b_t) =
-// (sum of h over the row's sources) W_t + rowsum(A_t) b_t, which is exactly the sparse path with in-degree = row sums.  One scan of
-// [b, T, v, v] -> per-type (source, target) lists in the order (graph, target row, source column) and the row sums; false when an entry is
-// neither 0 nor 1 (a weighted matrix keeps the matrix walk).
+// The reference only ever feeds 0/1 adjacency (dense:30-36).  An adjacency IS a list of weighted messages: A_t.(h W_t + b_t) =
+// (sum of A_t[i,j] h_j over the row's sources j) W_t + rowsum(A_t) b_t, which is the CSR path with one weight per message and in-degree =
+// row sums (dense:107-112 adds the bias to every source row before A.m).  One scan of [b, T, v, v] -> per-type (source, target) lists and
+// their matrix entries in the order (graph, target row, source column), and the fp32 row sums in column order (the zero entries add
+// nothing); returns whether some nonzero entry differs from 1.  `weights` is filled, in the type-major message order, only then.
 // The scan is a stream over b*T*v*v floats (4 MB at cfg3) of which ~99 % are zero: memory-bound on one core (~0.5 ms), so the
 // graphs are split into contiguous ranges over a few OpenMP threads; every thread appends to its own per-type lists (order inside
 // a range: graph, target row, source column) and the ranges are concatenated in order -- the result is the single-thread list.
-static bool scan_binary_dense(int T, int b, int v, const float* adjm, std::vector<std::vector<int32_t>>& lists, std::vector<float>& indeg) {
+static bool scan_dense(int T, int b, int v, const float* adjm, std::vector<std::vector<int32_t>>& lists, std::vector<float>& weights,
+                       std::vector<float>& indeg) {
     const int V = b * v;
-    bool binary = true;
     lists.assign(T, std::vector<int32_t>());
-    {
+    weights.clear();
     indeg.assign((size_t)std::max(V, 1) * T, 0.0f);
     int nthreads = 1;   // graph ranges scanned concurrently
     int team = 1;       // OpenMP team size: ONE size per process (the sparse builder's), used only if its region entry is cheap here
@@ -1702,151 +1696,84 @@ static bool scan_binary_dense(int T, int b, int v, const float* adjm, std::vecto
     if (const char* nt = getenv("GGNN_HOST_THREADS")) { nthreads = std::max(1, std::min(atoi(nt), std::max(b, 1))); team = nthreads; }
 #endif
     std::vector<std::vector<std::vector<int32_t>>> part(nthreads, std::vector<std::vector<int32_t>>(T));
-    std::vector<int> bad(nthreads, 0);
+    std::vector<std::vector<std::vector<float>>> part_w(nthreads, std::vector<std::vector<float>>(T));
+    std::vector<int> part_weighted(nthreads, 0);
     const int chunk = (b + nthreads - 1) / std::max(nthreads, 1);
 #ifdef _OPENMP
 #pragma omp parallel for schedule(static, 1) num_threads(team) if (team > 1)
 #endif
     for (int k = 0; k < nthreads; ++k) {
-        std::vector<std::vector<int32_t>>& mine = part[k];
         const int g0 = k * chunk, g1 = std::min(b, g0 + chunk);
-        for (int t = 0; t < T; ++t) mine[t].reserve((size_t)std::max(g1 - g0, 0) * v * 3);
-        bool ok = true;
-        for (int g = g0; g < g1 && ok; ++g)
-            for (int t = 0; t < T && ok; ++t) {
+        for (int t = 0; t < T; ++t) {
+            part[k][t].reserve((size_t)std::max(g1 - g0, 0) * v * 3);
+            part_w[k][t].reserve((size_t)std::max(g1 - g0, 0) * v * 3 / 2);
+        }
+        bool weighted = false;
+        for (int g = g0; g < g1; ++g)
+            for (int t = 0; t < T; ++t) {
                 const float* m = adjm + ((size_t)g * T + t) * v * v;
-                std::vector<int32_t>& lst = mine[t];
-                for (int i = 0; i < v && ok; ++i) {
+                std::vector<int32_t>& lst = part[k][t];
+                std::vector<float>& wl = part_w[k][t];
+                for (int i = 0; i < v; ++i) {
                     const float* row = m + (size_t)i * v;
-                    int cnt = 0;
+                    float sum = 0.0f;
                     auto visit = [&](int j) {
                         const float a = row[j];
                         if (a != 0.0f) {
-                            if (a != 1.0f) { ok = false; return; }
                             lst.push_back(g * v + j);   // source
                             lst.push_back(g * v + i);   // target
-                            ++cnt;
+                            wl.push_back(a);
+                            sum += a;
+                            weighted |= a != 1.0f;
                         }
                     };
                     int j = 0;
-                    for (; j + 4 <= v && ok; j += 4) {   // test 16 bytes at a time
+                    for (; j + 4 <= v; j += 4) {   // test 16 bytes at a time
                         uint64_t w0, w1;
                         memcpy(&w0, row + j, 8); memcpy(&w1, row + j + 2, 8);
                         if ((w0 | w1) == 0) continue;
                         visit(j); visit(j + 1); visit(j + 2); visit(j + 3);
                     }
-                    for (; j < v && ok; ++j) visit(j);
-                    indeg[((size_t)g * v + i) * T + t] = (float)cnt;
+                    for (; j < v; ++j) visit(j);
+                    indeg[((size_t)g * v + i) * T + t] = sum;
                 }
             }
-        bad[k] = ok ? 0 : 1;
+        part_weighted[k] = weighted ? 1 : 0;
     }
-    for (int k = 0; k < nthreads; ++k) binary = binary && !bad[k];
-    if (binary)
-        for (int t = 0; t < T; ++t) {
-            size_t total = 0;
-            for (int k = 0; k < nthreads; ++k) total += part[k][t].size();
-            lists[t].resize(total);
-            size_t off = 0;
-            for (int k = 0; k < nthreads; ++k) {
-                if (!part[k][t].empty()) memcpy(lists[t].data() + off, part[k][t].data(), part[k][t].size() * sizeof(int32_t));
-                off += part[k][t].size();
-            }
+    const bool weighted = std::find(part_weighted.begin(), part_weighted.end(), 1) != part_weighted.end();
+    for (int t = 0; t < T; ++t) {
+        size_t total = 0;
+        for (int k = 0; k < nthreads; ++k) total += part[k][t].size();
+        lists[t].resize(total);
+        size_t off = 0;
+        for (int k = 0; k < nthreads; ++k) {
+            if (!part[k][t].empty()) memcpy(lists[t].data() + off, part[k][t].data(), part[k][t].size() * sizeof(int32_t));
+            off += part[k][t].size();
+            if (weighted) weights.insert(weights.end(), part_w[k][t].begin(), part_w[k][t].end());
         }
     }
-    return binary;
+    return weighted;
 }
 
-// Host half of ggnn_set_graph_dense for a weighted matrix (or any matrix under GGNN_DENSE_KEEP_MATRIX): the kernels walk the matrix
-// itself (GATHER_DENSE), so the image carries it along with the row-sum in-degrees, the denominators and the tiles.
-static int build_matrix_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const float* adjm) {
-    BatchPlan& p = g->plan;
-    const int T = g->shape.T, V = b * v;
-    std::vector<int> cuts;
-    for (int i = 0; i <= b; ++i) cuts.push_back(i * v);
-    std::vector<int> tile_start;
-    int rc = build_plan(g->shape, V, GATHER_DENSE, cuts, p, tile_start, g->err);
-    if (rc) return rc;
-    p.dense_v = v;
-    p.has_transpose = true;   // the dense adjacency is its own transpose source
-    const int ntiles = p.ntiles;
-    const size_t adj_elems = (size_t)b * T * v * v;
-    size_t off = 0;
-    p.off_row_ptr = off; off = align_up(off + 16, 16);
-    p.off_src = off; p.off_msg = off;
-    p.off_indeg = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1) * T, 16);
-    p.off_denom = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
-    p.off_tiles = off;   off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
-    p.off_mask = off;    off = align_up(off + sizeof(unsigned) * (size_t)std::max(ntiles, 1), 16);
-    p.off_adj = off;     off = align_up(off + sizeof(float) * std::max<size_t>(adj_elems, 1), 16);
-    CU_TRY(g, g->image.begin(off));
-    g->bytes = off;
-    char* base = g->image.ptr;
-    float* h_indeg = (float*)(base + p.off_indeg);
-    float* h_denom = (float*)(base + p.off_denom);
-    int* h_tiles = (int*)(base + p.off_tiles);
-    unsigned* h_mask = (unsigned*)(base + p.off_mask);
-    float* h_adj = (float*)(base + p.off_adj);
-    if (adj_elems) memcpy(h_adj, adjm, sizeof(float) * adj_elems);
-    // in-degree per type = row sums of A_t (the dense model adds the bias to every source row before A.m,
-    // dense:107-112, which equals bias * row-sum after the adjacency product)
-    for (int gi = 0; gi < b; ++gi)
-        for (int i = 0; i < v; ++i) {
-            float tot = 0.0f;
-            for (int t = 0; t < T; ++t) {
-                const float* row = adjm + (((size_t)gi * T + t) * v + i) * v;
-                float s = 0.0f;
-                for (int j = 0; j < v; ++j) s += row[j];
-                h_indeg[((size_t)gi * v + i) * T + t] = s;
-                tot += s;
-            }
-            h_denom[(size_t)gi * v + i] = tot + 1e-7f;
-        }
-    for (int i = 0; i <= ntiles; ++i) h_tiles[i] = tile_start[i];
-    for (int i = 0; i < ntiles; ++i) {
-        unsigned mask = 0;
-        for (int n = tile_start[i]; n < tile_start[i + 1]; ++n)
-            for (int t = 0; t < T; ++t)
-                if (h_indeg[(size_t)n * T + t] != 0.0f) mask |= 1u << t;
-        // rows with cancelling +/- entries would have zero row-sum but non-zero entries: scan those rows fully
-        if (mask != ((T >= 32) ? 0xffffffffu : ((1u << T) - 1u))) {
-            for (int n = tile_start[i]; n < tile_start[i + 1]; ++n) {
-                const int gi = n / v, ii = n % v;
-                for (int t = 0; t < T; ++t) {
-                    if (mask & (1u << t)) continue;
-                    const float* row = adjm + (((size_t)gi * T + t) * v + ii) * v;
-                    for (int j = 0; j < v; ++j) if (row[j] != 0.0f) { mask |= 1u << t; break; }
-                }
-            }
-        }
-        h_mask[i] = mask;
-        p.max_tile_types = std::max(p.max_tile_types, __builtin_popcount(mask));
-    }
-    g->valid = true;
-    return GGNN_OK;
-}
-
-// Host half of ggnn_set_graph_dense: a 0/1 adjacency is scanned to edge lists for the sparse builder; a weighted matrix (and any matrix
-// under GGNN_DENSE_KEEP_MATRIX) goes to the matrix builder when `matrix_ok`, else it is refused with GGNN_EUNSUPPORTED.
-static int build_dense_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const float* adjm, bool matrix_ok) {
+// Host half of ggnn_set_graph_dense: the matrix is scanned to message lists for the CSR builder.  A 0/1 matrix builds the image of its
+// edge lists; a weighted one (when `weighted_ok`, else it is refused with GGNN_EUNSUPPORTED) also carries its entries as slot weights.
+static int build_dense_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const float* adjm, bool weighted_ok) {
     g->valid = false;
     if (b < 0 || v <= 0 || (!adjm && b > 0)) return g->fail(GGNN_EINVAL, "null/negative argument");
     if (g->shape.use_att) return g->fail(GGNN_EUNSUPPORTED, "propagation attention exists only in the sparse model (sparse:170-196)");
     const int T = g->shape.T;
     if ((int64_t)b * v > 0x7fffffff / std::max(T, 1)) return g->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
     std::vector<std::vector<int32_t>> lists;
-    std::vector<float> indeg;
-    if (getenv("GGNN_DENSE_KEEP_MATRIX") || !scan_binary_dense(T, b, v, adjm, lists, indeg)) {
-        if (matrix_ok) return build_matrix_image(g, b, v, adjm);
-        return g->fail(GGNN_EUNSUPPORTED, "the adjacency matrix is not 0/1: a weighted matrix is fed through ggnn_set_graph_dense (matrix walk)");
-    }
+    std::vector<float> weights, indeg;
+    const bool weighted = scan_dense(T, b, v, adjm, lists, weights, indeg);
+    if (weighted && !weighted_ok)
+        return g->fail(GGNN_EUNSUPPORTED, "the adjacency matrix is not 0/1: a weighted matrix is fed through ggnn_set_graph_dense");
     std::vector<const int32_t*> ptrs(T);
     std::vector<int32_t> counts(T);
     for (int t = 0; t < T; ++t) { ptrs[t] = lists[t].data(); counts[t] = (int32_t)(lists[t].size() / 2); }
-    int rc = build_sparse_image(g, b * v, ptrs.data(), counts.data(), indeg.data(), false, nullptr);
+    int rc = build_sparse_image(g, b * v, ptrs.data(), counts.data(), indeg.data(), weighted, weights.data());
     if (rc) return rc;
-    g->plan.dense_v = v;
-    g->plan.plan_text += " [binary dense adjacency -> CSR]";
+    g->plan.plan_text += weighted ? " [weighted dense adjacency -> weighted CSR]" : " [binary dense adjacency -> CSR]";
     return GGNN_OK;
 }
 
@@ -1873,10 +1800,8 @@ int ggnn_set_graph_dense(ggnn_engine* e, int32_t b, int32_t v, const float* adjm
 // ------------------------------------------------------------------------------------------ forward drivers (host)
 // fp32 CUDA-core path (ggnn_fwd_ffma.cuh); the only one with propagation attention and CudnnCompatibleGRUCell.
 static int forward_ffma(ggnn_engine* e, const float* h0, float* h_out, cudaStream_t st) {
-    if (e->use_att) {
-        if (e->gather_mode != GATHER_SPARSE) return e->fail(GGNN_EUNSUPPORTED, "propagation attention needs the sparse graph format");
+    if (e->use_att)
         CU_TRY(e, e->att_buf.reserve(sizeof(float) * (size_t)std::max<int64_t>(e->M, 1) * (size_t)(e->save ? std::max(e->total_steps, 1) : 1)));
-    }
     FwdParams p;
     fill_common_params(e, p, h0, h_out);
     p.use_att = e->use_att; p.att = (float*)e->att_buf.ptr; p.att_stride = e->save ? (size_t)std::max<int64_t>(e->M, 1) : 0;
@@ -1950,7 +1875,7 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
     static_assert(tc::TILE_M == 128, "ggnn_tc_smem.h sizes the CSR slice for 128-row tiles");
     int ng_request = 0;
     if (const char* g = getenv("GGNN_TC_GATHER_TILES")) ng_request = std::max(2, atoi(g));
-    const TcSmemPlan sp = tc_smem_plan(DP, p.kgs, e->T, e->local, e->gather_mode == GATHER_SPARSE, e->use_bias != 0, e->max_tile_msgs,
+    const TcSmemPlan sp = tc_smem_plan(DP, p.kgs, e->T, e->local, !e->weighted, e->use_bias != 0, e->max_tile_msgs,
                                        e->max_tile_types, avail, tc::MAX_STAGES, ng_request);
     if (sp.nstages < 2) return e->fail(GGNN_EUNSUPPORTED, "not enough shared memory for the tensor-core tile (DP=%d)", DP);
     p.csr_cache = sp.csr_cache;
@@ -2648,7 +2573,7 @@ int ggnn_num_messages(const ggnn_engine* e, int64_t* out) {
 
 int ggnn_get_csr(ggnn_engine* e, int32_t* row_ptr, int32_t* src, int32_t* msg) {
     if (!e) return GGNN_EINVAL;
-    if (!e->graph_set || e->gather_mode != GATHER_SPARSE) return e->fail(GGNN_ESTATE, "no sparse graph set");
+    if (!e->graph_set) return e->fail(GGNN_ESTATE, "no graph set");
     CU_TRY(e, cudaSetDevice(e->device));
     CU_TRY(e, cudaDeviceSynchronize());
     if (row_ptr) CU_TRY(e, cudaMemcpy(row_ptr, e->gd.row_ptr, sizeof(int) * ((size_t)e->V * e->T + 1), cudaMemcpyDeviceToHost));

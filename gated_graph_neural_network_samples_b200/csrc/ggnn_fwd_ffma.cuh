@@ -234,51 +234,33 @@ __global__ void __launch_bounds__(RG * CS * 32, MINB) ggnn_fwd_ffma_kernel(const
                 }
                 // the same warp gathers the same rows below, so __syncwarp is all the ordering the att[] values need
             }
+            // per-slot message weights: the attention probabilities, or the entries of a weighted dense adjacency
+            const float* msg_w = att ? att : p.slot_w;
             for (int t = 0; t < T; ++t) {
                 if (!((tmask >> t) & 1u)) continue;
                 // A_t rows: sum of the source states of the row's incoming type-t messages (CSR order = message order)
                 for (int r = warp; r < rows; r += NWARP) {
                     const int v = row0 + r;
-                    if (p.gather_mode == GATHER_SPARSE) {
-                        const int beg = p.row_ptr[(size_t)v * T + t], end = p.row_ptr[(size_t)v * T + t + 1];
-                        for (int c4 = lane; c4 < D4; c4 += 32) {
-                            float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (att) {   // messages weighted by their attention probability (sparse:196)
-                                for (int m = beg; m < end; ++m) {
-                                    const int src = p.csr_src[m];
-                                    const float a = att[m];
-                                    const float* hp = LOCAL ? (sH + (size_t)(src - row0) * D) : (p.g_in + (size_t)src * D);
-                                    const float4 hv = *reinterpret_cast<const float4*>(hp + (c4 << 2));
-                                    sum.x = fmaf(a, hv.x, sum.x); sum.y = fmaf(a, hv.y, sum.y);
-                                    sum.z = fmaf(a, hv.z, sum.z); sum.w = fmaf(a, hv.w, sum.w);
-                                }
-                            } else
+                    const int beg = p.row_ptr[(size_t)v * T + t], end = p.row_ptr[(size_t)v * T + t + 1];
+                    for (int c4 = lane; c4 < D4; c4 += 32) {
+                        float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
+                        if (msg_w) {   // weighted messages (attention: sparse:196; a weighted adjacency: dense:110-112)
                             for (int m = beg; m < end; ++m) {
                                 const int src = p.csr_src[m];
+                                const float a = msg_w[m];
                                 const float* hp = LOCAL ? (sH + (size_t)(src - row0) * D) : (p.g_in + (size_t)src * D);
                                 const float4 hv = *reinterpret_cast<const float4*>(hp + (c4 << 2));
-                                sum.x += hv.x; sum.y += hv.y; sum.z += hv.z; sum.w += hv.w;
+                                sum.x = fmaf(a, hv.x, sum.x); sum.y = fmaf(a, hv.y, sum.y);
+                                sum.z = fmaf(a, hv.z, sum.z); sum.w = fmaf(a, hv.w, sum.w);
                             }
-                            *reinterpret_cast<float4*>(sA + r * D + (c4 << 2)) = sum;
+                        } else
+                        for (int m = beg; m < end; ++m) {
+                            const int src = p.csr_src[m];
+                            const float* hp = LOCAL ? (sH + (size_t)(src - row0) * D) : (p.g_in + (size_t)src * D);
+                            const float4 hv = *reinterpret_cast<const float4*>(hp + (c4 << 2));
+                            sum.x += hv.x; sum.y += hv.y; sum.z += hv.z; sum.w += hv.w;
                         }
-                    } else {
-                        const int nv = p.dense_v;
-                        const int g = v / nv, i = v - g * nv;
-                        const float* arow = p.dense_adj + (((size_t)g * T + t) * nv + i) * nv;
-                        for (int c4 = lane; c4 < D4; c4 += 32) {
-                            float4 sum = make_float4(0.f, 0.f, 0.f, 0.f);
-                            for (int j = 0; j < nv; ++j) {
-                                const float a = arow[j];
-                                if (a != 0.0f) {
-                                    const int src = g * nv + j;
-                                    const float* hp = LOCAL ? (sH + (size_t)(src - row0) * D) : (p.g_in + (size_t)src * D);
-                                    const float4 hv = *reinterpret_cast<const float4*>(hp + (c4 << 2));
-                                    sum.x = fmaf(a, hv.x, sum.x); sum.y = fmaf(a, hv.y, sum.y);
-                                    sum.z = fmaf(a, hv.z, sum.z); sum.w = fmaf(a, hv.w, sum.w);
-                                }
-                            }
-                            *reinterpret_cast<float4*>(sA + r * D + (c4 << 2)) = sum;
-                        }
+                        *reinterpret_cast<float4*>(sA + r * D + (c4 << 2)) = sum;
                     }
                 }
                 __syncthreads();

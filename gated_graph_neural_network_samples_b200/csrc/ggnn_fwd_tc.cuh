@@ -63,18 +63,18 @@ struct TcLayer {
 struct TcParams {
     int V, D, DP, T, L;
     int use_bias, use_avg, cell, act;
-    int gather_mode, dense_v, save;
+    int save;
     int nparts;   // 3: bf16x3 (fp32-accurate), 1: single bf16 MMA
     int nstages;  // weight ring depth
     int ngather;  // gather tiles (>= 2): the A_t of up to ngather edge types are gathered in one pass, then their MMAs run back to back
     int kgs;            // A-operand k-group stride in bytes: 2048 (128-row tiles) or 1024 (compact: every tile has <= 64 rows)
-    int csr_cache;      // LOCAL sparse only: the tile's CSR slice is staged in shared memory (uint16 row offsets, uint8 local sources)
+    int csr_cache;      // LOCAL unweighted only: the tile's CSR slice is staged in shared memory (uint16 row offsets, uint8 local sources)
     int csr_cap_msgs;   // capacity of the shared source array
     const int* tile_start;
     const unsigned* tile_mask;
     const int* row_ptr;
     const int* csr_src;
-    const float* dense_adj;
+    const float* slot_w;   // [M] weight of each CSR slot (weighted dense adjacency), or nullptr
     const float* indeg;
     const float* denom;
     const float* state[MAX_LAYERS + 1];
@@ -529,7 +529,7 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                 store_operand_pair(opH, KGS, PART_B, fr, fc, v.x, v.y);
             })
         }
-        const bool csr_smem = LOCAL && p.csr_cache && p.gather_mode == GATHER_SPARSE;
+        const bool csr_smem = LOCAL && p.csr_cache && !p.slot_w;   // (the staged slice carries no slot weights)
         if (csr_smem) {
             const int base = p.row_ptr[(size_t)row0 * T];
             const int nptr = rows * T + 1;
@@ -609,12 +609,10 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                     gt = gt + 1 == ngather ? 0 : gt + 1;
                     ++nty;
                     ++n;
-                    int beg = 0, end = 0, dg = 0, di = 0;
+                    int beg = 0, end = 0;
                     if (g_row_ok) {
-                        if (p.gather_mode == GATHER_SPARSE) {
-                            if (csr_smem) { beg = sRowPtr[g_row * T + t]; end = sRowPtr[g_row * T + t + 1]; }
-                            else { beg = p.row_ptr[(size_t)g_grow * T + t]; end = p.row_ptr[(size_t)g_grow * T + t + 1]; }
-                        } else { dg = g_grow / p.dense_v; di = g_grow - dg * p.dense_v; }
+                        if (csr_smem) { beg = sRowPtr[g_row * T + t]; end = sRowPtr[g_row * T + t + 1]; }
+                        else { beg = p.row_ptr[(size_t)g_grow * T + t]; end = p.row_ptr[(size_t)g_grow * T + t + 1]; }
                     }
                     for (int kc = g_cg; kc < g_nkc; kc += g_ncg) {
                         float a8[8];
@@ -642,15 +640,17 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                             } else {
                                 for (; m < end; ++m) unpack8_add(*reinterpret_cast<const uint4*>(colbase + (size_t)sSrc[m] * 16), a8, 1.0f);
                             }
-                        } else if (p.gather_mode == GATHER_SPARSE) {
+                        } else {
+                            // each message scaled by its slot weight (a weighted dense adjacency) or by 1: fmaf(1, x, y) rounds as x + y
                             for (int m = beg; m < end; ++m) {
                                 if (LOCAL) {
-                                    const int sl = csr_smem ? (int)sSrc[m] : (p.csr_src[m] - row0);
-                                    const uint8_t* sp = opH + (size_t)kc * KGS + (size_t)sl * 16;
-                                    unpack8_add(*reinterpret_cast<const uint4*>(sp), a8, 1.0f);
-                                    if (X3) unpack8_add(*reinterpret_cast<const uint4*>(sp + PART_B), a8, 1.0f);
+                                    const float a = p.slot_w ? p.slot_w[m] : 1.0f;
+                                    const uint8_t* sp = opH + (size_t)kc * KGS + (size_t)(p.csr_src[m] - row0) * 16;
+                                    unpack8_add(*reinterpret_cast<const uint4*>(sp), a8, a);
+                                    if (X3) unpack8_add(*reinterpret_cast<const uint4*>(sp + PART_B), a8, a);
                                 } else {
-                                    // GLOBAL mode: source rows come from the previous step's fp32 state in L2; keep 4 rows in flight
+                                    // GLOBAL mode: source rows come from the previous step's fp32 state in L2; keep 4 rows in flight (each
+                                    // weight is read at its accumulate step, not beside the row loads)
                                     float hv[4][8];
                                     const int nb = min(4, end - m);
 #pragma unroll
@@ -659,29 +659,11 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
 #pragma unroll
                                     for (int qq = 0; qq < 4; ++qq)
                                         if (qq < nb) {
+                                            const float a = p.slot_w ? p.slot_w[m + qq] : 1.0f;
 #pragma unroll
-                                            for (int j = 0; j < 8; ++j) a8[j] += hv[qq][j];
+                                            for (int j = 0; j < 8; ++j) a8[j] = fmaf(a, hv[qq][j], a8[j]);
                                         }
                                     m += nb - 1;
-                                }
-                            }
-                        } else if (g_row_ok) {
-                            const int nv = p.dense_v;
-                            const float* arow = p.dense_adj + (((size_t)dg * T + t) * nv + di) * nv;
-                            for (int jn = 0; jn < nv; ++jn) {
-                                const float a = arow[jn];
-                                if (a != 0.0f) {
-                                    const int src = dg * nv + jn;
-                                    if (LOCAL) {
-                                        const uint8_t* sp = opH + (size_t)kc * KGS + (size_t)(src - row0) * 16;
-                                        unpack8_add(*reinterpret_cast<const uint4*>(sp), a8, a);
-                                        if (X3) unpack8_add(*reinterpret_cast<const uint4*>(sp + PART_B), a8, a);
-                                    } else {
-                                        float hv[8];
-                                        load8_guarded_cg(p.g_in + (size_t)src * D, kc * 8, D, hv);
-#pragma unroll
-                                        for (int j = 0; j < 8; ++j) a8[j] = fmaf(a, hv[j], a8[j]);
-                                    }
                                 }
                             }
                         }

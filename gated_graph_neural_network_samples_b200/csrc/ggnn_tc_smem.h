@@ -18,14 +18,14 @@ struct TcSmemPlan {
 
 // avail: the opt-in shared memory per block less the kernel's static part.  max_tile_msgs / max_tile_types: the batch's largest message
 // count and largest number of edge types present in one tile.  ngather_request > 0 replaces max_tile_types (GGNN_TC_GATHER_TILES).
-//   1. Compact tile-local launches always stage the per-row constants.  The CSR slice (tile-local sparse graphs) is staged when it fits
+//   1. Compact tile-local launches always stage the per-row constants.  The CSR slice (tile-local unweighted graphs) is staged when it fits
 //      beside three operand tiles and the two ring slots a worker holds at once.
 //   2. Compact tile-local launches gather up to min(max_tile_types, what fits while the ring keeps MIN_RING_GATHER slots) edge types in
 //      one pass, never fewer than two; the 128-row and GLOBAL launches keep two gather tiles (their operand tiles are twice as large).
 //   3. The rest of the budget goes to the ring, up to max_stages slots.
 constexpr int MIN_RING_GATHER = 4;
 
-inline TcSmemPlan tc_smem_plan(int DP, int kgs, int T, bool local, bool sparse, bool use_bias, int max_tile_msgs, int max_tile_types,
+inline TcSmemPlan tc_smem_plan(int DP, int kgs, int T, bool local, bool unweighted, bool use_bias, int max_tile_msgs, int max_tile_types,
                                size_t avail, int max_stages, int ngather_request) {
     TcSmemPlan r;
     const size_t opb = (size_t)DP * (size_t)kgs / 4, stage = (size_t)DP * 128;
@@ -34,7 +34,7 @@ inline TcSmemPlan tc_smem_plan(int DP, int kgs, int T, bool local, bool sparse, 
     const bool compact = local && kgs == 1024;
     const size_t row_b = compact ? (size_t)(kgs / 16) * (1 + (use_bias ? T : 0)) * sizeof(float) : 0;
     size_t csr_b = 0;
-    if (local && sparse && T <= 16 && max_tile_msgs <= 4096) {
+    if (local && unweighted && T <= 16 && max_tile_msgs <= 4096) {
         const int cap = (max_tile_msgs + 15) / 16 * 16;
         const size_t b = (size_t)((128 * T + 1 + 7) & ~7) * 2 + (size_t)cap;
         if (avail >= ops2 + bias_b + row_b + b + 2 * stage) {

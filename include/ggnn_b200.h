@@ -139,8 +139,8 @@ int ggnn_host_prepare_graph_sparse(const ggnn_config* cfg, int32_t num_sms, int3
                                    const float* num_incoming_edges_per_type, ggnn_prepared_graph** inout);
 /* The dense wire format through the same two halves: a 0/1 adjacency_matrix [b, T, v, v] (all the reference ever feeds, dense:30-36) is
  * scanned into edge lists (order: graph, target row, source column; in-degree = row sums) and built like a sparse batch; the result is
- * adopted with ggnn_set_graph_prepared.  A matrix with other entries returns GGNN_EUNSUPPORTED: feed it with ggnn_set_graph_dense (matrix
- * walk).  ggnn_set_graph_dense itself takes this path for 0/1 matrices. */
+ * adopted with ggnn_set_graph_prepared.  A matrix with other entries returns GGNN_EUNSUPPORTED: feed it with ggnn_set_graph_dense, which
+ * builds it the same way with its entries as per-message weights. */
 int ggnn_prepare_graph_dense(const ggnn_engine* e, int32_t save_for_backward, int32_t num_graphs, int32_t num_vertices,
                              const float* adjacency_matrix, ggnn_prepared_graph** inout);
 int ggnn_host_prepare_graph_dense(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t num_graphs,

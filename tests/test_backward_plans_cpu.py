@@ -166,7 +166,7 @@ SPARSE_CASES = {c.name: c for c in PLAN_MATRIX + EDGE_SHAPES}
 PARTIAL_CASES = ["ffma1-local-gru-D36", "ffma1-local-rnn-D36", "ffma-local-cudnn-D100", "tc-local64-gru-D20"]
 DETERMINISM_CASES = ["tc-local64-gru-D100", "tc-global-rnn-D100", "stream-gru-D132", "ffma0-local-gru-D100"]
 
-# dense: (name, precision, hidden, weighted, plan text).  The binary case goes through the CSR builder; the weighted ones walk the matrix.
+# dense: (name, precision, hidden, weighted, plan text).  Every case goes through the CSR builder; the weighted ones with slot weights.
 DENSE_CASES = [("weighted-fp32-D24", "fp32", 24, True, r"^fp32-ffma LOCAL\("),
                ("weighted-tc-D100", "bf16x3", 100, True, TC_LOCAL_64),
                ("binary-tc-D100", "bf16x3", 100, False, TC_LOCAL_64)]

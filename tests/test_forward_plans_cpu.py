@@ -169,7 +169,7 @@ def gcn_graph(D, kind):
 
 # ---------------------------------------------------------------------------------------------------------------- the cases
 class Case:
-    """One forward of the GPU file.  ``kind``: ``sparse`` (GGNN on a batch kind), ``dense`` (weighted dense matrix, dense gather mode) or
+    """One forward of the GPU file.  ``kind``: ``sparse`` (GGNN on a batch kind), ``dense`` (weighted dense matrix, weighted CSR) or
     ``gcn``.  ``instance``: the kernel instance the case claims; ``keep``: state-dropout keep probability."""
 
     def __init__(self, name, kind, params, T, batch, precision, env, instance, keep=1.0):
@@ -235,7 +235,7 @@ def _tile_cases():
             Case("tc-nh%d-T32-D%d" % (nh, Db), "sparse", g(Db), 32, "comp", "bf16x3", {}, tc(True)),
             Case("tc-nh%d-msgs4k-D%d" % (nh, Da), "sparse", g(Da), 4, "msgs", "bf16x3", {}, tc(True)),
             Case("tc-nh%d-dropout-D%d" % (nh, Db), "sparse", g(Db, "RNN" if i % 2 else "GRU"), 4, "mol24", "bf16x3", {}, tc(True), keep=0.8),
-            Case("tc-nh%d-dense-D%d" % (nh, Da), "dense", dense_params(Da), 4, "dense", "bf16x3", {"GGNN_DENSE_KEEP_MATRIX": "1"}, tc(True)),
+            Case("tc-nh%d-dense-D%d" % (nh, Da), "dense", dense_params(Da), 4, "dense", "bf16x3", {}, tc(True)),
         ]
     return out
 

@@ -179,12 +179,11 @@ def test_d_h0_is_bit_identical_run_to_run(case, monkeypatch):
 
 # ---------------------------------------------------------------------------------------------------------------- dense
 @pytest.mark.parametrize("name,precision,D,weighted,pattern", DENSE_CASES, ids=[c[0] for c in DENSE_CASES])
-def test_dense_gradients_on_weighted_and_binary_matrices(name, precision, D, weighted, pattern, monkeypatch):
-    """A weighted ``[b, T, v, v]`` matrix walks the matrix in both orientations of the backward (dense_gather_sum_kernel); a binary one
-    goes through the CSR builder.  Reference: the dense oracle in float64, which takes weighted matrices."""
+def test_dense_gradients_on_weighted_and_binary_matrices(name, precision, D, weighted, pattern):
+    """A weighted ``[b, T, v, v]`` matrix goes through the CSR builder with its entries as slot weights, which weight both gathers of the
+    backward (target- and source-keyed CSR); a binary one goes through it unweighted.  Reference: the dense oracle in float64, which takes
+    weighted matrices."""
     import torch
-    if weighted:
-        monkeypatch.setenv("GGNN_DENSE_KEEP_MATRIX", "1")
     A, h0 = dense_batch(D, weighted)
     b, v = h0.shape[:2]
     dw = O.init_dense_weights({"hidden_size": D}, DENSE_T, np.random.default_rng(5))

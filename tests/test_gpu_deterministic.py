@@ -221,10 +221,8 @@ def test_attention_with_16_types_and_absent_types(monkeypatch):
 
 
 @pytest.mark.parametrize("name,precision,D,weighted,pattern", DENSE_CASES, ids=[c[0] for c in DENSE_CASES])
-def test_dense_gradients_are_bit_identical(name, precision, D, weighted, pattern, monkeypatch):
+def test_dense_gradients_are_bit_identical(name, precision, D, weighted, pattern):
     import torch
-    if weighted:
-        monkeypatch.setenv("GGNN_DENSE_KEEP_MATRIX", "1")
     A, h0 = dense_batch(D, weighted)
     b, v = h0.shape[:2]
     dw = O.init_dense_weights({"hidden_size": D}, DENSE_T, np.random.default_rng(5))

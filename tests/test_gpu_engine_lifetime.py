@@ -213,7 +213,7 @@ def test_cfg4_streaming_sequence_with_hub_nodes(monkeypatch):
 # ---------------------------------------------------------------------------------------------------------------- dense
 @pytest.mark.parametrize("precision", ["fp32", "bf16x3"])
 def test_dense_sequence_alternates_binary_and_weighted_matrices(precision):
-    """Binary matrices (CSR builder) alternate with weighted ones (matrix walk) on one engine, with b and v changing."""
+    """Binary matrices (CSR) alternate with weighted ones (CSR with slot weights) on one engine, with b and v changing."""
     import torch
     from gated_graph_neural_network_samples_b200.engine import PropagationEngine
     D = 100

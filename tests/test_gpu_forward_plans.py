@@ -109,7 +109,7 @@ def test_hidden_size_sweep(case, monkeypatch):
 def test_tile_wgmma_instances(case, monkeypatch):
     """The tile-local wgmma kernel at every NH: compact 64-row and 128-row LOCAL tiles, GLOBAL, bf16 LOCAL and GLOBAL, T = 17 / 32 (no
     shared-memory CSR cache; type 31 sets the tile mask's top bit), a tile with more than 4096 messages, state dropout, and a weighted
-    dense matrix (dense gather mode)."""
+    dense matrix (weighted CSR)."""
     _run_ggnn(CASES[case], monkeypatch)
 
 

@@ -232,9 +232,9 @@ def test_full_size_cfg4_properties():
 
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16x3"])
-def test_dense_weighted_adjacency_uses_the_matrix_path(precision, monkeypatch):
-    """A non-binary adjacency cannot be an edge list: the engine keeps the [b,T,v,v] matrix and multiplies by its entries
-    (the reference's matmul semantics, dense:110-112); a binary one is converted to CSR -- both must agree with the oracle."""
+def test_dense_weighted_adjacency_weights_its_messages(precision):
+    """A non-binary adjacency is converted to a CSR that carries its entries as per-message weights (the reference's matmul
+    semantics, dense:110-112); a binary one to a plain CSR -- both must agree with the oracle."""
     D, T, steps, b, v = 24, 3, 2, 5, 16
     rng = np.random.default_rng(11)
     A = (rng.random((b, T, v, v)) < 0.15).astype(np.float32)
@@ -246,6 +246,3 @@ def test_dense_weighted_adjacency_uses_the_matrix_path(precision, monkeypatch):
         ref = O.dense_propagation_loops(h0, adj, dw, dp)
         got = U.engine_dense(dp, T, dw, adj, h0, precision=precision)
         assert U.max_rel_err(got, ref) < 1e-4
-    monkeypatch.setenv("GGNN_DENSE_KEEP_MATRIX", "1")   # binary adjacency through the matrix path as well
-    got = U.engine_dense(dp, T, dw, A, h0, precision=precision)
-    assert U.max_rel_err(got, O.dense_propagation_loops(h0, A, dw, dp)) < 1e-4
