@@ -242,7 +242,7 @@ __global__ void __launch_bounds__(256) colsum_split_kernel(const float* __restri
 // One thread per 4 consecutive outputs (N is a multiple of 4), then one per bias entry; C == nullptr: the bias only.
 __global__ void __launch_bounds__(256) split_reduce_kernel(const float* __restrict__ part, const float* __restrict__ bias_part, int splits, int nseg,
                                                            int K, int N, float* __restrict__ C, int ldc, size_t c_stride, float* __restrict__ bias_out) {
-    const int per = K * N, quads = C ? nseg * per / 4 : 0, total = quads + (bias_out ? N : 0);   // K*N <= 256*512, nseg <= 16
+    const int per = K * N, quads = C ? nseg * per / 4 : 0, total = quads + (bias_out ? N : 0);   // K*N <= 512*1024, nseg <= 16
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
         if (i < quads) {
             const int e = i * 4, s = e / per, r = e - s * per, k = r / N, n = r - k * N;
@@ -413,7 +413,8 @@ __global__ void __launch_bounds__(256) csr_gather_all_kernel(GatherJob j0, Gathe
 // dsa[slot] = d s_m a_t is left for the source kernel; scratch[slot] holds d alpha in between.
 // ORDERED = false adds d a_t with shared then global atomics.  ORDERED = true (ggnn_set_deterministic): every warp's d a_t goes to its own
 // shared slot, the block adds the slots in warp order and stores its partial to d_att_w[blockIdx.x * T + t] (then ordered_colsum_kernel).
-template <bool ORDERED>
+// NJ: the columns of d h[v] a lane holds (column lane + 32 j), so D <= 32 * NJ: instances NJ = 8 (D <= 256) and 16 (D <= 512).
+template <int NJ, bool ORDERED>
 __device__ __forceinline__ void attention_bwd_target(const int* __restrict__ row_ptr, const int* __restrict__ csr_src, const float* __restrict__ h,
                                                      const float* __restrict__ P, const float* __restrict__ alpha, const float* __restrict__ att_w,
                                                      float* __restrict__ dsa, float* __restrict__ dh, float* __restrict__ d_att_w, int V, int D, int T) {
@@ -437,9 +438,9 @@ __device__ __forceinline__ void attention_bwd_target(const int* __restrict__ row
             }
         }
         __syncwarp();
-        float dhv[8];
+        float dhv[NJ];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) dhv[j] = 0.f;
+        for (int j = 0; j < NJ; ++j) dhv[j] = 0.f;
         for (int t = 0; t < T; ++t) {
             const float aw = att_w[t];
             float daw = 0.f;
@@ -448,7 +449,7 @@ __device__ __forceinline__ void attention_bwd_target(const int* __restrict__ row
                 const float ds = alpha[m] * (dsa[m] - acc);
                 float dot = 0.f;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
+                for (int j = 0; j < NJ; ++j) {
                     const int c = lane + 32 * j;
                     if (c < D) { const float x = hs[c]; dot = fmaf(x, hv[c], dot); dhv[j] = fmaf(ds * aw, x, dhv[j]); }
                 }
@@ -462,7 +463,7 @@ __device__ __forceinline__ void attention_bwd_target(const int* __restrict__ row
             else if (lane == 0 && d_att_w && daw != 0.f) atomicAdd(&s_daw[t], daw);
         }
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
+        for (int j = 0; j < NJ; ++j) {
             const int c = lane + 32 * j;
             if (c < D) dh[(size_t)v * D + c] += dhv[j];
         }
@@ -476,20 +477,22 @@ __device__ __forceinline__ void attention_bwd_target(const int* __restrict__ row
         }
     } else if (d_att_w && threadIdx.x < T && s_daw[threadIdx.x] != 0.f) atomicAdd(d_att_w + threadIdx.x, s_daw[threadIdx.x]);
 }
+template <int NJ>
 __global__ void __launch_bounds__(256) attention_bwd_target_kernel(const int* __restrict__ row_ptr, const int* __restrict__ csr_src,
                                                                    const float* __restrict__ h, const float* __restrict__ P,
                                                                    const float* __restrict__ alpha, const float* __restrict__ att_w,
                                                                    float* __restrict__ dsa, float* __restrict__ dh, float* __restrict__ d_att_w,
                                                                    int V, int D, int T) {
-    attention_bwd_target<false>(row_ptr, csr_src, h, P, alpha, att_w, dsa, dh, d_att_w, V, D, T);
+    attention_bwd_target<NJ, false>(row_ptr, csr_src, h, P, alpha, att_w, dsa, dh, d_att_w, V, D, T);
 }
 // d_att_part: [gridDim.x][T] block partials of d a_t, reduced by ordered_colsum_kernel
+template <int NJ>
 __global__ void __launch_bounds__(256) attention_bwd_target_ordered_kernel(const int* __restrict__ row_ptr, const int* __restrict__ csr_src,
                                                                            const float* __restrict__ h, const float* __restrict__ P,
                                                                            const float* __restrict__ alpha, const float* __restrict__ att_w,
                                                                            float* __restrict__ dsa, float* __restrict__ dh,
                                                                            float* __restrict__ d_att_part, int V, int D, int T) {
-    attention_bwd_target<true>(row_ptr, csr_src, h, P, alpha, att_w, dsa, dh, d_att_part, V, D, T);
+    attention_bwd_target<NJ, true>(row_ptr, csr_src, h, P, alpha, att_w, dsa, dh, d_att_part, V, D, T);
 }
 // d h[s] += sum over the messages LEAVING s of dsa[target-CSR slot] * h[target]     (source-keyed CSR, one warp per source)
 __global__ void __launch_bounds__(256) attention_bwd_source_kernel(const int* __restrict__ trow, const int* __restrict__ ttgt,

@@ -29,6 +29,7 @@
 #include "ggnn_fwd_ffma.cuh"
 #include "ggnn_fwd_tc.cuh"
 #include "ggnn_fwd_stream.cuh"
+#include "ggnn_fwd_step.cuh"
 #include "ggnn_gcn.cuh"
 #include "ggnn_tc_smem.h"
 
@@ -156,6 +157,7 @@ struct BatchPlan {
     bool stream = false;
     int ts_nc[2] = {0, 0}, ts_nblk[2] = {0, 0};      // [0]: DP-wide outputs (agg, candidate)  [1]: the 2*DP-wide gate output
     int ts_nv = 0;                                   // number of virtual rows of the current batch
+    bool stepwise = false;   // fp32 above hidden 256 (ggnn_fwd_step.cuh): a few launches over the whole batch per timestep
     int tc_row_budget = 128, tc_kgs = 2048;   // tensor-core plan: no tile has more rows than the budget; <= 64 selects compact operand tiles
     // the graph image: row_ptr | csr_src | csr_msg | indeg | denom | tile_start | tile_mask | ...
     size_t off_row_ptr = 0, off_src = 0, off_msg = 0, off_indeg = 0, off_denom = 0, off_tiles = 0, off_mask = 0;
@@ -222,6 +224,8 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     DevBuf bwd_buf;     // backward scratch
     WeightTiles tc_tiles;   // the weights tiled for the tile-local wgmma kernel (GGNN) or the GCN wgmma kernel
     WeightTiles ts_tiles;   // ... and for the streaming kernel
+    WeightTiles step_wt;    // ... and the transposed fp32 copies of the per-timestep fp32 path
+    DevBuf step_buf;        // the per-timestep fp32 path's scratch: gathered messages, cell input row, gates, candidate
     DevBuf tc_respre;   // residual pre-products [ntiles][128][3*DP]
     DevBuf err_flag;    // device int written by kernels on a barrier timeout
     // the state buffers of the last forward on the current graph; fwd_valid is cleared by every graph upload.  Without save_for_backward
@@ -450,6 +454,12 @@ size_t fwd_smem_bytes(int variant, int nb1, int D, int T) {
     return sizeof(float) * ((size_t)4 * MT * D + (size_t)2 * KC * pw + (size_t)2 * MT * KC + (size_t)T * D);
 }
 
+// Launches per timestep of the per-timestep fp32 path: gather, message GEMM, its epilogue, the candidate GEMM and the update; the attention
+// pre-pass; the gate GEMM and its epilogue (GRU cells); the recurrent projection (CudnnCompatibleGRUCell).
+int stepwise_launches(const ModelShape& s) {
+    return 5 + (s.use_att ? 1 : 0) + (s.cell != CELL_RNN ? 2 : 0) + (s.cell == CELL_CUDNN_GRU ? 1 : 0);
+}
+
 // Tiles of whole components: a tile closes before the component that would take it past `budget` rows.
 void pack_components(const std::vector<int>& cuts, int V, int budget, std::vector<int>& tile_start) {
     tile_start.assign(1, 0);
@@ -552,6 +562,14 @@ int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>
                      p.local ? "LOCAL(all layers+steps fused, 1 launch)" : "GLOBAL(1 launch per step)", p.ntiles, budget,
                      p.tc_kgs == 1024 ? " (compact 64-row operand tiles)" : "", s.DP, max_span);
         }
+    } else if (s.D > 256) {
+        // the fp32 tile kernel holds four MT x D tiles in shared memory and at most 256 columns in its register blocking: above hidden 256
+        // each timestep runs as a few launches over the whole batch.  Tiles play no part; fixed 128-row ones only split the host build.
+        p.stepwise = true;
+        fixed_tiles(V, ts::TILE_M, tile_start);
+        p.ntiles = (int)tile_start.size() - 1;
+        snprintf(buf, sizeof buf, "fp32-stepwise%s%s (%d launches per step) V=%d D=%d T=%d", s.use_att ? "+attention" : "",
+                 s.cell == CELL_CUDNN_GRU ? "+cudnn-gru" : "", stepwise_launches(s), V, s.D, s.T);
     } else {
         const int D = s.D;
         const bool a_ok = pick_nb1(0, D) > 0 && fwd_smem_bytes(0, pick_nb1(0, D), D, s.T) <= s.max_smem;
@@ -842,14 +860,15 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
             if (e->use_att) {   // softmax backward first (it adds to dh_new), then the gathers are weighted by the probabilities
                 const float* alpha = (const float*)e->att_buf.ptr + (size_t)(e->step_base[l] + s) * (size_t)std::max<int64_t>(e->M, 1);
                 gemm_nt(false, dxp, D, 0, w.edge_weights, D, 0, 1, Pall, TD, V, TD, D);   // P[v, t*D+k] = <dx'[v], W_t[k, :]>
+                // the target kernel holds 8 columns of d h[v] per lane up to hidden 256, 16 above
                 if (e->det && gw.edge_type_attention_weights) {   // per-block d a_t into ws, then added over the blocks in a fixed order
-                    attention_bwd_target_ordered_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, Pall, alpha,
-                                                                                      w.edge_type_attention_weights, dsa, dh_new, ws, V, D, T);
+                    (D <= 256 ? attention_bwd_target_ordered_kernel<8> : attention_bwd_target_ordered_kernel<16>)<<<nodes_blocks, 256, 0, st>>>(
+                        gd.row_ptr, gd.csr_src, h, Pall, alpha, w.edge_type_attention_weights, dsa, dh_new, ws, V, D, T);
                     ordered_colsum_kernel<<<T, 256, 0, st>>>(ws, nodes_blocks, T, gw.edge_type_attention_weights);
                     ++e->last_launches;
                 } else {
-                    attention_bwd_target_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, Pall, alpha, w.edge_type_attention_weights,
-                                                                              dsa, dh_new, gw.edge_type_attention_weights, V, D, T);
+                    (D <= 256 ? attention_bwd_target_kernel<8> : attention_bwd_target_kernel<16>)<<<nodes_blocks, 256, 0, st>>>(
+                        gd.row_ptr, gd.csr_src, h, Pall, alpha, w.edge_type_attention_weights, dsa, dh_new, gw.edge_type_attention_weights, V, D, T);
                 }
                 attention_bwd_source_kernel<<<nodes_blocks, 256, 0, st>>>(gd.trow, gd.ttgt, gd.tslot, h, dsa, dh_new, V, D, T);
                 e->last_launches += 2;
@@ -904,9 +923,11 @@ extern "C" {
 const char* ggnn_last_error(const ggnn_engine* e) { return e ? e->err.c_str() : g_create_error.c_str(); }
 
 // The checks and fields both model configs have; no CUDA (the text goes to `err`: this may run in any thread).
-static int init_common_shape(ModelShape& s, int hidden_size, int num_layers, int precision, int device, std::string& err) {
+// `max_hidden`: the widest hidden size of the model's kernels (GGNN 512: the readout and the attention backward hold 16 columns per lane;
+// GCN 256: its fp32 kernel).
+static int init_common_shape(ModelShape& s, int hidden_size, int max_hidden, int num_layers, int precision, int device, std::string& err) {
     if (hidden_size <= 0 || hidden_size % 4 != 0) { err = "hidden_size must be a positive multiple of 4"; return GGNN_EINVAL; }
-    if (hidden_size > 256) { err = "hidden_size > 256 is not supported by this build"; return GGNN_EUNSUPPORTED; }
+    if (hidden_size > max_hidden) { err = "hidden_size > " + std::to_string(max_hidden) + " is not supported by this build"; return GGNN_EUNSUPPORTED; }
     if (num_layers <= 0 || num_layers > MAX_LAYERS) { err = "num_layers must be in 1..16"; return GGNN_EINVAL; }
     if (precision != GGNN_PREC_FP32 && precision != GGNN_PREC_BF16X3 && precision != GGNN_PREC_BF16) { err = "unknown precision"; return GGNN_EINVAL; }
     s.D = hidden_size; s.L = num_layers; s.precision = precision; s.device = device;
@@ -918,7 +939,7 @@ static int init_common_shape(ModelShape& s, int hidden_size, int num_layers, int
 // prepared graphs.  Returns GGNN_OK or an error code.
 static int init_model_shape(ModelShape& s, const ggnn_config* cfg, std::string& err) {
     auto bad = [&](const char* msg) { err = msg; return (int)GGNN_EINVAL; };
-    if (int rc = init_common_shape(s, cfg->hidden_size, cfg->num_layers, cfg->precision, cfg->device, err)) return rc;
+    if (int rc = init_common_shape(s, cfg->hidden_size, 512, cfg->num_layers, cfg->precision, cfg->device, err)) return rc;
     if (cfg->num_edge_types <= 0 || cfg->num_edge_types > 32) return bad("num_edge_types must be in 1..32");
     if (!cfg->layer_timesteps) return bad("layer_timesteps is null");
     if (cfg->cell != GGNN_CELL_GRU && cfg->cell != GGNN_CELL_RNN && cfg->cell != GGNN_CELL_CUDNN_GRU) return bad("Unknown RNN cell type");   // sparse:112
@@ -957,7 +978,7 @@ static int init_model_shape(ModelShape& s, const ggnn_config* cfg, std::string& 
 // The model shape of a ggnn_gcn_config (chem_tensorflow_gcn.py:42-82): one edge type, one "timestep" per layer (the dropout's global step
 // is the layer index).
 static int init_gcn_shape(ModelShape& s, const ggnn_gcn_config* cfg, std::string& err) {
-    if (int rc = init_common_shape(s, cfg->hidden_size, cfg->num_layers, cfg->precision, cfg->device, err)) return rc;
+    if (int rc = init_common_shape(s, cfg->hidden_size, 256, cfg->num_layers, cfg->precision, cfg->device, err)) return rc;
     s.model = MODEL_GCN;
     s.T = 1;
     s.use_bias = cfg->use_bias != 0;
@@ -1002,6 +1023,7 @@ int ggnn_destroy(ggnn_engine* e) {
     cudaSetDevice(e->device);
     e->graph_buf.release(); e->state_buf.release(); e->save_bufs.release(); e->io_buf.release(); e->bwd_buf.release();
     e->tc_tiles.buf.release(); e->tc_respre.release(); e->ts_tiles.buf.release(); e->ts_images.release(); e->ts_virt.release(); e->err_flag.release();
+    e->step_wt.buf.release(); e->step_buf.release();
     if (e->own_prep) { ggnn_free_prepared_graph(e->own_prep); e->own_prep = nullptr; }
     e->ro_buf.release(); e->ro_stage.release(); e->att_buf.release(); e->ro_ws.release();
     delete e;
@@ -1238,10 +1260,10 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     if (const char* nt = getenv("GGNN_HOST_THREADS")) nth = std::max(1, std::min(atoi(nt), 64));
 #endif
     // ---- pass 1: validate, count per (target,type), mark which node boundaries are spanned by an edge (the cut points of the tile-local
-    // plans; the streaming plan of hidden sizes > 128 tiles by fixed 128-row blocks and skips that part)
+    // plans; the streaming plan of hidden sizes > 128 and the per-timestep fp32 path above 256 tile by fixed 128-row blocks and skip that part)
     std::vector<int>& counts = g->h_counts;
     std::vector<int>& reach = g->h_diff;   // reach[j] = the farthest node an edge whose lower end is node j touches
-    const bool need_cuts = !(shape.precision != GGNN_PREC_FP32 && shape.DP > 128);
+    const bool need_cuts = shape.precision == GGNN_PREC_FP32 ? shape.D <= 256 : shape.DP <= 128;
     counts.resize((size_t)V * T + 1);
     if (need_cuts) reach.resize((size_t)V + 1);
     std::vector<int64_t> type_base(T + 1, 0);   // position of every type's first message in the reference's type-major message order
@@ -1820,6 +1842,102 @@ static int forward_ffma(ggnn_engine* e, const float* h0, float* h_out, cudaStrea
     return launch_steps(e, p, st, [&](const FwdParams& q) { k<<<e->ntiles, 256, smem, st>>>(q); });
 }
 
+// The per-timestep fp32 path (ggnn_fwd_step.cuh) multiplies with bwd::gemm_nt_kernel, C = A . B^T: it reads transposed fp32 copies of the
+// weights, per layer the T edge matrices, the gate kernel and the candidate kernel.  Made again when the weights changed since (the
+// weights generation), at no other time.
+static int step_prepare_weights(ggnn_engine* e, cudaStream_t st) {
+    const size_t D = e->D, T = e->T;
+    WeightTiles& c = e->step_wt;
+    size_t off = 0;
+    for (int l = 0; l < e->L; ++l) {
+        const size_t rows = D * (e->nres[l] + 2);
+        c.off_edge[l] = off; off += T * D * D;
+        c.off_gate[l] = off; off += e->cell != CELL_RNN ? rows * 2 * D : 0;
+        c.off_cand[l] = off; off += rows * D;
+    }
+    bool retile = false;
+    CU_TRY(e, c.reserve(off * sizeof(float), 0, 0, e->weights_gen, retile));
+    if (!retile) return GGNN_OK;
+    float* base = (float*)c.buf.ptr;
+    auto transpose = [&](const float* W, size_t out, int rows, int cols, int batch) {
+        step::transpose_kernel<<<dim3((cols + 31) / 32, (rows + 31) / 32, batch), dim3(32, 8), 0, st>>>(W, base + out, rows, cols);
+        ++e->last_launches;
+    };
+    for (int l = 0; l < e->L; ++l) {
+        const int rows = (int)D * (e->nres[l] + 2);
+        transpose(e->w[l].edge_weights, c.off_edge[l], (int)D, (int)D, (int)T);
+        if (e->cell != CELL_RNN) transpose(e->w[l].gate_kernel, c.off_gate[l], rows, 2 * (int)D, 1);
+        transpose(e->w[l].cand_kernel, c.off_cand[l], rows, (int)D, 1);
+    }
+    CU_TRY(e, cudaGetLastError());
+    c.gen = e->weights_gen;
+    return GGNN_OK;
+}
+
+static int forward_stepwise(ggnn_engine* e, const float* h0, float* h_out, cudaStream_t st) {
+    using namespace ggnn::bwd;
+    if (int rc = step_prepare_weights(e, st)) return rc;
+    const int V = e->V, D = e->D, T = e->T;
+    const bool gru = e->cell != CELL_RNN, cudnn = e->cell == CELL_CUDNN_GRU;
+    int maxres = 0;
+    for (int l = 0; l < e->L; ++l) maxres = std::max(maxres, e->nres[l]);
+    const size_t vd = (size_t)V * D;
+    // scratch: gathered messages [V, T*D] | cell input row [V, D*(R+2)] | gates [V, 2D] | candidate GEMM [V, D] | q GEMM [V, D]
+    size_t off = 0;
+    auto take = [&](size_t floats) { size_t o = off; off = align_up(off + floats * sizeof(float), 256); return o; };
+    const size_t o_at = take(vd * T), o_x = take(vd * (maxres + 2)), o_g = take(gru ? 2 * vd : 0), o_c = take(vd), o_q = take(cudnn ? vd : 0);
+    CU_TRY(e, e->step_buf.reserve(off));
+    if (e->use_att)
+        CU_TRY(e, e->att_buf.reserve(sizeof(float) * (size_t)std::max<int64_t>(e->M, 1) * (size_t)(e->save ? std::max(e->total_steps, 1) : 1)));
+    char* sb = (char*)e->step_buf.ptr;
+    float *At = (float*)(sb + o_at), *X = (float*)(sb + o_x), *Gb = (float*)(sb + o_g), *Cb = (float*)(sb + o_c), *Qb = (float*)(sb + o_q);
+    const float* wt = (const float*)e->step_wt.buf.ptr;
+    const GraphDev& gd = e->gd;
+    const long long n = (long long)vd;
+    const int eb = (int)std::min<long long>((n + 255) / 256, 4096), nodes_blocks = (V + 7) / 8;
+    auto gemm = [&](const float* A, int lda, int a_stride, const float* B, int ldb, int b_stride, int nseg, float* C, int ldc, int N, int K) {
+        gemm_nt_kernel<false><<<dim3((N + NT_BN - 1) / NT_BN, (V + NT_BM - 1) / NT_BM), 128, 0, st>>>(A, lda, a_stride, B, ldb, b_stride, nseg, C,
+                                                                                                    ldc, V, N, K);
+    };
+    FwdParams p;   // the layer states and the step ping-pong of launch_steps
+    fill_common_params(e, p, h0, h_out);
+    cudaError_t copy_st = cudaSuccess;
+    const int rc = launch_steps(e, p, st, [&](const FwdParams& q) {
+        const int l = q.g_layer, R = e->nres[l], ldx = D * (R + 2), gs = e->step_base[l] + q.g_step;
+        const ggnn_layer_weights& w = e->w[l];
+        const float* h = q.g_in;
+        const SaveDev sv = saved_step(e, gs);
+        // the residual inputs are node_states_per_layer entries before this layer: fixed for all of its steps
+        if (q.g_step == 0)
+            for (int i = 0; i < R && copy_st == cudaSuccess; ++i)
+                copy_st = cudaMemcpy2DAsync(X + (size_t)i * D, sizeof(float) * ldx, q.state[e->res[l][i]], sizeof(float) * D, sizeof(float) * D, V,
+                                            cudaMemcpyDeviceToDevice, st);
+        const float* msg_w = q.slot_w;
+        if (e->use_att) {
+            float* att = (float*)e->att_buf.ptr + (size_t)gs * (e->save ? (size_t)std::max<int64_t>(e->M, 1) : 0);
+            step::attention_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, w.edge_type_attention_weights, att, V, D, T);
+            msg_w = att;
+        }
+        const GatherJob gj{gd.row_ptr, gd.csr_src, h, At, msg_w, nullptr};
+        csr_gather_all_kernel<<<dim3(nodes_blocks, 1), 256, 0, st>>>(gj, gj, V, D, T);
+        gemm(At, T * D, D, wt + e->step_wt.off_edge[l], D, D * D, T, X + (size_t)R * D, ldx, D, D);
+        step::agg_epilogue_kernel<<<eb, 256, 0, st>>>(X, ldx, R * D, (R + 1) * D, h, e->use_bias ? w.edge_biases : nullptr, gd.indeg,
+                                                      e->use_avg ? gd.denom : nullptr, sv.agg, sv.h_in, n, D, T);
+        if (gru) {
+            gemm(X, ldx, 0, wt + e->step_wt.off_gate[l], ldx, 0, 1, Gb, 2 * D, 2 * D, ldx);
+            step::gate_epilogue_kernel<<<eb, 256, 0, st>>>(Gb, w.gate_bias, h, cudnn ? nullptr : X, ldx, (R + 1) * D, sv.r, sv.u, n, D);
+            if (cudnn) gemm(h, D, 0, wt + e->step_wt.off_cand[l] + (size_t)(R + 1) * D, ldx, 0, 1, Qb, D, D, D);
+        }
+        // CudnnCompatibleGRUCell: the candidate's first D*(R+1) kernel rows see [res.., agg]; its recurrent rows went into q
+        gemm(X, ldx, 0, wt + e->step_wt.off_cand[l], ldx, 0, 1, Cb, D, D, cudnn ? ldx - D : ldx);
+        step::update_kernel<<<eb, 256, 0, st>>>(Cb, w.cand_bias, gru ? Gb : nullptr, cudnn ? Qb : nullptr, w.cand_hidden_bias, h, q.g_out, sv.c,
+                                                sv.q, e->act, e->drop_keep, e->drop_seed, gs, V, n, D);
+        e->last_launches += stepwise_launches(*e) - 1;   // launch_steps counts one per step
+    });
+    if (copy_st != cudaSuccess) return e->fail(GGNN_ECUDA, "residual input copy failed: %s", cudaGetErrorString(copy_st));
+    return rc;
+}
+
 // The tile-local wgmma layout (ggnn_fwd_tc.cuh): per layer the T edge blocks, then the gate and the candidate kernel in nres + 2 input
 // segments.  A GCN layer is one edge block.
 static int tc_prepare_weights(ggnn_engine* e, cudaStream_t st) {
@@ -2296,7 +2414,7 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
     }
     int rc;
     if (gcn) rc = forward_gcn(e, h0, h_out, st);
-    else if (e->precision == GGNN_PREC_FP32) rc = forward_ffma(e, h0, h_out, st);
+    else if (e->precision == GGNN_PREC_FP32) rc = e->stepwise ? forward_stepwise(e, h0, h_out, st) : forward_ffma(e, h0, h_out, st);
     else rc = e->stream ? forward_stream(e, h0, h_out, st) : forward_tc(e, h0, h_out, st);
     if (rc) return rc;
     CU_TRY(e, cudaGetLastError());
@@ -2462,15 +2580,23 @@ int ggnn_readout_backward(ggnn_engine* e, const float* h_last, const float* h0, 
         const int blocks = std::max(1, std::min((V + 7) / 8, readout::RO_ORDERED_BLOCKS)), cols = 3 * e->D + 2;
         CU_TRY(e, e->ro_ws.reserve(sizeof(float) * (size_t)blocks * cols));
         float* part = (float*)e->ro_ws.ptr;
-        readout::readout_bwd_ordered_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(h_last, h0, w, (const int*)(g + e->ro_off_graph_of), mask, d_out,
-                                                                                     d_h_last, part, V, e->D);
+        // 8 columns per lane up to hidden 256, 16 above (its 8 warp rows then need dynamic shared memory)
+        if (e->D <= 256) {
+            readout::readout_bwd_ordered_kernel<8><<<blocks, 256, 0, (cudaStream_t)stream>>>(h_last, h0, w, (const int*)(g + e->ro_off_graph_of), mask,
+                                                                                            d_out, d_h_last, part, V, e->D);
+        } else {
+            const size_t smem = readout::ro_ordered_smem<16>();
+            CU_TRY(e, cudaFuncSetAttribute(readout::readout_bwd_ordered_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            readout::readout_bwd_ordered_kernel<16><<<blocks, 256, smem, (cudaStream_t)stream>>>(h_last, h0, w, (const int*)(g + e->ro_off_graph_of),
+                                                                                                mask, d_out, d_h_last, part, V, e->D);
+        }
         readout::readout_bwd_reduce_kernel<<<cols, 256, 0, (cudaStream_t)stream>>>(part, blocks, e->D, d_w_gate, d_b_gate, d_w_trans, d_b_trans);
         CU_TRY(e, cudaGetLastError());
         return GGNN_OK;
     }
     const int blocks = std::max(1, std::min((V + 7) / 8, 4 * e->num_sms));
-    readout::readout_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(h_last, h0, w, (const int*)(g + e->ro_off_graph_of), mask, d_out, d_h_last,
-                                                                         d_w_gate, d_b_gate, d_w_trans, d_b_trans, V, e->D);
+    (e->D <= 256 ? readout::readout_bwd_kernel<8> : readout::readout_bwd_kernel<16>)<<<blocks, 256, 0, (cudaStream_t)stream>>>(
+        h_last, h0, w, (const int*)(g + e->ro_off_graph_of), mask, d_out, d_h_last, d_w_gate, d_b_gate, d_w_trans, d_b_trans, V, e->D);
     CU_TRY(e, cudaGetLastError());
     return GGNN_OK;
 }

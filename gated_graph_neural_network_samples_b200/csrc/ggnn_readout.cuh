@@ -13,7 +13,8 @@
 namespace ggnn {
 namespace readout {
 
-constexpr int MAX_D_PER_LANE = 8;   // D <= 256
+// The backward kernels hold DPL columns per lane (column lane + 32 j): instances DPL = 8 for D <= 256 and DPL = 16 for 256 < D <= 512.
+constexpr int MAX_D_PER_LANE = 16;
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -96,22 +97,31 @@ __global__ void __launch_bounds__(128) readout_sum_permuted_kernel(const float* 
 // sums to its own shared row, the block adds the rows in warp order and stores its partial [d_w_gate | d_w_trans | d_b_gate | d_b_trans]
 // ([3D+2]) to part[blockIdx.x]; readout_bwd_reduce_kernel adds the blocks.  The grid must then not depend on the GPU (the grid-stride loop
 // gives every warp its nodes by gridDim).
-constexpr int RO_ROW = 3 * 256 + 2;   // [d_w_gate(h_T part) | d_w_gate(h_0 part) | d_w_trans] for d < 256, then the two biases
+// A warp's row of sums: [d_w_gate(h_T part) | d_w_gate(h_0 part) | d_w_trans] for d < 32*DPL, then the two biases
+template <int DPL>
+__host__ __device__ constexpr int ro_row() { return 3 * 32 * DPL + 2; }
+// Shared memory of the ordered instance: 8 warp rows, over the 48 KiB of static shared memory at DPL = 16 (dynamic there)
+template <int DPL>
+__host__ __device__ constexpr size_t ro_ordered_smem() { return 8 * ro_row<DPL>() * sizeof(float); }
 constexpr int RO_ORDERED_BLOCKS = 512;
-template <bool ORDERED>
+template <int DPL, bool ORDERED>
 __device__ __forceinline__ void readout_bwd(const float* __restrict__ h_last, const float* __restrict__ h0, const Weights& w,
                                             const int* __restrict__ graph_of, const float* __restrict__ mask, const float* __restrict__ d_out,
                                             float* __restrict__ d_h_last, float* __restrict__ d_w_gate, float* __restrict__ d_b_gate,
                                             float* __restrict__ d_w_trans, float* __restrict__ d_b_trans, float* __restrict__ part, int V, int D) {
-    __shared__ float red[ORDERED ? 8 * RO_ROW : RO_ROW];
+    constexpr int RO_ROW = ro_row<DPL>(), W = 32 * DPL;
+    constexpr bool DYN = ORDERED && ro_ordered_smem<DPL>() > 48 * 1024;
+    __shared__ float red_static[DYN ? 1 : (ORDERED ? 8 * RO_ROW : RO_ROW)];
+    extern __shared__ float red_dynamic[];
+    float* red = DYN ? red_dynamic : red_static;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (!ORDERED) {
-        for (int i = threadIdx.x; i < 3 * 256 + 2; i += 256) red[i] = 0.f;
+        for (int i = threadIdx.x; i < RO_ROW; i += 256) red[i] = 0.f;
         __syncthreads();
     }
-    float gw_a[MAX_D_PER_LANE], gw_b[MAX_D_PER_LANE], tw[MAX_D_PER_LANE];
+    float gw_a[DPL], gw_b[DPL], tw[DPL];
 #pragma unroll
-    for (int j = 0; j < MAX_D_PER_LANE; ++j) gw_a[j] = gw_b[j] = tw[j] = 0.f;
+    for (int j = 0; j < DPL; ++j) gw_a[j] = gw_b[j] = tw[j] = 0.f;
     float gb = 0.f, tb = 0.f;
     for (int v = blockIdx.x * 8 + warp; v < V; v += gridDim.x * 8) {
         const float* hT = h_last + (size_t)v * D;
@@ -123,7 +133,7 @@ __device__ __forceinline__ void readout_bwd(const float* __restrict__ h_last, co
         const float dgp = go * tp * g * (1.0f - g);   // d gate pre-activation
         const float dt = go * g;                      // d transform output
 #pragma unroll
-        for (int j = 0; j < MAX_D_PER_LANE; ++j) {
+        for (int j = 0; j < DPL; ++j) {
             const int d = lane + 32 * j;
             if (d < D) {
                 const float a = hT[d];
@@ -138,16 +148,16 @@ __device__ __forceinline__ void readout_bwd(const float* __restrict__ h_last, co
     if (ORDERED) {
         float* row = red + warp * RO_ROW;
 #pragma unroll
-        for (int j = 0; j < MAX_D_PER_LANE; ++j) {
+        for (int j = 0; j < DPL; ++j) {
             const int d = lane + 32 * j;
-            if (d < D) { row[d] = gw_a[j]; row[256 + d] = gw_b[j]; row[512 + d] = tw[j]; }
+            if (d < D) { row[d] = gw_a[j]; row[W + d] = gw_b[j]; row[2 * W + d] = tw[j]; }
         }
-        if (lane == 0) { row[768] = gb; row[769] = tb; }
+        if (lane == 0) { row[3 * W] = gb; row[3 * W + 1] = tb; }
         __syncthreads();
         float* out = part + (size_t)blockIdx.x * (3 * D + 2);
         for (int c = threadIdx.x; c < 3 * D + 2; c += 256) {
             // column c of the partial: [0, 2D) d_w_gate, [2D, 3D) d_w_trans, 3D d_b_gate, 3D+1 d_b_trans
-            const int src = c < D ? c : c < 2 * D ? 256 + c - D : c < 3 * D ? 512 + c - 2 * D : 768 + c - 3 * D;
+            const int src = c < D ? c : c < 2 * D ? W + c - D : c < 3 * D ? 2 * W + c - 2 * D : 3 * W + c - 3 * D;
             float a = red[src];
             for (int q = 1; q < 8; ++q) a += red[q * RO_ROW + src];
             out[c] = a;
@@ -155,34 +165,37 @@ __device__ __forceinline__ void readout_bwd(const float* __restrict__ h_last, co
         return;
     }
 #pragma unroll
-    for (int j = 0; j < MAX_D_PER_LANE; ++j) {
+    for (int j = 0; j < DPL; ++j) {
         const int d = lane + 32 * j;
-        if (d < D) { atomicAdd(&red[d], gw_a[j]); atomicAdd(&red[256 + d], gw_b[j]); atomicAdd(&red[512 + d], tw[j]); }
+        if (d < D) { atomicAdd(&red[d], gw_a[j]); atomicAdd(&red[W + d], gw_b[j]); atomicAdd(&red[2 * W + d], tw[j]); }
     }
-    if (lane == 0) { atomicAdd(&red[768], gb); atomicAdd(&red[769], tb); }
+    if (lane == 0) { atomicAdd(&red[3 * W], gb); atomicAdd(&red[3 * W + 1], tb); }
     __syncthreads();
     for (int d = threadIdx.x; d < D; d += 256) {
-        if (d_w_gate) { atomicAdd(d_w_gate + d, red[d]); atomicAdd(d_w_gate + D + d, red[256 + d]); }
-        if (d_w_trans) atomicAdd(d_w_trans + d, red[512 + d]);
+        if (d_w_gate) { atomicAdd(d_w_gate + d, red[d]); atomicAdd(d_w_gate + D + d, red[W + d]); }
+        if (d_w_trans) atomicAdd(d_w_trans + d, red[2 * W + d]);
     }
     if (threadIdx.x == 0) {
-        if (d_b_gate) atomicAdd(d_b_gate, red[768]);
-        if (d_b_trans) atomicAdd(d_b_trans, red[769]);
+        if (d_b_gate) atomicAdd(d_b_gate, red[3 * W]);
+        if (d_b_trans) atomicAdd(d_b_trans, red[3 * W + 1]);
     }
 }
+template <int DPL>
 __global__ void __launch_bounds__(256) readout_bwd_kernel(const float* __restrict__ h_last, const float* __restrict__ h0, Weights w,
                                                           const int* __restrict__ graph_of, const float* __restrict__ mask,
                                                           const float* __restrict__ d_out, float* __restrict__ d_h_last,
                                                           float* __restrict__ d_w_gate, float* __restrict__ d_b_gate,
                                                           float* __restrict__ d_w_trans, float* __restrict__ d_b_trans, int V, int D) {
-    readout_bwd<false>(h_last, h0, w, graph_of, mask, d_out, d_h_last, d_w_gate, d_b_gate, d_w_trans, d_b_trans, nullptr, V, D);
+    readout_bwd<DPL, false>(h_last, h0, w, graph_of, mask, d_out, d_h_last, d_w_gate, d_b_gate, d_w_trans, d_b_trans, nullptr, V, D);
 }
-// part: [gridDim.x][3D+2] block partials, reduced by readout_bwd_reduce_kernel
+// part: [gridDim.x][3D+2] block partials, reduced by readout_bwd_reduce_kernel; launched with ro_ordered_smem<16>() bytes of dynamic shared
+// memory at DPL = 16
+template <int DPL>
 __global__ void __launch_bounds__(256) readout_bwd_ordered_kernel(const float* __restrict__ h_last, const float* __restrict__ h0, Weights w,
                                                                   const int* __restrict__ graph_of, const float* __restrict__ mask,
                                                                   const float* __restrict__ d_out, float* __restrict__ d_h_last,
                                                                   float* __restrict__ part, int V, int D) {
-    readout_bwd<true>(h_last, h0, w, graph_of, mask, d_out, d_h_last, nullptr, nullptr, nullptr, nullptr, part, V, D);
+    readout_bwd<DPL, true>(h_last, h0, w, graph_of, mask, d_out, d_h_last, nullptr, nullptr, nullptr, nullptr, part, V, D);
 }
 // one block per column of the [blocks][3D+2] partials: the blocks added in a fixed order (ggnn::bwd::ordered_column_sum), then once into the
 // caller's gradient (any of the four may be NULL)

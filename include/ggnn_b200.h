@@ -92,7 +92,12 @@ typedef struct ggnn_layer_grads {
     float* cand_hidden_bias;
 } ggnn_layer_grads;
 
-/* prepare_specific_graph_model (sparse:63-115 / dense:68-91): fix the model shape. */
+/* prepare_specific_graph_model (sparse:63-115 / dense:68-91): fix the model shape.
+ * Limits: hidden_size a positive multiple of 4 and <= 512 (larger: GGNN_EUNSUPPORTED), 1 <= num_edge_types <= 32 (<= 16 with propagation
+ * attention), 1 <= num_layers <= 16, at most 4 residual inputs per layer.  Kernels by hidden size: GGNN_PREC_BF16X3 / GGNN_PREC_BF16 run
+ * the tile-local wgmma kernel up to 128 and the streaming wgmma kernels above; GGNN_PREC_FP32 (and attention, and CudnnCompatibleGRUCell,
+ * at any precision) runs the fused fp32 tile kernel up to 256 and the per-timestep fp32 path above 256.  A weighted dense adjacency runs
+ * on tensor cores up to hidden 128 only. */
 int ggnn_create(const ggnn_config* cfg, ggnn_engine** out);
 int ggnn_destroy(ggnn_engine* e);
 const char* ggnn_last_error(const ggnn_engine* e); /* e may be NULL: error of the last failed ggnn_create */
