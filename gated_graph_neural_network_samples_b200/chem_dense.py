@@ -45,6 +45,7 @@ class DenseGGNNChemModel(ChemModel):
         self._padded_hidden = (h_dim + 3) // 4 * 4
         self.engine = PropagationEngine(dense_engine_params(dict(self.params, hidden_size=self._padded_hidden)), T,
                                         device=self.device.index or 0, precision=self.precision)
+        self._apply_backward_precision(self.engine)
         self._propagation = _propagation_function()
         self._readout = gated_readout_function()
 

@@ -93,6 +93,7 @@ class SparseGCNChemModel(ChemModel):
         self._padded_hidden = (h_dim + 3) // 4 * 4
         self.engine = GCNEngine(self._padded_hidden, L, self.params['gcn_use_bias'], device=self.device.index or 0,
                                 precision=self.precision)
+        self._apply_backward_precision(self.engine)
         self._propagation = _propagation_function()
         self._readout = gated_readout_function()
 

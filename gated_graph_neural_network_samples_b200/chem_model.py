@@ -57,6 +57,10 @@ class ChemModel(object):
         # against a stand-in engine (tests/test_chem_model_cpu.py)
         self.device = torch.device("cpu") if dev == "cpu" else torch.device("cuda", int(dev or 0))
         self.precision = args.get('--precision') or "fp32"
+        # the precision of the engine's backward GEMMs (ggnn_set_backward_precision); None leaves the engine's default (fp32) untouched
+        self.backward_precision = args.get('--backward-precision')
+        if self.backward_precision is not None and self.backward_precision not in ("fp32", "bf16x3"):
+            raise Exception("Unknown backward precision '%s' (expected fp32 or bf16x3)." % self.backward_precision)
 
         self.max_num_vertices = self.num_edge_types = self.annotation_size = 0
         self.train_data, self.valid_data = (self.load_data(self.params[k], is_training_data=t)
@@ -69,6 +73,11 @@ class ChemModel(object):
             self.train_step_id, self.valid_step_id = self.restore_progress(args.get('--restore'))
         else:
             self.initialize_model()
+
+    def _apply_backward_precision(self, engine):
+        """Hook 1 of the plug-ins: --backward-precision, only when it was given (an engine without the setting keeps working)."""
+        if self.backward_precision is not None:
+            engine.set_backward_precision(self.backward_precision)
 
     @classmethod
     def _resolve_params(cls, args) -> dict:

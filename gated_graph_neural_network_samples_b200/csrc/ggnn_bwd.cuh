@@ -114,6 +114,9 @@ __global__ void __launch_bounds__(128) gemm_nt_kernel(const float* __restrict__ 
 // 64x64 output tile, 64 threads x (8x8), rows in slabs of 16.  a_vec = 0 selects scalar loads of A (the [V,T] in-degree table
 // of the edge-bias gradient, whose row length need not be a multiple of 4); B, C, ldb, ldc, N as for gemm_nt.
 constexpr int MAX_SEGS = 16;
+// The output tile (K and N) of every weight-gradient kernel, FFMA and tensor-core (ggnn_bwd_tc.cuh): the host's split policy sizes its grids
+// and the deterministic workspace by it.
+constexpr int TN_TILE = 64;
 struct SegList {
     const float* p[MAX_SEGS];
     int ld[MAX_SEGS];

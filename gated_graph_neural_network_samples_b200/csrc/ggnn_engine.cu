@@ -25,6 +25,7 @@
 #include "../../include/ggnn_b200.h"
 #include "ggnn_common.cuh"
 #include "ggnn_bwd.cuh"
+#include "ggnn_bwd_tc.cuh"
 #include "ggnn_readout.cuh"
 #include "ggnn_fwd_ffma.cuh"
 #include "ggnn_fwd_tc.cuh"
@@ -236,6 +237,7 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     bool save = false;
     bool saved_valid = false;   // the saved activations are those of the last forward, with the current weights
     bool det = false;           // ggnn_set_deterministic: fixed-order weight-gradient and readout sums
+    int bwd_precision = GGNN_PREC_FP32;   // ggnn_set_backward_precision: the GEMMs of the backward on FFMA or on bf16x3 wgmma
     DevBuf ts_images;                                // the streaming plan's operand images and chunk-major states
     DevBuf ts_virt;                                  // the operand image of the streaming plan's virtual rows
     DevBuf att_buf;                  // attention probabilities per target-CSR slot ([steps][M] when saving for backward, else [M])
@@ -637,10 +639,11 @@ struct TnSplit {
 constexpr int DET_TARGET_CTAS = 512;
 constexpr int COLSUM_ROWS = 512;
 static TnSplit tn_split(int target_ctas, bool has_C, bool has_bias, int M, int N, int K, int nseg) {
+    using ggnn::bwd::TN_TILE;
     TnSplit p;
     if (has_C) {
-        const int kblocks = (K + 63) / 64;
-        const int tiles = ((N + 63) / 64) * nseg * kblocks;
+        const int kblocks = (K + TN_TILE - 1) / TN_TILE;
+        const int tiles = ((N + TN_TILE - 1) / TN_TILE) * nseg * kblocks;
         const int want = std::max(1, (target_ctas + tiles - 1) / tiles);
         const int splits = std::max(1, std::min(want, (M + 63) / 64));
         p.rows = ((M + splits - 1) / splits + ggnn::bwd::GEMM_BK - 1) / ggnn::bwd::GEMM_BK * ggnn::bwd::GEMM_BK;
@@ -663,12 +666,19 @@ static int gemm_tn(ggnn_engine* e, cudaStream_t st, float* ws, size_t ws_cap, co
                    int ldb, float* C, int ldc, size_t c_stride, float* bias, int M, int N, int K) {
     using namespace ggnn::bwd;
     if (!C && !bias) return GGNN_OK;
-    const int kblocks = (K + 63) / 64;
+    const int kblocks = (K + TN_TILE - 1) / TN_TILE;
+    const dim3 tiles((N + TN_TILE - 1) / TN_TILE, nseg * kblocks);
+    // bf16x3 backward: the tensor-core kernels take every vector-loaded A (the edge-bias gradient's in-degree table stays on FFMA)
+    const bool tcore = e->bwd_precision == GGNN_PREC_BF16X3 && a_vec;
     if (!e->det) {
         if (C) {
             const TnSplit p = tn_split(4 * e->num_sms, true, false, M, N, K, nseg);
-            gemm_tn_atomic_kernel<<<dim3((N + 63) / 64, nseg * kblocks, p.splits), 64, 0, st>>>(segs, kblocks, a_vec ? 1 : 0, B, ldb, C, ldc,
-                                                                                                c_stride, bias, M, N, K, p.rows);
+            const dim3 grid(tiles.x, tiles.y, p.splits);
+            if (tcore)
+                ggnn::bwd_tc::gemm_tn_tc_atomic_kernel<<<grid, ggnn::bwd_tc::TN_TC_THREADS, 0, st>>>(segs, kblocks, B, ldb, C, ldc, c_stride, bias,
+                                                                                                      M, N, K, p.rows);
+            else
+                gemm_tn_atomic_kernel<<<grid, 64, 0, st>>>(segs, kblocks, a_vec ? 1 : 0, B, ldb, C, ldc, c_stride, bias, M, N, K, p.rows);
         } else {
             colsum_atomic_kernel<<<dim3((N + 255) / 256, (M + COLSUM_ROWS - 1) / COLSUM_ROWS), 256, 0, st>>>(B, ldb, nullptr, 0, bias, M, N,
                                                                                                               COLSUM_ROWS);
@@ -681,13 +691,32 @@ static int gemm_tn(ggnn_engine* e, cudaStream_t st, float* ws, size_t ws_cap, co
         return e->fail(GGNN_ESTATE, "internal: the deterministic workspace holds %zu floats, a weight-gradient launch (M %d, N %d, K %d, %d segments) "
                                     "needs %zu", ws_cap, M, N, K, nseg, p.ws_floats);
     float* bias_part = bias ? ws + (C ? (size_t)p.splits * nseg * K * N : 0) : nullptr;
-    if (C) gemm_tn_split_kernel<<<dim3((N + 63) / 64, nseg * kblocks, p.splits), 64, 0, st>>>(segs, kblocks, a_vec ? 1 : 0, B, ldb, ws, bias_part,
-                                                                                               M, N, K, p.rows);
+    const dim3 grid(tiles.x, tiles.y, p.splits);
+    if (C && tcore)
+        ggnn::bwd_tc::gemm_tn_tc_split_kernel<<<grid, ggnn::bwd_tc::TN_TC_THREADS, 0, st>>>(segs, kblocks, B, ldb, ws, bias_part, M, N, K, p.rows);
+    else if (C) gemm_tn_split_kernel<<<grid, 64, 0, st>>>(segs, kblocks, a_vec ? 1 : 0, B, ldb, ws, bias_part, M, N, K, p.rows);
     else colsum_split_kernel<<<dim3((N + 255) / 256, p.splits), 256, 0, st>>>(B, ldb, bias_part, M, N, p.rows);
     const size_t work = (C ? (size_t)nseg * K * N / 4 : 0) + (bias ? N : 0);
     split_reduce_kernel<<<(int)std::min<size_t>((work + 255) / 256, 4096), 256, 0, st>>>(ws, bias_part, p.splits, nseg, K, N, C, ldc, c_stride, bias);
     e->last_launches += 2;
     return GGNN_OK;
+}
+// The data-gradient launch  C[M,N] (+)= sum_s A_s[M,K] . B_s[N,K]^T  of the GGNN and the GCN backward: gemm_nt_kernel (FFMA), or its bf16x3
+// wgmma twin when the engine's backward precision says so.  One CTA per output tile over the whole sum either way (no split-K).
+static void gemm_nt(ggnn_engine* e, cudaStream_t st, bool acc, const float* A, int lda, int a_stride, const float* B, int ldb, int b_stride, int nseg,
+                    float* C, int ldc, int M, int N, int K) {
+    using namespace ggnn::bwd;
+    using namespace ggnn::bwd_tc;
+    if (e->bwd_precision == GGNN_PREC_BF16X3) {
+        const dim3 grid((N + NT_TC_BN - 1) / NT_TC_BN, (M + NT_TC_BM - 1) / NT_TC_BM);
+        if (acc) gemm_nt_tc_kernel<true><<<grid, NT_TC_THREADS, 0, st>>>(A, lda, a_stride, B, ldb, b_stride, nseg, C, ldc, M, N, K);
+        else gemm_nt_tc_kernel<false><<<grid, NT_TC_THREADS, 0, st>>>(A, lda, a_stride, B, ldb, b_stride, nseg, C, ldc, M, N, K);
+    } else {
+        const dim3 grid((N + NT_BN - 1) / NT_BN, (M + NT_BM - 1) / NT_BM);
+        if (acc) gemm_nt_kernel<true><<<grid, 128, 0, st>>>(A, lda, a_stride, B, ldb, b_stride, nseg, C, ldc, M, N, K);
+        else gemm_nt_kernel<false><<<grid, 128, 0, st>>>(A, lda, a_stride, B, ldb, b_stride, nseg, C, ldc, M, N, K);
+    }
+    ++e->last_launches;
 }
 
 // The gradient fields of layer l the model has, with their sizes in floats, in ggnn_layer_grads order (a field the model lacks: size 0).
@@ -766,12 +795,7 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
     const long long n = (long long)vd;
     const int eb = (int)std::min<long long>((n + 255) / 256, 4096);
     auto gemm_nt = [&](bool acc, const float* A, int lda, int a_stride, const float* B, int ldb, int b_stride, int nseg, float* C, int ldc,
-                       int M, int N, int K) {
-        dim3 grid((N + NT_BN - 1) / NT_BN, (M + NT_BM - 1) / NT_BM);
-        if (acc) gemm_nt_kernel<true><<<grid, 128, 0, st>>>(A, lda, a_stride, B, ldb, b_stride, nseg, C, ldc, M, N, K);
-        else gemm_nt_kernel<false><<<grid, 128, 0, st>>>(A, lda, a_stride, B, ldb, b_stride, nseg, C, ldc, M, N, K);
-        ++e->last_launches;
-    };
+                       int M, int N, int K) { ::gemm_nt(e, st, acc, A, lda, a_stride, B, ldb, b_stride, nseg, C, ldc, M, N, K); };
     // C_s[K,N] += A_s^T . B for every segment (C_s = C + s*c_stride), bias[n] += sum_m B[m,n]
     int ws_rc = GGNN_OK;   // the first failure of a weight-gradient launch (none launches after it)
     auto gemm_tn = [&](const SegList& segs, int nseg, bool a_vec, const float* B, int ldb, float* C, int ldc, size_t c_stride, float* bias, int M,
@@ -2328,11 +2352,11 @@ static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream
     return GGNN_OK;
 }
 
-// Backward of the GCN layers, fp32 on CUDA cores, per layer in reverse:
+// Backward of the GCN layers, per layer in reverse (the two GEMMs on FFMA, or on bf16x3 wgmma: ggnn_set_backward_precision):
 //   dPre = dOut (last layer) or dOut * relu'(y) * mask / keep (gcn_relu_dropout_grad_kernel, from the saved output y)
 //   S    = A . H_l (recomputed from the saved layer input: one gather instead of L saved [V, D] arrays)
 //   dW  += S^T . dPre,  db += sum dPre            (gemm_tn: atomic or fixed-order split sums, the bias rides along)
-//   dS   = dPre . W^T                             (gemm_nt_kernel)
+//   dS   = dPre . W^T                             (gemm_nt)
 //   dH_l = A^T . dS                               (csr_gather_all_kernel over the source-keyed CSR with its per-slot weights: no float atomics)
 int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0, ggnn_stream_t stream) {
     using namespace ggnn::bwd;
@@ -2378,12 +2402,11 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
             if (int rc = gemm_tn(e, st, ws, ws_floats, none, 1, true, dpre, D, nullptr, D, 0, gw.bias, V, D, D)) return rc;
         }
         if (l == 0 && !d_h0) break;
-        gemm_nt_kernel<false><<<dim3((D + NT_BN - 1) / NT_BN, (V + NT_BM - 1) / NT_BM), 128, 0, st>>>(dpre, D, 0, e->gcn_w[l].kernel, D, 0, 1, dS, D, V,
-                                                                                                      D, D);
+        gemm_nt(e, st, false, dpre, D, 0, e->gcn_w[l].kernel, D, 0, 1, dS, D, V, D, D);
         float* dst = l == 0 ? d_h0 : dH;
         GatherJob j{gd.trow, gd.ttgt, dS, dst, gd.tslot_w, nullptr};
         csr_gather_all_kernel<<<gather_grid, 256, 0, st>>>(j, j, V, D, 1);
-        e->last_launches += 2;
+        ++e->last_launches;
         dout = dst;
     }
     CU_TRY(e, cudaGetLastError());
@@ -2665,6 +2688,15 @@ int ggnn_set_save_for_backward(ggnn_engine* e, int32_t enable) {
 int ggnn_set_deterministic(ggnn_engine* e, int32_t enable) {
     if (!e) return GGNN_EINVAL;
     e->det = enable != 0;
+    return GGNN_OK;
+}
+
+int ggnn_set_backward_precision(ggnn_engine* e, int32_t precision) {
+    if (!e) return GGNN_EINVAL;
+    if (precision != GGNN_PREC_FP32 && precision != GGNN_PREC_BF16X3)
+        return e->fail(GGNN_EINVAL, "backward precision must be GGNN_PREC_FP32 (%d) or GGNN_PREC_BF16X3 (%d), got %d", GGNN_PREC_FP32,
+                       GGNN_PREC_BF16X3, (int)precision);
+    e->bwd_precision = precision;
     return GGNN_OK;
 }
 

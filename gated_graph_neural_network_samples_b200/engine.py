@@ -13,6 +13,7 @@ import numpy as np
 from . import _lib
 
 PRECISIONS = {"fp32": 0, "bf16x3": 1, "bf16": 2}
+BACKWARD_PRECISIONS = ("fp32", "bf16x3")   # ggnn_set_backward_precision
 WEIGHT_FIELDS = ("edge_weights", "edge_biases", "gate_kernel", "gate_bias", "cand_kernel", "cand_bias", "edge_type_attention_weights",
                  "cand_hidden_bias")
 # params['graph_rnn_cell'].lower() (sparse:102-112) -> GGNN_CELL_*
@@ -438,6 +439,13 @@ class PropagationEngine:
         """``ggnn_set_deterministic``: fixed-order weight-gradient and readout sums from the next call on, so that the same inputs give
         the same bits in every output and gradient (the autograd nodes set it from ``torch.are_deterministic_algorithms_enabled()``)."""
         self._check(self.lib.ggnn_set_deterministic(self._h, int(bool(enable))))
+
+    def set_backward_precision(self, precision: str):
+        """``ggnn_set_backward_precision``: "fp32" (the default, FFMA) or "bf16x3" (the backward's GEMMs on tensor cores, each gradient
+        within 2e-4 of float64 relative to its largest entry).  Takes effect at the next backward; the forward is not touched."""
+        if precision not in BACKWARD_PRECISIONS:
+            raise ValueError("unknown backward precision %r (expected one of %s)" % (precision, ", ".join(BACKWARD_PRECISIONS)))
+        self._check(self.lib.ggnn_set_backward_precision(self._h, PRECISIONS[precision]))
 
     def backward(self, d_out, grads: Sequence[dict], d_h0=None):
         arr = (_lib.GgnnLayerGrads * len(grads))()

@@ -245,6 +245,15 @@ int ggnn_set_save_for_backward(ggnn_engine* e, int32_t enable);
  * graph_nodes_list is summed per graph in node order.  The forward and d h0 are bit-reproducible in either mode.  With it off the weight
  * gradients and an ungrouped readout sum are added with float atomics, equal only within their ordering noise. */
 int ggnn_set_deterministic(ggnn_engine* e, int32_t enable);
+/* Precision of the backward pass's GEMMs (GGNN and GCN engines; GGNN_PREC_FP32 by default).  GGNN_PREC_FP32: FFMA on CUDA cores.
+ * GGNN_PREC_BF16X3: sm_90a wgmma tensor cores with the forward's hi/lo split (three bf16 MMAs per product, fp32 accumulators) for every data
+ * gradient (the cell kernels, dh += sum_t G_t . W_t^T, attention's dx' . W^T, the GCN's dS) and every weight gradient but the edge biases;
+ * bias gradients stay fp32 column sums, the elementwise, gather and attention kernels are unchanged.  Expect each gradient tensor within
+ * max|err| / max|ref| < 2e-4 of float64 (the forward's bf16x3 bar).  Independent of the forward's precision and of ggnn_set_deterministic
+ * (which keeps its guarantees: d h0 bit-reproducible, the weight gradients too with it on).  Takes effect at the next backward call and
+ * touches nothing else (the forward, the saved activations, the plan): switching between two backward calls on one saved forward is fine.
+ * GGNN_PREC_BF16 and unknown values return GGNN_EINVAL and keep the setting. */
+int ggnn_set_backward_precision(ggnn_engine* e, int32_t precision);
 int ggnn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers,
                   float* d_h0, ggnn_stream_t stream);
 
