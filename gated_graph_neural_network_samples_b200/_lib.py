@@ -63,6 +63,7 @@ SYMBOLS = {
                                            C.POINTER(C.c_int32), C.c_char_p, C.c_int32]),
     "ggnn_prepared_graph_arrays": (C.c_int, [C.c_void_p] + [C.c_void_p] * 6),
     "ggnn_prepared_graph_image": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64]),
+    "ggnn_prepared_graph_tile_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "ggnn_set_graph_dense": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "ggnn_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ggnn_forward_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -100,6 +101,24 @@ SYMBOLS = {
     "ggnn_set_graph_gcn": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ggnn_prepared_graph_slot_weights": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "ggnn_gcn_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GcnLayerWeights), C.c_int32, C.c_void_p, C.c_void_p]),
+    "ggnn_dataset_create_sparse": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int32,
+                                             C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "ggnn_host_dataset_create_sparse": (C.c_int, [C.POINTER(GgnnConfig), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p),
+                                                  C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                                  C.POINTER(C.c_void_p)]),
+    "ggnn_dataset_create_gcn": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                          C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "ggnn_host_dataset_create_gcn": (C.c_int, [C.POINTER(GcnConfig), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
+    "ggnn_free_dataset": (C.c_int, [C.c_void_p]),
+    "ggnn_dataset_error": (C.c_char_p, [C.c_void_p]),
+    "ggnn_dataset_prepare_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]),
+    "ggnn_dataset_batch_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int64),
+                                          C.POINTER(C.c_int32), C.c_char_p, C.c_int32, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "ggnn_free_dataset_batch": (C.c_int, [C.c_void_p]),
+    "ggnn_dataset_batch_error": (C.c_char_p, [C.c_void_p]),
+    "ggnn_set_graph_dataset": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ggnn_graph_image": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int64), C.c_void_p]),
 }
 
 _lib = None

@@ -110,8 +110,10 @@ class SparseGCNChemModel(ChemModel):
         feed = self.feed
         D, DP = self.params['hidden_size'], self._padded_hidden
         h0 = self.initial_node_representation_tensor()
-        self.engine.set_save_for_backward(torch.is_grad_enabled())   # before set_graph: the source-keyed CSR is built there
-        if not self._adopt_prepared_graph(feed):
+        # a device-data batch was assembled on the device by forward_batch (_adopt_dataset_batch)
+        if not feed.get('_graph_adopted'):
+            self.engine.set_save_for_backward(torch.is_grad_enabled())   # before set_graph: the source-keyed CSR is built there
+        if not feed.get('_graph_adopted') and not self._adopt_prepared_graph(feed):
             self.engine.set_graph_gcn(h0.shape[0], feed[self.placeholders['adjacency_list']], feed[self.placeholders['adjacency_weights']])
         # tf.nn.dropout after the ReLU of every layer but the last (gcn:75-78): done inside the kernels; a fresh mask seed per run, drawn
         # from torch's generator (seeded by params['random_seed'] like tf.set_random_seed, chem_tensorflow.py:85)
@@ -146,6 +148,11 @@ class SparseGCNChemModel(ChemModel):
         # flattened once per dataset (packing.FlatGCNGraphs); every batch is then a handful of NumPy gathers instead of the per-graph loop
         # of gcn:150-197 -- same arrays, bit for bit, under the same strict node_offset + n < batch_size rule
         flat, order = self._flat_view(data, packing.FlatGCNGraphs)
+        if getattr(self, 'device_data', False):   # the same batches, assembled on the device from the uploaded list (forward_batch adopts them)
+            for ids in flat.iter_batch_ids(order, self.params['batch_size']):
+                yield {'num_graphs': len(ids), 'graph_state_keep_prob': keep, '_graph_sizes': flat.n_nodes[ids],
+                       '_dataset_batch': self._dataset_batch(flat, ids, is_training)}
+            return
         for b in flat.iter_minibatches(order, self.params['batch_size'], self.params['hidden_size']):
             feed = dict(b, graph_state_keep_prob=keep)
             # this generator runs in ChemModel.run_epoch's ThreadedIterator (chem_tensorflow.py:225): the engine's host half of the batch

@@ -61,6 +61,12 @@ class ChemModel(object):
         self.backward_precision = args.get('--backward-precision')
         if self.backward_precision is not None and self.backward_precision not in ("fp32", "bf16x3"):
             raise Exception("Unknown backward precision '%s' (expected fp32 or bf16x3)." % self.backward_precision)
+        # --device-data: the plug-in uploads each data list once (engine.DeviceDataset) and assembles every batch on the GPU instead of
+        # packing it on the host; same shuffle, same batches, same numbers.  A command-line option, not a params key: params are what a
+        # checkpoint must match (restore_progress), and where the data lives does not change the model.
+        self.device_data = bool(args.get('--device-data'))
+        if self.device_data and self.device.type != "cuda":
+            raise Exception("--device-data keeps the data on the GPU: it needs a CUDA device, not %s" % self.device)
 
         self.max_num_vertices = self.num_edge_types = self.annotation_size = 0
         self.train_data, self.valid_data = (self.load_data(self.params[k], is_training_data=t)
@@ -150,14 +156,14 @@ class ChemModel(object):
         """One ``sess.run`` worth of forward work on ``feed`` (chem_tensorflow.py:235 with the ops of :145-170)."""
         import torch
         self.feed = feed
+        self._adopt_dataset_batch(feed)
         keep = float(feed.get(self.placeholders['out_layer_dropout_keep_prob'], 1.0))
         if self.params['use_graph']:
             final = self.compute_final_node_representations()            # :145
         else:
             final = torch.zeros_like(self.initial_node_representation_tensor())   # :147
         self.ops['final_node_representations'] = final
-        tv = torch.as_tensor(np.asarray(feed[self.placeholders['target_values']], dtype=np.float32), device=self.device)
-        tm = torch.as_tensor(np.asarray(feed[self.placeholders['target_mask']], dtype=np.float32), device=self.device)
+        tv, tm = (self._as_device_tensor(feed[self.placeholders[k]]) for k in ('target_values', 'target_mask'))
         losses, accs = [], []
         self._task_sums = []      # per task: (ratio * sum of masked 0.5*diff^2 [graph attached], mask sum) -- what data parallelism exchanges
         for internal_id, task_id in enumerate(self.params['task_ids']):
@@ -263,9 +269,15 @@ class ChemModel(object):
     def after_weight_update(self):
         pass
 
-    def initial_node_representation_tensor(self):
+    def _as_device_tensor(self, x):
+        """A feed's float array as an fp32 tensor on the model's device; a device-data batch's feed already holds one."""
         import torch
-        return torch.as_tensor(np.asarray(self.feed[self.placeholders['initial_node_representation']], dtype=np.float32), device=self.device)
+        if torch.is_tensor(x):
+            return x
+        return torch.as_tensor(np.asarray(x, dtype=np.float32), device=self.device)
+
+    def initial_node_representation_tensor(self):
+        return self._as_device_tensor(self.feed[self.placeholders['initial_node_representation']])
 
     # ------------------------------------------------------------------ batch plumbing the plug-ins share
     def _flat_view(self, data, flatten):
@@ -301,6 +313,48 @@ class ChemModel(object):
         self.engine.set_graph_prepared(prepared)
         self.__dict__.setdefault('_prepared_pool', []).append(prepared)   # rebuilt in place for a later batch; a rebuild first waits for this upload
         return True
+
+    def _dataset_batch(self, flat, ids, is_training: bool):
+        """--device-data, in the batch producer thread: the host half of the batch of flat ids ``ids`` (engine.DatasetBatch), from the
+        dataset of ``flat`` -- uploaded at its first batch and kept while the list keeps its flattened view (one per data list, like
+        _flat_view).  Batches taken back from the pool are rebuilt in place."""
+        from .engine import DeviceDataset
+        cache = self.__dict__.setdefault('_dataset_cache', [])
+        ds = next((d for f, d in cache if f is flat), None)
+        if ds is None:
+            # stream 0: the legacy default stream of the engine's device, usable from this thread; the call returns once the upload ran
+            ds = DeviceDataset.for_engine(self.engine, flat, for_training=True, stream=0)
+            cache[:] = [c for c in cache if c[0] is not flat][-3:] + [(flat, ds)]
+        pool = self.__dict__.setdefault('_dataset_batch_pool', [])
+        reuse = next((b for b in pool if b.dataset is ds), None)
+        if reuse is not None:
+            pool.remove(reuse)
+        return ds.prepare_batch(ids, save_for_backward=is_training, reuse=reuse)
+
+    def _adopt_dataset_batch(self, feed) -> None:
+        """--device-data, on the engine's thread: assembles the feed's dataset batch on the device and puts its h0, targets and mask (CUDA
+        tensors) into the feed slots the hooks read.  The readout map is set with it.  A feed without a dataset batch is left as it is."""
+        import torch
+        batch = feed.pop('_dataset_batch', None)
+        if batch is None:
+            return
+        self.engine.set_save_for_backward(torch.is_grad_enabled())   # before the upload: the source-keyed CSR is part of the image
+        h0, tv, tm = self.engine.set_graph_from_dataset(batch)
+        D = self.params['hidden_size']
+        feed[self.placeholders['initial_node_representation']] = h0[:, :D] if h0.shape[1] != D else h0   # the engine's width may be padded
+        feed[self.placeholders['target_values']], feed[self.placeholders['target_mask']] = tv, tm
+        feed['_graph_adopted'] = True
+        self.__dict__.setdefault('_dataset_batch_pool', []).append(batch)   # rebuilt in place later; a rebuild first waits for this upload
+
+    def _graph_nodes_list(self):
+        """The batch's node -> graph map as a long tensor on the device: the feed's array, or for a device-data batch the graphs' node
+        counts expanded on the device."""
+        import torch
+        gnl = self.feed.get(self.placeholders['graph_nodes_list'])
+        if gnl is not None:
+            return torch.as_tensor(np.asarray(gnl), device=self.device, dtype=torch.long)
+        sizes = torch.as_tensor(self.feed['_graph_sizes'], device=self.device)
+        return torch.repeat_interleave(torch.arange(sizes.shape[0], device=self.device), sizes)
 
     # ------------------------------------------------------------------ epoch loop (chem_tensorflow.py:214-253)
     # per-task "chemical accuracy" thresholds of QM9 the reference reports error ratios against (chem_tensorflow.py:215-217)

@@ -162,11 +162,14 @@ class SparseGGNNChemModel(ChemModel):
         import torch
         feed = self.feed
         T, D = self.num_edge_types, self.params['hidden_size']
-        adjacency_lists = [feed[k] for k in self.placeholders['adjacency_lists']]
-        self.engine.set_save_for_backward(torch.is_grad_enabled())   # before set_graph: the source-keyed CSR is built there
-        # the host half (CSR, tile plan, pinned image) was built by the batch producer thread when the feed carries it: only the upload is left
-        if not self._adopt_prepared_graph(feed):
-            self.engine.set_graph_sparse(adjacency_lists, feed[self.placeholders['num_incoming_edges_per_type']])
+        # a device-data batch was assembled on the device by forward_batch (_adopt_dataset_batch)
+        if not feed.get('_graph_adopted'):
+            self.engine.set_save_for_backward(torch.is_grad_enabled())   # before set_graph: the source-keyed CSR is built there
+            # the host half (CSR, tile plan, pinned image) was built by the batch producer thread when the feed carries it: only the upload
+            # is left
+            if not self._adopt_prepared_graph(feed):
+                adjacency_lists = [feed[k] for k in self.placeholders['adjacency_lists']]
+                self.engine.set_graph_sparse(adjacency_lists, feed[self.placeholders['num_incoming_edges_per_type']])
         state_keep = float(feed.get(self.placeholders['graph_state_keep_prob'], 1.0))
         # DropoutWrapper(state_keep_prob), sparse:113-114: done inside the kernels; a fresh mask seed per run, drawn from
         # torch's generator (seeded by params['random_seed'] like tf.set_random_seed, chem_tensorflow.py:85)
@@ -231,14 +234,16 @@ class SparseGGNNChemModel(ChemModel):
         ag = regression_gate.affine() if fused and hasattr(regression_gate, 'affine') else None
         at = regression_transform.affine() if fused and hasattr(regression_transform, 'affine') else None
         if ag is not None and at is not None:
-            # the fused kernel: both dot products, sigmoid, product and the per-graph segment sum in one launch
-            self.engine.readout_set_graphs(int(self.feed[self.placeholders['num_graphs']]),
-                                           graph_nodes_list=self.feed[self.placeholders['graph_nodes_list']])
+            # the fused kernel: both dot products, sigmoid, product and the per-graph segment sum in one launch (a device-data batch set
+            # its readout map with its graph)
+            if self.feed.get(self.placeholders['graph_nodes_list']) is not None:
+                self.engine.readout_set_graphs(int(self.feed[self.placeholders['num_graphs']]),
+                                               graph_nodes_list=self.feed[self.placeholders['graph_nodes_list']])
             self.output = self._readout.apply(self.engine, last_h, h0, ag[0], ag[1], at[0], at[1])
             return self.output
         gate_input = torch.cat([last_h, h0], dim=-1)
         gated_outputs = torch.sigmoid(regression_gate(gate_input)) * regression_transform(last_h)   # [v, 1]
-        gnl = torch.as_tensor(np.asarray(self.feed[self.placeholders['graph_nodes_list']]), device=self.device, dtype=torch.long)
+        gnl = self._graph_nodes_list()
         num_graphs = int(self.feed[self.placeholders['num_graphs']])
         out = torch.zeros(num_graphs, 1, device=self.device).index_add_(0, gnl, gated_outputs)   # unsorted_segment_sum
         self.output = out.squeeze(-1)
@@ -264,6 +269,11 @@ class SparseGGNNChemModel(ChemModel):
         # the processed graphs are flattened once per dataset (packing.FlatSparseGraphs); every batch is then a handful of NumPy gathers
         # instead of the per-graph loop of sparse:288-350 -- same arrays, bit for bit (tests/test_packing.py)
         flat, order = self._flat_view(data, lambda d: packing.FlatSparseGraphs(d, self.num_edge_types))   # kept across epochs (sparse:281-282)
+        if getattr(self, 'device_data', False):   # the same batches, assembled on the device from the uploaded list (forward_batch adopts them)
+            for ids in flat.iter_batch_ids(order, self.params['batch_size']):
+                yield {'num_graphs': len(ids), 'graph_state_keep_prob': state_keep, 'edge_weight_dropout_keep_prob': edge_keep,
+                       '_graph_sizes': flat.n_nodes[ids], '_dataset_batch': self._dataset_batch(flat, ids, is_training)}
+            return
         for b in flat.iter_minibatches(order, self.params['batch_size'], self.params['hidden_size']):
             feed = {k: b[k] for k in ('initial_node_representation', 'num_incoming_edges_per_type', 'graph_nodes_list',
                                       'target_values', 'target_mask', 'num_graphs')}

@@ -32,6 +32,7 @@
 #include "ggnn_fwd_stream.cuh"
 #include "ggnn_fwd_step.cuh"
 #include "ggnn_gcn.cuh"
+#include "ggnn_dataset.cuh"
 #include "ggnn_tc_smem.h"
 
 using namespace ggnn;
@@ -212,6 +213,8 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
 
     // device memory
     DevBuf graph_buf;   // the graph image of the current batch
+    size_t graph_bytes = 0;
+    DevBuf ds_table;    // the batch table of a dataset batch (ggnn_set_graph_dataset): tile starts and per-graph offsets
     GraphDev gd;        // ... and the view of it every driver reads
     // readout (gated_regression): node -> graph map of the current batch
     DevBuf ro_buf; StagedImage ro_stage;
@@ -1045,7 +1048,7 @@ int ggnn_create(const ggnn_config* cfg, ggnn_engine** out) {
 int ggnn_destroy(ggnn_engine* e) {
     if (!e) return GGNN_OK;
     cudaSetDevice(e->device);
-    e->graph_buf.release(); e->state_buf.release(); e->save_bufs.release(); e->io_buf.release(); e->bwd_buf.release();
+    e->graph_buf.release(); e->ds_table.release(); e->state_buf.release(); e->save_bufs.release(); e->io_buf.release(); e->bwd_buf.release();
     e->tc_tiles.buf.release(); e->tc_respre.release(); e->ts_tiles.buf.release(); e->ts_images.release(); e->ts_virt.release(); e->err_flag.release();
     e->step_wt.buf.release(); e->step_buf.release();
     if (e->own_prep) { ggnn_free_prepared_graph(e->own_prep); e->own_prep = nullptr; }
@@ -1240,6 +1243,43 @@ static bool host_team_is_fast(int team) {
 }
 #endif
 
+// The layout of a batch's graph image from its plan (V, ntiles, stream, weighted) and sizes: M messages, nv virtual rows holding nvm
+// messages (streaming plan); `save`: the image carries the source-keyed CSR.  Fills the plan's offsets and returns the image's size.  Shared
+// by the edge-list builder and the device-resident dataset (ggnn_dataset_prepare_batch), whose kernels write the same sections.
+static size_t layout_image(const ModelShape& shape, BatchPlan& p, bool save, int64_t M, int nv, int64_t nvm) {
+    const int V = p.V, T = shape.T, ntiles = p.ntiles;
+    size_t off = 0;
+    p.M = M;
+    p.off_row_ptr = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
+    p.off_src = off;     off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
+    p.off_msg = off;     off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
+    p.off_indeg = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1) * T, 16);
+    p.off_denom = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
+    p.off_tiles = off;   off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
+    p.off_mask = off;    off = align_up(off + sizeof(unsigned) * (size_t)std::max(ntiles, 1), 16);
+    p.has_transpose = save;
+    if (p.has_transpose) {
+        p.off_trow = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
+        p.off_ttgt = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
+        p.off_tslot = off;
+        if (shape.use_att) off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
+    }
+    // streaming plan: per (target, type) pair the ONE node to copy from (or none / a virtual row), see ggnn_fwd_stream.cuh
+    if (p.stream) {
+        p.off_pair = off; off = align_up(off + sizeof(int) * (size_t)std::max(ntiles, 1) * ts::TILE_M * T, 16);
+        p.off_vptr = off; off = align_up(off + sizeof(int) * (size_t)(nv + 1), 16);
+        p.off_vsrc = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(nvm, 1), 16);
+        p.off_tvp = off;  off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
+        p.off_vinfo = off; off = align_up(off + sizeof(int) * 8 * (size_t)std::max(nv, 1), 16);
+    }
+    if (p.weighted) {   // per-slot adjacency weights
+        p.off_slotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16);
+        if (p.has_transpose) { p.off_tslotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16); }
+    }
+    p.ts_nv = nv;
+    return off;
+}
+
 // ---- the host half of ggnn_set_graph_sparse: validation, tile plan, stable target-sorted CSR, streaming tables -> g->image.
 // `weighted`: the batch has one weight per message, `w`, in the type-major message order (required when there are messages); the image
 // then carries them in target-CSR order and, with the source-keyed CSR, in source-CSR order.
@@ -1395,37 +1435,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     }
     for (int k = 0; k < nth; ++k) { part_msgs[k + 1] += part_msgs[k]; part_nv[k + 1] += part_nv[k]; part_nvm[k + 1] += part_nvm[k]; }
 
-    // ---- layout of the packed upload
-    size_t off = 0;
-    p.off_row_ptr = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
-    p.off_src = off;     off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
-    p.off_msg = off;     off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
-    p.off_indeg = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1) * T, 16);
-    p.off_denom = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
-    p.off_tiles = off;   off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
-    p.off_mask = off;    off = align_up(off + sizeof(unsigned) * (size_t)std::max(ntiles, 1), 16);
-    p.has_transpose = g->save;
-    if (p.has_transpose) {
-        p.off_trow = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
-        p.off_ttgt = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
-        p.off_tslot = off;
-        if (shape.use_att) off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
-    }
-    // streaming plan: per (target, type) pair the ONE node to copy from (or none / a virtual row), see ggnn_fwd_stream.cuh
-    const int nv = (int)part_nv[nth];
-    const int64_t nvm = part_nvm[nth];
-    if (p.stream) {
-        p.off_pair = off; off = align_up(off + sizeof(int) * (size_t)std::max(ntiles, 1) * ts::TILE_M * T, 16);
-        p.off_vptr = off; off = align_up(off + sizeof(int) * (size_t)(nv + 1), 16);
-        p.off_vsrc = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(nvm, 1), 16);
-        p.off_tvp = off;  off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
-        p.off_vinfo = off; off = align_up(off + sizeof(int) * 8 * (size_t)std::max(nv, 1), 16);
-    }
-    if (p.weighted) {   // per-slot adjacency weights
-        p.off_slotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16);
-        if (p.has_transpose) { p.off_tslotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16); }
-    }
-    p.ts_nv = nv;
+    const size_t off = layout_image(shape, p, g->save, M, (int)part_nv[nth], part_nvm[nth]);
     CU_TRY(g, g->image.begin(off));
     g->bytes = off;
     char* base = g->image.ptr;
@@ -1667,6 +1677,13 @@ int ggnn_prepared_graph_arrays(const ggnn_prepared_graph* g, int32_t* row_ptr, i
     return GGNN_OK;
 }
 
+int ggnn_prepared_graph_tile_stats(const ggnn_prepared_graph* g, int32_t* max_tile_msgs, int32_t* max_tile_types) {
+    if (!g || !g->valid) return GGNN_ESTATE;
+    if (max_tile_msgs) *max_tile_msgs = g->plan.max_tile_msgs;
+    if (max_tile_types) *max_tile_types = g->plan.max_tile_types;
+    return GGNN_OK;
+}
+
 int ggnn_prepared_graph_image(const ggnn_prepared_graph* g, void* dst, int64_t capacity) {
     if (!g || !g->valid || !dst) return GGNN_ESTATE;
     if (capacity < (int64_t)g->bytes) return GGNN_EINVAL;
@@ -1680,22 +1697,23 @@ int ggnn_prepare_graph_sparse(const ggnn_engine* e, int32_t save_for_backward, i
     return build_sparse_image(*inout, V, adj, num_edges, indeg, false, nullptr);
 }
 
-int ggnn_set_graph_prepared(ggnn_engine* e, ggnn_prepared_graph* g, ggnn_stream_t stream) {
-    if (!e) return GGNN_EINVAL;
-    forget_batch(e);
-    if (!g || !g->valid) return e->fail(GGNN_ESTATE, "the prepared graph is empty (its build failed or never ran)");
-    const ModelShape& q = g->shape;
+}  // extern "C"
+
+// Whether a batch planned for model shape `q` (`what` names it) may be adopted by engine `e`; with save_for_backward on, the plan must carry
+// the source-keyed CSR.
+static int check_batch_shape(ggnn_engine* e, const ModelShape& q, const BatchPlan& p, const char* what) {
     if (q.model != e->model)
-        return e->fail(GGNN_ESTATE, "the prepared graph was built for a %s engine, this is a %s engine", q.model == MODEL_GCN ? "GCN" : "GGNN",
+        return e->fail(GGNN_ESTATE, "the %s was built for a %s engine, this is a %s engine", what, q.model == MODEL_GCN ? "GCN" : "GGNN",
                        e->model == MODEL_GCN ? "GCN" : "GGNN");
     if (q.D != e->D || q.T != e->T || q.precision != e->precision || q.DP != e->DP || q.num_sms != e->num_sms || q.cell != e->cell || q.use_att != e->use_att)
-        return e->fail(GGNN_EINVAL, "the prepared graph was built for a different engine configuration");
-    if (e->save && !g->plan.has_transpose)
-        return e->fail(GGNN_ESTATE, "save_for_backward is on but the graph was prepared without it (the source-keyed CSR is built at prepare time)");
-    CU_TRY(e, cudaSetDevice(e->device));
-    static_cast<BatchPlan&>(*e) = g->plan;
-    CU_TRY(e, e->graph_buf.reserve(g->bytes));
-    CU_TRY(e, g->image.upload(e->graph_buf.ptr, g->bytes, (cudaStream_t)stream));
+        return e->fail(GGNN_EINVAL, "the %s was built for a different engine configuration", what);
+    if (e->save && !p.has_transpose)
+        return e->fail(GGNN_ESTATE, "save_for_backward is on but the %s was prepared without it (the source-keyed CSR is built at prepare time)", what);
+    return GGNN_OK;
+}
+
+// The typed view of the graph image in graph_buf (laid out by e's plan), then room for the states of the batch: the end of every graph upload.
+static int bind_graph(ggnn_engine* e) {
     const char* b = (const char*)e->graph_buf.ptr;
     GraphDev& d = e->gd;
     d.row_ptr = (const int*)(b + e->off_row_ptr); d.csr_src = (const int*)(b + e->off_src); d.csr_msg = (const int*)(b + e->off_msg);
@@ -1709,6 +1727,21 @@ int ggnn_set_graph_prepared(ggnn_engine* e, ggnn_prepared_graph* g, ggnn_stream_
     if (rc) return rc;
     e->graph_set = true;
     return GGNN_OK;
+}
+
+extern "C" {
+
+int ggnn_set_graph_prepared(ggnn_engine* e, ggnn_prepared_graph* g, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    forget_batch(e);
+    if (!g || !g->valid) return e->fail(GGNN_ESTATE, "the prepared graph is empty (its build failed or never ran)");
+    if (int rc = check_batch_shape(e, g->shape, g->plan, "prepared graph")) return rc;
+    CU_TRY(e, cudaSetDevice(e->device));
+    static_cast<BatchPlan&>(*e) = g->plan;
+    CU_TRY(e, e->graph_buf.reserve(g->bytes));
+    e->graph_bytes = g->bytes;
+    CU_TRY(e, g->image.upload(e->graph_buf.ptr, g->bytes, (cudaStream_t)stream));
+    return bind_graph(e);
 }
 
 int ggnn_set_graph_sparse(ggnn_engine* e, int32_t V, const int32_t* const* adj, const int32_t* num_edges,
@@ -2501,6 +2534,22 @@ int ggnn_run_dense_host(ggnn_engine* e, int32_t b, int32_t v, const float* adjac
 }
 
 // ------------------------------------------------------------------------------------------ readout (SURVEY 8f-1)
+}  // extern "C"
+
+// The layout of the readout map in ro_buf for V nodes in G graphs: graph_of [V] | start [G+1] | mask [V] | perm [V] | the device-only
+// per-node gated values.  Returns the offset of the values (the bytes an upload may fill).
+static size_t readout_layout(ggnn_engine* e, int V, int G) {
+    size_t off = 0;
+    e->ro_off_graph_of = off; off = align_up(off + sizeof(int) * (size_t)std::max(V, 1), 16);
+    e->ro_off_start = off;    off = align_up(off + sizeof(int) * (size_t)(G + 1), 16);
+    e->ro_off_mask = off;     off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
+    e->ro_off_perm = off;     off = align_up(off + sizeof(int) * (size_t)std::max(V, 1), 16);   // uploaded for ungrouped lists only
+    e->ro_off_val = off;      // device-only scratch: per-node gated value
+    return off;
+}
+
+extern "C" {
+
 int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* graph_nodes_list, int32_t num_graphs,
                             int32_t nodes_per_graph, const float* node_mask, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
@@ -2510,12 +2559,7 @@ int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* gr
         return e->fail(GGNN_EINVAL, "without a graph_nodes_list the batch must be num_graphs x nodes_per_graph (%d x %d != %d)", num_graphs, nodes_per_graph, num_nodes);
     CU_TRY(e, cudaSetDevice(e->device));
     const int V = num_nodes, G = num_graphs;
-    size_t off = 0;
-    e->ro_off_graph_of = off; off = align_up(off + sizeof(int) * (size_t)std::max(V, 1), 16);
-    e->ro_off_start = off;    off = align_up(off + sizeof(int) * (size_t)(G + 1), 16);
-    e->ro_off_mask = off;     off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
-    e->ro_off_perm = off;     off = align_up(off + sizeof(int) * (size_t)std::max(V, 1), 16);   // uploaded for ungrouped lists only
-    e->ro_off_val = off;      // device-only scratch: per-node gated value
+    const size_t off = readout_layout(e, V, G);
     const size_t dev_bytes = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
     CU_TRY(e, e->ro_stage.begin(off));
     CU_TRY(e, e->ro_buf.reserve(dev_bytes));
@@ -2763,5 +2807,477 @@ int ggnn_copy_layer_state(ggnn_engine* e, int32_t layer, float* dst, ggnn_stream
 
 int ggnn_last_launch_count(const ggnn_engine* e) { return e ? e->last_launches : 0; }
 const char* ggnn_plan_description(const ggnn_engine* e) { return e ? e->plan_text.c_str() : ""; }
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------ device-resident datasets (ggnn_dataset.cuh)
+// A dataset holds every graph's pieces of a batch image in graph-local numbering, uploaded once: its target-CSR rows and slots, in-degrees
+// and denominators, the source-keyed CSR (training datasets), the streaming tables (GGNN on tensor cores), the slot weights (GCN), and its
+// annotations and labels.  The host keeps what a batch plan needs and no edge: per graph its sizes and the dataset offsets of its pieces,
+// per edge type its message count, and per cut segment (node range between two cut points) its message count and edge-type mask.
+struct DsGraph {
+    int V = 0, M = 0, nv = 0, nvm = 0;
+    int seg0 = 0, nseg = 0;   // its segments in ggnn_dataset::seg_*
+};
+
+struct ggnn_dataset : ErrorText {
+    ModelShape shape;
+    bool train = false, stream_tables = false, weighted = false, on_device = false;
+    int N = 0, ann = 0, tasks = 0;
+    std::vector<DsGraph> graphs;
+    std::vector<int> type_msgs;   // [N][T]
+    std::vector<int> seg_end, seg_msgs;   // graph-local end node and messages (by target) of every cut segment
+    std::vector<unsigned> seg_mask;
+    DevBuf buf;
+    ds::DsArrays dev{};
+};
+
+struct ggnn_dataset_batch : ErrorText {
+    const ggnn_dataset* ds = nullptr;
+    ModelShape shape;
+    BatchPlan plan;
+    size_t bytes = 0;
+    int G = 0;
+    StagedImage table;       // tile starts [ntiles + 1] | the per-graph records [G][R_MBASE + T] (16-byte aligned)
+    size_t table_bytes = 0, off_records = 0;
+    bool valid = false;
+};
+
+// The host arrays of a dataset before its upload, section by section (each 16-byte aligned in the one image).
+struct DsHost {
+    std::vector<int> base, row_end, src, pos, trow_end, ttgt, tslot, pair, vend, vsrc, vpre;
+    std::vector<float> indeg, denom, slotw, tslotw;
+};
+
+// Adds one graph of V nodes: per edge type t its graph-local (source, target) list adj[t] of ne[t] messages in the reference's order, its
+// [V][T] in-degrees, and (weighted datasets) its per-message weights w in type-major order.  Builds its pieces with the batch builder's
+// own passes (fill_target_csr, number_virtual_rows, find_cuts) and appends them.
+static int ds_add_graph(ggnn_dataset* d, DsHost& h, int gi, int V, const int32_t* const* adj, const int32_t* ne, const float* indeg, const float* w) {
+    const int T = d->shape.T;
+    DsGraph g;
+    g.V = V;
+    std::vector<int> counts((size_t)V * T + 1, 0), reach((size_t)V + 1, 0);
+    std::vector<int> ltb(T + 1, 0);
+    for (int t = 0; t < T; ++t) {
+        ltb[t + 1] = ltb[t] + ne[t];
+        for (int i = 0; i < ne[t]; ++i) {
+            const int s = adj[t][2 * i], dd = adj[t][2 * i + 1];
+            if ((unsigned)s >= (unsigned)V || (unsigned)dd >= (unsigned)V)
+                return d->fail(GGNN_ERANGE, "graph %d: edge %d of type %d = (%d,%d) is out of range for its %d nodes", gi, i, t, s, dd, V);
+            ++counts[(size_t)dd * T + t + 1];
+            reach[std::min(s, dd)] = std::max(reach[std::min(s, dd)], std::max(s, dd));
+        }
+        d->type_msgs.push_back(ne[t]);
+    }
+    const int M = ltb[T];
+    g.M = M;
+    std::vector<int> row_ptr((size_t)V * T + 1), src((size_t)std::max(M, 1)), msg((size_t)std::max(M, 1));
+    fill_target_csr(V, T, adj, ne, counts, row_ptr.data(), src.data(), msg.data());
+    h.row_end.insert(h.row_end.end(), row_ptr.begin() + 1, row_ptr.end());
+    h.src.insert(h.src.end(), src.begin(), src.begin() + M);
+    for (size_t k = 0; k < (size_t)V * T; ++k)
+        for (int m = row_ptr[k]; m < row_ptr[k + 1]; ++m) h.pos.push_back(msg[m] - ltb[k % T]);
+    h.indeg.insert(h.indeg.end(), indeg, indeg + (size_t)V * T);
+    for (int v = 0; v < V; ++v) {   // as the builder: tf.reduce_sum over the type axis in fp32 (sparse:207), then + SMALL_NUMBER (:209)
+        float s = 0.0f;
+        for (int t = 0; t < T; ++t) s += indeg[(size_t)v * T + t];
+        h.denom.push_back(s + 1e-7f);
+    }
+    if (d->weighted)
+        for (int m = 0; m < M; ++m) h.slotw.push_back(w[msg[m]]);
+    if (d->train) {   // source-keyed CSR, filled in message order like the builder's
+        std::vector<int> trow((size_t)V * T + 1, 0), slot_of_msg((size_t)std::max(M, 1));
+        for (int t = 0; t < T; ++t)
+            for (int i = 0; i < ne[t]; ++i) ++trow[(size_t)adj[t][2 * i] * T + t + 1];
+        for (size_t k = 1; k <= (size_t)V * T; ++k) trow[k] += trow[k - 1];
+        h.trow_end.insert(h.trow_end.end(), trow.begin() + 1, trow.end());
+        for (int m = 0; m < M; ++m) slot_of_msg[msg[m]] = m;
+        const size_t t0 = h.ttgt.size();
+        h.ttgt.resize(t0 + M);
+        if (d->shape.use_att) h.tslot.resize(t0 + M);
+        if (d->weighted) h.tslotw.resize(t0 + M);
+        int m = 0;
+        for (int t = 0; t < T; ++t)
+            for (int i = 0; i < ne[t]; ++i, ++m) {
+                const int j = trow[(size_t)adj[t][2 * i] * T + t]++;
+                h.ttgt[t0 + j] = adj[t][2 * i + 1];
+                if (d->shape.use_att) h.tslot[t0 + j] = slot_of_msg[m];
+                if (d->weighted) h.tslotw[t0 + j] = w[m];
+            }
+    }
+    if (d->stream_tables) {   // the streaming plan's tables of the graph on its own, virtual rows numbered in row order
+        std::vector<int> pair((size_t)V * T), vptr(1, 0), vsrc, tvp(2);
+        int nv = 0;
+        for (size_t k = 0; k < (size_t)V * T; ++k) {
+            const int cnt = row_ptr[k + 1] - row_ptr[k];
+            pair[k] = cnt == 0 ? -1 : (cnt == 1 ? src[row_ptr[k]] : -2);
+            if (cnt >= 2) { ++nv; g.nvm += cnt; }
+        }
+        vptr.resize(nv + 1); vsrc.resize((size_t)std::max(g.nvm, 1));
+        const int tile[2] = {0, V};
+        if (V > 0) number_virtual_rows(1, T, tile, row_ptr.data(), src.data(), pair.data(), vptr.data(), vsrc.data(), tvp.data(), nullptr);
+        g.nv = nv;
+        int before = 0;
+        for (int v = 0; v < V; ++v) {
+            h.vpre.push_back(before);
+            for (int t = 0; t < T; ++t) before += pair[(size_t)v * T + t] <= -2;
+        }
+        h.pair.insert(h.pair.end(), pair.begin(), pair.end());
+        h.vend.insert(h.vend.end(), vptr.begin() + 1, vptr.end());
+        h.vsrc.insert(h.vsrc.end(), vsrc.begin(), vsrc.begin() + g.nvm);
+    }
+    std::vector<int> cuts;
+    find_cuts(reach.data(), V, cuts);
+    g.seg0 = (int)d->seg_end.size();
+    g.nseg = (int)cuts.size() - 1;
+    for (int k = 0; k < g.nseg; ++k) {
+        unsigned mask = 0;
+        for (size_t r = (size_t)cuts[k] * T; r < (size_t)cuts[k + 1] * T; ++r) mask |= (unsigned)(row_ptr[r + 1] > row_ptr[r]) << (r % T);
+        d->seg_end.push_back(cuts[k + 1]);
+        d->seg_msgs.push_back(row_ptr[(size_t)cuts[k + 1] * T] - row_ptr[(size_t)cuts[k] * T]);
+        d->seg_mask.push_back(mask);
+    }
+    d->graphs.push_back(g);
+    return GGNN_OK;
+}
+
+// After the graphs: the per-graph base table, the annotations and labels, and (with a device) the one upload of every section.
+static int ds_finish(ggnn_dataset* d, DsHost& h, const float* ann, const float* labels, const float* lmask, cudaStream_t stream) {
+    int64_t node = 0, slot = 0, vrow = 0, vs = 0;
+    for (const DsGraph& g : d->graphs) {
+        h.base.insert(h.base.end(), {(int)node, (int)slot, (int)vrow, (int)vs});
+        node += g.V; slot += g.M; vrow += g.nv; vs += g.nvm;
+        if (node * d->shape.T > 0x7fffffff || slot > 0x7fffffff || vs > 0x7fffffff)
+            return d->fail(GGNN_EUNSUPPORTED, "dataset too large for int32 indexing");
+    }
+    h.base.insert(h.base.end(), {(int)node, (int)slot, (int)vrow, (int)vs});
+    if (!d->on_device) return GGNN_OK;
+    const size_t nann = (size_t)node * d->ann, nlab = (size_t)d->N * d->tasks;
+    struct Section { const void* src; size_t bytes; const void** dst; };
+    ds::DsArrays& a = d->dev;
+    a = ds::DsArrays{};
+    a.ann_size = d->ann; a.tasks = d->tasks;
+    auto I = [](const std::vector<int>& v, const int** dst) { return Section{v.data(), v.size() * sizeof(int), (const void**)dst}; };
+    auto F = [](const std::vector<float>& v, const float** dst) { return Section{v.data(), v.size() * sizeof(float), (const void**)dst}; };
+    const Section secs[] = {I(h.base, &a.base), I(h.row_end, &a.row_end), I(h.src, &a.src), I(h.pos, &a.pos), F(h.indeg, &a.indeg),
+                            F(h.denom, &a.denom), I(h.trow_end, &a.trow_end), I(h.ttgt, &a.ttgt), I(h.tslot, &a.tslot), I(h.pair, &a.pair),
+                            I(h.vend, &a.vend), I(h.vsrc, &a.vsrc), I(h.vpre, &a.vpre), F(h.slotw, &a.slotw), F(h.tslotw, &a.tslotw),
+                            {ann, nann * sizeof(float), (const void**)&a.ann}, {labels, nlab * sizeof(float), (const void**)&a.labels},
+                            {lmask, nlab * sizeof(float), (const void**)&a.lmask}};
+    const bool present[] = {true, true, true, true, true, true, d->train, d->train, d->train && d->shape.use_att, d->stream_tables,
+                            d->stream_tables, d->stream_tables, d->stream_tables, d->weighted, d->weighted && d->train, true, true, true};
+    size_t total = 0;
+    for (const Section& s : secs) total = align_up(total + s.bytes, 16);
+    std::vector<char> image(total);
+    size_t off = 0;
+    std::vector<size_t> offs;
+    for (const Section& s : secs) {
+        if (s.bytes) memcpy(image.data() + off, s.src, s.bytes);
+        offs.push_back(off);
+        off = align_up(off + s.bytes, 16);
+    }
+    if (d->buf.reserve(std::max<size_t>(total, 16)) != cudaSuccess) {
+        cudaGetLastError();
+        return d->fail(GGNN_ECUDA, "cudaMalloc of the dataset's %zu bytes failed", total);
+    }
+    CU_TRY(d, cudaMemcpyAsync(d->buf.ptr, image.data(), total, cudaMemcpyHostToDevice, stream));
+    CU_TRY(d, cudaStreamSynchronize(stream));   // the staging image is pageable and freed on return
+    for (size_t i = 0; i < sizeof secs / sizeof secs[0]; ++i) *secs[i].dst = present[i] ? (const char*)d->buf.ptr + offs[i] : nullptr;
+    return GGNN_OK;
+}
+
+// The prologue of the four create calls: the model shape from the engine (`e`, whose model must be `model`) or from a config for a host of
+// `num_sms` SMs; the handle is allocated here and returned even on failure, with the text in ggnn_dataset_error.
+template <class Config>
+static int begin_dataset(ggnn_dataset** out, const ggnn_engine* e, const Config* cfg, int32_t num_sms, int32_t for_training, int32_t N,
+                         const int64_t* node_counts, int32_t ann, const float* annotations, int32_t tasks, const float* labels,
+                         const float* lmask, const char* fn) {
+    constexpr int model = std::is_same<Config, ggnn_gcn_config>::value ? MODEL_GCN : MODEL_GGNN;
+    if (!out || (!e && (!cfg || num_sms <= 0))) return GGNN_EINVAL;
+    ggnn_dataset* d = new ggnn_dataset();
+    *out = d;
+    if (e) {
+        if (e->model != model) return wrong_model(d, fn, e->model, model);
+        d->shape = *e;
+        if (cudaSetDevice(e->device) != cudaSuccess) return d->fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);
+    } else {
+        int rc;
+        if constexpr (model == MODEL_GCN) rc = init_gcn_shape(d->shape, cfg, d->err);
+        else rc = init_model_shape(d->shape, cfg, d->err);
+        if (rc) return rc;
+        d->shape.num_sms = num_sms; d->shape.max_smem = 227 * 1024;
+    }
+    d->on_device = e != nullptr;
+    d->train = for_training != 0;
+    d->weighted = model == MODEL_GCN;
+    d->stream_tables = model == MODEL_GGNN && d->shape.precision != GGNN_PREC_FP32;
+    d->N = N; d->ann = ann; d->tasks = tasks;
+    if (N < 0 || ann < 0 || tasks < 0 || (N > 0 && !node_counts) || (ann > 0 && N > 0 && !annotations) || (tasks > 0 && N > 0 && (!labels || !lmask)))
+        return d->fail(GGNN_EINVAL, "null/negative argument");
+    if (ann > d->shape.D) return d->fail(GGNN_EINVAL, "annotation_size %d exceeds hidden_size %d", ann, d->shape.D);
+    for (int i = 0; i < N; ++i)
+        if (node_counts[i] < 0 || node_counts[i] > 0x7fffffff) return d->fail(GGNN_EINVAL, "graph %d: node count %lld", i, (long long)node_counts[i]);
+    return GGNN_OK;
+}
+
+template <class Config>
+static int create_dataset_sparse(ggnn_dataset** out, const ggnn_engine* e, const Config* cfg, int32_t num_sms, int32_t for_training, int32_t N,
+                                 const int64_t* node_counts, const int32_t* const* edge_lists, const int64_t* edge_offsets, const float* indeg,
+                                 int32_t ann, const float* annotations, int32_t tasks, const float* labels, const float* lmask,
+                                 cudaStream_t stream, const char* fn) {
+    if (int rc = begin_dataset(out, e, cfg, num_sms, for_training, N, node_counts, ann, annotations, tasks, labels, lmask, fn)) return rc;
+    ggnn_dataset* d = *out;
+    const int T = d->shape.T;
+    if (N > 0 && (!edge_lists || !edge_offsets || !indeg)) return d->fail(GGNN_EINVAL, "null edge lists / offsets / in-degrees");
+    DsHost h;
+    std::vector<const int32_t*> adj(T);
+    std::vector<int32_t> ne(T);
+    int64_t node = 0;
+    for (int i = 0; i < N; ++i) {
+        for (int t = 0; t < T; ++t) {
+            const int64_t* eo = edge_offsets + (size_t)t * (N + 1);
+            if (eo[i] < 0 || eo[i + 1] < eo[i] || eo[i + 1] - eo[i] > 0x7fffffff || (eo[i + 1] > eo[i] && !edge_lists[t]))
+                return d->fail(GGNN_EINVAL, "graph %d: bad edge offsets of type %d", i, t);
+            adj[t] = eo[i + 1] > eo[i] ? edge_lists[t] + 2 * eo[i] : nullptr;
+            ne[t] = (int32_t)(eo[i + 1] - eo[i]);
+        }
+        if (int rc = ds_add_graph(d, h, i, (int)node_counts[i], adj.data(), ne.data(), indeg + (size_t)node * T, nullptr)) return rc;
+        node += node_counts[i];
+    }
+    return ds_finish(d, h, annotations, labels, lmask, stream);
+}
+
+// GCN entries (row i = output, column j = input, int64, graph-local) become one edge type j -> i with fp32 weights, as in build_gcn_image.
+template <class Config>
+static int create_dataset_gcn(ggnn_dataset** out, const ggnn_engine* e, const Config* cfg, int32_t num_sms, int32_t for_training, int32_t N,
+                              const int64_t* node_counts, const int64_t* lists, const int64_t* entry_offsets, const float* weights, int32_t ann,
+                              const float* annotations, int32_t tasks, const float* labels, const float* lmask, cudaStream_t stream,
+                              const char* fn) {
+    if (int rc = begin_dataset(out, e, cfg, num_sms, for_training, N, node_counts, ann, annotations, tasks, labels, lmask, fn)) return rc;
+    ggnn_dataset* d = *out;
+    if (N > 0 && !entry_offsets) return d->fail(GGNN_EINVAL, "null entry offsets");
+    DsHost h;
+    std::vector<int32_t> pairs;
+    for (int i = 0; i < N; ++i) {
+        const int64_t e0 = entry_offsets[i], e1 = entry_offsets[i + 1], V = node_counts[i];
+        if (e0 < 0 || e1 < e0 || e1 - e0 > 0x7fffffff || (e1 > e0 && (!lists || !weights))) return d->fail(GGNN_EINVAL, "graph %d: bad entry offsets", i);
+        pairs.resize((size_t)(e1 - e0) * 2);
+        for (int64_t k = e0; k < e1; ++k) {
+            const int64_t r = lists[2 * k], c = lists[2 * k + 1];
+            if (r < 0 || r >= V || c < 0 || c >= V)
+                return d->fail(GGNN_ERANGE, "graph %d: entry %lld = (%lld, %lld) is out of range for its %lld nodes", i, (long long)(k - e0),
+                               (long long)r, (long long)c, (long long)V);
+            pairs[2 * (k - e0)] = (int32_t)c;
+            pairs[2 * (k - e0) + 1] = (int32_t)r;
+        }
+        const std::vector<float> indeg((size_t)V, 0.0f);
+        const int32_t* adj[1] = {pairs.data()};
+        const int32_t ne[1] = {(int32_t)(e1 - e0)};
+        if (int rc = ds_add_graph(d, h, i, (int)V, adj, ne, indeg.data(), weights + e0)) return rc;
+    }
+    return ds_finish(d, h, annotations, labels, lmask, stream);
+}
+
+extern "C" {
+
+int ggnn_dataset_create_sparse(const ggnn_engine* e, int32_t for_training, int32_t num_graphs, const int64_t* node_counts,
+                               const int32_t* const* edge_lists, const int64_t* edge_offsets, const float* num_incoming_edges_per_type,
+                               int32_t annotation_size, const float* annotations, int32_t num_tasks, const float* labels, const float* label_mask,
+                               ggnn_stream_t stream, ggnn_dataset** out) {
+    if (!e) return GGNN_EINVAL;
+    return create_dataset_sparse<ggnn_config>(out, e, nullptr, 0, for_training, num_graphs, node_counts, edge_lists, edge_offsets,
+                                              num_incoming_edges_per_type, annotation_size, annotations, num_tasks, labels, label_mask,
+                                              (cudaStream_t)stream, __func__);
+}
+
+int ggnn_host_dataset_create_sparse(const ggnn_config* cfg, int32_t num_sms, int32_t for_training, int32_t num_graphs, const int64_t* node_counts,
+                                    const int32_t* const* edge_lists, const int64_t* edge_offsets, const float* num_incoming_edges_per_type,
+                                    int32_t annotation_size, const float* annotations, int32_t num_tasks, const float* labels,
+                                    const float* label_mask, ggnn_dataset** out) {
+    return create_dataset_sparse(out, nullptr, cfg, num_sms, for_training, num_graphs, node_counts, edge_lists, edge_offsets,
+                                 num_incoming_edges_per_type, annotation_size, annotations, num_tasks, labels, label_mask, nullptr, __func__);
+}
+
+int ggnn_dataset_create_gcn(const ggnn_engine* e, int32_t for_training, int32_t num_graphs, const int64_t* node_counts, const int64_t* adjacency_lists,
+                            const int64_t* entry_offsets, const float* adjacency_weights, int32_t annotation_size, const float* annotations,
+                            int32_t num_tasks, const float* labels, const float* label_mask, ggnn_stream_t stream, ggnn_dataset** out) {
+    if (!e) return GGNN_EINVAL;
+    return create_dataset_gcn<ggnn_gcn_config>(out, e, nullptr, 0, for_training, num_graphs, node_counts, adjacency_lists, entry_offsets,
+                                               adjacency_weights, annotation_size, annotations, num_tasks, labels, label_mask,
+                                               (cudaStream_t)stream, __func__);
+}
+
+int ggnn_host_dataset_create_gcn(const ggnn_gcn_config* cfg, int32_t num_sms, int32_t for_training, int32_t num_graphs, const int64_t* node_counts,
+                                 const int64_t* adjacency_lists, const int64_t* entry_offsets, const float* adjacency_weights,
+                                 int32_t annotation_size, const float* annotations, int32_t num_tasks, const float* labels,
+                                 const float* label_mask, ggnn_dataset** out) {
+    return create_dataset_gcn(out, nullptr, cfg, num_sms, for_training, num_graphs, node_counts, adjacency_lists, entry_offsets, adjacency_weights,
+                              annotation_size, annotations, num_tasks, labels, label_mask, nullptr, __func__);
+}
+
+int ggnn_free_dataset(ggnn_dataset* d) {
+    if (!d) return GGNN_OK;
+    if (d->on_device) { cudaSetDevice(d->shape.device); d->buf.release(); }
+    delete d;
+    return GGNN_OK;
+}
+
+const char* ggnn_dataset_error(const ggnn_dataset* d) { return d ? d->err.c_str() : "null dataset"; }
+
+int ggnn_dataset_prepare_batch(const ggnn_dataset* d, int32_t save_for_backward, const int64_t* graph_ids, int32_t num_graphs,
+                               ggnn_dataset_batch** inout) {
+    if (!d || !inout || num_graphs < 0 || (num_graphs > 0 && !graph_ids)) return GGNN_EINVAL;
+    ggnn_dataset_batch* b = *inout;
+    if (!b) { b = new ggnn_dataset_batch(); *inout = b; }
+    b->valid = false;
+    b->ds = d;
+    b->shape = d->shape;
+    b->table.use_cuda = d->on_device;
+    const bool save = save_for_backward != 0;
+    if (save && !d->train) return b->fail(GGNN_ESTATE, "save_for_backward needs a dataset created for training (the source-keyed CSR is built there)");
+    const int T = d->shape.T, G = num_graphs;
+    for (int i = 0; i < G; ++i)
+        if (graph_ids[i] < 0 || graph_ids[i] >= d->N)
+            return b->fail(GGNN_ERANGE, "graph_ids[%d] = %lld is out of range for a dataset of %d graphs", i, (long long)graph_ids[i], d->N);
+    // offsets and the cut points: every graph's segments, shifted by its node offset
+    int64_t V = 0, M = 0, nv = 0, nvm = 0;
+    std::vector<int64_t> type_tot(T, 0);
+    std::vector<int> cuts(1, 0);
+    for (int i = 0; i < G; ++i) {
+        const DsGraph& g = d->graphs[graph_ids[i]];
+        for (int k = 0; k < g.nseg; ++k) cuts.push_back((int)(V + d->seg_end[g.seg0 + k]));
+        V += g.V; M += g.M; nv += g.nv; nvm += g.nvm;
+        for (int t = 0; t < T; ++t) type_tot[t] += d->type_msgs[(size_t)graph_ids[i] * T + t];
+        if (M > 0x7fffffff || V * T + 1 > 0x7fffffff) return b->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
+    }
+    BatchPlan& p = b->plan;
+    std::vector<int> tile_start;
+    if (int rc = build_plan(d->shape, (int)V, d->weighted, cuts, p, tile_start, b->err)) return rc;
+    b->bytes = layout_image(d->shape, p, save, M, (int)nv, nvm);
+    if (p.local) {   // tiles of whole segments: their message counts and edge types from the segment summaries (only LOCAL launches read them)
+        size_t tile = 1;
+        int msgs = 0; unsigned mask = 0;
+        int64_t node = 0;
+        for (int i = 0; i < G; ++i) {
+            const DsGraph& g = d->graphs[graph_ids[i]];
+            for (int k = 0; k < g.nseg; ++k) {
+                msgs += d->seg_msgs[g.seg0 + k]; mask |= d->seg_mask[g.seg0 + k];
+                if (node + d->seg_end[g.seg0 + k] == tile_start[tile]) {
+                    p.max_tile_msgs = std::max(p.max_tile_msgs, msgs);
+                    p.max_tile_types = std::max(p.max_tile_types, __builtin_popcount(mask));
+                    msgs = 0; mask = 0; ++tile;
+                }
+            }
+            node += g.V;
+        }
+    }
+    // the batch table: tile starts, then per graph its id, offsets and per-type message bases (type base of the batch + earlier graphs')
+    const int rec = ds::R_MBASE + T;
+    b->off_records = align_up(sizeof(int) * tile_start.size(), 16);
+    b->table_bytes = b->off_records + sizeof(int) * (size_t)rec * G;
+    CU_TRY(b, b->table.begin(std::max<size_t>(b->table_bytes, 16)));
+    memcpy(b->table.ptr, tile_start.data(), sizeof(int) * tile_start.size());
+    int* r = (int*)(b->table.ptr + b->off_records);
+    std::vector<int64_t> mbase(T, 0);
+    for (int t = 1; t < T; ++t) mbase[t] = mbase[t - 1] + type_tot[t - 1];
+    int64_t node = 0, slot = 0, vrow = 0, vs = 0;
+    for (int i = 0; i < G; ++i, r += rec) {
+        const DsGraph& g = d->graphs[graph_ids[i]];
+        r[ds::R_GID] = (int)graph_ids[i]; r[ds::R_NODE] = (int)node; r[ds::R_SLOT] = (int)slot; r[ds::R_VROW] = (int)vrow; r[ds::R_VSRC] = (int)vs;
+        for (int t = 0; t < T; ++t) {
+            r[ds::R_MBASE + t] = (int)mbase[t];
+            mbase[t] += d->type_msgs[(size_t)graph_ids[i] * T + t];
+        }
+        node += g.V; slot += g.M; vrow += g.nv; vs += g.nvm;
+    }
+    b->G = G;
+    b->valid = true;
+    return GGNN_OK;
+}
+
+int ggnn_dataset_batch_info(const ggnn_dataset_batch* b, int32_t* num_nodes, int64_t* num_messages, int32_t* num_tiles, int64_t* image_bytes,
+                            int32_t* is_streaming, char* plan_text, int32_t plan_text_capacity, int32_t* tile_start, int32_t* max_tile_msgs,
+                            int32_t* max_tile_types) {
+    if (!b || !b->valid) return GGNN_ESTATE;
+    const BatchPlan& q = b->plan;
+    if (num_nodes) *num_nodes = q.V;
+    if (num_messages) *num_messages = q.M;
+    if (num_tiles) *num_tiles = q.ntiles;
+    if (image_bytes) *image_bytes = (int64_t)b->bytes;
+    if (is_streaming) *is_streaming = q.stream ? 1 : 0;
+    if (plan_text && plan_text_capacity > 0) snprintf(plan_text, (size_t)plan_text_capacity, "%s", q.plan_text.c_str());
+    if (tile_start) memcpy(tile_start, b->table.ptr, sizeof(int) * (size_t)(q.ntiles + 1));
+    if (max_tile_msgs) *max_tile_msgs = q.max_tile_msgs;
+    if (max_tile_types) *max_tile_types = q.max_tile_types;
+    return GGNN_OK;
+}
+
+int ggnn_free_dataset_batch(ggnn_dataset_batch* b) {
+    if (!b) return GGNN_OK;
+    if (b->table.use_cuda) { cudaSetDevice(b->shape.device); b->table.release(); }
+    delete b;
+    return GGNN_OK;
+}
+
+const char* ggnn_dataset_batch_error(const ggnn_dataset_batch* b) { return b ? b->err.c_str() : "null dataset batch"; }
+
+int ggnn_set_graph_dataset(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, float* target_values, float* target_mask, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    forget_batch(e);
+    if (!b || !b->valid) return e->fail(GGNN_ESTATE, "the dataset batch is empty (its prepare failed or never ran)");
+    const ggnn_dataset* d = b->ds;
+    if (!d->on_device) return e->fail(GGNN_EINVAL, "a host-only dataset has no device copy");
+    if (int rc = check_batch_shape(e, b->shape, b->plan, "dataset")) return rc;
+    if (b->shape.device != e->device)   // its arrays live in another GPU's memory
+        return e->fail(GGNN_EINVAL, "the dataset was built for an engine on device %d, this engine is on device %d", b->shape.device, e->device);
+    const BatchPlan& q = b->plan;
+    if ((q.V > 0 && !h0) || (d->tasks > 0 && b->G > 0 && (!target_values || !target_mask))) return e->fail(GGNN_EINVAL, "null output buffer");
+    CU_TRY(e, cudaSetDevice(e->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    static_cast<BatchPlan&>(*e) = q;
+    CU_TRY(e, e->graph_buf.reserve(b->bytes));
+    e->graph_bytes = b->bytes;
+    CU_TRY(e, e->ds_table.reserve(std::max<size_t>(b->table_bytes, 16)));
+    const size_t ro_bytes = readout_layout(e, q.V, b->G);
+    CU_TRY(e, e->ro_buf.reserve(align_up(ro_bytes + sizeof(float) * (size_t)std::max(q.V, 1), 16)));
+    CU_TRY(e, b->table.upload(e->ds_table.ptr, b->table_bytes, st));
+    CU_TRY(e, cudaMemsetAsync(e->graph_buf.ptr, 0, b->bytes, st));   // the alignment gaps, as in a fresh host image
+    CU_TRY(e, cudaMemsetAsync(e->ro_buf.ptr, 0, e->ro_off_perm, st));
+    char* base = (char*)e->graph_buf.ptr;
+    auto sec = [&](size_t off, bool present) { return present ? (void*)(base + off) : nullptr; };
+    ds::DsOut o;
+    o.row_ptr = (int*)sec(q.off_row_ptr, true); o.src = (int*)sec(q.off_src, true); o.msg = (int*)sec(q.off_msg, true);
+    o.indeg = (float*)sec(q.off_indeg, true); o.denom = (float*)sec(q.off_denom, true);
+    o.tile_start = (int*)sec(q.off_tiles, true); o.tile_mask = (unsigned*)sec(q.off_mask, true);
+    o.trow = (int*)sec(q.off_trow, q.has_transpose); o.ttgt = (int*)sec(q.off_ttgt, q.has_transpose);
+    o.tslot = (int*)sec(q.off_tslot, q.has_transpose && e->use_att);
+    o.pair = (int*)sec(q.off_pair, q.stream); o.vptr = (int*)sec(q.off_vptr, q.stream); o.vsrc = (int*)sec(q.off_vsrc, q.stream);
+    o.tvp = (int*)sec(q.off_tvp, q.stream); o.vinfo = (int*)sec(q.off_vinfo, q.stream);
+    o.slotw = (float*)sec(q.off_slotw, q.weighted); o.tslotw = (float*)sec(q.off_tslotw, q.weighted && q.has_transpose);
+    o.h0 = h0; o.tv = target_values; o.tm = target_mask;
+    o.ro_graph_of = (int*)((char*)e->ro_buf.ptr + e->ro_off_graph_of); o.ro_start = (int*)((char*)e->ro_buf.ptr + e->ro_off_start);
+    o.V = q.V; o.D = e->D; o.T = e->T; o.G = b->G; o.ntiles = q.ntiles; o.nv = q.ts_nv; o.rec = ds::R_MBASE + e->T;
+    const int* table = (const int*)((const char*)e->ds_table.ptr + b->off_records);
+    if (b->G > 0) ds::ds_graph_kernel<<<b->G, 256, 0, st>>>(d->dev, o, table);
+    const int tile_work = std::max(q.ntiles + 1, q.stream ? ts::TILE_M * e->T : 0);
+    ds::ds_tile_kernel<<<std::min(e->num_sms * 4, (tile_work + 255) / 256), 256, 0, st>>>(
+        d->dev, o, table, (const int*)e->ds_table.ptr);
+    CU_TRY(e, cudaGetLastError());
+    if (int rc = bind_graph(e)) return rc;
+    e->ro_V = q.V; e->ro_G = b->G; e->ro_grouped = true; e->ro_has_mask = false;
+    return GGNN_OK;
+}
+
+int ggnn_graph_image(ggnn_engine* e, void* dst, int64_t capacity, int64_t* image_bytes, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    if (!e->graph_set) return no_graph(e);
+    if (image_bytes) *image_bytes = (int64_t)e->graph_bytes;
+    if (!dst) return GGNN_OK;
+    if (capacity < (int64_t)e->graph_bytes) return e->fail(GGNN_EINVAL, "the image has %zu bytes, the buffer %lld", e->graph_bytes, (long long)capacity);
+    CU_TRY(e, cudaSetDevice(e->device));
+    CU_TRY(e, cudaMemcpyAsync(dst, e->graph_buf.ptr, e->graph_bytes, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+    CU_TRY(e, cudaStreamSynchronize((cudaStream_t)stream));
+    return GGNN_OK;
+}
 
 }  // extern "C"

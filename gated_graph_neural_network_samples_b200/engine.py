@@ -179,6 +179,13 @@ class PreparedGraph:
             out["pair_src"] = pair
         return out
 
+    def tile_stats(self) -> tuple:
+        """(largest message count, largest number of edge types) of one tile: what the tile-local wgmma kernel sizes its shared memory by."""
+        mm, mt = C.c_int32(), C.c_int32()
+        if self.lib.ggnn_prepared_graph_tile_stats(self._h, C.byref(mm), C.byref(mt)) != 0:
+            raise GgnnError("the prepared graph is empty")
+        return mm.value, mt.value
+
     def image(self) -> np.ndarray:
         """The packed image, byte for byte what ``set_graph_prepared`` uploads."""
         out = np.empty(self.info()["image_bytes"], np.uint8)
@@ -189,6 +196,151 @@ class PreparedGraph:
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
             self.lib.ggnn_free_prepared_graph(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class DeviceDataset:
+    """Handle of a ``ggnn_dataset`` (include/ggnn_b200.h): a whole graph set on the GPU, from which every batch of whole graphs is assembled on
+    the device.  Built from a ``packing.FlatSparseGraphs`` (GGNN engines) or ``packing.FlatGCNGraphs`` (GCN engines), whose arrays it reads
+    as they are.  ``for_engine`` uploads it for an engine; ``host_only`` / ``host_only_gcn`` build the same host summaries without a GPU, so
+    that batch plans can be checked anywhere."""
+
+    def __init__(self, lib=None):
+        self.lib = lib or _lib.load()
+        self._h = C.c_void_p()
+        self.num_tasks = 0
+
+    @staticmethod
+    def _common(flat):
+        labels = np.ascontiguousarray(flat.labels, np.float32)
+        mask = np.ascontiguousarray(flat.mask, np.float32)
+        ann = np.ascontiguousarray(flat.feat, np.float32)
+        return [np.ascontiguousarray(flat.n_nodes, np.int64), ann, labels, mask]
+
+    @staticmethod
+    def _sparse_arrays(flat, T: int):
+        if flat.num_edge_types != T:
+            raise GgnnError("the graph set has %d edge types, the engine %d" % (flat.num_edge_types, T))
+        edges = [np.ascontiguousarray(e, np.int32).reshape(-1, 2) for e in flat.edges]
+        offsets = np.ascontiguousarray(np.stack(flat.edge_off), np.int64) if T else np.zeros((0, 1), np.int64)
+        indeg = np.ascontiguousarray(flat.indeg, np.float32)
+        return edges, offsets, indeg
+
+    def _create(self, fn, flat, head, tail, keep):
+        """``fn(*head, N, node_counts, *tail, ann_size, ann, tasks, labels, mask, *stream, &handle)``; raises with the dataset's text."""
+        counts, ann, labels, mask = self._common(flat)
+        keep += [counts, ann, labels, mask]
+        h = C.c_void_p()
+        rc = fn(*head[0], int(flat.num_graphs), counts.ctypes.data, *tail, ann.shape[1] if ann.ndim == 2 else 0, ann.ctypes.data,
+                labels.shape[1], labels.ctypes.data, mask.ctypes.data, *head[1], C.byref(h))
+        self._h = h
+        if rc != 0:
+            err = GgnnError(self.lib.ggnn_dataset_error(h).decode() if h.value else "invalid argument")
+            err.code = rc
+            self.close()
+            raise err
+        self.num_tasks = labels.shape[1]
+        self.num_graphs = int(flat.num_graphs)
+        return self
+
+    @classmethod
+    def for_engine(cls, engine: "PropagationEngine", flat, for_training: bool = True, stream: Optional[int] = None) -> "DeviceDataset":
+        """Validates, builds and uploads ``flat`` for ``engine`` on ``stream`` (default: torch's current stream) and returns once the upload
+        completed.  ``for_training``: also build the source-keyed CSR that batches trained on need."""
+        d = cls(engine.lib)
+        d.engine_T, d.D = engine.T, engine.D
+        keep = []
+        head = ((engine._h, int(bool(for_training))), (engine._stream() if stream is None else int(stream),))
+        if isinstance(engine, GCNEngine):
+            lst, w = _gcn_arrays(flat.lists, flat.weights)
+            off = np.ascontiguousarray(flat.entry_off, np.int64)
+            keep += [lst, w, off]
+            return d._create(d.lib.ggnn_dataset_create_gcn, flat, head, (lst.ctypes.data, off.ctypes.data, w.ctypes.data), keep)
+        edges, offsets, indeg = cls._sparse_arrays(flat, engine.T)
+        keep += [edges, offsets, indeg]
+        ptrs = (C.c_void_p * max(engine.T, 1))(*[e.ctypes.data for e in edges])
+        return d._create(d.lib.ggnn_dataset_create_sparse, flat, head, (ptrs, offsets.ctypes.data, indeg.ctypes.data), keep)
+
+    @classmethod
+    def host_only(cls, params: dict, num_edge_types: int, flat, precision: str = "fp32", num_sms: int = 132,
+                  for_training: bool = True) -> "DeviceDataset":
+        """``ggnn_host_dataset_create_sparse``: the GGNN dataset's host summaries, no engine, no GPU."""
+        d = cls()
+        cfg, keep = make_config(params, num_edge_types, 0, precision)
+        edges, offsets, indeg = cls._sparse_arrays(flat, int(num_edge_types))
+        keep = [keep, edges, offsets, indeg]
+        ptrs = (C.c_void_p * max(int(num_edge_types), 1))(*[e.ctypes.data for e in edges])
+        head = ((C.byref(cfg), int(num_sms), int(bool(for_training))), ())
+        return d._create(d.lib.ggnn_host_dataset_create_sparse, flat, head, (ptrs, offsets.ctypes.data, indeg.ctypes.data), keep)
+
+    @classmethod
+    def host_only_gcn(cls, hidden_size: int, num_layers: int, flat, use_bias: bool = False, precision: str = "fp32", num_sms: int = 132,
+                      for_training: bool = True) -> "DeviceDataset":
+        """``ggnn_host_dataset_create_gcn``: the GCN dataset's host summaries, no engine, no GPU."""
+        d = cls()
+        cfg = _lib.GcnConfig(int(hidden_size), int(num_layers), int(bool(use_bias)), PRECISIONS[precision], 0)
+        lst, w = _gcn_arrays(flat.lists, flat.weights)
+        off = np.ascontiguousarray(flat.entry_off, np.int64)
+        head = ((C.byref(cfg), int(num_sms), int(bool(for_training))), ())
+        return d._create(d.lib.ggnn_host_dataset_create_gcn, flat, head, (lst.ctypes.data, off.ctypes.data, w.ctypes.data), [lst, w, off])
+
+    def prepare_batch(self, ids, save_for_backward: bool = True, reuse: Optional["DatasetBatch"] = None) -> "DatasetBatch":
+        """The HOST half of a batch of the graphs ``ids`` (dataset indices, in batch order): offsets, tile plan, image layout and a pinned
+        table of per-graph offsets, from the dataset's summaries alone -- may run in a producer thread.  ``reuse`` rebuilds a batch in place."""
+        ids = np.ascontiguousarray(np.asarray(ids, dtype=np.int64).reshape(-1))
+        b = reuse if reuse is not None else DatasetBatch(self)
+        h = C.c_void_p(b._h.value)
+        rc = self.lib.ggnn_dataset_prepare_batch(self._h, int(bool(save_for_backward)), ids.ctypes.data, ids.shape[0], C.byref(h))
+        b._h = h
+        if rc != 0:
+            err = GgnnError(self.lib.ggnn_dataset_batch_error(h).decode() if h.value else "invalid argument")
+            err.code = rc
+            raise err
+        b.dataset, b.G = self, ids.shape[0]
+        b.V = b.info()["num_nodes"]
+        return b
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h.value:
+            self.lib.ggnn_free_dataset(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class DatasetBatch:
+    """Handle of a ``ggnn_dataset_batch``: the host half of one dataset batch (adopt it with ``set_graph_from_dataset``)."""
+
+    def __init__(self, dataset: DeviceDataset):
+        self.lib = dataset.lib
+        self.dataset = dataset   # the dataset must outlive its batches
+        self._h = C.c_void_p()
+        self.V = self.G = 0
+
+    def info(self) -> dict:
+        V, M, nt, nb, st = C.c_int32(), C.c_int64(), C.c_int32(), C.c_int64(), C.c_int32()
+        buf = C.create_string_buffer(512)
+        if self.lib.ggnn_dataset_batch_info(self._h, C.byref(V), C.byref(M), C.byref(nt), C.byref(nb), C.byref(st), buf, 512, None, None, None) != 0:
+            raise GgnnError("the dataset batch is empty")
+        tiles = np.empty(nt.value + 1, np.int32)
+        mm, mt = C.c_int32(), C.c_int32()
+        self.lib.ggnn_dataset_batch_info(self._h, None, None, None, None, None, None, 0, tiles.ctypes.data, C.byref(mm), C.byref(mt))
+        return {"num_nodes": V.value, "num_messages": M.value, "num_tiles": nt.value, "image_bytes": nb.value, "streaming": bool(st.value),
+                "plan": buf.value.decode(), "tile_start": tiles, "max_tile_msgs": mm.value, "max_tile_types": mt.value}
+
+    def close(self):
+        if getattr(self, "_h", None) is not None and self._h.value:
+            self.lib.ggnn_free_dataset_batch(self._h)
             self._h = C.c_void_p()
 
     def __del__(self):
@@ -220,7 +372,9 @@ class PropagationEngine:
     # ------------------------------------------------------------------ plumbing
     def _check(self, rc: int):
         if rc != 0:
-            raise GgnnError(self.lib.ggnn_last_error(self._h).decode())
+            err = GgnnError(self.lib.ggnn_last_error(self._h).decode())
+            err.code = rc   # the GGNN_E* code of the call
+            raise err
 
     def close(self):
         if getattr(self, "_h", None) and self._h.value:
@@ -315,6 +469,32 @@ class PropagationEngine:
         self._check(self.lib.ggnn_set_graph_prepared(self._h, g._h, self._stream()))
         self.V = g.V
         self._graph_keepalive = (g,)
+
+    def set_graph_from_dataset(self, batch: "DatasetBatch"):
+        """The DEVICE half of a dataset batch: adopts its plan and assembles its graph image, h0, targets and readout map on the engine's
+        stream.  Returns ``(h0 [V, D], target_values [tasks, G], target_mask [tasks, G])`` as CUDA tensors; the readout map is set (no
+        ``readout_set_graphs`` needed).  Keep ``batch`` alive until the stream has passed it."""
+        import torch
+        dev = "cuda:%d" % self.device
+        h0 = torch.empty(batch.V, self.D, dtype=torch.float32, device=dev)
+        tv = torch.empty(batch.dataset.num_tasks, batch.G, dtype=torch.float32, device=dev)
+        tm = torch.empty_like(tv)
+        self.serial += 1
+        self._check(self.lib.ggnn_set_graph_dataset(self._h, batch._h, h0.data_ptr() if h0.numel() else None, tv.data_ptr() if tv.numel() else None,
+                                                    tm.data_ptr() if tm.numel() else None, self._stream()))
+        self.V = batch.V
+        self._graph_keepalive = (batch,)
+        self._readout_keepalive = None
+        self._readout_shape = (batch.V, batch.G)
+        return h0, tv, tm
+
+    def graph_image(self) -> np.ndarray:
+        """The engine's current graph image copied back (``ggnn_graph_image``): the bytes ``PreparedGraph.image`` holds for the same batch."""
+        n = C.c_int64()
+        self._check(self.lib.ggnn_graph_image(self._h, None, 0, C.byref(n), self._stream()))
+        out = np.empty(n.value, np.uint8)
+        self._check(self.lib.ggnn_graph_image(self._h, out.ctypes.data, out.nbytes, C.byref(n), self._stream()))
+        return out
 
     def run_sparse_host(self, adjacency_lists, num_incoming_edges_per_type, h0: np.ndarray, out: Optional[np.ndarray] = None) -> np.ndarray:
         """One call per batch (the shape of ``sess.run(fetch, feed_dict)``, chem_tensorflow.py:235): graph + initial

@@ -120,6 +120,11 @@ class _FlatGraphs:
 
     def iter_minibatches(self, order, batch_size_nodes: int, hidden_size: int):
         """The greedy node-budget batching of sparse:286-297 / gcn:150-162 over the graphs in ``order`` (flat ids)."""
+        for idx in self.iter_batch_ids(order, batch_size_nodes):
+            yield self.pack(idx, hidden_size)
+
+    def iter_batch_ids(self, order, batch_size_nodes: int):
+        """The flat ids of every batch ``iter_minibatches`` packs, in its order (what a device-resident dataset assembles batches from)."""
         order = np.asarray(order, dtype=np.int64)
         csum = np.cumsum(self.n_nodes[order])
         start, N = 0, order.shape[0]
@@ -129,7 +134,7 @@ class _FlatGraphs:
             if end == start:
                 raise Exception("graph %d has %d nodes and does not fit batch_size=%d"
                                 % (start, int(self.n_nodes[order[start]]), batch_size_nodes))
-            yield self.pack(order[start:end], hidden_size)
+            yield order[start:end]
             start = end
 
 

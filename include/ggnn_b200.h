@@ -161,6 +161,9 @@ int ggnn_prepared_graph_arrays(const ggnn_prepared_graph* g, int32_t* row_ptr, i
  * splits its passes over host threads by target ranges (GGNN_HOST_THREADS overrides the count); the tests require identical bytes for
  * every thread count. */
 int ggnn_prepared_graph_image(const ggnn_prepared_graph* g, void* dst, int64_t capacity);
+/* The plan's largest message count and largest number of edge types present in one tile: what the tile-local wgmma kernel sizes its shared
+ * memory by (its CSR cache and its gather tiles). */
+int ggnn_prepared_graph_tile_stats(const ggnn_prepared_graph* g, int32_t* max_tile_msgs, int32_t* max_tile_types);
 
 /* Dense wire format (dense:214-224): adjacency_matrix [b, T, v, v] float32 HOST pointer with
  * A[g, t, dest, src] (dense:30-36).  Rows are the b*v padded nodes. */
@@ -322,6 +325,75 @@ int ggnn_prepared_graph_slot_weights(const ggnn_prepared_graph* g, float* target
  * layer, accumulated into; d_h0 [V, D] DEVICE or NULL.  fp32 on CUDA cores whatever the forward precision. */
 int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0,
                       ggnn_stream_t stream);
+
+/* ---- Device-resident datasets: the training graphs uploaded once, every batch of whole graphs assembled on the device.
+ * Graphs never share edges, so a batch's graph image is its graphs' pieces (CSR slice, in-degrees, denominators, source-keyed CSR,
+ * attention slot map, streaming tables, slot weights) laid end to end with offsets.  A dataset holds those pieces, built once per graph at
+ * creation; a batch then costs O(number of graphs) on the host and a few kernels on the device, with no per-batch PCIe traffic but its
+ * table of per-graph offsets.  Batches are bit for bit the batches the packers build: the same image as ggnn_prepared_graph_image, the
+ * same h0, targets and readout map.
+ *
+ *   ggnn_dataset_create_sparse   GGNN engine.  num_graphs graphs; node_counts [N]; per edge type t, edge_lists[t] -> [E_t, 2] int32
+ *                                GRAPH-LOCAL (source, target) pairs of all graphs in graph order, each graph's in the reference's message
+ *                                order, with edge_offsets [T][N+1] int64 (graph i's type-t edges are rows edge_offsets[t][i] ..
+ *                                edge_offsets[t][i+1]); num_incoming_edges_per_type [sum V, T]; annotations [sum V, annotation_size] (the
+ *                                first columns of h0; annotation_size <= hidden_size); labels / label_mask [N, num_tasks].
+ *   ggnn_dataset_create_gcn      GCN engine.  adjacency_lists [sum nnz, 2] int64 graph-local (row i = output, column j = input) with
+ *                                entry_offsets [N+1], adjacency_weights [sum nnz] fp32 (as ggnn_prepare_graph_gcn takes them); the rest as above.
+ * Both validate every index (GGNN_ERANGE names the graph and the edge), record the engine's model shape (model, T, D, precision, SM count),
+ * build the pieces and upload them in one copy on `stream`, returning after it completed.  for_training = 1 also builds the source-keyed
+ * CSR that batches with save_for_backward need.  The source arrays stay the caller's; the dataset owns its device memory (an allocation
+ * failure returns GGNN_ECUDA naming the size).  *out is allocated even when the call fails: read ggnn_dataset_error, then free it.  The
+ * ggnn_host_* twins build the same host summaries without an engine or a GPU (for a host of num_sms SMs): their batches can be planned
+ * and inspected, not adopted. */
+typedef struct ggnn_dataset ggnn_dataset;
+int ggnn_dataset_create_sparse(const ggnn_engine* e, int32_t for_training, int32_t num_graphs, const int64_t* node_counts,
+                               const int32_t* const* edge_lists, const int64_t* edge_offsets, const float* num_incoming_edges_per_type,
+                               int32_t annotation_size, const float* annotations, int32_t num_tasks, const float* labels, const float* label_mask,
+                               ggnn_stream_t stream, ggnn_dataset** out);
+int ggnn_host_dataset_create_sparse(const ggnn_config* cfg, int32_t num_sms, int32_t for_training, int32_t num_graphs, const int64_t* node_counts,
+                                    const int32_t* const* edge_lists, const int64_t* edge_offsets, const float* num_incoming_edges_per_type,
+                                    int32_t annotation_size, const float* annotations, int32_t num_tasks, const float* labels,
+                                    const float* label_mask, ggnn_dataset** out);
+int ggnn_dataset_create_gcn(const ggnn_engine* e, int32_t for_training, int32_t num_graphs, const int64_t* node_counts, const int64_t* adjacency_lists,
+                            const int64_t* entry_offsets, const float* adjacency_weights, int32_t annotation_size, const float* annotations,
+                            int32_t num_tasks, const float* labels, const float* label_mask, ggnn_stream_t stream, ggnn_dataset** out);
+int ggnn_host_dataset_create_gcn(const ggnn_gcn_config* cfg, int32_t num_sms, int32_t for_training, int32_t num_graphs, const int64_t* node_counts,
+                                 const int64_t* adjacency_lists, const int64_t* entry_offsets, const float* adjacency_weights,
+                                 int32_t annotation_size, const float* annotations, int32_t num_tasks, const float* labels,
+                                 const float* label_mask, ggnn_dataset** out);
+int ggnn_free_dataset(ggnn_dataset* d);
+const char* ggnn_dataset_error(const ggnn_dataset* d);
+/* The two halves of a dataset batch, like ggnn_prepare_graph_* / ggnn_set_graph_prepared:
+ *   ggnn_dataset_prepare_batch   host only, from the dataset's summaries (no edge is read, the device is not touched but for the pinned
+ *                                table): the batch of graph_ids [num_graphs] (int64 dataset indices, in batch order; an id out of range is
+ *                                GGNN_ERANGE) -- its offsets, its cut points through the same tile planner, the image layout -- and a small
+ *                                pinned table of tile starts and per-graph offsets.  Reads the dataset and nothing else: callable from a
+ *                                producer thread.  save_for_backward 1 needs a training dataset.  *inout as for ggnn_prepare_graph_sparse
+ *                                (a rebuilt batch first waits for its previous table upload).
+ *   ggnn_set_graph_dataset       engine thread: adopts the plan and enqueues on `stream` the table upload and the kernels that write the
+ *                                batch's graph image into the engine's graph buffer, h0 [V, D] (the annotation columns, zeros elsewhere),
+ *                                target_values / target_mask [num_tasks, num_graphs] (DEVICE buffers of the caller) and the readout map
+ *                                (what ggnn_readout_set_graphs builds from the batch's graph_nodes_list).  No host synchronisation, no
+ *                                atomics, no allocation but the engine's buffers growing as for any upload.  The batch must stay alive
+ *                                until the stream passed it.  Like every graph upload it first forgets the previous batch (ggnn_layer_state,
+ *                                saved activations) -- and the readout map it replaces.  A batch prepared for an engine of another shape or
+ *                                on another device is refused (GGNN_EINVAL; another model: GGNN_ESTATE).
+ * A batch reads its dataset in every call: the dataset must outlive every batch prepared from it (free the batches first).
+ * ggnn_dataset_batch_info: as ggnn_prepared_graph_info, plus the tile starts [num_tiles + 1] and, for LOCAL (tile-local) plans, the values of
+ * ggnn_prepared_graph_tile_stats -- other plans' launches do not read them, and they are 0 there.  NULL pointers are skipped. */
+typedef struct ggnn_dataset_batch ggnn_dataset_batch;
+int ggnn_dataset_prepare_batch(const ggnn_dataset* d, int32_t save_for_backward, const int64_t* graph_ids, int32_t num_graphs,
+                               ggnn_dataset_batch** inout);
+int ggnn_dataset_batch_info(const ggnn_dataset_batch* b, int32_t* num_nodes, int64_t* num_messages, int32_t* num_tiles, int64_t* image_bytes,
+                            int32_t* is_streaming, char* plan_text, int32_t plan_text_capacity, int32_t* tile_start, int32_t* max_tile_msgs,
+                            int32_t* max_tile_types);
+int ggnn_free_dataset_batch(ggnn_dataset_batch* b);
+const char* ggnn_dataset_batch_error(const ggnn_dataset_batch* b);
+int ggnn_set_graph_dataset(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, float* target_values, float* target_mask, ggnn_stream_t stream);
+/* The engine's current graph image copied back to the host (the counterpart of ggnn_prepared_graph_image, whatever upload made it):
+ * *image_bytes gets its size; dst NULL only asks for it.  Synchronises `stream`. */
+int ggnn_graph_image(ggnn_engine* e, void* dst, int64_t capacity, int64_t* image_bytes, ggnn_stream_t stream);
 
 /* Introspection used by the parity tests and the benchmark. */
 int ggnn_num_messages(const ggnn_engine* e, int64_t* out);
