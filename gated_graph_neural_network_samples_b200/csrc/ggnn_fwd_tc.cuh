@@ -339,6 +339,41 @@ __device__ __forceinline__ void gemm_narrow(RingReader& ring, float (&acc)[WN / 
     retire_last(ring, prev, lane);
 }
 
+// gemm_narrow with A from registers (wgmma RS), for the compact bf16x3 instances: per K-step each warp loads its A_hi and A_lo fragments
+// once (ldmatrix) and the three MMAs take A from there, instead of each MMA reading A from shared memory again.  The same MMAs in the same
+// order as gemm_narrow, so the sums are bit-identical.  Every K-step is its own wgmma group: wait_group 1 after K-step k retires k-1,
+// whose A registers K-step k+1 reuses; slot i is released once its last K-step has retired.  `a_frag` = op + a_row + 16 * 16 * (warp
+// in warpgroup) + wg::lds_a_offset(lane, KGS).
+template <int WN, int DP, bool X3, uint32_t KGS>
+__device__ __forceinline__ void gemm_narrow_rs(RingReader& ring, float (&acc)[WN / 2], uint32_t a_frag, int col0, int lane) {
+    constexpr int NKS = DP / 16;
+    constexpr uint32_t STAGE_B = DP * 64u, PART_B = DP * KGS / 8u;
+    uint32_t sl = 0, prev = 0;
+#pragma unroll
+    for (int k = 0; k < NKS; ++k) {
+        if (k % 2 == 0) sl = ring.take();
+        const uint32_t b = ring.base + sl * 2u * STAGE_B + (uint32_t)(k % 2) * STAGE_B + (uint32_t)col0 * 16u;
+        const uint32_t a = a_frag + (uint32_t)k * 2u * KGS;
+        uint32_t ah[4], al[4];
+        wg::ldsm_a(ah, a);
+        if (X3) wg::ldsm_a(al, a + PART_B);
+        const uint64_t bd = wg::make_desc(b, 16u * DP, 128);
+        wg::fence();
+        wg::Mma<WN>::run(acc, ah, bd);
+        if (X3) {
+            wg::Mma<WN>::run(acc, ah, wg::make_desc(b + 32u * DP, 16u * DP, 128));
+            wg::Mma<WN>::run(acc, al, bd);
+        }
+        wg::commit();
+        if (k > 0) wg::wait<1>();
+        if (k % 2 == 0) {
+            if (k > 0) ring.release(prev, lane);   // K-step k-1, the previous slot's last, has retired
+            prev = sl;
+        }
+    }
+    retire_last(ring, prev, lane);
+}
+
 // The same product one slot at a time (commit, wait for every group, release), for the 128-row layout of ggnn_fwd_tc_kernel: its
 // accumulator fragments are twice as wide as the compact ones, ptxas cannot keep a wgmma pipeline under the 96-register cap of 17 warps,
 // and an unrolled pipelined body only lengthens live ranges and spills.  A warpgroup without rows (mma_rows false) skips the MMAs but
@@ -455,16 +490,45 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
         RingReader rd{bar_full, bar_empty, abortp, smem_u32(ring), (uint32_t)nst};
         const uint32_t a_row = (uint32_t)m0 * 16u;   // this warpgroup's first row inside an A operand
         const bool mma_rows = m0 < rows;             // warpgroup-uniform: the warpgroup has rows at all (always, on compact tiles)
-        // Compact tiles pipeline the MMAs (gemm_narrow); 128-row tiles issue one slot at a time (gemm_narrow_serial).
-        auto gemm_narrow = [&](float (&acc)[NF], const uint8_t* op) {
-            if constexpr (COMPACT) tc::gemm_narrow<WN, DP, X3, KGS>(rd, acc, smem_u32(op), a_row, col0, lane);
-            else tc::gemm_narrow_serial<WN, DP, X3, KGS>(rd, acc, smem_u32(op), a_row, col0, mma_rows, lane);
+        // Compact tiles pipeline the MMAs (gemm_narrow); 128-row tiles issue one slot at a time (gemm_narrow_serial).  `rs` (a constant
+        // at every call): on compact tiles, A from registers -- gemm_narrow_rs at bf16x3 (A_hi feeds two MMAs); a bf16 K-step has one MMA
+        // per A, so it stays in shared memory.  The residual pre-products keep A in shared memory: with their three accumulators and the
+        // state live, register A makes ptxas serialise every MMA of the NH 56 and 64 instances.
+        const uint32_t a_frag = a_row + (uint32_t)(warp & 3) * 256u + wg::lds_a_offset(lane, KGS);   // this warp's ldsm_a offset
+        auto gemm_narrow = [&](float (&acc)[NF], const uint8_t* op, bool rs) {
+            if constexpr (COMPACT) {
+                if (X3 && rs) tc::gemm_narrow_rs<WN, DP, X3, KGS>(rd, acc, smem_u32(op) + a_frag, col0, lane);
+                else tc::gemm_narrow<WN, DP, X3, KGS>(rd, acc, smem_u32(op), a_row, col0, lane);
+            } else {
+                tc::gemm_narrow_serial<WN, DP, X3, KGS>(rd, acc, smem_u32(op), a_row, col0, mma_rows, lane);
+            }
         };
         // [r | u] += A(op) . B(one segment of the N = 2*DP gate block: NKS slots, stage 0 = hi, stage 1 = lo); columns of r and of u.
         // One K-step per slot; slot i's MMAs stay in flight while slot i+1's are issued (compact), or one slot at a time (128-row).
-        auto wide_mmas = [&](float (&ar)[NF], float (&au)[NF], uint32_t sl, uint32_t a) {
+        // `rs`, compact tiles: A from registers, at both precisions (every A part feeds the MMAs of r and of u), loaded once per K-step;
+        // the same MMAs in the same order.  The group of slot i-1 has retired before slot i+1 reloads the registers (retire_slot's
+        // wait_group 1).
+        auto wide_mmas = [&](float (&ar)[NF], float (&au)[NF], uint32_t sl, uint32_t a, bool rs) {
             const uint32_t bh = rd.base + sl * 2u * STAGE_B, bl = bh + STAGE_B;
             const uint32_t cr = (uint32_t)col0 * 16u, cu = (uint32_t)(DP + col0) * 16u, lbo = 32u * DP;
+            if constexpr (COMPACT) {
+                if (rs) {
+                    uint32_t ah[4], al[4];
+                    wg::ldsm_a(ah, a - a_row + a_frag);
+                    if (X3) wg::ldsm_a(al, a - a_row + a_frag + PART_B);
+                    wg::fence();
+                    wg::Mma<WN>::run(ar, ah, wg::make_desc(bh + cr, lbo, 128));
+                    wg::Mma<WN>::run(au, ah, wg::make_desc(bh + cu, lbo, 128));
+                    if (X3) {
+                        wg::Mma<WN>::run(ar, ah, wg::make_desc(bl + cr, lbo, 128));
+                        wg::Mma<WN>::run(au, ah, wg::make_desc(bl + cu, lbo, 128));
+                        wg::Mma<WN>::run(ar, al, wg::make_desc(bh + cr, lbo, 128));
+                        wg::Mma<WN>::run(au, al, wg::make_desc(bh + cu, lbo, 128));
+                    }
+                    wg::commit();
+                    return;
+                }
+            }
             const uint64_t ad = wg::make_desc(a, KGS, 128);
             wg::fence();
             wg::Mma<WN>::run(ar, ad, wg::make_desc(bh + cr, lbo, 128));
@@ -478,13 +542,13 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
             }
             wg::commit();
         };
-        auto gemm_wide = [&](float (&ar)[NF], float (&au)[NF], const uint8_t* op) {
+        auto gemm_wide = [&](float (&ar)[NF], float (&au)[NF], const uint8_t* op, bool rs) {
             if constexpr (COMPACT) {
                 uint32_t prev = 0;
 #pragma unroll
                 for (int i = 0; i < NKS; ++i) {
                     const uint32_t sl = rd.take();
-                    wide_mmas(ar, au, sl, smem_u32(op) + (uint32_t)i * 2u * KGS + a_row);
+                    wide_mmas(ar, au, sl, smem_u32(op) + (uint32_t)i * 2u * KGS + a_row, rs);
                     retire_slot(rd, sl, prev, i == 0, lane);
                 }
                 retire_last(rd, prev, lane);
@@ -493,7 +557,7 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                 for (int i = 0; i < NKS; ++i) {
                     const uint32_t sl = rd.take();
                     if (mma_rows) {
-                        wide_mmas(ar, au, sl, smem_u32(op) + (uint32_t)i * 2u * KGS + a_row);
+                        wide_mmas(ar, au, sl, smem_u32(op) + (uint32_t)i * 2u * KGS + a_row, rs);
                         wg::wait_all();
                     }
                     rd.release(sl, lane);
@@ -572,8 +636,8 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                     })
                     publish_sync();
                     if (!ok) break;
-                    if (gru) gemm_wide(pr, pu, opA);
-                    gemm_narrow(pc, opA);
+                    if (gru) gemm_wide(pr, pu, opA, false);
+                    gemm_narrow(pc, opA, false);
                     workers_sync();   // opA is rewritten next
                 }
                 GGNN_FRAG_PAIRS({
@@ -673,9 +737,9 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                     publish_sync();
                     if (!ok) break;
                     if constexpr (COMPACT) {
-                        for (int k = 0, j = gt0; k < n; ++k, j = (j + 1 == ngather) ? 0 : j + 1) gemm_narrow(acc, opX + (size_t)j * OPB);
+                        for (int k = 0, j = gt0; k < n; ++k, j = (j + 1 == ngather) ? 0 : j + 1) gemm_narrow(acc, opX + (size_t)j * OPB, true);
                     } else {
-                        gemm_narrow(acc, gdst);
+                        gemm_narrow(acc, gdst, false);
                     }
                     n = 0;
                 }
@@ -707,8 +771,8 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                         // -------------------------------------------------------- gates: r*h -> opA, u stays in registers
                         float gr[NF];
                         zero(gr); zero(gu);
-                        gemm_wide(gr, gu, opX);
-                        gemm_wide(gr, gu, opH);
+                        gemm_wide(gr, gu, opX, true);
+                        gemm_wide(gr, gu, opH, true);
                         GGNN_FRAG_PAIRS({
                             float br0 = sBias[fc], br1 = sBias[fc + 1], bu0 = sBias[DP + fc], bu1 = sBias[DP + fc + 1];
                             if (ly.nres > 0) {
@@ -731,8 +795,8 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                     // ------------------------------------------------------------ candidate [agg | r*h] . K_c (GRU), [agg | h] . K_c (RNN); new state
                     float gc[NF];
                     zero(gc);
-                    gemm_narrow(gc, opX);
-                    gemm_narrow(gc, gru ? opA : opH);
+                    gemm_narrow(gc, opX, true);
+                    gemm_narrow(gc, gru ? opA : opH, true);
                     GGNN_FRAG_PAIRS({
                         float bc0 = sBias[2 * DP + fc], bc1 = sBias[2 * DP + fc + 1];
                         if (ly.nres > 0) {
@@ -757,8 +821,8 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                         // -------------------------------------------------------- gates: r*h -> opA, u stays in registers
                         float gr[NF], gu[NF];
                         zero(gr); zero(gu);
-                        gemm_wide(gr, gu, opX);
-                        gemm_wide(gr, gu, opH);
+                        gemm_wide(gr, gu, opX, false);
+                        gemm_wide(gr, gu, opH, false);
                         GGNN_FRAG_PAIRS({
                             float br0 = sBias[fc], br1 = sBias[fc + 1], bu0 = sBias[DP + fc], bu1 = sBias[DP + fc + 1];
                             if (ly.nres > 0) {
@@ -780,8 +844,8 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                         // -------------------------------------------------------- candidate, new state
                         float gc[NF];
                         zero(gc);
-                        gemm_narrow(gc, opX);
-                        gemm_narrow(gc, opA);
+                        gemm_narrow(gc, opX, false);
+                        gemm_narrow(gc, opA, false);
                         GGNN_FRAG_PAIRS({
                             float bc0 = sBias[2 * DP + fc], bc1 = sBias[2 * DP + fc + 1];
                             if (ly.nres > 0) {
@@ -798,8 +862,8 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                     } else {
                         float gc[NF];
                         zero(gc);
-                        gemm_narrow(gc, opX);
-                        gemm_narrow(gc, opH);
+                        gemm_narrow(gc, opX, false);
+                        gemm_narrow(gc, opH, false);
                         GGNN_FRAG_PAIRS({
                             float bc0 = sBias[2 * DP + fc], bc1 = sBias[2 * DP + fc + 1];
                             if (ly.nres > 0) {

@@ -1,5 +1,10 @@
 // wgmma (Hopper warpgroup MMA) wrappers: D[64 x N] (+)= A[64 x 16] . B[16 x N], BF16 inputs, FP32 accumulators in registers,
 // both operands K-major in shared memory, described by make_desc().  One specialisation per N: the instruction's N is an immediate.
+// N <= 32 also has a register-A form (RS): A as four .b32 registers per thread, loaded by ldsm_a(); B stays in shared memory.
+//
+// Register A fragment of thread t (warp w of the warpgroup, lane l, g = l/4, c = l%4), bf16 pairs: a[0] = (16w + g, 2c..2c+1),
+// a[1] = (16w + g + 8, 2c..), a[2] = (16w + g, 2c+8..), a[3] = (16w + g + 8, 2c+8..).  The registers must stay unchanged until a
+// wait_group retires the MMA that reads them.
 //
 // Accumulator fragment of thread t of the warpgroup (warp w = t / 32, lane l): rows r0 = 16*w + l/4 and r0 + 8; for every 8-column
 // block j, columns c = 8*j + 2*(l%4) and c + 1:  d[4j] = (r0, c), d[4j+1] = (r0, c+1), d[4j+2] = (r0+8, c), d[4j+3] = (r0+8, c+1).
@@ -21,6 +26,13 @@ __device__ __forceinline__ void wait_all() { asm volatile("wgmma.wait_group.sync
 template <int N>
 __device__ __forceinline__ void wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
+// This warp's A fragment of one K-step from a canonical K-major no-swizzle operand (core matrix = 8 rows x 16 bytes, k-group stride KGS):
+// ldmatrix.x4 of its four 8x8 core matrices.  `addr` = the K-step's first k-group + row 16w, plus lds_a_offset(lane, KGS).
+__device__ __forceinline__ uint32_t lds_a_offset(int lane, uint32_t kgs) { return (uint32_t)(lane >> 4) * kgs + (uint32_t)(lane & 15) * 16u; }
+__device__ __forceinline__ void ldsm_a(uint32_t (&a)[4], uint32_t addr) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(a[0]), "=r"(a[1]), "=r"(a[2]), "=r"(a[3]) : "r"(addr));
+}
+
 template <int N>
 struct Mma;
 
@@ -32,6 +44,12 @@ struct Mma<8> {
                      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
                      : "l"(a), "l"(b), "r"(1));
     }
+    static __device__ __forceinline__ void run(float (&d)[4], const uint32_t (&a)[4], uint64_t b) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %9, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0,%1,%2,%3}, {%4,%5,%6,%7}, %8, p, 1, 1, 0;\n\t}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1));
+    }
 };
 
 template <>
@@ -41,6 +59,12 @@ struct Mma<16> {
                      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}\n"
                      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
                      : "l"(a), "l"(b), "r"(1));
+    }
+    static __device__ __forceinline__ void run(float (&d)[8], const uint32_t (&a)[4], uint64_t b) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, 0;\n\t}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1));
     }
 };
 
@@ -52,6 +76,12 @@ struct Mma<24> {
                      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
                      : "l"(a), "l"(b), "r"(1));
     }
+    static __device__ __forceinline__ void run(float (&d)[12], const uint32_t (&a)[4], uint64_t b) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %17, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n24k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, %16, p, 1, 1, 0;\n\t}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1));
+    }
 };
 
 template <>
@@ -61,6 +91,12 @@ struct Mma<32> {
                      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}\n"
                      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
                      : "l"(a), "l"(b), "r"(1));
+    }
+    static __device__ __forceinline__ void run(float (&d)[16], const uint32_t (&a)[4], uint64_t b) {
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+                     "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1, 0;\n\t}\n"
+                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(1));
     }
 };
 
