@@ -16,7 +16,8 @@
 // the gates, the candidate and their epilogues line up element for element in each thread's wgmma accumulator fragment, and the fp32
 // master copy of the node states stays in registers for the whole launch (LOCAL mode: the recurrence never leaves the SM).  On compact
 // tiles (<= 64 rows) all four warpgroups work on rows 0..63 and split the columns four ways instead (COMPACT_WIDTH), so none of them
-// idles on rows that do not exist.  The gathers are row-per-thread over all 16 worker warps.
+// idles on rows that do not exist.  The gathers are row-per-thread over all 16 worker warps (compact tiles with the CSR slice in shared
+// memory: one task per real row and 8-column chunk).
 //
 // Shared memory (ggnn_tc_smem.h): A-operand tiles, each hi+lo in the canonical K-major no-swizzle layout
 //   byte(row, k) = part*PART_B + (k/8)*KGS + row*16 + (k%8)*2     (KGS = 16 * allocated rows: 2048, or 1024 for compact <= 64-row tiles)
@@ -658,6 +659,7 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                 zero(acc);
                 const int gsz = __popc(tmask) <= ngather ? ngather : ngather / 2;   // (compact)
                 int nty = 0, n = 0, gt = 0, gt0 = 0;   // types gathered; of them in the open group; the next gather tile; the group's first
+                unsigned grp = 0u;   // (compact, CSR slice in shared memory) the open group's types, gathered when it closes
                 // The gather touches shared memory only, so with compact tiles -- rows 0..63 only -- all 16 worker warps share it:
                 // row group = warp & 1, eight column-chunk groups instead of four.
                 const bool gsplit = KGS == 1024u;
@@ -673,67 +675,116 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                     gt = gt + 1 == ngather ? 0 : gt + 1;
                     ++nty;
                     ++n;
-                    int beg = 0, end = 0;
-                    if (g_row_ok) {
-                        if (csr_smem) { beg = sRowPtr[g_row * T + t]; end = sRowPtr[g_row * T + t + 1]; }
-                        else { beg = p.row_ptr[(size_t)g_grow * T + t]; end = p.row_ptr[(size_t)g_grow * T + t + 1]; }
-                    }
-                    for (int kc = g_cg; kc < g_nkc; kc += g_ncg) {
-                        float a8[8];
+                    if (COMPACT && csr_smem) {
+                        grp |= 1u << t;
+                    } else {
+                        int beg = 0, end = 0;
+                        if (g_row_ok) {
+                            if (csr_smem) { beg = sRowPtr[g_row * T + t]; end = sRowPtr[g_row * T + t + 1]; }
+                            else { beg = p.row_ptr[(size_t)g_grow * T + t]; end = p.row_ptr[(size_t)g_grow * T + t + 1]; }
+                        }
+                        for (int kc = g_cg; kc < g_nkc; kc += g_ncg) {
+                            float a8[8];
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) a8[j] = 0.0f;
-                        if (LOCAL && csr_smem) {
-                            // fast path: local source indices from shared memory, two messages in flight
-                            const uint8_t* colbase = opH + (size_t)kc * KGS;
-                            const uint32_t lo_off = PART_B;
-                            int m = beg;
-                            if (X3) {
-                                for (; m + 1 < end; m += 2) {
-                                    const uint8_t* s0 = colbase + (size_t)sSrc[m] * 16;
-                                    const uint8_t* s1 = colbase + (size_t)sSrc[m + 1] * 16;
-                                    const uint4 h0 = *reinterpret_cast<const uint4*>(s0), l0 = *reinterpret_cast<const uint4*>(s0 + lo_off);
-                                    const uint4 h1 = *reinterpret_cast<const uint4*>(s1), l1 = *reinterpret_cast<const uint4*>(s1 + lo_off);
-                                    unpack8_add(h0, a8, 1.0f); unpack8_add(h1, a8, 1.0f);
-                                    unpack8_add(l0, a8, 1.0f); unpack8_add(l1, a8, 1.0f);
-                                }
-                                if (m < end) {
-                                    const uint8_t* s0 = colbase + (size_t)sSrc[m] * 16;
-                                    unpack8_add(*reinterpret_cast<const uint4*>(s0), a8, 1.0f);
-                                    unpack8_add(*reinterpret_cast<const uint4*>(s0 + lo_off), a8, 1.0f);
+                            for (int j = 0; j < 8; ++j) a8[j] = 0.0f;
+                            if (LOCAL && csr_smem) {
+                                // fast path: local source indices from shared memory, two messages in flight
+                                const uint8_t* colbase = opH + (size_t)kc * KGS;
+                                const uint32_t lo_off = PART_B;
+                                int m = beg;
+                                if (X3) {
+                                    for (; m + 1 < end; m += 2) {
+                                        const uint8_t* s0 = colbase + (size_t)sSrc[m] * 16;
+                                        const uint8_t* s1 = colbase + (size_t)sSrc[m + 1] * 16;
+                                        const uint4 h0 = *reinterpret_cast<const uint4*>(s0), l0 = *reinterpret_cast<const uint4*>(s0 + lo_off);
+                                        const uint4 h1 = *reinterpret_cast<const uint4*>(s1), l1 = *reinterpret_cast<const uint4*>(s1 + lo_off);
+                                        unpack8_add(h0, a8, 1.0f); unpack8_add(h1, a8, 1.0f);
+                                        unpack8_add(l0, a8, 1.0f); unpack8_add(l1, a8, 1.0f);
+                                    }
+                                    if (m < end) {
+                                        const uint8_t* s0 = colbase + (size_t)sSrc[m] * 16;
+                                        unpack8_add(*reinterpret_cast<const uint4*>(s0), a8, 1.0f);
+                                        unpack8_add(*reinterpret_cast<const uint4*>(s0 + lo_off), a8, 1.0f);
+                                    }
+                                } else {
+                                    for (; m < end; ++m) unpack8_add(*reinterpret_cast<const uint4*>(colbase + (size_t)sSrc[m] * 16), a8, 1.0f);
                                 }
                             } else {
-                                for (; m < end; ++m) unpack8_add(*reinterpret_cast<const uint4*>(colbase + (size_t)sSrc[m] * 16), a8, 1.0f);
-                            }
-                        } else {
-                            // each message scaled by its slot weight (a weighted dense adjacency) or by 1: fmaf(1, x, y) rounds as x + y
-                            for (int m = beg; m < end; ++m) {
-                                if (LOCAL) {
-                                    const float a = p.slot_w ? p.slot_w[m] : 1.0f;
-                                    const uint8_t* sp = opH + (size_t)kc * KGS + (size_t)(p.csr_src[m] - row0) * 16;
-                                    unpack8_add(*reinterpret_cast<const uint4*>(sp), a8, a);
-                                    if (X3) unpack8_add(*reinterpret_cast<const uint4*>(sp + PART_B), a8, a);
-                                } else {
-                                    // GLOBAL mode: source rows come from the previous step's fp32 state in L2; keep 4 rows in flight (each
-                                    // weight is read at its accumulate step, not beside the row loads)
-                                    float hv[4][8];
-                                    const int nb = min(4, end - m);
+                                // each message scaled by its slot weight (a weighted dense adjacency) or by 1: fmaf(1, x, y) rounds as x + y
+                                for (int m = beg; m < end; ++m) {
+                                    if (LOCAL) {
+                                        const float a = p.slot_w ? p.slot_w[m] : 1.0f;
+                                        const uint8_t* sp = opH + (size_t)kc * KGS + (size_t)(p.csr_src[m] - row0) * 16;
+                                        unpack8_add(*reinterpret_cast<const uint4*>(sp), a8, a);
+                                        if (X3) unpack8_add(*reinterpret_cast<const uint4*>(sp + PART_B), a8, a);
+                                    } else {
+                                        // GLOBAL mode: source rows come from the previous step's fp32 state in L2; keep 4 rows in flight (each
+                                        // weight is read at its accumulate step, not beside the row loads)
+                                        float hv[4][8];
+                                        const int nb = min(4, end - m);
 #pragma unroll
-                                    for (int qq = 0; qq < 4; ++qq)
-                                        if (qq < nb) load8_guarded_cg(p.g_in + (size_t)p.csr_src[m + qq] * D, kc * 8, D, hv[qq]);
+                                        for (int qq = 0; qq < 4; ++qq)
+                                            if (qq < nb) load8_guarded_cg(p.g_in + (size_t)p.csr_src[m + qq] * D, kc * 8, D, hv[qq]);
 #pragma unroll
-                                    for (int qq = 0; qq < 4; ++qq)
-                                        if (qq < nb) {
-                                            const float a = p.slot_w ? p.slot_w[m + qq] : 1.0f;
+                                        for (int qq = 0; qq < 4; ++qq)
+                                            if (qq < nb) {
+                                                const float a = p.slot_w ? p.slot_w[m + qq] : 1.0f;
 #pragma unroll
-                                            for (int j = 0; j < 8; ++j) a8[j] = fmaf(a, hv[qq][j], a8[j]);
-                                        }
-                                    m += nb - 1;
+                                                for (int j = 0; j < 8; ++j) a8[j] = fmaf(a, hv[qq][j], a8[j]);
+                                            }
+                                        m += nb - 1;
+                                    }
                                 }
                             }
+                            store_operand_chunk(gdst, KGS, PART_B, kc, g_row, a8);
                         }
-                        store_operand_chunk(gdst, KGS, PART_B, kc, g_row, a8);
                     }
                     if (COMPACT && n < gsz && ((tmask >> t) >> 1) != 0) continue;   // the group is open and another type follows
+                    if (COMPACT && csr_smem) {
+                        // One task per (real row, 8-column chunk), spread over all 512 worker threads, rows fastest (a warp's stores
+                        // are contiguous); a task sums the messages of each of the group's types in turn into its gather tile, in the
+                        // order of the row-per-thread loop (CSR order, a pair added h0, h1, l0, l1, the odd message last).  Pad rows
+                        // (>= rows) of the gather tiles are not written and may hold anything, NaN included: wgmma output row i reads
+                        // A row i only, so they reach pad rows of acc only, which the agg epilogue replaces by 0 (v0 = fr < rows ? ... :
+                        // 0); every operand of the gate and candidate GEMMs (opX, opA, opH) thus has finite pad rows, and so has hs.
+                        const int dk = NUM_WORKERS / rows, dr = NUM_WORKERS - dk * rows;   // task += 512 in (chunk, row); rows >= 1
+                        for (int kc = tid / rows, trow = tid - kc * rows; kc < NKC;) {
+                            const uint16_t* rp = sRowPtr + trow * T;
+                            const uint8_t* colbase = opH + (size_t)kc * KGS;
+                            int j = gt0;
+                            for (unsigned g = grp; g != 0u; g &= g - 1u) {
+                                const int tg = __ffs(g) - 1;
+                                float a8[8];
+#pragma unroll
+                                for (int e = 0; e < 8; ++e) a8[e] = 0.0f;
+                                int m = rp[tg];
+                                const int end = rp[tg + 1];
+                                if (X3) {
+                                    for (; m + 1 < end; m += 2) {
+                                        const uint8_t* s0 = colbase + (size_t)sSrc[m] * 16;
+                                        const uint8_t* s1 = colbase + (size_t)sSrc[m + 1] * 16;
+                                        const uint4 h0 = *reinterpret_cast<const uint4*>(s0), l0 = *reinterpret_cast<const uint4*>(s0 + PART_B);
+                                        const uint4 h1 = *reinterpret_cast<const uint4*>(s1), l1 = *reinterpret_cast<const uint4*>(s1 + PART_B);
+                                        unpack8_add(h0, a8, 1.0f); unpack8_add(h1, a8, 1.0f);
+                                        unpack8_add(l0, a8, 1.0f); unpack8_add(l1, a8, 1.0f);
+                                    }
+                                    if (m < end) {
+                                        const uint8_t* s0 = colbase + (size_t)sSrc[m] * 16;
+                                        unpack8_add(*reinterpret_cast<const uint4*>(s0), a8, 1.0f);
+                                        unpack8_add(*reinterpret_cast<const uint4*>(s0 + PART_B), a8, 1.0f);
+                                    }
+                                } else {
+                                    for (; m < end; ++m) unpack8_add(*reinterpret_cast<const uint4*>(colbase + (size_t)sSrc[m] * 16), a8, 1.0f);
+                                }
+                                store_operand_chunk(opX + (size_t)j * OPB, KGS, PART_B, kc, trow, a8);
+                                j = j + 1 == ngather ? 0 : j + 1;
+                            }
+                            kc += dk;
+                            trow += dr;
+                            if (trow >= rows) { trow -= rows; ++kc; }
+                        }
+                        grp = 0u;
+                    }
                     publish_sync();
                     if (!ok) break;
                     if constexpr (COMPACT) {
@@ -878,8 +929,13 @@ __global__ void __launch_bounds__(NTHREADS<COMPACT>, 1) ggnn_fwd_tc_kernel(const
                         for (int i = 0; i < NF; ++i) hs[i] = gc[i];
                     }
                 }
-                workers_sync();   // every MMA that reads opH is complete before the state update rewrites it
-                if (!ok) break;
+                // Every MMA that reads opH must be complete before the state update rewrites it.  On compact GRU tiles they are already:
+                // each warpgroup's gate GEMM, the last reader, drained before the barrier after the gate epilogue, and the candidate reads
+                // opX and opA only.  (Writing the state from the candidate epilogue instead keeps more of it live there and spills more.)
+                if (!COMPACT || !gru) {
+                    workers_sync();
+                    if (!ok) break;
+                }
                 GGNN_FRAG_PAIRS({
                     if (p.drop_keep < 1.0f) {
                         hs[fi] = dropout_apply(hs[fi], p.drop_seed, p.step_base[l] + s, p.V, D, fg, fc, p.drop_keep);
