@@ -64,11 +64,14 @@ class DenseGGNNChemModel(ChemModel):
         import torch
         feed = self.feed
         T, D = self.num_edge_types, self.params['hidden_size']
-        adj = np.asarray(feed[self.placeholders['adjacency_matrix']], dtype=np.float32)          # [b, e, v, v]
-        b, v = adj.shape[0], adj.shape[2]
-        self.engine.set_save_for_backward(torch.is_grad_enabled())
-        if not self._adopt_prepared_graph(feed):     # a graph built by the batch producer thread leaves only the upload
-            self.engine.set_graph_dense(adj)
+        if feed.get('_graph_adopted'):   # a device-data batch, assembled on the device by forward_batch (_adopt_dataset_batch)
+            b, v = int(feed[self.placeholders['num_graphs']]), int(feed[self.placeholders['num_vertices']])
+        else:
+            adj = np.asarray(feed[self.placeholders['adjacency_matrix']], dtype=np.float32)      # [b, e, v, v]
+            b, v = adj.shape[0], adj.shape[2]
+            self.engine.set_save_for_backward(torch.is_grad_enabled())
+            if not self._adopt_prepared_graph(feed):     # a graph built by the batch producer thread leaves only the upload
+                self.engine.set_graph_dense(adj)
         keep = float(feed.get(self.placeholders['edge_weight_dropout_keep_prob'], 1.0))
         edge_weights = self.weights['edge_weights']
         if keep < 1.0:
@@ -97,19 +100,20 @@ class DenseGGNNChemModel(ChemModel):
     def gated_regression(self, last_h, regression_gate, regression_transform):   # dense:119-129
         import torch
         D = self.params['hidden_size']
-        h0 = self.initial_node_representation_tensor()
+        h0 = self.initial_node_representation_tensor().reshape(last_h.shape)   # a device-data batch's h0 is [b*v, D]
         fused = last_h.is_cuda and getattr(self, '_padded_hidden', D) == D   # affine() draws the weight-dropout mask: only when it is used
         ag = regression_gate.affine() if fused and hasattr(regression_gate, 'affine') else None
         at = regression_transform.affine() if fused and hasattr(regression_transform, 'affine') else None
         if ag is not None and at is not None:   # fused kernel (SURVEY 8f-1): masked per-graph sum included
             b, v = last_h.shape[0], last_h.shape[1]
-            self.engine.readout_set_graphs(b, nodes_per_graph=v, node_mask=self.feed[self.placeholders['node_mask']])
+            if not self.feed.get('_graph_adopted'):   # a device-data batch set the readout map and mask with its graph
+                self.engine.readout_set_graphs(b, nodes_per_graph=v, node_mask=self.feed[self.placeholders['node_mask']])
             self.output = self._readout.apply(self.engine, last_h.reshape(b * v, D), h0.reshape(b * v, D), ag[0], ag[1], at[0], at[1])
             return self.output
         gate_input = torch.cat([last_h, h0], dim=2).reshape(-1, 2 * D)
         gated = torch.sigmoid(regression_gate(gate_input)) * regression_transform(last_h.reshape(-1, D))
         gated = gated.reshape(last_h.shape[0], last_h.shape[1])
-        mask = torch.as_tensor(np.asarray(self.feed[self.placeholders['node_mask']], dtype=np.float32), device=self.device)
+        mask = self._as_device_tensor(self.feed[self.placeholders['node_mask']])
         self.output = (gated * mask).sum(dim=1)
         return self.output
 
@@ -144,9 +148,23 @@ class DenseGGNNChemModel(ChemModel):
                 np.random.shuffle(b)
         counters = defaultdict(int)
         keep = self.params['graph_state_dropout_keep_prob'] if is_training else 1.
+        device_data = getattr(self, 'device_data', False)
+        if device_data:
+            # --device-data: one dataset of every bucket's graphs, uploaded once; after the same shuffles as above, a batch's graphs are
+            # found by identity (their flat ids) and the batch is assembled on the device (forward_batch adopts it)
+            keys = list(bucketed)
+            flat, order = self._flat_view([g for k in keys for g in bucketed[k]], lambda d: packing.FlatDenseGraphs(
+                d, self.params['task_ids'], self.params['tie_fwd_bkwd']), key=bucketed)
+            first = dict(zip(keys, np.cumsum([0] + [len(bucketed[k]) for k in keys]).tolist()))
         for bucket in bucket_at_step:
             start = counters[bucket] * self.params['batch_size']
             elements = bucketed[bucket][start:start + self.params['batch_size']]
+            if device_data:
+                counters[bucket] += 1
+                v, ids = int(bucket_sizes[bucket]), order[first[bucket] + start:first[bucket] + start + len(elements)]
+                yield {'num_graphs': len(ids), 'num_vertices': v, 'graph_state_keep_prob': keep, 'edge_weight_dropout_keep_prob': keep,
+                       '_dataset_batch': self._dataset_batch(flat, ids, is_training, nodes_per_graph=v)}
+                continue
             feed = packing.pack_dense_batch(elements, int(bucket_sizes[bucket]), self.params['hidden_size'], self.num_edge_types,
                                             self.params['task_ids'], self.params['tie_fwd_bkwd'])
             feed['graph_state_keep_prob'] = keep

@@ -280,19 +280,21 @@ class ChemModel(object):
         return self._as_device_tensor(self.feed[self.placeholders['initial_node_representation']])
 
     # ------------------------------------------------------------------ batch plumbing the plug-ins share
-    def _flat_view(self, data, flatten):
+    def _flat_view(self, data, flatten, key=None):
         """(``flatten(data)``, the flat ids of ``data``'s graphs in the list's current order).  The flattened graphs are built once per list
         object and kept while the list keeps its graphs (it is shuffled in place every epoch); graphs are identified by object identity, so
-        copies of the list or a changed membership simply rebuild."""
+        copies of the list or a changed membership simply rebuild.  ``key``: the object that owns the graphs when ``data`` is a fresh list of
+        them (the dense plug-in's buckets)."""
+        key = data if key is None else key
         cache = self.__dict__.setdefault('_flat_cache', [])
         for ref, flat, pos in cache:
-            if ref is data and flat.num_graphs == len(data):
+            if ref is key and flat.num_graphs == len(data):
                 try:
                     return flat, np.fromiter((pos[id(g)] for g in data), dtype=np.int64, count=len(data))
                 except KeyError:
                     break
         flat = flatten(data)
-        cache[:] = [c for c in cache if c[0] is not data][-3:] + [(data, flat, {id(g): i for i, g in enumerate(data)})]
+        cache[:] = [c for c in cache if c[0] is not key][-3:] + [(key, flat, {id(g): i for i, g in enumerate(data)})]
         return flat, np.arange(len(data), dtype=np.int64)
 
     def _prepare_from_pool(self, prepare, is_training: bool):
@@ -314,10 +316,10 @@ class ChemModel(object):
         self.__dict__.setdefault('_prepared_pool', []).append(prepared)   # rebuilt in place for a later batch; a rebuild first waits for this upload
         return True
 
-    def _dataset_batch(self, flat, ids, is_training: bool):
+    def _dataset_batch(self, flat, ids, is_training: bool, nodes_per_graph=None):
         """--device-data, in the batch producer thread: the host half of the batch of flat ids ``ids`` (engine.DatasetBatch), from the
         dataset of ``flat`` -- uploaded at its first batch and kept while the list keeps its flattened view (one per data list, like
-        _flat_view).  Batches taken back from the pool are rebuilt in place."""
+        _flat_view).  Batches taken back from the pool are rebuilt in place.  ``nodes_per_graph``: the bucket size of a dense batch."""
         from .engine import DeviceDataset
         cache = self.__dict__.setdefault('_dataset_cache', [])
         ds = next((d for f, d in cache if f is flat), None)
@@ -329,17 +331,20 @@ class ChemModel(object):
         reuse = next((b for b in pool if b.dataset is ds), None)
         if reuse is not None:
             pool.remove(reuse)
-        return ds.prepare_batch(ids, save_for_backward=is_training, reuse=reuse)
+        return ds.prepare_batch(ids, save_for_backward=is_training, reuse=reuse, nodes_per_graph=nodes_per_graph)
 
     def _adopt_dataset_batch(self, feed) -> None:
         """--device-data, on the engine's thread: assembles the feed's dataset batch on the device and puts its h0, targets and mask (CUDA
-        tensors) into the feed slots the hooks read.  The readout map is set with it.  A feed without a dataset batch is left as it is."""
+        tensors) into the feed slots the hooks read -- a dense batch's node mask too.  The readout map is set with it.  A feed without a
+        dataset batch is left as it is."""
         import torch
         batch = feed.pop('_dataset_batch', None)
         if batch is None:
             return
         self.engine.set_save_for_backward(torch.is_grad_enabled())   # before the upload: the source-keyed CSR is part of the image
-        h0, tv, tm = self.engine.set_graph_from_dataset(batch)
+        h0, tv, tm, *mask = self.engine.set_graph_from_dataset(batch)
+        if mask:
+            feed[self.placeholders['node_mask']] = mask[0]
         D = self.params['hidden_size']
         feed[self.placeholders['initial_node_representation']] = h0[:, :D] if h0.shape[1] != D else h0   # the engine's width may be padded
         feed[self.placeholders['target_values']], feed[self.placeholders['target_mask']] = tv, tm

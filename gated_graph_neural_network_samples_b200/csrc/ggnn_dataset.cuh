@@ -10,6 +10,10 @@
 // ds_graph_kernel: one block per graph of the batch, each writes its graph's rows, slots, nodes and labels -- no two blocks write the same
 // byte, so there are no atomics and the image is a function of the dataset and the id list.  ds_tile_kernel then fills what depends on
 // the tiles (tile starts, edge-type masks, first virtual row per tile) and the pair-table rows beyond the last node.
+//
+// A dense batch (ggnn_dataset_prepare_batch_dense, DsOut::v > 0) gives graph i the rows i*v .. i*v+v-1: the graph's own V_g rows, then
+// v - V_g isolated padding rows, written as the host builder writes a row without messages (row_ptr = the graph's slot end, in-degree 0,
+// denominator 0 + 1e-7, no source, h0 zero, node mask 0).  Sparse and GCN batches (v = 0) skip every padding branch.
 #pragma once
 #include "ggnn_common.cuh"
 #include "ggnn_fwd_stream.cuh"
@@ -42,6 +46,7 @@ struct DsArrays {
     const float* ann;      // [sum V][ann_size]
     const float* labels;   // [N][tasks]
     const float* lmask;    // [N][tasks]
+    const int* nfeat;      // [N] dense datasets: the graph's feature count (its node mask is local row < nfeat)
     int ann_size, tasks;
 };
 
@@ -57,7 +62,9 @@ struct DsOut {
     float* h0;               // [V][D]
     float *tv, *tm;          // [tasks][G]
     int *ro_graph_of, *ro_start;
+    float *node_mask, *ro_mask;       // dense batches: [V] the caller's node mask and the readout's copy
     int V, D, T, G, ntiles, nv, rec;   // rec: ints per batch record (R_MBASE + T)
+    int v;                             // dense batches: rows per graph (nodes_per_graph); 0 for sparse and GCN batches
 };
 
 __global__ void __launch_bounds__(256) ds_graph_kernel(const DsArrays a, const DsOut o, const int* __restrict__ table) {
@@ -110,6 +117,26 @@ __global__ void __launch_bounds__(256) ds_graph_kernel(const DsArrays a, const D
         const int v = (int)(k / D), c = (int)(k % D);
         o.h0[(size_t)noff * D + k] = c < A ? a.ann[(size_t)(nb + v) * A + c] : 0.0f;
     }
+    if (o.v > 0) {   // dense: the node mask of the real rows, then the padding rows Vg .. v-1 (isolated, every slot pointer at the graph's end)
+        const int nf = a.nfeat[gid], Mg = a.base[(size_t)(gid + 1) * B_WIDTH + B_SLOT] - sb, npad = o.v - Vg;
+        for (int v = threadIdx.x; v < Vg; v += blockDim.x) {
+            const float m = v < nf ? 1.0f : 0.0f;
+            o.node_mask[noff + v] = m; o.ro_mask[noff + v] = m;
+        }
+        for (int k = threadIdx.x; k < npad * T; k += blockDim.x) {
+            const size_t R = (size_t)(noff + Vg) * T + k;
+            o.row_ptr[R + 1] = soff + Mg;
+            o.indeg[R] = 0.0f;
+            if (o.trow) o.trow[R + 1] = soff + Mg;
+            if (o.pair) o.pair[R] = -1;
+        }
+        for (int v = Vg + threadIdx.x; v < o.v; v += blockDim.x) {
+            o.denom[noff + v] = 0.0f + 1e-7f;
+            o.ro_graph_of[noff + v] = i;
+            o.node_mask[noff + v] = 0.0f; o.ro_mask[noff + v] = 0.0f;
+        }
+        for (size_t k = threadIdx.x; k < (size_t)npad * D; k += blockDim.x) o.h0[(size_t)(noff + Vg) * D + k] = 0.0f;
+    }
     for (int t = threadIdx.x; t < a.tasks; t += blockDim.x) {
         o.tv[(size_t)t * o.G + i] = a.labels[(size_t)gid * a.tasks + t];
         o.tm[(size_t)t * o.G + i] = a.lmask[(size_t)gid * a.tasks + t];
@@ -142,7 +169,12 @@ __global__ void __launch_bounds__(256) ds_tile_kernel(const DsArrays a, const Ds
                     if (table[(size_t)mid * o.rec + R_NODE] <= n) lo = mid; else hi = mid - 1;
                 }
                 const int* r = table + (size_t)lo * o.rec;
-                v = r[R_VROW] + a.vpre[a.base[(size_t)r[R_GID] * B_WIDTH + B_NODE] + (n - r[R_NODE])];
+                const int* gb = a.base + (size_t)r[R_GID] * B_WIDTH;
+                const int local = n - r[R_NODE];
+                if (o.v > 0 && local >= gb[B_WIDTH + B_NODE] - gb[B_NODE])   // dense: a tile starting in the graph's padding rows
+                    v = r[R_VROW] + (gb[B_WIDTH + B_VROW] - gb[B_VROW]);
+                else
+                    v = r[R_VROW] + a.vpre[gb[B_NODE] + local];
             }
             o.tvp[i] = v;
         }

@@ -2823,6 +2823,7 @@ struct DsGraph {
 struct ggnn_dataset : ErrorText {
     ModelShape shape;
     bool train = false, stream_tables = false, weighted = false, on_device = false;
+    bool dense = false;   // ggnn_dataset_create_dense: batches of nodes_per_graph rows per graph (ggnn_dataset_prepare_batch_dense)
     int N = 0, ann = 0, tasks = 0;
     std::vector<DsGraph> graphs;
     std::vector<int> type_msgs;   // [N][T]
@@ -2838,6 +2839,7 @@ struct ggnn_dataset_batch : ErrorText {
     BatchPlan plan;
     size_t bytes = 0;
     int G = 0;
+    int v = 0;               // a dense batch's rows per graph; 0 for sparse and GCN batches
     StagedImage table;       // tile starts [ntiles + 1] | the per-graph records [G][R_MBASE + T] (16-byte aligned)
     size_t table_bytes = 0, off_records = 0;
     bool valid = false;
@@ -2845,7 +2847,7 @@ struct ggnn_dataset_batch : ErrorText {
 
 // The host arrays of a dataset before its upload, section by section (each 16-byte aligned in the one image).
 struct DsHost {
-    std::vector<int> base, row_end, src, pos, trow_end, ttgt, tslot, pair, vend, vsrc, vpre;
+    std::vector<int> base, row_end, src, pos, trow_end, ttgt, tslot, pair, vend, vsrc, vpre, nfeat;
     std::vector<float> indeg, denom, slotw, tslotw;
 };
 
@@ -2963,9 +2965,9 @@ static int ds_finish(ggnn_dataset* d, DsHost& h, const float* ann, const float* 
                             F(h.denom, &a.denom), I(h.trow_end, &a.trow_end), I(h.ttgt, &a.ttgt), I(h.tslot, &a.tslot), I(h.pair, &a.pair),
                             I(h.vend, &a.vend), I(h.vsrc, &a.vsrc), I(h.vpre, &a.vpre), F(h.slotw, &a.slotw), F(h.tslotw, &a.tslotw),
                             {ann, nann * sizeof(float), (const void**)&a.ann}, {labels, nlab * sizeof(float), (const void**)&a.labels},
-                            {lmask, nlab * sizeof(float), (const void**)&a.lmask}};
+                            {lmask, nlab * sizeof(float), (const void**)&a.lmask}, I(h.nfeat, &a.nfeat)};
     const bool present[] = {true, true, true, true, true, true, d->train, d->train, d->train && d->shape.use_att, d->stream_tables,
-                            d->stream_tables, d->stream_tables, d->stream_tables, d->weighted, d->weighted && d->train, true, true, true};
+                            d->stream_tables, d->stream_tables, d->stream_tables, d->weighted, d->weighted && d->train, true, true, true, d->dense};
     size_t total = 0;
     for (const Section& s : secs) total = align_up(total + s.bytes, 16);
     std::vector<char> image(total);
@@ -3078,6 +3080,64 @@ static int create_dataset_gcn(ggnn_dataset** out, const ggnn_engine* e, const Co
     return ds_finish(d, h, annotations, labels, lmask, stream);
 }
 
+// Dense graphs: the reference's raw (src, bond, dest) triples, int64 [sum E, 3] with graph offsets [N+1], and each graph's feature count.
+// Each triple sets A[bond-1, dest, src] and A[bond-1+bwd, src, dest] (dense:30-36, bwd = 0 tied, T/2 untied); as assignments, duplicates
+// collapse.  The graph's per-type lists are those entries in the order scan_dense emits them -- target row, then source column -- and
+// its in-degrees the number of distinct sources.  A graph spans V_g = max(features, largest id + 1) rows; annotations arrive for its
+// feature rows only and are stored for all V_g (zero beyond the features), so that the kernels read them like a sparse graph's.
+template <class Config>
+static int create_dataset_dense(ggnn_dataset** out, const ggnn_engine* e, const Config* cfg, int32_t num_sms, int32_t for_training, int32_t N,
+                                const int64_t* feature_counts, const int64_t* triples, const int64_t* graph_offsets, int32_t tie_fwd_bkwd,
+                                int32_t ann, const float* annotations, int32_t tasks, const float* labels, const float* lmask,
+                                cudaStream_t stream, const char* fn) {
+    if (int rc = begin_dataset(out, e, cfg, num_sms, for_training, N, feature_counts, ann, annotations, tasks, labels, lmask, fn)) return rc;
+    ggnn_dataset* d = *out;
+    d->dense = true;
+    if (d->shape.use_att) return d->fail(GGNN_EUNSUPPORTED, "propagation attention exists only in the sparse model (sparse:170-196)");
+    if (N > 0 && !graph_offsets) return d->fail(GGNN_EINVAL, "null graph offsets");
+    const int T = d->shape.T, bwd = tie_fwd_bkwd ? 0 : T / 2;
+    DsHost h;
+    std::vector<float> ann_rows;   // [sum V_g][ann]
+    std::vector<std::array<int, 3>> ent;   // (type, target, source)
+    std::vector<std::vector<int32_t>> lists(T);
+    std::vector<const int32_t*> adj(T);
+    std::vector<int32_t> ne(T);
+    int64_t feat_row = 0;
+    for (int i = 0; i < N; ++i) {
+        const int64_t e0 = graph_offsets[i], e1 = graph_offsets[i + 1];
+        if (e0 < 0 || e1 < e0 || (e1 > e0 && !triples)) return d->fail(GGNN_EINVAL, "graph %d: bad graph offsets", i);
+        int64_t Vg = feature_counts[i];
+        ent.clear();
+        for (int64_t k = e0; k < e1; ++k) {
+            const int64_t s = triples[3 * k], b = triples[3 * k + 1], t = triples[3 * k + 2];
+            if (s < 0 || t < 0 || s >= 0x7fffffff || t >= 0x7fffffff || b < 1 || b - 1 + bwd >= T)
+                return d->fail(GGNN_ERANGE, "graph %d: edge %lld = (%lld, %lld, %lld) is out of range (node ids >= 0, bond types 1..%d)", i,
+                               (long long)(k - e0), (long long)s, (long long)b, (long long)t, T - bwd);
+            ent.push_back({(int)(b - 1), (int)t, (int)s});
+            ent.push_back({(int)(b - 1 + bwd), (int)s, (int)t});
+            Vg = std::max(Vg, std::max(s, t) + 1);
+        }
+        std::sort(ent.begin(), ent.end());
+        ent.erase(std::unique(ent.begin(), ent.end()), ent.end());
+        for (int t = 0; t < T; ++t) lists[t].clear();
+        std::vector<float> indeg((size_t)Vg * T, 0.0f);
+        for (const auto& x : ent) {
+            lists[x[0]].push_back(x[2]);
+            lists[x[0]].push_back(x[1]);
+            indeg[(size_t)x[1] * T + x[0]] += 1.0f;
+        }
+        for (int t = 0; t < T; ++t) { adj[t] = lists[t].data(); ne[t] = (int32_t)(lists[t].size() / 2); }
+        if (int rc = ds_add_graph(d, h, i, (int)Vg, adj.data(), ne.data(), indeg.data(), nullptr)) return rc;
+        h.nfeat.push_back((int)feature_counts[i]);
+        if (ann > 0) {
+            ann_rows.insert(ann_rows.end(), annotations + feat_row * ann, annotations + (feat_row + feature_counts[i]) * ann);
+            ann_rows.resize(ann_rows.size() + (size_t)(Vg - feature_counts[i]) * ann, 0.0f);
+        }
+        feat_row += feature_counts[i];
+    }
+    return ds_finish(d, h, ann_rows.data(), labels, lmask, stream);
+}
+
 extern "C" {
 
 int ggnn_dataset_create_sparse(const ggnn_engine* e, int32_t for_training, int32_t num_graphs, const int64_t* node_counts,
@@ -3115,6 +3175,21 @@ int ggnn_host_dataset_create_gcn(const ggnn_gcn_config* cfg, int32_t num_sms, in
                               annotation_size, annotations, num_tasks, labels, label_mask, nullptr, __func__);
 }
 
+int ggnn_dataset_create_dense(const ggnn_engine* e, int32_t for_training, int32_t num_graphs, const int64_t* feature_counts, const int64_t* graphs,
+                              const int64_t* graph_offsets, int32_t tie_fwd_bkwd, int32_t annotation_size, const float* annotations,
+                              int32_t num_tasks, const float* labels, const float* label_mask, ggnn_stream_t stream, ggnn_dataset** out) {
+    if (!e) return GGNN_EINVAL;
+    return create_dataset_dense<ggnn_config>(out, e, nullptr, 0, for_training, num_graphs, feature_counts, graphs, graph_offsets, tie_fwd_bkwd,
+                                             annotation_size, annotations, num_tasks, labels, label_mask, (cudaStream_t)stream, __func__);
+}
+
+int ggnn_host_dataset_create_dense(const ggnn_config* cfg, int32_t num_sms, int32_t for_training, int32_t num_graphs, const int64_t* feature_counts,
+                                   const int64_t* graphs, const int64_t* graph_offsets, int32_t tie_fwd_bkwd, int32_t annotation_size,
+                                   const float* annotations, int32_t num_tasks, const float* labels, const float* label_mask, ggnn_dataset** out) {
+    return create_dataset_dense(out, nullptr, cfg, num_sms, for_training, num_graphs, feature_counts, graphs, graph_offsets, tie_fwd_bkwd,
+                                annotation_size, annotations, num_tasks, labels, label_mask, nullptr, __func__);
+}
+
 int ggnn_free_dataset(ggnn_dataset* d) {
     if (!d) return GGNN_OK;
     if (d->on_device) { cudaSetDevice(d->shape.device); d->buf.release(); }
@@ -3124,37 +3199,54 @@ int ggnn_free_dataset(ggnn_dataset* d) {
 
 const char* ggnn_dataset_error(const ggnn_dataset* d) { return d ? d->err.c_str() : "null dataset"; }
 
-int ggnn_dataset_prepare_batch(const ggnn_dataset* d, int32_t save_for_backward, const int64_t* graph_ids, int32_t num_graphs,
-                               ggnn_dataset_batch** inout) {
+}  // extern "C"
+
+// The host half of both batch kinds.  v = 0: a sparse or GCN batch, graphs end to end.  v > 0: a dense batch, graph i at node offset i*v
+// followed by its padding rows, each an isolated node -- a cut point after every one, as the host builder finds them.
+static int prepare_dataset_batch(const ggnn_dataset* d, int32_t save_for_backward, const int64_t* graph_ids, int32_t num_graphs, bool dense,
+                                 int v, ggnn_dataset_batch** inout) {
     if (!d || !inout || num_graphs < 0 || (num_graphs > 0 && !graph_ids)) return GGNN_EINVAL;
     ggnn_dataset_batch* b = *inout;
     if (!b) { b = new ggnn_dataset_batch(); *inout = b; }
     b->valid = false;
     b->ds = d;
     b->shape = d->shape;
+    b->v = dense ? v : 0;
     b->table.use_cuda = d->on_device;
+    if (d->dense != dense)
+        return b->fail(GGNN_EINVAL, d->dense ? "a dense dataset's batches are prepared with ggnn_dataset_prepare_batch_dense"
+                                             : "ggnn_dataset_prepare_batch_dense needs a dataset made by ggnn_dataset_create_dense");
+    if (dense && v <= 0) return b->fail(GGNN_EINVAL, "nodes_per_graph = %d", v);
+    v = b->v;
     const bool save = save_for_backward != 0;
     if (save && !d->train) return b->fail(GGNN_ESTATE, "save_for_backward needs a dataset created for training (the source-keyed CSR is built there)");
     const int T = d->shape.T, G = num_graphs;
     for (int i = 0; i < G; ++i)
         if (graph_ids[i] < 0 || graph_ids[i] >= d->N)
             return b->fail(GGNN_ERANGE, "graph_ids[%d] = %lld is out of range for a dataset of %d graphs", i, (long long)graph_ids[i], d->N);
-    // offsets and the cut points: every graph's segments, shifted by its node offset
+    for (int i = 0; i < G && v > 0; ++i)
+        if (d->graphs[graph_ids[i]].V > v)
+            return b->fail(GGNN_EINVAL, "graph_ids[%d] = %lld: graph of %d nodes does not fit nodes_per_graph = %d", i, (long long)graph_ids[i],
+                           d->graphs[graph_ids[i]].V, v);
+    // offsets and the cut points: every graph's segments, shifted by its node offset (dense: then one per padding row)
     int64_t V = 0, M = 0, nv = 0, nvm = 0;
     std::vector<int64_t> type_tot(T, 0);
     std::vector<int> cuts(1, 0);
     for (int i = 0; i < G; ++i) {
         const DsGraph& g = d->graphs[graph_ids[i]];
         for (int k = 0; k < g.nseg; ++k) cuts.push_back((int)(V + d->seg_end[g.seg0 + k]));
-        V += g.V; M += g.M; nv += g.nv; nvm += g.nvm;
+        for (int r = g.V + 1; r <= v; ++r) cuts.push_back((int)(V + r));
+        V += v > 0 ? v : g.V; M += g.M; nv += g.nv; nvm += g.nvm;
         for (int t = 0; t < T; ++t) type_tot[t] += d->type_msgs[(size_t)graph_ids[i] * T + t];
         if (M > 0x7fffffff || V * T + 1 > 0x7fffffff) return b->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
     }
     BatchPlan& p = b->plan;
     std::vector<int> tile_start;
     if (int rc = build_plan(d->shape, (int)V, d->weighted, cuts, p, tile_start, b->err)) return rc;
+    if (d->dense) p.plan_text += " [binary dense adjacency -> CSR]";
     b->bytes = layout_image(d->shape, p, save, M, (int)nv, nvm);
     if (p.local) {   // tiles of whole segments: their message counts and edge types from the segment summaries (only LOCAL launches read them)
+        // (a dense batch's padding rows are segments of no message and no edge type: a tile may end inside them)
         size_t tile = 1;
         int msgs = 0; unsigned mask = 0;
         int64_t node = 0;
@@ -3168,7 +3260,13 @@ int ggnn_dataset_prepare_batch(const ggnn_dataset* d, int32_t save_for_backward,
                     msgs = 0; mask = 0; ++tile;
                 }
             }
-            node += g.V;
+            for (int r = g.V + 1; r <= v; ++r)
+                if (node + r == tile_start[tile]) {
+                    p.max_tile_msgs = std::max(p.max_tile_msgs, msgs);
+                    p.max_tile_types = std::max(p.max_tile_types, __builtin_popcount(mask));
+                    msgs = 0; mask = 0; ++tile;
+                }
+            node += v > 0 ? v : g.V;
         }
     }
     // the batch table: tile starts, then per graph its id, offsets and per-type message bases (type base of the batch + earlier graphs')
@@ -3188,11 +3286,23 @@ int ggnn_dataset_prepare_batch(const ggnn_dataset* d, int32_t save_for_backward,
             r[ds::R_MBASE + t] = (int)mbase[t];
             mbase[t] += d->type_msgs[(size_t)graph_ids[i] * T + t];
         }
-        node += g.V; slot += g.M; vrow += g.nv; vs += g.nvm;
+        node += v > 0 ? v : g.V; slot += g.M; vrow += g.nv; vs += g.nvm;
     }
     b->G = G;
     b->valid = true;
     return GGNN_OK;
+}
+
+extern "C" {
+
+int ggnn_dataset_prepare_batch(const ggnn_dataset* d, int32_t save_for_backward, const int64_t* graph_ids, int32_t num_graphs,
+                               ggnn_dataset_batch** inout) {
+    return prepare_dataset_batch(d, save_for_backward, graph_ids, num_graphs, false, 0, inout);
+}
+
+int ggnn_dataset_prepare_batch_dense(const ggnn_dataset* d, int32_t save_for_backward, const int64_t* graph_ids, int32_t num_graphs,
+                                     int32_t nodes_per_graph, ggnn_dataset_batch** inout) {
+    return prepare_dataset_batch(d, save_for_backward, graph_ids, num_graphs, true, nodes_per_graph, inout);
 }
 
 int ggnn_dataset_batch_info(const ggnn_dataset_batch* b, int32_t* num_nodes, int64_t* num_messages, int32_t* num_tiles, int64_t* image_bytes,
@@ -3221,17 +3331,24 @@ int ggnn_free_dataset_batch(ggnn_dataset_batch* b) {
 
 const char* ggnn_dataset_batch_error(const ggnn_dataset_batch* b) { return b ? b->err.c_str() : "null dataset batch"; }
 
-int ggnn_set_graph_dataset(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, float* target_values, float* target_mask, ggnn_stream_t stream) {
+}  // extern "C"
+
+// The device half of both batch kinds: node_mask is the dense call's [V] output (null for the sparse call, which refuses a dense batch).
+static int set_graph_dataset(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, float* target_values, float* target_mask, bool dense,
+                             float* node_mask, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
     forget_batch(e);
     if (!b || !b->valid) return e->fail(GGNN_ESTATE, "the dataset batch is empty (its prepare failed or never ran)");
+    if ((b->v > 0) != dense)
+        return e->fail(GGNN_EINVAL, dense ? "ggnn_set_graph_dataset_dense needs a dense dataset batch" : "a dense dataset batch is adopted with ggnn_set_graph_dataset_dense");
     const ggnn_dataset* d = b->ds;
     if (!d->on_device) return e->fail(GGNN_EINVAL, "a host-only dataset has no device copy");
     if (int rc = check_batch_shape(e, b->shape, b->plan, "dataset")) return rc;
     if (b->shape.device != e->device)   // its arrays live in another GPU's memory
         return e->fail(GGNN_EINVAL, "the dataset was built for an engine on device %d, this engine is on device %d", b->shape.device, e->device);
     const BatchPlan& q = b->plan;
-    if ((q.V > 0 && !h0) || (d->tasks > 0 && b->G > 0 && (!target_values || !target_mask))) return e->fail(GGNN_EINVAL, "null output buffer");
+    if ((q.V > 0 && (!h0 || (dense && !node_mask))) || (d->tasks > 0 && b->G > 0 && (!target_values || !target_mask)))
+        return e->fail(GGNN_EINVAL, "null output buffer");
     CU_TRY(e, cudaSetDevice(e->device));
     cudaStream_t st = (cudaStream_t)stream;
     static_cast<BatchPlan&>(*e) = q;
@@ -3256,7 +3373,8 @@ int ggnn_set_graph_dataset(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, flo
     o.slotw = (float*)sec(q.off_slotw, q.weighted); o.tslotw = (float*)sec(q.off_tslotw, q.weighted && q.has_transpose);
     o.h0 = h0; o.tv = target_values; o.tm = target_mask;
     o.ro_graph_of = (int*)((char*)e->ro_buf.ptr + e->ro_off_graph_of); o.ro_start = (int*)((char*)e->ro_buf.ptr + e->ro_off_start);
-    o.V = q.V; o.D = e->D; o.T = e->T; o.G = b->G; o.ntiles = q.ntiles; o.nv = q.ts_nv; o.rec = ds::R_MBASE + e->T;
+    o.node_mask = node_mask; o.ro_mask = dense ? (float*)((char*)e->ro_buf.ptr + e->ro_off_mask) : nullptr;
+    o.V = q.V; o.D = e->D; o.T = e->T; o.G = b->G; o.ntiles = q.ntiles; o.nv = q.ts_nv; o.rec = ds::R_MBASE + e->T; o.v = b->v;
     const int* table = (const int*)((const char*)e->ds_table.ptr + b->off_records);
     if (b->G > 0) ds::ds_graph_kernel<<<b->G, 256, 0, st>>>(d->dev, o, table);
     const int tile_work = std::max(q.ntiles + 1, q.stream ? ts::TILE_M * e->T : 0);
@@ -3264,8 +3382,19 @@ int ggnn_set_graph_dataset(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, flo
         d->dev, o, table, (const int*)e->ds_table.ptr);
     CU_TRY(e, cudaGetLastError());
     if (int rc = bind_graph(e)) return rc;
-    e->ro_V = q.V; e->ro_G = b->G; e->ro_grouped = true; e->ro_has_mask = false;
+    e->ro_V = q.V; e->ro_G = b->G; e->ro_grouped = true; e->ro_has_mask = dense;
     return GGNN_OK;
+}
+
+extern "C" {
+
+int ggnn_set_graph_dataset(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, float* target_values, float* target_mask, ggnn_stream_t stream) {
+    return set_graph_dataset(e, b, h0, target_values, target_mask, false, nullptr, stream);
+}
+
+int ggnn_set_graph_dataset_dense(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, float* target_values, float* target_mask, float* node_mask,
+                                 ggnn_stream_t stream) {
+    return set_graph_dataset(e, b, h0, target_values, target_mask, true, node_mask, stream);
 }
 
 int ggnn_graph_image(ggnn_engine* e, void* dst, int64_t capacity, int64_t* image_bytes, ggnn_stream_t stream) {

@@ -10,7 +10,7 @@ from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
-from . import _lib
+from . import _lib, packing
 
 PRECISIONS = {"fp32": 0, "bf16x3": 1, "bf16": 2}
 BACKWARD_PRECISIONS = ("fp32", "bf16x3")   # ggnn_set_backward_precision
@@ -207,9 +207,10 @@ class PreparedGraph:
 
 class DeviceDataset:
     """Handle of a ``ggnn_dataset`` (include/ggnn_b200.h): a whole graph set on the GPU, from which every batch of whole graphs is assembled on
-    the device.  Built from a ``packing.FlatSparseGraphs`` (GGNN engines) or ``packing.FlatGCNGraphs`` (GCN engines), whose arrays it reads
-    as they are.  ``for_engine`` uploads it for an engine; ``host_only`` / ``host_only_gcn`` build the same host summaries without a GPU, so
-    that batch plans can be checked anywhere."""
+    the device.  Built from a ``packing.FlatSparseGraphs`` or ``packing.FlatDenseGraphs`` (GGNN engines) or ``packing.FlatGCNGraphs`` (GCN
+    engines), whose arrays it reads as they are.  ``for_engine`` uploads it for an engine; ``host_only`` / ``host_only_dense`` /
+    ``host_only_gcn`` build the same host summaries without a GPU, so that batch plans can be checked anywhere.  A dense dataset's batches
+    have ``nodes_per_graph`` rows per graph, as the dense model's bucketed batches."""
 
     def __init__(self, lib=None):
         self.lib = lib or _lib.load()
@@ -247,6 +248,7 @@ class DeviceDataset:
             raise err
         self.num_tasks = labels.shape[1]
         self.num_graphs = int(flat.num_graphs)
+        self.dense = isinstance(flat, packing.FlatDenseGraphs)
         return self
 
     @classmethod
@@ -262,10 +264,29 @@ class DeviceDataset:
             off = np.ascontiguousarray(flat.entry_off, np.int64)
             keep += [lst, w, off]
             return d._create(d.lib.ggnn_dataset_create_gcn, flat, head, (lst.ctypes.data, off.ctypes.data, w.ctypes.data), keep)
+        if isinstance(flat, packing.FlatDenseGraphs):
+            tri, off = cls._dense_arrays(flat)
+            keep += [tri, off]
+            return d._create(d.lib.ggnn_dataset_create_dense, flat, head, (tri.ctypes.data, off.ctypes.data, int(flat.tie_fwd_bkwd)), keep)
         edges, offsets, indeg = cls._sparse_arrays(flat, engine.T)
         keep += [edges, offsets, indeg]
         ptrs = (C.c_void_p * max(engine.T, 1))(*[e.ctypes.data for e in edges])
         return d._create(d.lib.ggnn_dataset_create_sparse, flat, head, (ptrs, offsets.ctypes.data, indeg.ctypes.data), keep)
+
+    @staticmethod
+    def _dense_arrays(flat):
+        return (np.ascontiguousarray(flat.triples, np.int64).reshape(-1, 3), np.ascontiguousarray(flat.edge_off, np.int64))
+
+    @classmethod
+    def host_only_dense(cls, params: dict, num_edge_types: int, flat, precision: str = "fp32", num_sms: int = 132,
+                        for_training: bool = True) -> "DeviceDataset":
+        """``ggnn_host_dataset_create_dense``: the dense dataset's host summaries (from a ``packing.FlatDenseGraphs``), no engine, no GPU."""
+        d = cls()
+        cfg, keep = make_config(params, num_edge_types, 0, precision)
+        tri, off = cls._dense_arrays(flat)
+        head = ((C.byref(cfg), int(num_sms), int(bool(for_training))), ())
+        return d._create(d.lib.ggnn_host_dataset_create_dense, flat, head, (tri.ctypes.data, off.ctypes.data, int(flat.tie_fwd_bkwd)),
+                         [keep, tri, off])
 
     @classmethod
     def host_only(cls, params: dict, num_edge_types: int, flat, precision: str = "fp32", num_sms: int = 132,
@@ -290,13 +311,19 @@ class DeviceDataset:
         head = ((C.byref(cfg), int(num_sms), int(bool(for_training))), ())
         return d._create(d.lib.ggnn_host_dataset_create_gcn, flat, head, (lst.ctypes.data, off.ctypes.data, w.ctypes.data), [lst, w, off])
 
-    def prepare_batch(self, ids, save_for_backward: bool = True, reuse: Optional["DatasetBatch"] = None) -> "DatasetBatch":
+    def prepare_batch(self, ids, save_for_backward: bool = True, reuse: Optional["DatasetBatch"] = None,
+                      nodes_per_graph: Optional[int] = None) -> "DatasetBatch":
         """The HOST half of a batch of the graphs ``ids`` (dataset indices, in batch order): offsets, tile plan, image layout and a pinned
-        table of per-graph offsets, from the dataset's summaries alone -- may run in a producer thread.  ``reuse`` rebuilds a batch in place."""
+        table of per-graph offsets, from the dataset's summaries alone -- may run in a producer thread.  ``reuse`` rebuilds a batch in place.
+        A dense dataset's batch needs ``nodes_per_graph`` (the bucket size v: graph i owns rows i*v .. i*v+v-1); other datasets take none."""
         ids = np.ascontiguousarray(np.asarray(ids, dtype=np.int64).reshape(-1))
         b = reuse if reuse is not None else DatasetBatch(self)
         h = C.c_void_p(b._h.value)
-        rc = self.lib.ggnn_dataset_prepare_batch(self._h, int(bool(save_for_backward)), ids.ctypes.data, ids.shape[0], C.byref(h))
+        if nodes_per_graph is not None or self.dense:
+            rc = self.lib.ggnn_dataset_prepare_batch_dense(self._h, int(bool(save_for_backward)), ids.ctypes.data, ids.shape[0],
+                                                           int(nodes_per_graph or 0), C.byref(h))
+        else:
+            rc = self.lib.ggnn_dataset_prepare_batch(self._h, int(bool(save_for_backward)), ids.ctypes.data, ids.shape[0], C.byref(h))
         b._h = h
         if rc != 0:
             err = GgnnError(self.lib.ggnn_dataset_batch_error(h).decode() if h.value else "invalid argument")
@@ -304,6 +331,7 @@ class DeviceDataset:
             raise err
         b.dataset, b.G = self, ids.shape[0]
         b.V = b.info()["num_nodes"]
+        b.nodes_per_graph = int(nodes_per_graph) if self.dense else 0
         return b
 
     def close(self):
@@ -325,7 +353,7 @@ class DatasetBatch:
         self.lib = dataset.lib
         self.dataset = dataset   # the dataset must outlive its batches
         self._h = C.c_void_p()
-        self.V = self.G = 0
+        self.V = self.G = self.nodes_per_graph = 0
 
     def info(self) -> dict:
         V, M, nt, nb, st = C.c_int32(), C.c_int64(), C.c_int32(), C.c_int64(), C.c_int32()
@@ -472,21 +500,26 @@ class PropagationEngine:
 
     def set_graph_from_dataset(self, batch: "DatasetBatch"):
         """The DEVICE half of a dataset batch: adopts its plan and assembles its graph image, h0, targets and readout map on the engine's
-        stream.  Returns ``(h0 [V, D], target_values [tasks, G], target_mask [tasks, G])`` as CUDA tensors; the readout map is set (no
-        ``readout_set_graphs`` needed).  Keep ``batch`` alive until the stream has passed it."""
+        stream.  Returns ``(h0 [V, D], target_values [tasks, G], target_mask [tasks, G])`` as CUDA tensors, and for a dense batch also its
+        ``node_mask [G, nodes_per_graph]``; the readout map (with a dense batch's mask) is set (no ``readout_set_graphs`` needed).  Keep
+        ``batch`` alive until the stream has passed it."""
         import torch
         dev = "cuda:%d" % self.device
         h0 = torch.empty(batch.V, self.D, dtype=torch.float32, device=dev)
         tv = torch.empty(batch.dataset.num_tasks, batch.G, dtype=torch.float32, device=dev)
         tm = torch.empty_like(tv)
+        ptr = lambda t: t.data_ptr() if t.numel() else None
         self.serial += 1
-        self._check(self.lib.ggnn_set_graph_dataset(self._h, batch._h, h0.data_ptr() if h0.numel() else None, tv.data_ptr() if tv.numel() else None,
-                                                    tm.data_ptr() if tm.numel() else None, self._stream()))
+        if batch.dataset.dense:
+            mask = torch.empty(batch.G, batch.nodes_per_graph, dtype=torch.float32, device=dev)
+            self._check(self.lib.ggnn_set_graph_dataset_dense(self._h, batch._h, ptr(h0), ptr(tv), ptr(tm), ptr(mask), self._stream()))
+        else:
+            self._check(self.lib.ggnn_set_graph_dataset(self._h, batch._h, ptr(h0), ptr(tv), ptr(tm), self._stream()))
         self.V = batch.V
         self._graph_keepalive = (batch,)
         self._readout_keepalive = None
         self._readout_shape = (batch.V, batch.G)
-        return h0, tv, tm
+        return (h0, tv, tm, mask) if batch.dataset.dense else (h0, tv, tm)
 
     def graph_image(self) -> np.ndarray:
         """The engine's current graph image copied back (``ggnn_graph_image``): the bytes ``PreparedGraph.image`` holds for the same batch."""

@@ -253,6 +253,37 @@ def pack_dense_batch(raw_graphs: Sequence[dict], bucket_size: int, hidden_size: 
             "target_mask": np.asarray(tm, np.float32).T.reshape(-1, b)}
 
 
+class FlatDenseGraphs:
+    """The dense plug-in's processed graphs (raw molecule dicts, ``DenseGGNNChemModel.process_raw_graphs``) flattened ONCE for a
+    device-resident dataset (``engine.DeviceDataset``): ``n_nodes`` the node_features rows of every graph (its node mask's extent; edges may
+    name nodes beyond it), ``triples`` the raw ``(src, bond, dest)`` rows ``[sum E, 3]`` int64 with ``edge_off`` ``[N+1]``, ``feat`` the
+    node features ``[sum n_nodes, ann]``, and per task of ``task_ids`` the label and its mask ``[N, tasks]`` -- a ``None`` target (dropped
+    by ``task_sample_ratios``, dense:153-158) has mask 0, as ``pack_dense_batch`` gives it."""
+
+    def __init__(self, graphs: Sequence[dict], task_ids=(0,), tie_fwd_bkwd: bool = True):
+        N = len(graphs)
+        self.num_graphs, self.tie_fwd_bkwd = N, bool(tie_fwd_bkwd)
+        edges = [np.asarray(d["graph"], dtype=np.int64).reshape(-1, 3) for d in graphs]
+        self.edge_off = np.concatenate([[0], np.cumsum([e.shape[0] for e in edges])]).astype(np.int64)
+        self.triples = np.concatenate(edges, axis=0) if N else np.zeros((0, 3), np.int64)
+        feats = [np.asarray(d["node_features"], dtype=np.float32) for d in graphs]
+        self.n_nodes = np.fromiter((f.shape[0] for f in feats), dtype=np.int64, count=N)
+        self.ann = max((f.shape[1] for f in feats if f.ndim == 2), default=0)
+        self.feat = np.zeros((int(self.n_nodes.sum()), self.ann), np.float32)
+        self.labels = np.zeros((N, len(task_ids)), np.float32)
+        self.mask = np.zeros((N, len(task_ids)), np.float32)
+        o = 0
+        for i, (d, f) in enumerate(zip(graphs, feats)):
+            if f.size:
+                self.feat[o:o + f.shape[0], :f.shape[1]] = f
+            o += f.shape[0]
+            for k, t in enumerate(task_ids):
+                v = d["targets"][t][0]
+                if v is not None:
+                    self.labels[i, k] = v
+                    self.mask[i, k] = 1.0
+
+
 def choose_bucket(graph, bucket_sizes=DEFAULT_BUCKET_SIZES) -> int:
     """dense:138-140 -- first bucket strictly larger than the largest node id."""
     g = np.asarray(graph).reshape(-1, 3)

@@ -345,7 +345,18 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
  * CSR that batches with save_for_backward need.  The source arrays stay the caller's; the dataset owns its device memory (an allocation
  * failure returns GGNN_ECUDA naming the size).  *out is allocated even when the call fails: read ggnn_dataset_error, then free it.  The
  * ggnn_host_* twins build the same host summaries without an engine or a GPU (for a host of num_sms SMs): their batches can be planned
- * and inspected, not adopted. */
+ * and inspected, not adopted.
+ *   ggnn_dataset_create_dense    GGNN engine, the dense model's graphs (dense:30-36, 132-164).  feature_counts [N] (rows of node_features);
+ *                                graphs [sum E, 3] int64, the reference's raw (src, bond, dest) triples with graph_offsets [N+1]
+ *                                (graph i's rows graph_offsets[i] .. graph_offsets[i+1]); tie_fwd_bkwd as the model's parameter (0: the
+ *                                reverse direction is type bond-1 + T/2); annotations [sum features, annotation_size]; labels / label_mask
+ *                                as above.  Every triple is the two 0/1 entries A[bond-1, dest, src] and A[bond-1+bwd, src, dest]:
+ *                                duplicates collapse, a self-loop is one entry, the in-degree is the number of distinct sources, and each
+ *                                type's messages are in the order ggnn_prepare_graph_dense scans the matrix (target row, source column).
+ *                                A graph spans V_g = max(features, largest id + 1) nodes, stored unpadded; rows at or beyond its feature
+ *                                count are masked out (node_mask 0, h0 zero) but still send and receive messages.  A bond type outside
+ *                                1 .. T - bwd or a negative id is GGNN_ERANGE naming the graph and the edge; an attention model is
+ *                                GGNN_EUNSUPPORTED (the dense model has none). */
 typedef struct ggnn_dataset ggnn_dataset;
 int ggnn_dataset_create_sparse(const ggnn_engine* e, int32_t for_training, int32_t num_graphs, const int64_t* node_counts,
                                const int32_t* const* edge_lists, const int64_t* edge_offsets, const float* num_incoming_edges_per_type,
@@ -381,7 +392,16 @@ const char* ggnn_dataset_error(const ggnn_dataset* d);
  *                                on another device is refused (GGNN_EINVAL; another model: GGNN_ESTATE).
  * A batch reads its dataset in every call: the dataset must outlive every batch prepared from it (free the batches first).
  * ggnn_dataset_batch_info: as ggnn_prepared_graph_info, plus the tile starts [num_tiles + 1] and, for LOCAL (tile-local) plans, the values of
- * ggnn_prepared_graph_tile_stats -- other plans' launches do not read them, and they are 0 there.  NULL pointers are skipped. */
+ * ggnn_prepared_graph_tile_stats -- other plans' launches do not read them, and they are 0 there.  NULL pointers are skipped.
+ *
+ * Dense datasets have their own pair of calls; each kind refuses the other's dataset or batch with GGNN_EINVAL:
+ *   ggnn_dataset_prepare_batch_dense   the batch ggnn_prepare_graph_dense builds from pack_dense_batch's [b, T, v, v] matrix, with
+ *                                      v = nodes_per_graph: graph i owns rows i*v .. i*v+v-1, its V_g rows first, then v - V_g isolated
+ *                                      padding rows.  A graph with V_g > v is GGNN_EINVAL naming it.  Plan text, tile starts, layout and
+ *                                      image are those of the host-built batch, the plan text ending in " [binary dense adjacency -> CSR]".
+ *   ggnn_set_graph_dataset_dense       as ggnn_set_graph_dataset, plus node_mask [V = b*v] (DEVICE, the caller's): 1 for the rows below
+ *                                      the graph's feature count, 0 elsewhere.  The readout map is that of ggnn_readout_set_graphs(b,
+ *                                      nodes_per_graph = v, node_mask): the fused readout sums each graph's masked rows. */
 typedef struct ggnn_dataset_batch ggnn_dataset_batch;
 int ggnn_dataset_prepare_batch(const ggnn_dataset* d, int32_t save_for_backward, const int64_t* graph_ids, int32_t num_graphs,
                                ggnn_dataset_batch** inout);
@@ -391,6 +411,16 @@ int ggnn_dataset_batch_info(const ggnn_dataset_batch* b, int32_t* num_nodes, int
 int ggnn_free_dataset_batch(ggnn_dataset_batch* b);
 const char* ggnn_dataset_batch_error(const ggnn_dataset_batch* b);
 int ggnn_set_graph_dataset(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, float* target_values, float* target_mask, ggnn_stream_t stream);
+int ggnn_dataset_create_dense(const ggnn_engine* e, int32_t for_training, int32_t num_graphs, const int64_t* feature_counts, const int64_t* graphs,
+                              const int64_t* graph_offsets, int32_t tie_fwd_bkwd, int32_t annotation_size, const float* annotations,
+                              int32_t num_tasks, const float* labels, const float* label_mask, ggnn_stream_t stream, ggnn_dataset** out);
+int ggnn_host_dataset_create_dense(const ggnn_config* cfg, int32_t num_sms, int32_t for_training, int32_t num_graphs, const int64_t* feature_counts,
+                                   const int64_t* graphs, const int64_t* graph_offsets, int32_t tie_fwd_bkwd, int32_t annotation_size,
+                                   const float* annotations, int32_t num_tasks, const float* labels, const float* label_mask, ggnn_dataset** out);
+int ggnn_dataset_prepare_batch_dense(const ggnn_dataset* d, int32_t save_for_backward, const int64_t* graph_ids, int32_t num_graphs,
+                                     int32_t nodes_per_graph, ggnn_dataset_batch** inout);
+int ggnn_set_graph_dataset_dense(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, float* target_values, float* target_mask, float* node_mask,
+                                 ggnn_stream_t stream);
 /* The engine's current graph image copied back to the host (the counterpart of ggnn_prepared_graph_image, whatever upload made it):
  * *image_bytes gets its size; dst NULL only asks for it.  Synchronises `stream`. */
 int ggnn_graph_image(ggnn_engine* e, void* dst, int64_t capacity, int64_t* image_bytes, ggnn_stream_t stream);

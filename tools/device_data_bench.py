@@ -1,9 +1,10 @@
-"""Host-packed batches against device-resident datasets (``--device-data``) in the two node-budget plug-ins, in one process.
+"""Host-packed batches against device-resident datasets (``--device-data``) in the three plug-ins, in one process.
 
-    python tools/device_data_bench.py [--molecules N] [--reps R] [--out FILE]
+    python tools/device_data_bench.py [--molecules N] [--reps R] [--models ggnn,gcn,dense] [--out FILE]
 
 For SparseGGNNChemModel and SparseGCNChemModel (bf16x3, the reference's default shapes), at a batch of about 256 molecules and at the
-reference's 100 000-node batch, the two paths are measured alternately, R times each, and the medians printed as one JSON line:
+reference's 100 000-node batch, and for DenseGGNNChemModel (bf16x3) at BASELINE cfg3's 64-graph batch and the reference's default of 256
+graphs per bucketed batch, the two paths are measured alternately, R times each, and the medians printed as one JSON line:
   producer_ms_per_batch  host time of the batch producer (make_minibatch_iterator) per batch, the dataset upload excluded (done once before)
   step_ms                one training step on the consumer thread (forward_batch + train_step) between CUDA events
   instances_per_s        run_epoch (training) over the whole synthetic set, the producer thread overlapping the GPU as in training
@@ -34,12 +35,13 @@ def gpu_info() -> dict:
         return {"gpu": torch.cuda.get_device_name(0), "power_limit": "unknown (%s)" % ex}
 
 
-def make_model(kind: str, mols, batch_nodes: int, device_data: bool):
+def make_model(kind: str, mols, batch_size: int, device_data: bool):
+    from gated_graph_neural_network_samples_b200.chem_dense import DenseGGNNChemModel
     from gated_graph_neural_network_samples_b200.chem_gcn import SparseGCNChemModel
     from gated_graph_neural_network_samples_b200.chem_sparse import SparseGGNNChemModel
-    model = {"ggnn": SparseGGNNChemModel, "gcn": SparseGCNChemModel}[kind]
+    model = {"ggnn": SparseGGNNChemModel, "gcn": SparseGCNChemModel, "dense": DenseGGNNChemModel}[kind]
     args = {"--log_dir": "/tmp/device_data_bench", "--train_data": mols, "--valid_data": mols[:64], "--precision": "bf16x3",
-            "--config": {"batch_size": batch_nodes, "random_seed": 0}}
+            "--config": {"batch_size": batch_size, "random_seed": 0}}
     if device_data:
         args["--device-data"] = True
     return model(args)
@@ -77,6 +79,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--molecules", type=int, default=60000, help="synthetic training molecules (~18 nodes each)")
     ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--models", default="ggnn,gcn,dense", help="comma-separated subset of ggnn, gcn, dense")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     import torch
@@ -86,9 +89,12 @@ def main():
     mols = synthetic.make_molecules(a.molecules, seed=0)
     mean_nodes = float(np.mean([len(m["node_features"]) for m in mols]))
     result = {"bench": "device_data", "molecules": a.molecules, **gpu_info(), "rows": []}
-    for kind in ("ggnn", "gcn"):
-        for label, batch_nodes in (("256 molecules", int(256 * mean_nodes)), ("100000 nodes", 100000)):
-            models = {dd: make_model(kind, mols, batch_nodes, dd) for dd in (False, True)}
+    sizes = {"ggnn": (("256 molecules", int(256 * mean_nodes)), ("100000 nodes", 100000)),   # batch_size: a node budget
+             "gcn": (("256 molecules", int(256 * mean_nodes)), ("100000 nodes", 100000)),
+             "dense": (("64 graphs", 64), ("256 graphs", 256))}                            # batch_size: graphs per bucketed batch
+    for kind in a.models.split(","):
+        for label, batch_size in sizes[kind]:
+            models = {dd: make_model(kind, mols, batch_size, dd) for dd in (False, True)}
             for m in models.values():   # warm-up: flattening, the dataset upload, kernel first launches
                 m.run_epoch("warm-up", m.train_data, True)
             samples = {dd: {"producer_ms_per_batch": [], "step_ms": [], "instances_per_s": []} for dd in models}
@@ -98,7 +104,7 @@ def main():
                     samples[dd]["step_ms"].append(step_ms(m))
                     samples[dd]["instances_per_s"].append(m.run_epoch("bench", m.train_data, True)[3])
             for dd in models:
-                result["rows"].append({"model": kind, "batch": label, "batch_size_nodes": batch_nodes,
+                result["rows"].append({"model": kind, "batch": label, "batch_size": batch_size,
                                        "path": "device-data" if dd else "host-packed",
                                        **{k: round(statistics.median(v), 3) for k, v in samples[dd].items()}})
             del models
