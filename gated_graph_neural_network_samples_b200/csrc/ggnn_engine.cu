@@ -2453,6 +2453,12 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
     if (!e->graph_set) return no_graph(e);
     if ((!h0 || !h_out) && e->V > 0) return e->fail(GGNN_EINVAL, "null state pointer");
     if (((uintptr_t)h0 & 15) || ((uintptr_t)h_out & 15)) return e->fail(GGNN_EINVAL, "state pointers must be 16-byte aligned");
+    // In place is refused: the GLOBAL launches gather h0 rows that other CTAs of the same launch overwrite, and the backward reads h0 as
+    // node_states_per_layer[0] after the forward.
+    const uintptr_t vd_bytes = (uintptr_t)e->V * e->D * sizeof(float), a = (uintptr_t)h0, b = (uintptr_t)h_out;
+    if (vd_bytes > 0 && a < b + vd_bytes && b < a + vd_bytes)
+        return e->fail(GGNN_EINVAL, "h_out (%p) overlaps h0 (%p) over their %zu bytes: the forward does not run in place", (const void*)h_out,
+                       (const void*)h0, (size_t)vd_bytes);
     CU_TRY(e, cudaSetDevice(e->device));
     cudaStream_t st = (cudaStream_t)stream;
     e->last_launches = 0;
@@ -2465,7 +2471,7 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
     if (e->V == 0) return done(true, e->save);   // the backward of an empty batch has nothing to compute either
     if (e->save) { int rc = reserve_states(e); if (rc) return rc; }
     if (!gcn && e->total_steps == 0) {  // no propagation at all: result is the input (sparse:152 with empty loops)
-        if (h_out != h0) CU_TRY(e, cudaMemcpyAsync(h_out, h0, (size_t)e->V * e->D * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        CU_TRY(e, cudaMemcpyAsync(h_out, h0, (size_t)e->V * e->D * sizeof(float), cudaMemcpyDeviceToDevice, st));
         return done(false, false);
     }
     int rc;

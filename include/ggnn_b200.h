@@ -171,7 +171,11 @@ int ggnn_set_graph_dense(ggnn_engine* e, int32_t num_graphs, int32_t num_vertice
                          const float* adjacency_matrix, ggnn_stream_t stream);
 
 /* compute_final_node_representations (sparse:117-218 / dense:93-117).
- * h0, h_out: DEVICE [V, D] fp32 (dense: [b*v, D]).  Asynchronous on `stream`. */
+ * h0, h_out: DEVICE [V, D] fp32 (dense: [b*v, D]).  Asynchronous on `stream`.
+ * Aliasing: the V*D floats at h_out must not overlap those at h0, on any model and plan (the GLOBAL launches gather h0 rows that other
+ * blocks overwrite, and the backward reads h0 again); an overlap returns GGNN_EINVAL naming both pointers, before any launch and with the
+ * engine's state untouched.  ggnn_backward / ggnn_gcn_backward and ggnn_layer_state read h0 and h_out of the last forward again (they are
+ * node_states_per_layer[0] and [L]): both must stay unchanged until the backward has run. */
 int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t stream);
 
 /* Same with HOST buffers: H2D copy of h0, propagation, D2H copy of the result, stream-synchronised. */
@@ -238,7 +242,8 @@ int ggnn_state_dropout_mask(int32_t V, int32_t D, int32_t global_step, float kee
 
 /* Gradient of the propagation (what optimizer.compute_gradients builds, chem_tensorflow.py:184).
  * Must follow a ggnn_forward on the same graph with save_for_backward enabled.
- * d_h_out: DEVICE [V, D]; grads: per layer, accumulated into; d_h0: DEVICE [V, D] or NULL. */
+ * d_h_out: DEVICE [V, D]; grads: per layer, accumulated into; d_h0: DEVICE [V, D] or NULL.  d_h0 may be d_h_out or overlap it (here and
+ * in ggnn_gcn_backward): d_h_out is read in full before d_h0 is written, so the result is the out-of-place one, bit for bit. */
 int ggnn_set_save_for_backward(ggnn_engine* e, int32_t enable);
 /* Deterministic mode (off by default; GGNN and GCN engines; takes effect from the next call).  With it on, the same engine configuration,
  * batch, weights, dropout seed and caller buffer contents produce identical bits in every output and every accumulated gradient buffer,
