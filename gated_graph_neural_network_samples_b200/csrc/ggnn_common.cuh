@@ -26,6 +26,19 @@ struct LayerDev {
     int res[MAX_RES];      // indices into node_states_per_layer
 };
 
+// The sections of a batch's graph image as typed pointers into one copy of it: the host image the builder fills, the device image the
+// engine reads, or the device image the dataset kernels write.  The engine's image_view() makes it from the plan's layout; a section the
+// plan does not carry is null.
+struct ImageView {
+    int *row_ptr, *src, *msg;                  // target CSR: rows target*T+type, the source and message id of every slot
+    float *indeg, *denom;
+    int* tile_start;
+    unsigned* tile_mask;
+    int *trow, *ttgt, *tslot;                  // source-keyed CSR (save_for_backward); tslot: attention only
+    int *pair, *vptr, *vsrc, *tvp, *vinfo;     // streaming plan
+    float *slotw, *tslotw;                     // weighted batches: per-slot weights in target-CSR / source-CSR order
+};
+
 // Per-(layer,step) activations kept for the backward pass; each [V][D] (device), index = global step.
 struct SaveDev {
     float* h_in;   // state entering the step

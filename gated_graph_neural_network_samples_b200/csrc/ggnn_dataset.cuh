@@ -52,13 +52,7 @@ struct DsArrays {
 
 // The batch's outputs: the sections of the graph image (null when the plan has none) and the caller's / the readout's buffers.
 struct DsOut {
-    int *row_ptr, *src, *msg;
-    float *indeg, *denom;
-    int* tile_start;
-    unsigned* tile_mask;
-    int *trow, *ttgt, *tslot;
-    int *pair, *vptr, *vsrc, *tvp, *vinfo;
-    float *slotw, *tslotw;
+    ImageView img;
     float* h0;               // [V][D]
     float *tv, *tm;          // [tasks][G]
     int *ro_graph_of, *ro_start;
@@ -79,37 +73,37 @@ __global__ void __launch_bounds__(256) ds_graph_kernel(const DsArrays a, const D
         const size_t dk = (size_t)nb * T + k, R = (size_t)noff * T + k;
         const int lo = k ? a.row_end[dk - 1] : 0, hi = a.row_end[dk];
         const int mb = r[R_MBASE + k % T];
-        o.row_ptr[R + 1] = soff + hi;
+        o.img.row_ptr[R + 1] = soff + hi;
         for (int m = lo; m < hi; ++m) {
-            o.src[soff + m] = a.src[sb + m] + noff;
-            o.msg[soff + m] = mb + a.pos[sb + m];
-            if (o.slotw) o.slotw[soff + m] = a.slotw[sb + m];
+            o.img.src[soff + m] = a.src[sb + m] + noff;
+            o.img.msg[soff + m] = mb + a.pos[sb + m];
+            if (o.img.slotw) o.img.slotw[soff + m] = a.slotw[sb + m];
         }
-        o.indeg[R] = a.indeg[dk];
-        if (o.trow) {
+        o.img.indeg[R] = a.indeg[dk];
+        if (o.img.trow) {
             const int tlo = k ? a.trow_end[dk - 1] : 0, thi = a.trow_end[dk];
-            o.trow[R + 1] = soff + thi;
+            o.img.trow[R + 1] = soff + thi;
             for (int m = tlo; m < thi; ++m) {
-                o.ttgt[soff + m] = a.ttgt[sb + m] + noff;
-                if (o.tslot) o.tslot[soff + m] = a.tslot[sb + m] + soff;
-                if (o.tslotw) o.tslotw[soff + m] = a.tslotw[sb + m];
+                o.img.ttgt[soff + m] = a.ttgt[sb + m] + noff;
+                if (o.img.tslot) o.img.tslot[soff + m] = a.tslot[sb + m] + soff;
+                if (o.img.tslotw) o.img.tslotw[soff + m] = a.tslotw[sb + m];
             }
         }
-        if (o.pair) {
+        if (o.img.pair) {
             const int p = a.pair[dk];
-            o.pair[R] = p == -1 ? -1 : (p >= 0 ? p + noff : p - voff);   // -(2 + vid) - voff = -(2 + vid + voff)
+            o.img.pair[R] = p == -1 ? -1 : (p >= 0 ? p + noff : p - voff);   // -(2 + vid) - voff = -(2 + vid + voff)
         }
     }
-    if (o.pair)
+    if (o.img.pair)
         for (int j = threadIdx.x; j < nvg; j += blockDim.x) {
             const int lo = j ? a.vend[vb + j - 1] : 0, hi = a.vend[vb + j], cnt = hi - lo, vid = voff + j;
-            o.vptr[vid + 1] = vsoff + hi;
-            o.vinfo[8 * vid] = cnt;
-            for (int m = 0; m < 7; ++m) o.vinfo[8 * vid + 1 + m] = m < cnt ? a.vsrc[vsb + lo + m] + noff : 0;
-            for (int m = 0; m < cnt; ++m) o.vsrc[vsoff + lo + m] = a.vsrc[vsb + lo + m] + noff;
+            o.img.vptr[vid + 1] = vsoff + hi;
+            o.img.vinfo[8 * vid] = cnt;
+            for (int m = 0; m < 7; ++m) o.img.vinfo[8 * vid + 1 + m] = m < cnt ? a.vsrc[vsb + lo + m] + noff : 0;
+            for (int m = 0; m < cnt; ++m) o.img.vsrc[vsoff + lo + m] = a.vsrc[vsb + lo + m] + noff;
         }
     for (int v = threadIdx.x; v < Vg; v += blockDim.x) {
-        o.denom[noff + v] = a.denom[nb + v];
+        o.img.denom[noff + v] = a.denom[nb + v];
         o.ro_graph_of[noff + v] = i;
     }
     const int D = o.D, A = a.ann_size;
@@ -125,13 +119,13 @@ __global__ void __launch_bounds__(256) ds_graph_kernel(const DsArrays a, const D
         }
         for (int k = threadIdx.x; k < npad * T; k += blockDim.x) {
             const size_t R = (size_t)(noff + Vg) * T + k;
-            o.row_ptr[R + 1] = soff + Mg;
-            o.indeg[R] = 0.0f;
-            if (o.trow) o.trow[R + 1] = soff + Mg;
-            if (o.pair) o.pair[R] = -1;
+            o.img.row_ptr[R + 1] = soff + Mg;
+            o.img.indeg[R] = 0.0f;
+            if (o.img.trow) o.img.trow[R + 1] = soff + Mg;
+            if (o.img.pair) o.img.pair[R] = -1;
         }
         for (int v = Vg + threadIdx.x; v < o.v; v += blockDim.x) {
-            o.denom[noff + v] = 0.0f + 1e-7f;
+            o.img.denom[noff + v] = 0.0f + 1e-7f;
             o.ro_graph_of[noff + v] = i;
             o.node_mask[noff + v] = 0.0f; o.ro_mask[noff + v] = 0.0f;
         }
@@ -154,13 +148,13 @@ __global__ void __launch_bounds__(256) ds_tile_kernel(const DsArrays a, const Ds
     const size_t stride = (size_t)gridDim.x * blockDim.x, tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     for (size_t i = tid; i <= (size_t)o.ntiles; i += stride) {
         const int n = tiles[i];
-        o.tile_start[i] = n;
+        o.img.tile_start[i] = n;
         if (i < (size_t)o.ntiles) {
             unsigned mask = 0;
-            for (size_t k = (size_t)n * T, kend = (size_t)tiles[i + 1] * T; k < kend; ++k) mask |= (unsigned)(o.row_ptr[k + 1] > o.row_ptr[k]) << (k % T);
-            o.tile_mask[i] = mask;
+            for (size_t k = (size_t)n * T, kend = (size_t)tiles[i + 1] * T; k < kend; ++k) mask |= (unsigned)(o.img.row_ptr[k + 1] > o.img.row_ptr[k]) << (k % T);
+            o.img.tile_mask[i] = mask;
         }
-        if (o.pair) {   // virtual rows before node n: those of the graph holding n (the last graph starting at or before n) before it
+        if (o.img.pair) {   // virtual rows before node n: those of the graph holding n (the last graph starting at or before n) before it
             int v = o.nv;
             if (n < o.V) {
                 int lo = 0, hi = o.G - 1;
@@ -176,11 +170,11 @@ __global__ void __launch_bounds__(256) ds_tile_kernel(const DsArrays a, const Ds
                 else
                     v = r[R_VROW] + a.vpre[gb[B_NODE] + local];
             }
-            o.tvp[i] = v;
+            o.img.tvp[i] = v;
         }
     }
-    if (o.pair)
-        for (size_t k = (size_t)o.V * T + tid, kend = (size_t)max(o.ntiles, 1) * ts::TILE_M * T; k < kend; k += stride) o.pair[k] = -1;
+    if (o.img.pair)
+        for (size_t k = (size_t)o.V * T + tid, kend = (size_t)max(o.ntiles, 1) * ts::TILE_M * T; k < kend; k += stride) o.img.pair[k] = -1;
 }
 
 }  // namespace ds

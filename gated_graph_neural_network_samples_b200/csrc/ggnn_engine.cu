@@ -142,6 +142,10 @@ struct ModelShape {
     size_t max_smem = 0;
 };
 
+// The shared memory per block of a model shape made without a device (host-only prepare calls, datasets and tile plans): an H100's
+// opt-in maximum.
+constexpr size_t HOST_MAX_SMEM = 227 * 1024;
+
 // What build_plan and the image builders derive from one batch: the tile plan and the layout of the graph image.
 struct BatchPlan {
     bool weighted = false;   // every message has a weight (GCN, weighted dense adjacency): the image carries the slot weights
@@ -168,19 +172,6 @@ struct BatchPlan {
     size_t off_tslot = 0;            // source-keyed CSR entry -> target-CSR slot (attention backward)
     size_t off_pair = 0, off_vptr = 0, off_vsrc = 0, off_tvp = 0, off_vinfo = 0;   // streaming plan: (target,type) -> source table, virtual rows (pairs with several messages)
     size_t off_slotw = 0, off_tslotw = 0;   // weighted: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
-};
-
-// Typed device pointers into the uploaded graph image of the current batch, made once per upload by ggnn_set_graph_prepared.  An array
-// the plan does not carry points at the start of the image.
-struct GraphDev {
-    const int *row_ptr, *csr_src, *csr_msg;
-    const float *indeg, *denom;
-    const int* tile_start;
-    const unsigned* tile_mask;
-    const int *trow, *ttgt, *tslot;                      // source-keyed CSR (save_for_backward)
-    const int *pair_src, *vrow_ptr, *vsrc, *tile_vptr;   // streaming plan
-    const int4* vinfo;
-    const float *slot_w, *tslot_w;                       // weighted batches: per-slot adjacency weights
 };
 
 // The weights in the pre-split, pre-tiled bf16 layout of one tensor-core kernel family, with each layer's offsets.  The tiles are rebuilt
@@ -215,7 +206,7 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     DevBuf graph_buf;   // the graph image of the current batch
     size_t graph_bytes = 0;
     DevBuf ds_table;    // the batch table of a dataset batch (ggnn_set_graph_dataset): tile starts and per-graph offsets
-    GraphDev gd;        // ... and the view of it every driver reads
+    ImageView gd;       // the view of graph_buf every driver reads, made by every graph upload (bind_graph)
     // readout (gated_regression): node -> graph map of the current batch
     DevBuf ro_buf; StagedImage ro_stage;
     int ro_V = -1, ro_G = 0; bool ro_grouped = false, ro_has_mask = false;
@@ -313,9 +304,9 @@ static void fill_common_params(const ggnn_engine* e, Params& p, const float* h0,
     p.use_bias = e->use_bias; p.use_avg = e->use_avg; p.cell = e->cell; p.act = e->act;
     p.save = e->save ? 1 : 0;
     p.drop_keep = e->drop_keep; p.drop_seed = e->drop_seed;
-    const GraphDev& gd = e->gd;
-    p.tile_start = gd.tile_start; p.tile_mask = gd.tile_mask; p.row_ptr = gd.row_ptr; p.csr_src = gd.csr_src;
-    p.slot_w = e->weighted ? gd.slot_w : nullptr; p.indeg = gd.indeg; p.denom = gd.denom;
+    const ImageView& gd = e->gd;
+    p.tile_start = gd.tile_start; p.tile_mask = gd.tile_mask; p.row_ptr = gd.row_ptr; p.csr_src = gd.src;
+    p.slot_w = gd.slotw; p.indeg = gd.indeg; p.denom = gd.denom;
     set_layer_states(e, p, h0, h_out);
     p.save_buf = saved_step(e, 0);   // the kernels index it by global step
     for (int l = 0; l < e->L; ++l) {
@@ -794,7 +785,7 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
     // forward values of node_states_per_layer
     std::vector<const float*> fstate(L + 1);
     for (int l = 0; l <= L; ++l) fstate[l] = layer_state(e, l, e->last_h0, e->last_out);
-    const GraphDev& gd = e->gd;
+    const ImageView& gd = e->gd;
     const long long n = (long long)vd;
     const int eb = (int)std::min<long long>((n + 255) / 256, 4096);
     auto gemm_nt = [&](bool acc, const float* A, int lda, int a_stride, const float* B, int ldb, int b_stride, int nseg, float* C, int ldc,
@@ -883,27 +874,27 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
             }
             // ---- messages: all edge types at once.  At[v, t*D..] = sum of h over the type-t sources of v, Gt[s, t*D..] = sum of dx' over
             // the type-t targets of s.  A weighted batch weights both by the adjacency entry of the slot.
-            GatherJob j0{gd.row_ptr, gd.csr_src, h, At, nullptr, nullptr}, j1{gd.trow, gd.ttgt, dxp, Gt, nullptr, nullptr};
+            GatherJob j0{gd.row_ptr, gd.src, h, At, nullptr, nullptr}, j1{gd.trow, gd.ttgt, dxp, Gt, nullptr, nullptr};
             if (e->use_att) {   // softmax backward first (it adds to dh_new), then the gathers are weighted by the probabilities
                 const float* alpha = (const float*)e->att_buf.ptr + (size_t)(e->step_base[l] + s) * (size_t)std::max<int64_t>(e->M, 1);
                 gemm_nt(false, dxp, D, 0, w.edge_weights, D, 0, 1, Pall, TD, V, TD, D);   // P[v, t*D+k] = <dx'[v], W_t[k, :]>
                 // the target kernel holds 8 columns of d h[v] per lane up to hidden 256, 16 above
                 if (e->det && gw.edge_type_attention_weights) {   // per-block d a_t into ws, then added over the blocks in a fixed order
                     (D <= 256 ? attention_bwd_target_ordered_kernel<8> : attention_bwd_target_ordered_kernel<16>)<<<nodes_blocks, 256, 0, st>>>(
-                        gd.row_ptr, gd.csr_src, h, Pall, alpha, w.edge_type_attention_weights, dsa, dh_new, ws, V, D, T);
+                        gd.row_ptr, gd.src, h, Pall, alpha, w.edge_type_attention_weights, dsa, dh_new, ws, V, D, T);
                     ordered_colsum_kernel<<<T, 256, 0, st>>>(ws, nodes_blocks, T, gw.edge_type_attention_weights);
                     ++e->last_launches;
                 } else {
                     (D <= 256 ? attention_bwd_target_kernel<8> : attention_bwd_target_kernel<16>)<<<nodes_blocks, 256, 0, st>>>(
-                        gd.row_ptr, gd.csr_src, h, Pall, alpha, w.edge_type_attention_weights, dsa, dh_new, gw.edge_type_attention_weights, V, D, T);
+                        gd.row_ptr, gd.src, h, Pall, alpha, w.edge_type_attention_weights, dsa, dh_new, gw.edge_type_attention_weights, V, D, T);
                 }
                 attention_bwd_source_kernel<<<nodes_blocks, 256, 0, st>>>(gd.trow, gd.ttgt, gd.tslot, h, dsa, dh_new, V, D, T);
                 e->last_launches += 2;
                 j0.w = j1.w = alpha;
                 j1.widx = gd.tslot;
             } else if (e->weighted) {
-                j0.w = gd.slot_w;
-                j1.w = gd.tslot_w;
+                j0.w = gd.slotw;
+                j1.w = gd.tslotw;
             }
             csr_gather_all_kernel<<<dim3(nodes_blocks, 2), 256, 0, st>>>(j0, j1, V, D, T);
             ++e->last_launches;
@@ -1107,9 +1098,10 @@ static void fill_target_csr(int V, int T, const int32_t* const* adj, const int32
 }
 
 // Streaming plan: number the (target, type) pairs marked -2 ("several messages") in row order, replace the mark by -(2 + vid) and list
-// their sources (vinfo: count + the first seven inline; vptr / vsrc: the complete lists).  `pair` already holds -1 / the single source.
+// their sources (vptr / vsrc).  `pair` already holds -1 / the single source.  The independent reference of ggnn_host_stream_tables, which
+// the CPU tests hold the builder's own tables (stream_rows) against.
 static void number_virtual_rows(int ntiles, int T, const int* tile_start, const int* row_ptr, const int* csr_src, int* pair, int* vptr, int* vsrc,
-                                int* tvp, int* vinfo) {
+                                int* tvp) {
     int vid = 0, vm = 0;
     vptr[0] = 0;
     for (int i = 0; i < ntiles; ++i) {
@@ -1118,10 +1110,6 @@ static void number_virtual_rows(int ntiles, int T, const int* tile_start, const 
             if (pair[k] != -2) continue;
             const int b = row_ptr[k], cnt = row_ptr[k + 1] - b;
             pair[k] = -(2 + vid);
-            if (vinfo) {
-                vinfo[8 * vid] = cnt;
-                for (int m = 0; m < 7; ++m) vinfo[8 * vid + 1 + m] = m < cnt ? csr_src[b + m] : 0;
-            }
             for (int m = 0; m < cnt; ++m) vsrc[vm++] = csr_src[b + m];
             vptr[++vid] = vm;
         }
@@ -1147,7 +1135,7 @@ int ggnn_host_tile_plan(int32_t hidden_size, int32_t num_edge_types, int32_t pre
     std::vector<int> cuts;
     find_cuts(reach.data(), V, cuts);
     ModelShape s;
-    s.D = hidden_size; s.T = num_edge_types; s.precision = precision; s.num_sms = num_sms; s.max_smem = 227 * 1024;
+    s.D = hidden_size; s.T = num_edge_types; s.precision = precision; s.num_sms = num_sms; s.max_smem = HOST_MAX_SMEM;
     if (precision != GGNN_PREC_FP32) s.DP = (hidden_size + 15) / 16 * 16;
     BatchPlan p;
     std::string err;
@@ -1201,7 +1189,7 @@ int ggnn_host_stream_tables(int32_t V, int32_t T, const int32_t* const* adj, con
     }
     for (size_t k = (size_t)V * T; k < (size_t)ntiles * ts::TILE_M * T; ++k) pair_src[k] = -1;
     if (nv + 1 > vrow_capacity || nvm > vsrc_capacity) return GGNN_EINVAL;
-    number_virtual_rows(ntiles, T, tile_start.data(), row_ptr.data(), src.data(), pair_src, vrow_ptr, vsrc, tile_vptr, nullptr);
+    number_virtual_rows(ntiles, T, tile_start.data(), row_ptr.data(), src.data(), pair_src, vrow_ptr, vsrc, tile_vptr);
     *num_virtual_rows = nv;
     return GGNN_OK;
 }
@@ -1280,6 +1268,176 @@ static size_t layout_image(const ModelShape& shape, BatchPlan& p, bool save, int
     return off;
 }
 
+// The typed view of an image laid out by plan `p` (layout_image) at `base`.  The one statement of which sections a plan carries: the
+// source-keyed CSR with save_for_backward (its slot map with attention, its weights on a weighted batch), the streaming tables on the
+// streaming plan, the slot weights on a weighted batch.  Every other section is null.
+static ImageView image_view(const BatchPlan& p, bool use_att, char* base) {
+    auto sec = [&](size_t off, bool present) { return present ? (void*)(base + off) : nullptr; };
+    ImageView v;
+    v.row_ptr = (int*)sec(p.off_row_ptr, true); v.src = (int*)sec(p.off_src, true); v.msg = (int*)sec(p.off_msg, true);
+    v.indeg = (float*)sec(p.off_indeg, true); v.denom = (float*)sec(p.off_denom, true);
+    v.tile_start = (int*)sec(p.off_tiles, true); v.tile_mask = (unsigned*)sec(p.off_mask, true);
+    v.trow = (int*)sec(p.off_trow, p.has_transpose); v.ttgt = (int*)sec(p.off_ttgt, p.has_transpose);
+    v.tslot = (int*)sec(p.off_tslot, p.has_transpose && use_att);
+    v.pair = (int*)sec(p.off_pair, p.stream); v.vptr = (int*)sec(p.off_vptr, p.stream); v.vsrc = (int*)sec(p.off_vsrc, p.stream);
+    v.tvp = (int*)sec(p.off_tvp, p.stream); v.vinfo = (int*)sec(p.off_vinfo, p.stream);
+    v.slotw = (float*)sec(p.off_slotw, p.weighted); v.tslotw = (float*)sec(p.off_tslotw, p.weighted && p.has_transpose);
+    return v;
+}
+
+// ---- the sections' builders: the batch builder below runs them over a whole batch, ds_add_graph over one graph of a dataset, so every
+// section has one format.
+
+// Pass 1 over the edge lists (adj[t]: type t's (source, target) pairs; type_base[t]: the position of its first message in the reference's
+// type-major message order, type_base[T] = M): checks every edge against V nodes, counts the messages of every (target, type) row into
+// counts[k + 1] (V*T + 1 entries) and, with `reach` (V + 1 entries), sets reach[j] = the farthest node an edge whose lower end is node j
+// touches.  Split over `nth` threads by EDGE ranges: counting is commutative, so the threads add into the shared per-row counts with relaxed
+// atomic increments (and an atomic max for `reach`) -- same totals for every thread count; a single thread uses plain increments.  Returns
+// false when an edge is out of range (first_bad_edge names it).
+static bool count_edges(int V, int T, const int32_t* const* adj, const int64_t* type_base, int nth, int* counts, int* reach) {
+    const int64_t M = type_base[T];
+    const bool need_cuts = reach != nullptr;
+    int bad_edge = 0;
+#ifdef _OPENMP
+#pragma omp parallel num_threads(nth) if (nth > 1)
+#endif
+    {
+        int k = 0, n = 1;
+#ifdef _OPENMP
+        k = omp_get_thread_num(); n = omp_get_num_threads();
+#endif
+        {   // clear this thread's slice of the scratch arrays
+            const size_t nc = (size_t)V * T + 1, c0 = nc * k / n, c1 = nc * (k + 1) / n;
+            std::fill(counts + c0, counts + c1, 0);
+            if (need_cuts) {
+                const size_t nr = (size_t)V + 1, r0 = nr * k / n, r1 = nr * (k + 1) / n;
+                std::fill(reach + r0, reach + r1, 0);
+            }
+        }
+#ifdef _OPENMP
+#pragma omp barrier
+#endif
+        const int64_t e0 = M * k / n, e1 = M * (k + 1) / n;   // this thread's messages, in the type-major order
+        int* const cnt = counts;
+        int* const rch = reach;
+        bool bad = false;
+        for (int t = 0; t < T && !bad; ++t) {
+            const int32_t* a = adj[t];
+            const int i0 = (int)(std::max(e0, type_base[t]) - type_base[t]);
+            const int i1 = (int)(std::min(e1, type_base[t + 1]) - type_base[t]);
+            if (n == 1) {
+                for (int i = i0; i < i1; ++i) {
+                    const int s = a[2 * i], d = a[2 * i + 1];
+                    if ((unsigned)s >= (unsigned)V || (unsigned)d >= (unsigned)V) { bad = true; break; }
+                    ++cnt[(size_t)d * T + t + 1];
+                    if (need_cuts) {
+                        const int lo = std::min(s, d), hi = std::max(s, d);
+                        rch[lo] = std::max(rch[lo], hi);   // unconditional store: the compare-and-branch form mispredicts on every other edge
+                    }
+                }
+            } else {
+                for (int i = i0; i < i1; ++i) {
+                    const int s = a[2 * i], d = a[2 * i + 1];
+                    if ((unsigned)s >= (unsigned)V || (unsigned)d >= (unsigned)V) { bad = true; break; }
+                    __atomic_fetch_add(cnt + ((size_t)d * T + t + 1), 1, __ATOMIC_RELAXED);
+                    if (need_cuts) {
+                        const int lo = std::min(s, d), hi = std::max(s, d);
+                        int cur = __atomic_load_n(rch + lo, __ATOMIC_RELAXED);
+                        while (hi > cur && !__atomic_compare_exchange_n(rch + lo, &cur, hi, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
+                    }
+                }
+            }
+        }
+        if (bad) {
+#ifdef _OPENMP
+#pragma omp atomic write
+#endif
+            bad_edge = 1;
+        }
+    }
+    return !bad_edge;
+}
+
+// The first edge in the lists' order that is out of range for V nodes (after count_edges found one): its type and index.
+static void first_bad_edge(int V, int T, const int32_t* const* adj, const int32_t* num_edges, int& bad_t, int& bad_i) {
+    bad_t = bad_i = 0;
+    for (int t = 0; t < T; ++t)
+        for (int i = 0; i < num_edges[t]; ++i) {
+            const int s = adj[t][2 * i], d = adj[t][2 * i + 1];
+            if ((unsigned)s >= (unsigned)V || (unsigned)d >= (unsigned)V) { bad_t = t; bad_i = i; return; }
+        }
+}
+
+// The denominators of nodes [v0, v1) from the [V][T] in-degrees: tf.reduce_sum over the type axis in fp32 (sparse:207), then
+// + SMALL_NUMBER (:209).
+static void fill_denominators(int v0, int v1, int T, const float* indeg, float* denom) {
+    for (int v = v0; v < v1; ++v) {
+        const float* row = indeg + (size_t)v * T;
+        float s = 0.0f;
+        for (int t = 0; t < T; ++t) s += row[t];
+        denom[v] = s + 1e-7f;
+    }
+}
+
+// The source-keyed CSR of the backward pass (rows source*T+type -> targets, in message order), which turns its scatter into a gather:
+// trow [V*T + 1], ttgt [M]; `tslot` (when non-null) the target-CSR slot of every entry, from csr_msg (the message of every target-CSR slot);
+// `tslotw` (when non-null) its weight, from the per-message weights w.
+static void fill_source_csr(int V, int T, const int32_t* const* adj, const int32_t* num_edges, int64_t M, const int* csr_msg, const float* w,
+                            int* trow, int* ttgt, int* tslot, float* tslotw) {
+    std::vector<int> cnt((size_t)V * T + 1, 0);
+    for (int t = 0; t < T; ++t)
+        for (int i = 0; i < num_edges[t]; ++i) ++cnt[(size_t)adj[t][2 * i] * T + t + 1];
+    trow[0] = 0;
+    for (size_t k = 1; k <= (size_t)V * T; ++k) trow[k] = trow[k - 1] + cnt[k];
+    for (size_t k = 0; k < (size_t)V * T; ++k) cnt[k] = trow[k];
+    std::vector<int> slot_of_msg;
+    if (tslot) {
+        slot_of_msg.resize((size_t)std::max<int64_t>(M, 1));
+        for (int64_t k = 0; k < M; ++k) slot_of_msg[csr_msg[k]] = (int)k;
+    }
+    int m = 0;
+    for (int t = 0; t < T; ++t)
+        for (int i = 0; i < num_edges[t]; ++i, ++m) {
+            const int j = cnt[(size_t)adj[t][2 * i] * T + t]++;
+            ttgt[j] = adj[t][2 * i + 1];
+            if (tslot) tslot[j] = slot_of_msg[m];
+            if (tslotw) tslotw[j] = w[m];
+        }
+}
+
+// The streaming plan's tables of the (target, type) rows [r0, r1), one sequential pass: pair[r] = -1 (no message), its one source, or
+// -(2 + vid) for a virtual row (several messages), numbered on from `vid`; a virtual row's sources go to vsrc from `vm` on, its end to
+// vptr[vid + 1] and, when `vinfo` is non-null, its count and first seven sources to vinfo[8 * vid ..].  Advances vid and vm.
+static void stream_rows(size_t r0, size_t r1, const int* row_ptr, const int* csr_src, int* pair, int* vptr, int* vsrc, int* vinfo, int& vid,
+                        int& vm) {
+    for (size_t r = r0; r < r1; ++r) {
+        const int b = row_ptr[r], cnt = row_ptr[r + 1] - b;
+        if (cnt == 0) pair[r] = -1;
+        else if (cnt == 1) pair[r] = csr_src[b];
+        else {
+            pair[r] = -(2 + vid);
+            if (vinfo) {
+                vinfo[8 * vid] = cnt;
+                for (int m = 0; m < 7; ++m) vinfo[8 * vid + 1 + m] = m < cnt ? csr_src[b + m] : 0;
+            }
+            for (int m = 0; m < cnt; ++m) vsrc[vm++] = csr_src[b + m];
+            vptr[++vid] = vm;
+        }
+    }
+}
+
+// GCN entries (row i = output, column j = input, int64) as one edge type j -> i: checks every entry against V nodes and writes the int32
+// (source j, target i) pairs in list order.  Returns the index of the first entry out of range, or -1.
+static int64_t gcn_pairs(int64_t V, int64_t nnz, const int64_t* list, int32_t* pairs) {
+    for (int64_t k = 0; k < nnz; ++k) {
+        const int64_t i = list[2 * k], j = list[2 * k + 1];
+        if (i < 0 || i >= V || j < 0 || j >= V) return k;
+        pairs[2 * k] = (int32_t)j;
+        pairs[2 * k + 1] = (int32_t)i;
+    }
+    return -1;
+}
+
 // ---- the host half of ggnn_set_graph_sparse: validation, tile plan, stable target-sorted CSR, streaming tables -> g->image.
 // `weighted`: the batch has one weight per message, `w`, in the type-major message order (required when there are messages); the image
 // then carries them in target-CSR order and, with the source-keyed CSR, in source-CSR order.
@@ -1332,73 +1490,10 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     if (need_cuts) reach.resize((size_t)V + 1);
     std::vector<int64_t> type_base(T + 1, 0);   // position of every type's first message in the reference's type-major message order
     for (int t = 0; t < T; ++t) type_base[t + 1] = type_base[t] + num_edges[t];
-    int bad_edge = 0;
-    // Pass 1 is split by EDGE ranges: counting is commutative, so the threads add into the shared per-row counts with relaxed atomic
-    // increments (and an atomic max for `reach`) -- same totals for every thread count; a single thread uses plain increments.
-#ifdef _OPENMP
-#pragma omp parallel num_threads(nth) if (nth > 1)
-#endif
-    {
-        int k = 0, n = 1;
-#ifdef _OPENMP
-        k = omp_get_thread_num(); n = omp_get_num_threads();
-#endif
-        {   // clear this thread's slice of the scratch arrays
-            const size_t nc = (size_t)V * T + 1, c0 = nc * k / n, c1 = nc * (k + 1) / n;
-            std::fill(counts.begin() + c0, counts.begin() + c1, 0);
-            if (need_cuts) {
-                const size_t nr = (size_t)V + 1, r0 = nr * k / n, r1 = nr * (k + 1) / n;
-                std::fill(reach.begin() + r0, reach.begin() + r1, 0);
-            }
-        }
-#ifdef _OPENMP
-#pragma omp barrier
-#endif
-        const int64_t e0 = M * k / n, e1 = M * (k + 1) / n;   // this thread's messages, in the type-major order
-        int* const cnt = counts.data();
-        int* const rch = need_cuts ? reach.data() : nullptr;
-        bool bad = false;
-        for (int t = 0; t < T && !bad; ++t) {
-            const int32_t* a = adj[t];
-            const int i0 = (int)(std::max(e0, type_base[t]) - type_base[t]);
-            const int i1 = (int)(std::min(e1, type_base[t + 1]) - type_base[t]);
-            if (n == 1) {
-                for (int i = i0; i < i1; ++i) {
-                    const int s = a[2 * i], d = a[2 * i + 1];
-                    if ((unsigned)s >= (unsigned)V || (unsigned)d >= (unsigned)V) { bad = true; break; }
-                    ++cnt[(size_t)d * T + t + 1];
-                    if (need_cuts) {
-                        const int lo = std::min(s, d), hi = std::max(s, d);
-                        rch[lo] = std::max(rch[lo], hi);   // unconditional store: the compare-and-branch form mispredicts on every other edge
-                    }
-                }
-            } else {
-                for (int i = i0; i < i1; ++i) {
-                    const int s = a[2 * i], d = a[2 * i + 1];
-                    if ((unsigned)s >= (unsigned)V || (unsigned)d >= (unsigned)V) { bad = true; break; }
-                    __atomic_fetch_add(cnt + ((size_t)d * T + t + 1), 1, __ATOMIC_RELAXED);
-                    if (need_cuts) {
-                        const int lo = std::min(s, d), hi = std::max(s, d);
-                        int cur = __atomic_load_n(rch + lo, __ATOMIC_RELAXED);
-                        while (hi > cur && !__atomic_compare_exchange_n(rch + lo, &cur, hi, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {}
-                    }
-                }
-            }
-        }
-        if (bad) {
-#ifdef _OPENMP
-#pragma omp atomic write
-#endif
-            bad_edge = 1;
-        }
-    }
-    if (bad_edge) {   // name the first offending edge, like the single pass did
-        for (int t = 0; t < T; ++t)
-            for (int i = 0; i < num_edges[t]; ++i) {
-                const int s = adj[t][2 * i], d = adj[t][2 * i + 1];
-                if ((unsigned)s >= (unsigned)V || (unsigned)d >= (unsigned)V)
-                    return g->fail(GGNN_ERANGE, "edge %d of type %d = (%d,%d) is out of range for %d nodes", i, t, s, d, V);
-            }
+    if (!count_edges(V, T, adj, type_base.data(), nth, counts.data(), need_cuts ? reach.data() : nullptr)) {
+        int t, i;
+        first_bad_edge(V, T, adj, num_edges, t, i);
+        return g->fail(GGNN_ERANGE, "edge %d of type %d = (%d,%d) is out of range for %d nodes", i, t, adj[t][2 * i], adj[t][2 * i + 1], V);
     }
     lap("  edges pass 1", t_lap);
     std::vector<int> cuts;
@@ -1438,19 +1533,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     const size_t off = layout_image(shape, p, g->save, M, (int)part_nv[nth], part_nvm[nth]);
     CU_TRY(g, g->image.begin(off));
     g->bytes = off;
-    char* base = g->image.ptr;
-    int* row_ptr = (int*)(base + p.off_row_ptr);
-    int* csr_src = (int*)(base + p.off_src);
-    int* csr_msg = (int*)(base + p.off_msg);
-    float* h_indeg = (float*)(base + p.off_indeg);
-    float* h_denom = (float*)(base + p.off_denom);
-    int* h_tiles = (int*)(base + p.off_tiles);
-    unsigned* h_mask = (unsigned*)(base + p.off_mask);
-    int* pair = p.stream ? (int*)(base + p.off_pair) : nullptr;   // streaming plan: (target, type) -> its one source / virtual row
-    int* vptr = p.stream ? (int*)(base + p.off_vptr) : nullptr;
-    int* vsrc = p.stream ? (int*)(base + p.off_vsrc) : nullptr;
-    int* tvp = p.stream ? (int*)(base + p.off_tvp) : nullptr;
-    int* vinfo = p.stream ? (int*)(base + p.off_vinfo) : nullptr;
+    const ImageView img = image_view(p, shape.use_att, g->image.ptr);
     lap("stage reserve", t_lap);
 
     // ---- pass 2, per thread over its tile range: exclusive scan of the (target, type) rows -> row_ptr, fill cursors, the tiles'
@@ -1461,8 +1544,8 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     std::vector<int>& cursor = g->h_cursor;   // next free slot of every (target, type) row (its own array: the counts of a range's last
     cursor.resize((size_t)V * T + 1);         // row are read by one thread while the next range's thread already writes cursors)
     int max_tile_msgs = 0, max_tile_types = 0;
-    row_ptr[0] = 0;
-    if (vptr) vptr[0] = 0;
+    img.row_ptr[0] = 0;
+    if (img.vptr) img.vptr[0] = 0;
 #ifdef _OPENMP
 #pragma omp parallel for schedule(static, 1) num_threads(nth) if (nth > 1) reduction(max : max_tile_msgs, max_tile_types)
 #endif
@@ -1476,15 +1559,15 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
                     const int c = counts[r + t + 1];
                     cursor[r + t] = run;
                     run += c;
-                    row_ptr[r + t + 1] = run;
+                    img.row_ptr[r + t + 1] = run;
                     mask |= (unsigned)(c > 0) << t;
                 }
-            h_mask[i] = mask;
+            img.tile_mask[i] = mask;
             max_tile_msgs = std::max(max_tile_msgs, run - tile_first);
             max_tile_types = std::max(max_tile_types, __builtin_popcount(mask));
-            h_tiles[i] = tile_start[i];
+            img.tile_start[i] = tile_start[i];
         }
-        if (k == nth - 1) h_tiles[ntiles] = tile_start[ntiles];
+        if (k == nth - 1) img.tile_start[ntiles] = tile_start[ntiles];
     }
     p.max_tile_msgs = max_tile_msgs;
     p.max_tile_types = max_tile_types;
@@ -1494,6 +1577,8 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
 #endif
     for (int k = 0; k < nth; ++k) {
         const int v0 = tile_start[tb[k]], v1 = tile_start[tb[k + 1]];
+        int* const csr_src = img.src;
+        int* const csr_msg = img.msg;
         for (int t = 0; t < T; ++t) {
             const int32_t* a = adj[t];
             const int ne = num_edges[t];
@@ -1519,70 +1604,27 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
                 }
             }
         }
-        if (pair) {   // one sequential pass over the range's rows: no message -> -1, one -> its source, several -> virtual row
+        if (img.pair) {   // the range's rows: no message -> -1, one -> its source, several -> virtual row; then the last tile's rows beyond V
             int vid = (int)part_nv[k], vm = (int)part_nvm[k];
             for (int i = tb[k]; i < tb[k + 1]; ++i) {
-                tvp[i] = vid;
-                size_t r = (size_t)tile_start[i] * T;
+                img.tvp[i] = vid;
                 const size_t rend = (size_t)tile_start[i + 1] * T, rpad = (size_t)(i + 1) * ts::TILE_M * T;
-                for (; r < rend; ++r) {
-                    const int b = row_ptr[r], cnt = row_ptr[r + 1] - b;
-                    if (cnt == 0) pair[r] = -1;
-                    else if (cnt == 1) pair[r] = csr_src[b];
-                    else {
-                        pair[r] = -(2 + vid);
-                        vinfo[8 * vid] = cnt;
-                        for (int m = 0; m < 7; ++m) vinfo[8 * vid + 1 + m] = m < cnt ? csr_src[b + m] : 0;
-                        for (int m = 0; m < cnt; ++m) vsrc[vm++] = csr_src[b + m];
-                        vptr[++vid] = vm;
-                    }
-                }
-                for (; r < rpad; ++r) pair[r] = -1;   // rows of the last tile beyond V
+                stream_rows((size_t)tile_start[i] * T, rend, img.row_ptr, csr_src, img.pair, img.vptr, img.vsrc, img.vinfo, vid, vm);
+                for (size_t r = rend; r < rpad; ++r) img.pair[r] = -1;
             }
-            if (k == nth - 1) tvp[ntiles] = vid;
+            if (k == nth - 1) img.tvp[ntiles] = vid;
         }
-        if (weighted) {   // the weights of this range's slots, in target-CSR order
-            float* slotw = (float*)(base + p.off_slotw);
-            for (int64_t m = part_msgs[k]; m < part_msgs[k + 1]; ++m) slotw[m] = w[csr_msg[m]];
-        }
-        if (v1 > v0) memcpy(h_indeg + (size_t)v0 * T, indeg + (size_t)v0 * T, sizeof(float) * (size_t)(v1 - v0) * T);
-        for (int v = v0; v < v1; ++v) {
-            const float* row = indeg + (size_t)v * T;
-            float s = 0.0f;  // tf.reduce_sum over the type axis in fp32 (sparse:207), then + SMALL_NUMBER (:209)
-            for (int t = 0; t < T; ++t) s += row[t];
-            h_denom[v] = s + 1e-7f;
-        }
+        if (img.slotw)   // the weights of this range's slots, in target-CSR order
+            for (int64_t m = part_msgs[k]; m < part_msgs[k + 1]; ++m) img.slotw[m] = w[csr_msg[m]];
+        if (v1 > v0) memcpy(img.indeg + (size_t)v0 * T, indeg + (size_t)v0 * T, sizeof(float) * (size_t)(v1 - v0) * T);
+        fill_denominators(v0, v1, T, indeg, img.denom);
     }
     if (ntiles == 0) {
-        h_tiles[0] = 0;
-        if (pair) { for (size_t r = 0; r < (size_t)ts::TILE_M * T; ++r) pair[r] = -1; tvp[0] = 0; }
+        img.tile_start[0] = 0;
+        if (img.pair) { for (size_t r = 0; r < (size_t)ts::TILE_M * T; ++r) img.pair[r] = -1; img.tvp[0] = 0; }
     }
     lap("csr fill", t_lap);
-    if (p.has_transpose) {   // messages keyed by (source, type): the scatter of the backward pass becomes a gather
-        int* trow = (int*)(base + p.off_trow);
-        int* ttgt = (int*)(base + p.off_ttgt);
-        std::vector<int> cnt((size_t)V * T + 1, 0);
-        for (int t = 0; t < T; ++t)
-            for (int i = 0; i < num_edges[t]; ++i) ++cnt[(size_t)adj[t][2 * i] * T + t + 1];
-        trow[0] = 0;
-        for (size_t k = 1; k <= (size_t)V * T; ++k) trow[k] = trow[k - 1] + cnt[k];
-        for (size_t k = 0; k < (size_t)V * T; ++k) cnt[k] = trow[k];
-        std::vector<int> slot_of_msg;
-        int* tslot = shape.use_att ? (int*)(base + p.off_tslot) : nullptr;
-        float* tslotw = weighted ? (float*)(base + p.off_tslotw) : nullptr;
-        if (tslot) {
-            slot_of_msg.resize((size_t)std::max<int64_t>(M, 1));
-            for (int64_t k = 0; k < M; ++k) slot_of_msg[csr_msg[k]] = (int)k;
-        }
-        int m = 0;
-        for (int t = 0; t < T; ++t)
-            for (int i = 0; i < num_edges[t]; ++i, ++m) {
-                const int j = cnt[(size_t)adj[t][2 * i] * T + t]++;
-                ttgt[j] = adj[t][2 * i + 1];
-                if (tslot) tslot[j] = slot_of_msg[m];
-                if (tslotw) tslotw[j] = w[m];
-            }
-    }
+    if (img.trow) fill_source_csr(V, T, adj, num_edges, M, img.msg, w, img.trow, img.ttgt, img.tslot, img.tslotw);
     lap("denom+masks+extra", t_lap);
     g->valid = true;
     return GGNN_OK;
@@ -1602,34 +1644,53 @@ const char* ggnn_prepared_graph_error(const ggnn_prepared_graph* g) { return g ?
 
 }  // extern "C"
 
-// The prologue of the six prepare calls: reuse or allocate *inout and give it a model shape.  With an engine `e` (which must be a
-// `model` engine, the model of Config), the shape and -- for save_for_backward = -1 -- the save flag are the engine's, and the image
-// is pinned on its device; without one, the shape comes from `cfg` for a host of `num_sms` SMs with 227 KiB of shared memory each,
-// and the image is plain memory.
+// The model shape of a prepared graph or a dataset (`t` takes the error): with an engine `e`, which must be a `model` engine (the model of
+// Config), the engine's, made current on this thread -- which may be a producer thread; without one, the shape `cfg` describes for a host
+// of `num_sms` SMs with HOST_MAX_SMEM of shared memory each.
+template <class Config>
+static int model_shape_for(ErrorText* t, ModelShape& s, const ggnn_engine* e, const Config* cfg, int32_t num_sms, const char* fn) {
+    constexpr int model = std::is_same<Config, ggnn_gcn_config>::value ? MODEL_GCN : MODEL_GGNN;
+    if (e) {
+        s = *e;
+        if (e->model != model) return wrong_model(t, fn, e->model, model);
+        if (cudaSetDevice(e->device) != cudaSuccess) return t->fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);
+        return GGNN_OK;
+    }
+    s = ModelShape();
+    int rc;
+    if constexpr (model == MODEL_GCN) rc = init_gcn_shape(s, cfg, t->err);
+    else rc = init_model_shape(s, cfg, t->err);
+    if (rc) return rc;
+    s.num_sms = num_sms; s.max_smem = HOST_MAX_SMEM;
+    return GGNN_OK;
+}
+
+// The prologue of the six prepare calls: reuse or allocate *inout and give it a model shape (model_shape_for).  With an engine, the save
+// flag for save_for_backward = -1 is the engine's and the image is pinned on its device; without one, the image is plain memory.
 template <class Config>
 static int begin_prepare(ggnn_prepared_graph** inout, const ggnn_engine* e, const Config* cfg, int32_t num_sms, int32_t save_for_backward,
                          const char* fn) {
-    constexpr int model = std::is_same<Config, ggnn_gcn_config>::value ? MODEL_GCN : MODEL_GGNN;
     if (!inout || (!e && (!cfg || num_sms <= 0))) return GGNN_EINVAL;
     ggnn_prepared_graph* g = *inout;
     if (!g) { g = new ggnn_prepared_graph(); *inout = g; }
     g->valid = false;
     g->image.use_cuda = e != nullptr;
-    if (e) {
-        g->shape = *e;
-        if (e->model != model) return wrong_model(g, fn, e->model, model);
-        g->save = save_for_backward >= 0 ? save_for_backward != 0 : e->save;   // a producer thread says what the batch will be used for
-        if (cudaSetDevice(e->device) != cudaSuccess) return g->fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);   // this may be a producer thread
-        return GGNN_OK;
-    }
-    g->shape = ModelShape();
-    int rc;
-    if constexpr (model == MODEL_GCN) rc = init_gcn_shape(g->shape, cfg, g->err);
-    else rc = init_model_shape(g->shape, cfg, g->err);
-    if (rc) return rc;
-    g->shape.num_sms = num_sms; g->shape.max_smem = 227 * 1024;
-    g->save = save_for_backward != 0;
+    if (int rc = model_shape_for(g, g->shape, e, cfg, num_sms, fn)) return rc;
+    g->save = e && save_for_backward < 0 ? e->save : save_for_backward != 0;   // a producer thread says what the batch will be used for
     return GGNN_OK;
+}
+
+// The plan fields the info calls of a prepared graph and a dataset batch report (image_bytes: the size of its image); null outputs are skipped.
+static void report_plan(const BatchPlan& q, size_t bytes, int32_t* num_nodes, int64_t* num_messages, int32_t* num_tiles, int64_t* image_bytes,
+                        int32_t* is_streaming, char* plan_text, int32_t plan_text_capacity, int32_t* max_tile_msgs, int32_t* max_tile_types) {
+    if (num_nodes) *num_nodes = q.V;
+    if (num_messages) *num_messages = q.M;
+    if (num_tiles) *num_tiles = q.ntiles;
+    if (image_bytes) *image_bytes = (int64_t)bytes;
+    if (is_streaming) *is_streaming = q.stream ? 1 : 0;
+    if (plan_text && plan_text_capacity > 0) snprintf(plan_text, (size_t)plan_text_capacity, "%s", q.plan_text.c_str());
+    if (max_tile_msgs) *max_tile_msgs = q.max_tile_msgs;
+    if (max_tile_types) *max_tile_types = q.max_tile_types;
 }
 
 // The common body of the ggnn_set_graph_* calls: build(&e->own_prep) prepares the batch in the engine's own prepared graph (the same two
@@ -1653,12 +1714,7 @@ int ggnn_host_prepare_graph_sparse(const ggnn_config* cfg, int32_t num_sms, int3
 int ggnn_prepared_graph_info(const ggnn_prepared_graph* g, int32_t* num_nodes, int64_t* num_messages, int32_t* num_tiles, int64_t* image_bytes,
                              int32_t* is_streaming, char* plan_text, int32_t plan_text_capacity) {
     if (!g || !g->valid) return GGNN_ESTATE;
-    if (num_nodes) *num_nodes = g->plan.V;
-    if (num_messages) *num_messages = g->plan.M;
-    if (num_tiles) *num_tiles = g->plan.ntiles;
-    if (image_bytes) *image_bytes = (int64_t)g->bytes;
-    if (is_streaming) *is_streaming = g->plan.stream ? 1 : 0;
-    if (plan_text && plan_text_capacity > 0) snprintf(plan_text, (size_t)plan_text_capacity, "%s", g->plan.plan_text.c_str());
+    report_plan(g->plan, g->bytes, num_nodes, num_messages, num_tiles, image_bytes, is_streaming, plan_text, plan_text_capacity, nullptr, nullptr);
     return GGNN_OK;
 }
 
@@ -1666,21 +1722,20 @@ int ggnn_prepared_graph_arrays(const ggnn_prepared_graph* g, int32_t* row_ptr, i
                                int32_t* pair_src) {
     if (!g || !g->valid) return GGNN_ESTATE;
     const BatchPlan& q = g->plan;
-    const char* base = g->image.ptr;
+    const ImageView img = image_view(q, g->shape.use_att, g->image.ptr);
     const size_t V = (size_t)q.V, T = (size_t)g->shape.T, M = (size_t)q.M;
-    if (row_ptr) memcpy(row_ptr, base + q.off_row_ptr, sizeof(int) * (V * T + 1));
-    if (src && M) memcpy(src, base + q.off_src, sizeof(int) * M);
-    if (msg && M) memcpy(msg, base + q.off_msg, sizeof(int) * M);
-    if (tile_start) memcpy(tile_start, base + q.off_tiles, sizeof(int) * (size_t)(q.ntiles + 1));
-    if (denom && V) memcpy(denom, base + q.off_denom, sizeof(float) * V);
-    if (pair_src && q.stream) memcpy(pair_src, base + q.off_pair, sizeof(int) * (size_t)std::max(q.ntiles, 1) * ts::TILE_M * T);
+    if (row_ptr) memcpy(row_ptr, img.row_ptr, sizeof(int) * (V * T + 1));
+    if (src && M) memcpy(src, img.src, sizeof(int) * M);
+    if (msg && M) memcpy(msg, img.msg, sizeof(int) * M);
+    if (tile_start) memcpy(tile_start, img.tile_start, sizeof(int) * (size_t)(q.ntiles + 1));
+    if (denom && V) memcpy(denom, img.denom, sizeof(float) * V);
+    if (pair_src && img.pair) memcpy(pair_src, img.pair, sizeof(int) * (size_t)std::max(q.ntiles, 1) * ts::TILE_M * T);
     return GGNN_OK;
 }
 
 int ggnn_prepared_graph_tile_stats(const ggnn_prepared_graph* g, int32_t* max_tile_msgs, int32_t* max_tile_types) {
     if (!g || !g->valid) return GGNN_ESTATE;
-    if (max_tile_msgs) *max_tile_msgs = g->plan.max_tile_msgs;
-    if (max_tile_types) *max_tile_types = g->plan.max_tile_types;
+    report_plan(g->plan, g->bytes, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, max_tile_msgs, max_tile_types);
     return GGNN_OK;
 }
 
@@ -1714,15 +1769,7 @@ static int check_batch_shape(ggnn_engine* e, const ModelShape& q, const BatchPla
 
 // The typed view of the graph image in graph_buf (laid out by e's plan), then room for the states of the batch: the end of every graph upload.
 static int bind_graph(ggnn_engine* e) {
-    const char* b = (const char*)e->graph_buf.ptr;
-    GraphDev& d = e->gd;
-    d.row_ptr = (const int*)(b + e->off_row_ptr); d.csr_src = (const int*)(b + e->off_src); d.csr_msg = (const int*)(b + e->off_msg);
-    d.indeg = (const float*)(b + e->off_indeg); d.denom = (const float*)(b + e->off_denom);
-    d.tile_start = (const int*)(b + e->off_tiles); d.tile_mask = (const unsigned*)(b + e->off_mask);
-    d.trow = (const int*)(b + e->off_trow); d.ttgt = (const int*)(b + e->off_ttgt); d.tslot = (const int*)(b + e->off_tslot);
-    d.pair_src = (const int*)(b + e->off_pair); d.vrow_ptr = (const int*)(b + e->off_vptr); d.vsrc = (const int*)(b + e->off_vsrc);
-    d.tile_vptr = (const int*)(b + e->off_tvp); d.vinfo = (const int4*)(b + e->off_vinfo);
-    d.slot_w = (const float*)(b + e->off_slotw); d.tslot_w = (const float*)(b + e->off_tslotw);
+    e->gd = image_view(*e, e->use_att, (char*)e->graph_buf.ptr);
     int rc = reserve_states(e);
     if (rc) return rc;
     e->graph_set = true;
@@ -1949,7 +1996,7 @@ static int forward_stepwise(ggnn_engine* e, const float* h0, float* h_out, cudaS
     char* sb = (char*)e->step_buf.ptr;
     float *At = (float*)(sb + o_at), *X = (float*)(sb + o_x), *Gb = (float*)(sb + o_g), *Cb = (float*)(sb + o_c), *Qb = (float*)(sb + o_q);
     const float* wt = (const float*)e->step_wt.buf.ptr;
-    const GraphDev& gd = e->gd;
+    const ImageView& gd = e->gd;
     const long long n = (long long)vd;
     const int eb = (int)std::min<long long>((n + 255) / 256, 4096), nodes_blocks = (V + 7) / 8;
     auto gemm = [&](const float* A, int lda, int a_stride, const float* B, int ldb, int b_stride, int nseg, float* C, int ldc, int N, int K) {
@@ -1972,10 +2019,10 @@ static int forward_stepwise(ggnn_engine* e, const float* h0, float* h_out, cudaS
         const float* msg_w = q.slot_w;
         if (e->use_att) {
             float* att = (float*)e->att_buf.ptr + (size_t)gs * (e->save ? (size_t)std::max<int64_t>(e->M, 1) : 0);
-            step::attention_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.csr_src, h, w.edge_type_attention_weights, att, V, D, T);
+            step::attention_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.src, h, w.edge_type_attention_weights, att, V, D, T);
             msg_w = att;
         }
-        const GatherJob gj{gd.row_ptr, gd.csr_src, h, At, msg_w, nullptr};
+        const GatherJob gj{gd.row_ptr, gd.src, h, At, msg_w, nullptr};
         csr_gather_all_kernel<<<dim3(nodes_blocks, 1), 256, 0, st>>>(gj, gj, V, D, T);
         gemm(At, T * D, D, wt + e->step_wt.off_edge[l], D, D * D, T, X + (size_t)R * D, ldx, D, D);
         step::agg_epilogue_kernel<<<eb, 256, 0, st>>>(X, ldx, R * D, (R + 1) * D, h, e->use_bias ? w.edge_biases : nullptr, gd.indeg,
@@ -2143,7 +2190,7 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     float* u_chk = (float*)(cb + (size_t)(L + 3) * img_b);
     const size_t vd_bytes = (size_t)V * D * sizeof(float);
     const bool gru = e->cell == CELL_GRU;
-    const GraphDev& gd = e->gd;
+    const ImageView& gd = e->gd;
 
     // shared-memory budgets
     const size_t avail = (e->max_smem > 2048 ? e->max_smem - 2048 : 0);
@@ -2165,7 +2212,7 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     base.nparts = e->precision == GGNN_PREC_BF16X3 ? 3 : 1;
     base.cell = e->cell; base.act = e->act; base.use_bias = e->use_bias; base.use_avg = e->use_avg;
     base.tile_mask = gd.tile_mask;
-    base.pair_src = gd.pair_src; base.vrow_ptr = gd.vrow_ptr; base.vsrc = gd.vsrc; base.tile_vptr = gd.tile_vptr; base.vinfo = gd.vinfo;
+    base.pair_src = gd.pair; base.vrow_ptr = gd.vptr; base.vsrc = gd.vsrc; base.tile_vptr = gd.tvp; base.vinfo = (const int4*)gd.vinfo;
     base.virt_img = (uint8_t*)e->ts_virt.ptr;   // pairs with several messages, pre-summed by the prologue of every gather launch
     base.indeg = gd.indeg; base.denom = gd.denom;
     base.drop_keep = e->drop_keep; base.drop_seed = e->drop_seed;
@@ -2265,13 +2312,9 @@ static int build_gcn_image(ggnn_prepared_graph* g, int32_t V, int64_t nnz, const
     if (V < 0 || nnz < 0 || (nnz > 0 && (!list || !w))) return g->fail(GGNN_EINVAL, "null/negative argument");
     if (nnz > 0x7fffffff) return g->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
     std::vector<int32_t> pairs((size_t)nnz * 2);
-    for (int64_t k = 0; k < nnz; ++k) {
-        const int64_t i = list[2 * k], j = list[2 * k + 1];
-        if (i < 0 || i >= V || j < 0 || j >= V)
-            return g->fail(GGNN_ERANGE, "adjacency_list[%lld] = (%lld, %lld) is out of range for %d nodes", (long long)k, (long long)i, (long long)j, V);
-        pairs[2 * k] = (int32_t)j;
-        pairs[2 * k + 1] = (int32_t)i;
-    }
+    if (const int64_t k = gcn_pairs(V, nnz, list, pairs.data()); k >= 0)
+        return g->fail(GGNN_ERANGE, "adjacency_list[%lld] = (%lld, %lld) is out of range for %d nodes", (long long)k, (long long)list[2 * k],
+                       (long long)list[2 * k + 1], V);
     const std::vector<float> indeg((size_t)std::max(V, 1), 0.0f);
     const int32_t* lists[1] = {pairs.data()};
     const int32_t counts[1] = {(int32_t)nnz};
@@ -2324,9 +2367,10 @@ int ggnn_set_graph_gcn(ggnn_engine* e, int32_t V, int64_t nnz, const int64_t* li
 int ggnn_prepared_graph_slot_weights(const ggnn_prepared_graph* g, float* target_csr_w, float* source_csr_w) {
     if (!g || !g->valid || !g->plan.weighted) return GGNN_ESTATE;
     const BatchPlan& q = g->plan;
-    if (source_csr_w && !q.has_transpose) return GGNN_ESTATE;
-    if (target_csr_w && q.M) memcpy(target_csr_w, g->image.ptr + q.off_slotw, sizeof(float) * (size_t)q.M);
-    if (source_csr_w && q.M) memcpy(source_csr_w, g->image.ptr + q.off_tslotw, sizeof(float) * (size_t)q.M);
+    const ImageView img = image_view(q, g->shape.use_att, g->image.ptr);
+    if (source_csr_w && !img.tslotw) return GGNN_ESTATE;
+    if (target_csr_w && q.M) memcpy(target_csr_w, img.slotw, sizeof(float) * (size_t)q.M);
+    if (source_csr_w && q.M) memcpy(source_csr_w, img.tslotw, sizeof(float) * (size_t)q.M);
     return GGNN_OK;
 }
 
@@ -2341,7 +2385,7 @@ static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream
     p.V = V; p.D = D; p.DP = DP; p.L = L;
     p.nparts = e->precision == GGNN_PREC_BF16X3 ? 3 : 1;
     p.save = e->save ? 1 : 0;
-    p.tile_start = e->gd.tile_start; p.row_ptr = e->gd.row_ptr; p.csr_src = e->gd.csr_src; p.slot_w = e->gd.slot_w;
+    p.tile_start = e->gd.tile_start; p.row_ptr = e->gd.row_ptr; p.csr_src = e->gd.src; p.slot_w = e->gd.slotw;
     set_layer_states(e, p, h0, h_out);
     for (int l = 0; l < L; ++l) { p.kernel[l] = e->gcn_w[l].kernel; p.bias[l] = e->gcn_w[l].bias; }
     p.drop_keep = e->drop_keep; p.drop_seed = e->drop_seed;
@@ -2405,7 +2449,7 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
     CU_TRY(e, e->bwd_buf.reserve(4 * slab + ws_floats * sizeof(float)));
     char* bb = (char*)e->bwd_buf.ptr;
     float *dH = (float*)bb, *dP = (float*)(bb + slab), *S = (float*)(bb + 2 * slab), *dS = (float*)(bb + 3 * slab), *ws = (float*)(bb + 4 * slab);
-    const GraphDev& gd = e->gd;
+    const ImageView& gd = e->gd;
     std::vector<const float*> fstate(L + 1);
     for (int l = 0; l <= L; ++l) fstate[l] = layer_state(e, l, e->last_h0, e->last_out);
     const long long n = (long long)vd;
@@ -2422,7 +2466,7 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
         }
         const ggnn_gcn_layer_grads& gw = grads[l];
         if (gw.kernel) {
-            GatherJob j{gd.row_ptr, gd.csr_src, fstate[l], S, gd.slot_w, nullptr};
+            GatherJob j{gd.row_ptr, gd.src, fstate[l], S, gd.slotw, nullptr};
             csr_gather_all_kernel<<<gather_grid, 256, 0, st>>>(j, j, V, D, 1);
             ++e->last_launches;
             SegList sl;
@@ -2437,7 +2481,7 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
         if (l == 0 && !d_h0) break;
         gemm_nt(e, st, false, dpre, D, 0, e->gcn_w[l].kernel, D, 0, 1, dS, D, V, D, D);
         float* dst = l == 0 ? d_h0 : dH;
-        GatherJob j{gd.trow, gd.ttgt, dS, dst, gd.tslot_w, nullptr};
+        GatherJob j{gd.trow, gd.ttgt, dS, dst, gd.tslotw, nullptr};
         csr_gather_all_kernel<<<gather_grid, 256, 0, st>>>(j, j, V, D, 1);
         ++e->last_launches;
         dout = dst;
@@ -2785,8 +2829,8 @@ int ggnn_get_csr(ggnn_engine* e, int32_t* row_ptr, int32_t* src, int32_t* msg) {
     CU_TRY(e, cudaSetDevice(e->device));
     CU_TRY(e, cudaDeviceSynchronize());
     if (row_ptr) CU_TRY(e, cudaMemcpy(row_ptr, e->gd.row_ptr, sizeof(int) * ((size_t)e->V * e->T + 1), cudaMemcpyDeviceToHost));
-    if (src && e->M) CU_TRY(e, cudaMemcpy(src, e->gd.csr_src, sizeof(int) * (size_t)e->M, cudaMemcpyDeviceToHost));
-    if (msg && e->M) CU_TRY(e, cudaMemcpy(msg, e->gd.csr_msg, sizeof(int) * (size_t)e->M, cudaMemcpyDeviceToHost));
+    if (src && e->M) CU_TRY(e, cudaMemcpy(src, e->gd.src, sizeof(int) * (size_t)e->M, cudaMemcpyDeviceToHost));
+    if (msg && e->M) CU_TRY(e, cudaMemcpy(msg, e->gd.msg, sizeof(int) * (size_t)e->M, cudaMemcpyDeviceToHost));
     return GGNN_OK;
 }
 
@@ -2859,80 +2903,59 @@ struct DsHost {
 
 // Adds one graph of V nodes: per edge type t its graph-local (source, target) list adj[t] of ne[t] messages in the reference's order, its
 // [V][T] in-degrees, and (weighted datasets) its per-message weights w in type-major order.  Builds its pieces with the batch builder's
-// own passes (fill_target_csr, number_virtual_rows, find_cuts) and appends them.
+// section builders (count_edges, fill_denominators, fill_source_csr, stream_rows; find_cuts) and its target CSR with fill_target_csr, on
+// the graph alone, and appends them.
 static int ds_add_graph(ggnn_dataset* d, DsHost& h, int gi, int V, const int32_t* const* adj, const int32_t* ne, const float* indeg, const float* w) {
     const int T = d->shape.T;
     DsGraph g;
     g.V = V;
-    std::vector<int> counts((size_t)V * T + 1, 0), reach((size_t)V + 1, 0);
-    std::vector<int> ltb(T + 1, 0);
-    for (int t = 0; t < T; ++t) {
-        ltb[t + 1] = ltb[t] + ne[t];
-        for (int i = 0; i < ne[t]; ++i) {
-            const int s = adj[t][2 * i], dd = adj[t][2 * i + 1];
-            if ((unsigned)s >= (unsigned)V || (unsigned)dd >= (unsigned)V)
-                return d->fail(GGNN_ERANGE, "graph %d: edge %d of type %d = (%d,%d) is out of range for its %d nodes", gi, i, t, s, dd, V);
-            ++counts[(size_t)dd * T + t + 1];
-            reach[std::min(s, dd)] = std::max(reach[std::min(s, dd)], std::max(s, dd));
-        }
-        d->type_msgs.push_back(ne[t]);
+    std::vector<int64_t> type_base(T + 1, 0);
+    for (int t = 0; t < T; ++t) type_base[t + 1] = type_base[t] + ne[t];
+    std::vector<int> counts((size_t)V * T + 1), reach((size_t)V + 1);
+    if (!count_edges(V, T, adj, type_base.data(), 1, counts.data(), reach.data())) {
+        int t, i;
+        first_bad_edge(V, T, adj, ne, t, i);
+        return d->fail(GGNN_ERANGE, "graph %d: edge %d of type %d = (%d,%d) is out of range for its %d nodes", gi, i, t, adj[t][2 * i],
+                       adj[t][2 * i + 1], V);
     }
-    const int M = ltb[T];
+    d->type_msgs.insert(d->type_msgs.end(), ne, ne + T);
+    const int M = (int)type_base[T];
     g.M = M;
     std::vector<int> row_ptr((size_t)V * T + 1), src((size_t)std::max(M, 1)), msg((size_t)std::max(M, 1));
     fill_target_csr(V, T, adj, ne, counts, row_ptr.data(), src.data(), msg.data());
     h.row_end.insert(h.row_end.end(), row_ptr.begin() + 1, row_ptr.end());
     h.src.insert(h.src.end(), src.begin(), src.begin() + M);
     for (size_t k = 0; k < (size_t)V * T; ++k)
-        for (int m = row_ptr[k]; m < row_ptr[k + 1]; ++m) h.pos.push_back(msg[m] - ltb[k % T]);
+        for (int m = row_ptr[k]; m < row_ptr[k + 1]; ++m) h.pos.push_back(msg[m] - (int)type_base[k % T]);
     h.indeg.insert(h.indeg.end(), indeg, indeg + (size_t)V * T);
-    for (int v = 0; v < V; ++v) {   // as the builder: tf.reduce_sum over the type axis in fp32 (sparse:207), then + SMALL_NUMBER (:209)
-        float s = 0.0f;
-        for (int t = 0; t < T; ++t) s += indeg[(size_t)v * T + t];
-        h.denom.push_back(s + 1e-7f);
-    }
+    const size_t d0 = h.denom.size();
+    h.denom.resize(d0 + V);
+    fill_denominators(0, V, T, indeg, h.denom.data() + d0);
     if (d->weighted)
         for (int m = 0; m < M; ++m) h.slotw.push_back(w[msg[m]]);
-    if (d->train) {   // source-keyed CSR, filled in message order like the builder's
-        std::vector<int> trow((size_t)V * T + 1, 0), slot_of_msg((size_t)std::max(M, 1));
-        for (int t = 0; t < T; ++t)
-            for (int i = 0; i < ne[t]; ++i) ++trow[(size_t)adj[t][2 * i] * T + t + 1];
-        for (size_t k = 1; k <= (size_t)V * T; ++k) trow[k] += trow[k - 1];
-        h.trow_end.insert(h.trow_end.end(), trow.begin() + 1, trow.end());
-        for (int m = 0; m < M; ++m) slot_of_msg[msg[m]] = m;
+    if (d->train) {
+        std::vector<int> trow((size_t)V * T + 1);
         const size_t t0 = h.ttgt.size();
         h.ttgt.resize(t0 + M);
         if (d->shape.use_att) h.tslot.resize(t0 + M);
         if (d->weighted) h.tslotw.resize(t0 + M);
-        int m = 0;
-        for (int t = 0; t < T; ++t)
-            for (int i = 0; i < ne[t]; ++i, ++m) {
-                const int j = trow[(size_t)adj[t][2 * i] * T + t]++;
-                h.ttgt[t0 + j] = adj[t][2 * i + 1];
-                if (d->shape.use_att) h.tslot[t0 + j] = slot_of_msg[m];
-                if (d->weighted) h.tslotw[t0 + j] = w[m];
-            }
+        fill_source_csr(V, T, adj, ne, M, msg.data(), w, trow.data(), h.ttgt.data() + t0, d->shape.use_att ? h.tslot.data() + t0 : nullptr,
+                        d->weighted ? h.tslotw.data() + t0 : nullptr);
+        h.trow_end.insert(h.trow_end.end(), trow.begin() + 1, trow.end());
     }
-    if (d->stream_tables) {   // the streaming plan's tables of the graph on its own, virtual rows numbered in row order
-        std::vector<int> pair((size_t)V * T), vptr(1, 0), vsrc, tvp(2);
-        int nv = 0;
-        for (size_t k = 0; k < (size_t)V * T; ++k) {
-            const int cnt = row_ptr[k + 1] - row_ptr[k];
-            pair[k] = cnt == 0 ? -1 : (cnt == 1 ? src[row_ptr[k]] : -2);
-            if (cnt >= 2) { ++nv; g.nvm += cnt; }
-        }
-        vptr.resize(nv + 1); vsrc.resize((size_t)std::max(g.nvm, 1));
-        const int tile[2] = {0, V};
-        if (V > 0) number_virtual_rows(1, T, tile, row_ptr.data(), src.data(), pair.data(), vptr.data(), vsrc.data(), tvp.data(), nullptr);
-        g.nv = nv;
+    if (d->stream_tables) {   // the graph's streaming tables on its own, virtual rows numbered in row order from 0
+        std::vector<int> pair((size_t)V * T), vptr((size_t)V * T + 1, 0), vsrc((size_t)std::max(M, 1));
+        int nv = 0, nvm = 0;
+        stream_rows(0, (size_t)V * T, row_ptr.data(), src.data(), pair.data(), vptr.data(), vsrc.data(), nullptr, nv, nvm);
+        g.nv = nv; g.nvm = nvm;
         int before = 0;
         for (int v = 0; v < V; ++v) {
             h.vpre.push_back(before);
             for (int t = 0; t < T; ++t) before += pair[(size_t)v * T + t] <= -2;
         }
         h.pair.insert(h.pair.end(), pair.begin(), pair.end());
-        h.vend.insert(h.vend.end(), vptr.begin() + 1, vptr.end());
-        h.vsrc.insert(h.vsrc.end(), vsrc.begin(), vsrc.begin() + g.nvm);
+        h.vend.insert(h.vend.end(), vptr.begin() + 1, vptr.begin() + 1 + nv);
+        h.vsrc.insert(h.vsrc.end(), vsrc.begin(), vsrc.begin() + nvm);
     }
     std::vector<int> cuts;
     find_cuts(reach.data(), V, cuts);
@@ -2994,31 +3017,20 @@ static int ds_finish(ggnn_dataset* d, DsHost& h, const float* ann, const float* 
     return GGNN_OK;
 }
 
-// The prologue of the four create calls: the model shape from the engine (`e`, whose model must be `model`) or from a config for a host of
-// `num_sms` SMs; the handle is allocated here and returned even on failure, with the text in ggnn_dataset_error.
+// The prologue of the four create calls: the model shape (model_shape_for), then the argument checks; the handle is allocated here and
+// returned even on failure, with the text in ggnn_dataset_error.
 template <class Config>
 static int begin_dataset(ggnn_dataset** out, const ggnn_engine* e, const Config* cfg, int32_t num_sms, int32_t for_training, int32_t N,
                          const int64_t* node_counts, int32_t ann, const float* annotations, int32_t tasks, const float* labels,
                          const float* lmask, const char* fn) {
-    constexpr int model = std::is_same<Config, ggnn_gcn_config>::value ? MODEL_GCN : MODEL_GGNN;
     if (!out || (!e && (!cfg || num_sms <= 0))) return GGNN_EINVAL;
     ggnn_dataset* d = new ggnn_dataset();
     *out = d;
-    if (e) {
-        if (e->model != model) return wrong_model(d, fn, e->model, model);
-        d->shape = *e;
-        if (cudaSetDevice(e->device) != cudaSuccess) return d->fail(GGNN_ECUDA, "cudaSetDevice(%d) failed", e->device);
-    } else {
-        int rc;
-        if constexpr (model == MODEL_GCN) rc = init_gcn_shape(d->shape, cfg, d->err);
-        else rc = init_model_shape(d->shape, cfg, d->err);
-        if (rc) return rc;
-        d->shape.num_sms = num_sms; d->shape.max_smem = 227 * 1024;
-    }
+    if (int rc = model_shape_for(d, d->shape, e, cfg, num_sms, fn)) return rc;
     d->on_device = e != nullptr;
     d->train = for_training != 0;
-    d->weighted = model == MODEL_GCN;
-    d->stream_tables = model == MODEL_GGNN && d->shape.precision != GGNN_PREC_FP32;
+    d->weighted = d->shape.model == MODEL_GCN;
+    d->stream_tables = d->shape.model == MODEL_GGNN && d->shape.precision != GGNN_PREC_FP32;
     d->N = N; d->ann = ann; d->tasks = tasks;
     if (N < 0 || ann < 0 || tasks < 0 || (N > 0 && !node_counts) || (ann > 0 && N > 0 && !annotations) || (tasks > 0 && N > 0 && (!labels || !lmask)))
         return d->fail(GGNN_EINVAL, "null/negative argument");
@@ -3070,14 +3082,9 @@ static int create_dataset_gcn(ggnn_dataset** out, const ggnn_engine* e, const Co
         const int64_t e0 = entry_offsets[i], e1 = entry_offsets[i + 1], V = node_counts[i];
         if (e0 < 0 || e1 < e0 || e1 - e0 > 0x7fffffff || (e1 > e0 && (!lists || !weights))) return d->fail(GGNN_EINVAL, "graph %d: bad entry offsets", i);
         pairs.resize((size_t)(e1 - e0) * 2);
-        for (int64_t k = e0; k < e1; ++k) {
-            const int64_t r = lists[2 * k], c = lists[2 * k + 1];
-            if (r < 0 || r >= V || c < 0 || c >= V)
-                return d->fail(GGNN_ERANGE, "graph %d: entry %lld = (%lld, %lld) is out of range for its %lld nodes", i, (long long)(k - e0),
-                               (long long)r, (long long)c, (long long)V);
-            pairs[2 * (k - e0)] = (int32_t)c;
-            pairs[2 * (k - e0) + 1] = (int32_t)r;
-        }
+        if (const int64_t k = gcn_pairs(V, e1 - e0, lists + 2 * e0, pairs.data()); k >= 0)
+            return d->fail(GGNN_ERANGE, "graph %d: entry %lld = (%lld, %lld) is out of range for its %lld nodes", i, (long long)k,
+                           (long long)lists[2 * (e0 + k)], (long long)lists[2 * (e0 + k) + 1], (long long)V);
         const std::vector<float> indeg((size_t)V, 0.0f);
         const int32_t* adj[1] = {pairs.data()};
         const int32_t ne[1] = {(int32_t)(e1 - e0)};
@@ -3315,16 +3322,9 @@ int ggnn_dataset_batch_info(const ggnn_dataset_batch* b, int32_t* num_nodes, int
                             int32_t* is_streaming, char* plan_text, int32_t plan_text_capacity, int32_t* tile_start, int32_t* max_tile_msgs,
                             int32_t* max_tile_types) {
     if (!b || !b->valid) return GGNN_ESTATE;
-    const BatchPlan& q = b->plan;
-    if (num_nodes) *num_nodes = q.V;
-    if (num_messages) *num_messages = q.M;
-    if (num_tiles) *num_tiles = q.ntiles;
-    if (image_bytes) *image_bytes = (int64_t)b->bytes;
-    if (is_streaming) *is_streaming = q.stream ? 1 : 0;
-    if (plan_text && plan_text_capacity > 0) snprintf(plan_text, (size_t)plan_text_capacity, "%s", q.plan_text.c_str());
-    if (tile_start) memcpy(tile_start, b->table.ptr, sizeof(int) * (size_t)(q.ntiles + 1));
-    if (max_tile_msgs) *max_tile_msgs = q.max_tile_msgs;
-    if (max_tile_types) *max_tile_types = q.max_tile_types;
+    report_plan(b->plan, b->bytes, num_nodes, num_messages, num_tiles, image_bytes, is_streaming, plan_text, plan_text_capacity, max_tile_msgs,
+                max_tile_types);
+    if (tile_start) memcpy(tile_start, b->table.ptr, sizeof(int) * (size_t)(b->plan.ntiles + 1));
     return GGNN_OK;
 }
 
@@ -3366,17 +3366,8 @@ static int set_graph_dataset(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, f
     CU_TRY(e, b->table.upload(e->ds_table.ptr, b->table_bytes, st));
     CU_TRY(e, cudaMemsetAsync(e->graph_buf.ptr, 0, b->bytes, st));   // the alignment gaps, as in a fresh host image
     CU_TRY(e, cudaMemsetAsync(e->ro_buf.ptr, 0, e->ro_off_perm, st));
-    char* base = (char*)e->graph_buf.ptr;
-    auto sec = [&](size_t off, bool present) { return present ? (void*)(base + off) : nullptr; };
     ds::DsOut o;
-    o.row_ptr = (int*)sec(q.off_row_ptr, true); o.src = (int*)sec(q.off_src, true); o.msg = (int*)sec(q.off_msg, true);
-    o.indeg = (float*)sec(q.off_indeg, true); o.denom = (float*)sec(q.off_denom, true);
-    o.tile_start = (int*)sec(q.off_tiles, true); o.tile_mask = (unsigned*)sec(q.off_mask, true);
-    o.trow = (int*)sec(q.off_trow, q.has_transpose); o.ttgt = (int*)sec(q.off_ttgt, q.has_transpose);
-    o.tslot = (int*)sec(q.off_tslot, q.has_transpose && e->use_att);
-    o.pair = (int*)sec(q.off_pair, q.stream); o.vptr = (int*)sec(q.off_vptr, q.stream); o.vsrc = (int*)sec(q.off_vsrc, q.stream);
-    o.tvp = (int*)sec(q.off_tvp, q.stream); o.vinfo = (int*)sec(q.off_vinfo, q.stream);
-    o.slotw = (float*)sec(q.off_slotw, q.weighted); o.tslotw = (float*)sec(q.off_tslotw, q.weighted && q.has_transpose);
+    o.img = image_view(q, e->use_att, (char*)e->graph_buf.ptr);
     o.h0 = h0; o.tv = target_values; o.tm = target_mask;
     o.ro_graph_of = (int*)((char*)e->ro_buf.ptr + e->ro_off_graph_of); o.ro_start = (int*)((char*)e->ro_buf.ptr + e->ro_off_start);
     o.node_mask = node_mask; o.ro_mask = dense ? (float*)((char*)e->ro_buf.ptr + e->ro_off_mask) : nullptr;
