@@ -71,7 +71,14 @@ SYMBOLS = {
     "ggnn_run_dense_host": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ggnn_run_sparse_host_readout": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                                C.POINTER(GgnnReadoutTask), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "ggnn_forward_host_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ggnn_readout_predict": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.POINTER(GgnnReadoutTask), C.c_void_p, C.c_int32, C.c_void_p,
+                                       C.c_void_p]),
+    "ggnn_dataset_batch_slots": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
+    "ggnn_run_sparse_host_predict": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                               C.c_int32, C.POINTER(GgnnReadoutTask), C.c_void_p, C.c_void_p]),
+    "ggnn_run_dense_host_predict": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                              C.POINTER(GgnnReadoutTask), C.c_void_p, C.c_void_p]),
+    "ggnn_forward_host_async":(C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ggnn_sync_check": (C.c_int, [C.c_void_p, C.c_void_p]),
     "ggnn_readout_set_graphs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "ggnn_readout_forward": (C.c_int, [C.c_void_p] + [C.c_void_p] * 7 + [C.c_void_p]),

@@ -107,7 +107,7 @@ class DenseGGNNChemModel(ChemModel):
         if ag is not None and at is not None:   # fused kernel (SURVEY 8f-1): masked per-graph sum included
             b, v = last_h.shape[0], last_h.shape[1]
             if not self.feed.get('_graph_adopted'):   # a device-data batch set the readout map and mask with its graph
-                self.engine.readout_set_graphs(b, nodes_per_graph=v, node_mask=self.feed[self.placeholders['node_mask']])
+                self._set_readout_map()
             self.output = self._readout.apply(self.engine, last_h.reshape(b * v, D), h0.reshape(b * v, D), ag[0], ag[1], at[0], at[1])
             return self.output
         gate_input = torch.cat([last_h, h0], dim=2).reshape(-1, 2 * D)
@@ -116,6 +116,65 @@ class DenseGGNNChemModel(ChemModel):
         mask = self._as_device_tensor(self.feed[self.placeholders['node_mask']])
         self.output = (gated * mask).sum(dim=1)
         return self.output
+
+    def _set_readout_map(self) -> None:
+        mask = np.asarray(self.feed[self.placeholders['node_mask']], dtype=np.float32)
+        self.engine.readout_set_graphs(mask.shape[0], nodes_per_graph=mask.shape[1], node_mask=mask)
+
+    # ------------------------------------------------------------------ prediction (dense:230-265)
+    def _prediction_batches(self, raw_graphs, batch_size: int, device_data: bool):
+        """The bucketed batches of packing.bucket_batches, packed without targets on the host or assembled from a target-free device dataset."""
+        ds = None
+        if device_data:
+            from .engine import DeviceDataset
+            ds = DeviceDataset.for_engine(self.engine, packing.FlatDenseGraphs(raw_graphs, (), self.params['tie_fwd_bkwd']), for_training=False,
+                                          stream=0)
+        for v, ids in packing.bucket_batches(raw_graphs, batch_size):
+            if ds is not None:
+                yield {'num_graphs': len(ids), 'num_vertices': v, '_dataset_batch': self._pooled_dataset_batch(ds, ids, False, nodes_per_graph=v)}, ids
+                continue
+            feed = packing.pack_dense_batch([raw_graphs[i] for i in ids], v, self.params['hidden_size'], self.num_edge_types, (),
+                                            self.params['tie_fwd_bkwd'])
+            eng = getattr(self, 'engine', None)
+            if hasattr(eng, 'prepare_graph_dense'):   # the host half in this producer thread, as in training
+                feed['_prepared_graph'] = self._prepare_from_pool(
+                    lambda reuse: eng.prepare_graph_dense(feed['adjacency_matrix'], save_for_backward=False, reuse=reuse), False)
+            yield feed, ids
+
+    def evaluate_one_batch(self, initial_node_representations, adjacency_matrices, node_masks=None):
+        """dense:230-249: one batch of ``b`` graphs -- their node annotations (``b`` lists of rows; the batch has as many rows per graph as
+        the first), ``[b, T, v, v]`` adjacency matrices and optionally ``[b, v]`` node masks, by default 1 for each graph's given rows and 0
+        beyond, as the reference builds it -- run as in validation.  Returns the reference's fetch ``self.output``: the readout of the LAST
+        task of ``task_ids`` only, ``[b]``.  ``predict`` gives every task."""
+        import torch
+        num_vertices = len(initial_node_representations[0])
+        if node_masks is None:
+            node_masks = [[1. for _ in r] + [0. for _ in range(num_vertices - len(r))] for r in initial_node_representations]
+        b = len(initial_node_representations)
+        h0 = np.zeros((b, num_vertices, self.params['hidden_size']), np.float32)   # pad_annotations, dense:166-169
+        for i, r in enumerate(initial_node_representations):
+            a = np.asarray(r, dtype=np.float32).reshape(len(r), -1)
+            h0[i, :a.shape[0], :a.shape[1]] = a
+        feed = {'initial_node_representation': h0, 'num_graphs': b, 'num_vertices': num_vertices,
+                'adjacency_matrix': np.asarray(adjacency_matrices, dtype=np.float32), 'node_mask': np.asarray(node_masks, dtype=np.float32),
+                'graph_state_keep_prob': 1.0, 'out_layer_dropout_keep_prob': 1.0, 'edge_weight_dropout_keep_prob': 1.0}
+        with torch.inference_mode():
+            return self._last_task_output(self._final_node_representations(feed)).cpu().numpy()
+
+    def example_evaluation(self, valid_file: str = 'molecules_valid.json', n: int = 10):
+        """dense:251-265: the targets of the first ``n`` molecules of ``valid_file``, then the predictions of one batch of them in the single
+        bucket [29] (rows padded to 29, so the default mask of evaluate_one_batch counts every row, as the reference's does)."""
+        import json
+        with open(valid_file, 'r') as fh:
+            example_molecules = json.load(fh)[:n]
+        for mol in example_molecules:
+            print(mol['targets'])
+        bucketed, bucket_sizes, _ = self.process_raw_graphs(example_molecules, is_training_data=False, bucket_sizes=np.array([29]))
+        elements = bucketed[0]
+        batch = packing.pack_dense_batch(elements, 29, self.annotation_size, self.num_edge_types, (), self.params['tie_fwd_bkwd'])
+        out = self.evaluate_one_batch(list(batch['initial_node_representation']), batch['adjacency_matrix'])
+        print(out)
+        return out
 
     def process_raw_graphs(self, raw_data: Sequence[Any], is_training_data: bool, bucket_sizes=None) -> Any:   # dense:132-164
         if bucket_sizes is None:

@@ -128,6 +128,23 @@ class SparseGCNChemModel(ChemModel):
 
     # ------------------------------------------------------------------ readout (gcn:84-93 == sparse:220-231)
     gated_regression = SparseGGNNChemModel.gated_regression
+    _set_readout_map = SparseGGNNChemModel._set_readout_map
+
+    # ------------------------------------------------------------------ prediction (the sparse model's, sparse:352-376)
+    evaluate_one_batch = SparseGGNNChemModel.evaluate_one_batch
+    example_evaluation = SparseGGNNChemModel.example_evaluation
+
+    def _prediction_batches(self, raw_graphs, batch_size: int, device_data: bool):
+        def host_feed(b):
+            feed = dict(b)
+            eng = getattr(self, 'engine', None)
+            if hasattr(eng, 'prepare_graph_gcn'):   # the host half in this producer thread, as in training
+                feed['_prepared_graph'] = self._prepare_from_pool(
+                    lambda reuse: eng.prepare_graph_gcn(b['initial_node_representation'].shape[0], b['adjacency_list'], b['adjacency_weights'],
+                                                        save_for_backward=False, reuse=reuse), False)
+            return feed
+        flat = packing.FlatGCNGraphs(packing.process_raw_graphs_gcn(raw_graphs, self.params['task_ids'], labels=False))
+        return self._flat_prediction_batches(flat, batch_size, device_data, host_feed)
 
     # ------------------------------------------------------------------ data (gcn:96-199) via packing.py
     def process_raw_graphs(self, raw_data: Sequence[Any], is_training_data: bool) -> Any:

@@ -155,14 +155,8 @@ class ChemModel(object):
     def forward_batch(self, feed: dict):
         """One ``sess.run`` worth of forward work on ``feed`` (chem_tensorflow.py:235 with the ops of :145-170)."""
         import torch
-        self.feed = feed
-        self._adopt_dataset_batch(feed)
+        final = self._final_node_representations(feed)
         keep = float(feed.get(self.placeholders['out_layer_dropout_keep_prob'], 1.0))
-        if self.params['use_graph']:
-            final = self.compute_final_node_representations()            # :145
-        else:
-            final = torch.zeros_like(self.initial_node_representation_tensor())   # :147
-        self.ops['final_node_representations'] = final
         tv, tm = (self._as_device_tensor(feed[self.placeholders[k]]) for k in ('target_values', 'target_mask'))
         losses, accs = [], []
         self._task_sums = []      # per task: (ratio * sum of masked 0.5*diff^2 [graph attached], mask sum) -- what data parallelism exchanges
@@ -177,6 +171,95 @@ class ChemModel(object):
             self._task_sums.append((numer, float(tm[internal_id, :].sum())))
             losses.append(numer / num)                                                          # :166
         return torch.stack(losses).sum(), accs                                                  # :170
+
+    def _final_node_representations(self, feed: dict):
+        """Adopts ``feed`` (a device-data batch is assembled here) and returns its final node states (chem_tensorflow.py:145-147)."""
+        import torch
+        self.feed = feed
+        self._adopt_dataset_batch(feed)
+        if self.params['use_graph']:
+            final = self.compute_final_node_representations()            # :145
+        else:
+            final = torch.zeros_like(self.initial_node_representation_tensor())   # :147
+        self.ops['final_node_representations'] = final
+        return final
+
+    # ------------------------------------------------------------------ prediction (sparse:352-376, dense:230-265)
+    def predict(self, raw_graphs: Sequence[dict], batch_size=None, device_data: bool = False) -> np.ndarray:
+        """Predictions of every task of ``params['task_ids']`` for the molecules ``raw_graphs`` (the reference's JSON dicts; a ``"targets"``
+        key is not needed): ``[len(task_ids), len(raw_graphs)]`` float32, column i for ``raw_graphs[i]`` whatever order the batches are cut
+        in.  Runs what a validation epoch runs (every keep probability 1.0, no gradients) in batches of ``batch_size`` (default
+        ``params['batch_size']``: nodes for the sparse models, graphs per bucket for the dense one), then every task's readout in one kernel
+        pass per batch, written through a slot map into one ``[tasks, N]`` device buffer that is copied back once.  ``device_data``: upload
+        the list once (a target-free device dataset) and assemble every batch on the GPU."""
+        import torch
+        graphs = list(raw_graphs)
+        if device_data and self.device.type != "cuda":
+            raise Exception("device_data keeps the data on the GPU: it needs a CUDA device, not %s" % self.device)
+        task_ids = self.params['task_ids']
+        out = torch.zeros(len(task_ids), len(graphs), dtype=torch.float32, device=self.device)
+        if not graphs:
+            return out.cpu().numpy()
+        with torch.inference_mode():
+            batches = ThreadedIterator(self._prediction_batches(graphs, int(batch_size or self.params['batch_size']), device_data), max_queue_size=5)
+            for feed, ids in batches:
+                for k in ('out_layer_dropout_keep_prob', 'graph_state_keep_prob', 'edge_weight_dropout_keep_prob'):
+                    if k in self.placeholders:
+                        feed[self.placeholders[k]] = 1.0
+                batch = feed.get('_dataset_batch')
+                final = self._final_node_representations(feed)
+                if self.device.type != "cuda":   # the CPU stand-in engines of the unit tests: each task's gated_regression, as forward_batch
+                    out[:, torch.as_tensor(ids)] = torch.stack([self.gated_regression(final, *self._readout_mlps(t, 1.0)) for t in task_ids])
+                    continue
+                if batch is None:
+                    self._set_readout_map()
+                slot = batch.slot_table if batch is not None else torch.as_tensor(ids, dtype=torch.int32).to(self.device)
+                h_last, h0 = self._readout_inputs(final)
+                self.engine.readout_predict(h_last, h0, self._readout_task_weights(), slot=slot, out=out, out_stride=len(graphs))
+        return out.cpu().numpy()
+
+    def _readout_mlps(self, task_id, keep: float):
+        return (self.weights['regression_gate_task%i' % task_id].bind(keep), self.weights['regression_transform_task%i' % task_id].bind(keep))
+
+    def _readout_inputs(self, final):
+        """``(h_T, h_0)`` of the batch as contiguous ``[V, DP]`` tensors at the engine's (padded) hidden width; padded columns are 0."""
+        import torch
+        D = self.params['hidden_size']
+        DP = getattr(self, '_padded_hidden', D)
+        h_last, h0 = final.reshape(-1, D), self.initial_node_representation_tensor().reshape(-1, D)
+        if DP != D:
+            h_last, h0 = (torch.nn.functional.pad(t, (0, DP - D)) for t in (h_last, h0))
+        return h_last.contiguous(), h0.contiguous()
+
+    def _readout_task_weights(self):
+        """Per task of ``params['task_ids']``: (w_gate [2DP], b_gate [1], w_trans [DP], b_trans [1]), the readout MLPs' single affine maps
+        zero-padded to the engine's hidden width (the gate's two D-row halves, h_T then h_0, padded each)."""
+        import torch
+        D = self.params['hidden_size']
+        DP = getattr(self, '_padded_hidden', D)
+        pad = lambda w: torch.nn.functional.pad(w.reshape(-1), (0, DP - D))
+        out = []
+        for t in self.params['task_ids']:
+            gate, trans = self.weights['regression_gate_task%i' % t], self.weights['regression_transform_task%i' % t]
+            if len(gate.weights) != 1 or len(trans.weights) != 1:
+                raise Exception("the fused readout needs readout MLPs without hidden layers (chem_tensorflow.py:153-157)")
+            wg = gate.weights[0].reshape(2, D)
+            out.append((torch.cat([pad(wg[0]), pad(wg[1])]).contiguous(), gate.biases[0].contiguous(), pad(trans.weights[0]).contiguous(),
+                        trans.biases[0].contiguous()))
+        return out
+
+    def _prediction_batches(self, raw_graphs: Sequence[dict], batch_size: int, device_data: bool):
+        """Yields ``(feed, ids)`` per batch of ``predict``: a feed without targets and the input indices of its graphs, in batch order."""
+        raise Exception("Models have to implement _prediction_batches!")
+
+    def _set_readout_map(self) -> None:
+        """Sets the engine's readout map from the current host-packed feed."""
+        raise Exception("Models have to implement _set_readout_map!")
+
+    def _last_task_output(self, final):
+        """``self.output`` of the reference after its readout loop: the LAST task's gated_regression (chem_tensorflow.py:151-160 overwrites
+        it per task), with the out-layer dropout off."""
+        return self.gated_regression(final, *self._readout_mlps(self.params['task_ids'][-1], 1.0))
 
     # ------------------------------------------------------------------ training step (chem_tensorflow.py:172-193)
     def trainable_variables(self):
@@ -327,11 +410,26 @@ class ChemModel(object):
             # stream 0: the legacy default stream of the engine's device, usable from this thread; the call returns once the upload ran
             ds = DeviceDataset.for_engine(self.engine, flat, for_training=True, stream=0)
             cache[:] = [c for c in cache if c[0] is not flat][-3:] + [(flat, ds)]
+        return self._pooled_dataset_batch(ds, ids, is_training, nodes_per_graph)
+
+    def _pooled_dataset_batch(self, ds, ids, is_training: bool, nodes_per_graph=None):
+        """The host half of a batch of ``ds``, rebuilt in place from a batch of the same dataset taken back from the pool when there is one."""
         pool = self.__dict__.setdefault('_dataset_batch_pool', [])
         reuse = next((b for b in pool if b.dataset is ds), None)
         if reuse is not None:
             pool.remove(reuse)
         return ds.prepare_batch(ids, save_for_backward=is_training, reuse=reuse, nodes_per_graph=nodes_per_graph)
+
+    def _flat_prediction_batches(self, flat, batch_size: int, device_data: bool, host_feed):
+        """``_prediction_batches`` of the sparse models over a flattened, target-free graph set: the node-budget batches of the graphs in
+        input order, each a device-data batch of a target-free dataset uploaded once (``device_data``) or ``host_feed(flat.pack(ids))``."""
+        from .engine import DeviceDataset
+        ds = DeviceDataset.for_engine(self.engine, flat, for_training=False, stream=0) if device_data else None
+        for ids in flat.iter_batch_ids(np.arange(flat.num_graphs), batch_size):
+            if ds is not None:
+                yield {'num_graphs': len(ids), '_graph_sizes': flat.n_nodes[ids], '_dataset_batch': self._pooled_dataset_batch(ds, ids, False)}, ids
+            else:
+                yield host_feed(flat.pack(ids, self.params['hidden_size'])), ids
 
     def _adopt_dataset_batch(self, feed) -> None:
         """--device-data, on the engine's thread: assembles the feed's dataset batch on the device and puts its h0, targets and mask (CUDA

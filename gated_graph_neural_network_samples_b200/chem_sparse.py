@@ -237,8 +237,7 @@ class SparseGGNNChemModel(ChemModel):
             # the fused kernel: both dot products, sigmoid, product and the per-graph segment sum in one launch (a device-data batch set
             # its readout map with its graph)
             if self.feed.get(self.placeholders['graph_nodes_list']) is not None:
-                self.engine.readout_set_graphs(int(self.feed[self.placeholders['num_graphs']]),
-                                               graph_nodes_list=self.feed[self.placeholders['graph_nodes_list']])
+                self._set_readout_map()
             self.output = self._readout.apply(self.engine, last_h, h0, ag[0], ag[1], at[0], at[1])
             return self.output
         gate_input = torch.cat([last_h, h0], dim=-1)
@@ -248,6 +247,47 @@ class SparseGGNNChemModel(ChemModel):
         out = torch.zeros(num_graphs, 1, device=self.device).index_add_(0, gnl, gated_outputs)   # unsorted_segment_sum
         self.output = out.squeeze(-1)
         return self.output
+
+    def _set_readout_map(self) -> None:
+        self.engine.readout_set_graphs(int(self.feed[self.placeholders['num_graphs']]), graph_nodes_list=self.feed[self.placeholders['graph_nodes_list']])
+
+    # ------------------------------------------------------------------ prediction (sparse:352-376)
+    def _prediction_batches(self, raw_graphs, batch_size: int, device_data: bool):
+        processed = packing.process_raw_graphs_sparse(raw_graphs, self.params['task_ids'], self.params['tie_fwd_bkwd'], labels=False)
+        flat = packing.FlatSparseGraphs(processed, self.num_edge_types)
+
+        def host_feed(b):
+            feed = {k: b[k] for k in ('initial_node_representation', 'num_incoming_edges_per_type', 'graph_nodes_list', 'num_graphs')}
+            for e, key in enumerate(self.placeholders['adjacency_lists']):
+                feed[key] = b['adjacency_lists'][e]
+            if hasattr(getattr(self, 'engine', None), 'prepare_graph_sparse'):   # the host half in this producer thread, as in training
+                feed['_prepared_graph'] = self._prepare_from_pool(
+                    lambda reuse: self.engine.prepare_graph_sparse(b['adjacency_lists'], b['num_incoming_edges_per_type'], save_for_backward=False,
+                                                                   reuse=reuse), False)
+            return feed
+        return self._flat_prediction_batches(flat, batch_size, device_data, host_feed)
+
+    def evaluate_one_batch(self, data):
+        """sparse:352-362: every batch of the processed graphs ``data`` (``process_raw_graphs``) run as in validation, its ``self.output``
+        printed.  That is the reference's fetch, the readout of the LAST task of ``task_ids`` only (gated_regression overwrites it per
+        task); returns those values for all of ``data``, in its order.  ``predict`` gives every task."""
+        import torch
+        outs = []
+        with torch.inference_mode():
+            for feed in self.make_minibatch_iterator(data, False):
+                out = self._last_task_output(self._final_node_representations(feed)).cpu().numpy()
+                print(out)
+                outs.append(out)
+        return np.concatenate(outs) if outs else np.zeros(0, np.float32)
+
+    def example_evaluation(self, valid_file: str = 'molecules_valid.json', n: int = 10):
+        """sparse:364-376: the targets of the first ``n`` molecules of ``valid_file``, then their predictions (evaluate_one_batch)."""
+        import json
+        with open(valid_file, 'r') as fh:
+            example_molecules = json.load(fh)[:n]
+        for mol in example_molecules:
+            print(mol['targets'])
+        return self.evaluate_one_batch(self.process_raw_graphs(example_molecules, is_training_data=False))
 
     # ------------------------------------------------------------------ data (sparse:234-350) via packing.py
     def process_raw_graphs(self, raw_data: Sequence[Any], is_training_data: bool) -> Any:

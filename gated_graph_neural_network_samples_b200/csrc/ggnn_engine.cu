@@ -213,6 +213,9 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     size_t ro_off_graph_of = 0, ro_off_start = 0, ro_off_mask = 0, ro_off_val = 0;
     size_t ro_off_perm = 0;   // ungrouped lists: the stable by-graph node permutation (graph g owns perm[start[g] .. start[g+1]))
     DevBuf ro_ws;             // deterministic readout backward: per-block partials of the weight gradients
+    DevBuf ro_kval;           // ggnn_readout_predict: the per-node gated values of every task [K][V]
+    bool ro_from_dataset = false;          // the map came with a dataset batch, whose graphs' dataset indices are ...
+    const int* ro_dataset_slots = nullptr;  // ... this device table [G] (in ds_table)
     DevBuf state_buf;   // intermediate layer states (L-1) + 2 ping-pong step buffers, each [V][D]
     DevBuf save_bufs;   // 5 (CudnnCompatibleGRUCell: 6) x total_steps x [V][D]
     DevBuf io_buf;      // h0 / h_out staging for ggnn_forward_host
@@ -1043,7 +1046,7 @@ int ggnn_destroy(ggnn_engine* e) {
     e->tc_tiles.buf.release(); e->tc_respre.release(); e->ts_tiles.buf.release(); e->ts_images.release(); e->ts_virt.release(); e->err_flag.release();
     e->step_wt.buf.release(); e->step_buf.release();
     if (e->own_prep) { ggnn_free_prepared_graph(e->own_prep); e->own_prep = nullptr; }
-    e->ro_buf.release(); e->ro_stage.release(); e->att_buf.release(); e->ro_ws.release();
+    e->ro_buf.release(); e->ro_stage.release(); e->att_buf.release(); e->ro_ws.release(); e->ro_kval.release();
     delete e;
     return GGNN_OK;
 }
@@ -2639,7 +2642,7 @@ int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* gr
     }
     if (node_mask) memcpy(base + e->ro_off_mask, node_mask, sizeof(float) * (size_t)V);
     CU_TRY(e, e->ro_stage.upload(e->ro_buf.ptr, grouped ? e->ro_off_perm : off, (cudaStream_t)stream));
-    e->ro_V = V; e->ro_G = G; e->ro_grouped = grouped; e->ro_has_mask = node_mask != nullptr;
+    e->ro_V = V; e->ro_G = G; e->ro_grouped = grouped; e->ro_has_mask = node_mask != nullptr; e->ro_from_dataset = false;
     return GGNN_OK;
 }
 
@@ -2653,31 +2656,79 @@ static int readout_check(ggnn_engine* e, const void* const* ptrs, int n) {
     return GGNN_OK;
 }
 
+}  // extern "C"
+
+// The readout forward of K tasks over the current map: stage 1 into val [K][V] (device scratch), stage 2 into out[k * stride + slot[g]].
+static int readout_run(ggnn_engine* e, const float* h_last, const float* h0, int K, const readout::TaskWeights& tw, const int* slot, int stride,
+                       float* out, float* val, cudaStream_t st) {
+    const int V = e->ro_V, G = e->ro_G;
+    char* g = (char*)e->ro_buf.ptr;
+    const float* mask = e->ro_has_mask ? (const float*)(g + e->ro_off_mask) : nullptr;
+    if (V > 0) {
+        if (K == 1) readout::readout_node_kernel<1><<<(V + 7) / 8, 256, 0, st>>>(h_last, h0, tw, K, mask, val, V, e->D);
+        else readout::readout_node_kernel<readout::MAX_TASKS><<<(V + 7) / 8, 256, 0, st>>>(h_last, h0, tw, K, mask, val, V, e->D);
+    }
+    const dim3 per_graph((G + 127) / 128, K);
+    if (e->ro_grouped || V == 0) {
+        readout::readout_sum_grouped_kernel<<<per_graph, 128, 0, st>>>(val, (const int*)(g + e->ro_off_start), slot, out, G, V, stride);
+    } else if (e->det) {
+        readout::readout_sum_permuted_kernel<<<per_graph, 128, 0, st>>>(val, (const int*)(g + e->ro_off_start), (const int*)(g + e->ro_off_perm),
+                                                                       slot, out, G, V, stride);
+    } else {
+        readout::readout_zero_kernel<<<per_graph, 128, 0, st>>>(slot, out, G, stride);
+        readout::readout_sum_atomic_kernel<<<dim3((V + 255) / 256, K), 256, 0, st>>>(val, (const int*)(g + e->ro_off_graph_of), slot, out, V,
+                                                                                      stride);
+    }
+    CU_TRY(e, cudaGetLastError());
+    return GGNN_OK;
+}
+
+extern "C" {
+
 int ggnn_readout_forward(ggnn_engine* e, const float* h_last, const float* h0, const float* w_gate, const float* b_gate,
                          const float* w_trans, const float* b_trans, float* out, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
     const void* ps[7] = {h_last, h0, w_gate, b_gate, w_trans, b_trans, out};
     if (int rc = readout_check(e, ps, e->ro_V > 0 ? 7 : 0)) return rc;
     CU_TRY(e, cudaSetDevice(e->device));
-    cudaStream_t st = (cudaStream_t)stream;
+    if (e->ro_G == 0) return GGNN_OK;
+    if (!out) return e->fail(GGNN_EINVAL, "null output");
+    readout::TaskWeights tw{};
+    tw.w[0] = readout::Weights{w_gate, b_gate, w_trans, b_trans};
+    return readout_run(e, h_last, h0, 1, tw, nullptr, e->ro_G, out, (float*)((char*)e->ro_buf.ptr + e->ro_off_val), (cudaStream_t)stream);
+}
+
+int ggnn_readout_predict(ggnn_engine* e, const float* h_last, const float* h0, int32_t num_tasks, const ggnn_readout_task* tasks,
+                         const int32_t* slot, int32_t out_stride, float* out, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    if (num_tasks < 1 || num_tasks > readout::MAX_TASKS)
+        return e->fail(GGNN_EINVAL, "num_tasks = %d: the readout runs 1 .. %d tasks per call", (int)num_tasks, readout::MAX_TASKS);
+    if (!tasks) return e->fail(GGNN_EINVAL, "null tasks");
+    const void* ps[2] = {h_last, h0};
+    if (int rc = readout_check(e, ps, e->ro_V > 0 ? 2 : 0)) return rc;
     const int V = e->ro_V, G = e->ro_G;
+    readout::TaskWeights tw{};
+    for (int k = 0; k < num_tasks; ++k) {
+        const void* w[4] = {tasks[k].w_gate, tasks[k].b_gate, tasks[k].w_trans, tasks[k].b_trans};
+        for (int i = 0; i < 4; ++i) {
+            if (!w[i]) return e->fail(GGNN_EINVAL, "task %d: null readout weight %d", k, i);
+            if ((i == 0 || i == 2) && ((uintptr_t)w[i] & 15)) return e->fail(GGNN_EINVAL, "task %d: readout weight %d must be 16-byte aligned", k, i);
+        }
+        tw.w[k] = readout::Weights{tasks[k].w_gate, tasks[k].b_gate, tasks[k].w_trans, tasks[k].b_trans};
+    }
     if (G == 0) return GGNN_OK;
     if (!out) return e->fail(GGNN_EINVAL, "null output");
-    char* g = (char*)e->ro_buf.ptr;
-    const float* mask = e->ro_has_mask ? (const float*)(g + e->ro_off_mask) : nullptr;
-    readout::Weights w{w_gate, b_gate, w_trans, b_trans};
-    float* val = (float*)(g + e->ro_off_val);
-    if (V > 0) readout::readout_node_kernel<<<(V + 7) / 8, 256, 0, st>>>(h_last, h0, w, mask, val, V, e->D);
-    if (e->ro_grouped || V == 0) {
-        readout::readout_sum_grouped_kernel<<<(G + 127) / 128, 128, 0, st>>>(val, (const int*)(g + e->ro_off_start), out, G);
-    } else if (e->det) {
-        readout::readout_sum_permuted_kernel<<<(G + 127) / 128, 128, 0, st>>>(val, (const int*)(g + e->ro_off_start), (const int*)(g + e->ro_off_perm),
-                                                                            out, G);
-    } else {
-        CU_TRY(e, cudaMemsetAsync(out, 0, sizeof(float) * (size_t)G, st));
-        readout::readout_sum_atomic_kernel<<<(V + 255) / 256, 256, 0, st>>>(val, (const int*)(g + e->ro_off_graph_of), out, V);
-    }
-    CU_TRY(e, cudaGetLastError());
+    if (out_stride < 1 || (!slot && out_stride < G))
+        return e->fail(GGNN_EINVAL, "out_stride = %d: without a slot map each task's row needs the batch's %d graphs", (int)out_stride, G);
+    CU_TRY(e, cudaSetDevice(e->device));
+    CU_TRY(e, e->ro_kval.reserve(sizeof(float) * (size_t)num_tasks * std::max(V, 1)));
+    return readout_run(e, h_last, h0, num_tasks, tw, slot, out_stride, out, (float*)e->ro_kval.ptr, (cudaStream_t)stream);
+}
+
+int ggnn_dataset_batch_slots(const ggnn_engine* e, const int32_t** slot) {
+    if (!e || !slot) return GGNN_EINVAL;
+    if (e->ro_V < 0 || !e->ro_from_dataset) return GGNN_ESTATE;
+    *slot = e->ro_dataset_slots;
     return GGNN_OK;
 }
 
@@ -2757,6 +2808,54 @@ int ggnn_run_sparse_host_readout(ggnn_engine* e, int32_t V, const int32_t* const
     CU_TRY(e, cudaStreamSynchronize(st));
     for (int t = 0; t < num_tasks; ++t) { loss_out[t] = res[t]; accuracy_out[t] = res[num_tasks + t]; }
     return GGNN_OK;
+}
+
+}  // extern "C"
+
+// The reference's evaluate_one_batch (sparse:352-362, dense:230-249) in one call: the upload and the forward without saving for backward
+// (the save flag is restored afterwards), the readout map, every task's readout into [num_tasks][G] on the device, one D2H copy.
+template <class SetGraph, class SetMap>
+static int run_host_predict(ggnn_engine* e, int64_t V, const float* h0_host, int32_t G, int32_t num_tasks, const ggnn_readout_task* tasks,
+                            float* out_host, cudaStream_t st, SetGraph set_graph, SetMap set_map) {
+    if (!e) return GGNN_EINVAL;
+    if (V < 0 || G < 0 || (V > 0 && !h0_host) || (G > 0 && !out_host)) return e->fail(GGNN_EINVAL, "null host pointer / negative size");
+    const size_t bytes = (size_t)V * e->D * sizeof(float), kg = (size_t)std::max(num_tasks, 1) * std::max(G, 1);
+    IoSlots io;
+    int rc = stage_io(e, h0_host, bytes, sizeof(float) * kg, st, io);
+    if (rc) return rc;
+    const bool save = e->save;
+    e->save = false;
+    rc = set_graph();
+    if (!rc && (int64_t)e->V != V) rc = e->fail(GGNN_EINVAL, "graph has %d nodes, h0 has %lld rows", e->V, (long long)V);
+    if (!rc) rc = set_map();
+    if (!rc) rc = ggnn_forward(e, io.in, io.out, (ggnn_stream_t)st);
+    e->save = save;
+    e->saved_valid = false;
+    if (rc) return rc;
+    float* res = (float*)io.scratch;
+    rc = ggnn_readout_predict(e, io.out, io.in, num_tasks, tasks, nullptr, G, res, (ggnn_stream_t)st);
+    if (rc) return rc;
+    if (G > 0) CU_TRY(e, cudaMemcpyAsync(out_host, res, sizeof(float) * (size_t)num_tasks * G, cudaMemcpyDeviceToHost, st));
+    CU_TRY(e, cudaStreamSynchronize(st));
+    return GGNN_OK;
+}
+
+extern "C" {
+
+int ggnn_run_sparse_host_predict(ggnn_engine* e, int32_t V, const int32_t* const* adjacency_lists, const int32_t* num_edges, const float* indeg,
+                                 const float* h0_host, const int32_t* graph_nodes_list, int32_t G, int32_t num_tasks,
+                                 const ggnn_readout_task* tasks, float* out_host, ggnn_stream_t stream) {
+    if (e && V > 0 && !graph_nodes_list) return e->fail(GGNN_EINVAL, "null graph_nodes_list");
+    return run_host_predict(e, V, h0_host, G, num_tasks, tasks, out_host, (cudaStream_t)stream,
+                            [&]() { return ggnn_set_graph_sparse(e, V, adjacency_lists, num_edges, indeg, stream); },
+                            [&]() { return ggnn_readout_set_graphs(e, V, graph_nodes_list, G, 0, nullptr, stream); });
+}
+
+int ggnn_run_dense_host_predict(ggnn_engine* e, int32_t b, int32_t v, const float* adjacency_matrix, const float* h0_host, const float* node_mask,
+                                int32_t num_tasks, const ggnn_readout_task* tasks, float* out_host, ggnn_stream_t stream) {
+    return run_host_predict(e, (int64_t)b * v, h0_host, b, num_tasks, tasks, out_host, (cudaStream_t)stream,
+                            [&]() { return ggnn_set_graph_dense(e, b, v, adjacency_matrix, stream); },
+                            [&]() { return ggnn_readout_set_graphs(e, b * v, nullptr, b, v, node_mask, stream); });
 }
 
 int ggnn_sync_check(ggnn_engine* e, ggnn_stream_t stream) {
@@ -2890,8 +2989,8 @@ struct ggnn_dataset_batch : ErrorText {
     size_t bytes = 0;
     int G = 0;
     int v = 0;               // a dense batch's rows per graph; 0 for sparse and GCN batches
-    StagedImage table;       // tile starts [ntiles + 1] | the per-graph records [G][R_MBASE + T] (16-byte aligned)
-    size_t table_bytes = 0, off_records = 0;
+    StagedImage table;       // tile starts [ntiles + 1] | the per-graph records [G][R_MBASE + T] | the graphs' dataset indices [G] (16-byte aligned)
+    size_t table_bytes = 0, off_records = 0, off_slots = 0;
     bool valid = false;
 };
 
@@ -2996,7 +3095,8 @@ static int ds_finish(ggnn_dataset* d, DsHost& h, const float* ann, const float* 
                             {ann, nann * sizeof(float), (const void**)&a.ann}, {labels, nlab * sizeof(float), (const void**)&a.labels},
                             {lmask, nlab * sizeof(float), (const void**)&a.lmask}, I(h.nfeat, &a.nfeat)};
     const bool present[] = {true, true, true, true, true, true, d->train, d->train, d->train && d->shape.use_att, d->stream_tables,
-                            d->stream_tables, d->stream_tables, d->stream_tables, d->weighted, d->weighted && d->train, true, true, true, d->dense};
+                            d->stream_tables, d->stream_tables, d->stream_tables, d->weighted, d->weighted && d->train, true, d->tasks > 0,
+                            d->tasks > 0, d->dense};
     size_t total = 0;
     for (const Section& s : secs) total = align_up(total + s.bytes, 16);
     std::vector<char> image(total);
@@ -3233,6 +3333,7 @@ static int prepare_dataset_batch(const ggnn_dataset* d, int32_t save_for_backwar
     v = b->v;
     const bool save = save_for_backward != 0;
     if (save && !d->train) return b->fail(GGNN_ESTATE, "save_for_backward needs a dataset created for training (the source-keyed CSR is built there)");
+    if (save && d->tasks == 0) return b->fail(GGNN_EINVAL, "the dataset has no targets: its batches can be predicted, not trained on");
     const int T = d->shape.T, G = num_graphs;
     for (int i = 0; i < G; ++i)
         if (graph_ids[i] < 0 || graph_ids[i] >= d->N)
@@ -3285,7 +3386,8 @@ static int prepare_dataset_batch(const ggnn_dataset* d, int32_t save_for_backwar
     // the batch table: tile starts, then per graph its id, offsets and per-type message bases (type base of the batch + earlier graphs')
     const int rec = ds::R_MBASE + T;
     b->off_records = align_up(sizeof(int) * tile_start.size(), 16);
-    b->table_bytes = b->off_records + sizeof(int) * (size_t)rec * G;
+    b->off_slots = align_up(b->off_records + sizeof(int) * (size_t)rec * G, 16);
+    b->table_bytes = b->off_slots + sizeof(int) * (size_t)G;
     CU_TRY(b, b->table.begin(std::max<size_t>(b->table_bytes, 16)));
     memcpy(b->table.ptr, tile_start.data(), sizeof(int) * tile_start.size());
     int* r = (int*)(b->table.ptr + b->off_records);
@@ -3301,6 +3403,8 @@ static int prepare_dataset_batch(const ggnn_dataset* d, int32_t save_for_backwar
         }
         node += v > 0 ? v : g.V; slot += g.M; vrow += g.nv; vs += g.nvm;
     }
+    int* slots = (int*)(b->table.ptr + b->off_slots);   // the slot map of ggnn_readout_predict: batch graph i -> its dataset index
+    for (int i = 0; i < G; ++i) slots[i] = (int)graph_ids[i];
     b->G = G;
     b->valid = true;
     return GGNN_OK;
@@ -3380,6 +3484,7 @@ static int set_graph_dataset(ggnn_engine* e, ggnn_dataset_batch* b, float* h0, f
     CU_TRY(e, cudaGetLastError());
     if (int rc = bind_graph(e)) return rc;
     e->ro_V = q.V; e->ro_G = b->G; e->ro_grouped = true; e->ro_has_mask = dense;
+    e->ro_from_dataset = true; e->ro_dataset_slots = (const int*)((const char*)e->ds_table.ptr + b->off_slots);
     return GGNN_OK;
 }
 

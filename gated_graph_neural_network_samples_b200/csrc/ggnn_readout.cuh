@@ -2,9 +2,9 @@
 //   val[v]  = sigmoid([h_T[v] | h_0[v]] . w_gate + b_gate) * (h_T[v] . w_trans + b_trans) * mask[v]
 //   out[g]  = sum of val over the nodes of graph g          (tf.unsorted_segment_sum / masked reduce_sum)
 // The reference's readout MLPs have no hidden layers (chem_tensorflow.py:153-157), so each is one affine map to a scalar.
-// Forward: one warp per node computes val[v] (every node row read once, float4), then one thread per graph adds its nodes in
-// order (the serial order of TF's CPU segment sum, deterministic); node lists not grouped by graph take an atomicAdd stage (in deterministic
-// mode, the same per-graph order through a by-graph permutation).  Backward: one warp per node recomputes the two dot products, writes d h_T,
+// Forward, for K tasks at once: one warp per node computes val[k][v] for every task (every node row read once, float4), then one thread
+// per graph and task adds its nodes in order (the serial order of TF's CPU segment sum, deterministic); node lists not grouped by graph
+// take an atomicAdd stage (in deterministic mode, the same per-graph order through a by-graph permutation).  Backward: one warp per node recomputes the two dot products, writes d h_T,
 // accumulates the weight gradients in registers and reduces them per block.
 #pragma once
 #include "ggnn_common.cuh"
@@ -42,54 +42,88 @@ __device__ __forceinline__ void node_dots(const float* __restrict__ hT, const fl
     trans_pre = warp_sum(t) + w.b_trans[0];
 }
 
-// stage 1: one warp per node -> val[v]   (fully parallel; the node rows are read exactly once, 16 bytes per lane)
-__global__ void __launch_bounds__(256) readout_node_kernel(const float* __restrict__ h_last, const float* __restrict__ h0, Weights w,
-                                                           const float* __restrict__ mask, float* __restrict__ val, int V, int D) {
+// The forward runs K tasks at once (ggnn_readout_predict; ggnn_readout_forward is K = 1).  Up to MAX_TASKS of them: stage 1 keeps two
+// accumulators per task in registers, and the kernel parameters carry every task's four weight pointers.
+constexpr int MAX_TASKS = 16;
+struct TaskWeights {
+    Weights w[MAX_TASKS];
+};
+
+// stage 1: one warp per node -> val[k][v] for the K <= KMAX tasks.  The node's h_T and h_0 rows are read exactly once, 16 bytes per
+// lane, whatever K is; per task the arithmetic (lane order, products, warp_sum, sigmoid, mask) is that of a single-task pass.
+// val: [K][V], task-major.
+template <int KMAX>
+__global__ void __launch_bounds__(256) readout_node_kernel(const float* __restrict__ h_last, const float* __restrict__ h0, const TaskWeights tw,
+                                                           int K, const float* __restrict__ mask, float* __restrict__ val, int V, int D) {
     const int v = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (v >= V) return;
     const float4* hT = reinterpret_cast<const float4*>(h_last + (size_t)v * D);
     const float4* hz = reinterpret_cast<const float4*>(h0 + (size_t)v * D);
-    const float4* wa = reinterpret_cast<const float4*>(w.w_gate);
-    const float4* wb = reinterpret_cast<const float4*>(w.w_gate + D);
-    const float4* wt = reinterpret_cast<const float4*>(w.w_trans);
-    float g = 0.f, t = 0.f;
+    float g[KMAX], t[KMAX];
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) g[k] = t[k] = 0.f;
     for (int q = lane; q < (D >> 2); q += 32) {
-        const float4 a = hT[q], z = hz[q], ga = wa[q], gb = wb[q], tt = wt[q];
-        g += a.x * ga.x + a.y * ga.y + a.z * ga.z + a.w * ga.w + z.x * gb.x + z.y * gb.y + z.z * gb.z + z.w * gb.w;
-        t += a.x * tt.x + a.y * tt.y + a.z * tt.z + a.w * tt.w;
+        const float4 a = hT[q], z = hz[q];
+#pragma unroll
+        for (int k = 0; k < KMAX; ++k) {
+            if (k < K) {
+                const float4 ga = reinterpret_cast<const float4*>(tw.w[k].w_gate)[q], gb = reinterpret_cast<const float4*>(tw.w[k].w_gate + D)[q];
+                const float4 tt = reinterpret_cast<const float4*>(tw.w[k].w_trans)[q];
+                g[k] += a.x * ga.x + a.y * ga.y + a.z * ga.z + a.w * ga.w + z.x * gb.x + z.y * gb.y + z.z * gb.z + z.w * gb.w;
+                t[k] += a.x * tt.x + a.y * tt.y + a.z * tt.z + a.w * tt.w;
+            }
+        }
     }
-    g = warp_sum(g) + w.b_gate[0];
-    t = warp_sum(t) + w.b_trans[0];
-    float r = sigmoidf_acc(g) * t;
-    if (mask) r *= mask[v];
-    if (lane == 0) val[v] = r;
+    const float m = mask ? mask[v] : 1.0f;
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) {
+        if (k < K) {
+            const float gs = warp_sum(g[k]) + tw.w[k].b_gate[0];
+            const float ts = warp_sum(t[k]) + tw.w[k].b_trans[0];
+            float r = sigmoidf_acc(gs) * ts;
+            if (mask) r *= m;
+            if (lane == 0) val[(size_t)k * V + v] = r;
+        }
+    }
+}
+
+// Stage 2 writes task k of batch graph g to out[k * stride + slot[g]] (slot NULL: g).  blockIdx.y is the task.
+__device__ __forceinline__ size_t out_index(const int* __restrict__ slot, int g, int k, int stride) {
+    return (size_t)k * stride + (slot ? slot[g] : g);
 }
 // stage 2, graphs grouped: graph g owns nodes [graph_start[g], graph_start[g+1]); summed in node order (deterministic, the order of
 // TF's CPU unsorted_segment_sum)
 __global__ void __launch_bounds__(128) readout_sum_grouped_kernel(const float* __restrict__ val, const int* __restrict__ graph_start,
-                                                                  float* __restrict__ out, int G) {
-    const int g = blockIdx.x * 128 + threadIdx.x;
+                                                                  const int* __restrict__ slot, float* __restrict__ out, int G, int V, int stride) {
+    const int g = blockIdx.x * 128 + threadIdx.x, k = blockIdx.y;
     if (g >= G) return;
+    const float* vk = val + (size_t)k * V;
     float acc = 0.f;
-    for (int v = graph_start[g]; v < graph_start[g + 1]; ++v) acc += val[v];
-    out[g] = acc;
+    for (int v = graph_start[g]; v < graph_start[g + 1]; ++v) acc += vk[v];
+    out[out_index(slot, g, k, stride)] = acc;
 }
-// stage 2, arbitrary graph_of[v]: out must be zeroed by the caller
+// stage 2, arbitrary graph_of[v]: readout_zero_kernel first clears the outputs
+__global__ void __launch_bounds__(128) readout_zero_kernel(const int* __restrict__ slot, float* __restrict__ out, int G, int stride) {
+    const int g = blockIdx.x * 128 + threadIdx.x;
+    if (g < G) out[out_index(slot, g, blockIdx.y, stride)] = 0.f;
+}
 __global__ void __launch_bounds__(256) readout_sum_atomic_kernel(const float* __restrict__ val, const int* __restrict__ graph_of,
-                                                                 float* __restrict__ out, int V) {
-    const int v = blockIdx.x * 256 + threadIdx.x;
-    if (v < V) atomicAdd(out + graph_of[v], val[v]);
+                                                                 const int* __restrict__ slot, float* __restrict__ out, int V, int stride) {
+    const int v = blockIdx.x * 256 + threadIdx.x, k = blockIdx.y;
+    if (v < V) atomicAdd(out + out_index(slot, graph_of[v], k, stride), val[(size_t)k * V + v]);
 }
 
 // stage 2 of an ungrouped graph_of[v] in deterministic mode: graph g owns positions [graph_start[g], graph_start[g+1]) of the stable by-graph
 // permutation `perm` (node index order inside a graph), summed in that order -- the grouped kernel's order, through one indirection
 __global__ void __launch_bounds__(128) readout_sum_permuted_kernel(const float* __restrict__ val, const int* __restrict__ graph_start,
-                                                                   const int* __restrict__ perm, float* __restrict__ out, int G) {
-    const int g = blockIdx.x * 128 + threadIdx.x;
+                                                                   const int* __restrict__ perm, const int* __restrict__ slot,
+                                                                   float* __restrict__ out, int G, int V, int stride) {
+    const int g = blockIdx.x * 128 + threadIdx.x, k = blockIdx.y;
     if (g >= G) return;
+    const float* vk = val + (size_t)k * V;
     float acc = 0.f;
-    for (int i = graph_start[g]; i < graph_start[g + 1]; ++i) acc += val[perm[i]];
-    out[g] = acc;
+    for (int i = graph_start[g]; i < graph_start[g + 1]; ++i) acc += vk[perm[i]];
+    out[out_index(slot, g, k, stride)] = acc;
 }
 
 // d_out[G] -> d_h_last[V,D] (written), d_w_gate[2D] / d_b_gate[1] / d_w_trans[D] / d_b_trans[1].

@@ -329,7 +329,7 @@ class DeviceDataset:
             err = GgnnError(self.lib.ggnn_dataset_batch_error(h).decode() if h.value else "invalid argument")
             err.code = rc
             raise err
-        b.dataset, b.G = self, ids.shape[0]
+        b.dataset, b.G, b.ids = self, ids.shape[0], ids
         b.V = b.info()["num_nodes"]
         b.nodes_per_graph = int(nodes_per_graph) if self.dense else 0
         return b
@@ -354,6 +354,10 @@ class DatasetBatch:
         self.dataset = dataset   # the dataset must outlive its batches
         self._h = C.c_void_p()
         self.V = self.G = self.nodes_per_graph = 0
+        self.ids = np.zeros(0, np.int64)   # the batch's graphs' dataset indices, in batch order
+        # the same ids as the engine's DEVICE int32 table [G] once the batch is adopted (set_graph_from_dataset): the slot map with which
+        # readout_predict writes each graph's predictions at its dataset index; valid until the engine's next graph upload
+        self.slot_table = None
 
     def info(self) -> dict:
         V, M, nt, nb, st = C.c_int32(), C.c_int64(), C.c_int32(), C.c_int64(), C.c_int32()
@@ -519,6 +523,9 @@ class PropagationEngine:
         self._graph_keepalive = (batch,)
         self._readout_keepalive = None
         self._readout_shape = (batch.V, batch.G)
+        slots = C.c_void_p()
+        self._check(self.lib.ggnn_dataset_batch_slots(self._h, C.byref(slots)))
+        batch.slot_table = slots.value
         return (h0, tv, tm, mask) if batch.dataset.dense else (h0, tv, tm)
 
     def graph_image(self) -> np.ndarray:
@@ -558,10 +565,7 @@ class PropagationEngine:
         tm = np.ascontiguousarray(np.asarray(target_mask, dtype=np.float32).reshape(nt, G))
         if h0.size != V * self.D or gnl.shape[0] != V:
             raise GgnnError("h0 / graph_nodes_list do not match the %d nodes of the graph" % V)
-        arr = (_lib.GgnnReadoutTask * nt)()
-        for i, (wg, bg, wt, bt) in enumerate(readout_tasks):
-            arr[i].w_gate, arr[i].b_gate = self._f32(wg, 2 * self.D, "w_gate"), self._f32(bg, 1, "b_gate")
-            arr[i].w_trans, arr[i].b_trans = self._f32(wt, self.D, "w_trans"), self._f32(bt, 1, "b_trans")
+        arr = self._readout_tasks(readout_tasks)
         loss, acc = np.empty(nt, np.float32), np.empty(nt, np.float32)
         self.serial += 1
         self._check(self.lib.ggnn_run_sparse_host_readout(self._h, V, ptrs, counts, indeg.ctypes.data, h0.ctypes.data, gnl.ctypes.data, G, nt, arr,
@@ -569,6 +573,54 @@ class PropagationEngine:
         self.V = V
         self._graph_keepalive = (adjs, indeg)
         return loss, acc
+
+    def _readout_tasks(self, readout_tasks):
+        """``ggnn_readout_task[]`` of ``(w_gate [2D], b_gate [1], w_trans [D], b_trans [1])`` CUDA tensors, one tuple per task."""
+        arr = (_lib.GgnnReadoutTask * len(readout_tasks))()
+        for i, (wg, bg, wt, bt) in enumerate(readout_tasks):
+            arr[i].w_gate, arr[i].b_gate = self._f32(wg, 2 * self.D, "w_gate"), self._f32(bg, 1, "b_gate")
+            arr[i].w_trans, arr[i].b_trans = self._f32(wt, self.D, "w_trans"), self._f32(bt, 1, "b_trans")
+        return arr
+
+    def run_sparse_host_predict(self, adjacency_lists, num_incoming_edges_per_type, h0, graph_nodes_list, num_graphs, readout_tasks) -> np.ndarray:
+        """``sess.run(self.output, feed)`` of the reference's evaluate_one_batch (sparse:352-362) for every task in one call: the batch in
+        HOST arrays without targets, the readout trainables as for ``run_sparse_host_readout``; returns ``[tasks, num_graphs]`` (HOST)."""
+        adjs, indeg, ptrs, counts = self._sparse_args(adjacency_lists, num_incoming_edges_per_type)
+        V, G = indeg.shape[0], int(num_graphs)
+        h0 = np.ascontiguousarray(h0, dtype=np.float32)
+        gnl = np.ascontiguousarray(np.asarray(graph_nodes_list, dtype=np.int32).reshape(-1))
+        if h0.size != V * self.D or gnl.shape[0] != V:
+            raise GgnnError("h0 / graph_nodes_list do not match the %d nodes of the graph" % V)
+        arr = self._readout_tasks(readout_tasks)
+        out = np.empty((len(readout_tasks), G), np.float32)
+        self.serial += 1
+        self._check(self.lib.ggnn_run_sparse_host_predict(self._h, V, ptrs, counts, indeg.ctypes.data, h0.ctypes.data, gnl.ctypes.data, G,
+                                                          len(readout_tasks), arr, out.ctypes.data, self._stream()))
+        self.V = V
+        self._graph_keepalive = (adjs, indeg)
+        self._readout_shape = (V, G)
+        return out
+
+    def run_dense_host_predict(self, adjacency_matrix, h0, node_mask, readout_tasks) -> np.ndarray:
+        """The dense evaluate_one_batch (dense:230-249) in one call: ``[b, T, v, v]`` adjacency, ``h0 [b*v, D]`` and ``node_mask [b, v]``
+        HOST arrays; returns ``[tasks, b]`` (HOST)."""
+        a = np.ascontiguousarray(np.asarray(adjacency_matrix, dtype=np.float32))
+        if a.ndim != 4 or a.shape[1] != self.T or a.shape[2] != a.shape[3]:
+            raise GgnnError("adjacency_matrix must be [b, %d, v, v]" % self.T)
+        b, v = a.shape[0], a.shape[2]
+        h0 = np.ascontiguousarray(h0, dtype=np.float32)
+        mask = np.ascontiguousarray(np.asarray(node_mask, dtype=np.float32).reshape(-1))
+        if h0.size != b * v * self.D or mask.shape[0] != b * v:
+            raise GgnnError("h0 / node_mask do not match the %d x %d nodes of the batch" % (b, v))
+        arr = self._readout_tasks(readout_tasks)
+        out = np.empty((len(readout_tasks), b), np.float32)
+        self.serial += 1
+        self._check(self.lib.ggnn_run_dense_host_predict(self._h, b, v, a.ctypes.data, h0.ctypes.data, mask.ctypes.data, len(readout_tasks), arr,
+                                                         out.ctypes.data, self._stream()))
+        self.V = b * v
+        self._graph_keepalive = (a,)
+        self._readout_shape = (b * v, b)
+        return out
 
     def run_dense_host(self, adjacency_matrix: np.ndarray, h0: np.ndarray, out: Optional[np.ndarray] = None) -> np.ndarray:
         a = np.ascontiguousarray(np.asarray(adjacency_matrix, dtype=np.float32))
@@ -702,6 +754,32 @@ class PropagationEngine:
         self._check(self.lib.ggnn_readout_forward(
             self._h, self._f32(h_last, V * D, "h_last"), self._f32(h0, V * D, "h0"), self._f32(w_gate, 2 * D, "w_gate"), self._f32(b_gate, 1, "b_gate"),
             self._f32(w_trans, D, "w_trans"), self._f32(b_trans, 1, "b_trans"), out.data_ptr(), self._stream()))
+        return out
+
+    def readout_predict(self, h_last, h0, readout_tasks, slot=None, out=None, out_stride: Optional[int] = None):
+        """``ggnn_readout_predict``: every task's readout over the current map in one pass over the node rows.  ``readout_tasks``: one
+        ``(w_gate, b_gate, w_trans, b_trans)`` tuple of CUDA tensors per task (at most 16).  Task k of batch graph g goes to
+        ``out.view(-1)[k * out_stride + slot[g]]``: ``slot`` None (slot[g] = g), an int32 CUDA tensor [G], or a device address such as
+        ``DatasetBatch.slot_table``.  ``out`` defaults to a new ``[tasks, G]`` tensor; returns it."""
+        import torch
+        V, G = self._readout_shape
+        D, K = self.D, len(readout_tasks)
+        if out is None:
+            out = torch.empty(K, G, dtype=torch.float32, device=h_last.device)
+            out_stride = G
+        if not (out.is_cuda and out.is_contiguous() and out.dtype == torch.float32):
+            raise GgnnError("out must be a contiguous fp32 CUDA tensor")
+        stride = G if out_stride is None else int(out_stride)
+        if torch.is_tensor(slot):
+            if not (slot.is_cuda and slot.dtype == torch.int32 and slot.is_contiguous() and slot.numel() == G):
+                raise GgnnError("slot must be a contiguous int32 CUDA tensor with %d elements" % G)
+            slot_ptr = slot.data_ptr()
+        else:
+            slot_ptr = slot
+        if G and out.numel() < (K - 1) * stride + 1:
+            raise GgnnError("out has %d elements for %d tasks at stride %d" % (out.numel(), K, stride))
+        self._check(self.lib.ggnn_readout_predict(self._h, self._f32(h_last, V * D, "h_last"), self._f32(h0, V * D, "h0"), K,
+                                                  self._readout_tasks(readout_tasks), slot_ptr, stride, out.data_ptr(), self._stream()))
         return out
 
     def readout_backward(self, h_last, h0, w_gate, b_gate, w_trans, b_trans, d_out):

@@ -44,13 +44,14 @@ def graph_to_adjacency_lists(graph: Sequence[Sequence[int]], tie_fwd_bkwd: bool 
     return adj, indeg
 
 
-def process_raw_graphs_sparse(raw_data: Iterable[dict], task_ids=(0,), tie_fwd_bkwd: bool = True) -> List[dict]:
-    """sparse:234-252 without the training-time shuffle / task sub-sampling (caller's business)."""
+def process_raw_graphs_sparse(raw_data: Iterable[dict], task_ids=(0,), tie_fwd_bkwd: bool = True, labels: bool = True) -> List[dict]:
+    """sparse:234-252 without the training-time shuffle / task sub-sampling (caller's business).  ``labels=False``: graphs to predict,
+    which need no ``"targets"`` key -- every graph gets an empty label list (batches of them have ``[0, G]`` targets)."""
     out = []
     for d in raw_data:
         adj, indeg = graph_to_adjacency_lists(d["graph"], tie_fwd_bkwd)
         out.append({"adjacency_lists": adj, "num_incoming_edge_per_type": indeg, "init": d["node_features"],
-                    "labels": [d["targets"][t][0] for t in task_ids]})
+                    "labels": [d["targets"][t][0] for t in task_ids] if labels else []})
     return out
 
 
@@ -284,6 +285,18 @@ class FlatDenseGraphs:
                     self.mask[i, k] = 1.0
 
 
+def bucket_batches(raw_graphs: Sequence[dict], batch_size: int, bucket_sizes=DEFAULT_BUCKET_SIZES):
+    """The dense model's bucketing (dense:132-141) for prediction: ``(bucket size, input indices)`` of every batch -- each bucket's graphs
+    in input order, cut into batches of at most ``batch_size`` graphs, the last one short (training drops it, dense:159-160; a prediction
+    needs every graph).  Reads no ``"targets"``: pack the batches with ``pack_dense_batch(..., task_ids=())``."""
+    by_bucket: Dict[int, List[int]] = {}
+    for i, d in enumerate(raw_graphs):
+        by_bucket.setdefault(choose_bucket(d["graph"], bucket_sizes), []).append(i)
+    for b, idx in by_bucket.items():
+        for s in range(0, len(idx), batch_size):
+            yield int(bucket_sizes[b]), np.asarray(idx[s:s + batch_size], np.int64)
+
+
 def choose_bucket(graph, bucket_sizes=DEFAULT_BUCKET_SIZES) -> int:
     """dense:138-140 -- first bucket strictly larger than the largest node id."""
     g = np.asarray(graph).reshape(-1, 3)
@@ -307,13 +320,14 @@ def graph_to_gcn_adjacency(graph, num_nodes: int):
     return np.stack([i, j], axis=1).astype(np.int64).reshape(-1, 2), a[i, j]
 
 
-def process_raw_graphs_gcn(raw_data: Iterable[dict], task_ids=(0,)) -> List[dict]:
-    """chem_tensorflow_gcn.py:96-103 without the training-time shuffle / task sub-sampling (caller's business)."""
+def process_raw_graphs_gcn(raw_data: Iterable[dict], task_ids=(0,), labels: bool = True) -> List[dict]:
+    """chem_tensorflow_gcn.py:96-103 without the training-time shuffle / task sub-sampling (caller's business).  ``labels=False`` as for
+    ``process_raw_graphs_sparse``."""
     out = []
     for d in raw_data:
         lst, w = graph_to_gcn_adjacency(d["graph"], len(d["node_features"]))
         out.append({"adjacency_list": lst, "adjacency_weights": w, "init": d["node_features"],
-                    "labels": [d["targets"][t][0] for t in task_ids]})
+                    "labels": [d["targets"][t][0] for t in task_ids] if labels else []})
     return out
 
 

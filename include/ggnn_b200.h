@@ -227,6 +227,29 @@ int ggnn_run_sparse_host_readout(ggnn_engine* e, int32_t num_nodes, const int32_
                                  int32_t num_graphs, int32_t num_tasks, const ggnn_readout_task* tasks, const float* target_values,
                                  const float* target_mask, float* loss_out, float* accuracy_out, ggnn_stream_t stream);
 
+/* ---- Prediction: every task's readout in one pass over the node rows (the reference's evaluate_one_batch, sparse:352-362 / dense:230-249,
+ * fetches self.output; here all tasks come back).  Over the current readout map (ggnn_readout_set_graphs or a dataset batch), task k of batch
+ * graph g is written to out[k * out_stride + slot[g]]:
+ *   slot      DEVICE int32 [num_graphs], or NULL for slot[g] = g (out_stride >= num_graphs then).  Each task's values are those
+ *             ggnn_readout_forward computes with that task's weights, bit for bit when the sums are ordered (grouped node lists, or
+ *             ggnn_set_deterministic).  Entries must be distinct and below out_stride: nothing else of `out` is written.
+ *   tasks     1 .. 16 tasks (more is GGNN_EINVAL), DEVICE weights as for ggnn_readout_forward (w_gate / w_trans 16-byte aligned).
+ * ggnn_dataset_batch_slots: the slot table of the dataset batch the engine adopted last -- its graphs' dataset indices [G], DEVICE, valid
+ * until the next graph upload -- so that a whole dataset's predictions land in one [num_tasks, N] buffer; GGNN_ESTATE when the current
+ * readout map did not come from a dataset batch.
+ * ggnn_run_sparse_host_predict / ggnn_run_dense_host_predict: one synchronous call per batch with HOST buffers and no targets, the shape of
+ * sess.run(self.output, feed) -- upload, the forward without saving for backward, the readout map (sparse: graph_nodes_list [V]; dense:
+ * num_graphs x num_vertices with node_mask [b*v]), every task, and out_host [num_tasks, num_graphs] back. */
+int ggnn_readout_predict(ggnn_engine* e, const float* h_last, const float* h0, int32_t num_tasks, const ggnn_readout_task* tasks,
+                         const int32_t* slot, int32_t out_stride, float* out, ggnn_stream_t stream);
+int ggnn_dataset_batch_slots(const ggnn_engine* e, const int32_t** slot);
+int ggnn_run_sparse_host_predict(ggnn_engine* e, int32_t num_nodes, const int32_t* const* adjacency_lists, const int32_t* num_edges,
+                                 const float* num_incoming_edges_per_type, const float* h0_host, const int32_t* graph_nodes_list,
+                                 int32_t num_graphs, int32_t num_tasks, const ggnn_readout_task* tasks, float* out_host, ggnn_stream_t stream);
+int ggnn_run_dense_host_predict(ggnn_engine* e, int32_t num_graphs, int32_t num_vertices, const float* adjacency_matrix, const float* h0_host,
+                                const float* node_mask, int32_t num_tasks, const ggnn_readout_task* tasks, float* out_host,
+                                ggnn_stream_t stream);
+
 /* Synchronises `stream` and reports asynchronous kernel-side failures (a bounded barrier wait that expired). */
 int ggnn_sync_check(ggnn_engine* e, ggnn_stream_t stream);
 
@@ -384,8 +407,9 @@ const char* ggnn_dataset_error(const ggnn_dataset* d);
  *   ggnn_dataset_prepare_batch   host only, from the dataset's summaries (no edge is read, the device is not touched but for the pinned
  *                                table): the batch of graph_ids [num_graphs] (int64 dataset indices, in batch order; an id out of range is
  *                                GGNN_ERANGE) -- its offsets, its cut points through the same tile planner, the image layout -- and a small
- *                                pinned table of tile starts and per-graph offsets.  Reads the dataset and nothing else: callable from a
- *                                producer thread.  save_for_backward 1 needs a training dataset.  *inout as for ggnn_prepare_graph_sparse
+ *                                pinned table of tile starts, per-graph offsets and the graph ids (ggnn_dataset_batch_slots).  Reads the
+ *                                dataset and nothing else: callable from a producer thread.  save_for_backward 1 needs a training dataset
+ *                                with targets (a dataset created with num_tasks = 0 is for prediction: GGNN_EINVAL).  *inout as for ggnn_prepare_graph_sparse
  *                                (a rebuilt batch first waits for its previous table upload).
  *   ggnn_set_graph_dataset       engine thread: adopts the plan and enqueues on `stream` the table upload and the kernels that write the
  *                                batch's graph image into the engine's graph buffer, h0 [V, D] (the annotation columns, zeros elsewhere),
