@@ -36,6 +36,7 @@ struct ImageView {
     unsigned* tile_mask;
     int *trow, *ttgt, *tslot;                  // source-keyed CSR (save_for_backward); tslot: attention only
     int *pair, *vptr, *vsrc, *tvp, *vinfo;     // streaming plan
+    int* vslot;                                // weighted streaming plan: first target-CSR slot of every virtual row
     float *slotw, *tslotw;                     // weighted batches: per-slot weights in target-CSR / source-CSR order
 };
 

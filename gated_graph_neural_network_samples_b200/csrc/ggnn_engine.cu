@@ -171,6 +171,7 @@ struct BatchPlan {
     bool has_transpose = false;
     size_t off_tslot = 0;            // source-keyed CSR entry -> target-CSR slot (attention backward)
     size_t off_pair = 0, off_vptr = 0, off_vsrc = 0, off_tvp = 0, off_vinfo = 0;   // streaming plan: (target,type) -> source table, virtual rows (pairs with several messages)
+    size_t off_vslot = 0;   // weighted streaming plan: the first target-CSR slot of every virtual row (its weights are slot_w[vslot[vid] + m])
     size_t off_slotw = 0, off_tslotw = 0;   // weighted: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
 };
 
@@ -491,10 +492,11 @@ int pack_to_fill_chip(const std::vector<int>& cuts, int V, int max_span, int num
 }
 
 // The tile plan of a batch of V nodes: which kernel, and the tiles.  `cuts` are the sorted node indices where the batch may be split
-// between connected components (cuts.front() == 0, cuts.back() == V); `weighted`: every message has a weight.  Starts `p` afresh; the image
-// builders fill in the rest.
+// between connected components (cuts.front() == 0, cuts.back() == V); `weighted`: every message has a weight; `stream_weighted`: a weighted
+// batch may take the streaming plan above hidden 128 on the tensor-core precisions (the ..._dense_weighted entries), else it is refused
+// there.  Starts `p` afresh; the image builders fill in the rest.
 int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>& cuts, BatchPlan& p, std::vector<int>& tile_start,
-               std::string& err) {
+               std::string& err, bool stream_weighted = false) {
     p = BatchPlan();
     p.V = V;
     p.weighted = weighted;
@@ -526,13 +528,16 @@ int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>
         const char* fs = getenv("GGNN_TC_STREAM");
         // a component larger than a tile cannot use the tile-local fused kernel: the streaming plan beats one launch per timestep of that
         // kernel (cfg5 on an H100: 0.77 vs 0.94 ms), so it is the default there; GGNN_TC_STREAM=0/1 and GGNN_FORCE_GLOBAL=1 override.
-        // The streaming kernels sum unweighted messages only: a weighted batch stays on the tile kernel.
+        // A weighted batch streams only above hidden 128, where the tile kernel cannot run, and only when its caller asked for it; up to 128 it
+        // keeps the tile kernel's plans (GLOBAL for a component over 128 rows), on which every pair is gathered with its weights and none
+        // becomes a virtual row.
         const bool big_component = max_span > tc::TILE_M && !weighted && !force_global && !(fs && fs[0] == '0');
         if (s.DP > 128 || big_component || (fs && fs[0] == '1' && !weighted)) {
             // streaming plan: fixed 128-row tiles (the gather reads the previous state from L2, so tiles need not respect components),
             // one launch per GEMM of a timestep; N blocks sized so that small batches still spread over the chip
-            if (weighted) {
-                err = "hidden_size > 128 on the tensor-core path needs unweighted messages (a weighted dense adjacency runs on GGNN_PREC_FP32)";
+            if (weighted && !stream_weighted) {
+                err = "hidden_size > 128 on the tensor-core path needs unweighted messages here (a weighted dense adjacency runs on GGNN_PREC_FP32, "
+                      "or on the streaming wgmma kernels through ggnn_set_graph_dense_weighted / ggnn_prepare_graph_dense_weighted)";
                 return GGNN_EUNSUPPORTED;
             }
             p.stream = true; p.variant = 3;
@@ -1262,6 +1267,7 @@ static size_t layout_image(const ModelShape& shape, BatchPlan& p, bool save, int
         p.off_vsrc = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(nvm, 1), 16);
         p.off_tvp = off;  off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
         p.off_vinfo = off; off = align_up(off + sizeof(int) * 8 * (size_t)std::max(nv, 1), 16);
+        if (p.weighted) { p.off_vslot = off; off = align_up(off + sizeof(int) * (size_t)std::max(nv, 1), 16); }
     }
     if (p.weighted) {   // per-slot adjacency weights
         p.off_slotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16);
@@ -1273,7 +1279,7 @@ static size_t layout_image(const ModelShape& shape, BatchPlan& p, bool save, int
 
 // The typed view of an image laid out by plan `p` (layout_image) at `base`.  The one statement of which sections a plan carries: the
 // source-keyed CSR with save_for_backward (its slot map with attention, its weights on a weighted batch), the streaming tables on the
-// streaming plan, the slot weights on a weighted batch.  Every other section is null.
+// streaming plan (the virtual rows' first slots on a weighted one), the slot weights on a weighted batch.  Every other section is null.
 static ImageView image_view(const BatchPlan& p, bool use_att, char* base) {
     auto sec = [&](size_t off, bool present) { return present ? (void*)(base + off) : nullptr; };
     ImageView v;
@@ -1283,7 +1289,7 @@ static ImageView image_view(const BatchPlan& p, bool use_att, char* base) {
     v.trow = (int*)sec(p.off_trow, p.has_transpose); v.ttgt = (int*)sec(p.off_ttgt, p.has_transpose);
     v.tslot = (int*)sec(p.off_tslot, p.has_transpose && use_att);
     v.pair = (int*)sec(p.off_pair, p.stream); v.vptr = (int*)sec(p.off_vptr, p.stream); v.vsrc = (int*)sec(p.off_vsrc, p.stream);
-    v.tvp = (int*)sec(p.off_tvp, p.stream); v.vinfo = (int*)sec(p.off_vinfo, p.stream);
+    v.tvp = (int*)sec(p.off_tvp, p.stream); v.vinfo = (int*)sec(p.off_vinfo, p.stream); v.vslot = (int*)sec(p.off_vslot, p.stream && p.weighted);
     v.slotw = (float*)sec(p.off_slotw, p.weighted); v.tslotw = (float*)sec(p.off_tslotw, p.weighted && p.has_transpose);
     return v;
 }
@@ -1411,14 +1417,17 @@ static void fill_source_csr(int V, int T, const int32_t* const* adj, const int32
 // The streaming plan's tables of the (target, type) rows [r0, r1), one sequential pass: pair[r] = -1 (no message), its one source, or
 // -(2 + vid) for a virtual row (several messages), numbered on from `vid`; a virtual row's sources go to vsrc from `vm` on, its end to
 // vptr[vid + 1] and, when `vinfo` is non-null, its count and first seven sources to vinfo[8 * vid ..].  Advances vid and vm.
-static void stream_rows(size_t r0, size_t r1, const int* row_ptr, const int* csr_src, int* pair, int* vptr, int* vsrc, int* vinfo, int& vid,
-                        int& vm) {
+// Weighted batches (`slotw`: the slot weights of these rows, in target-CSR order): a row is a copy only if its one message weighs exactly
+// 1.0f, every other row with messages is a virtual row, and vslot[vid] = its first slot.
+static void stream_rows(size_t r0, size_t r1, const int* row_ptr, const int* csr_src, const float* slotw, int* pair, int* vptr, int* vsrc,
+                        int* vinfo, int* vslot, int& vid, int& vm) {
     for (size_t r = r0; r < r1; ++r) {
         const int b = row_ptr[r], cnt = row_ptr[r + 1] - b;
         if (cnt == 0) pair[r] = -1;
-        else if (cnt == 1) pair[r] = csr_src[b];
+        else if (cnt == 1 && (!slotw || slotw[b] == 1.0f)) pair[r] = csr_src[b];
         else {
             pair[r] = -(2 + vid);
+            if (vslot) vslot[vid] = b;
             if (vinfo) {
                 vinfo[8 * vid] = cnt;
                 for (int m = 0; m < 7; ++m) vinfo[8 * vid + 1 + m] = m < cnt ? csr_src[b + m] : 0;
@@ -1443,10 +1452,10 @@ static int64_t gcn_pairs(int64_t V, int64_t nnz, const int64_t* list, int32_t* p
 
 // ---- the host half of ggnn_set_graph_sparse: validation, tile plan, stable target-sorted CSR, streaming tables -> g->image.
 // `weighted`: the batch has one weight per message, `w`, in the type-major message order (required when there are messages); the image
-// then carries them in target-CSR order and, with the source-keyed CSR, in source-CSR order.
+// then carries them in target-CSR order and, with the source-keyed CSR, in source-CSR order.  `stream_weighted`: see build_plan.
 // Nothing here touches the device except the pinned allocation of the image and the wait for the previous upload out of it.
 static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* const* adj, const int32_t* num_edges, const float* indeg,
-                              bool weighted, const float* w) {
+                              bool weighted, const float* w, bool stream_weighted = false) {
     const ModelShape& shape = g->shape;
     BatchPlan& p = g->plan;
     g->valid = false;
@@ -1503,7 +1512,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     find_cuts(need_cuts ? reach.data() : nullptr, V, cuts);
     lap("validate+count", t_lap);
     std::vector<int> tile_start;
-    int rc = build_plan(shape, V, weighted, cuts, p, tile_start, g->err);
+    int rc = build_plan(shape, V, weighted, cuts, p, tile_start, g->err, stream_weighted);
     if (rc) return rc;
     p.M = M;
     const int ntiles = p.ntiles;
@@ -1512,6 +1521,18 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     // tile ranges of the threads for all later passes: tiles [tb[k], tb[k+1]), i.e. nodes [tile_start[tb[k]], tile_start[tb[k+1]])
     std::vector<int> tb(nth + 1);
     for (int k = 0; k <= nth; ++k) tb[k] = (int)((int64_t)ntiles * k / nth);
+    // weighted streaming plan: the rows whose one message weighs other than 1.0f, which stream_rows makes virtual rows too (each such row
+    // has one message, so no two writes meet)
+    std::vector<uint8_t> scaled_single;
+    if (p.stream && weighted) {
+        scaled_single.assign((size_t)V * T, 0);
+        for (int t = 0; t < T; ++t)
+            for (int i = 0; i < num_edges[t]; ++i) {
+                const size_t r = (size_t)adj[t][2 * i + 1] * T + t;
+                if (counts[r + 1] == 1 && w[type_base[t] + i] != 1.0f) scaled_single[r] = 1;
+            }
+    }
+    const uint8_t* scaled = scaled_single.empty() ? nullptr : scaled_single.data();
     // per-range totals: messages, and (streaming plan) virtual rows = (target, type) pairs with several messages, with their message count
     std::vector<int64_t> part_msgs(nth + 1, 0), part_nv(nth + 1, 0), part_nvm(nth + 1, 0);
 #ifdef _OPENMP
@@ -1524,7 +1545,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
             for (size_t r = k0; r < k1; ++r) {
                 const int c = counts[r + 1];
                 sm += c;
-                if (c >= 2) { ++nv; nvm += c; }
+                if (c >= 2 || (scaled && scaled[r])) { ++nv; nvm += c; }
             }
         } else {
             for (size_t r = k0; r < k1; ++r) sm += counts[r + 1];
@@ -1607,18 +1628,19 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
                 }
             }
         }
+        if (img.slotw)   // the weights of this range's slots, in target-CSR order
+            for (int64_t m = part_msgs[k]; m < part_msgs[k + 1]; ++m) img.slotw[m] = w[csr_msg[m]];
         if (img.pair) {   // the range's rows: no message -> -1, one -> its source, several -> virtual row; then the last tile's rows beyond V
             int vid = (int)part_nv[k], vm = (int)part_nvm[k];
             for (int i = tb[k]; i < tb[k + 1]; ++i) {
                 img.tvp[i] = vid;
                 const size_t rend = (size_t)tile_start[i + 1] * T, rpad = (size_t)(i + 1) * ts::TILE_M * T;
-                stream_rows((size_t)tile_start[i] * T, rend, img.row_ptr, csr_src, img.pair, img.vptr, img.vsrc, img.vinfo, vid, vm);
+                stream_rows((size_t)tile_start[i] * T, rend, img.row_ptr, csr_src, img.slotw, img.pair, img.vptr, img.vsrc, img.vinfo, img.vslot,
+                            vid, vm);
                 for (size_t r = rend; r < rpad; ++r) img.pair[r] = -1;
             }
             if (k == nth - 1) img.tvp[ntiles] = vid;
         }
-        if (img.slotw)   // the weights of this range's slots, in target-CSR order
-            for (int64_t m = part_msgs[k]; m < part_msgs[k + 1]; ++m) img.slotw[m] = w[csr_msg[m]];
         if (v1 > v0) memcpy(img.indeg + (size_t)v0 * T, indeg + (size_t)v0 * T, sizeof(float) * (size_t)(v1 - v0) * T);
         fill_denominators(v0, v1, T, indeg, img.denom);
     }
@@ -1733,6 +1755,23 @@ int ggnn_prepared_graph_arrays(const ggnn_prepared_graph* g, int32_t* row_ptr, i
     if (tile_start) memcpy(tile_start, img.tile_start, sizeof(int) * (size_t)(q.ntiles + 1));
     if (denom && V) memcpy(denom, img.denom, sizeof(float) * V);
     if (pair_src && img.pair) memcpy(pair_src, img.pair, sizeof(int) * (size_t)std::max(q.ntiles, 1) * ts::TILE_M * T);
+    return GGNN_OK;
+}
+
+int ggnn_prepared_graph_stream_tables(const ggnn_prepared_graph* g, int32_t* num_virtual_rows, int64_t* num_virtual_messages, int32_t* vrow_ptr,
+                                      int32_t* vsrc, int32_t* vinfo, int32_t* vslot, int32_t* tile_vptr) {
+    if (!g || !g->valid || !g->plan.stream) return GGNN_ESTATE;
+    const BatchPlan& q = g->plan;
+    const ImageView img = image_view(q, g->shape.use_att, g->image.ptr);
+    if (vslot && !img.vslot) return GGNN_ESTATE;
+    const size_t nv = (size_t)q.ts_nv, nvm = (size_t)img.vptr[nv];
+    if (num_virtual_rows) *num_virtual_rows = (int32_t)nv;
+    if (num_virtual_messages) *num_virtual_messages = (int64_t)nvm;
+    if (vrow_ptr) memcpy(vrow_ptr, img.vptr, sizeof(int) * (nv + 1));
+    if (vsrc && nvm) memcpy(vsrc, img.vsrc, sizeof(int) * nvm);
+    if (vinfo && nv) memcpy(vinfo, img.vinfo, sizeof(int) * 8 * nv);
+    if (vslot && nv) memcpy(vslot, img.vslot, sizeof(int) * nv);
+    if (tile_vptr) memcpy(tile_vptr, img.tvp, sizeof(int) * (size_t)(q.ntiles + 1));
     return GGNN_OK;
 }
 
@@ -1884,9 +1923,13 @@ static bool scan_dense(int T, int b, int v, const float* adjm, std::vector<std::
     return weighted;
 }
 
+// How the dense entries take a weighted matrix: refused (the binary prepare calls), as weighted messages that run on the tile kernel or on
+// fp32 (ggnn_set_graph_dense), or also on the streaming wgmma kernels above hidden 128 (the ..._dense_weighted entries).
+enum DenseWeights { DENSE_BINARY_ONLY, DENSE_WEIGHTED, DENSE_WEIGHTED_STREAM };
+
 // Host half of ggnn_set_graph_dense: the matrix is scanned to message lists for the CSR builder.  A 0/1 matrix builds the image of its
-// edge lists; a weighted one (when `weighted_ok`, else it is refused with GGNN_EUNSUPPORTED) also carries its entries as slot weights.
-static int build_dense_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const float* adjm, bool weighted_ok) {
+// edge lists; a weighted one (refused with GGNN_EUNSUPPORTED under DENSE_BINARY_ONLY) also carries its entries as slot weights.
+static int build_dense_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const float* adjm, DenseWeights mode) {
     g->valid = false;
     if (b < 0 || v <= 0 || (!adjm && b > 0)) return g->fail(GGNN_EINVAL, "null/negative argument");
     if (g->shape.use_att) return g->fail(GGNN_EUNSUPPORTED, "propagation attention exists only in the sparse model (sparse:170-196)");
@@ -1895,12 +1938,12 @@ static int build_dense_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const
     std::vector<std::vector<int32_t>> lists;
     std::vector<float> weights, indeg;
     const bool weighted = scan_dense(T, b, v, adjm, lists, weights, indeg);
-    if (weighted && !weighted_ok)
+    if (weighted && mode == DENSE_BINARY_ONLY)
         return g->fail(GGNN_EUNSUPPORTED, "the adjacency matrix is not 0/1: a weighted matrix is fed through ggnn_set_graph_dense");
     std::vector<const int32_t*> ptrs(T);
     std::vector<int32_t> counts(T);
     for (int t = 0; t < T; ++t) { ptrs[t] = lists[t].data(); counts[t] = (int32_t)(lists[t].size() / 2); }
-    int rc = build_sparse_image(g, b * v, ptrs.data(), counts.data(), indeg.data(), weighted, weights.data());
+    int rc = build_sparse_image(g, b * v, ptrs.data(), counts.data(), indeg.data(), weighted, weights.data(), mode == DENSE_WEIGHTED_STREAM);
     if (rc) return rc;
     g->plan.plan_text += weighted ? " [weighted dense adjacency -> weighted CSR]" : " [binary dense adjacency -> CSR]";
     return GGNN_OK;
@@ -1908,13 +1951,25 @@ static int build_dense_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const
 
 int ggnn_prepare_graph_dense(const ggnn_engine* e, int32_t save_for_backward, int32_t b, int32_t v, const float* adjm, ggnn_prepared_graph** inout) {
     if (int rc = begin_prepare<ggnn_config>(inout, e, nullptr, 0, save_for_backward, __func__)) return rc;
-    return build_dense_image(*inout, b, v, adjm, false);
+    return build_dense_image(*inout, b, v, adjm, DENSE_BINARY_ONLY);
 }
 
 int ggnn_host_prepare_graph_dense(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t b, int32_t v, const float* adjm,
                                   ggnn_prepared_graph** inout) {
     if (int rc = begin_prepare(inout, nullptr, cfg, num_sms, save_for_backward, __func__)) return rc;
-    return build_dense_image(*inout, b, v, adjm, false);
+    return build_dense_image(*inout, b, v, adjm, DENSE_BINARY_ONLY);
+}
+
+int ggnn_host_prepare_graph_dense_weighted(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t b, int32_t v,
+                                           const float* adjm, ggnn_prepared_graph** inout) {
+    if (int rc = begin_prepare(inout, nullptr, cfg, num_sms, save_for_backward, __func__)) return rc;
+    return build_dense_image(*inout, b, v, adjm, DENSE_WEIGHTED_STREAM);
+}
+
+int ggnn_prepare_graph_dense_weighted(const ggnn_engine* e, int32_t save_for_backward, int32_t b, int32_t v, const float* adjm,
+                                      ggnn_prepared_graph** inout) {
+    if (int rc = begin_prepare<ggnn_config>(inout, e, nullptr, 0, save_for_backward, __func__)) return rc;
+    return build_dense_image(*inout, b, v, adjm, DENSE_WEIGHTED_STREAM);
 }
 
 int ggnn_set_graph_dense(ggnn_engine* e, int32_t b, int32_t v, const float* adjm, ggnn_stream_t stream) {
@@ -1922,7 +1977,16 @@ int ggnn_set_graph_dense(ggnn_engine* e, int32_t b, int32_t v, const float* adjm
     GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
     return set_graph_from_own_prep(e, stream, [&](ggnn_prepared_graph** g) {
         if (int rc = begin_prepare<ggnn_config>(g, e, nullptr, 0, -1, "ggnn_set_graph_dense")) return rc;
-        return build_dense_image(*g, b, v, adjm, true);
+        return build_dense_image(*g, b, v, adjm, DENSE_WEIGHTED);
+    });
+}
+
+int ggnn_set_graph_dense_weighted(ggnn_engine* e, int32_t b, int32_t v, const float* adjm, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
+    return set_graph_from_own_prep(e, stream, [&](ggnn_prepared_graph** g) {
+        if (int rc = begin_prepare<ggnn_config>(g, e, nullptr, 0, -1, "ggnn_set_graph_dense_weighted")) return rc;
+        return build_dense_image(*g, b, v, adjm, DENSE_WEIGHTED_STREAM);
     });
 }
 
@@ -2217,6 +2281,7 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     base.tile_mask = gd.tile_mask;
     base.pair_src = gd.pair; base.vrow_ptr = gd.vptr; base.vsrc = gd.vsrc; base.tile_vptr = gd.tvp; base.vinfo = (const int4*)gd.vinfo;
     base.virt_img = (uint8_t*)e->ts_virt.ptr;   // pairs with several messages, pre-summed by the prologue of every gather launch
+    base.slot_w = gd.slotw; base.vslot = gd.vslot;   // weighted batches: the virtual rows' message weights (null for a binary batch)
     base.indeg = gd.indeg; base.denom = gd.denom;
     base.drop_keep = e->drop_keep; base.drop_seed = e->drop_seed;
     base.error_flag = (int*)e->err_flag.ptr;
@@ -3045,7 +3110,7 @@ static int ds_add_graph(ggnn_dataset* d, DsHost& h, int gi, int V, const int32_t
     if (d->stream_tables) {   // the graph's streaming tables on its own, virtual rows numbered in row order from 0
         std::vector<int> pair((size_t)V * T), vptr((size_t)V * T + 1, 0), vsrc((size_t)std::max(M, 1));
         int nv = 0, nvm = 0;
-        stream_rows(0, (size_t)V * T, row_ptr.data(), src.data(), pair.data(), vptr.data(), vsrc.data(), nullptr, nv, nvm);
+        stream_rows(0, (size_t)V * T, row_ptr.data(), src.data(), nullptr, pair.data(), vptr.data(), vsrc.data(), nullptr, nullptr, nv, nvm);
         g.nv = nv; g.nvm = nvm;
         int before = 0;
         for (int v = 0; v < V; ++v) {

@@ -9,7 +9,8 @@
 //                         a (target, type) pair with ONE message is a 64-byte asynchronous copy (cp.async, completion on the stage's
 //                         mbarrier) of the source row's image chunks, a pair with none is zeros, and the few pairs with several
 //                         messages are summed once per launch into "virtual rows" (prologue) and then copied like the others --
-//                         no load latency sits between two K-steps of a gather warp
+//                         no load latency sits between two K-steps of a gather warp.  In a weighted batch every pair whose messages are
+//                         not one of weight 1 is a virtual row, summed with its slot weights
 //   EPI_GATE  [r | u]   = sigmoid([res.. | agg | h] . K_g + b_g)          writes r*h (operand image) and u
 //   EPI_CAND  h'        = u*h + (1-u)*act([res.. | agg | r*h] . K_c + b_c) (RNN: act([res.. | agg | h] . K + b))
 // Node-state operands live in HBM/L2 as bf16 hi/lo "images" in the canonical K-major no-swizzle layout, tile-major:
@@ -75,12 +76,15 @@ struct StreamParams {
     // ---- A operand, gathered (EPI_AGG): per present edge type a DP-wide segment of per-type source sums
     const uint8_t* g_img;        // image of the state the messages are gathered from (a row with one type-t message is a 64-byte copy)
     const unsigned* tile_mask;   // [ntiles] bit t: some row of the tile receives a type-t message
-    const int* pair_src;         // [ntiles*128*T] per (target, type): -1 no message | source node (exactly one message) | -(2 + vid) several
+    const int* pair_src;         // [ntiles*128*T] per (target, type): -1 no message | source node (exactly one message, of weight 1) | -(2 + vid)
+                                 // several, or one of another weight
     const int* vrow_ptr;         // [NV+1] messages of the pairs with several messages (their "virtual rows"), CSR over vid ...
     const int* vsrc;             // ... source nodes in message order
     const int4* vinfo;           // [NV][2]: {count, src0, src1, src2 | src3 .. src6}: the first sources inline, one 32-byte load per virtual row
     const int* tile_vptr;        // [ntiles+1] vid range of each tile
     uint8_t* virt_img;           // image rows of the virtual rows (written in the prologue of every launch, row index = vid)
+    const float* slot_w;         // weighted batches: [M] target-CSR slot weights, or null (binary: every message weighs 1) ...
+    const int* vslot;            // ... and [NV] the first slot of every virtual row: message m of virtual row vid weighs slot_w[vslot[vid] + m]
     // ---- B operand
     const uint8_t* w;            // [nblk][kt_all] stages of 64*NC bytes: [hi: 2 k-groups x NC x 16 B | lo: same]
     int kt_all;                  // K-steps per N block in `w`
@@ -160,6 +164,31 @@ __device__ __forceinline__ void sum_pair_sources(const uint8_t* __restrict__ g_i
     if (cnt > 5) add_row(img_row(i1.z));
     if (cnt > 6) add_row(img_row(i1.w));
     for (int m = 7; m < cnt; ++m) add_row(img_row(vsrc_tail[m]));   // rare tail, in message order
+    tc::split8(a0, h0, l0);
+    tc::split8(a1, h1, l1);
+}
+
+// The same for a weighted batch's virtual row, which may have a single message: sum of w_m * (hi + lo) of its source rows, fp32 fmaf in
+// CSR order, hi part then lo part of each row (the accumulation order of the tile kernel's weighted gather).  `w` = its slot weights.
+__device__ __forceinline__ void sum_pair_sources_weighted(const uint8_t* __restrict__ g_img, int NKS, int ks, const int4& i0, const int4& i1,
+                                                          const int* __restrict__ vsrc_tail, const float* __restrict__ w, uint4& h0, uint4& h1,
+                                                          uint4& l0, uint4& l1) {
+    float a0[8], a1[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) { a0[j] = 0.0f; a1[j] = 0.0f; }
+    auto add_row = [&](int src, float wm) {
+        const uint8_t* sp = g_img + ((size_t)(src >> 7) * NKS + ks) * A_STAGE_B + (size_t)(src & 127) * 16;
+        const uint4 y0 = __ldcg(reinterpret_cast<const uint4*>(sp)), y1 = __ldcg(reinterpret_cast<const uint4*>(sp + 2048));
+        const uint4 y2 = __ldcg(reinterpret_cast<const uint4*>(sp + 4096)), y3 = __ldcg(reinterpret_cast<const uint4*>(sp + 6144));
+        tc::unpack8_add(y0, a0, wm); tc::unpack8_add(y2, a0, wm);
+        tc::unpack8_add(y1, a1, wm); tc::unpack8_add(y3, a1, wm);
+    };
+    const int cnt = i0.x;
+    const int inl[7] = {i0.y, i0.z, i0.w, i1.x, i1.y, i1.z, i1.w};
+#pragma unroll
+    for (int m = 0; m < 7; ++m)
+        if (m < cnt) add_row(inl[m], __ldg(w + m));
+    for (int m = 7; m < cnt; ++m) add_row(vsrc_tail[m], __ldg(w + m));   // rare tail, in message order
     tc::split8(a0, h0, l0);
     tc::split8(a1, h1, l1);
 }
@@ -314,7 +343,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_stream_kernel(const __grid_c
                     const int vl = task / nks, vid = v0 + vl, ks = ks0 + (task - vl * nks);
                     const int4 i0 = __ldg(p.vinfo + 2 * (size_t)vid), i1 = __ldg(p.vinfo + 2 * (size_t)vid + 1);
                     uint4 h0, l0, h1, l1;
-                    sum_pair_sources(p.g_img, NKS, ks, i0, i1, p.vsrc + p.vrow_ptr[i0.x > 7 ? vid : 0], h0, h1, l0, l1);
+                    if (p.slot_w)
+                        sum_pair_sources_weighted(p.g_img, NKS, ks, i0, i1, p.vsrc + p.vrow_ptr[i0.x > 7 ? vid : 0], p.slot_w + p.vslot[vid], h0, h1,
+                                                  l0, l1);
+                    else
+                        sum_pair_sources(p.g_img, NKS, ks, i0, i1, p.vsrc + p.vrow_ptr[i0.x > 7 ? vid : 0], h0, h1, l0, l1);
                     uint8_t* vp = p.virt_img + ((size_t)(vid >> 7) * NKS + ks) * A_STAGE_B + (size_t)(vid & 127) * 16;
                     *reinterpret_cast<uint4*>(vp) = h0;
                     *reinterpret_cast<uint4*>(vp + 2048) = h1;

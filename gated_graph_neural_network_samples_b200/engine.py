@@ -128,6 +128,17 @@ class PreparedGraph:
                        int(bool(save_for_backward)), a.shape[0], a.shape[2], a.ctypes.data)
 
     @classmethod
+    def host_only_dense_weighted(cls, params: dict, num_edge_types: int, adjacency_matrix, precision: str = "fp32", num_sms: int = 132,
+                                 save_for_backward: bool = False, reuse: Optional["PreparedGraph"] = None) -> "PreparedGraph":
+        """``ggnn_host_prepare_graph_dense_weighted``: any ``[b, T, v, v]`` adjacency as ``set_graph_dense_weighted`` builds it (a weighted one
+        with its entries as slot weights), no engine, no GPU."""
+        g = reuse if reuse is not None else cls()
+        cfg, keep = make_config(params, num_edge_types, 0, precision)
+        a = np.ascontiguousarray(np.asarray(adjacency_matrix, dtype=np.float32))
+        return g._fill(g.lib.ggnn_host_prepare_graph_dense_weighted, a.shape[0] * a.shape[2], int(num_edge_types), C.byref(cfg), int(num_sms),
+                       int(bool(save_for_backward)), a.shape[0], a.shape[2], a.ctypes.data)
+
+    @classmethod
     def host_only_gcn(cls, hidden_size: int, num_layers: int, num_nodes: int, adjacency_list, adjacency_weights, use_bias: bool = False,
                       precision: str = "fp32", num_sms: int = 132, save_for_backward: bool = False,
                       reuse: Optional["PreparedGraph"] = None) -> "PreparedGraph":
@@ -177,6 +188,22 @@ class PreparedGraph:
             raise GgnnError("the prepared graph is empty")
         if pair is not None:
             out["pair_src"] = pair
+        return out
+
+    def stream_tables(self) -> dict:
+        """A streaming plan's virtual rows: ``vrow_ptr`` [NV+1], ``vsrc``, ``vinfo`` [NV, 8], ``tile_vptr`` [num_tiles+1] and, on a weighted
+        batch, ``vslot`` [NV] (the first target-CSR slot of every virtual row; None on a binary batch)."""
+        nv, nvm = C.c_int32(), C.c_int64()
+        if self.lib.ggnn_prepared_graph_stream_tables(self._h, C.byref(nv), C.byref(nvm), None, None, None, None, None) != 0:
+            raise GgnnError("the prepared graph is empty or does not stream")
+        out = {"vrow_ptr": np.empty(nv.value + 1, np.int32), "vsrc": np.empty(nvm.value, np.int32), "vinfo": np.empty((nv.value, 8), np.int32),
+               "tile_vptr": np.empty(self.info()["num_tiles"] + 1, np.int32), "vslot": np.empty(nv.value, np.int32)}
+        weighted = self.lib.ggnn_prepared_graph_stream_tables(self._h, None, None, None, None, None, out["vslot"].ctypes.data, None) == 0
+        if not weighted:
+            out["vslot"] = None
+        if self.lib.ggnn_prepared_graph_stream_tables(self._h, None, None, out["vrow_ptr"].ctypes.data, out["vsrc"].ctypes.data,
+                                                      out["vinfo"].ctypes.data, None, out["tile_vptr"].ctypes.data) != 0:
+            raise GgnnError("the prepared graph is empty or does not stream")
         return out
 
     def tile_stats(self) -> tuple:
@@ -487,13 +514,26 @@ class PropagationEngine:
     def prepare_graph_dense(self, adjacency_matrix, save_for_backward: Optional[bool] = None,
                             reuse: Optional["PreparedGraph"] = None) -> "PreparedGraph":
         """The HOST half of ``set_graph_dense`` for a 0/1 adjacency ``[b, T, v, v]`` (scan to edge lists + the CSR builder); raises
-        ``GgnnError`` for a weighted matrix, which only ``set_graph_dense`` takes."""
+        ``GgnnError`` for a weighted matrix, which ``set_graph_dense`` and ``prepare_graph_dense_weighted`` take."""
+        return self._prepare_dense(self.lib.ggnn_prepare_graph_dense, adjacency_matrix, save_for_backward, reuse)
+
+    def prepare_graph_dense_weighted(self, adjacency_matrix, save_for_backward: Optional[bool] = None,
+                                     reuse: Optional["PreparedGraph"] = None) -> "PreparedGraph":
+        """The HOST half of ``set_graph_dense_weighted``: any ``[b, T, v, v]`` adjacency, a weighted one with its entries as slot weights
+        and, above hidden 128 on bf16x3 / bf16, on the streaming wgmma kernels."""
+        return self._prepare_dense(self.lib.ggnn_prepare_graph_dense_weighted, adjacency_matrix, save_for_backward, reuse)
+
+    def _prepare_dense(self, fn, adjacency_matrix, save_for_backward, reuse):
+        a = self._dense_matrix(adjacency_matrix)
+        g = reuse if reuse is not None else PreparedGraph(self.lib)
+        return g._fill(fn, a.shape[0] * a.shape[2], self.T, self._h, -1 if save_for_backward is None else int(bool(save_for_backward)),
+                       a.shape[0], a.shape[2], a.ctypes.data)
+
+    def _dense_matrix(self, adjacency_matrix) -> np.ndarray:
         a = np.ascontiguousarray(np.asarray(adjacency_matrix, dtype=np.float32))
         if a.ndim != 4 or a.shape[1] != self.T or a.shape[2] != a.shape[3]:
             raise GgnnError("adjacency_matrix must be [b, %d, v, v]" % self.T)
-        g = reuse if reuse is not None else PreparedGraph(self.lib)
-        return g._fill(self.lib.ggnn_prepare_graph_dense, a.shape[0] * a.shape[2], self.T, self._h,
-                       -1 if save_for_backward is None else int(bool(save_for_backward)), a.shape[0], a.shape[2], a.ctypes.data)
+        return a
 
     def set_graph_prepared(self, g: "PreparedGraph"):
         """The DEVICE half: adopt the plan, enqueue the one H2D copy of the image.  Keep ``g`` alive until the stream has passed it."""
@@ -640,11 +680,17 @@ class PropagationEngine:
 
     def set_graph_dense(self, adjacency_matrix: np.ndarray):
         """Dense wire format (dense:214-224): ``[b, T, v, v]`` float32 with ``A[g, t, dest, src]``."""
-        a = np.ascontiguousarray(np.asarray(adjacency_matrix, dtype=np.float32))
-        if a.ndim != 4 or a.shape[1] != self.T or a.shape[2] != a.shape[3]:
-            raise GgnnError("adjacency_matrix must be [b, %d, v, v]" % self.T)
+        self._set_dense(self.lib.ggnn_set_graph_dense, adjacency_matrix)
+
+    def set_graph_dense_weighted(self, adjacency_matrix: np.ndarray):
+        """``set_graph_dense`` that also runs a weighted matrix above hidden 128 on bf16x3 / bf16, on the streaming wgmma kernels (where
+        ``set_graph_dense`` refuses it)."""
+        self._set_dense(self.lib.ggnn_set_graph_dense_weighted, adjacency_matrix)
+
+    def _set_dense(self, fn, adjacency_matrix):
+        a = self._dense_matrix(adjacency_matrix)
         self.serial += 1
-        self._check(self.lib.ggnn_set_graph_dense(self._h, a.shape[0], a.shape[2], a.ctypes.data, self._stream()))
+        self._check(fn(self._h, a.shape[0], a.shape[2], a.ctypes.data, self._stream()))
         self.V = a.shape[0] * a.shape[2]
         self._graph_keepalive = (a,)
 

@@ -96,8 +96,10 @@ typedef struct ggnn_layer_grads {
  * Limits: hidden_size a positive multiple of 4 and <= 512 (larger: GGNN_EUNSUPPORTED), 1 <= num_edge_types <= 32 (<= 16 with propagation
  * attention), 1 <= num_layers <= 16, at most 4 residual inputs per layer.  Kernels by hidden size: GGNN_PREC_BF16X3 / GGNN_PREC_BF16 run
  * the tile-local wgmma kernel up to 128 and the streaming wgmma kernels above; GGNN_PREC_FP32 (and attention, and CudnnCompatibleGRUCell,
- * at any precision) runs the fused fp32 tile kernel up to 256 and the per-timestep fp32 path above 256.  A weighted dense adjacency runs
- * on tensor cores up to hidden 128 only. */
+ * at any precision) runs the fused fp32 tile kernel up to 256 and the per-timestep fp32 path above 256.  A weighted dense adjacency runs on
+ * tensor cores up to hidden 128 on the tile-local kernel (GLOBAL when a component exceeds 128 rows) whichever dense entry feeds it; above
+ * 128, ggnn_set_graph_dense / ggnn_run_dense_host(_predict) refuse it as before (run it on GGNN_PREC_FP32), and the ..._dense_weighted
+ * entries run it on the streaming kernels, whose gather sums each weighted (target, type) pair into a virtual row. */
 int ggnn_create(const ggnn_config* cfg, ggnn_engine** out);
 int ggnn_destroy(ggnn_engine* e);
 const char* ggnn_last_error(const ggnn_engine* e); /* e may be NULL: error of the last failed ggnn_create */
@@ -150,6 +152,14 @@ int ggnn_prepare_graph_dense(const ggnn_engine* e, int32_t save_for_backward, in
                              const float* adjacency_matrix, ggnn_prepared_graph** inout);
 int ggnn_host_prepare_graph_dense(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t num_graphs,
                                   int32_t num_vertices, const float* adjacency_matrix, ggnn_prepared_graph** inout);
+/* Any matrix, a weighted one with its entries as per-message (slot) weights and the plan text ending in
+ * " [weighted dense adjacency -> weighted CSR]"; a 0/1 matrix exactly as ggnn_prepare_graph_dense builds it.  Unlike ggnn_set_graph_dense,
+ * a weighted matrix above hidden 128 on GGNN_PREC_BF16X3 / GGNN_PREC_BF16 takes the streaming plan.  ggnn_set_graph_dense_weighted (below)
+ * is the prepare and the upload in one call; the host-only form needs no engine or GPU. */
+int ggnn_prepare_graph_dense_weighted(const ggnn_engine* e, int32_t save_for_backward, int32_t num_graphs, int32_t num_vertices,
+                                      const float* adjacency_matrix, ggnn_prepared_graph** inout);
+int ggnn_host_prepare_graph_dense_weighted(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t num_graphs,
+                                           int32_t num_vertices, const float* adjacency_matrix, ggnn_prepared_graph** inout);
 /* Introspection of a prepared graph: sizes and plan text; copies of its CSR (row_ptr [V*T+1], src [M], msg [M]), tile starts
  * [num_tiles+1], per-node mean-aggregation denominators [V] and, for a streaming plan, the (target, type) -> source table
  * [ceil(V/128)*128*T] (NULL pointers are skipped; pair_src of a non-streaming plan is left untouched and *is_streaming = 0). */
@@ -164,11 +174,23 @@ int ggnn_prepared_graph_image(const ggnn_prepared_graph* g, void* dst, int64_t c
 /* The plan's largest message count and largest number of edge types present in one tile: what the tile-local wgmma kernel sizes its shared
  * memory by (its CSR cache and its gather tiles). */
 int ggnn_prepared_graph_tile_stats(const ggnn_prepared_graph* g, int32_t* max_tile_msgs, int32_t* max_tile_types);
+/* A streaming plan's virtual rows (the (target, type) pairs the gather sums before copying; pair_src of ggnn_prepared_graph_arrays holds
+ * -(2 + vid) for them): their count NV and message count, vrow_ptr [NV+1] / vsrc (their sources in target-CSR order), vinfo [8*NV] (count,
+ * then the first seven sources, zero-filled), tile_vptr [num_tiles+1] (first vid of every tile) and, on a weighted batch only, vslot [NV]
+ * (the first target-CSR slot of every virtual row: message m weighs slot weight vslot[vid] + m).  In a weighted batch a pair is a virtual
+ * row unless it has exactly one message of weight exactly 1.0f.  NULL pointers are skipped; GGNN_ESTATE for a plan that does not stream,
+ * and for vslot on a binary one. */
+int ggnn_prepared_graph_stream_tables(const ggnn_prepared_graph* g, int32_t* num_virtual_rows, int64_t* num_virtual_messages, int32_t* vrow_ptr,
+                                      int32_t* vsrc, int32_t* vinfo, int32_t* vslot, int32_t* tile_vptr);
 
 /* Dense wire format (dense:214-224): adjacency_matrix [b, T, v, v] float32 HOST pointer with
  * A[g, t, dest, src] (dense:30-36).  Rows are the b*v padded nodes. */
 int ggnn_set_graph_dense(ggnn_engine* e, int32_t num_graphs, int32_t num_vertices,
                          const float* adjacency_matrix, ggnn_stream_t stream);
+/* The same, and a weighted matrix above hidden 128 on the tensor-core precisions runs on the streaming kernels (ggnn_set_graph_dense
+ * refuses it there with GGNN_EUNSUPPORTED). */
+int ggnn_set_graph_dense_weighted(ggnn_engine* e, int32_t num_graphs, int32_t num_vertices,
+                                  const float* adjacency_matrix, ggnn_stream_t stream);
 
 /* compute_final_node_representations (sparse:117-218 / dense:93-117).
  * h0, h_out: DEVICE [V, D] fp32 (dense: [b*v, D]).  Asynchronous on `stream`.
