@@ -19,6 +19,10 @@ class GgnnConfig(C.Structure):
                 ("use_propagation_attention", C.c_int32)]
 
 
+# values of GgnnConfig.use_propagation_attention (GGNN_ATT_*): off, on the fp32 kernels, at the configured precision
+ATT_OFF, ATT_FP32, ATT_TENSOR_CORES = 0, 1, 2
+
+
 class GgnnLayerWeights(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in
                 ("edge_weights", "edge_biases", "gate_kernel", "gate_bias", "cand_kernel", "cand_bias", "edge_type_attention_weights",

@@ -43,6 +43,8 @@ class DenseGGNNChemModel(ChemModel):
                                     'cand_kernel': var(glorot_init([2 * h_dim, h_dim])), 'cand_bias': var(np.zeros(h_dim))}
         # hidden sizes that are not multiples of 4 run zero-padded at the engine boundary (see SparseGGNNChemModel.prepare_specific_graph_model)
         self._padded_hidden = (h_dim + 3) // 4 * 4
+        if self.attention_tensor_cores:
+            raise Exception("--attention-tensor-cores applies to the sparse GGNN model's propagation attention; the dense model has none")
         self.engine = PropagationEngine(dense_engine_params(dict(self.params, hidden_size=self._padded_hidden)), T,
                                         device=self.device.index or 0, precision=self.precision)
         self._apply_backward_precision(self.engine)

@@ -91,6 +91,8 @@ class SparseGCNChemModel(ChemModel):
         # columns, kernel rows / columns and bias entries are zero, so padded units stay exactly 0 (relu(0) = 0) and add nothing to the
         # real units' sums.  Variables keep the reference's shapes.
         self._padded_hidden = (h_dim + 3) // 4 * 4
+        if self.attention_tensor_cores:
+            raise Exception("--attention-tensor-cores applies to the sparse GGNN model's propagation attention; the GCN model has none")
         self.engine = GCNEngine(self._padded_hidden, L, self.params['gcn_use_bias'], device=self.device.index or 0,
                                 precision=self.precision)
         self._apply_backward_precision(self.engine)

@@ -61,6 +61,9 @@ class ChemModel(object):
         self.backward_precision = args.get('--backward-precision')
         if self.backward_precision is not None and self.backward_precision not in ("fp32", "bf16x3"):
             raise Exception("Unknown backward precision '%s' (expected fp32 or bf16x3)." % self.backward_precision)
+        # --attention-tensor-cores: the sparse GGNN model's propagation attention runs at --precision (on bf16x3 / bf16 the streaming
+        # wgmma plan) instead of on the fp32 kernels.  Opt-in, because it changes the attention model's numerics from fp32 to --precision
+        self.attention_tensor_cores = bool(args.get('--attention-tensor-cores'))
         # --device-data: the plug-in uploads each data list once (engine.DeviceDataset) and assembles every batch on the GPU instead of
         # packing it on the host; same shuffle, same batches, same numbers.  A command-line option, not a params key: params are what a
         # checkpoint must match (restore_progress), and where the data lives does not change the model.

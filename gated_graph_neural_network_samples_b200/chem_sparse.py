@@ -125,8 +125,10 @@ class SparseGGNNChemModel(ChemModel):
         # exactly 0 through every cell (c = act(0) = 0, h' = u*0 + (1-u)*0) and out of every real unit's sums -- hook 2 pads, the engine
         # works at the padded width, the result is sliced back.  Variables keep the reference's shapes.
         self._padded_hidden = (h_dim + 3) // 4 * 4
+        # the keyword only when the option was given (an engine without it keeps working)
+        att = {'attention_tensor_cores': True} if self.attention_tensor_cores else {}
         self.engine = PropagationEngine(dict(self.params, hidden_size=self._padded_hidden), T, device=self.device.index or 0,
-                                        precision=self.precision)
+                                        precision=self.precision, **att)
         self._apply_backward_precision(self.engine)
         self._propagation = _propagation_function()
         self._readout = gated_readout_function()

@@ -4,7 +4,7 @@
 // Graphs never share edges, so every section of a batch's image is the graphs' own pieces laid end to end with offsets: a graph's
 // target-CSR rows get the slots of earlier graphs added, its sources the node offset, its message ids the batch's type base plus the
 // type's messages in earlier graphs; the source-keyed CSR, the attention slot map, the slot weights and the streaming tables (virtual row
-// ids offset by the earlier graphs' virtual rows) the same.  The dataset holds each graph's pieces in graph-local numbering; the host half
+// ids offset by the earlier graphs' virtual rows, their first slots by the earlier graphs' slots) the same.  The dataset holds each graph's pieces in graph-local numbering; the host half
 // (ggnn_dataset_prepare_batch) computes the per-graph offsets, one record per graph of the batch.
 //
 // ds_graph_kernel: one block per graph of the batch, each writes its graph's rows, slots, nodes and labels -- no two blocks write the same
@@ -41,6 +41,7 @@ struct DsArrays {
     const int* vend;       // [sum nv] end of every virtual row within the graph's virtual-row sources
     const int* vsrc;       // [sum nvm]
     const int* vpre;       // [sum V] virtual rows of the graph before every node
+    const int* vslot;      // [sum nv] attention on the streaming plan: the first target-CSR slot of every virtual row within the graph's slots
     const float* slotw;    // [sum M] weighted (GCN): weight of every target-CSR slot
     const float* tslotw;   // [sum M] ... and of every source-keyed entry (training)
     const float* ann;      // [sum V][ann_size]
@@ -98,6 +99,7 @@ __global__ void __launch_bounds__(256) ds_graph_kernel(const DsArrays a, const D
         for (int j = threadIdx.x; j < nvg; j += blockDim.x) {
             const int lo = j ? a.vend[vb + j - 1] : 0, hi = a.vend[vb + j], cnt = hi - lo, vid = voff + j;
             o.img.vptr[vid + 1] = vsoff + hi;
+            if (o.img.vslot) o.img.vslot[vid] = a.vslot[vb + j] + soff;   // a graph's (node, type) rows are contiguous: its slots are too
             o.img.vinfo[8 * vid] = cnt;
             for (int m = 0; m < 7; ++m) o.img.vinfo[8 * vid + 1 + m] = m < cnt ? a.vsrc[vsb + lo + m] + noff : 0;
             for (int m = 0; m < cnt; ++m) o.img.vsrc[vsoff + lo + m] = a.vsrc[vsb + lo + m] + noff;

@@ -137,7 +137,8 @@ struct ModelShape {
     int step_base[MAX_LAYERS] = {0};
     int total_steps = 0;
     int use_bias = 0, use_avg = 0, cell = 0, act = 0, precision = 0, device = 0;
-    int use_att = 0;    // use_propagation_attention (sparse:170-196): fp32 path only
+    int use_att = 0;    // use_propagation_attention (sparse:170-196): on the fp32 kernels, or on the streaming wgmma kernels when the
+                        // precision is not fp32 (GGNN_ATT_TENSOR_CORES)
     int num_sms = 132;
     size_t max_smem = 0;
 };
@@ -172,7 +173,13 @@ struct BatchPlan {
     size_t off_tslot = 0;            // source-keyed CSR entry -> target-CSR slot (attention backward)
     size_t off_pair = 0, off_vptr = 0, off_vsrc = 0, off_tvp = 0, off_vinfo = 0;   // streaming plan: (target,type) -> source table, virtual rows (pairs with several messages)
     size_t off_vslot = 0;   // weighted streaming plan: the first target-CSR slot of every virtual row (its weights are slot_w[vslot[vid] + m])
+    bool all_virtual = false;   // attention on the streaming plan: every (target, type) pair with messages is a virtual row, weighted by the
+                                // step's attention probabilities through vslot (the image has vslot and no slot weights)
     size_t off_slotw = 0, off_tslotw = 0;   // weighted: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
+    // (offset, bytes) of the image's bytes no section builder writes: alignment gaps and the one-element room of empty sections.  The host
+    // builder zeroes them (the device dataset zeroes its whole image), so that an image is one function of its batch, whatever the
+    // staging memory held before
+    std::vector<std::pair<size_t, size_t>> pads;
 };
 
 // The weights in the pre-split, pre-tiled bf16 layout of one tensor-core kernel family, with each layer's offsets.  The tiles are rebuilt
@@ -532,7 +539,7 @@ int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>
         // keeps the tile kernel's plans (GLOBAL for a component over 128 rows), on which every pair is gathered with its weights and none
         // becomes a virtual row.
         const bool big_component = max_span > tc::TILE_M && !weighted && !force_global && !(fs && fs[0] == '0');
-        if (s.DP > 128 || big_component || (fs && fs[0] == '1' && !weighted)) {
+        if (s.DP > 128 || big_component || (fs && fs[0] == '1' && !weighted) || s.use_att) {
             // streaming plan: fixed 128-row tiles (the gather reads the previous state from L2, so tiles need not respect components),
             // one launch per GEMM of a timestep; N blocks sized so that small batches still spread over the chip
             if (weighted && !stream_weighted) {
@@ -541,6 +548,7 @@ int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>
                 return GGNN_EUNSUPPORTED;
             }
             p.stream = true; p.variant = 3;
+            p.all_virtual = s.use_att != 0;   // (attention runs on the streaming plan at every hidden size)
             fixed_tiles(V, ts::TILE_M, tile_start);
             p.ntiles = (int)tile_start.size() - 1;
             for (int i = 0; i < 2; ++i) {
@@ -549,8 +557,10 @@ int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>
                 p.ts_nblk[i] = (width + ts::MMA_N - 1) / ts::MMA_N;
                 p.ts_nc[i] = ts::MMA_N;
             }
-            int len = snprintf(buf, sizeof buf, "wgmma-%s STREAM(3 launches per step: gather-GEMM, gate GEMM, candidate GEMM) tiles=%d DP=%d N-blocks agg/cand=%dx%d gate=%dx%d",
-                               prec, p.ntiles, s.DP, p.ts_nblk[0], p.ts_nc[0], p.ts_nblk[1], p.ts_nc[1]);
+            int len = snprintf(buf, sizeof buf, "wgmma-%s STREAM%s tiles=%d DP=%d N-blocks agg/cand=%dx%d gate=%dx%d", prec,
+                               s.use_att ? "+attention(4 launches per step: attention, gather-GEMM, gate GEMM, candidate GEMM)"
+                                         : "(3 launches per step: gather-GEMM, gate GEMM, candidate GEMM)",
+                               p.ntiles, s.DP, p.ts_nblk[0], p.ts_nc[0], p.ts_nblk[1], p.ts_nc[1]);
             if (s.DP <= 128) snprintf(buf + len, sizeof buf - len, " max_component=%d", max_span);   // (not computed for hidden sizes > 128: fixed tiles)
         } else {
             p.variant = 2;
@@ -976,7 +986,9 @@ static int init_model_shape(ModelShape& s, const ggnn_config* cfg, std::string& 
     s.cell = cfg->cell; s.act = cfg->activation;
     s.use_att = cfg->use_propagation_attention != 0;
     if (s.use_att && s.T > 16) { err = "propagation attention supports at most 16 edge types"; return GGNN_EUNSUPPORTED; }
-    if (s.use_att) s.precision = GGNN_PREC_FP32;   // the softmax-weighted gather lives in the fp32 kernel only (the plan text says so)
+    // GGNN_ATT_FP32: the softmax-weighted gather runs on the fp32 kernels (the plan text says so); GGNN_ATT_TENSOR_CORES keeps the precision,
+    // so attention at a tensor-core precision means the streaming plan with its attention pre-pass
+    if (s.use_att && (cfg->use_propagation_attention != GGNN_ATT_TENSOR_CORES || s.cell == CELL_CUDNN_GRU)) s.precision = GGNN_PREC_FP32;
     if (s.cell == CELL_CUDNN_GRU) s.precision = GGNN_PREC_FP32;   // so does the reset-after-matmul candidate of CudnnCompatibleGRUCell
     int total = 0;
     for (int l = 0; l < s.L; ++l) {
@@ -1246,32 +1258,43 @@ static size_t layout_image(const ModelShape& shape, BatchPlan& p, bool save, int
     const int V = p.V, T = shape.T, ntiles = p.ntiles;
     size_t off = 0;
     p.M = M;
-    p.off_row_ptr = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
-    p.off_src = off;     off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
-    p.off_msg = off;     off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
-    p.off_indeg = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1) * T, 16);
-    p.off_denom = off;   off = align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16);
-    p.off_tiles = off;   off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
-    p.off_mask = off;    off = align_up(off + sizeof(unsigned) * (size_t)std::max(ntiles, 1), 16);
+    p.pads.clear();
+    // a section whose builders write its first `used` bytes, in room for `room` bytes (at least one element), 16-byte aligned; the bytes
+    // after `used` up to the next section are recorded in p.pads
+    auto place = [&](size_t used, size_t room) {
+        const size_t at = off;
+        off = align_up(at + room, 16);
+        if (off > at + used) p.pads.push_back({at + used, off - at - used});
+        return at;
+    };
+    const size_t I = sizeof(int), Mu = (size_t)M, Mr = (size_t)std::max<int64_t>(M, 1);
+    const size_t VT = (size_t)V * T, nvu = (size_t)nv, nvr = (size_t)std::max(nv, 1), nvmu = (size_t)nvm;
+    p.off_row_ptr = place(I * (VT + 1), I * (VT + 1));
+    p.off_src = place(I * Mu, I * Mr);
+    p.off_msg = place(I * Mu, I * Mr);
+    p.off_indeg = place(sizeof(float) * VT, sizeof(float) * (size_t)std::max(V, 1) * T);
+    p.off_denom = place(sizeof(float) * (size_t)V, sizeof(float) * (size_t)std::max(V, 1));
+    p.off_tiles = place(I * (size_t)(ntiles + 1), I * (size_t)(ntiles + 1));
+    p.off_mask = place(sizeof(unsigned) * (size_t)ntiles, sizeof(unsigned) * (size_t)std::max(ntiles, 1));
     p.has_transpose = save;
     if (p.has_transpose) {
-        p.off_trow = off; off = align_up(off + sizeof(int) * ((size_t)V * T + 1), 16);
-        p.off_ttgt = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
-        p.off_tslot = off;
-        if (shape.use_att) off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(M, 1), 16);
+        p.off_trow = place(I * (VT + 1), I * (VT + 1));
+        p.off_ttgt = place(I * Mu, I * Mr);
+        p.off_tslot = shape.use_att ? place(I * Mu, I * Mr) : off;
     }
     // streaming plan: per (target, type) pair the ONE node to copy from (or none / a virtual row), see ggnn_fwd_stream.cuh
     if (p.stream) {
-        p.off_pair = off; off = align_up(off + sizeof(int) * (size_t)std::max(ntiles, 1) * ts::TILE_M * T, 16);
-        p.off_vptr = off; off = align_up(off + sizeof(int) * (size_t)(nv + 1), 16);
-        p.off_vsrc = off; off = align_up(off + sizeof(int) * (size_t)std::max<int64_t>(nvm, 1), 16);
-        p.off_tvp = off;  off = align_up(off + sizeof(int) * (size_t)(ntiles + 1), 16);
-        p.off_vinfo = off; off = align_up(off + sizeof(int) * 8 * (size_t)std::max(nv, 1), 16);
-        if (p.weighted) { p.off_vslot = off; off = align_up(off + sizeof(int) * (size_t)std::max(nv, 1), 16); }
+        const size_t pairs = I * (size_t)std::max(ntiles, 1) * ts::TILE_M * T;
+        p.off_pair = place(pairs, pairs);
+        p.off_vptr = place(I * (nvu + 1), I * (nvu + 1));
+        p.off_vsrc = place(I * nvmu, I * (size_t)std::max<int64_t>(nvm, 1));
+        p.off_tvp = place(I * (size_t)(ntiles + 1), I * (size_t)(ntiles + 1));
+        p.off_vinfo = place(I * 8 * nvu, I * 8 * nvr);
+        if (p.weighted || p.all_virtual) p.off_vslot = place(I * nvu, I * nvr);
     }
     if (p.weighted) {   // per-slot adjacency weights
-        p.off_slotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16);
-        if (p.has_transpose) { p.off_tslotw = off; off = align_up(off + sizeof(float) * (size_t)std::max<int64_t>(M, 1), 16); }
+        p.off_slotw = place(sizeof(float) * Mu, sizeof(float) * Mr);
+        if (p.has_transpose) p.off_tslotw = place(sizeof(float) * Mu, sizeof(float) * Mr);
     }
     p.ts_nv = nv;
     return off;
@@ -1279,7 +1302,7 @@ static size_t layout_image(const ModelShape& shape, BatchPlan& p, bool save, int
 
 // The typed view of an image laid out by plan `p` (layout_image) at `base`.  The one statement of which sections a plan carries: the
 // source-keyed CSR with save_for_backward (its slot map with attention, its weights on a weighted batch), the streaming tables on the
-// streaming plan (the virtual rows' first slots on a weighted one), the slot weights on a weighted batch.  Every other section is null.
+// streaming plan (the virtual rows' first slots on a weighted one and with attention), the slot weights on a weighted batch.  Every other section is null.
 static ImageView image_view(const BatchPlan& p, bool use_att, char* base) {
     auto sec = [&](size_t off, bool present) { return present ? (void*)(base + off) : nullptr; };
     ImageView v;
@@ -1289,7 +1312,7 @@ static ImageView image_view(const BatchPlan& p, bool use_att, char* base) {
     v.trow = (int*)sec(p.off_trow, p.has_transpose); v.ttgt = (int*)sec(p.off_ttgt, p.has_transpose);
     v.tslot = (int*)sec(p.off_tslot, p.has_transpose && use_att);
     v.pair = (int*)sec(p.off_pair, p.stream); v.vptr = (int*)sec(p.off_vptr, p.stream); v.vsrc = (int*)sec(p.off_vsrc, p.stream);
-    v.tvp = (int*)sec(p.off_tvp, p.stream); v.vinfo = (int*)sec(p.off_vinfo, p.stream); v.vslot = (int*)sec(p.off_vslot, p.stream && p.weighted);
+    v.tvp = (int*)sec(p.off_tvp, p.stream); v.vinfo = (int*)sec(p.off_vinfo, p.stream); v.vslot = (int*)sec(p.off_vslot, p.stream && (p.weighted || p.all_virtual));
     v.slotw = (float*)sec(p.off_slotw, p.weighted); v.tslotw = (float*)sec(p.off_tslotw, p.weighted && p.has_transpose);
     return v;
 }
@@ -1418,13 +1441,14 @@ static void fill_source_csr(int V, int T, const int32_t* const* adj, const int32
 // -(2 + vid) for a virtual row (several messages), numbered on from `vid`; a virtual row's sources go to vsrc from `vm` on, its end to
 // vptr[vid + 1] and, when `vinfo` is non-null, its count and first seven sources to vinfo[8 * vid ..].  Advances vid and vm.
 // Weighted batches (`slotw`: the slot weights of these rows, in target-CSR order): a row is a copy only if its one message weighs exactly
-// 1.0f, every other row with messages is a virtual row, and vslot[vid] = its first slot.
-static void stream_rows(size_t r0, size_t r1, const int* row_ptr, const int* csr_src, const float* slotw, int* pair, int* vptr, int* vsrc,
-                        int* vinfo, int* vslot, int& vid, int& vm) {
+// 1.0f, every other row with messages is a virtual row, and vslot[vid] = its first slot.  `all_virtual` (attention, whose probability of a
+// lone message is 1 / (1 + 1e-7), not 1): every row with messages is a virtual row.
+static void stream_rows(size_t r0, size_t r1, const int* row_ptr, const int* csr_src, const float* slotw, bool all_virtual, int* pair, int* vptr,
+                        int* vsrc, int* vinfo, int* vslot, int& vid, int& vm) {
     for (size_t r = r0; r < r1; ++r) {
         const int b = row_ptr[r], cnt = row_ptr[r + 1] - b;
         if (cnt == 0) pair[r] = -1;
-        else if (cnt == 1 && (!slotw || slotw[b] == 1.0f)) pair[r] = csr_src[b];
+        else if (cnt == 1 && !all_virtual && (!slotw || slotw[b] == 1.0f)) pair[r] = csr_src[b];
         else {
             pair[r] = -(2 + vid);
             if (vslot) vslot[vid] = b;
@@ -1545,7 +1569,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
             for (size_t r = k0; r < k1; ++r) {
                 const int c = counts[r + 1];
                 sm += c;
-                if (c >= 2 || (scaled && scaled[r])) { ++nv; nvm += c; }
+                if (c >= 2 || (scaled && scaled[r]) || (p.all_virtual && c == 1)) { ++nv; nvm += c; }
             }
         } else {
             for (size_t r = k0; r < k1; ++r) sm += counts[r + 1];
@@ -1558,6 +1582,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     CU_TRY(g, g->image.begin(off));
     g->bytes = off;
     const ImageView img = image_view(p, shape.use_att, g->image.ptr);
+    for (const auto& pad : p.pads) memset(g->image.ptr + pad.first, 0, pad.second);
     lap("stage reserve", t_lap);
 
     // ---- pass 2, per thread over its tile range: exclusive scan of the (target, type) rows -> row_ptr, fill cursors, the tiles'
@@ -1635,8 +1660,8 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
             for (int i = tb[k]; i < tb[k + 1]; ++i) {
                 img.tvp[i] = vid;
                 const size_t rend = (size_t)tile_start[i + 1] * T, rpad = (size_t)(i + 1) * ts::TILE_M * T;
-                stream_rows((size_t)tile_start[i] * T, rend, img.row_ptr, csr_src, img.slotw, img.pair, img.vptr, img.vsrc, img.vinfo, img.vslot,
-                            vid, vm);
+                stream_rows((size_t)tile_start[i] * T, rend, img.row_ptr, csr_src, img.slotw, p.all_virtual, img.pair, img.vptr, img.vsrc, img.vinfo,
+                            img.vslot, vid, vm);
                 for (size_t r = rend; r < rpad; ++r) img.pair[r] = -1;
             }
             if (k == nth - 1) img.tvp[ntiles] = vid;
@@ -2263,6 +2288,8 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     const size_t avail = (e->max_smem > 2048 ? e->max_smem - 2048 : 0);
     const size_t csr_b = (size_t)ts::TILE_M * T * 4;   // the tile's (target, type) -> source table
     CU_TRY(e, e->ts_virt.reserve((size_t)((e->ts_nv + ts::TILE_M - 1) / ts::TILE_M + 1) * NKS * ts::A_STAGE_B));
+    const size_t att_stride = e->save ? (size_t)std::max<int64_t>(e->M, 1) : 0;   // attention probabilities of a step, [steps][M] when saving
+    if (e->use_att) CU_TRY(e, e->att_buf.reserve(sizeof(float) * (size_t)std::max<int64_t>(e->M, 1) * (size_t)(e->save ? std::max(e->total_steps, 1) : 1)));
     // a ring stage carries KS K-steps, the largest of 4, 2, 1 that divides the K-steps of a segment (the producer thread pays several
     // hundred cycles per bulk copy whatever its size; KS is a template parameter so that a stage's MMAs are straight-line code)
     const char* env_ks = getenv("GGNN_TS_KSTEPS");
@@ -2281,7 +2308,8 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     base.tile_mask = gd.tile_mask;
     base.pair_src = gd.pair; base.vrow_ptr = gd.vptr; base.vsrc = gd.vsrc; base.tile_vptr = gd.tvp; base.vinfo = (const int4*)gd.vinfo;
     base.virt_img = (uint8_t*)e->ts_virt.ptr;   // pairs with several messages, pre-summed by the prologue of every gather launch
-    base.slot_w = gd.slotw; base.vslot = gd.vslot;   // weighted batches: the virtual rows' message weights (null for a binary batch)
+    base.slot_w = gd.slotw; base.vslot = gd.vslot;   // weighted batches: the virtual rows' message weights (null for a binary batch; with
+                                                     // attention the step's probabilities, set per step)
     base.indeg = gd.indeg; base.denom = gd.denom;
     base.drop_keep = e->drop_keep; base.drop_seed = e->drop_seed;
     base.error_flag = (int*)e->err_flag.ptr;
@@ -2334,8 +2362,15 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
             float* chk_out = last ? chk_state(l + 1) : chk_tmp[s & 1];
             const int gs = e->step_base[l] + s;
             const SaveDev sv = saved_step(e, gs);
-            // ---- aggregated messages
+            // ---- aggregated messages (with attention: the step's probabilities first, the gather's slot weights)
             ts::StreamParams p = base;
+            if (e->use_att) {
+                float* att = (float*)e->att_buf.ptr + (size_t)gs * att_stride;
+                ts::attention_chunk_kernel<<<(V + 7) / 8, 256, 0, st>>>(gd.row_ptr, gd.src, chk_in, e->w[l].edge_type_attention_weights, att, V, D,
+                                                                        DP, T);
+                ++e->last_launches;
+                p.slot_w = att;
+            }
             p.epi = ts::EPI_AGG; p.NC = nc0; p.nstages = ns_edge;
             p.g_img = img_in; p.w = wb + wt.off_edge[l]; p.kt_all = T * NKS;
             p.bias = e->use_bias ? e->w[l].edge_biases : nullptr;
@@ -3061,7 +3096,7 @@ struct ggnn_dataset_batch : ErrorText {
 
 // The host arrays of a dataset before its upload, section by section (each 16-byte aligned in the one image).
 struct DsHost {
-    std::vector<int> base, row_end, src, pos, trow_end, ttgt, tslot, pair, vend, vsrc, vpre, nfeat;
+    std::vector<int> base, row_end, src, pos, trow_end, ttgt, tslot, pair, vend, vsrc, vpre, vslot, nfeat;
     std::vector<float> indeg, denom, slotw, tslotw;
 };
 
@@ -3107,10 +3142,14 @@ static int ds_add_graph(ggnn_dataset* d, DsHost& h, int gi, int V, const int32_t
                         d->weighted ? h.tslotw.data() + t0 : nullptr);
         h.trow_end.insert(h.trow_end.end(), trow.begin() + 1, trow.end());
     }
-    if (d->stream_tables) {   // the graph's streaming tables on its own, virtual rows numbered in row order from 0
-        std::vector<int> pair((size_t)V * T), vptr((size_t)V * T + 1, 0), vsrc((size_t)std::max(M, 1));
+    if (d->stream_tables) {   // the graph's streaming tables on its own, virtual rows numbered in row order from 0 (with attention every row
+                              // with messages, and vslot graph-local)
+        const bool att = d->shape.use_att != 0;
+        std::vector<int> pair((size_t)V * T), vptr((size_t)V * T + 1, 0), vsrc((size_t)std::max(M, 1)), vslot(att ? (size_t)V * T : 0);
         int nv = 0, nvm = 0;
-        stream_rows(0, (size_t)V * T, row_ptr.data(), src.data(), nullptr, pair.data(), vptr.data(), vsrc.data(), nullptr, nullptr, nv, nvm);
+        stream_rows(0, (size_t)V * T, row_ptr.data(), src.data(), nullptr, att, pair.data(), vptr.data(), vsrc.data(), nullptr,
+                    att ? vslot.data() : nullptr, nv, nvm);
+        if (att) h.vslot.insert(h.vslot.end(), vslot.begin(), vslot.begin() + nv);
         g.nv = nv; g.nvm = nvm;
         int before = 0;
         for (int v = 0; v < V; ++v) {
@@ -3156,11 +3195,12 @@ static int ds_finish(ggnn_dataset* d, DsHost& h, const float* ann, const float* 
     auto F = [](const std::vector<float>& v, const float** dst) { return Section{v.data(), v.size() * sizeof(float), (const void**)dst}; };
     const Section secs[] = {I(h.base, &a.base), I(h.row_end, &a.row_end), I(h.src, &a.src), I(h.pos, &a.pos), F(h.indeg, &a.indeg),
                             F(h.denom, &a.denom), I(h.trow_end, &a.trow_end), I(h.ttgt, &a.ttgt), I(h.tslot, &a.tslot), I(h.pair, &a.pair),
-                            I(h.vend, &a.vend), I(h.vsrc, &a.vsrc), I(h.vpre, &a.vpre), F(h.slotw, &a.slotw), F(h.tslotw, &a.tslotw),
+                            I(h.vend, &a.vend), I(h.vsrc, &a.vsrc), I(h.vpre, &a.vpre), I(h.vslot, &a.vslot), F(h.slotw, &a.slotw), F(h.tslotw, &a.tslotw),
                             {ann, nann * sizeof(float), (const void**)&a.ann}, {labels, nlab * sizeof(float), (const void**)&a.labels},
                             {lmask, nlab * sizeof(float), (const void**)&a.lmask}, I(h.nfeat, &a.nfeat)};
     const bool present[] = {true, true, true, true, true, true, d->train, d->train, d->train && d->shape.use_att, d->stream_tables,
-                            d->stream_tables, d->stream_tables, d->stream_tables, d->weighted, d->weighted && d->train, true, d->tasks > 0,
+                            d->stream_tables, d->stream_tables, d->stream_tables, d->stream_tables && d->shape.use_att, d->weighted,
+                            d->weighted && d->train, true, d->tasks > 0,
                             d->tasks > 0, d->dense};
     size_t total = 0;
     for (const Section& s : secs) total = align_up(total + s.bytes, 16);

@@ -10,7 +10,8 @@
 //                         mbarrier) of the source row's image chunks, a pair with none is zeros, and the few pairs with several
 //                         messages are summed once per launch into "virtual rows" (prologue) and then copied like the others --
 //                         no load latency sits between two K-steps of a gather warp.  In a weighted batch every pair whose messages are
-//                         not one of weight 1 is a virtual row, summed with its slot weights
+//                         not one of weight 1 is a virtual row, summed with its slot weights; with propagation attention every pair
+//                         with messages is a virtual row, weighted by the step's probabilities (attention_chunk_kernel, launched first)
 //   EPI_GATE  [r | u]   = sigmoid([res.. | agg | h] . K_g + b_g)          writes r*h (operand image) and u
 //   EPI_CAND  h'        = u*h + (1-u)*act([res.. | agg | r*h] . K_c + b_c) (RNN: act([res.. | agg | h] . K + b))
 // Node-state operands live in HBM/L2 as bf16 hi/lo "images" in the canonical K-major no-swizzle layout, tile-major:
@@ -83,7 +84,8 @@ struct StreamParams {
     const int4* vinfo;           // [NV][2]: {count, src0, src1, src2 | src3 .. src6}: the first sources inline, one 32-byte load per virtual row
     const int* tile_vptr;        // [ntiles+1] vid range of each tile
     uint8_t* virt_img;           // image rows of the virtual rows (written in the prologue of every launch, row index = vid)
-    const float* slot_w;         // weighted batches: [M] target-CSR slot weights, or null (binary: every message weighs 1) ...
+    const float* slot_w;         // weighted batches: [M] target-CSR slot weights (attention: the step's probabilities), or null (binary:
+                                 // every message weighs 1) ...
     const int* vslot;            // ... and [NV] the first slot of every virtual row: message m of virtual row vid weighs slot_w[vslot[vid] + m]
     // ---- B operand
     const uint8_t* w;            // [nblk][kt_all] stages of 64*NC bytes: [hi: 2 k-groups x NC x 16 B | lo: same]
@@ -522,6 +524,52 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_stream_kernel(const __grid_c
         if (!ok && lane == 0) atomicExch(p.error_flag, 11);
     }
     __syncthreads();
+}
+
+// Propagation attention (sparse:170-196) on the streaming plan: the pre-pass of a timestep, before its gather launch.  The arithmetic of
+// step::attention_kernel (one warp per target node, fp32 scores <h[src], h[v]> * a_t, max-shifted expf, sum + 1e-7, a division), read
+// from the chunk-major fp32 master `chk` of the step's input state -- never from the bf16 images, whose split error times a score of
+// order 100 would move the probabilities far off -- and only over the D real columns.  att[slot] = the probability of each target-CSR
+// slot, which the gather launch reads as its slot weights.  No atomics.
+__global__ void __launch_bounds__(256) attention_chunk_kernel(const int* __restrict__ row_ptr, const int* __restrict__ csr_src,
+                                                              const float* __restrict__ chk, const float* __restrict__ att_w,
+                                                              float* __restrict__ att, int V, int D, int DP, int T) {
+    const int v = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (v >= V) return;
+    const int D4 = D >> 2, NKC = DP >> 3;
+    const float* hv = chk + chunk_off(NKC, v >> 7, 0, v & 127);
+    const int mbeg = row_ptr[(size_t)v * T], mend = row_ptr[(size_t)(v + 1) * T];
+    float mx = -INFINITY;
+    for (int t = 0; t < T; ++t) {
+        const float aw = att_w[t];
+        const int beg = row_ptr[(size_t)v * T + t], end = row_ptr[(size_t)v * T + t + 1];
+        for (int m = beg; m < end; ++m) {
+            const int src = csr_src[m];
+            const float* hp = chk + chunk_off(NKC, src >> 7, 0, src & 127);
+            float dot = 0.f;
+            for (int c4 = lane; c4 < D4; c4 += 32) {   // columns 4*c4 .. 4*c4+3: half c4 & 1 of chunk c4 / 2, 128 rows x 8 floats apart
+                const size_t o = (size_t)(c4 >> 1) * (TILE_M * 8) + (c4 & 1) * 4;
+                const float4 a = *reinterpret_cast<const float4*>(hp + o), b = *reinterpret_cast<const float4*>(hv + o);
+                dot += a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w;
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+            const float sc = dot * aw;
+            if (lane == 0) att[m] = sc;
+            mx = fmaxf(mx, sc);
+        }
+    }
+    __syncwarp();
+    float sum = 0.f;
+    for (int m = mbeg + lane; m < mend; m += 32) {
+        const float ex = expf(att[m] - mx);
+        att[m] = ex;
+        sum += ex;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    const float den = sum + 1e-7f;   // SMALL_NUMBER, sparse:194
+    for (int m = mbeg + lane; m < mend; m += 32) att[m] = att[m] / den;
 }
 
 // fp32 [V][D] row-major -> tile-major bf16 hi/lo image + chunk-major fp32 copy ([ntiles*128][DP], zero padded)

@@ -39,6 +39,12 @@ enum { GGNN_ACT_TANH = 0, GGNN_ACT_RELU = 1 };  /* params['graph_rnn_activation'
 enum { GGNN_PREC_FP32 = 0,   /* fp32 FFMA on CUDA cores (bit-for-bit fp32 semantics, order aside) */
        GGNN_PREC_BF16X3 = 1, /* wgmma tensor cores, bf16 hi/lo split, 3 MMAs (~2^-16 rel / product) */
        GGNN_PREC_BF16 = 2 }; /* wgmma tensor cores, single bf16 MMA ("fast", outside the 1e-4 bar) */
+/* values of ggnn_config.use_propagation_attention */
+enum { GGNN_ATT_OFF = 0,
+       GGNN_ATT_FP32 = 1,           /* attention on the fp32 kernels whatever the precision (every nonzero value but 2 means this) */
+       GGNN_ATT_TENSOR_CORES = 2 }; /* attention at the configured precision: on GGNN_PREC_BF16X3 / GGNN_PREC_BF16 every batch takes the
+                                       streaming wgmma plan (a softmax pre-pass per step feeding the slot-weighted gather); on
+                                       GGNN_PREC_FP32, and with CudnnCompatibleGRUCell, exactly GGNN_ATT_FP32 */
 
 /* Mirrors the keys of self.params the two hooks read (sparse:40-61, chem_tensorflow.py:17-37). */
 typedef struct ggnn_config {
@@ -54,7 +60,7 @@ typedef struct ggnn_config {
     int32_t activation;                   /* GGNN_ACT_*                                                */
     int32_t precision;                    /* GGNN_PREC_*                                               */
     int32_t device;                       /* CUDA device ordinal                                       */
-    int32_t use_propagation_attention;    /* sparse:46,94-96,147-149,170-196 (fp32 path; <= 16 edge types) */
+    int32_t use_propagation_attention;    /* GGNN_ATT_*, sparse:46,94-96,147-149,170-196 (<= 16 edge types) */
 } ggnn_config;
 
 /* Device pointers to one layer's trainables, fp32 row-major, shapes as created at sparse:86-115:
@@ -95,8 +101,9 @@ typedef struct ggnn_layer_grads {
 /* prepare_specific_graph_model (sparse:63-115 / dense:68-91): fix the model shape.
  * Limits: hidden_size a positive multiple of 4 and <= 512 (larger: GGNN_EUNSUPPORTED), 1 <= num_edge_types <= 32 (<= 16 with propagation
  * attention), 1 <= num_layers <= 16, at most 4 residual inputs per layer.  Kernels by hidden size: GGNN_PREC_BF16X3 / GGNN_PREC_BF16 run
- * the tile-local wgmma kernel up to 128 and the streaming wgmma kernels above; GGNN_PREC_FP32 (and attention, and CudnnCompatibleGRUCell,
- * at any precision) runs the fused fp32 tile kernel up to 256 and the per-timestep fp32 path above 256.  A weighted dense adjacency runs on
+ * the tile-local wgmma kernel up to 128 and the streaming wgmma kernels above; attention with GGNN_ATT_TENSOR_CORES runs the streaming
+ * wgmma kernels at every hidden size.  GGNN_PREC_FP32 (and GGNN_ATT_FP32 attention, and CudnnCompatibleGRUCell, at any precision) runs
+ * the fused fp32 tile kernel up to 256 and the per-timestep fp32 path above 256.  A weighted dense adjacency runs on
  * tensor cores up to hidden 128 on the tile-local kernel (GLOBAL when a component exceeds 128 rows) whichever dense entry feeds it; above
  * 128, ggnn_set_graph_dense / ggnn_run_dense_host(_predict) refuse it as before (run it on GGNN_PREC_FP32), and the ..._dense_weighted
  * entries run it on the streaming kernels, whose gather sums each weighted (target, type) pair into a virtual row. */
