@@ -21,6 +21,8 @@ class GgnnConfig(C.Structure):
 
 # values of GgnnConfig.use_propagation_attention (GGNN_ATT_*): off, on the fp32 kernels, at the configured precision
 ATT_OFF, ATT_FP32, ATT_TENSOR_CORES = 0, 1, 2
+# the GgnnConfig.cell value of CudnnCompatibleGRUCell at the configured precision (GGNN_CELL_CUDNN_GRU_TENSOR_CORES; 2 runs it on fp32)
+CELL_CUDNN_GRU_TENSOR_CORES = 3
 
 
 class GgnnLayerWeights(C.Structure):

@@ -45,6 +45,8 @@ class DenseGGNNChemModel(ChemModel):
         self._padded_hidden = (h_dim + 3) // 4 * 4
         if self.attention_tensor_cores:
             raise Exception("--attention-tensor-cores applies to the sparse GGNN model's propagation attention; the dense model has none")
+        if self.cudnn_gru_tensor_cores:
+            raise Exception("--cudnn-gru-tensor-cores applies to the sparse GGNN model's CudnnCompatibleGRUCell; the dense model has no cell option")
         self.engine = PropagationEngine(dense_engine_params(dict(self.params, hidden_size=self._padded_hidden)), T,
                                         device=self.device.index or 0, precision=self.precision)
         self._apply_backward_precision(self.engine)

@@ -93,6 +93,8 @@ class SparseGCNChemModel(ChemModel):
         self._padded_hidden = (h_dim + 3) // 4 * 4
         if self.attention_tensor_cores:
             raise Exception("--attention-tensor-cores applies to the sparse GGNN model's propagation attention; the GCN model has none")
+        if self.cudnn_gru_tensor_cores:
+            raise Exception("--cudnn-gru-tensor-cores applies to the sparse GGNN model's CudnnCompatibleGRUCell; the GCN model has no RNN cell")
         self.engine = GCNEngine(self._padded_hidden, L, self.params['gcn_use_bias'], device=self.device.index or 0,
                                 precision=self.precision)
         self._apply_backward_precision(self.engine)

@@ -64,6 +64,9 @@ class ChemModel(object):
         # --attention-tensor-cores: the sparse GGNN model's propagation attention runs at --precision (on bf16x3 / bf16 the streaming
         # wgmma plan) instead of on the fp32 kernels.  Opt-in, because it changes the attention model's numerics from fp32 to --precision
         self.attention_tensor_cores = bool(args.get('--attention-tensor-cores'))
+        # --cudnn-gru-tensor-cores: the sparse GGNN model's CudnnCompatibleGRUCell runs at --precision likewise.  Both are command-line options,
+        # not params keys: the trainables are the same, so a checkpoint restores into a model with or without them
+        self.cudnn_gru_tensor_cores = bool(args.get('--cudnn-gru-tensor-cores'))
         # --device-data: the plug-in uploads each data list once (engine.DeviceDataset) and assembles every batch on the GPU instead of
         # packing it on the host; same shuffle, same batches, same numbers.  A command-line option, not a params key: params are what a
         # checkpoint must match (restore_progress), and where the data lives does not change the model.

@@ -127,6 +127,8 @@ class SparseGGNNChemModel(ChemModel):
         self._padded_hidden = (h_dim + 3) // 4 * 4
         # the keyword only when the option was given (an engine without it keeps working)
         att = {'attention_tensor_cores': True} if self.attention_tensor_cores else {}
+        if self.cudnn_gru_tensor_cores:
+            att['cudnn_gru_tensor_cores'] = True
         self.engine = PropagationEngine(dict(self.params, hidden_size=self._padded_hidden), T, device=self.device.index or 0,
                                         precision=self.precision, **att)
         self._apply_backward_precision(self.engine)

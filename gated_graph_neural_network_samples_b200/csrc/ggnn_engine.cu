@@ -139,6 +139,7 @@ struct ModelShape {
     int use_bias = 0, use_avg = 0, cell = 0, act = 0, precision = 0, device = 0;
     int use_att = 0;    // use_propagation_attention (sparse:170-196): on the fp32 kernels, or on the streaming wgmma kernels when the
                         // precision is not fp32 (GGNN_ATT_TENSOR_CORES)
+    int cudnn_tc = 0;   // GGNN_CELL_CUDNN_GRU_TENSOR_CORES: cell is CELL_CUDNN_GRU and keeps the configured precision (the streaming plan)
     int num_sms = 132;
     size_t max_smem = 0;
 };
@@ -188,6 +189,7 @@ struct BatchPlan {
 struct WeightTiles {
     DevBuf buf;
     size_t off_edge[MAX_LAYERS] = {0}, off_gate[MAX_LAYERS] = {0}, off_cand[MAX_LAYERS] = {0};
+    size_t off_hproj[MAX_LAYERS] = {0};   // streaming layout, CudnnCompatibleGRUCell: the hidden projection K_hid (the last D rows of cand_kernel)
     uint64_t gen = 0;     // the weights generation the tiles were made from (0: none)
     size_t bytes = 0;     // the layout they were made for: its size and, for the streaming layout, its N-block widths
     int nc[2] = {0, 0};
@@ -539,7 +541,9 @@ int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>
         // keeps the tile kernel's plans (GLOBAL for a component over 128 rows), on which every pair is gathered with its weights and none
         // becomes a virtual row.
         const bool big_component = max_span > tc::TILE_M && !weighted && !force_global && !(fs && fs[0] == '0');
-        if (s.DP > 128 || big_component || (fs && fs[0] == '1' && !weighted) || s.use_att) {
+        // attention and CudnnCompatibleGRUCell (GGNN_CELL_CUDNN_GRU_TENSOR_CORES: the tile kernel has no candidate for it) always stream
+        const bool cudnn = s.cell == CELL_CUDNN_GRU;
+        if (s.DP > 128 || big_component || (fs && fs[0] == '1' && !weighted) || s.use_att || cudnn) {
             // streaming plan: fixed 128-row tiles (the gather reads the previous state from L2, so tiles need not respect components),
             // one launch per GEMM of a timestep; N blocks sized so that small batches still spread over the chip
             if (weighted && !stream_weighted) {
@@ -557,10 +561,13 @@ int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>
                 p.ts_nblk[i] = (width + ts::MMA_N - 1) / ts::MMA_N;
                 p.ts_nc[i] = ts::MMA_N;
             }
-            int len = snprintf(buf, sizeof buf, "wgmma-%s STREAM%s tiles=%d DP=%d N-blocks agg/cand=%dx%d gate=%dx%d", prec,
-                               s.use_att ? "+attention(4 launches per step: attention, gather-GEMM, gate GEMM, candidate GEMM)"
-                                         : "(3 launches per step: gather-GEMM, gate GEMM, candidate GEMM)",
-                               p.ntiles, s.DP, p.ts_nblk[0], p.ts_nc[0], p.ts_nblk[1], p.ts_nc[1]);
+            const char* steps = s.use_att ? (cudnn ? "+attention+cudnn-gru(5 launches per step: attention, gather-GEMM, gate GEMM, hidden-projection "
+                                                     "GEMM, candidate GEMM)"
+                                                   : "+attention(4 launches per step: attention, gather-GEMM, gate GEMM, candidate GEMM)")
+                                          : (cudnn ? "+cudnn-gru(4 launches per step: gather-GEMM, gate GEMM, hidden-projection GEMM, candidate GEMM)"
+                                                   : "(3 launches per step: gather-GEMM, gate GEMM, candidate GEMM)");
+            int len = snprintf(buf, sizeof buf, "wgmma-%s STREAM%s tiles=%d DP=%d N-blocks agg/cand=%dx%d gate=%dx%d", prec, steps, p.ntiles, s.DP,
+                               p.ts_nblk[0], p.ts_nc[0], p.ts_nblk[1], p.ts_nc[1]);
             if (s.DP <= 128) snprintf(buf + len, sizeof buf - len, " max_component=%d", max_span);   // (not computed for hidden sizes > 128: fixed tiles)
         } else {
             p.variant = 2;
@@ -978,18 +985,24 @@ static int init_model_shape(ModelShape& s, const ggnn_config* cfg, std::string& 
     if (int rc = init_common_shape(s, cfg->hidden_size, 512, cfg->num_layers, cfg->precision, cfg->device, err)) return rc;
     if (cfg->num_edge_types <= 0 || cfg->num_edge_types > 32) return bad("num_edge_types must be in 1..32");
     if (!cfg->layer_timesteps) return bad("layer_timesteps is null");
-    if (cfg->cell != GGNN_CELL_GRU && cfg->cell != GGNN_CELL_RNN && cfg->cell != GGNN_CELL_CUDNN_GRU) return bad("Unknown RNN cell type");   // sparse:112
-    if (cfg->cell == GGNN_CELL_CUDNN_GRU && cfg->activation != GGNN_ACT_TANH) return bad("CudnnCompatibleGRUCell requires the tanh activation");   // sparse:106
+    const bool cudnn_tc = cfg->cell == GGNN_CELL_CUDNN_GRU_TENSOR_CORES;
+    if (cfg->cell != GGNN_CELL_GRU && cfg->cell != GGNN_CELL_RNN && cfg->cell != GGNN_CELL_CUDNN_GRU && !cudnn_tc)
+        return bad("Unknown RNN cell type");   // sparse:112
+    if ((cfg->cell == GGNN_CELL_CUDNN_GRU || cudnn_tc) && cfg->activation != GGNN_ACT_TANH)
+        return bad("CudnnCompatibleGRUCell requires the tanh activation");   // sparse:106
     if (cfg->activation != GGNN_ACT_TANH && cfg->activation != GGNN_ACT_RELU) return bad("Unknown activation function type");  // sparse:81
     s.T = cfg->num_edge_types;
     s.use_bias = cfg->use_edge_bias != 0; s.use_avg = cfg->use_edge_msg_avg_aggregation != 0;
-    s.cell = cfg->cell; s.act = cfg->activation;
+    s.cell = cudnn_tc ? (int)CELL_CUDNN_GRU : cfg->cell; s.act = cfg->activation;
+    s.cudnn_tc = cudnn_tc ? 1 : 0;
     s.use_att = cfg->use_propagation_attention != 0;
     if (s.use_att && s.T > 16) { err = "propagation attention supports at most 16 edge types"; return GGNN_EUNSUPPORTED; }
     // GGNN_ATT_FP32: the softmax-weighted gather runs on the fp32 kernels (the plan text says so); GGNN_ATT_TENSOR_CORES keeps the precision,
     // so attention at a tensor-core precision means the streaming plan with its attention pre-pass
-    if (s.use_att && (cfg->use_propagation_attention != GGNN_ATT_TENSOR_CORES || s.cell == CELL_CUDNN_GRU)) s.precision = GGNN_PREC_FP32;
-    if (s.cell == CELL_CUDNN_GRU) s.precision = GGNN_PREC_FP32;   // so does the reset-after-matmul candidate of CudnnCompatibleGRUCell
+    const bool cudnn_fp32 = s.cell == CELL_CUDNN_GRU && !cudnn_tc;
+    if (s.use_att && (cfg->use_propagation_attention != GGNN_ATT_TENSOR_CORES || cudnn_fp32)) s.precision = GGNN_PREC_FP32;
+    // so does the reset-after-matmul candidate of CudnnCompatibleGRUCell, unless GGNN_CELL_CUDNN_GRU_TENSOR_CORES asks for the streaming plan
+    if (cudnn_fp32) s.precision = GGNN_PREC_FP32;
     int total = 0;
     for (int l = 0; l < s.L; ++l) {
         if (cfg->layer_timesteps[l] < 0) return bad("negative layer_timesteps entry");
@@ -1958,6 +1971,7 @@ static int build_dense_image(ggnn_prepared_graph* g, int32_t b, int32_t v, const
     g->valid = false;
     if (b < 0 || v <= 0 || (!adjm && b > 0)) return g->fail(GGNN_EINVAL, "null/negative argument");
     if (g->shape.use_att) return g->fail(GGNN_EUNSUPPORTED, "propagation attention exists only in the sparse model (sparse:170-196)");
+    if (g->shape.cudnn_tc) return g->fail(GGNN_EUNSUPPORTED, "CudnnCompatibleGRUCell exists only in the sparse model (sparse:105-108)");
     const int T = g->shape.T;
     if ((int64_t)b * v > 0x7fffffff / std::max(T, 1)) return g->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
     std::vector<std::vector<int32_t>> lists;
@@ -2230,16 +2244,20 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
 
 // ------------------------------------------------------------------------------------------ streaming tensor-core path (host)
 // The streaming layout (ggnn_fwd_stream.cuh): per layer, in N blocks of ts_nc columns, the T edge blocks, the gate and the candidate kernel.
+// CudnnCompatibleGRUCell splits the candidate kernel in two: K_in (its first (R+1) D rows, the [res.. | agg] segments) and, at off_hproj,
+// K_hid (its last D rows, one segment).
 static int ts_prepare_weights(ggnn_engine* e, cudaStream_t st) {
     const int D = e->D, DP = e->DP, T = e->T, NKS = DP / 16;
     const int nc0 = e->ts_nc[0], nb0 = e->ts_nblk[0], nc1 = e->ts_nc[1], nb1 = e->ts_nblk[1];
+    const bool cudnn = e->cell == CELL_CUDNN_GRU;
     WeightTiles& c = e->ts_tiles;
     size_t off = 0;
     for (int l = 0; l < e->L; ++l) {
-        const int nseg = e->nres[l] + 2;
+        const int nseg = e->nres[l] + 2, ncand = cudnn ? nseg - 1 : nseg;
         c.off_edge[l] = off; off += (size_t)nb0 * T * NKS * 64 * nc0;
         c.off_gate[l] = off; off += (size_t)nb1 * nseg * NKS * 64 * nc1;
-        c.off_cand[l] = off; off += (size_t)nb0 * nseg * NKS * 64 * nc0;
+        c.off_cand[l] = off; off += (size_t)nb0 * ncand * NKS * 64 * nc0;
+        c.off_hproj[l] = off; off += cudnn ? (size_t)nb0 * NKS * 64 * nc0 : 0;
     }
     bool retile = false;
     CU_TRY(e, c.reserve(off, nc0, nc1, e->weights_gen, retile));
@@ -2254,8 +2272,13 @@ static int ts_prepare_weights(ggnn_engine* e, cudaStream_t st) {
             ++e->last_launches;
         };
         launch(e->w[l].edge_weights, base + c.off_edge[l], T, 1, D, nc0, nb0);
-        if (e->cell == CELL_GRU) launch(e->w[l].gate_kernel, base + c.off_gate[l], nseg, 2, 2 * D, nc1, nb1);
-        launch(e->w[l].cand_kernel, base + c.off_cand[l], nseg, 1, D, nc0, nb0);
+        if (e->cell != CELL_RNN) launch(e->w[l].gate_kernel, base + c.off_gate[l], nseg, 2, 2 * D, nc1, nb1);
+        if (cudnn) {
+            launch(e->w[l].cand_kernel, base + c.off_cand[l], nseg - 1, 1, D, nc0, nb0);
+            launch(e->w[l].cand_kernel + (size_t)(nseg - 1) * D * D, base + c.off_hproj[l], 1, 1, D, nc0, nb0);
+        } else {
+            launch(e->w[l].cand_kernel, base + c.off_cand[l], nseg, 1, D, nc0, nb0);
+        }
     }
     CU_TRY(e, cudaGetLastError());
     c.gen = e->weights_gen;
@@ -2268,7 +2291,8 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     int rc = ts_prepare_weights(e, st);
     if (rc) return rc;
     const size_t img_b = (size_t)ntiles * NKS * ts::A_STAGE_B;   // one operand image == one chunk-major fp32 copy, in bytes
-    const int n_img = L + 1 + 4;    // images: node_states_per_layer, two step temporaries, agg, r*h
+    // images: node_states_per_layer, two step temporaries, agg, r*h (CudnnCompatibleGRUCell: the same bytes hold r, then r*q, chunk-major fp32)
+    const int n_img = L + 1 + 4;
     const int n_chk = L + 1 + 3;    // chunk-major fp32: node_states_per_layer, two step temporaries, u
     CU_TRY(e, e->ts_images.reserve(img_b * (n_img + n_chk)));
     uint8_t* ib = (uint8_t*)e->ts_images.ptr;
@@ -2281,7 +2305,8 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     float* chk_tmp[2] = {(float*)(cb + (size_t)(L + 1) * img_b), (float*)(cb + (size_t)(L + 2) * img_b)};
     float* u_chk = (float*)(cb + (size_t)(L + 3) * img_b);
     const size_t vd_bytes = (size_t)V * D * sizeof(float);
-    const bool gru = e->cell == CELL_GRU;
+    const bool gated = e->cell != CELL_RNN, cudnn = e->cell == CELL_CUDNN_GRU;
+    float* rq_chk = (float*)img_rh;   // CudnnCompatibleGRUCell: r (gate launch), then r*q (hidden-projection launch)
     const ImageView& gd = e->gd;
 
     // shared-memory budgets
@@ -2314,7 +2339,8 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     base.drop_keep = e->drop_keep; base.drop_seed = e->drop_seed;
     base.error_flag = (int*)e->err_flag.ptr;
     const int nc0 = e->ts_nc[0], nb0 = e->ts_nblk[0], nc1 = e->ts_nc[1], nb1 = e->ts_nblk[1];
-    // one CTA per SM for all three kernels: the whole shared memory is the ring
+    // one CTA per SM for all three kernels: the whole shared memory is the ring (CudnnCompatibleGRUCell's hidden-projection launch has the
+    // candidate's N blocks, and so its ring)
     const int ns_edge = stages_for(nc0, avail > csr_b ? avail - csr_b : 0);
     const int ns_gate = stages_for(nc1, avail), ns_cand = stages_for(nc0, avail);
     // the kernel's parity waits are only sound if every ring has at least as many stages as there are gather groups (ts::MIN_NS)
@@ -2377,27 +2403,40 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
             p.img_out = img_agg; p.sv_agg = sv.agg; p.gstep = gs;
             k_edge<<<dim3(ntiles, nb0), ts::NTHREADS, sm_edge, st>>>(p);
             ++e->last_launches;
+            // [res.. | agg | last_img], or without last_img (null: CudnnCompatibleGRUCell's candidate, whose recurrent half is its own launch)
             auto set_segs = [&](ts::StreamParams& q, const uint8_t* last_img) {
-                q.nseg = nseg;
+                q.nseg = last_img ? nseg : nseg - 1;
                 for (int i = 0; i < R; ++i) q.seg[i] = img_state(e->res[l][i]);
-                q.seg[R] = img_agg; q.seg[R + 1] = last_img;
-                q.kt_all = nseg * NKS;
+                q.seg[R] = img_agg;
+                if (last_img) q.seg[R + 1] = last_img;
+                q.kt_all = q.nseg * NKS;
             };
-            if (gru) {
+            if (gated) {
                 ts::StreamParams q = base;
                 q.epi = ts::EPI_GATE; q.NC = nc1; q.nstages = ns_gate;
                 set_segs(q, img_in);
-                q.w = wb + wt.off_gate[l]; q.bias = e->w[l].gate_bias; q.h_chk = chk_in; q.u_buf = u_chk; q.img_out = img_rh;
+                q.w = wb + wt.off_gate[l]; q.bias = e->w[l].gate_bias; q.h_chk = chk_in; q.u_buf = u_chk;
+                if (cudnn) q.rq_chk = rq_chk; else q.img_out = img_rh;
                 q.sv_r = sv.r; q.sv_h = sv.h_in; q.sv_u = sv.u;
                 q.gstep = gs;
                 k_fed<<<dim3(ntiles, nb1), ts::NTHREADS, smem_of(nc1, ns_gate, false), st>>>(q);
                 ++e->last_launches;
             }
+            if (cudnn) {   // q = h . K_hid + b_hid over the step's input state; r <- r*q
+                ts::StreamParams q = base;
+                q.epi = ts::EPI_HPROJ; q.NC = nc0; q.nstages = ns_cand;
+                q.nseg = 1; q.seg[0] = img_in; q.kt_all = NKS;
+                q.w = wb + wt.off_hproj[l]; q.b_hid = e->w[l].cand_hidden_bias; q.rq_chk = rq_chk; q.sv_q = sv.q;
+                q.gstep = gs;
+                k_fed<<<dim3(ntiles, nb0), ts::NTHREADS, smem_of(nc0, ns_cand, false), st>>>(q);
+                ++e->last_launches;
+            }
             ts::StreamParams c = base;
             c.epi = ts::EPI_CAND; c.NC = nc0; c.nstages = ns_cand;
-            set_segs(c, gru ? img_rh : img_in);
+            set_segs(c, cudnn ? nullptr : (gated ? img_rh : img_in));
             c.w = wb + wt.off_cand[l]; c.bias = e->w[l].cand_bias; c.h_chk = chk_in; c.u_buf = u_chk; c.h_chk_out = chk_out; c.h_out = out; c.img_out = img_out;
-            if (gru) c.sv_c = sv.c; else c.sv_h = sv.h_in;
+            if (cudnn) c.rq_chk = rq_chk;
+            if (gated) c.sv_c = sv.c; else c.sv_h = sv.h_in;
             c.gstep = gs;
             k_fed<<<dim3(ntiles, nb0), ts::NTHREADS, smem_of(nc0, ns_cand, false), st>>>(c);
             ++e->last_launches;
@@ -3312,6 +3351,7 @@ static int create_dataset_dense(ggnn_dataset** out, const ggnn_engine* e, const 
     ggnn_dataset* d = *out;
     d->dense = true;
     if (d->shape.use_att) return d->fail(GGNN_EUNSUPPORTED, "propagation attention exists only in the sparse model (sparse:170-196)");
+    if (d->shape.cudnn_tc) return d->fail(GGNN_EUNSUPPORTED, "CudnnCompatibleGRUCell exists only in the sparse model (sparse:105-108)");
     if (N > 0 && !graph_offsets) return d->fail(GGNN_EINVAL, "null graph offsets");
     const int T = d->shape.T, bwd = tie_fwd_bkwd ? 0 : T / 2;
     DsHost h;

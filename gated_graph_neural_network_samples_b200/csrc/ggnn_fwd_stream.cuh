@@ -14,6 +14,10 @@
 //                         with messages is a virtual row, weighted by the step's probabilities (attention_chunk_kernel, launched first)
 //   EPI_GATE  [r | u]   = sigmoid([res.. | agg | h] . K_g + b_g)          writes r*h (operand image) and u
 //   EPI_CAND  h'        = u*h + (1-u)*act([res.. | agg | r*h] . K_c + b_c) (RNN: act([res.. | agg | h] . K + b))
+// CudnnCompatibleGRUCell (sparse:105-108) applies the reset gate after the recurrent product, so a timestep is four launches:
+//   EPI_GATE  as above, but writes r itself (chunk-major fp32) instead of the r*h image
+//   EPI_HPROJ q         = h . K_hid + b_hid                                  saves q, overwrites the r chunk with r*q
+//   EPI_CAND  h'        = u*h + (1-u)*tanh([res.. | agg] . K_in + b_in + r*q)
 // Node-state operands live in HBM/L2 as bf16 hi/lo "images" in the canonical K-major no-swizzle layout, tile-major:
 //   byte(tile, kstep, part, kgroup, row, j) = ((tile*NKS + kstep)*2 + part)*4096 + kgroup*2048 + row*16 + j*2
 // so one K-step of a 128-row A operand (hi + lo) is ONE contiguous 8 KB bulk copy (cp.async.bulk, 1-D TMA), and an
@@ -62,7 +66,7 @@ __host__ __device__ inline size_t ring_bytes(size_t nstages, size_t stage_b) {
     const size_t acc_b = (size_t)TILE_M * ACC_LD * sizeof(float);
     return nstages * stage_b > acc_b ? nstages * stage_b : acc_b;
 }
-enum { EPI_AGG = 0, EPI_GATE = 1, EPI_CAND = 2 };
+enum { EPI_AGG = 0, EPI_GATE = 1, EPI_CAND = 2, EPI_HPROJ = 3 };
 
 struct StreamParams {
     int V, D, DP, T;
@@ -101,6 +105,10 @@ struct StreamParams {
     float* sv_u;                 // GATE: row-major copy of u for the backward pass, or null
     uint8_t* img_out;            // AGG: agg image; GATE: r*h image; CAND: image of the new state
     float* sv_h; float* sv_agg; float* sv_r; float* sv_c;   // this step's save-for-backward slots or null
+    // ---- CudnnCompatibleGRUCell
+    const float* b_hid;          // HPROJ: cand_hidden_bias [D]
+    float* rq_chk;               // chunk-major fp32: r (written by GATE), r*q (HPROJ), read by CAND
+    float* sv_q;                 // HPROJ: row-major save slot of q = h . K_hid + b_hid, or null
     float drop_keep; unsigned long long drop_seed; int gstep;
     int* error_flag;
 };
@@ -400,23 +408,27 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_stream_kernel(const __grid_c
         // ---- epilogue: parked accumulator -> registers -> outputs.  The global operands of the first chunk are requested BEFORE the wait for the
         // accumulator, those of chunk c+1 before the math of chunk c (the loads are L2 hits after the prefetch above).
         const bool have_acc = nk > 0;
-        const bool gru = p.cell == CELL_GRU;
+        // the cells: GRU and CudnnCompatibleGRUCell have gates (u blends the candidate with h), CudnnCompatibleGRUCell resets after the
+        // recurrent product, RNN has neither
+        const bool gated = p.cell != CELL_RNN, cudnn = p.cell == CELL_CUDNN_GRU;
         const int colb = nb0 * NC;                    // first (padded) output column of this CTA
         const float* acc_row = accs + (size_t)row * ACC_LD;
         // the global operands of this thread's next chunk are requested before the math of the current one
         float hA[8], uA[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) { hA[j] = 0.0f; uA[j] = 0.0f; }
-        const bool cand_h = p.epi == EPI_CAND && (gru || p.sv_h);
+        const bool cand_h = p.epi == EPI_CAND && (gated || p.sv_h);
         auto load_ops = [&](int c, float (&hb)[8], float (&ub)[8]) {   // operands of chunk c (if it exists)
             const int colp = colb + c * 8;
             if (c >= nchunks) return;
             if (p.epi == EPI_CAND) {
                 if (colp >= DP) return;
                 if (cand_h) chunk_load(p.h_chk, NKC, tile, colp >> 3, row, hb);
-                if (gru) chunk_load(p.u_buf, NKC, tile, colp >> 3, row, ub);
+                if (gated) chunk_load(p.u_buf, NKC, tile, colp >> 3, row, ub);
             } else if (p.epi == EPI_GATE) {
                 if (colp < DP) chunk_load(p.h_chk, NKC, tile, colp >> 3, row, hb);
+            } else if (p.epi == EPI_HPROJ) {
+                if (colp < DP) chunk_load(p.rq_chk, NKC, tile, colp >> 3, row, hb);   // r
             }
         };
         if (!GATHER) load_ops(cgp, hA, uA);
@@ -468,14 +480,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_stream_kernel(const __grid_c
 #pragma unroll
                     for (int j = 0; j < 8; ++j) g[j] = tc::sigmoid_fast(g[j] + b[j]);
                     if (is_r) {
-                        float rh[8];
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) rh[j] = g[j] * h[j];
                         if (p.sv_r && row_ok) {
                             tc::store8_guarded(p.sv_r + (size_t)grow * D, col, D, g);
                             tc::store8_guarded(p.sv_h + (size_t)grow * D, col, D, h);
                         }
-                        img_store_chunk(p.img_out, NKS, tile, row, col, rh);
+                        if (cudnn) {   // r itself: the hidden-projection launch multiplies it by q
+                            chunk_store(p.rq_chk, NKC, tile, col >> 3, row, g);
+                        } else {
+                            float rh[8];
+#pragma unroll
+                            for (int j = 0; j < 8; ++j) rh[j] = g[j] * h[j];
+                            img_store_chunk(p.img_out, NKS, tile, row, col, rh);
+                        }
                     } else {
                         chunk_store(p.u_buf, NKC, tile, col >> 3, row, g);
                         if (p.sv_u && row_ok) tc::store8_guarded(p.sv_u + (size_t)grow * D, col, D, g);
@@ -484,6 +500,25 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_stream_kernel(const __grid_c
                 };
                 for (int c = cgp; c < nchunks; c += NCG)
                     if (!gate_chunk(c, hA, uA)) break;
+            } else if (p.epi == EPI_HPROJ) {
+                // CudnnCompatibleGRUCell: q = h . K_hid + b_hid (saved for the backward pass), and the r chunk becomes r*q
+                auto hproj_chunk = [&](int c, float (&hb)[8], float (&ub)[8]) -> bool {
+                    const int col = colb + c * 8;
+                    if (c >= nchunks || col >= DP) return false;
+                    float q[8], b[8], r[8];
+                    tc::lds8(acc_row + c * 8, q);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) r[j] = hb[j];
+                    load_ops(c + NCG, hb, ub);
+                    tc::load8_guarded(p.b_hid, col, D, b);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) { q[j] += b[j]; r[j] *= q[j]; }
+                    if (p.sv_q && row_ok) tc::store8_guarded(p.sv_q + (size_t)grow * D, col, D, q);
+                    chunk_store(p.rq_chk, NKC, tile, col >> 3, row, r);
+                    return true;
+                };
+                for (int c = cgp; c < nchunks; c += NCG)
+                    if (!hproj_chunk(c, hA, uA)) break;
             } else {
                 auto cand_chunk = [&](int c, float (&hb)[8], float (&ub)[8]) -> bool {
                     const int col = colb + c * 8;
@@ -494,12 +529,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_stream_kernel(const __grid_c
                     for (int j = 0; j < 8; ++j) { h[j] = hb[j]; u[j] = ub[j]; }
                     load_ops(c + NCG, hb, ub);
                     tc::load8_guarded(p.bias, col, D, b);
-                    if (gru) {
+                    if (gated) {
+                        if (cudnn) {   // c = tanh(x . K_in + b_in + r*q), r*q from the hidden-projection launch
+                            float rq[8];
+                            chunk_load(p.rq_chk, NKC, tile, col >> 3, row, rq);
 #pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            cv[j] = tc::act_fast(cv[j] + b[j], p.act);
-                            hn[j] = fmaf(u[j], h[j] - cv[j], cv[j]);   // u*h + (1-u)*c
+                            for (int j = 0; j < 8; ++j) cv[j] = tc::act_fast(cv[j] + b[j] + rq[j], p.act);
+                        } else {
+#pragma unroll
+                            for (int j = 0; j < 8; ++j) cv[j] = tc::act_fast(cv[j] + b[j], p.act);
                         }
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) hn[j] = fmaf(u[j], h[j] - cv[j], cv[j]);   // u*h + (1-u)*c
                         if (p.sv_c && row_ok) tc::store8_guarded(p.sv_c + (size_t)grow * D, col, D, cv);
                     } else {
 #pragma unroll

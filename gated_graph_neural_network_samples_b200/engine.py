@@ -49,10 +49,13 @@ def weight_shapes(params: dict, num_edge_types: int, layer_idx: int) -> Dict[str
     return shapes
 
 
-def make_config(params: dict, num_edge_types: int, device: int = 0, precision: str = "fp32", attention_tensor_cores: bool = False):
+def make_config(params: dict, num_edge_types: int, device: int = 0, precision: str = "fp32", attention_tensor_cores: bool = False,
+                cudnn_gru_tensor_cores: bool = False):
     """``ggnn_config`` of a parameter dict (the keys the two hooks read, sparse:40-61) + the ctypes arrays it points into (keep them alive).
     ``attention_tensor_cores``: propagation attention runs at ``precision`` (GGNN_ATT_TENSOR_CORES: on bf16x3 / bf16 the streaming wgmma
-    plan) instead of on the fp32 kernels; it changes nothing when attention is off."""
+    plan) instead of on the fp32 kernels; it changes nothing when attention is off.  ``cudnn_gru_tensor_cores``: CudnnCompatibleGRUCell
+    runs at ``precision`` (GGNN_CELL_CUDNN_GRU_TENSOR_CORES: on bf16x3 / bf16 the streaming wgmma plan) instead of on the fp32 kernels; it
+    changes nothing for the other cells."""
     steps = [int(s) for s in params["layer_timesteps"]]
     L = len(steps)
     act = params.get("graph_rnn_activation", "tanh").lower()
@@ -71,9 +74,12 @@ def make_config(params: dict, num_edge_types: int, device: int = 0, precision: s
     att = _lib.ATT_OFF
     if params.get("use_propagation_attention", False):
         att = _lib.ATT_TENSOR_CORES if attention_tensor_cores else _lib.ATT_FP32
+    code = CELL_CODES[cell]
+    if cell == "cudnncompatiblegrucell" and cudnn_gru_tensor_cores:
+        code = _lib.CELL_CUDNN_GRU_TENSOR_CORES
     cfg = _lib.GgnnConfig(int(params["hidden_size"]), int(num_edge_types), L, keep[0], keep[1], keep[2],
                           int(bool(params.get("use_edge_bias", False))), int(bool(params.get("use_edge_msg_avg_aggregation", False))),
-                          CELL_CODES[cell], 0 if act == "tanh" else 1, PRECISIONS[precision], int(device), att)
+                          code, 0 if act == "tanh" else 1, PRECISIONS[precision], int(device), att)
     return cfg, keep
 
 
@@ -110,11 +116,11 @@ class PreparedGraph:
     @classmethod
     def host_only(cls, params: dict, num_edge_types: int, adjacency_lists, num_incoming_edges_per_type, precision: str = "fp32",
                   num_sms: int = 132, save_for_backward: bool = False, reuse: Optional["PreparedGraph"] = None,
-                  attention_tensor_cores: bool = False) -> "PreparedGraph":
-        """``ggnn_host_prepare_graph_sparse``: no engine, no GPU (plain memory instead of pinned).  ``attention_tensor_cores``: as in
-        ``make_config``."""
+                  attention_tensor_cores: bool = False, cudnn_gru_tensor_cores: bool = False) -> "PreparedGraph":
+        """``ggnn_host_prepare_graph_sparse``: no engine, no GPU (plain memory instead of pinned).  ``attention_tensor_cores``,
+        ``cudnn_gru_tensor_cores``: as in ``make_config``."""
         g = reuse if reuse is not None else cls()
-        cfg, keep = make_config(params, num_edge_types, 0, precision, attention_tensor_cores)
+        cfg, keep = make_config(params, num_edge_types, 0, precision, attention_tensor_cores, cudnn_gru_tensor_cores)
         T = int(num_edge_types)
         adjs = [np.ascontiguousarray(np.asarray(a, dtype=np.int32).reshape(-1, 2)) for a in adjacency_lists]
         indeg = np.ascontiguousarray(np.asarray(num_incoming_edges_per_type, dtype=np.float32))
@@ -323,11 +329,11 @@ class DeviceDataset:
 
     @classmethod
     def host_only(cls, params: dict, num_edge_types: int, flat, precision: str = "fp32", num_sms: int = 132,
-                  for_training: bool = True, attention_tensor_cores: bool = False) -> "DeviceDataset":
-        """``ggnn_host_dataset_create_sparse``: the GGNN dataset's host summaries, no engine, no GPU.  ``attention_tensor_cores``: as in
-        ``make_config``."""
+                  for_training: bool = True, attention_tensor_cores: bool = False, cudnn_gru_tensor_cores: bool = False) -> "DeviceDataset":
+        """``ggnn_host_dataset_create_sparse``: the GGNN dataset's host summaries, no engine, no GPU.  ``attention_tensor_cores``,
+        ``cudnn_gru_tensor_cores``: as in ``make_config``."""
         d = cls()
-        cfg, keep = make_config(params, num_edge_types, 0, precision, attention_tensor_cores)
+        cfg, keep = make_config(params, num_edge_types, 0, precision, attention_tensor_cores, cudnn_gru_tensor_cores)
         edges, offsets, indeg = cls._sparse_arrays(flat, int(num_edge_types))
         keep = [keep, edges, offsets, indeg]
         ptrs = (C.c_void_p * max(int(num_edge_types), 1))(*[e.ctypes.data for e in edges])
@@ -417,15 +423,17 @@ class DatasetBatch:
 
 
 class PropagationEngine:
-    def __init__(self, params: dict, num_edge_types: int, device: int = 0, precision: str = "fp32", attention_tensor_cores: bool = False):
-        """``attention_tensor_cores``: propagation attention at ``precision`` instead of on the fp32 kernels (see ``make_config``)."""
+    def __init__(self, params: dict, num_edge_types: int, device: int = 0, precision: str = "fp32", attention_tensor_cores: bool = False,
+                 cudnn_gru_tensor_cores: bool = False):
+        """``attention_tensor_cores``: propagation attention at ``precision`` instead of on the fp32 kernels; ``cudnn_gru_tensor_cores``:
+        CudnnCompatibleGRUCell at ``precision`` likewise (see ``make_config``)."""
         self._h = C.c_void_p()
         self.lib = _lib.load()
         self.params = dict(params)
         self.D = int(params["hidden_size"])
         self.T = int(num_edge_types)
         self.L = len(params["layer_timesteps"])
-        cfg, self._cfg_keepalive = make_config(params, num_edge_types, device, precision, attention_tensor_cores)
+        cfg, self._cfg_keepalive = make_config(params, num_edge_types, device, precision, attention_tensor_cores, cudnn_gru_tensor_cores)
         rc = self.lib.ggnn_create(C.byref(cfg), C.byref(self._h))
         if rc != 0:
             self._h = C.c_void_p()

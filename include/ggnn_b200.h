@@ -33,7 +33,13 @@ typedef void* ggnn_stream_t; /* a cudaStream_t (0 = default stream) */
 
 enum { GGNN_OK = 0, GGNN_EINVAL = -1, GGNN_ECUDA = -2, GGNN_ESTATE = -3, GGNN_EUNSUPPORTED = -4, GGNN_ERANGE = -5 };
 enum { GGNN_CELL_GRU = 0, GGNN_CELL_RNN = 1,    /* params['graph_rnn_cell']        sparse:102-112 */
-       GGNN_CELL_CUDNN_GRU = 2 };               /* 'CudnnCompatibleGRUCell', sparse:105-108 (fp32 path; tanh only, as the reference asserts) */
+       GGNN_CELL_CUDNN_GRU = 2,                 /* 'CudnnCompatibleGRUCell', sparse:105-108 (fp32 path at every precision; tanh only, as the
+                                                   reference asserts) */
+       GGNN_CELL_CUDNN_GRU_TENSOR_CORES = 3 };  /* CudnnCompatibleGRUCell at the configured precision: the same weights, cand_hidden_bias, tanh
+                                                   requirement and gradients as GGNN_CELL_CUDNN_GRU; on GGNN_PREC_BF16X3 / GGNN_PREC_BF16 every batch
+                                                   takes the streaming wgmma plan (a hidden-projection GEMM per step), on GGNN_PREC_FP32 and with
+                                                   GGNN_ATT_FP32 attention exactly GGNN_CELL_CUDNN_GRU.  Sparse model only: the dense entries and
+                                                   the dense dataset refuse it (GGNN_EUNSUPPORTED) */
 enum { GGNN_ACT_TANH = 0, GGNN_ACT_RELU = 1 };  /* params['graph_rnn_activation']  sparse:75-81   */
 /* arithmetic of the dense contractions */
 enum { GGNN_PREC_FP32 = 0,   /* fp32 FFMA on CUDA cores (bit-for-bit fp32 semantics, order aside) */
@@ -44,7 +50,9 @@ enum { GGNN_ATT_OFF = 0,
        GGNN_ATT_FP32 = 1,           /* attention on the fp32 kernels whatever the precision (every nonzero value but 2 means this) */
        GGNN_ATT_TENSOR_CORES = 2 }; /* attention at the configured precision: on GGNN_PREC_BF16X3 / GGNN_PREC_BF16 every batch takes the
                                        streaming wgmma plan (a softmax pre-pass per step feeding the slot-weighted gather); on
-                                       GGNN_PREC_FP32, and with CudnnCompatibleGRUCell, exactly GGNN_ATT_FP32 */
+                                       GGNN_PREC_FP32, and with GGNN_CELL_CUDNN_GRU, exactly GGNN_ATT_FP32; with
+                                       GGNN_CELL_CUDNN_GRU_TENSOR_CORES the streaming plan runs both the pre-pass and the cell's
+                                       hidden-projection GEMM */
 
 /* Mirrors the keys of self.params the two hooks read (sparse:40-61, chem_tensorflow.py:17-37). */
 typedef struct ggnn_config {
@@ -101,9 +109,9 @@ typedef struct ggnn_layer_grads {
 /* prepare_specific_graph_model (sparse:63-115 / dense:68-91): fix the model shape.
  * Limits: hidden_size a positive multiple of 4 and <= 512 (larger: GGNN_EUNSUPPORTED), 1 <= num_edge_types <= 32 (<= 16 with propagation
  * attention), 1 <= num_layers <= 16, at most 4 residual inputs per layer.  Kernels by hidden size: GGNN_PREC_BF16X3 / GGNN_PREC_BF16 run
- * the tile-local wgmma kernel up to 128 and the streaming wgmma kernels above; attention with GGNN_ATT_TENSOR_CORES runs the streaming
- * wgmma kernels at every hidden size.  GGNN_PREC_FP32 (and GGNN_ATT_FP32 attention, and CudnnCompatibleGRUCell, at any precision) runs
- * the fused fp32 tile kernel up to 256 and the per-timestep fp32 path above 256.  A weighted dense adjacency runs on
+ * the tile-local wgmma kernel up to 128 and the streaming wgmma kernels above; attention with GGNN_ATT_TENSOR_CORES, and
+ * GGNN_CELL_CUDNN_GRU_TENSOR_CORES, run the streaming wgmma kernels at every hidden size.  GGNN_PREC_FP32 (and GGNN_ATT_FP32 attention, and
+ * GGNN_CELL_CUDNN_GRU, at any precision) runs the fused fp32 tile kernel up to 256 and the per-timestep fp32 path above 256.  A weighted dense adjacency runs on
  * tensor cores up to hidden 128 on the tile-local kernel (GLOBAL when a component exceeds 128 rows) whichever dense entry feeds it; above
  * 128, ggnn_set_graph_dense / ggnn_run_dense_host(_predict) refuse it as before (run it on GGNN_PREC_FP32), and the ..._dense_weighted
  * entries run it on the streaming kernels, whose gather sums each weighted (target, type) pair into a virtual row. */
