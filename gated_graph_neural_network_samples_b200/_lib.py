@@ -43,7 +43,7 @@ class GgnnLayerGrads(C.Structure):
 
 class GcnConfig(C.Structure):
     _fields_ = [("hidden_size", C.c_int32), ("num_layers", C.c_int32), ("use_bias", C.c_int32), ("precision", C.c_int32),
-                ("device", C.c_int32)]
+                ("device", C.c_int32), ("wide_hidden", C.c_int32)]
 
 
 class GcnLayerWeights(C.Structure):

@@ -47,6 +47,9 @@ class DenseGGNNChemModel(ChemModel):
             raise Exception("--attention-tensor-cores applies to the sparse GGNN model's propagation attention; the dense model has none")
         if self.cudnn_gru_tensor_cores:
             raise Exception("--cudnn-gru-tensor-cores applies to the sparse GGNN model's CudnnCompatibleGRUCell; the dense model has no cell option")
+        if self.gcn_wide_hidden:
+            raise Exception("--gcn-wide-hidden applies to the sparse GCN model's hidden sizes; the dense model runs hidden sizes up to 512 "
+                            "without it")
         self.engine = PropagationEngine(dense_engine_params(dict(self.params, hidden_size=self._padded_hidden)), T,
                                         device=self.device.index or 0, precision=self.precision)
         self._apply_backward_precision(self.engine)

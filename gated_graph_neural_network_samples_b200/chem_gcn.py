@@ -95,8 +95,9 @@ class SparseGCNChemModel(ChemModel):
             raise Exception("--attention-tensor-cores applies to the sparse GGNN model's propagation attention; the GCN model has none")
         if self.cudnn_gru_tensor_cores:
             raise Exception("--cudnn-gru-tensor-cores applies to the sparse GGNN model's CudnnCompatibleGRUCell; the GCN model has no RNN cell")
+        wide = {'wide_hidden': True} if self.gcn_wide_hidden else {}   # the keyword only when the option was given
         self.engine = GCNEngine(self._padded_hidden, L, self.params['gcn_use_bias'], device=self.device.index or 0,
-                                precision=self.precision)
+                                precision=self.precision, **wide)
         self._apply_backward_precision(self.engine)
         self._propagation = _propagation_function()
         self._readout = gated_readout_function()

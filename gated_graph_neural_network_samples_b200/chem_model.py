@@ -67,6 +67,9 @@ class ChemModel(object):
         # --cudnn-gru-tensor-cores: the sparse GGNN model's CudnnCompatibleGRUCell runs at --precision likewise.  Both are command-line options,
         # not params keys: the trainables are the same, so a checkpoint restores into a model with or without them
         self.cudnn_gru_tensor_cores = bool(args.get('--cudnn-gru-tensor-cores'))
+        # --gcn-wide-hidden: the sparse GCN model accepts hidden sizes up to 512 and runs those above 128 at --precision (on bf16x3 / bf16 the
+        # streaming wgmma plan) instead of on its fp32 kernel.  An option for the same reason: the trainables do not change
+        self.gcn_wide_hidden = bool(args.get('--gcn-wide-hidden'))
         # --device-data: the plug-in uploads each data list once (engine.DeviceDataset) and assembles every batch on the GPU instead of
         # packing it on the host; same shuffle, same batches, same numbers.  A command-line option, not a params key: params are what a
         # checkpoint must match (restore_progress), and where the data lives does not change the model.

@@ -125,6 +125,9 @@ class SparseGGNNChemModel(ChemModel):
         # exactly 0 through every cell (c = act(0) = 0, h' = u*0 + (1-u)*0) and out of every real unit's sums -- hook 2 pads, the engine
         # works at the padded width, the result is sliced back.  Variables keep the reference's shapes.
         self._padded_hidden = (h_dim + 3) // 4 * 4
+        if self.gcn_wide_hidden:
+            raise Exception("--gcn-wide-hidden applies to the sparse GCN model's hidden sizes; the sparse GGNN model runs hidden sizes up to 512 "
+                            "without it")
         # the keyword only when the option was given (an engine without it keeps working)
         att = {'attention_tensor_cores': True} if self.attention_tensor_cores else {}
         if self.cudnn_gru_tensor_cores:

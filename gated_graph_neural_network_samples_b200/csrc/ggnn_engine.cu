@@ -140,6 +140,7 @@ struct ModelShape {
     int use_att = 0;    // use_propagation_attention (sparse:170-196): on the fp32 kernels, or on the streaming wgmma kernels when the
                         // precision is not fp32 (GGNN_ATT_TENSOR_CORES)
     int cudnn_tc = 0;   // GGNN_CELL_CUDNN_GRU_TENSOR_CORES: cell is CELL_CUDNN_GRU and keeps the configured precision (the streaming plan)
+    int wide_hidden = 0;   // GCN, ggnn_gcn_config.wide_hidden: hidden sizes up to 512, on the streaming plan above 128 on bf16x3 / bf16
     int num_sms = 132;
     size_t max_smem = 0;
 };
@@ -500,6 +501,10 @@ int pack_to_fill_chip(const std::vector<int>& cuts, int V, int max_span, int num
     return tc::TILE_M;
 }
 
+// Whether a GCN runs on the streaming plan: hidden sizes above 128 on the tensor-core precisions, when its config asked for wide_hidden (else
+// those sizes run the fp32 kernel, up to 256).
+bool gcn_streams(const ModelShape& s) { return s.wide_hidden && s.precision != GGNN_PREC_FP32 && s.DP > 128; }
+
 // The tile plan of a batch of V nodes: which kernel, and the tiles.  `cuts` are the sorted node indices where the batch may be split
 // between connected components (cuts.front() == 0, cuts.back() == V); `weighted`: every message has a weight; `stream_weighted`: a weighted
 // batch may take the streaming plan above hidden 128 on the tensor-core precisions (the ..._dense_weighted entries), else it is refused
@@ -516,7 +521,17 @@ int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>
     const bool force_global = fg && fg[0] == '1';
     const char* prec = s.precision == GGNN_PREC_BF16X3 ? "bf16x3" : "bf16";
     char buf[256];
-    if (s.model == MODEL_GCN) {
+    if (s.model == MODEL_GCN && gcn_streams(s)) {
+        // streaming plan (wide_hidden, hidden > 128, bf16x3 / bf16): fixed 128-row tiles, per layer a weighted gather into the operand
+        // image and one TMA-fed streaming GEMM launch of N blocks of MMA_N columns.  No pair tables: the gather reads the target CSR.
+        p.variant = 4;
+        fixed_tiles(V, ts::TILE_M, tile_start);
+        p.ntiles = (int)tile_start.size() - 1;
+        p.ts_nblk[0] = (s.DP + ts::MMA_N - 1) / ts::MMA_N;
+        p.ts_nc[0] = ts::MMA_N;
+        snprintf(buf, sizeof buf, "gcn-stream-%s (2 launches per layer: weighted gather, GEMM) tiles=%d DP=%d N-blocks=%dx%d", prec, p.ntiles,
+                 s.DP, p.ts_nblk[0], p.ts_nc[0]);
+    } else if (s.model == MODEL_GCN) {
         // wgmma path (hidden <= 128, bf16x3 / bf16): LOCAL when every connected component fits a 128-row tile -- tiles are unions of whole
         // components, shrunk like the GGNN plan when the batch cannot fill the chip -- else GLOBAL with fixed 128-row tiles.  fp32 path:
         // fixed 32-row blocks, one launch per layer.
@@ -967,7 +982,7 @@ const char* ggnn_last_error(const ggnn_engine* e) { return e ? e->err.c_str() : 
 
 // The checks and fields both model configs have; no CUDA (the text goes to `err`: this may run in any thread).
 // `max_hidden`: the widest hidden size of the model's kernels (GGNN 512: the readout and the attention backward hold 16 columns per lane;
-// GCN 256: its fp32 kernel).
+// GCN 256 by default, as before its streaming plan existed; 512 with wide_hidden).
 static int init_common_shape(ModelShape& s, int hidden_size, int max_hidden, int num_layers, int precision, int device, std::string& err) {
     if (hidden_size <= 0 || hidden_size % 4 != 0) { err = "hidden_size must be a positive multiple of 4"; return GGNN_EINVAL; }
     if (hidden_size > max_hidden) { err = "hidden_size > " + std::to_string(max_hidden) + " is not supported by this build"; return GGNN_EUNSUPPORTED; }
@@ -1029,8 +1044,10 @@ static int init_model_shape(ModelShape& s, const ggnn_config* cfg, std::string& 
 // The model shape of a ggnn_gcn_config (chem_tensorflow_gcn.py:42-82): one edge type, one "timestep" per layer (the dropout's global step
 // is the layer index).
 static int init_gcn_shape(ModelShape& s, const ggnn_gcn_config* cfg, std::string& err) {
-    if (int rc = init_common_shape(s, cfg->hidden_size, 256, cfg->num_layers, cfg->precision, cfg->device, err)) return rc;
+    const int max_hidden = cfg->wide_hidden ? 512 : 256;
+    if (int rc = init_common_shape(s, cfg->hidden_size, max_hidden, cfg->num_layers, cfg->precision, cfg->device, err)) return rc;
     s.model = MODEL_GCN;
+    s.wide_hidden = cfg->wide_hidden != 0;
     s.T = 1;
     s.use_bias = cfg->use_bias != 0;
     s.cell = CELL_RNN; s.act = ACT_RELU;
@@ -1531,7 +1548,8 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     if (const char* nt = getenv("GGNN_HOST_THREADS")) nth = std::max(1, std::min(atoi(nt), 64));
 #endif
     // ---- pass 1: validate, count per (target,type), mark which node boundaries are spanned by an edge (the cut points of the tile-local
-    // plans; the streaming plan of hidden sizes > 128 and the per-timestep fp32 path above 256 tile by fixed 128-row blocks and skip that part)
+    // plans; the streaming plan of hidden sizes > 128 and the per-timestep fp32 path above 256 tile by fixed 128-row blocks and skip that part.
+    // A GCN needs them only on its wgmma kernel (DP <= 128 on bf16x3 / bf16): its fp32 kernel and its streaming plan tile by fixed blocks)
     std::vector<int>& counts = g->h_counts;
     std::vector<int>& reach = g->h_diff;   // reach[j] = the farthest node an edge whose lower end is node j touches
     const bool need_cuts = shape.precision == GGNN_PREC_FP32 ? shape.D <= 256 : shape.DP <= 128;
@@ -1840,7 +1858,8 @@ static int check_batch_shape(ggnn_engine* e, const ModelShape& q, const BatchPla
     if (q.model != e->model)
         return e->fail(GGNN_ESTATE, "the %s was built for a %s engine, this is a %s engine", what, q.model == MODEL_GCN ? "GCN" : "GGNN",
                        e->model == MODEL_GCN ? "GCN" : "GGNN");
-    if (q.D != e->D || q.T != e->T || q.precision != e->precision || q.DP != e->DP || q.num_sms != e->num_sms || q.cell != e->cell || q.use_att != e->use_att)
+    if (q.D != e->D || q.T != e->T || q.precision != e->precision || q.DP != e->DP || q.num_sms != e->num_sms || q.cell != e->cell || q.use_att != e->use_att ||
+        q.wide_hidden != e->wide_hidden)
         return e->fail(GGNN_EINVAL, "the %s was built for a different engine configuration", what);
     if (e->save && !p.has_transpose)
         return e->fail(GGNN_ESTATE, "save_for_backward is on but the %s was prepared without it (the source-keyed CSR is built at prepare time)", what);
@@ -2245,14 +2264,15 @@ static int forward_tc(ggnn_engine* e, const float* h0, float* h_out, cudaStream_
 // ------------------------------------------------------------------------------------------ streaming tensor-core path (host)
 // The streaming layout (ggnn_fwd_stream.cuh): per layer, in N blocks of ts_nc columns, the T edge blocks, the gate and the candidate kernel.
 // CudnnCompatibleGRUCell splits the candidate kernel in two: K_in (its first (R+1) D rows, the [res.. | agg] segments) and, at off_hproj,
-// K_hid (its last D rows, one segment).
+// K_hid (its last D rows, one segment).  A GCN layer is one segment: W_l at off_edge.
 static int ts_prepare_weights(ggnn_engine* e, cudaStream_t st) {
     const int D = e->D, DP = e->DP, T = e->T, NKS = DP / 16;
     const int nc0 = e->ts_nc[0], nb0 = e->ts_nblk[0], nc1 = e->ts_nc[1], nb1 = e->ts_nblk[1];
-    const bool cudnn = e->cell == CELL_CUDNN_GRU;
+    const bool cudnn = e->cell == CELL_CUDNN_GRU, gcn = e->model == MODEL_GCN;
     WeightTiles& c = e->ts_tiles;
     size_t off = 0;
     for (int l = 0; l < e->L; ++l) {
+        if (gcn) { c.off_edge[l] = off; off += (size_t)nb0 * NKS * 64 * nc0; continue; }
         const int nseg = e->nres[l] + 2, ncand = cudnn ? nseg - 1 : nseg;
         c.off_edge[l] = off; off += (size_t)nb0 * T * NKS * 64 * nc0;
         c.off_gate[l] = off; off += (size_t)nb1 * nseg * NKS * 64 * nc1;
@@ -2271,6 +2291,7 @@ static int ts_prepare_weights(ggnn_engine* e, cudaStream_t st) {
             ts::ggnn_tile_weights_stream_kernel<<<blocks, 256, 0, st>>>(W, out, D, DP, segs, ncolblk, src_ld, NC, nblk);
             ++e->last_launches;
         };
+        if (gcn) { launch(e->gcn_w[l].kernel, base + c.off_edge[l], 1, 1, D, nc0, nb0); continue; }
         launch(e->w[l].edge_weights, base + c.off_edge[l], T, 1, D, nc0, nb0);
         if (e->cell != CELL_RNN) launch(e->w[l].gate_kernel, base + c.off_gate[l], nseg, 2, 2 * D, nc1, nb1);
         if (cudnn) {
@@ -2283,6 +2304,40 @@ static int ts_prepare_weights(ggnn_engine* e, cudaStream_t st) {
     CU_TRY(e, cudaGetLastError());
     c.gen = e->weights_gen;
     return GGNN_OK;
+}
+
+// The ring of the streaming kernels and the two instances a forward launches (the GGNN's and the GCN's streaming forward).  A ring stage
+// carries KS K-steps, the largest of 4, 2, 1 that divides the K-steps of a segment (the producer thread pays several hundred cycles per bulk
+// copy whatever its size; KS is a template parameter so that a stage's MMAs are straight-line code); GGNN_TS_KSTEPS caps it and
+// GGNN_TS_STAGES caps the ring depth.  `edge` is the gather-fed instance, `fed` the TMA-fed one.
+struct StreamLaunch {
+    int KS = 4;
+    int max_ns = ts::MAX_NS;   // the kernel has MAX_NS stage barriers
+    void (*edge)(ts::StreamParams) = nullptr;
+    void (*fed)(ts::StreamParams) = nullptr;
+    size_t stage_bytes(int NC) const { return (size_t)KS * ((size_t)ts::A_STAGE_B + 64 * (size_t)NC); }
+    int stages(int NC, size_t budget) const { return (int)std::min<size_t>((size_t)max_ns, budget / stage_bytes(NC)); }
+    size_t smem(int NC, int ns, size_t extra) const { return (size_t)1024 + ts::ring_bytes(ns, stage_bytes(NC)) + extra; }
+};
+
+static StreamLaunch stream_launch(const ggnn_engine* e) {
+    StreamLaunch k;
+    const int NKS = e->DP / 16;
+    const char* env_ks = getenv("GGNN_TS_KSTEPS");
+    const char* env_ns = getenv("GGNN_TS_STAGES");
+    if (env_ks) k.KS = atoi(env_ks) >= 4 ? 4 : (atoi(env_ks) >= 2 ? 2 : 1);
+    while (NKS % k.KS) k.KS /= 2;
+    if (env_ns) k.max_ns = std::max(0, std::min(atoi(env_ns), ts::MAX_NS));
+    const bool x3 = e->precision == GGNN_PREC_BF16X3;
+    const int KS = k.KS;
+#define GGNN_TS_PICK(X, K)                              \
+    if (x3 == X && KS == K) {                           \
+        k.edge = ts::ggnn_stream_kernel<true, X, K>;    \
+        k.fed = ts::ggnn_stream_kernel<false, X, K>;    \
+    }
+    GGNN_TS_PICK(true, 4) GGNN_TS_PICK(true, 2) GGNN_TS_PICK(true, 1) GGNN_TS_PICK(false, 4) GGNN_TS_PICK(false, 2) GGNN_TS_PICK(false, 1)
+#undef GGNN_TS_PICK
+    return k;
 }
 
 static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStream_t st) {
@@ -2315,16 +2370,8 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     CU_TRY(e, e->ts_virt.reserve((size_t)((e->ts_nv + ts::TILE_M - 1) / ts::TILE_M + 1) * NKS * ts::A_STAGE_B));
     const size_t att_stride = e->save ? (size_t)std::max<int64_t>(e->M, 1) : 0;   // attention probabilities of a step, [steps][M] when saving
     if (e->use_att) CU_TRY(e, e->att_buf.reserve(sizeof(float) * (size_t)std::max<int64_t>(e->M, 1) * (size_t)(e->save ? std::max(e->total_steps, 1) : 1)));
-    // a ring stage carries KS K-steps, the largest of 4, 2, 1 that divides the K-steps of a segment (the producer thread pays several
-    // hundred cycles per bulk copy whatever its size; KS is a template parameter so that a stage's MMAs are straight-line code)
-    const char* env_ks = getenv("GGNN_TS_KSTEPS");
-    const char* env_ns = getenv("GGNN_TS_STAGES");
-    int KS = 4;
-    if (env_ks) KS = atoi(env_ks) >= 4 ? 4 : (atoi(env_ks) >= 2 ? 2 : 1);
-    while (NKS % KS) KS /= 2;
-    auto stage_bytes = [&](int NC) { return (size_t)KS * ((size_t)ts::A_STAGE_B + 64 * (size_t)NC); };
-    const int max_ns = env_ns ? std::max(0, std::min(atoi(env_ns), ts::MAX_NS)) : ts::MAX_NS;   // the kernel has MAX_NS stage barriers
-    auto stages_for = [&](int NC, size_t budget) { return (int)std::min<size_t>((size_t)max_ns, budget / stage_bytes(NC)); };
+    const StreamLaunch kl = stream_launch(e);
+    auto stages_for = [&](int NC, size_t budget) { return kl.stages(NC, budget); };
     ts::StreamParams base;
     memset(&base, 0, sizeof base);
     base.V = V; base.D = D; base.DP = DP; base.T = T;
@@ -2348,17 +2395,9 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
     if (ns_min < ts::MIN_NS)
         return e->fail(GGNN_EUNSUPPORTED, "streaming ring of %d stages (DP=%d): it needs at least %d, one per gather group", ns_min, DP,
                        ts::MIN_NS);
-    auto smem_of = [&](int NC, int ns, bool gather) { return (size_t)1024 + ts::ring_bytes(ns, stage_bytes(NC)) + (gather ? csr_b : 0); };
-    const bool x3 = e->precision == GGNN_PREC_BF16X3;
-    void (*k_edge)(ts::StreamParams) = nullptr;
-    void (*k_fed)(ts::StreamParams) = nullptr;
-#define GGNN_TS_PICK(X, K)                              \
-    if (x3 == X && KS == K) {                           \
-        k_edge = ts::ggnn_stream_kernel<true, X, K>;    \
-        k_fed = ts::ggnn_stream_kernel<false, X, K>;    \
-    }
-    GGNN_TS_PICK(true, 4) GGNN_TS_PICK(true, 2) GGNN_TS_PICK(true, 1) GGNN_TS_PICK(false, 4) GGNN_TS_PICK(false, 2) GGNN_TS_PICK(false, 1)
-#undef GGNN_TS_PICK
+    auto smem_of = [&](int NC, int ns, bool gather) { return kl.smem(NC, ns, gather ? csr_b : 0); };
+    void (*k_edge)(ts::StreamParams) = kl.edge;
+    void (*k_fed)(ts::StreamParams) = kl.fed;
     const size_t sm_edge = smem_of(nc0, ns_edge, true);
     const size_t sm_fed = std::max(smem_of(nc1, ns_gate, false), smem_of(nc0, ns_cand, false));
     CU_TRY(e, cudaFuncSetAttribute(k_edge, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm_edge));
@@ -2516,10 +2555,53 @@ int ggnn_prepared_graph_slot_weights(const ggnn_prepared_graph* g, float* target
     return GGNN_OK;
 }
 
-// Whether the GCN runs on its wgmma kernel (else on the fp32 kernel, one launch per layer).
+// Whether the GCN runs on its fused wgmma kernel (hidden <= 128); else on the streaming plan (gcn_streams) or on the fp32 kernel, one launch
+// per layer.
 static bool gcn_on_tensor_cores(const ggnn_engine* e) { return e->precision != GGNN_PREC_FP32 && e->DP <= 128; }
 
+// The GCN's streaming plan (wide_hidden, hidden > 128 on bf16x3 / bf16), two launches per layer on fixed 128-row tiles:
+//   gcn_gather_image_kernel  S = A . H_l from the row-major fp32 state -> the operand image (one, reused by every layer)
+//   ggnn_stream_kernel       TMA-fed, one segment: S . W_l, then EPI_GCN (bias; relu and state dropout but on the last layer) -> H_{l+1},
+//                            row-major fp32, on every layer (the backward and ggnn_layer_state read them)
+static int forward_gcn_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStream_t st) {
+    const int D = e->D, DP = e->DP, L = e->L, V = e->V, NKS = DP / 16, ntiles = e->ntiles;
+    if (int rc = ts_prepare_weights(e, st)) return rc;
+    CU_TRY(e, e->ts_images.reserve((size_t)ntiles * NKS * ts::A_STAGE_B));
+    uint8_t* img_s = (uint8_t*)e->ts_images.ptr;
+    const StreamLaunch kl = stream_launch(e);
+    const int nc = e->ts_nc[0], nb = e->ts_nblk[0];
+    const int ns = kl.stages(nc, e->max_smem > 2048 ? e->max_smem - 2048 : 0);
+    if (ns < ts::MIN_NS)
+        return e->fail(GGNN_EUNSUPPORTED, "streaming ring of %d stages (DP=%d): it needs at least %d, one per gather group", ns, DP, ts::MIN_NS);
+    const size_t smem = kl.smem(nc, ns, 0);
+    CU_TRY(e, cudaFuncSetAttribute(kl.fed, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    ts::StreamParams p;
+    memset(&p, 0, sizeof p);
+    p.V = V; p.D = D; p.DP = DP; p.T = 1;
+    p.nparts = e->precision == GGNN_PREC_BF16X3 ? 3 : 1;
+    p.epi = ts::EPI_GCN; p.NC = nc; p.nstages = ns;
+    p.nseg = 1; p.seg[0] = img_s; p.kt_all = NKS;
+    p.drop_keep = e->drop_keep; p.drop_seed = e->drop_seed;
+    p.error_flag = (int*)e->err_flag.ptr;
+    const WeightTiles& wt = e->ts_tiles;
+    const ImageView& gd = e->gd;
+    const long long gather_threads = (long long)ntiles * (ts::TILE_M / 4) * ((DP / 8 + 7) / 8) * 32;
+    for (int l = 0; l < L; ++l) {
+        gcn::gcn_gather_image_kernel<<<(int)((gather_threads + 255) / 256), 256, 0, st>>>(gd.row_ptr, gd.src, gd.slotw,
+                                                                                      layer_state(e, l, h0, h_out), img_s, V, D, DP, ntiles);
+        p.w = (const uint8_t*)wt.buf.ptr + wt.off_edge[l];
+        p.bias = e->gcn_w[l].bias;
+        p.relu_dropout = l < L - 1;
+        p.gstep = l;   // the dropout's global step is the layer index
+        p.h_out = layer_state(e, l + 1, h0, h_out);
+        kl.fed<<<dim3(ntiles, nb), ts::NTHREADS, smem, st>>>(p);
+        e->last_launches += 2;
+    }
+    return GGNN_OK;
+}
+
 static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream_t st) {
+    if (gcn_streams(*e)) return forward_gcn_stream(e, h0, h_out, st);
     const int D = e->D, DP = e->DP, L = e->L, V = e->V;
     const bool tcore = gcn_on_tensor_cores(e);
     gcn::GcnParams p;

@@ -18,6 +18,8 @@
 //   EPI_GATE  as above, but writes r itself (chunk-major fp32) instead of the r*h image
 //   EPI_HPROJ q         = h . K_hid + b_hid                                  saves q, overwrites the r chunk with r*q
 //   EPI_CAND  h'        = u*h + (1-u)*tanh([res.. | agg] . K_in + b_in + r*q)
+// The sparse GCN's streaming plan (ggnn_gcn.cuh, gcn_gather_image_kernel) uses the TMA-fed instance for its layer GEMM:
+//   EPI_GCN   H'        = S . W_l + b_l, then relu and state dropout on every layer but the last    S = A . H, gathered into an image
 // Node-state operands live in HBM/L2 as bf16 hi/lo "images" in the canonical K-major no-swizzle layout, tile-major:
 //   byte(tile, kstep, part, kgroup, row, j) = ((tile*NKS + kstep)*2 + part)*4096 + kgroup*2048 + row*16 + j*2
 // so one K-step of a 128-row A operand (hi + lo) is ONE contiguous 8 KB bulk copy (cp.async.bulk, 1-D TMA), and an
@@ -66,7 +68,7 @@ __host__ __device__ inline size_t ring_bytes(size_t nstages, size_t stage_b) {
     const size_t acc_b = (size_t)TILE_M * ACC_LD * sizeof(float);
     return nstages * stage_b > acc_b ? nstages * stage_b : acc_b;
 }
-enum { EPI_AGG = 0, EPI_GATE = 1, EPI_CAND = 2, EPI_HPROJ = 3 };
+enum { EPI_AGG = 0, EPI_GATE = 1, EPI_CAND = 2, EPI_HPROJ = 3, EPI_GCN = 4 };
 
 struct StreamParams {
     int V, D, DP, T;
@@ -109,6 +111,8 @@ struct StreamParams {
     const float* b_hid;          // HPROJ: cand_hidden_bias [D]
     float* rq_chk;               // chunk-major fp32: r (written by GATE), r*q (HPROJ), read by CAND
     float* sv_q;                 // HPROJ: row-major save slot of q = h . K_hid + b_hid, or null
+    // ---- GCN (EPI_GCN): bias = b_l or null, h_out = H_{l+1} row-major [V][D]
+    int relu_dropout;            // relu, then state dropout (every layer but the last)
     float drop_keep; unsigned long long drop_seed; int gstep;
     int* error_flag;
 };
@@ -500,6 +504,28 @@ __global__ void __launch_bounds__(NTHREADS, 1) ggnn_stream_kernel(const __grid_c
                 };
                 for (int c = cgp; c < nchunks; c += NCG)
                     if (!gate_chunk(c, hA, uA)) break;
+            } else if (p.epi == EPI_GCN) {
+                // GCN layer: the arithmetic and the dropout mask of gcn::epilogue (ggnn_gcn.cuh); only the D real columns are written
+                for (int c = cgp; c < nchunks && row_ok; c += NCG) {
+                    const int col = colb + c * 8;
+                    if (col >= D) break;
+                    float v[8];
+                    tc::lds8(acc_row + c * 8, v);
+                    if (p.bias) {
+                        float b[8];
+                        tc::load8_guarded(p.bias, col, D, b);
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) v[j] += b[j];
+                    }
+                    if (p.relu_dropout) {
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            v[j] = fmaxf(v[j], 0.0f);
+                            if (p.drop_keep < 1.0f) v[j] = dropout_apply(v[j], p.drop_seed, p.gstep, p.V, D, grow, col + j, p.drop_keep);
+                        }
+                    }
+                    tc::store8_guarded(p.h_out + (size_t)grow * D, col, D, v);
+                }
             } else if (p.epi == EPI_HPROJ) {
                 // CudnnCompatibleGRUCell: q = h . K_hid + b_hid (saved for the backward pass), and the r chunk becomes r*q
                 auto hproj_chunk = [&](int c, float (&hb)[8], float (&ub)[8]) -> bool {

@@ -11,11 +11,14 @@
 //                     columns NH*(w/2) .. +NH (NH = DP/2) of S . W; S is split into bf16 hi/lo in the canonical no-swizzle K-major layout.
 //                     The pre-split, pre-tiled W_l (tc::ggnn_tile_weights_kernel) streams through the tile kernels' weight ring
 //                     (tc::RingWriter / tc::RingReader, tc::gemm_narrow); a timeout sets the engine's error flag (ggnn_sync_check).
-//   gcn_fp32_kernel   fp32 precision and hidden sizes in (128, 256]: per layer, 32 rows per CTA, weighted CSR gather into shared memory,
-//                     FFMA GEMM with W_l from L1/L2, same epilogue.
+//   gcn_fp32_kernel   fp32 precision, and hidden sizes above 128 without ggnn_gcn_config.wide_hidden: per layer, 32 rows per CTA,
+//                     weighted CSR gather into shared memory, FFMA GEMM with W_l from L1/L2, same epilogue.
+//   gcn_gather_image_kernel  hidden sizes above 128 on bf16x3 / bf16 with wide_hidden: S = A . H into the streaming operand image, which the
+//                     TMA-fed ts::ggnn_stream_kernel multiplies by W_l (EPI_GCN: the same epilogue); two launches per layer.
 // The backward pass (ggnn_engine.cu) reuses ggnn_bwd.cuh; only the relu / dropout gradient below is GCN-specific.
 #pragma once
 #include "ggnn_common.cuh"
+#include "ggnn_fwd_stream.cuh"
 #include "ggnn_fwd_tc.cuh"
 #include "ggnn_wgmma.cuh"
 
@@ -222,6 +225,38 @@ __global__ void __launch_bounds__(F32_THREADS) gcn_fp32_kernel(const __grid_cons
             *reinterpret_cast<float4*>(out + (size_t)v * D + c) = o;
         }
     }
+}
+
+// ------------------------------------------------------------------------------------------------ streaming plan: the gather
+// S = A . H of one layer, straight into the tile-major bf16 hi/lo operand image of ggnn_fwd_stream.cuh (ts::img_store_chunk), from the
+// layer input's row-major fp32 state.  The arithmetic of gcn_wgmma_kernel's gather: per (row, 8 columns), acc = fmaf(w, x, acc) from 0 over
+// the row's target-CSR slots in list order.  Rows V .. ntiles*128 and columns D .. DP are written as zeros; no read leaves the V x D state.
+// A warp covers 4 rows x 8 column chunks, so each message it reads is 256 contiguous bytes of a row and each image store 64 contiguous
+// bytes of a k-group.
+__global__ void __launch_bounds__(256) gcn_gather_image_kernel(const int* __restrict__ row_ptr, const int* __restrict__ csr_src,
+                                                               const float* __restrict__ slot_w, const float* __restrict__ h,
+                                                               uint8_t* __restrict__ img, int V, int D, int DP, int ntiles) {
+    const int NKC = DP >> 3, NKS = DP >> 4, ncg = (NKC + 7) >> 3;
+    const long long nwarps = (long long)ntiles * (ts::TILE_M / 4) * ncg;
+    const long long w = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (w >= nwarps) return;
+    const int rg = (int)(w / ncg), cg = (int)(w - (long long)rg * ncg);
+    const int row = rg * 4 + (lane & 3), kc = cg * 8 + (lane >> 2);
+    if (kc >= NKC) return;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (row < V) {
+        const int beg = __ldg(row_ptr + row), end = __ldg(row_ptr + row + 1);
+        for (int m = beg; m < end; ++m) {
+            const int s = __ldg(csr_src + m);
+            const float wm = __ldg(slot_w + m);
+            float x[8];
+            tc::load8_guarded_cg(h + (size_t)s * D, kc * 8, D, x);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) acc[j] = fmaf(wm, x[j], acc[j]);
+        }
+    }
+    ts::img_store_chunk(img, NKS, row >> 7, row & 127, kc * 8, acc);
 }
 
 // ------------------------------------------------------------------------------------------------ backward helper

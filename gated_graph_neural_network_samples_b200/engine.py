@@ -153,11 +153,11 @@ class PreparedGraph:
     @classmethod
     def host_only_gcn(cls, hidden_size: int, num_layers: int, num_nodes: int, adjacency_list, adjacency_weights, use_bias: bool = False,
                       precision: str = "fp32", num_sms: int = 132, save_for_backward: bool = False,
-                      reuse: Optional["PreparedGraph"] = None) -> "PreparedGraph":
+                      reuse: Optional["PreparedGraph"] = None, wide_hidden: bool = False) -> "PreparedGraph":
         """``ggnn_host_prepare_graph_gcn``: a GCN batch (``[nnz, 2]`` int64 (row i = output, column j = input) list and ``[nnz]`` weights)
-        through the same builder, no engine, no GPU."""
+        through the same builder, no engine, no GPU.  ``wide_hidden``: as for ``GCNEngine``."""
         g = reuse if reuse is not None else cls()
-        cfg = _lib.GcnConfig(int(hidden_size), int(num_layers), int(bool(use_bias)), PRECISIONS[precision], 0)
+        cfg = _lib.GcnConfig(int(hidden_size), int(num_layers), int(bool(use_bias)), PRECISIONS[precision], 0, int(bool(wide_hidden)))
         lst, w = _gcn_arrays(adjacency_list, adjacency_weights)
         return g._fill(g.lib.ggnn_host_prepare_graph_gcn, int(num_nodes), 1, C.byref(cfg), int(num_sms), int(bool(save_for_backward)),
                        int(num_nodes), lst.shape[0], lst.ctypes.data, w.ctypes.data)
@@ -342,10 +342,10 @@ class DeviceDataset:
 
     @classmethod
     def host_only_gcn(cls, hidden_size: int, num_layers: int, flat, use_bias: bool = False, precision: str = "fp32", num_sms: int = 132,
-                      for_training: bool = True) -> "DeviceDataset":
-        """``ggnn_host_dataset_create_gcn``: the GCN dataset's host summaries, no engine, no GPU."""
+                      for_training: bool = True, wide_hidden: bool = False) -> "DeviceDataset":
+        """``ggnn_host_dataset_create_gcn``: the GCN dataset's host summaries, no engine, no GPU.  ``wide_hidden``: as for ``GCNEngine``."""
         d = cls()
-        cfg = _lib.GcnConfig(int(hidden_size), int(num_layers), int(bool(use_bias)), PRECISIONS[precision], 0)
+        cfg = _lib.GcnConfig(int(hidden_size), int(num_layers), int(bool(use_bias)), PRECISIONS[precision], 0, int(bool(wide_hidden)))
         lst, w = _gcn_arrays(flat.lists, flat.weights)
         off = np.ascontiguousarray(flat.entry_off, np.int64)
         head = ((C.byref(cfg), int(num_sms), int(bool(for_training))), ())
@@ -894,15 +894,20 @@ class PropagationEngine:
 class GCNEngine(PropagationEngine):
     """The sparse GCN model (chem_tensorflow_gcn.py:42-82) on the same C ABI: ``ggnn_gcn_create`` / ``ggnn_gcn_set_weights`` /
     ``ggnn_set_graph_gcn`` / ``ggnn_gcn_backward``; forward, readout, dropout, save-for-backward, prepared graphs and introspection are
-    the inherited calls.  The GGNN-only calls raise ``GgnnError`` (the library refuses them on a GCN engine)."""
+    the inherited calls.  The GGNN-only calls raise ``GgnnError`` (the library refuses them on a GCN engine).
 
-    def __init__(self, hidden_size: int, num_layers: int, use_bias: bool = False, device: int = 0, precision: str = "fp32"):
+    ``wide_hidden`` (``ggnn_gcn_config.wide_hidden``): hidden sizes up to 512, and above 128 on bf16x3 / bf16 the streaming wgmma plan
+    (a weighted gather and one GEMM launch per layer) instead of the fp32 kernel.  Batches and datasets must be prepared with the same value."""
+
+    def __init__(self, hidden_size: int, num_layers: int, use_bias: bool = False, device: int = 0, precision: str = "fp32",
+                 wide_hidden: bool = False):
         self._h = C.c_void_p()
         self.lib = _lib.load()
         self.params = {"hidden_size": int(hidden_size), "num_timesteps": int(num_layers), "gcn_use_bias": bool(use_bias)}
         self.D, self.T, self.L = int(hidden_size), 1, int(num_layers)
         self.use_bias = bool(use_bias)
-        cfg = _lib.GcnConfig(self.D, self.L, int(self.use_bias), PRECISIONS[precision], int(device))
+        self.wide_hidden = bool(wide_hidden)
+        cfg = _lib.GcnConfig(self.D, self.L, int(self.use_bias), PRECISIONS[precision], int(device), int(self.wide_hidden))
         rc = self.lib.ggnn_gcn_create(C.byref(cfg), C.byref(self._h))
         if rc != 0:
             self._h = C.c_void_p()

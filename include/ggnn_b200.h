@@ -356,14 +356,22 @@ int ggnn_host_tile_plan(int32_t hidden_size, int32_t num_edge_types, int32_t pre
  * src = the input column j, msg = position in the input list) work on it as on a GGNN engine.  The GGNN-only calls
  * (ggnn_set_weights, ggnn_set_graph_sparse/dense, ggnn_prepare_graph_sparse/dense, ggnn_run_*, ggnn_backward) return GGNN_ESTATE on a
  * GCN engine, and the GCN calls below return GGNN_ESTATE on a GGNN engine.
- * Limits: hidden_size a positive multiple of 4 and <= 256, 1 <= num_layers <= 16.  precision GGNN_PREC_BF16X3 / GGNN_PREC_BF16 run the
- * wgmma kernel for hidden_size <= 128; GGNN_PREC_FP32, and hidden sizes above 128, run the fp32 CUDA-core kernel. */
+ * Limits: hidden_size a positive multiple of 4 and <= 256 (<= 512 with wide_hidden), 1 <= num_layers <= 16.  precision
+ * GGNN_PREC_BF16X3 / GGNN_PREC_BF16 run the fused wgmma kernel for hidden_size <= 128; GGNN_PREC_FP32 runs the fp32 CUDA-core kernel at
+ * every hidden size.  Above 128 on GGNN_PREC_BF16X3 / GGNN_PREC_BF16:
+ *   wide_hidden = 0  hidden sizes up to 256 run the fp32 CUDA-core kernel (the plan says gcn-fp32-ffma), larger ones are refused;
+ *   wide_hidden = 1  every layer is two launches on fixed 128-row tiles (the plan says gcn-stream-...): a weighted gather writes S = A . H
+ *                    as a bf16 hi/lo operand image, and the streaming wgmma kernel of the GGNN model's wide hidden sizes multiplies it by
+ *                    W_l, adds the bias and applies relu and state dropout (the same masks as the fp32 kernel's).
+ * At hidden_size <= 128 the flag changes nothing: the same plans and the same image bytes.  The two paths from 129 to 256 exist only because
+ * the default, 0, is kept as it was; a batch or dataset prepared with one value of the flag is refused by an engine created with the other. */
 typedef struct ggnn_gcn_config {
     int32_t hidden_size; /* params['hidden_size'] (D)                   */
     int32_t num_layers;  /* params['num_timesteps']                     */
     int32_t use_bias;    /* params['gcn_use_bias']                      */
     int32_t precision;   /* GGNN_PREC_*                                 */
     int32_t device;      /* CUDA device ordinal                         */
+    int32_t wide_hidden; /* 0: as above; 1: hidden sizes up to 512, on the streaming wgmma plan above 128 on bf16x3 / bf16 */
 } ggnn_gcn_config;
 /* DEVICE pointers, fp32: kernel [D, D] row-major (gcn_weights_l), bias [D] (gcn_bias_l) or NULL when !use_bias. */
 typedef struct ggnn_gcn_layer_weights { const float* kernel; const float* bias; } ggnn_gcn_layer_weights;
