@@ -24,17 +24,24 @@ def _propagation_function():
     import torch
 
     class Propagation(torch.autograd.Function):
-        """Autograd node around the C ABI: forward = ggnn_forward, backward = ggnn_backward."""
+        """Autograd node around the C ABI: forward = ggnn_forward, backward = ggnn_backward.  ``flat`` holds the tensors ``layout`` indexes
+        and, when it holds one more, the message weights [num_messages()] of a message-weighted batch (set before the forward, their gradient
+        from ggnn_backward_weighted)."""
 
         @staticmethod
         def forward(ctx, engine, layout, h0, *flat):
             layers = [{k: flat[i] for k, i in lay.items()} for lay in layout]
+            n_layer = sum(len(lay) for lay in layout)
+            mw = flat[n_layer] if len(flat) > n_layer else None
             # ctx.needs_input_grad is all False under torch.no_grad() (validation epochs): no activations are saved there
             need = any(ctx.needs_input_grad[2:])
             engine.set_weights([{k: v.detach().contiguous() for k, v in lw.items()} for lw in layers])
+            if mw is not None:
+                engine.set_message_weights(mw.detach().contiguous())
             engine.set_deterministic(torch.are_deterministic_algorithms_enabled())
             engine.set_save_for_backward(need)
             out = engine.forward(h0.detach().contiguous())
+            ctx.mw_index = n_layer if mw is not None and ctx.needs_input_grad[3 + n_layer] else None
             ctx.serial = engine.serial   # the backward refuses once another forward, graph or weights replaced this one's
             ctx.engine, ctx.layout, ctx.shapes = engine, layout, [t.shape for t in flat]
             ctx.h0_needs = bool(ctx.needs_input_grad[2])
@@ -48,10 +55,31 @@ def _propagation_function():
             grads = [{k: grads_flat[i] for k, i in lay.items()} for lay in ctx.layout]
             d_h0 = torch.zeros_like(d_out) if ctx.h0_needs else None
             ctx.engine.set_deterministic(torch.are_deterministic_algorithms_enabled())
-            ctx.engine.backward(d_out.contiguous(), grads, d_h0)
+            if ctx.mw_index is None:
+                ctx.engine.backward(d_out.contiguous(), grads, d_h0)
+            else:
+                ctx.engine.backward(d_out.contiguous(), grads, d_h0, d_message_weights=grads_flat[ctx.mw_index])
             return (None, None, d_h0) + tuple(grads_flat)
 
     return Propagation
+
+
+def propagate(engine: PropagationEngine, h0, layers: Sequence[dict], message_weights=None):
+    """The sparse GGNN propagation as a differentiable torch function, without a ChemModel: ``engine`` holds the current batch (for
+    ``message_weights``, a message-weighted one: ``prepare_graph_sparse_weighted`` + ``set_graph_prepared``), ``h0`` [V, D] and
+    ``layers[l]`` dicts of fp32 CUDA tensors keyed like ``ggnn_layer_weights`` (``engine.WEIGHT_FIELDS``) and ``message_weights`` an fp32
+    CUDA tensor [num_messages()] in the reference's type-major message order.  Returns the final node states [V, D]; gradients reach
+    ``h0``, every layer tensor and ``message_weights``.  The in-degree table of the batch scales the edge bias and the mean unweighted."""
+    layout, flat = [], []
+    for lw in layers:
+        lay = {}
+        for k, v in lw.items():
+            lay[k] = len(flat)
+            flat.append(v)
+        layout.append(lay)
+    if message_weights is not None:
+        flat.append(message_weights)
+    return _propagation_function().apply(engine, layout, h0, *flat)
 
 
 class SparseGGNNChemModel(ChemModel):

@@ -33,6 +33,7 @@
 #include "ggnn_fwd_step.cuh"
 #include "ggnn_gcn.cuh"
 #include "ggnn_dataset.cuh"
+#include "ggnn_msgw.cuh"
 #include "ggnn_tc_smem.h"
 
 using namespace ggnn;
@@ -176,7 +177,10 @@ struct BatchPlan {
     size_t off_pair = 0, off_vptr = 0, off_vsrc = 0, off_tvp = 0, off_vinfo = 0;   // streaming plan: (target,type) -> source table, virtual rows (pairs with several messages)
     size_t off_vslot = 0;   // weighted streaming plan: the first target-CSR slot of every virtual row (its weights are slot_w[vslot[vid] + m])
     bool all_virtual = false;   // attention on the streaming plan: every (target, type) pair with messages is a virtual row, weighted by the
-                                // step's attention probabilities through vslot (the image has vslot and no slot weights)
+                                // step's attention probabilities through vslot (the image has vslot and no slot weights); a message-weighted
+                                // batch likewise, weighted by its slot weights, so that the plan does not depend on their values
+    bool msg_weighted = false;  // ggnn_prepare_graph_sparse_weighted: weighted, its slot weights zero in the image until ggnn_set_message_weights
+                                // writes them on the device; the image carries the source-keyed CSR's slot map (tslot) with save_for_backward
     size_t off_slotw = 0, off_tslotw = 0;   // weighted: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
     // (offset, bytes) of the image's bytes no section builder writes: alignment gaps and the one-element room of empty sections.  The host
     // builder zeroes them (the device dataset zeroes its whole image), so that an image is one function of its batch, whatever the
@@ -212,6 +216,7 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     ggnn_layer_weights w[MAX_LAYERS];
     ggnn_gcn_layer_weights gcn_w[MAX_LAYERS] = {};
     bool graph_set = false;
+    bool msg_weights_set = false;   // a message-weighted batch: ggnn_set_message_weights ran since its upload
 
     // device memory
     DevBuf graph_buf;   // the graph image of the current batch
@@ -361,7 +366,7 @@ static int launch_steps(ggnn_engine* e, Params& p, cudaStream_t st, Launch launc
 // Everything the engine knows about the previous batch beyond its buffers: the graph, the last forward and its saved activations, and the
 // readout's node -> graph map.  Called first by every graph upload, so a failed upload leaves no batch behind either.
 static void forget_batch(ggnn_engine* e) {
-    e->graph_set = false; e->saved_valid = false;
+    e->graph_set = false; e->saved_valid = false; e->msg_weights_set = false;
     e->last_h0 = nullptr; e->last_out = nullptr; e->fwd_valid = false; e->layers_written = false;
     e->ro_V = -1;
 }
@@ -510,10 +515,11 @@ bool gcn_streams(const ModelShape& s) { return s.wide_hidden && s.precision != G
 // batch may take the streaming plan above hidden 128 on the tensor-core precisions (the ..._dense_weighted entries), else it is refused
 // there.  Starts `p` afresh; the image builders fill in the rest.
 int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>& cuts, BatchPlan& p, std::vector<int>& tile_start,
-               std::string& err, bool stream_weighted = false) {
+               std::string& err, bool stream_weighted = false, bool msg_weighted = false) {
     p = BatchPlan();
     p.V = V;
     p.weighted = weighted;
+    p.msg_weighted = msg_weighted;
     int max_span = 0;
     for (size_t i = 1; i < cuts.size(); ++i) max_span = std::max(max_span, cuts[i] - cuts[i - 1]);
     p.max_span = max_span;
@@ -567,7 +573,7 @@ int build_plan(const ModelShape& s, int V, bool weighted, const std::vector<int>
                 return GGNN_EUNSUPPORTED;
             }
             p.stream = true; p.variant = 3;
-            p.all_virtual = s.use_att != 0;   // (attention runs on the streaming plan at every hidden size)
+            p.all_virtual = s.use_att != 0 || msg_weighted;   // (attention runs on the streaming plan at every hidden size)
             fixed_tiles(V, ts::TILE_M, tile_start);
             p.ntiles = (int)tile_start.size() - 1;
             for (int i = 0; i < 2; ++i) {
@@ -766,8 +772,9 @@ static float** grad_field(ggnn_layer_grads& g, int i) {
     return f[i];
 }
 
+// d_dw (DEVICE [M] or null): the message weights' gradient, accumulated into (message-weighted batches only).
 static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers,
-                              float* d_h0, ggnn_stream_t stream) {
+                              float* d_h0, float* d_dw, ggnn_stream_t stream) {
     using namespace ggnn::bwd;
     if (int rc = begin_backward(e, "ggnn_backward", "ggnn_set_graph_sparse", d_h_out, grads, num_layers, d_h0)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
@@ -782,7 +789,9 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
     auto take = [&](size_t floats) { size_t o = off; off = align_up(off + floats * sizeof(float), 256); return o; };
     const size_t o_dstate = take(vd * (L + 1)), o_dha = take(vd), o_dhb = take(vd), o_dpc = take(vd), o_dpg = take(2 * vd);
     const size_t o_dxc = take((size_t)V * ldx_max), o_dxg = take((size_t)V * ldx_max), o_rh = take(vd), o_dxp = take(vd), o_at = take(vd * T), o_gt = take(vd * T);
-    const size_t o_pall = take(e->use_att ? vd * T : 0), o_dsa = take(e->use_att ? (size_t)std::max<int64_t>(e->M, 1) : 0);
+    // P = dx' . W^T: attention's softmax backward and the message weights' gradient (dw_slot: its per-slot sums over the steps)
+    const size_t o_pall = take(e->use_att || d_dw ? vd * T : 0), o_dsa = take(e->use_att ? (size_t)std::max<int64_t>(e->M, 1) : 0);
+    const size_t o_dws = take(d_dw ? (size_t)std::max<int64_t>(e->M, 1) : 0);
     // deterministic mode: room for the partials of every weight-gradient launch below (the need is not monotone in the segment count --
     // fewer segments get more splits -- so every launched shape is sized), and the attention's per-block d a_t
     const int nodes_blocks = (V + 7) / 8;
@@ -820,6 +829,8 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
     float *At = (float*)(bb + o_at), *Gt = (float*)(bb + o_gt), *Pall = (float*)(bb + o_pall), *dsa = (float*)(bb + o_dsa);
     float** d_ptrs = (float**)(bb + o_ptrs);
     float* ws = (float*)(bb + o_ws);
+    float* dw_slot = (float*)(bb + o_dws);
+    if (d_dw && e->M > 0) CU_TRY(e, cudaMemsetAsync(dw_slot, 0, sizeof(float) * (size_t)e->M, st));
     CU_TRY(e, cudaMemsetAsync(dstate, 0, vd * L * sizeof(float), st));
     CU_TRY(e, cudaMemcpyAsync(dstate + vd * L, d_h_out, vd * sizeof(float), cudaMemcpyDeviceToDevice, st));
     // forward values of node_states_per_layer
@@ -935,6 +946,11 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
             } else if (e->weighted) {
                 j0.w = gd.slotw;
                 j1.w = gd.tslotw;
+                if (d_dw) {   // d w_m += <P[v, t], h[src_m]>: the message's own term of the gathered sum
+                    gemm_nt(false, dxp, D, 0, w.edge_weights, D, 0, 1, Pall, TD, V, TD, D);   // P[v, t*D+k] = <dx'[v], W_t[k, :]>
+                    msgw::message_weight_grad_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.src, Pall, h, dw_slot, V, D, T);
+                    ++e->last_launches;
+                }
             }
             csr_gather_all_kernel<<<dim3(nodes_blocks, 2), 256, 0, st>>>(j0, j1, V, D, T);
             ++e->last_launches;
@@ -970,6 +986,10 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
         else { add_inplace_kernel<<<eb, 256, 0, st>>>(dstate + (size_t)l * vd, dstate + (size_t)(l + 1) * vd, n); ++e->last_launches; }
     }
     if (ws_rc != GGNN_OK) return ws_rc;
+    if (d_dw && e->M > 0) {
+        msgw::add_slot_grads_kernel<<<(int)std::min<int64_t>((e->M + 255) / 256, 4096), 256, 0, st>>>(gd.msg, dw_slot, d_dw, e->M);
+        ++e->last_launches;
+    }
     if (d_h0) CU_TRY(e, cudaMemcpyAsync(d_h0, dstate, vd * sizeof(float), cudaMemcpyDeviceToDevice, st));
     CU_TRY(e, cudaGetLastError());
     return GGNN_OK;
@@ -1310,7 +1330,7 @@ static size_t layout_image(const ModelShape& shape, BatchPlan& p, bool save, int
     if (p.has_transpose) {
         p.off_trow = place(I * (VT + 1), I * (VT + 1));
         p.off_ttgt = place(I * Mu, I * Mr);
-        p.off_tslot = shape.use_att ? place(I * Mu, I * Mr) : off;
+        p.off_tslot = shape.use_att || p.msg_weighted ? place(I * Mu, I * Mr) : off;
     }
     // streaming plan: per (target, type) pair the ONE node to copy from (or none / a virtual row), see ggnn_fwd_stream.cuh
     if (p.stream) {
@@ -1331,7 +1351,7 @@ static size_t layout_image(const ModelShape& shape, BatchPlan& p, bool save, int
 }
 
 // The typed view of an image laid out by plan `p` (layout_image) at `base`.  The one statement of which sections a plan carries: the
-// source-keyed CSR with save_for_backward (its slot map with attention, its weights on a weighted batch), the streaming tables on the
+// source-keyed CSR with save_for_backward (its slot map with attention and on a message-weighted batch, its weights on a weighted batch), the streaming tables on the
 // streaming plan (the virtual rows' first slots on a weighted one and with attention), the slot weights on a weighted batch.  Every other section is null.
 static ImageView image_view(const BatchPlan& p, bool use_att, char* base) {
     auto sec = [&](size_t off, bool present) { return present ? (void*)(base + off) : nullptr; };
@@ -1340,7 +1360,7 @@ static ImageView image_view(const BatchPlan& p, bool use_att, char* base) {
     v.indeg = (float*)sec(p.off_indeg, true); v.denom = (float*)sec(p.off_denom, true);
     v.tile_start = (int*)sec(p.off_tiles, true); v.tile_mask = (unsigned*)sec(p.off_mask, true);
     v.trow = (int*)sec(p.off_trow, p.has_transpose); v.ttgt = (int*)sec(p.off_ttgt, p.has_transpose);
-    v.tslot = (int*)sec(p.off_tslot, p.has_transpose && use_att);
+    v.tslot = (int*)sec(p.off_tslot, p.has_transpose && (use_att || p.msg_weighted));
     v.pair = (int*)sec(p.off_pair, p.stream); v.vptr = (int*)sec(p.off_vptr, p.stream); v.vsrc = (int*)sec(p.off_vsrc, p.stream);
     v.tvp = (int*)sec(p.off_tvp, p.stream); v.vinfo = (int*)sec(p.off_vinfo, p.stream); v.vslot = (int*)sec(p.off_vslot, p.stream && (p.weighted || p.all_virtual));
     v.slotw = (float*)sec(p.off_slotw, p.weighted); v.tslotw = (float*)sec(p.off_tslotw, p.weighted && p.has_transpose);
@@ -1443,7 +1463,7 @@ static void fill_denominators(int v0, int v1, int T, const float* indeg, float* 
 
 // The source-keyed CSR of the backward pass (rows source*T+type -> targets, in message order), which turns its scatter into a gather:
 // trow [V*T + 1], ttgt [M]; `tslot` (when non-null) the target-CSR slot of every entry, from csr_msg (the message of every target-CSR slot);
-// `tslotw` (when non-null) its weight, from the per-message weights w.
+// `tslotw` (when non-null) its weight, from the per-message weights w (zero without them).
 static void fill_source_csr(int V, int T, const int32_t* const* adj, const int32_t* num_edges, int64_t M, const int* csr_msg, const float* w,
                             int* trow, int* ttgt, int* tslot, float* tslotw) {
     std::vector<int> cnt((size_t)V * T + 1, 0);
@@ -1463,7 +1483,7 @@ static void fill_source_csr(int V, int T, const int32_t* const* adj, const int32
             const int j = cnt[(size_t)adj[t][2 * i] * T + t]++;
             ttgt[j] = adj[t][2 * i + 1];
             if (tslot) tslot[j] = slot_of_msg[m];
-            if (tslotw) tslotw[j] = w[m];
+            if (tslotw) tslotw[j] = w ? w[m] : 0.0f;
         }
 }
 
@@ -1507,9 +1527,11 @@ static int64_t gcn_pairs(int64_t V, int64_t nnz, const int64_t* list, int32_t* p
 // ---- the host half of ggnn_set_graph_sparse: validation, tile plan, stable target-sorted CSR, streaming tables -> g->image.
 // `weighted`: the batch has one weight per message, `w`, in the type-major message order (required when there are messages); the image
 // then carries them in target-CSR order and, with the source-keyed CSR, in source-CSR order.  `stream_weighted`: see build_plan.
+// `msg_weighted` (with weighted and stream_weighted, and w null): the weights come later, on the device -- the weight sections are zero and
+// the plan is the one every weight vector shares.
 // Nothing here touches the device except the pinned allocation of the image and the wait for the previous upload out of it.
 static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* const* adj, const int32_t* num_edges, const float* indeg,
-                              bool weighted, const float* w, bool stream_weighted = false) {
+                              bool weighted, const float* w, bool stream_weighted = false, bool msg_weighted = false) {
     const ModelShape& shape = g->shape;
     BatchPlan& p = g->plan;
     g->valid = false;
@@ -1530,7 +1552,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
         M += num_edges[t];
     }
     if (M > 0x7fffffff || (int64_t)V * T + 1 > 0x7fffffff) return g->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
-    if (weighted && M > 0 && !w) return g->fail(GGNN_EINVAL, "null message weights");
+    if (weighted && !msg_weighted && M > 0 && !w) return g->fail(GGNN_EINVAL, "null message weights");
 
     // ---- host threads.  Every pass below is split over `nth` threads by TARGET ranges (pass 1: equal node ranges; later passes: equal
     // tile ranges): each thread scans the whole edge list (sequential reads) and performs only the scattered writes of its own rows, in the
@@ -1567,7 +1589,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     find_cuts(need_cuts ? reach.data() : nullptr, V, cuts);
     lap("validate+count", t_lap);
     std::vector<int> tile_start;
-    int rc = build_plan(shape, V, weighted, cuts, p, tile_start, g->err, stream_weighted);
+    int rc = build_plan(shape, V, weighted, cuts, p, tile_start, g->err, stream_weighted, msg_weighted);
     if (rc) return rc;
     p.M = M;
     const int ntiles = p.ntiles;
@@ -1577,9 +1599,9 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
     std::vector<int> tb(nth + 1);
     for (int k = 0; k <= nth; ++k) tb[k] = (int)((int64_t)ntiles * k / nth);
     // weighted streaming plan: the rows whose one message weighs other than 1.0f, which stream_rows makes virtual rows too (each such row
-    // has one message, so no two writes meet)
+    // has one message, so no two writes meet).  Not on an all-virtual plan, whose rows with messages are all virtual whatever the weights
     std::vector<uint8_t> scaled_single;
-    if (p.stream && weighted) {
+    if (p.stream && weighted && !p.all_virtual) {
         scaled_single.assign((size_t)V * T, 0);
         for (int t = 0; t < T; ++t)
             for (int i = 0; i < num_edges[t]; ++i) {
@@ -1685,7 +1707,7 @@ static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* 
             }
         }
         if (img.slotw)   // the weights of this range's slots, in target-CSR order
-            for (int64_t m = part_msgs[k]; m < part_msgs[k + 1]; ++m) img.slotw[m] = w[csr_msg[m]];
+            for (int64_t m = part_msgs[k]; m < part_msgs[k + 1]; ++m) img.slotw[m] = w ? w[csr_msg[m]] : 0.0f;
         if (img.pair) {   // the range's rows: no message -> -1, one -> its source, several -> virtual row; then the last tile's rows beyond V
             int vid = (int)part_nv[k], vm = (int)part_nvm[k];
             for (int i = tb[k]; i < tb[k + 1]; ++i) {
@@ -1848,6 +1870,32 @@ int ggnn_prepare_graph_sparse(const ggnn_engine* e, int32_t save_for_backward, i
                               const float* indeg, ggnn_prepared_graph** inout) {
     if (int rc = begin_prepare<ggnn_config>(inout, e, nullptr, 0, save_for_backward, __func__)) return rc;
     return build_sparse_image(*inout, V, adj, num_edges, indeg, false, nullptr);
+}
+
+}  // extern "C"
+
+// The host half of the two message-weighted prepare calls: the sparse builder with zero weight sections and the value-independent plan.
+static int build_message_weighted_image(ggnn_prepared_graph* g, int32_t V, const int32_t* const* adj, const int32_t* num_edges, const float* indeg) {
+    g->valid = false;
+    if (g->shape.use_att)
+        return g->fail(GGNN_EUNSUPPORTED, "message weights with propagation attention are not supported (the probabilities are the slot weights)");
+    if (int rc = build_sparse_image(g, V, adj, num_edges, indeg, true, nullptr, true, true)) return rc;
+    g->plan.plan_text += " [message-weighted]";
+    return GGNN_OK;
+}
+
+extern "C" {
+
+int ggnn_prepare_graph_sparse_weighted(const ggnn_engine* e, int32_t save_for_backward, int32_t V, const int32_t* const* adj,
+                                       const int32_t* num_edges, const float* indeg, ggnn_prepared_graph** inout) {
+    if (int rc = begin_prepare<ggnn_config>(inout, e, nullptr, 0, save_for_backward, __func__)) return rc;
+    return build_message_weighted_image(*inout, V, adj, num_edges, indeg);
+}
+
+int ggnn_host_prepare_graph_sparse_weighted(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t V,
+                                            const int32_t* const* adj, const int32_t* num_edges, const float* indeg, ggnn_prepared_graph** inout) {
+    if (int rc = begin_prepare(inout, nullptr, cfg, num_sms, save_for_backward, __func__)) return rc;
+    return build_message_weighted_image(*inout, V, adj, num_edges, indeg);
 }
 
 }  // extern "C"
@@ -2719,6 +2767,8 @@ int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t st
     const bool gcn = e->model == MODEL_GCN;
     if (!e->weights_set) return e->fail(GGNN_ESTATE, "%s has not been called", gcn ? "ggnn_gcn_set_weights" : "ggnn_set_weights");
     if (!e->graph_set) return no_graph(e);
+    if (e->msg_weighted && !e->msg_weights_set)
+        return e->fail(GGNN_ESTATE, "the batch is message-weighted: ggnn_set_message_weights must follow its upload before a forward");
     if ((!h0 || !h_out) && e->V > 0) return e->fail(GGNN_EINVAL, "null state pointer");
     if (((uintptr_t)h0 & 15) || ((uintptr_t)h_out & 15)) return e->fail(GGNN_EINVAL, "state pointers must be 16-byte aligned");
     // In place is refused: the GLOBAL launches gather h0 rows that other CTAs of the same launch overwrite, and the backward reads h0 as
@@ -3134,7 +3184,35 @@ int ggnn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* 
                   float* d_h0, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
     GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
-    return ggnn_backward_impl(e, d_h_out, grads, num_layers, d_h0, stream);
+    return ggnn_backward_impl(e, d_h_out, grads, num_layers, d_h0, nullptr, stream);
+}
+
+int ggnn_backward_weighted(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers, float* d_h0,
+                           float* d_message_weights, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
+    if (d_message_weights && !e->msg_weighted)
+        return e->fail(GGNN_ESTATE, "d_message_weights needs a message-weighted batch (ggnn_prepare_graph_sparse_weighted)");
+    return ggnn_backward_impl(e, d_h_out, grads, num_layers, d_h0, d_message_weights, stream);
+}
+
+int ggnn_set_message_weights(ggnn_engine* e, const float* message_weights, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
+    if (!e->graph_set) return no_graph(e);
+    if (!e->msg_weighted) return e->fail(GGNN_ESTATE, "the current batch is not message-weighted (ggnn_prepare_graph_sparse_weighted)");
+    if (!message_weights && e->M > 0) return e->fail(GGNN_EINVAL, "null message weights");
+    CU_TRY(e, cudaSetDevice(e->device));
+    e->msg_weights_set = false;
+    e->saved_valid = false;   // the backward's gathers read the slot weights: they must be the saved forward's
+    if (e->M > 0) {
+        const ImageView& gd = e->gd;
+        msgw::scatter_message_weights_kernel<<<(int)std::min<int64_t>((e->M + 255) / 256, 4096), 256, 0, (cudaStream_t)stream>>>(
+            message_weights, gd.msg, gd.tslot, gd.slotw, gd.tslotw, e->M);
+        CU_TRY(e, cudaGetLastError());
+    }
+    e->msg_weights_set = true;
+    return GGNN_OK;
 }
 
 int ggnn_num_messages(const ggnn_engine* e, int64_t* out) {

@@ -151,6 +151,22 @@ class PreparedGraph:
                        int(bool(save_for_backward)), a.shape[0], a.shape[2], a.ctypes.data)
 
     @classmethod
+    def host_only_weighted(cls, params: dict, num_edge_types: int, adjacency_lists, num_incoming_edges_per_type, precision: str = "fp32",
+                           num_sms: int = 132, save_for_backward: bool = False, reuse: Optional["PreparedGraph"] = None,
+                           cudnn_gru_tensor_cores: bool = False) -> "PreparedGraph":
+        """``ggnn_host_prepare_graph_sparse_weighted``: a message-weighted sparse batch (see
+        ``PropagationEngine.prepare_graph_sparse_weighted``), no engine, no GPU."""
+        g = reuse if reuse is not None else cls()
+        cfg, keep = make_config(params, num_edge_types, 0, precision, False, cudnn_gru_tensor_cores)
+        T = int(num_edge_types)
+        adjs = [np.ascontiguousarray(np.asarray(a, dtype=np.int32).reshape(-1, 2)) for a in adjacency_lists]
+        indeg = np.ascontiguousarray(np.asarray(num_incoming_edges_per_type, dtype=np.float32))
+        ptrs = (C.c_void_p * T)(*[a.ctypes.data for a in adjs])
+        counts = (C.c_int32 * T)(*[a.shape[0] for a in adjs])
+        return g._fill(g.lib.ggnn_host_prepare_graph_sparse_weighted, indeg.shape[0], T, C.byref(cfg), int(num_sms), int(bool(save_for_backward)),
+                       indeg.shape[0], ptrs, counts, indeg.ctypes.data)
+
+    @classmethod
     def host_only_gcn(cls, hidden_size: int, num_layers: int, num_nodes: int, adjacency_list, adjacency_weights, use_bias: bool = False,
                       precision: str = "fp32", num_sms: int = 132, save_for_backward: bool = False,
                       reuse: Optional["PreparedGraph"] = None, wide_hidden: bool = False) -> "PreparedGraph":
@@ -527,6 +543,31 @@ class PropagationEngine:
         return g._fill(self.lib.ggnn_prepare_graph_sparse, indeg.shape[0], self.T, self._h,
                        -1 if save_for_backward is None else int(bool(save_for_backward)), indeg.shape[0], ptrs, counts, indeg.ctypes.data)
 
+    def prepare_graph_sparse_weighted(self, adjacency_lists=None, num_incoming_edges_per_type=None, save_for_backward: Optional[bool] = None,
+                                      reuse: Optional["PreparedGraph"] = None, marshalled=None) -> "PreparedGraph":
+        """``prepare_graph_sparse`` for a MESSAGE-WEIGHTED batch (``ggnn_prepare_graph_sparse_weighted``): after ``set_graph_prepared``,
+        ``set_message_weights`` puts one weight per message on the device, and every forward scales message m's state term by w_m:
+        incoming[v] = (sum_t (sum_m w_m h[s_m]) W_t + sum_t indeg[v,t] b_t) / denom[v].  The in-degree table is used as fed, for the edge bias
+        and the mean, and gets no gradient: to weight the bias too (A.(hW + b)), feed the weighted row sums as the table -- the weights'
+        gradient then lacks the bias path.  Refused with propagation attention."""
+        adjs, indeg, ptrs, counts = marshalled if marshalled is not None else self._sparse_args(adjacency_lists, num_incoming_edges_per_type)
+        g = reuse if reuse is not None else PreparedGraph(self.lib)
+        return g._fill(self.lib.ggnn_prepare_graph_sparse_weighted, indeg.shape[0], self.T, self._h,
+                       -1 if save_for_backward is None else int(bool(save_for_backward)), indeg.shape[0], ptrs, counts, indeg.ctypes.data)
+
+    def set_message_weights(self, w):
+        """``ggnn_set_message_weights``: ``w`` a contiguous fp32 CUDA tensor of ``num_messages()`` entries, message m of type t at position
+        ``sum_{t' < t} E_t' + i`` (the reference's type-major order, ``oracle.ggnn_oracle.message_arrays``), for the current
+        message-weighted batch.  The engine copies them on its stream; ``w`` may be reused once the stream passed the call."""
+        import torch
+        if not (isinstance(w, torch.Tensor) and w.is_cuda and w.dtype == torch.float32 and w.is_contiguous()):
+            raise GgnnError("message weights must be a contiguous fp32 CUDA tensor")
+        M = self.num_messages()
+        if w.numel() != M:
+            raise GgnnError("message weights have %d entries, the batch has %d messages" % (w.numel(), M))
+        self.serial += 1
+        self._check(self.lib.ggnn_set_message_weights(self._h, w.data_ptr() if M else None, self._stream()))
+
     def prepare_graph_dense(self, adjacency_matrix, save_for_backward: Optional[bool] = None,
                             reuse: Optional["PreparedGraph"] = None) -> "PreparedGraph":
         """The HOST half of ``set_graph_dense`` for a 0/1 adjacency ``[b, T, v, v]`` (scan to edge lists + the CSR builder); raises
@@ -774,14 +815,24 @@ class PropagationEngine:
             raise ValueError("unknown backward precision %r (expected one of %s)" % (precision, ", ".join(BACKWARD_PRECISIONS)))
         self._check(self.lib.ggnn_set_backward_precision(self._h, PRECISIONS[precision]))
 
-    def backward(self, d_out, grads: Sequence[dict], d_h0=None):
+    def backward(self, d_out, grads: Sequence[dict], d_h0=None, d_message_weights=None):
+        """``ggnn_backward``; with ``d_message_weights`` (fp32 CUDA [num_messages()], accumulated into; message-weighted batches only)
+        ``ggnn_backward_weighted``, which also forms the message weights' gradient."""
         arr = (_lib.GgnnLayerGrads * len(grads))()
         for l, g in enumerate(grads):
             for f in WEIGHT_FIELDS:
                 t = g.get(f)
                 setattr(arr[l], f, None if t is None else t.data_ptr())
-        self._check(self.lib.ggnn_backward(self._h, d_out.data_ptr(), arr, len(grads),
-                                           None if d_h0 is None else d_h0.data_ptr(), self._stream()))
+        if d_message_weights is None:
+            self._check(self.lib.ggnn_backward(self._h, d_out.data_ptr(), arr, len(grads),
+                                               None if d_h0 is None else d_h0.data_ptr(), self._stream()))
+            return
+        import torch
+        if not (d_message_weights.is_cuda and d_message_weights.dtype == torch.float32 and d_message_weights.is_contiguous()
+                and d_message_weights.numel() == self.num_messages()):
+            raise GgnnError("d_message_weights must be a contiguous fp32 CUDA tensor of num_messages() entries")
+        self._check(self.lib.ggnn_backward_weighted(self._h, d_out.data_ptr(), arr, len(grads), None if d_h0 is None else d_h0.data_ptr(),
+                                                    d_message_weights.data_ptr() if d_message_weights.numel() else None, self._stream()))
 
     # ------------------------------------------------------------------ readout (gated_regression, sparse:220-231 / dense:119-129)
     def readout_set_graphs(self, num_graphs: int, graph_nodes_list=None, nodes_per_graph: int = 0, node_mask=None):

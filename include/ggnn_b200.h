@@ -175,6 +175,36 @@ int ggnn_prepare_graph_dense_weighted(const ggnn_engine* e, int32_t save_for_bac
                                       const float* adjacency_matrix, ggnn_prepared_graph** inout);
 int ggnn_host_prepare_graph_dense_weighted(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t num_graphs,
                                            int32_t num_vertices, const float* adjacency_matrix, ggnn_prepared_graph** inout);
+/* ---- Message weights (sparse GGNN model): message m of type t, from source s to target v, weighs w_m, the messages numbered in the
+ * reference's type-major order (type t's list, in fed order, starts at sum_{t' < t} E_t'):
+ *     incoming[v] = ( sum_t (sum_{m into v, type t} w_m h[s_m]) W_t  +  sum_t indeg[v,t] b_t ) / denom[v]      (/ only with avg aggregation)
+ * The weight scales the state term only: the in-degree table is used as fed, for the edge bias and the mean, and is data (no gradient).
+ * Weights may be zero, negative or any finite value; weights of 1.0 give the unweighted model.  The gradient, per timestep of every layer
+ * with step input state h:  d w_m += <P[v, t], h[s_m]>,  P = dx' . W_t^T, dx' the gradient of the pre-mean message sum.
+ *   ggnn_prepare_graph_sparse_weighted   as ggnn_prepare_graph_sparse (same validation, CSR, tile plan, pinned image), the batch marked
+ *                                        message-weighted and its plan text ending in " [message-weighted]".  Its slot-weight sections
+ *                                        are zero until ggnn_set_message_weights writes them on the device; with save_for_backward the image
+ *                                        also carries the source-keyed CSR's slot map.  The plan depends on the structure alone: on the
+ *                                        streaming plan (hidden sizes above 128 on GGNN_PREC_BF16X3 / GGNN_PREC_BF16, and
+ *                                        GGNN_CELL_CUDNN_GRU_TENSOR_CORES) every (target, type) pair with messages is a virtual row.  Refused:
+ *                                        propagation attention (GGNN_EUNSUPPORTED: its probabilities are the slot weights), a GCN engine
+ *                                        (GGNN_ESTATE).  The host-only twin needs no engine or GPU.
+ *   ggnn_set_message_weights             message_weights DEVICE fp32 [M] (ggnn_num_messages), in the order above: one kernel on `stream`
+ *                                        scatters them into the current batch's slot weights; the buffer is free once the stream passed
+ *                                        the call.  GGNN_ESTATE when the current batch is not message-weighted.  Every graph upload forgets
+ *                                        the weights, and ggnn_forward on a message-weighted batch without them is GGNN_ESTATE.  Like
+ *                                        ggnn_set_weights it drops the saved activations of the last forward.
+ *   ggnn_backward_weighted               ggnn_backward, and with d_message_weights (DEVICE fp32 [M], accumulated into) the weights' gradient:
+ *                                        one P GEMM per timestep (wgmma under ggnn_set_backward_precision(GGNN_PREC_BF16X3)) and a per-slot
+ *                                        sum in a fixed order, without atomics -- bit-identical from call to call in both deterministic
+ *                                        modes.  ggnn_backward is this call with d_message_weights = NULL; a non-NULL one on a batch that is not
+ *                                        message-weighted is GGNN_ESTATE. */
+int ggnn_prepare_graph_sparse_weighted(const ggnn_engine* e, int32_t save_for_backward, int32_t num_nodes, const int32_t* const* adjacency_lists,
+                                       const int32_t* num_edges, const float* num_incoming_edges_per_type, ggnn_prepared_graph** inout);
+int ggnn_host_prepare_graph_sparse_weighted(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t num_nodes,
+                                            const int32_t* const* adjacency_lists, const int32_t* num_edges,
+                                            const float* num_incoming_edges_per_type, ggnn_prepared_graph** inout);
+int ggnn_set_message_weights(ggnn_engine* e, const float* message_weights, ggnn_stream_t stream);
 /* Introspection of a prepared graph: sizes and plan text; copies of its CSR (row_ptr [V*T+1], src [M], msg [M]), tile starts
  * [num_tiles+1], per-node mean-aggregation denominators [V] and, for a streaming plan, the (target, type) -> source table
  * [ceil(V/128)*128*T] (NULL pointers are skipped; pair_src of a non-streaming plan is left untouched and *is_streaming = 0). */
@@ -324,6 +354,9 @@ int ggnn_set_deterministic(ggnn_engine* e, int32_t enable);
 int ggnn_set_backward_precision(ggnn_engine* e, int32_t precision);
 int ggnn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers,
                   float* d_h0, ggnn_stream_t stream);
+/* ggnn_backward with the message weights' gradient (see ggnn_set_message_weights above). */
+int ggnn_backward_weighted(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers, float* d_h0,
+                           float* d_message_weights, ggnn_stream_t stream);
 
 /* The CSR build of ggnn_set_graph_sparse on its own -- host arithmetic only, no engine, no GPU: row_ptr [V*T+1], src [M], msg [M]
  * (msg = position of the slot's message in the reference's type-major message order, sparse:124-129).  Returns GGNN_ERANGE for an
@@ -354,7 +387,8 @@ int ggnn_host_tile_plan(int32_t hidden_size, int32_t num_edge_types, int32_t pre
  * ggnn_layer_state (intermediate layers: after a forward with save_for_backward on), ggnn_plan_description,
  * ggnn_last_launch_count, ggnn_prepared_graph_info and ggnn_prepared_graph_arrays (T = 1: row_ptr [V+1] keyed by the output row i,
  * src = the input column j, msg = position in the input list) work on it as on a GGNN engine.  The GGNN-only calls
- * (ggnn_set_weights, ggnn_set_graph_sparse/dense, ggnn_prepare_graph_sparse/dense, ggnn_run_*, ggnn_backward) return GGNN_ESTATE on a
+ * (ggnn_set_weights, ggnn_set_graph_sparse/dense, ggnn_prepare_graph_sparse/dense, ggnn_prepare_graph_sparse_weighted, ggnn_run_*,
+ * ggnn_set_message_weights, ggnn_backward, ggnn_backward_weighted) return GGNN_ESTATE on a
  * GCN engine, and the GCN calls below return GGNN_ESTATE on a GGNN engine.
  * Limits: hidden_size a positive multiple of 4 and <= 256 (<= 512 with wide_hidden), 1 <= num_layers <= 16.  precision
  * GGNN_PREC_BF16X3 / GGNN_PREC_BF16 run the fused wgmma kernel for hidden_size <= 128; GGNN_PREC_FP32 runs the fp32 CUDA-core kernel at
