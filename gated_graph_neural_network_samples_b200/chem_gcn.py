@@ -7,14 +7,14 @@ propagation replaced by the H100 engine.
 """
 from __future__ import annotations
 
-from typing import Any, Sequence
+from typing import Any, Optional, Sequence
 
 import numpy as np
 
 from . import packing
 from .chem_model import ChemModel
 from .chem_sparse import SparseGGNNChemModel
-from .engine import GCNEngine
+from .engine import GCNEngine, GgnnError
 from .readout import gated_readout_function
 from .utils import glorot_init
 
@@ -24,19 +24,26 @@ def _propagation_function():
 
     class GCNPropagation(torch.autograd.Function):
         """Autograd node around the C ABI: forward = ggnn_gcn_set_weights + ggnn_forward, backward = ggnn_gcn_backward.
-        ``weights`` are the L kernels, then the L biases when the engine uses them."""
+        ``weights`` are the L kernels, then the L biases when the engine uses them, and, when they hold one more, the adjacency weights
+        [num_messages()] of a message-weighted batch (set before the forward, their gradient from ggnn_gcn_backward_weighted)."""
 
         @staticmethod
         def forward(ctx, engine, h0, *weights):
             L = engine.L
+            n_layer = L * (2 if engine.use_bias else 1)
+            aw = weights[n_layer] if len(weights) > n_layer else None
             # ctx.needs_input_grad is all False under torch.no_grad() (validation epochs): no activations are saved there
             need = any(ctx.needs_input_grad[1:])
             kernels = [k.detach().contiguous() for k in weights[:L]]
-            biases = [b.detach().contiguous() for b in weights[L:]] or None
+            biases = [b.detach().contiguous() for b in weights[L:n_layer]] or None
             engine.set_weights(kernels, biases)
+            if aw is not None:
+                aw = aw.detach().contiguous()
+                engine.set_message_weights(aw)
             engine.set_deterministic(torch.are_deterministic_algorithms_enabled())
             engine.set_save_for_backward(need)
             out = engine.forward(h0.detach().contiguous())
+            ctx.aw_index = n_layer if aw is not None and ctx.needs_input_grad[2 + n_layer] else None
             ctx.serial = engine.serial   # the backward refuses once another forward, graph or weights replaced this one's
             ctx.engine, ctx.shapes = engine, [t.shape for t in weights]
             ctx.h0_needs = bool(ctx.needs_input_grad[1])
@@ -47,14 +54,33 @@ def _propagation_function():
         def backward(ctx, d_out):
             ctx.engine.require_serial(ctx.serial, "the GCN propagation's backward")
             L = ctx.engine.L
+            n_layer = L * (2 if ctx.engine.use_bias else 1)
             grads = [torch.zeros(s, dtype=torch.float32, device=d_out.device) for s in ctx.shapes]
-            layers = [{'kernel': grads[l], 'bias': grads[L + l] if len(grads) > L else None} for l in range(L)]
+            layers = [{'kernel': grads[l], 'bias': grads[L + l] if n_layer > L else None} for l in range(L)]
             d_h0 = torch.zeros_like(d_out) if ctx.h0_needs else None
             ctx.engine.set_deterministic(torch.are_deterministic_algorithms_enabled())
-            ctx.engine.backward(d_out.contiguous(), layers, d_h0)
+            if ctx.aw_index is None:
+                ctx.engine.backward(d_out.contiguous(), layers, d_h0)
+            else:
+                ctx.engine.backward(d_out.contiguous(), layers, d_h0, d_adjacency_weights=grads[ctx.aw_index])
             return (None, d_h0) + tuple(grads)
 
     return GCNPropagation
+
+
+def propagate(engine: GCNEngine, h0, kernels: Sequence, biases: Optional[Sequence] = None, adjacency_weights=None):
+    """The sparse GCN propagation as a differentiable torch function, without a ChemModel: ``engine`` holds the current batch (for
+    ``adjacency_weights``, a message-weighted one: ``prepare_graph_gcn_message_weighted`` + ``set_graph_prepared``), ``h0`` [V, D],
+    ``kernels[l]`` [D, D] and, when the engine uses biases, ``biases[l]`` [D], fp32 CUDA tensors, and ``adjacency_weights`` an fp32 CUDA
+    tensor [nnz] in list order (the weights of ``adjacency_weights`` in ``set_graph_gcn``, computed in torch: a learned or renormalized
+    ``D^-1/2 (A+I) D^-1/2``, a DropEdge mask).  Returns the last layer's node states [V, D]; gradients reach ``h0``, every kernel and bias,
+    and ``adjacency_weights``."""
+    if (biases is not None) != engine.use_bias or len(kernels) != engine.L:
+        raise GgnnError("expected %d kernels%s" % (engine.L, " and %d biases" % engine.L if engine.use_bias else " and no biases"))
+    weights = list(kernels) + (list(biases) if biases is not None else [])
+    if adjacency_weights is not None:
+        weights.append(adjacency_weights)
+    return _propagation_function().apply(engine, h0, *weights)
 
 
 class SparseGCNChemModel(ChemModel):

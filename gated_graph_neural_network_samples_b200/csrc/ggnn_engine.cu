@@ -179,8 +179,9 @@ struct BatchPlan {
     bool all_virtual = false;   // attention on the streaming plan: every (target, type) pair with messages is a virtual row, weighted by the
                                 // step's attention probabilities through vslot (the image has vslot and no slot weights); a message-weighted
                                 // batch likewise, weighted by its slot weights, so that the plan does not depend on their values
-    bool msg_weighted = false;  // ggnn_prepare_graph_sparse_weighted: weighted, its slot weights zero in the image until ggnn_set_message_weights
-                                // writes them on the device; the image carries the source-keyed CSR's slot map (tslot) with save_for_backward
+    bool msg_weighted = false;  // ggnn_prepare_graph_sparse_weighted / ggnn_prepare_graph_gcn_message_weighted: weighted, its slot weights
+                                // zero in the image until ggnn_set_message_weights writes them on the device; the image carries the
+                                // source-keyed CSR's slot map (tslot) with save_for_backward
     size_t off_slotw = 0, off_tslotw = 0;   // weighted: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
     // (offset, bytes) of the image's bytes no section builder writes: alignment gaps and the one-element room of empty sections.  The host
     // builder zeroes them (the device dataset zeroes its whole image), so that an image is one function of its batch, whatever the
@@ -1527,8 +1528,8 @@ static int64_t gcn_pairs(int64_t V, int64_t nnz, const int64_t* list, int32_t* p
 // ---- the host half of ggnn_set_graph_sparse: validation, tile plan, stable target-sorted CSR, streaming tables -> g->image.
 // `weighted`: the batch has one weight per message, `w`, in the type-major message order (required when there are messages); the image
 // then carries them in target-CSR order and, with the source-keyed CSR, in source-CSR order.  `stream_weighted`: see build_plan.
-// `msg_weighted` (with weighted and stream_weighted, and w null): the weights come later, on the device -- the weight sections are zero and
-// the plan is the one every weight vector shares.
+// `msg_weighted` (with weighted and w null; for the GGNN with stream_weighted): the weights come later, on the device -- the weight sections
+// are zero and the plan is the one every weight vector shares.
 // Nothing here touches the device except the pinned allocation of the image and the wait for the previous upload out of it.
 static int build_sparse_image(ggnn_prepared_graph* g, int32_t V, const int32_t* const* adj, const int32_t* num_edges, const float* indeg,
                               bool weighted, const float* w, bool stream_weighted = false, bool msg_weighted = false) {
@@ -2535,10 +2536,12 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
 
 // ------------------------------------------------------------------------------------------ sparse GCN (chem_tensorflow_gcn.py:42-82)
 // Host half of a GCN batch: validate the int64 (row i = output, column j = input) list, feed it to the GGNN builder as one edge type
-// (source j -> target i, list order kept) with the weights as per-message weights.
-static int build_gcn_image(ggnn_prepared_graph* g, int32_t V, int64_t nnz, const int64_t* list, const float* w) {
+// (source j -> target i, list order kept) with the weights as per-message weights.  `msg_weighted` (w null): the weights come later, on the
+// device (ggnn_set_message_weights) -- the weight sections are zero and, with save_for_backward, the image carries the source-keyed CSR's
+// slot map.  No GCN plan depends on the weights' values.
+static int build_gcn_image(ggnn_prepared_graph* g, int32_t V, int64_t nnz, const int64_t* list, const float* w, bool msg_weighted = false) {
     g->valid = false;
-    if (V < 0 || nnz < 0 || (nnz > 0 && (!list || !w))) return g->fail(GGNN_EINVAL, "null/negative argument");
+    if (V < 0 || nnz < 0 || (nnz > 0 && (!list || (!w && !msg_weighted)))) return g->fail(GGNN_EINVAL, "null/negative argument");
     if (nnz > 0x7fffffff) return g->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
     std::vector<int32_t> pairs((size_t)nnz * 2);
     if (const int64_t k = gcn_pairs(V, nnz, list, pairs.data()); k >= 0)
@@ -2547,7 +2550,10 @@ static int build_gcn_image(ggnn_prepared_graph* g, int32_t V, int64_t nnz, const
     const std::vector<float> indeg((size_t)std::max(V, 1), 0.0f);
     const int32_t* lists[1] = {pairs.data()};
     const int32_t counts[1] = {(int32_t)nnz};
-    return build_sparse_image(g, V, lists, counts, indeg.data(), true, w);
+    if (!msg_weighted) return build_sparse_image(g, V, lists, counts, indeg.data(), true, w);
+    if (int rc = build_sparse_image(g, V, lists, counts, indeg.data(), true, nullptr, false, true)) return rc;
+    g->plan.plan_text += " [message-weighted]";
+    return GGNN_OK;
 }
 
 int ggnn_gcn_create(const ggnn_gcn_config* cfg, ggnn_engine** out) {
@@ -2585,6 +2591,18 @@ int ggnn_host_prepare_graph_gcn(const ggnn_gcn_config* cfg, int32_t num_sms, int
                                 const int64_t* list, const float* w, ggnn_prepared_graph** inout) {
     if (int rc = begin_prepare(inout, nullptr, cfg, num_sms, save_for_backward, __func__)) return rc;
     return build_gcn_image(*inout, V, nnz, list, w);
+}
+
+int ggnn_prepare_graph_gcn_message_weighted(const ggnn_engine* e, int32_t save_for_backward, int32_t V, int64_t nnz, const int64_t* list,
+                                            ggnn_prepared_graph** inout) {
+    if (int rc = begin_prepare<ggnn_gcn_config>(inout, e, nullptr, 0, save_for_backward, __func__)) return rc;
+    return build_gcn_image(*inout, V, nnz, list, nullptr, true);
+}
+
+int ggnn_host_prepare_graph_gcn_message_weighted(const ggnn_gcn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t V,
+                                                 int64_t nnz, const int64_t* list, ggnn_prepared_graph** inout) {
+    if (int rc = begin_prepare(inout, nullptr, cfg, num_sms, save_for_backward, __func__)) return rc;
+    return build_gcn_image(*inout, V, nnz, list, nullptr, true);
 }
 
 int ggnn_set_graph_gcn(ggnn_engine* e, int32_t V, int64_t nnz, const int64_t* list, const float* w, ggnn_stream_t stream) {
@@ -2707,10 +2725,12 @@ static int forward_gcn(ggnn_engine* e, const float* h0, float* h_out, cudaStream
 //   dW  += S^T . dPre,  db += sum dPre            (gemm_tn: atomic or fixed-order split sums, the bias rides along)
 //   dS   = dPre . W^T                             (gemm_nt)
 //   dH_l = A^T . dS                               (csr_gather_all_kernel over the source-keyed CSR with its per-slot weights: no float atomics)
-int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0, ggnn_stream_t stream) {
+// With d_dw (DEVICE [nnz] or null: the adjacency weights' gradient of a message-weighted batch, accumulated into) dS is formed on every
+// layer, layer 0 included, and gcn_source_grad_kernel replaces the last gather: the same dH_l bits, and d w_k += <dS_l[i_k], H_l[j_k]> into
+// a per-target-slot sum (dw_slot) that msgw::add_slot_grads_kernel adds into d_dw at the end.
+static int gcn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0,
+                             float* d_dw, ggnn_stream_t stream) {
     using namespace ggnn::bwd;
-    if (!e) return GGNN_EINVAL;
-    GGNN_REQUIRE_MODEL(e, MODEL_GCN);
     if (int rc = begin_backward(e, "ggnn_gcn_backward", "setting the graph", d_h_out, grads, num_layers, d_h0)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int V = e->V, D = e->D, L = e->L;
@@ -2718,9 +2738,13 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
     const size_t vd = (size_t)V * D;
     const size_t slab = align_up(vd * sizeof(float), 256);
     const size_t ws_floats = std::max(gemm_tn_workspace(e, true, e->use_bias, V, D, D, 1), gemm_tn_workspace(e, false, e->use_bias, V, D, D, 1));
-    CU_TRY(e, e->bwd_buf.reserve(4 * slab + ws_floats * sizeof(float)));
+    const bool want_dw = d_dw && e->M > 0;
+    const size_t o_dws = align_up(4 * slab + ws_floats * sizeof(float), 256);
+    CU_TRY(e, e->bwd_buf.reserve(want_dw ? o_dws + sizeof(float) * (size_t)e->M : 4 * slab + ws_floats * sizeof(float)));
     char* bb = (char*)e->bwd_buf.ptr;
     float *dH = (float*)bb, *dP = (float*)(bb + slab), *S = (float*)(bb + 2 * slab), *dS = (float*)(bb + 3 * slab), *ws = (float*)(bb + 4 * slab);
+    float* dw_slot = (float*)(bb + o_dws);
+    if (want_dw) CU_TRY(e, cudaMemsetAsync(dw_slot, 0, sizeof(float) * (size_t)e->M, st));
     const ImageView& gd = e->gd;
     std::vector<const float*> fstate(L + 1);
     for (int l = 0; l <= L; ++l) fstate[l] = layer_state(e, l, e->last_h0, e->last_out);
@@ -2750,16 +2774,48 @@ int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer
             memset(&none, 0, sizeof none);
             if (int rc = gemm_tn(e, st, ws, ws_floats, none, 1, true, dpre, D, nullptr, D, 0, gw.bias, V, D, D)) return rc;
         }
-        if (l == 0 && !d_h0) break;
+        if (l == 0 && !d_h0 && !want_dw) break;
         gemm_nt(e, st, false, dpre, D, 0, e->gcn_w[l].kernel, D, 0, 1, dS, D, V, D, D);
         float* dst = l == 0 ? d_h0 : dH;
-        GatherJob j{gd.trow, gd.ttgt, dS, dst, gd.tslotw, nullptr};
-        csr_gather_all_kernel<<<gather_grid, 256, 0, st>>>(j, j, V, D, 1);
+        if (want_dw) {
+            const bool want_dh = dst != nullptr;
+            void (*kern)(const int*, const int*, const int*, const float*, const float*, const float*, float*, float*, int, int) = nullptr;
+            switch ((D + 127) / 128) {
+#define GGNN_GCN_SRC_CASE(ch) \
+    case ch: kern = want_dh ? gcn::gcn_source_grad_kernel<ch, true> : gcn::gcn_source_grad_kernel<ch, false>; break;
+                GGNN_GCN_SRC_CASE(1) GGNN_GCN_SRC_CASE(2) GGNN_GCN_SRC_CASE(3) GGNN_GCN_SRC_CASE(4)
+#undef GGNN_GCN_SRC_CASE
+                default: return e->fail(GGNN_EUNSUPPORTED, "no GCN source-row gradient kernel for D=%d", D);
+            }
+            kern<<<gather_grid, 256, 0, st>>>(gd.trow, gd.ttgt, gd.tslot, gd.tslotw, dS, fstate[l], dst, dw_slot, V, D);
+        } else {
+            GatherJob j{gd.trow, gd.ttgt, dS, dst, gd.tslotw, nullptr};
+            csr_gather_all_kernel<<<gather_grid, 256, 0, st>>>(j, j, V, D, 1);
+        }
         ++e->last_launches;
         dout = dst;
     }
+    if (want_dw) {
+        msgw::add_slot_grads_kernel<<<(int)std::min<int64_t>((e->M + 255) / 256, 4096), 256, 0, st>>>(gd.msg, dw_slot, d_dw, e->M);
+        ++e->last_launches;
+    }
     CU_TRY(e, cudaGetLastError());
     return GGNN_OK;
+}
+
+int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GCN);
+    return gcn_backward_impl(e, d_h_out, grads, num_layers, d_h0, nullptr, stream);
+}
+
+int ggnn_gcn_backward_weighted(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0,
+                               float* d_adjacency_weights, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GCN);
+    if (d_adjacency_weights && !e->msg_weighted)
+        return e->fail(GGNN_ESTATE, "d_adjacency_weights needs a message-weighted batch (ggnn_prepare_graph_gcn_message_weighted)");
+    return gcn_backward_impl(e, d_h_out, grads, num_layers, d_h0, d_adjacency_weights, stream);
 }
 
 int ggnn_forward(ggnn_engine* e, const float* h0, float* h_out, ggnn_stream_t stream) {
@@ -3196,11 +3252,13 @@ int ggnn_backward_weighted(ggnn_engine* e, const float* d_h_out, const ggnn_laye
     return ggnn_backward_impl(e, d_h_out, grads, num_layers, d_h0, d_message_weights, stream);
 }
 
+// GGNN and GCN engines: a GCN's adjacency weights are its one edge type's message weights, in list order.
 int ggnn_set_message_weights(ggnn_engine* e, const float* message_weights, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
-    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
     if (!e->graph_set) return no_graph(e);
-    if (!e->msg_weighted) return e->fail(GGNN_ESTATE, "the current batch is not message-weighted (ggnn_prepare_graph_sparse_weighted)");
+    if (!e->msg_weighted)
+        return e->fail(GGNN_ESTATE, "the current batch is not message-weighted (%s)",
+                       e->model == MODEL_GCN ? "ggnn_prepare_graph_gcn_message_weighted" : "ggnn_prepare_graph_sparse_weighted");
     if (!message_weights && e->M > 0) return e->fail(GGNN_EINVAL, "null message weights");
     CU_TRY(e, cudaSetDevice(e->device));
     e->msg_weights_set = false;

@@ -15,7 +15,8 @@
 //                     weighted CSR gather into shared memory, FFMA GEMM with W_l from L1/L2, same epilogue.
 //   gcn_gather_image_kernel  hidden sizes above 128 on bf16x3 / bf16 with wide_hidden: S = A . H into the streaming operand image, which the
 //                     TMA-fed ts::ggnn_stream_kernel multiplies by W_l (EPI_GCN: the same epilogue); two launches per layer.
-// The backward pass (ggnn_engine.cu) reuses ggnn_bwd.cuh; only the relu / dropout gradient below is GCN-specific.
+// The backward pass (ggnn_engine.cu) reuses ggnn_bwd.cuh; only the relu / dropout gradient below is GCN-specific, and on a
+// message-weighted batch the source-row pass that also forms the adjacency weights' gradient (gcn_source_grad_kernel).
 #pragma once
 #include "ggnn_common.cuh"
 #include "ggnn_fwd_stream.cuh"
@@ -266,6 +267,60 @@ __global__ void gcn_relu_dropout_grad_kernel(const float* __restrict__ dy, const
                                              long long n) {
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
         dpre[i] = y[i] > 0.0f ? dy[i] * inv_keep : 0.0f;
+}
+
+// ------------------------------------------------------------------------------------------------ message-weighted batches: d w
+// One layer's source-row pass of the backward on a message-weighted batch (ggnn_gcn_backward_weighted), over the source-keyed CSR
+// (trow [V+1], ttgt / tslot / tslotw [nnz]): for every source row j and each of its entries e (target i = ttgt[e]), in order,
+//   dH[j]               = sum_e tslotw[e] * dS[i]     per element fmaf(w, x, acc) from 0: csr_gather_all_kernel's arithmetic, bit for bit
+//   dw_slot[tslot[e]]  += <dS[i], H[j]>               the entry's term of d w = sum_l <dS_l[i], H_l[j]>
+// dS[i] is read once for both.  One warp per source row; lane c owns the float4 column chunks c, c + 32, ... (CHUNKS of them, so
+// D <= 128 * CHUNKS), H[j] stays in registers.  The lanes' partial dots are added by a fixed butterfly and lane 0 adds the sum into the
+// entry's target slot, which no other entry shares: no atomics, the same bits on every call.  WANT_DH = false (layer 0 without d h0) forms
+// d w alone.  D is a multiple of 4; rows are 16-byte aligned.
+template <int CHUNKS, bool WANT_DH>
+__global__ void __launch_bounds__(256) gcn_source_grad_kernel(const int* __restrict__ trow, const int* __restrict__ ttgt,
+                                                              const int* __restrict__ tslot, const float* __restrict__ tslotw,
+                                                              const float* __restrict__ dS, const float* __restrict__ H, float* __restrict__ dH,
+                                                              float* __restrict__ dw_slot, int V, int D) {
+    const int j = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (j >= V) return;
+    const int D4 = D >> 2;
+    float4 h[CHUNKS], acc[CHUNKS];
+#pragma unroll
+    for (int c = 0; c < CHUNKS; ++c) {
+        const int c4 = lane + 32 * c;
+        h[c] = c4 < D4 ? reinterpret_cast<const float4*>(H + (size_t)j * D)[c4] : make_float4(0.f, 0.f, 0.f, 0.f);
+        acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    const int beg = trow[j], end = trow[j + 1];
+    for (int e = beg; e < end; ++e) {
+        const float a = tslotw[e];
+        const float4* row = reinterpret_cast<const float4*>(dS + (size_t)ttgt[e] * D);
+        float s = 0.f;
+#pragma unroll
+        for (int c = 0; c < CHUNKS; ++c) {
+            const int c4 = lane + 32 * c;
+            if (c4 < D4) {
+                const float4 x = row[c4];
+                if (WANT_DH) {
+                    acc[c].x = fmaf(a, x.x, acc[c].x); acc[c].y = fmaf(a, x.y, acc[c].y);
+                    acc[c].z = fmaf(a, x.z, acc[c].z); acc[c].w = fmaf(a, x.w, acc[c].w);
+                }
+                s = fmaf(x.x, h[c].x, s); s = fmaf(x.y, h[c].y, s); s = fmaf(x.z, h[c].z, s); s = fmaf(x.w, h[c].w, s);
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (lane == 0) dw_slot[tslot[e]] += s;
+    }
+    if (WANT_DH) {
+#pragma unroll
+        for (int c = 0; c < CHUNKS; ++c) {
+            const int c4 = lane + 32 * c;
+            if (c4 < D4) reinterpret_cast<float4*>(dH + (size_t)j * D)[c4] = acc[c];
+        }
+    }
 }
 
 }  // namespace gcn

@@ -87,15 +87,20 @@ class GgnnError(Exception):
     """Raised for every non-zero return of the C ABI (the reference raises plain ``Exception``s too)."""
 
 
-def _gcn_arrays(adjacency_list, adjacency_weights):
-    """The GCN feed as the C ABI takes it: ``[nnz, 2]`` int64 and ``[nnz]`` float32, contiguous (float64 packer weights are cast here,
-    as the reference's float32 placeholder does at the feed)."""
+def _gcn_list(adjacency_list):
+    """A GCN adjacency list as the C ABI takes it: ``[nnz, 2]`` int64, contiguous."""
     lst = np.asarray(adjacency_list)
     if lst.size == 0:
         lst = lst.reshape(0, 2)
     if lst.ndim != 2 or lst.shape[1] != 2:
         raise GgnnError("adjacency_list must be [nnz, 2] (row i = output, column j = input), got shape %s" % (lst.shape,))
-    lst = np.ascontiguousarray(lst, dtype=np.int64)
+    return np.ascontiguousarray(lst, dtype=np.int64)
+
+
+def _gcn_arrays(adjacency_list, adjacency_weights):
+    """The GCN feed as the C ABI takes it: ``[nnz, 2]`` int64 and ``[nnz]`` float32, contiguous (float64 packer weights are cast here,
+    as the reference's float32 placeholder does at the feed)."""
+    lst = _gcn_list(adjacency_list)
     w = np.asarray(adjacency_weights)
     if w.ndim != 1:
         raise GgnnError("adjacency_weights must be [nnz], got shape %s" % (w.shape,))
@@ -177,6 +182,18 @@ class PreparedGraph:
         lst, w = _gcn_arrays(adjacency_list, adjacency_weights)
         return g._fill(g.lib.ggnn_host_prepare_graph_gcn, int(num_nodes), 1, C.byref(cfg), int(num_sms), int(bool(save_for_backward)),
                        int(num_nodes), lst.shape[0], lst.ctypes.data, w.ctypes.data)
+
+    @classmethod
+    def host_only_gcn_message_weighted(cls, hidden_size: int, num_layers: int, num_nodes: int, adjacency_list, use_bias: bool = False,
+                                       precision: str = "fp32", num_sms: int = 132, save_for_backward: bool = False,
+                                       reuse: Optional["PreparedGraph"] = None, wide_hidden: bool = False) -> "PreparedGraph":
+        """``ggnn_host_prepare_graph_gcn_message_weighted``: a GCN batch whose adjacency weights come later on the device (see
+        ``GCNEngine.prepare_graph_gcn_message_weighted``), no engine, no GPU."""
+        g = reuse if reuse is not None else cls()
+        cfg = _lib.GcnConfig(int(hidden_size), int(num_layers), int(bool(use_bias)), PRECISIONS[precision], 0, int(bool(wide_hidden)))
+        lst = _gcn_list(adjacency_list)
+        return g._fill(g.lib.ggnn_host_prepare_graph_gcn_message_weighted, int(num_nodes), 1, C.byref(cfg), int(num_sms),
+                       int(bool(save_for_backward)), int(num_nodes), lst.shape[0], lst.ctypes.data)
 
     def _fill(self, prepare, V: int, T: int, *args) -> "PreparedGraph":
         """Runs the C prepare call ``prepare(*args, &handle)`` into this handle (the call allocates it when empty)."""
@@ -948,7 +965,10 @@ class GCNEngine(PropagationEngine):
     the inherited calls.  The GGNN-only calls raise ``GgnnError`` (the library refuses them on a GCN engine).
 
     ``wide_hidden`` (``ggnn_gcn_config.wide_hidden``): hidden sizes up to 512, and above 128 on bf16x3 / bf16 the streaming wgmma plan
-    (a weighted gather and one GEMM launch per layer) instead of the fp32 kernel.  Batches and datasets must be prepared with the same value."""
+    (a weighted gather and one GEMM launch per layer) instead of the fp32 kernel.  Batches and datasets must be prepared with the same value.
+
+    Adjacency weights on the device: ``prepare_graph_gcn_message_weighted`` + ``set_graph_prepared``, then ``set_message_weights(w)`` (the
+    inherited call) before every forward that should use new weights, and ``backward(..., d_adjacency_weights=)`` for their gradient."""
 
     def __init__(self, hidden_size: int, num_layers: int, use_bias: bool = False, device: int = 0, precision: str = "fp32",
                  wide_hidden: bool = False):
@@ -1002,11 +1022,34 @@ class GCNEngine(PropagationEngine):
         return g._fill(self.lib.ggnn_prepare_graph_gcn, int(num_nodes), 1, self._h, -1 if save_for_backward is None else int(bool(save_for_backward)),
                        int(num_nodes), lst.shape[0], lst.ctypes.data, w.ctypes.data)
 
-    def backward(self, d_out, grads: Sequence[dict], d_h0=None):
-        """``grads[l]``: dict with optional ``kernel`` [D, D] / ``bias`` [D] fp32 CUDA tensors, accumulated into."""
+    def prepare_graph_gcn_message_weighted(self, num_nodes: int, adjacency_list, save_for_backward: Optional[bool] = None,
+                                           reuse: Optional[PreparedGraph] = None) -> PreparedGraph:
+        """``prepare_graph_gcn`` for a MESSAGE-WEIGHTED batch (``ggnn_prepare_graph_gcn_message_weighted``): the list alone, no host weights.
+        After ``set_graph_prepared``, ``set_message_weights(w)`` puts the adjacency weights on the device -- ``w`` a contiguous fp32 CUDA
+        tensor of ``num_messages()`` = nnz entries in list order -- and every forward uses them as ``adjacency_weights``; ``backward(...,
+        d_adjacency_weights=)`` adds their gradient.  One prepared batch takes new weights every step (learned edge weights, DropEdge with
+        renormalization) without host work."""
+        lst = _gcn_list(adjacency_list)
+        g = reuse if reuse is not None else PreparedGraph(self.lib)
+        return g._fill(self.lib.ggnn_prepare_graph_gcn_message_weighted, int(num_nodes), 1, self._h,
+                       -1 if save_for_backward is None else int(bool(save_for_backward)), int(num_nodes), lst.shape[0], lst.ctypes.data)
+
+    def backward(self, d_out, grads: Sequence[dict], d_h0=None, d_adjacency_weights=None):
+        """``grads[l]``: dict with optional ``kernel`` [D, D] / ``bias`` [D] fp32 CUDA tensors, accumulated into.  With
+        ``d_adjacency_weights`` (fp32 CUDA [num_messages()], accumulated into; message-weighted batches only) ``ggnn_gcn_backward_weighted``,
+        which also forms the adjacency weights' gradient."""
         arr = (_lib.GcnLayerWeights * len(grads))()
         for l, g in enumerate(grads):
             arr[l].kernel = None if g.get("kernel") is None else g["kernel"].data_ptr()
             arr[l].bias = None if g.get("bias") is None else g["bias"].data_ptr()
-        self._check(self.lib.ggnn_gcn_backward(self._h, d_out.data_ptr(), arr, len(grads), None if d_h0 is None else d_h0.data_ptr(),
-                                               self._stream()))
+        if d_adjacency_weights is None:
+            self._check(self.lib.ggnn_gcn_backward(self._h, d_out.data_ptr(), arr, len(grads), None if d_h0 is None else d_h0.data_ptr(),
+                                                   self._stream()))
+            return
+        import torch
+        if not (isinstance(d_adjacency_weights, torch.Tensor) and d_adjacency_weights.is_cuda and d_adjacency_weights.dtype == torch.float32
+                and d_adjacency_weights.is_contiguous() and d_adjacency_weights.numel() == self.num_messages()):
+            raise GgnnError("d_adjacency_weights must be a contiguous fp32 CUDA tensor of num_messages() entries")
+        self._check(self.lib.ggnn_gcn_backward_weighted(self._h, d_out.data_ptr(), arr, len(grads), None if d_h0 is None else d_h0.data_ptr(),
+                                                        d_adjacency_weights.data_ptr() if d_adjacency_weights.numel() else None,
+                                                        self._stream()))

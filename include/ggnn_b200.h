@@ -386,10 +386,10 @@ int ggnn_host_tile_plan(int32_t hidden_size, int32_t num_edge_types, int32_t pre
  * ggnn_set_state_dropout (outputs of layers 0..L-2, global step = layer index), ggnn_set_save_for_backward, ggnn_readout_*,
  * ggnn_layer_state (intermediate layers: after a forward with save_for_backward on), ggnn_plan_description,
  * ggnn_last_launch_count, ggnn_prepared_graph_info and ggnn_prepared_graph_arrays (T = 1: row_ptr [V+1] keyed by the output row i,
- * src = the input column j, msg = position in the input list) work on it as on a GGNN engine.  The GGNN-only calls
- * (ggnn_set_weights, ggnn_set_graph_sparse/dense, ggnn_prepare_graph_sparse/dense, ggnn_prepare_graph_sparse_weighted, ggnn_run_*,
- * ggnn_set_message_weights, ggnn_backward, ggnn_backward_weighted) return GGNN_ESTATE on a
- * GCN engine, and the GCN calls below return GGNN_ESTATE on a GGNN engine.
+ * src = the input column j, msg = position in the input list) work on it as on a GGNN engine, and so does ggnn_set_message_weights on a
+ * message-weighted GCN batch (below).  The GGNN-only calls (ggnn_set_weights, ggnn_set_graph_sparse/dense,
+ * ggnn_prepare_graph_sparse/dense, ggnn_prepare_graph_sparse_weighted, ggnn_run_*, ggnn_backward, ggnn_backward_weighted) return
+ * GGNN_ESTATE on a GCN engine, and the GCN calls below return GGNN_ESTATE on a GGNN engine.
  * Limits: hidden_size a positive multiple of 4 and <= 256 (<= 512 with wide_hidden), 1 <= num_layers <= 16.  precision
  * GGNN_PREC_BF16X3 / GGNN_PREC_BF16 run the fused wgmma kernel for hidden_size <= 128; GGNN_PREC_FP32 runs the fp32 CUDA-core kernel at
  * every hidden size.  Above 128 on GGNN_PREC_BF16X3 / GGNN_PREC_BF16:
@@ -432,6 +432,30 @@ int ggnn_prepared_graph_slot_weights(const ggnn_prepared_graph* g, float* target
  * layer, accumulated into; d_h0 [V, D] DEVICE or NULL.  fp32 on CUDA cores whatever the forward precision. */
 int ggnn_gcn_backward(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0,
                       ggnn_stream_t stream);
+/* ---- Adjacency weights on the device (GCN engine).  Entry k of the list, (i_k, j_k), weighs w_k, from a DEVICE fp32 [nnz] buffer in list
+ * order; per layer l with input H_l:
+ *     S_l[i] = sum_{k : i_k = i} w_k H_l[j_k]   (list order, as above)      d w_k = sum_l <dS_l[i_k], H_l[j_k]>,  dS_l = dPre_l . W_l^T
+ * Duplicate entries keep their own weight and gradient; any finite weight is allowed.  The same values fed as host weights through
+ * ggnn_prepare_graph_gcn give the same forward and the same d_h0 / kernel / bias gradients, bit for bit.
+ *   ggnn_prepare_graph_gcn_message_weighted   ggnn_prepare_graph_gcn without host weights (same validation and GGNN_ERANGE, CSR, tile plan,
+ *                                             pinned image; no plan depends on the weights' values): the batch is marked message-weighted,
+ *                                             its slot-weight sections are zero until ggnn_set_message_weights writes them on the device, and
+ *                                             with save_for_backward the image also carries the source-keyed CSR's slot map.  The plan text
+ *                                             ends in " [message-weighted]".  The host-only twin needs no engine or GPU.
+ *   ggnn_set_message_weights                  (see the sparse GGNN's message weights above) message_weights = w, [nnz] (ggnn_num_messages):
+ *                                             GGNN_ESTATE on a batch that is not message-weighted; every upload forgets the weights, a forward
+ *                                             without them is GGNN_ESTATE, and setting them drops the saved activations.
+ *   ggnn_gcn_backward_weighted                ggnn_gcn_backward, and with d_adjacency_weights (DEVICE fp32 [nnz], accumulated into) the weights'
+ *                                             gradient: dS_l on every layer and one source-row pass per layer that forms dH_l (the same bits as
+ *                                             ggnn_gcn_backward's gather) and each entry's dot product into a per-entry sum, without atomics --
+ *                                             bit-identical from call to call in both deterministic modes.  ggnn_gcn_backward is this call with
+ *                                             d_adjacency_weights = NULL; a non-NULL one on a batch that is not message-weighted is GGNN_ESTATE. */
+int ggnn_prepare_graph_gcn_message_weighted(const ggnn_engine* e, int32_t save_for_backward, int32_t num_nodes, int64_t nnz,
+                                            const int64_t* adjacency_list, ggnn_prepared_graph** inout);
+int ggnn_host_prepare_graph_gcn_message_weighted(const ggnn_gcn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t num_nodes,
+                                                 int64_t nnz, const int64_t* adjacency_list, ggnn_prepared_graph** inout);
+int ggnn_gcn_backward_weighted(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0,
+                               float* d_adjacency_weights, ggnn_stream_t stream);
 
 /* ---- Device-resident datasets: the training graphs uploaded once, every batch of whole graphs assembled on the device.
  * Graphs never share edges, so a batch's graph image is its graphs' pieces (CSR slice, in-degrees, denominators, source-keyed CSR,
