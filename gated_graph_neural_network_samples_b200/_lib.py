@@ -74,7 +74,9 @@ SYMBOLS = {
     "ggnn_set_graph_dense_weighted": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "ggnn_host_prepare_graph_dense_weighted": (C.c_int, [C.POINTER(GgnnConfig), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                                          C.POINTER(C.c_void_p)]),
-    "ggnn_prepared_graph_stream_tables": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int64)] + [C.c_void_p] * 5),
+    "ggnn_prepare_graph_dense_device": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]),
+    "ggnn_host_prepare_graph_dense_device": (C.c_int, [C.POINTER(GgnnConfig), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]),
+    "ggnn_prepared_graph_stream_tables":(C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int64)] + [C.c_void_p] * 5),
     "ggnn_set_graph_dense": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "ggnn_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ggnn_forward_host": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -17,6 +17,19 @@ from .utils import glorot_init
 from .workloads import dense_engine_params
 
 
+def propagate(engine: PropagationEngine, h0, layer: dict, adjacency):
+    """The dense GGNN propagation as a differentiable torch function, without a ChemModel: ``engine`` holds a batch of
+    ``prepare_graph_dense_device(b, v)`` (adopted with ``set_graph_prepared``), ``h0`` [b*v, D], ``layer`` a dict of fp32 CUDA tensors keyed
+    like ``ggnn_layer_weights`` (``engine.WEIGHT_FIELDS``) and ``adjacency`` the fp32 CUDA ``[b, T, v, v]`` matrix, ``A[g, t, i, j]`` the
+    weight of the type-t message from node j to node i of graph g (any finite values).  Returns the final node states [b*v, D]; gradients
+    reach ``h0``, every layer tensor and every entry of ``adjacency``."""
+    lay, flat = {}, []
+    for k, v in layer.items():
+        lay[k] = len(flat)
+        flat.append(v)
+    return _propagation_function().apply(engine, [lay], h0, *flat, adjacency)
+
+
 class DenseGGNNChemModel(ChemModel):
     @classmethod
     def default_params(cls):
@@ -71,8 +84,17 @@ class DenseGGNNChemModel(ChemModel):
         import torch
         feed = self.feed
         T, D = self.num_edge_types, self.params['hidden_size']
+        device_adj = None
         if feed.get('_graph_adopted'):   # a device-data batch, assembled on the device by forward_batch (_adopt_dataset_batch)
             b, v = int(feed[self.placeholders['num_graphs']]), int(feed[self.placeholders['num_vertices']])
+        elif isinstance(feed[self.placeholders['adjacency_matrix']], torch.Tensor):
+            # a torch tensor (a computed or learned adjacency, [b, e, v, v]): the batch is planned from its shape, the matrix goes to the
+            # engine's device as it is (ggnn_set_message_weights) and whatever produced it gets its gradient
+            device_adj = feed[self.placeholders['adjacency_matrix']].to(self.device, torch.float32).contiguous()
+            b, v = device_adj.shape[0], device_adj.shape[2]
+            self.engine.set_save_for_backward(torch.is_grad_enabled())
+            self._dense_device_graph = self.engine.prepare_graph_dense_device(b, v, reuse=getattr(self, '_dense_device_graph', None))
+            self.engine.set_graph_prepared(self._dense_device_graph)
         else:
             adj = np.asarray(feed[self.placeholders['adjacency_matrix']], dtype=np.float32)      # [b, e, v, v]
             b, v = adj.shape[0], adj.shape[2]
@@ -96,12 +118,13 @@ class DenseGGNNChemModel(ChemModel):
             lay[k] = len(flat); flat.append(t)
         h0 = self.initial_node_representation_tensor().reshape(b * v, D)                         # dense:97
         DP = getattr(self, '_padded_hidden', D)
+        adj = [] if device_adj is None else [device_adj]   # the trailing message-weight slot of the autograd node
         if DP != D:
             from .chem_sparse import SparseGGNNChemModel
             flat = [SparseGGNNChemModel._pad_hidden(k, flat[i], D, DP) for k, i in lay.items()]
             h0 = torch.nn.functional.pad(h0, (0, DP - D)).contiguous()
-            return self._propagation.apply(self.engine, [lay], h0, *flat)[:, :D].reshape(b, v, D)
-        out = self._propagation.apply(self.engine, [lay], h0, *flat)
+            return self._propagation.apply(self.engine, [lay], h0, *flat, *adj)[:, :D].reshape(b, v, D)
+        out = self._propagation.apply(self.engine, [lay], h0, *flat, *adj)
         return out.reshape(b, v, D)                                                              # dense:116
 
     def gated_regression(self, last_h, regression_gate, regression_transform):   # dense:119-129

@@ -34,6 +34,7 @@
 #include "ggnn_gcn.cuh"
 #include "ggnn_dataset.cuh"
 #include "ggnn_msgw.cuh"
+#include "ggnn_dense_adj.cuh"
 #include "ggnn_tc_smem.h"
 
 using namespace ggnn;
@@ -183,6 +184,12 @@ struct BatchPlan {
                                 // zero in the image until ggnn_set_message_weights writes them on the device; the image carries the
                                 // source-keyed CSR's slot map (tslot) with save_for_backward
     size_t off_slotw = 0, off_tslotw = 0;   // weighted: per-slot adjacency weights in target-CSR order / source-CSR order (with the transpose)
+    // ggnn_prepare_graph_dense_device (also msg_weighted): the [b, T, v, v] adjacency is set on the device (ggnn_set_message_weights), its row
+    // sums become the in-degree section.  The image lists no messages (its CSR sections are empty) and M counts the matrix's b*T*v*v
+    // entries; on the streaming plan every (row, type) pair is virtual row row*T + type, written by the dense aggregation kernel
+    // (ggnn_dense_adj.cuh) before every gather launch
+    bool dense_device = false;
+    int dense_b = 0, dense_v = 0;
     // (offset, bytes) of the image's bytes no section builder writes: alignment gaps and the one-element room of empty sections.  The host
     // builder zeroes them (the device dataset zeroes its whole image), so that an image is one function of its batch, whatever the
     // staging memory held before
@@ -218,6 +225,7 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     ggnn_gcn_layer_weights gcn_w[MAX_LAYERS] = {};
     bool graph_set = false;
     bool msg_weights_set = false;   // a message-weighted batch: ggnn_set_message_weights ran since its upload
+    DevBuf dense_adj;               // a dense-device batch: the engine's copy of its [b, T, v, v] adjacency (ggnn_set_message_weights)
 
     // device memory
     DevBuf graph_buf;   // the graph image of the current batch
@@ -760,6 +768,25 @@ static void gemm_nt(ggnn_engine* e, cudaStream_t st, bool acc, const float* A, i
     ++e->last_launches;
 }
 
+// The dense-device kernels (ggnn_dense_adj.cuh) over the current batch's b graphs of v rows: X = A.x (trans: A^T.x) from the row-major
+// [V][D] `x` into `out` [V][T*D] fp32 or, with `img`, from the chunk-major `x` into the streaming plan's virtual-row image; and dA += the
+// step's adjacency gradient.  Grid-stride blocks over the (graph, type, tile) list, at most 2^20 of them.  The callers count the launches.
+static void dense_apply_launch(ggnn_engine* e, cudaStream_t st, bool trans, const float* A, const float* x, float* out, uint8_t* img) {
+    using namespace ggnn::dadj;
+    const int64_t rt = (e->dense_v + BI - 1) / BI, ct = ((img ? e->DP : e->D) + BK - 1) / BK;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)e->dense_b * e->T * rt * ct, 1 << 20));
+    const int b = e->dense_b, v = e->dense_v, T = e->T, D = e->D, DP = e->DP;
+    if (img) dense_apply_kernel<false, true, true><<<grid, THREADS, 0, st>>>(A, x, nullptr, img, b, v, T, D, DP);
+    else if (trans) dense_apply_kernel<true, false, false><<<grid, THREADS, 0, st>>>(A, x, out, nullptr, b, v, T, D, DP);
+    else dense_apply_kernel<false, false, false><<<grid, THREADS, 0, st>>>(A, x, out, nullptr, b, v, T, D, DP);
+}
+static void dense_adj_launch(ggnn_engine* e, cudaStream_t st, const float* P, const float* h, const float* dx, const float* bias, float* dA) {
+    using namespace ggnn::dadj;
+    const int64_t rt = (e->dense_v + BI - 1) / BI;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)e->dense_b * e->T * rt * rt, 1 << 20));
+    dense_adj_grad_kernel<<<grid, THREADS, 0, st>>>(P, h, dx, bias, dA, e->dense_b, e->dense_v, e->T, e->D);
+}
+
 // The gradient fields of layer l the model has, with their sizes in floats, in ggnn_layer_grads order (a field the model lacks: size 0).
 static std::array<size_t, 8> layer_grad_floats(const ggnn_engine* e, int l) {
     const size_t D = e->D, T = e->T, rows = D * (2 + e->nres[l]);   // [res.. | x | h] rows of the cell kernels
@@ -773,11 +800,14 @@ static float** grad_field(ggnn_layer_grads& g, int i) {
     return f[i];
 }
 
-// d_dw (DEVICE [M] or null): the message weights' gradient, accumulated into (message-weighted batches only).
+// d_dw (DEVICE [M] or null): the message weights' gradient, accumulated into (message-weighted batches only); on a dense-device batch the
+// adjacency's gradient [b, T, v, v] (d_dA below), added into step by step.
 static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_layer_grads* grads, int32_t num_layers,
                               float* d_h0, float* d_dw, ggnn_stream_t stream) {
     using namespace ggnn::bwd;
     if (int rc = begin_backward(e, "ggnn_backward", "ggnn_set_graph_sparse", d_h_out, grads, num_layers, d_h0)) return rc;
+    float* const d_dA = e->dense_device ? d_dw : nullptr;
+    if (e->dense_device) d_dw = nullptr;
     cudaStream_t st = (cudaStream_t)stream;
     const int V = e->V, D = e->D, T = e->T, L = e->L;
     if (V == 0) return GGNN_OK;
@@ -791,7 +821,7 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
     const size_t o_dstate = take(vd * (L + 1)), o_dha = take(vd), o_dhb = take(vd), o_dpc = take(vd), o_dpg = take(2 * vd);
     const size_t o_dxc = take((size_t)V * ldx_max), o_dxg = take((size_t)V * ldx_max), o_rh = take(vd), o_dxp = take(vd), o_at = take(vd * T), o_gt = take(vd * T);
     // P = dx' . W^T: attention's softmax backward and the message weights' gradient (dw_slot: its per-slot sums over the steps)
-    const size_t o_pall = take(e->use_att || d_dw ? vd * T : 0), o_dsa = take(e->use_att ? (size_t)std::max<int64_t>(e->M, 1) : 0);
+    const size_t o_pall = take(e->use_att || d_dw || d_dA ? vd * T : 0), o_dsa = take(e->use_att ? (size_t)std::max<int64_t>(e->M, 1) : 0);
     const size_t o_dws = take(d_dw ? (size_t)std::max<int64_t>(e->M, 1) : 0);
     // deterministic mode: room for the partials of every weight-gradient launch below (the need is not monotone in the segment count --
     // fewer segments get more splits -- so every launched shape is sized), and the attention's per-block d a_t
@@ -927,7 +957,17 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
             // ---- messages: all edge types at once.  At[v, t*D..] = sum of h over the type-t sources of v, Gt[s, t*D..] = sum of dx' over
             // the type-t targets of s.  A weighted batch weights both by the adjacency entry of the slot.
             GatherJob j0{gd.row_ptr, gd.src, h, At, nullptr, nullptr}, j1{gd.trow, gd.ttgt, dxp, Gt, nullptr, nullptr};
-            if (e->use_att) {   // softmax backward first (it adds to dh_new), then the gathers are weighted by the probabilities
+            if (e->dense_device) {   // the matrix products of the dense kernels instead of the gathers, and dA += <P_t[i], h[j]> + <dx'[i], b_t>
+                const float* A = (const float*)e->dense_adj.ptr;
+                if (d_dA) {
+                    gemm_nt(false, dxp, D, 0, w.edge_weights, D, 0, 1, Pall, TD, V, TD, D);   // P[v, t*D+k] = <dx'[v], W_t[k, :]>
+                    dense_adj_launch(e, st, Pall, h, dxp, e->use_bias ? w.edge_biases : nullptr, d_dA);
+                    ++e->last_launches;
+                }
+                dense_apply_launch(e, st, false, A, h, At, nullptr);
+                dense_apply_launch(e, st, true, A, dxp, Gt, nullptr);
+                e->last_launches += 2;
+            } else if (e->use_att) {   // softmax backward first (it adds to dh_new), then the gathers are weighted by the probabilities
                 const float* alpha = (const float*)e->att_buf.ptr + (size_t)(e->step_base[l] + s) * (size_t)std::max<int64_t>(e->M, 1);
                 gemm_nt(false, dxp, D, 0, w.edge_weights, D, 0, 1, Pall, TD, V, TD, D);   // P[v, t*D+k] = <dx'[v], W_t[k, :]>
                 // the target kernel holds 8 columns of d h[v] per lane up to hidden 256, 16 above
@@ -953,8 +993,10 @@ static int ggnn_backward_impl(ggnn_engine* e, const float* d_h_out, const ggnn_l
                     ++e->last_launches;
                 }
             }
-            csr_gather_all_kernel<<<dim3(nodes_blocks, 2), 256, 0, st>>>(j0, j1, V, D, T);
-            ++e->last_launches;
+            if (!e->dense_device) {
+                csr_gather_all_kernel<<<dim3(nodes_blocks, 2), 256, 0, st>>>(j0, j1, V, D, T);
+                ++e->last_launches;
+            }
             if (e->use_bias && gw.edge_biases) {   // dB[t,:] += sum_v indeg[v,t] dx'[v,:]  =  indeg^T . dx'
                 SegList sl;
                 memset(&sl, 0, sizeof sl);
@@ -1112,7 +1154,7 @@ int ggnn_destroy(ggnn_engine* e) {
     cudaSetDevice(e->device);
     e->graph_buf.release(); e->ds_table.release(); e->state_buf.release(); e->save_bufs.release(); e->io_buf.release(); e->bwd_buf.release();
     e->tc_tiles.buf.release(); e->tc_respre.release(); e->ts_tiles.buf.release(); e->ts_images.release(); e->ts_virt.release(); e->err_flag.release();
-    e->step_wt.buf.release(); e->step_buf.release();
+    e->step_wt.buf.release(); e->step_buf.release(); e->dense_adj.release();
     if (e->own_prep) { ggnn_free_prepared_graph(e->own_prep); e->own_prep = nullptr; }
     e->ro_buf.release(); e->ro_stage.release(); e->att_buf.release(); e->ro_ws.release(); e->ro_kval.release();
     delete e;
@@ -1827,7 +1869,7 @@ int ggnn_prepared_graph_arrays(const ggnn_prepared_graph* g, int32_t* row_ptr, i
     if (!g || !g->valid) return GGNN_ESTATE;
     const BatchPlan& q = g->plan;
     const ImageView img = image_view(q, g->shape.use_att, g->image.ptr);
-    const size_t V = (size_t)q.V, T = (size_t)g->shape.T, M = (size_t)q.M;
+    const size_t V = (size_t)q.V, T = (size_t)g->shape.T, M = q.dense_device ? 0 : (size_t)q.M;   // (a dense-device image lists none)
     if (row_ptr) memcpy(row_ptr, img.row_ptr, sizeof(int) * (V * T + 1));
     if (src && M) memcpy(src, img.src, sizeof(int) * M);
     if (msg && M) memcpy(msg, img.msg, sizeof(int) * M);
@@ -1843,6 +1885,15 @@ int ggnn_prepared_graph_stream_tables(const ggnn_prepared_graph* g, int32_t* num
     const BatchPlan& q = g->plan;
     const ImageView img = image_view(q, g->shape.use_att, g->image.ptr);
     if (vslot && !img.vslot) return GGNN_ESTATE;
+    if (q.dense_device) {   // V*T virtual rows, whose image rows the dense aggregation kernel writes: no row lists a source
+        const size_t nv = (size_t)q.ts_nv;
+        if (num_virtual_rows) *num_virtual_rows = (int32_t)nv;
+        if (num_virtual_messages) *num_virtual_messages = 0;
+        if (vrow_ptr) memset(vrow_ptr, 0, sizeof(int) * (nv + 1));
+        if (vinfo && nv) memset(vinfo, 0, sizeof(int) * 8 * nv);
+        if (tile_vptr) memcpy(tile_vptr, img.tvp, sizeof(int) * (size_t)(q.ntiles + 1));
+        return GGNN_OK;
+    }
     const size_t nv = (size_t)q.ts_nv, nvm = (size_t)img.vptr[nv];
     if (num_virtual_rows) *num_virtual_rows = (int32_t)nv;
     if (num_virtual_messages) *num_virtual_messages = (int64_t)nvm;
@@ -2079,6 +2130,84 @@ int ggnn_prepare_graph_dense_weighted(const ggnn_engine* e, int32_t save_for_bac
     return build_dense_image(*inout, b, v, adjm, DENSE_WEIGHTED_STREAM);
 }
 
+}  // extern "C"
+
+// Host half of ggnn_prepare_graph_dense_device: the plan and the image of b graphs of v rows, from (b, v) and the model shape alone.  The
+// tensor-core precisions take the streaming plan at every hidden size (fixed 128-row tiles, every tile's mask has all T types, every
+// (row, type) pair is virtual row row*T + type, no tile lists virtual-row sources); fp32 takes the per-timestep path at every hidden size.
+// The image's CSR sections are empty and its in-degree section zero until ggnn_set_message_weights writes the row sums.  One thread: the
+// work is a few integers per row.
+static int build_dense_device_image(ggnn_prepared_graph* g, int32_t b, int32_t v) {
+    const ModelShape& shape = g->shape;
+    BatchPlan& p = g->plan;
+    g->valid = false;
+    if (b < 0 || v <= 0) return g->fail(GGNN_EINVAL, "null/negative argument");
+    if (shape.use_att) return g->fail(GGNN_EUNSUPPORTED, "propagation attention exists only in the sparse model (sparse:170-196)");
+    if (shape.cudnn_tc) return g->fail(GGNN_EUNSUPPORTED, "CudnnCompatibleGRUCell exists only in the sparse model (sparse:105-108)");
+    if (shape.use_avg)
+        return g->fail(GGNN_EUNSUPPORTED, "use_edge_msg_avg_aggregation with a device adjacency is not supported (its denominator would depend on A)");
+    const int T = shape.T;
+    const int64_t V64 = (int64_t)b * v;
+    if (V64 * T + 1 > 0x7fffffff) return g->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
+    const int V = (int)V64;
+    p = BatchPlan();
+    p.V = V;
+    p.msg_weighted = p.dense_device = true;
+    p.dense_b = b; p.dense_v = v;
+    std::vector<int> tile_start;
+    fixed_tiles(V, ts::TILE_M, tile_start);
+    p.ntiles = (int)tile_start.size() - 1;
+    char buf[320];
+    if (shape.precision != GGNN_PREC_FP32) {
+        p.stream = true; p.variant = 3;
+        for (int i = 0; i < 2; ++i) { p.ts_nblk[i] = ((i + 1) * shape.DP + ts::MMA_N - 1) / ts::MMA_N; p.ts_nc[i] = ts::MMA_N; }
+        snprintf(buf, sizeof buf, "wgmma-%s STREAM(4 launches per step: dense aggregation, gather-GEMM, gate GEMM, candidate GEMM) tiles=%d DP=%d "
+                 "N-blocks agg/cand=%dx%d gate=%dx%d [dense adjacency on the device]", shape.precision == GGNN_PREC_BF16X3 ? "bf16x3" : "bf16",
+                 p.ntiles, shape.DP, p.ts_nblk[0], p.ts_nc[0], p.ts_nblk[1], p.ts_nc[1]);
+    } else {
+        p.stepwise = true;
+        snprintf(buf, sizeof buf, "fp32-stepwise%s (%d launches per step) V=%d D=%d T=%d [dense adjacency on the device]",
+                 shape.cell == CELL_CUDNN_GRU ? "+cudnn-gru" : "", stepwise_launches(shape), V, shape.D, T);
+    }
+    p.plan_text = buf;
+    const size_t off = layout_image(shape, p, g->save, 0, 0, 0);
+    p.M = V64 * T * v;
+    if (p.stream) p.ts_nv = V * T;
+    CU_TRY(g, g->image.begin(off));
+    g->bytes = off;
+    const ImageView img = image_view(p, shape.use_att, g->image.ptr);
+    for (const auto& pad : p.pads) memset(g->image.ptr + pad.first, 0, pad.second);
+    const size_t VT = (size_t)V * T;
+    memset(img.row_ptr, 0, sizeof(int) * (VT + 1));
+    memset(img.indeg, 0, sizeof(float) * VT);
+    fill_denominators(0, V, T, img.indeg, img.denom);
+    const unsigned all_types = T == 32 ? 0xffffffffu : (1u << T) - 1u;
+    for (int i = 0; i <= p.ntiles; ++i) img.tile_start[i] = tile_start[i];
+    for (int i = 0; i < p.ntiles; ++i) img.tile_mask[i] = all_types;
+    if (img.trow) memset(img.trow, 0, sizeof(int) * (VT + 1));
+    if (img.pair) {
+        const size_t rows = (size_t)std::max(p.ntiles, 1) * ts::TILE_M * T;
+        for (size_t r = 0; r < rows; ++r) img.pair[r] = r < VT ? -(2 + (int)r) : -1;
+        img.vptr[0] = 0;
+        for (int i = 0; i <= p.ntiles; ++i) img.tvp[i] = 0;
+    }
+    g->valid = true;
+    return GGNN_OK;
+}
+
+extern "C" {
+
+int ggnn_prepare_graph_dense_device(const ggnn_engine* e, int32_t save_for_backward, int32_t b, int32_t v, ggnn_prepared_graph** inout) {
+    if (int rc = begin_prepare<ggnn_config>(inout, e, nullptr, 0, save_for_backward, __func__)) return rc;
+    return build_dense_device_image(*inout, b, v);
+}
+
+int ggnn_host_prepare_graph_dense_device(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t b, int32_t v,
+                                         ggnn_prepared_graph** inout) {
+    if (int rc = begin_prepare(inout, nullptr, cfg, num_sms, save_for_backward, __func__)) return rc;
+    return build_dense_device_image(*inout, b, v);
+}
+
 int ggnn_set_graph_dense(ggnn_engine* e, int32_t b, int32_t v, const float* adjm, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
     GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
@@ -2196,8 +2325,12 @@ static int forward_stepwise(ggnn_engine* e, const float* h0, float* h_out, cudaS
             step::attention_kernel<<<nodes_blocks, 256, 0, st>>>(gd.row_ptr, gd.src, h, w.edge_type_attention_weights, att, V, D, T);
             msg_w = att;
         }
-        const GatherJob gj{gd.row_ptr, gd.src, h, At, msg_w, nullptr};
-        csr_gather_all_kernel<<<dim3(nodes_blocks, 1), 256, 0, st>>>(gj, gj, V, D, T);
+        if (e->dense_device) {   // X = [A_0 h | .. | A_{T-1} h] where the gather would write it
+            dense_apply_launch(e, st, false, (const float*)e->dense_adj.ptr, h, At, nullptr);
+        } else {
+            const GatherJob gj{gd.row_ptr, gd.src, h, At, msg_w, nullptr};
+            csr_gather_all_kernel<<<dim3(nodes_blocks, 1), 256, 0, st>>>(gj, gj, V, D, T);
+        }
         gemm(At, T * D, D, wt + e->step_wt.off_edge[l], D, D * D, T, X + (size_t)R * D, ldx, D, D);
         step::agg_epilogue_kernel<<<eb, 256, 0, st>>>(X, ldx, R * D, (R + 1) * D, h, e->use_bias ? w.edge_biases : nullptr, gd.indeg,
                                                       e->use_avg ? gd.denom : nullptr, sv.agg, sv.h_in, n, D, T);
@@ -2484,6 +2617,10 @@ static int forward_stream(ggnn_engine* e, const float* h0, float* h_out, cudaStr
                                                                         DP, T);
                 ++e->last_launches;
                 p.slot_w = att;
+            }
+            if (e->dense_device) {   // every (row, type) pair's A_t . h row, into its virtual row
+                dense_apply_launch(e, st, false, (const float*)e->dense_adj.ptr, chk_in, nullptr, (uint8_t*)e->ts_virt.ptr);
+                ++e->last_launches;
             }
             p.epi = ts::EPI_AGG; p.NC = nc0; p.nstages = ns_edge;
             p.g_img = img_in; p.w = wb + wt.off_edge[l]; p.kt_all = T * NKS;
@@ -3263,7 +3400,17 @@ int ggnn_set_message_weights(ggnn_engine* e, const float* message_weights, ggnn_
     CU_TRY(e, cudaSetDevice(e->device));
     e->msg_weights_set = false;
     e->saved_valid = false;   // the backward's gathers read the slot weights: they must be the saved forward's
-    if (e->M > 0) {
+    if (e->dense_device) {   // the engine's own copy of the [b, T, v, v] matrix, and its row sums as the in-degree table
+        if (e->M > 0) {
+            const size_t bytes = sizeof(float) * (size_t)e->M;
+            CU_TRY(e, e->dense_adj.reserve(bytes));
+            CU_TRY(e, cudaMemcpyAsync(e->dense_adj.ptr, message_weights, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+            const int64_t rows = (int64_t)e->dense_b * e->T * e->dense_v;
+            dadj::dense_row_sums_kernel<<<(int)std::min<int64_t>((rows + 255) / 256, 4096), 256, 0, (cudaStream_t)stream>>>(
+                (const float*)e->dense_adj.ptr, e->gd.indeg, e->dense_b, e->dense_v, e->T);
+            CU_TRY(e, cudaGetLastError());
+        }
+    } else if (e->M > 0) {
         const ImageView& gd = e->gd;
         msgw::scatter_message_weights_kernel<<<(int)std::min<int64_t>((e->M + 255) / 256, 4096), 256, 0, (cudaStream_t)stream>>>(
             message_weights, gd.msg, gd.tslot, gd.slotw, gd.tslotw, e->M);
@@ -3285,8 +3432,9 @@ int ggnn_get_csr(ggnn_engine* e, int32_t* row_ptr, int32_t* src, int32_t* msg) {
     CU_TRY(e, cudaSetDevice(e->device));
     CU_TRY(e, cudaDeviceSynchronize());
     if (row_ptr) CU_TRY(e, cudaMemcpy(row_ptr, e->gd.row_ptr, sizeof(int) * ((size_t)e->V * e->T + 1), cudaMemcpyDeviceToHost));
-    if (src && e->M) CU_TRY(e, cudaMemcpy(src, e->gd.src, sizeof(int) * (size_t)e->M, cudaMemcpyDeviceToHost));
-    if (msg && e->M) CU_TRY(e, cudaMemcpy(msg, e->gd.msg, sizeof(int) * (size_t)e->M, cudaMemcpyDeviceToHost));
+    const size_t M = e->dense_device ? 0 : (size_t)e->M;   // (a dense-device image lists no messages)
+    if (src && M) CU_TRY(e, cudaMemcpy(src, e->gd.src, sizeof(int) * M, cudaMemcpyDeviceToHost));
+    if (msg && M) CU_TRY(e, cudaMemcpy(msg, e->gd.msg, sizeof(int) * M, cudaMemcpyDeviceToHost));
     return GGNN_OK;
 }
 

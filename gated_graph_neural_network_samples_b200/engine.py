@@ -156,6 +156,17 @@ class PreparedGraph:
                        int(bool(save_for_backward)), a.shape[0], a.shape[2], a.ctypes.data)
 
     @classmethod
+    def host_only_dense_device(cls, params: dict, num_edge_types: int, num_graphs: int, num_vertices: int, precision: str = "fp32",
+                               num_sms: int = 132, save_for_backward: bool = False, reuse: Optional["PreparedGraph"] = None,
+                               cudnn_gru_tensor_cores: bool = False) -> "PreparedGraph":
+        """``ggnn_host_prepare_graph_dense_device``: a dense batch whose adjacency comes later on the device (see
+        ``PropagationEngine.prepare_graph_dense_device``), from its shape alone, no engine, no GPU."""
+        g = reuse if reuse is not None else cls()
+        cfg, keep = make_config(params, num_edge_types, 0, precision, False, cudnn_gru_tensor_cores)
+        return g._fill(g.lib.ggnn_host_prepare_graph_dense_device, int(num_graphs) * int(num_vertices), int(num_edge_types), C.byref(cfg),
+                       int(num_sms), int(bool(save_for_backward)), int(num_graphs), int(num_vertices))
+
+    @classmethod
     def host_only_weighted(cls, params: dict, num_edge_types: int, adjacency_lists, num_incoming_edges_per_type, precision: str = "fp32",
                            num_sms: int = 132, save_for_backward: bool = False, reuse: Optional["PreparedGraph"] = None,
                            cudnn_gru_tensor_cores: bool = False) -> "PreparedGraph":
@@ -572,10 +583,21 @@ class PropagationEngine:
         return g._fill(self.lib.ggnn_prepare_graph_sparse_weighted, indeg.shape[0], self.T, self._h,
                        -1 if save_for_backward is None else int(bool(save_for_backward)), indeg.shape[0], ptrs, counts, indeg.ctypes.data)
 
+    def prepare_graph_dense_device(self, num_graphs: int, num_vertices: int, save_for_backward: Optional[bool] = None,
+                                   reuse: Optional["PreparedGraph"] = None) -> "PreparedGraph":
+        """The batch of ``num_graphs`` dense graphs of ``num_vertices`` rows whose ``[b, T, v, v]`` adjacency lives on the device
+        (``ggnn_prepare_graph_dense_device``): after ``set_graph_prepared``, ``set_message_weights(A)`` sets the matrix (any finite values)
+        and ``backward(..., d_message_weights=dA)`` returns its gradient at every entry.  The plan depends on (b, v) only, so a new matrix on
+        the same batch needs no new prepare.  Refused with propagation attention, mean aggregation and ``cudnn_gru_tensor_cores``."""
+        g = reuse if reuse is not None else PreparedGraph(self.lib)
+        return g._fill(self.lib.ggnn_prepare_graph_dense_device, int(num_graphs) * int(num_vertices), self.T, self._h,
+                       -1 if save_for_backward is None else int(bool(save_for_backward)), int(num_graphs), int(num_vertices))
+
     def set_message_weights(self, w):
         """``ggnn_set_message_weights``: ``w`` a contiguous fp32 CUDA tensor of ``num_messages()`` entries, message m of type t at position
         ``sum_{t' < t} E_t' + i`` (the reference's type-major order, ``oracle.ggnn_oracle.message_arrays``), for the current
-        message-weighted batch.  The engine copies them on its stream; ``w`` may be reused once the stream passed the call."""
+        message-weighted batch; on a batch of ``prepare_graph_dense_device``, the ``[b, T, v, v]`` adjacency itself.  The engine copies
+        them on its stream; ``w`` may be reused once the stream passed the call."""
         import torch
         if not (isinstance(w, torch.Tensor) and w.is_cuda and w.dtype == torch.float32 and w.is_contiguous()):
             raise GgnnError("message weights must be a contiguous fp32 CUDA tensor")
@@ -834,7 +856,7 @@ class PropagationEngine:
 
     def backward(self, d_out, grads: Sequence[dict], d_h0=None, d_message_weights=None):
         """``ggnn_backward``; with ``d_message_weights`` (fp32 CUDA [num_messages()], accumulated into; message-weighted batches only)
-        ``ggnn_backward_weighted``, which also forms the message weights' gradient."""
+        ``ggnn_backward_weighted``, which also forms the message weights' gradient (on a dense-device batch: dA, ``[b, T, v, v]``)."""
         arr = (_lib.GgnnLayerGrads * len(grads))()
         for l, g in enumerate(grads):
             for f in WEIGHT_FIELDS:

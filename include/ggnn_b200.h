@@ -205,6 +205,30 @@ int ggnn_host_prepare_graph_sparse_weighted(const ggnn_config* cfg, int32_t num_
                                             const int32_t* const* adjacency_lists, const int32_t* num_edges,
                                             const float* num_incoming_edges_per_type, ggnn_prepared_graph** inout);
 int ggnn_set_message_weights(ggnn_engine* e, const float* message_weights, ggnn_stream_t stream);
+/* ---- Dense adjacency on the device (dense GGNN model): the [b, T, v, v] matrix A of the reference's dense model (dense:78-80, 110-112) as a
+ * DEVICE fp32 buffer, A[g, t, i, j] the weight of the type-t message from node j to node i of graph g, the batch's rows g*v + i.  Any finite
+ * values (negative, zero, or a full matrix).  Per timestep with input state h (no averaging):
+ *     X_t[g*v+i] = sum_j A[g,t,i,j] h[g*v+j]    (j ascending, fmaf from +0)
+ *     agg        = sum_t X_t W_t + sum_t rowsum(A[g,t,i,:]) b_t       (fp32 row sums in column order, on the device)
+ * and the gradient at every entry, zeros included:  dA[g,t,i,j] += <P_t[g*v+i], h[g*v+j]> + <dx'[g*v+i], b_t>,  P = dx' . W_t^T.
+ *   ggnn_prepare_graph_dense_device      the plan and image of b graphs of v rows from (b, v) alone: no matrix is read.  ggnn_num_messages
+ *                                        of the batch is b*T*v*v and its plan text ends in " [dense adjacency on the device]".
+ *                                        GGNN_PREC_BF16X3 / GGNN_PREC_BF16 run the streaming plan at every hidden size (a dense aggregation
+ *                                        launch before every gather-GEMM), GGNN_PREC_FP32 the per-timestep fp32 path at every hidden size.
+ *                                        Refused with GGNN_EUNSUPPORTED: propagation attention, use_edge_msg_avg_aggregation (its denominator
+ *                                        would depend on A), GGNN_CELL_CUDNN_GRU_TENSOR_CORES.  Adopt it with ggnn_set_graph_prepared; the
+ *                                        host-only twin needs no engine or GPU.
+ *   ggnn_set_message_weights             on such a batch: message_weights = A [b, T, v, v], copied into an engine buffer on `stream` (the
+ *                                        caller's buffer is free once the stream passed the call), its row sums computed in the same call.
+ *                                        The rules above hold: every upload forgets A, a forward without it is GGNN_ESTATE, setting it drops
+ *                                        the saved activations.  A new A on the same batch needs no new prepare.
+ *   ggnn_backward_weighted               d_message_weights = dA [b, T, v, v], accumulated into; every entry has one writer per timestep and
+ *                                        the timesteps are added in the backward's fixed order, so dA repeats bit for bit in both
+ *                                        deterministic modes. */
+int ggnn_prepare_graph_dense_device(const ggnn_engine* e, int32_t save_for_backward, int32_t num_graphs, int32_t num_vertices,
+                                    ggnn_prepared_graph** inout);
+int ggnn_host_prepare_graph_dense_device(const ggnn_config* cfg, int32_t num_sms, int32_t save_for_backward, int32_t num_graphs,
+                                         int32_t num_vertices, ggnn_prepared_graph** inout);
 /* Introspection of a prepared graph: sizes and plan text; copies of its CSR (row_ptr [V*T+1], src [M], msg [M]), tile starts
  * [num_tiles+1], per-node mean-aggregation denominators [V] and, for a streaming plan, the (target, type) -> source table
  * [ceil(V/128)*128*T] (NULL pointers are skipped; pair_src of a non-streaming plan is left untouched and *is_streaming = 0). */
