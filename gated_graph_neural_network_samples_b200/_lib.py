@@ -108,6 +108,7 @@ SYMBOLS = {
     "ggnn_host_prepare_graph_sparse_weighted": (C.c_int, [C.POINTER(GgnnConfig), C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p), c_i32p,
                                                           C.c_void_p, C.POINTER(C.c_void_p)]),
     "ggnn_set_message_weights": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ggnn_set_graph_sparse_device": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), c_i32p, C.c_void_p, C.c_int32, C.c_void_p]),
     "ggnn_num_messages": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),
     "ggnn_get_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ggnn_layer_state": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]),

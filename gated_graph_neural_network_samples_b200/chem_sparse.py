@@ -66,7 +66,8 @@ def _propagation_function():
 
 def propagate(engine: PropagationEngine, h0, layers: Sequence[dict], message_weights=None):
     """The sparse GGNN propagation as a differentiable torch function, without a ChemModel: ``engine`` holds the current batch (for
-    ``message_weights``, a message-weighted one: ``prepare_graph_sparse_weighted`` + ``set_graph_prepared``), ``h0`` [V, D] and
+    ``message_weights``, a message-weighted one: ``prepare_graph_sparse_weighted`` + ``set_graph_prepared``, or, with the lists on the GPU,
+    ``set_graph_sparse_device(..., message_weighted=True)``), ``h0`` [V, D] and
     ``layers[l]`` dicts of fp32 CUDA tensors keyed like ``ggnn_layer_weights`` (``engine.WEIGHT_FIELDS``) and ``message_weights`` an fp32
     CUDA tensor [num_messages()] in the reference's type-major message order.  Returns the final node states [V, D]; gradients reach
     ``h0``, every layer tensor and ``message_weights``.  The in-degree table of the batch scales the edge bias and the mean unweighted."""
@@ -204,7 +205,16 @@ class SparseGGNNChemModel(ChemModel):
             # is left
             if not self._adopt_prepared_graph(feed):
                 adjacency_lists = [feed[k] for k in self.placeholders['adjacency_lists']]
-                self.engine.set_graph_sparse(adjacency_lists, feed[self.placeholders['num_incoming_edges_per_type']])
+                indeg = feed[self.placeholders['num_incoming_edges_per_type']]
+                if all(isinstance(a, torch.Tensor) and a.is_cuda for a in adjacency_lists):
+                    # lists already on the GPU (a device data pipeline, graphs built by torch ops): the batch is built there
+                    # (set_graph_sparse_device), with the host builder's plan and image
+                    dev = torch.device('cuda', self.engine.device)
+                    lists = [a.to(dev, torch.int32).reshape(-1, 2).contiguous() for a in adjacency_lists]
+                    indeg = torch.as_tensor(indeg, dtype=torch.float32, device=dev).contiguous()
+                    self.engine.set_graph_sparse_device(indeg.shape[0], lists, indeg)
+                else:
+                    self.engine.set_graph_sparse(adjacency_lists, indeg)
         state_keep = float(feed.get(self.placeholders['graph_state_keep_prob'], 1.0))
         # DropoutWrapper(state_keep_prob), sparse:113-114: done inside the kernels; a fresh mask seed per run, drawn from
         # torch's generator (seeded by params['random_seed'] like tf.set_random_seed, chem_tensorflow.py:85)

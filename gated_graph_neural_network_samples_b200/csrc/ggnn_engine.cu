@@ -35,7 +35,11 @@
 #include "ggnn_dataset.cuh"
 #include "ggnn_msgw.cuh"
 #include "ggnn_dense_adj.cuh"
+#include "ggnn_device_graph.cuh"
 #include "ggnn_tc_smem.h"
+
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 using namespace ggnn;
 
@@ -226,6 +230,7 @@ struct ggnn_engine : ModelShape, BatchPlan, ErrorText {
     bool graph_set = false;
     bool msg_weights_set = false;   // a message-weighted batch: ggnn_set_message_weights ran since its upload
     DevBuf dense_adj;               // a dense-device batch: the engine's copy of its [b, T, v, v] adjacency (ggnn_set_message_weights)
+    DevBuf dg_scratch;              // ggnn_set_graph_sparse_device: counts, sort keys, scans, CUB's temporary storage
 
     // device memory
     DevBuf graph_buf;   // the graph image of the current batch
@@ -1154,7 +1159,7 @@ int ggnn_destroy(ggnn_engine* e) {
     cudaSetDevice(e->device);
     e->graph_buf.release(); e->ds_table.release(); e->state_buf.release(); e->save_bufs.release(); e->io_buf.release(); e->bwd_buf.release();
     e->tc_tiles.buf.release(); e->tc_respre.release(); e->ts_tiles.buf.release(); e->ts_images.release(); e->ts_virt.release(); e->err_flag.release();
-    e->step_wt.buf.release(); e->step_buf.release(); e->dense_adj.release();
+    e->step_wt.buf.release(); e->step_buf.release(); e->dense_adj.release(); e->dg_scratch.release();
     if (e->own_prep) { ggnn_free_prepared_graph(e->own_prep); e->own_prep = nullptr; }
     e->ro_buf.release(); e->ro_stage.release(); e->att_buf.release(); e->ro_ws.release(); e->ro_kval.release();
     delete e;
@@ -1995,6 +2000,183 @@ int ggnn_set_graph_sparse(ggnn_engine* e, int32_t V, const int32_t* const* adj, 
     if (!e) return GGNN_EINVAL;
     GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
     return set_graph_from_own_prep(e, stream, [&](ggnn_prepared_graph** g) { return ggnn_prepare_graph_sparse(e, -1, V, adj, num_edges, indeg, g); });
+}
+
+}  // extern "C"
+
+// ---- ggnn_set_graph_sparse_device: build_sparse_image's passes with the edges on the device (ggnn_device_graph.cuh).  The host keeps the
+// plan (build_plan on the cut points read back), the layout (layout_image) and the section map (image_view); the kernels fill the sections
+// into graph_buf.  Three small reads back, each a stream synchronise: the summary, the cut points (only when the plan needs them and there
+// are some), and the two per-tile maxima at the end.
+
+// An int array of `n` elements carved from the engine's build scratch, 256-byte aligned (CUB's temporary storage is the last carve).
+struct ScratchCarver {
+    size_t off = 0;
+    size_t take(size_t bytes) { const size_t at = off; off = align_up(off + std::max<size_t>(bytes, 4), 256); return at; }
+};
+
+struct MaxOp {
+    __host__ __device__ int operator()(int a, int b) const { return a > b ? a : b; }
+};
+
+static int grid_for(const ggnn_engine* e, int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)e->num_sms * 8, (n + 255) / 256)); }
+
+// Whether `p` is device (or managed) memory of `device`.
+static bool on_device(const void* p, int device) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device;
+}
+
+static int build_sparse_device(ggnn_engine* e, int32_t V, const int32_t* const* adj, const int32_t* num_edges, const float* indeg,
+                               bool msg_weighted, cudaStream_t st) {
+    if (msg_weighted && e->use_att)
+        return e->fail(GGNN_EUNSUPPORTED, "message weights with propagation attention are not supported (the probabilities are the slot weights)");
+    if (V < 0 || !adj || !num_edges) return e->fail(GGNN_EINVAL, "null/negative argument");
+    const int T = e->T;
+    int64_t M = 0;
+    for (int t = 0; t < T; ++t) {
+        if (num_edges[t] < 0 || (num_edges[t] > 0 && !adj[t])) return e->fail(GGNN_EINVAL, "adjacency list %d is null/negative", t);
+        M += num_edges[t];
+    }
+    if (M > 0x7fffffff || (int64_t)V * T + 1 > 0x7fffffff) return e->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
+    CU_TRY(e, cudaSetDevice(e->device));
+    for (int t = 0; t < T; ++t)
+        if (num_edges[t] > 0 && !on_device(adj[t], e->device))
+            return e->fail(GGNN_EINVAL, "adjacency list %d is not device memory of device %d", t, e->device);
+    if (indeg && V > 0 && !on_device(indeg, e->device))
+        return e->fail(GGNN_EINVAL, "num_incoming_edges_per_type is not device memory of device %d", e->device);
+
+    const ModelShape& shape = *e;
+    const int64_t VT = (int64_t)V * T;
+    const bool need_cuts = shape.precision == GGNN_PREC_FP32 ? shape.D <= 256 : shape.DP <= 128;   // as build_sparse_image
+    const bool save = e->save;
+    dg::EdgeLists L{};
+    L.T = T;
+    for (int t = 0; t < T; ++t) { L.adj[t] = adj[t]; L.base[t + 1] = L.base[t] + num_edges[t]; }
+
+    // ---- scratch: row counts, cut-point arrays, per-message keys / ids / endpoints, virtual-row scans, the summary, tile starts, CUB's storage
+    const size_t I = sizeof(int), Mr = (size_t)std::max<int64_t>(M, 1), rows = (size_t)VT + 1, Vr = (size_t)std::max(V, 1);
+    ScratchCarver c;
+    const size_t o_counts = c.take(I * rows), o_tcounts = c.take(I * rows), o_reach = c.take(I * Vr), o_far = c.take(I * Vr),
+                 o_flag = c.take(I * Vr), o_pos = c.take(I * Vr), o_cuts = c.take(I * Vr), o_key = c.take(I * Mr), o_tkey = c.take(I * Mr),
+                 o_ids = c.take(I * Mr), o_es = c.take(I * Mr), o_ed = c.take(I * Mr), o_key_out = c.take(I * Mr), o_tmsg = c.take(I * Mr),
+                 o_slot_of = c.take(I * Mr), o_vid = c.take(I * rows), o_vm = c.take(I * rows), o_summary = c.take(I * dg::S_COUNT),
+                 o_maxima = c.take(I * 2), o_tiles = c.take(I * (Vr + 2)), o_temp = c.off;
+    const int key_bits = VT > 1 ? 32 - __builtin_clz((unsigned)(VT - 1)) : 1;
+    size_t temp = 0, need = 0;
+    CU_TRY(e, cub::DeviceScan::ExclusiveSum(nullptr, need, (int*)nullptr, (int*)nullptr, (int)rows, st));
+    temp = std::max(temp, need);
+    CU_TRY(e, cub::DeviceScan::InclusiveScan(nullptr, need, (int*)nullptr, (int*)nullptr, MaxOp(), (int)Vr, st));
+    temp = std::max(temp, need);
+    CU_TRY(e, cub::DeviceRadixSort::SortPairs(nullptr, need, (const int*)nullptr, (int*)nullptr, (const int*)nullptr, (int*)nullptr, (int)Mr, 0,
+                                              key_bits, st));
+    temp = std::max(temp, need);
+    CU_TRY(e, e->dg_scratch.reserve(o_temp + temp));
+    char* s0 = (char*)e->dg_scratch.ptr;
+    auto at = [&](size_t off) { return (int*)(s0 + off); };
+    int *counts = at(o_counts), *tcounts = save ? at(o_tcounts) : nullptr, *reach = need_cuts ? at(o_reach) : nullptr;
+    unsigned* summary = (unsigned*)at(o_summary);
+    void* tmp = s0 + o_temp;
+
+    // ---- passes 1-2: validate and count, reach, the virtual-row totals, the first bad edge, the cut points
+    CU_TRY(e, cudaMemsetAsync(counts, 0, I * rows, st));
+    if (tcounts) CU_TRY(e, cudaMemsetAsync(tcounts, 0, I * rows, st));
+    if (reach) CU_TRY(e, cudaMemsetAsync(reach, 0, I * Vr, st));
+    CU_TRY(e, cudaMemsetAsync(summary, 0, I * dg::S_COUNT, st));
+    CU_TRY(e, cudaMemsetAsync(summary + dg::S_BAD, 0xff, sizeof(unsigned), st));
+    if (M > 0)
+        dg::count_kernel<<<grid_for(e, M), 256, 0, st>>>(L, V, M, counts, tcounts, reach, at(o_key), save ? at(o_tkey) : nullptr, at(o_ids), at(o_es),
+                                                         at(o_ed), summary);
+    dg::summary_kernel<<<grid_for(e, VT), 256, 0, st>>>(L, counts, VT, summary);
+    if (reach && V > 1) {
+        CU_TRY(e, cub::DeviceScan::InclusiveScan(tmp, temp, reach, at(o_far), MaxOp(), V - 1, st));
+        dg::cut_flags_kernel<<<grid_for(e, V), 256, 0, st>>>(at(o_far), V, at(o_flag));
+        CU_TRY(e, cub::DeviceScan::ExclusiveSum(tmp, temp, at(o_flag), at(o_pos), V, st));
+        dg::cut_list_kernel<<<grid_for(e, V), 256, 0, st>>>(at(o_flag), at(o_pos), V, at(o_cuts), summary);
+    }
+    CU_TRY(e, cudaGetLastError());
+
+    // ---- read 1: the summary
+    unsigned sum[dg::S_COUNT];
+    CU_TRY(e, cudaMemcpyAsync(sum, summary, sizeof sum, cudaMemcpyDeviceToHost, st));
+    CU_TRY(e, cudaStreamSynchronize(st));
+    if (sum[dg::S_BAD] != 0xffffffffu)
+        return e->fail(GGNN_ERANGE, "edge %d of type %d = (%d,%d) is out of range for %d nodes", (int)sum[dg::S_BAD_I], (int)sum[dg::S_BAD_T],
+                       (int)sum[dg::S_BAD_S], (int)sum[dg::S_BAD_D], V);
+    // ---- read 2 (plans that need them): the cut points, then the host plans the tiles and lays out the image
+    std::vector<int> cuts(1, 0);
+    if (reach && sum[dg::S_NCUT] > 0) {
+        cuts.resize(1 + (size_t)sum[dg::S_NCUT]);
+        CU_TRY(e, cudaMemcpyAsync(cuts.data() + 1, at(o_cuts), I * sum[dg::S_NCUT], cudaMemcpyDeviceToHost, st));
+        CU_TRY(e, cudaStreamSynchronize(st));
+    }
+    if (V > 0) cuts.push_back(V);
+    BatchPlan p;
+    std::vector<int> tile_start;
+    if (int rc = build_plan(shape, V, msg_weighted, cuts, p, tile_start, e->err, msg_weighted, msg_weighted)) return rc;
+    if (msg_weighted) p.plan_text += " [message-weighted]";
+    const int ntiles = p.ntiles;
+    const int nv = p.stream ? (int)(p.all_virtual ? sum[dg::S_NV1] : sum[dg::S_NV2]) : 0;
+    const int64_t nvm = p.stream ? (p.all_virtual ? M : (int64_t)sum[dg::S_NVM2]) : 0;
+    const size_t bytes = layout_image(shape, p, save, M, nv, nvm);
+    CU_TRY(e, e->graph_buf.reserve(bytes));
+    const ImageView img = image_view(p, shape.use_att, (char*)e->graph_buf.ptr);
+
+    // ---- pass 5: every section the plan carries (the memset leaves the pads and the zero slot-weight sections)
+    CU_TRY(e, cudaMemsetAsync(e->graph_buf.ptr, 0, bytes, st));
+    CU_TRY(e, cub::DeviceScan::ExclusiveSum(tmp, temp, counts, img.row_ptr, (int)rows, st));
+    int* slot_of = img.tslot ? at(o_slot_of) : nullptr;
+    if (M > 0) {
+        CU_TRY(e, cub::DeviceRadixSort::SortPairs(tmp, temp, at(o_key), at(o_key_out), at(o_ids), img.msg, (int)M, 0, key_bits, st));
+        dg::csr_src_kernel<<<grid_for(e, M), 256, 0, st>>>(img.msg, at(o_es), M, img.src, slot_of);
+    }
+    if (V > 0) {
+        if (indeg) CU_TRY(e, cudaMemcpyAsync(img.indeg, indeg, sizeof(float) * (size_t)VT, cudaMemcpyDeviceToDevice, st));
+        else dg::indeg_kernel<<<grid_for(e, VT), 256, 0, st>>>(counts, VT, img.indeg);
+        dg::denom_kernel<<<grid_for(e, V), 256, 0, st>>>(img.indeg, V, T, img.denom);
+    }
+    int* vid = nullptr;
+    if (p.stream) {
+        vid = at(o_vid);
+        dg::virtual_flags_kernel<<<grid_for(e, (int64_t)rows), 256, 0, st>>>(counts, VT, p.all_virtual, vid, at(o_vm));
+        CU_TRY(e, cub::DeviceScan::ExclusiveSum(tmp, temp, vid, vid, (int)rows, st));
+        CU_TRY(e, cub::DeviceScan::ExclusiveSum(tmp, temp, at(o_vm), at(o_vm), (int)rows, st));
+        const int64_t npairs = (int64_t)std::max(ntiles, 1) * ts::TILE_M * T;
+        dg::stream_rows_kernel<<<grid_for(e, npairs), 256, 0, st>>>(img.row_ptr, img.src, vid, at(o_vm), VT, npairs, p.all_virtual, img.pair, img.vptr,
+                                                                    img.vsrc, img.vinfo, img.vslot);
+    }
+    if (img.trow) {
+        CU_TRY(e, cub::DeviceScan::ExclusiveSum(tmp, temp, tcounts, img.trow, (int)rows, st));
+        if (M > 0) {
+            CU_TRY(e, cub::DeviceRadixSort::SortPairs(tmp, temp, at(o_tkey), at(o_key_out), at(o_ids), at(o_tmsg), (int)M, 0, key_bits, st));
+            dg::source_csr_kernel<<<grid_for(e, M), 256, 0, st>>>(at(o_tmsg), at(o_ed), slot_of, M, img.ttgt, img.tslot);
+        }
+    }
+    // ---- pass 4: tile starts, masks, first virtual rows and the per-tile maxima; read 3: the maxima
+    int* maxima = at(o_maxima);
+    CU_TRY(e, cudaMemsetAsync(maxima, 0, 2 * I, st));
+    CU_TRY(e, cudaMemcpyAsync(at(o_tiles), tile_start.data(), I * tile_start.size(), cudaMemcpyHostToDevice, st));
+    dg::tile_kernel<<<grid_for(e, ntiles + 1), 256, 0, st>>>(at(o_tiles), ntiles, T, img.row_ptr, vid, img.tile_start, img.tile_mask, img.tvp, maxima);
+    CU_TRY(e, cudaGetLastError());
+    int mx[2];
+    CU_TRY(e, cudaMemcpyAsync(mx, maxima, sizeof mx, cudaMemcpyDeviceToHost, st));
+    CU_TRY(e, cudaStreamSynchronize(st));
+    p.max_tile_msgs = mx[0];
+    p.max_tile_types = mx[1];
+    static_cast<BatchPlan&>(*e) = p;
+    e->graph_bytes = bytes;
+    return bind_graph(e);
+}
+
+extern "C" {
+
+int ggnn_set_graph_sparse_device(ggnn_engine* e, int32_t num_nodes, const int32_t* const* adjacency_lists, const int32_t* num_edges,
+                                 const float* num_incoming_edges_per_type, int32_t message_weighted, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
+    forget_batch(e);
+    return build_sparse_device(e, num_nodes, adjacency_lists, num_edges, num_incoming_edges_per_type, message_weighted != 0, (cudaStream_t)stream);
 }
 
 

@@ -555,6 +555,45 @@ class PropagationEngine:
         self.V = V
         self._graph_keepalive = (adjs, indeg)
 
+    def _sparse_device_args(self, num_nodes, adjacency_lists, num_incoming_edges_per_type):
+        """Checks and marshals the feeds of ``set_graph_sparse_device``; raises ``GgnnError`` before any call into the library."""
+        import torch
+        V = int(num_nodes)
+        if V < 0:
+            raise GgnnError("num_nodes must be >= 0, got %d" % V)
+        if len(adjacency_lists) != self.T:
+            raise GgnnError("expected %d adjacency lists, got %d" % (self.T, len(adjacency_lists)))
+        dev = torch.device("cuda", self.device)
+        for t, a in enumerate(adjacency_lists):
+            if not isinstance(a, torch.Tensor) or a.device != dev:
+                raise GgnnError("adjacency list %d must be a torch tensor on cuda:%d" % (t, self.device))
+            if a.dtype != torch.int32 or a.dim() != 2 or a.shape[1] != 2 or not a.is_contiguous():
+                raise GgnnError("adjacency list %d must be a contiguous int32 [E, 2] tensor, got %s %s" % (t, a.dtype, tuple(a.shape)))
+        indeg = num_incoming_edges_per_type
+        if indeg is not None:
+            if not isinstance(indeg, torch.Tensor) or indeg.device != dev:
+                raise GgnnError("num_incoming_edges_per_type must be a torch tensor on cuda:%d or None" % self.device)
+            if indeg.dtype != torch.float32 or tuple(indeg.shape) != (V, self.T) or not indeg.is_contiguous():
+                raise GgnnError("num_incoming_edges_per_type must be a contiguous float32 [%d, %d] tensor, got %s %s"
+                                % (V, self.T, indeg.dtype, tuple(indeg.shape)))
+        ptrs = (C.c_void_p * self.T)(*[a.data_ptr() if a.shape[0] else None for a in adjacency_lists])
+        counts = (C.c_int32 * self.T)(*[a.shape[0] for a in adjacency_lists])
+        return V, ptrs, counts, indeg
+
+    def set_graph_sparse_device(self, num_nodes: int, adjacency_lists, num_incoming_edges_per_type=None, message_weighted: bool = False):
+        """``set_graph_sparse`` with the graph already on the GPU (``ggnn_set_graph_sparse_device``): per type a contiguous int32 CUDA tensor
+        ``[E_t, 2]`` of (source, target) pairs on the engine's device, and optionally the fp32 CUDA ``[V, T]`` in-degree table (None: the
+        per-(target, type) message counts, which is what the reference's packer feeds).  The batch is built on the device, with the host's
+        plan, into the image ``prepare_graph_sparse`` (``message_weighted``: ``prepare_graph_sparse_weighted``, then ``set_message_weights``)
+        would upload, byte for byte.  The call waits for the current stream for three small reads at most; the tensors are kept alive until
+        the next graph upload."""
+        V, ptrs, counts, indeg = self._sparse_device_args(num_nodes, adjacency_lists, num_incoming_edges_per_type)
+        self.serial += 1
+        self._check(self.lib.ggnn_set_graph_sparse_device(self._h, V, ptrs, counts, indeg.data_ptr() if indeg is not None and V else None,
+                                                          int(bool(message_weighted)), self._stream()))
+        self.V = V
+        self._graph_keepalive = (list(adjacency_lists), indeg)
+
     def marshal_sparse(self, adjacency_lists, num_incoming_edges_per_type):
         """The ctypes view of one batch's graph feeds (contiguous int32 / float32 arrays, pointer and count tables), reusable across calls:
         pass it as ``marshalled=`` to keep a producer thread's time under the GIL to a few microseconds per batch."""
@@ -596,7 +635,8 @@ class PropagationEngine:
     def set_message_weights(self, w):
         """``ggnn_set_message_weights``: ``w`` a contiguous fp32 CUDA tensor of ``num_messages()`` entries, message m of type t at position
         ``sum_{t' < t} E_t' + i`` (the reference's type-major order, ``oracle.ggnn_oracle.message_arrays``), for the current
-        message-weighted batch; on a batch of ``prepare_graph_dense_device``, the ``[b, T, v, v]`` adjacency itself.  The engine copies
+        message-weighted batch (``prepare_graph_sparse_weighted`` + ``set_graph_prepared``, or
+        ``set_graph_sparse_device(..., message_weighted=True)``); on a batch of ``prepare_graph_dense_device``, the ``[b, T, v, v]`` adjacency itself.  The engine copies
         them on its stream; ``w`` may be reused once the stream passed the call."""
         import torch
         if not (isinstance(w, torch.Tensor) and w.is_cuda and w.dtype == torch.float32 and w.is_contiguous()):

@@ -205,6 +205,24 @@ int ggnn_host_prepare_graph_sparse_weighted(const ggnn_config* cfg, int32_t num_
                                             const int32_t* const* adjacency_lists, const int32_t* num_edges,
                                             const float* num_incoming_edges_per_type, ggnn_prepared_graph** inout);
 int ggnn_set_message_weights(ggnn_engine* e, const float* message_weights, ggnn_stream_t stream);
+/* ---- Sparse graphs on the device: ggnn_set_graph_sparse with the adjacency lists already in the engine's device memory.
+ *   adjacency_lists[t]           DEVICE pointer to [num_edges[t], 2] int32 (source, target), as in ggnn_set_graph_sparse (the T pointers
+ *                                themselves and num_edges are host arrays)
+ *   num_incoming_edges_per_type  DEVICE [V, T] fp32 used as given, or NULL for the per-(target, type) message counts as fp32 (what the
+ *                                reference's packer feeds, sparse:260,263)
+ *   message_weighted             0: as ggnn_prepare_graph_sparse + ggnn_set_graph_prepared; 1: as ggnn_prepare_graph_sparse_weighted +
+ *                                ggnn_set_graph_prepared (ggnn_set_message_weights must follow before a forward)
+ * The engine is left exactly as those two calls leave it: the same plan and plan text, per-tile maxima, ggnn_num_messages and graph image,
+ * every byte included; the engine's save_for_backward flag decides whether the source-keyed CSR is built.  The validation, counting, CSR
+ * sorts and section fills run as kernels on `stream` into the engine's graph buffer; the host plans the tiles from the cut points and lays
+ * out the image exactly as the host builder does.  No edge is copied to the host.  The call synchronises `stream` two or three times, each
+ * for a small read back: a summary (first bad edge, virtual-row totals, number of cut points), the cut points when the plan needs them and
+ * the batch has any, and the two per-tile maxima.  The image does not depend on the order of any atomic.  Refusals match the host builder:
+ * GGNN_ERANGE names the first out-of-range edge in (type, index) order with its values; GGNN_EINVAL for null / negative arguments and for
+ * lists or a table that are not device memory of the engine's device; GGNN_EUNSUPPORTED for batches beyond int32 indexing and for
+ * message_weighted with propagation attention.  Like every upload, a failed call first forgets the previous batch. */
+int ggnn_set_graph_sparse_device(ggnn_engine* e, int32_t num_nodes, const int32_t* const* adjacency_lists, const int32_t* num_edges,
+                                 const float* num_incoming_edges_per_type, int32_t message_weighted, ggnn_stream_t stream);
 /* ---- Dense adjacency on the device (dense GGNN model): the [b, T, v, v] matrix A of the reference's dense model (dense:78-80, 110-112) as a
  * DEVICE fp32 buffer, A[g, t, i, j] the weight of the type-t message from node j to node i of graph g, the batch's rows g*v + i.  Any finite
  * values (negative, zero, or a full matrix).  Per timestep with input state h (no averaging):
