@@ -132,6 +132,7 @@ SYMBOLS = {
     "ggnn_host_prepare_graph_gcn_message_weighted": (C.c_int, [C.POINTER(GcnConfig), C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_void_p,
                                                                C.POINTER(C.c_void_p)]),
     "ggnn_gcn_backward_weighted": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GcnLayerWeights), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ggnn_set_graph_gcn_device": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
     "ggnn_dataset_create_sparse": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int32,
                                              C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
     "ggnn_host_dataset_create_sparse": (C.c_int, [C.POINTER(GgnnConfig), C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p),

@@ -2,7 +2,8 @@
 propagation replaced by the H100 engine.
 
     prepare_specific_graph_model()        gcn:42-57   -> creates the trainables + the GCN engine handle
-    compute_final_node_representations()  gcn:59-82   -> ggnn_set_graph_gcn (or a prepared graph) + ggnn_forward (C ABI)
+    compute_final_node_representations()  gcn:59-82   -> ggnn_set_graph_gcn (or a prepared graph, or ggnn_set_graph_gcn_device for a
+                                                         CUDA feed) + ggnn_forward (C ABI)
     gated_regression()                    gcn:84-93   -> the sparse GGNN's readout (sparse:220-231 is the same graph)
 """
 from __future__ import annotations
@@ -70,7 +71,8 @@ def _propagation_function():
 
 def propagate(engine: GCNEngine, h0, kernels: Sequence, biases: Optional[Sequence] = None, adjacency_weights=None):
     """The sparse GCN propagation as a differentiable torch function, without a ChemModel: ``engine`` holds the current batch (for
-    ``adjacency_weights``, a message-weighted one: ``prepare_graph_gcn_message_weighted`` + ``set_graph_prepared``), ``h0`` [V, D],
+    ``adjacency_weights``, a message-weighted one: ``prepare_graph_gcn_message_weighted`` + ``set_graph_prepared``, or, with the list on
+    the GPU, the device-built batch of ``set_graph_gcn_device``), ``h0`` [V, D],
     ``kernels[l]`` [D, D] and, when the engine uses biases, ``biases[l]`` [D], fp32 CUDA tensors, and ``adjacency_weights`` an fp32 CUDA
     tensor [nnz] in list order (the weights of ``adjacency_weights`` in ``set_graph_gcn``, computed in torch: a learned or renormalized
     ``D^-1/2 (A+I) D^-1/2``, a DropEdge mask).  Returns the last layer's node states [V, D]; gradients reach ``h0``, every kernel and bias,
@@ -144,18 +146,29 @@ class SparseGCNChemModel(ChemModel):
         # a device-data batch was assembled on the device by forward_batch (_adopt_dataset_batch)
         if not feed.get('_graph_adopted'):
             self.engine.set_save_for_backward(torch.is_grad_enabled())   # before set_graph: the source-keyed CSR is built there
+        adjacency_weights = None   # a device-built batch's weights: the autograd node's trailing input
         if not feed.get('_graph_adopted') and not self._adopt_prepared_graph(feed):
-            self.engine.set_graph_gcn(h0.shape[0], feed[self.placeholders['adjacency_list']], feed[self.placeholders['adjacency_weights']])
+            lst, w = feed[self.placeholders['adjacency_list']], feed[self.placeholders['adjacency_weights']]
+            if isinstance(lst, torch.Tensor) and lst.is_cuda:
+                # a list already on the GPU (a device data pipeline, graphs built by torch ops): the batch is built there
+                # (set_graph_gcn_device, the host builder's plan and image) and its weights are device data, so a requires_grad tensor
+                # gets its gradient and a plain one costs no d w
+                dev = torch.device('cuda', self.engine.device)
+                self.engine.set_graph_gcn_device(h0.shape[0], lst.to(dev, torch.int64).reshape(-1, 2).contiguous())
+                adjacency_weights = (w if isinstance(w, torch.Tensor) else torch.as_tensor(w)).to(dev, torch.float32).contiguous()
+            else:
+                self.engine.set_graph_gcn(h0.shape[0], lst, w)
         # tf.nn.dropout after the ReLU of every layer but the last (gcn:75-78): done inside the kernels; a fresh mask seed per run, drawn
         # from torch's generator (seeded by params['random_seed'] like tf.set_random_seed, chem_tensorflow.py:85)
         keep = float(feed.get(self.placeholders['graph_state_keep_prob'], 1.0))
         self.engine.set_state_dropout(keep, int(torch.randint(0, 2 ** 62, (1,)).item()) if keep < 1.0 else 0)
         weights = list(self.weights['edge_weights']) + list(self.weights.get('edge_biases', []))
+        aw = [adjacency_weights] if adjacency_weights is not None else []
         if DP != D:
             pad = torch.nn.functional.pad
             weights = [pad(w, (0, DP - D) if w.dim() == 1 else (0, DP - D, 0, DP - D)) for w in weights]
-            return self._propagation.apply(self.engine, pad(h0, (0, DP - D)).contiguous(), *weights)[:, :D]
-        return self._propagation.apply(self.engine, h0, *weights)                                          # [V, D]
+            return self._propagation.apply(self.engine, pad(h0, (0, DP - D)).contiguous(), *weights, *aw)[:, :D]
+        return self._propagation.apply(self.engine, h0, *weights, *aw)                                     # [V, D]
 
     # ------------------------------------------------------------------ readout (gcn:84-93 == sparse:220-231)
     gated_regression = SparseGGNNChemModel.gated_regression

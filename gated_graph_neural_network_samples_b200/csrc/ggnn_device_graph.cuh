@@ -1,5 +1,5 @@
-// Sparse batches from DEVICE adjacency lists (ggnn_set_graph_sparse_device): the section fills of build_sparse_image as kernels, writing the
-// same image into the engine's graph buffer.  The plan and the layout stay on the host (build_plan, layout_image, image_view): these
+// Sparse batches from DEVICE adjacency lists (ggnn_set_graph_sparse_device, and ggnn_set_graph_gcn_device after dg_gcn's pass): the section
+// fills of build_sparse_image as kernels, writing the same image into the engine's graph buffer.  The plan and the layout stay on the host (build_plan, layout_image, image_view): these
 // kernels only count, derive the cut points and totals the plan needs, and fill the sections the plan carries.
 //
 // Determinism: atomics only count (per-row message counts, reach maxima, the first bad edge as a minimum, the per-tile maxima), and every
@@ -196,4 +196,23 @@ __global__ void __launch_bounds__(256) tile_kernel(const int* __restrict__ tiles
 }
 
 }  // namespace dg
+
+// The GCN entry's one pass ahead of dg's (ggnn_set_graph_gcn_device): gcn_pairs on the device.  It lives beside dg, which holds the passes
+// both entries share.
+namespace dg_gcn {
+
+// One thread per entry k of the caller's [nnz, 2] int64 list (row i = output, column j = input): checks 0 <= i, j < V in int64 and writes
+// the int32 pair (source j, target i) into `pairs`, the GCN's one edge type in list order.  An out-of-range entry lowers the first-bad
+// minimum and writes (-1, -1), which count_kernel rejects, so nothing of it is counted.
+__global__ void __launch_bounds__(256) gcn_pairs_kernel(const int64_t* __restrict__ list, int64_t nnz, int V, int32_t* __restrict__ pairs,
+                                                        unsigned* __restrict__ summary) {
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nnz; k += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t i = list[2 * k], j = list[2 * k + 1];   // two 8-byte loads: the ABI promises no more than int64 alignment
+        const bool ok = (uint64_t)i < (uint64_t)V && (uint64_t)j < (uint64_t)V;
+        if (!ok) atomicMin(summary + dg::S_BAD, (unsigned)k);
+        reinterpret_cast<int2*>(pairs)[k] = ok ? make_int2((int)j, (int)i) : make_int2(-1, -1);
+    }
+}
+
+}  // namespace dg_gcn
 }  // namespace ggnn

@@ -2004,10 +2004,11 @@ int ggnn_set_graph_sparse(ggnn_engine* e, int32_t V, const int32_t* const* adj, 
 
 }  // extern "C"
 
-// ---- ggnn_set_graph_sparse_device: build_sparse_image's passes with the edges on the device (ggnn_device_graph.cuh).  The host keeps the
-// plan (build_plan on the cut points read back), the layout (layout_image) and the section map (image_view); the kernels fill the sections
-// into graph_buf.  Three small reads back, each a stream synchronise: the summary, the cut points (only when the plan needs them and there
-// are some), and the two per-tile maxima at the end.
+// ---- ggnn_set_graph_sparse_device and ggnn_set_graph_gcn_device: build_sparse_image's passes with the edges on the device
+// (ggnn_device_graph.cuh).  The host keeps the plan (build_plan on the cut points read back), the layout (layout_image) and the section map
+// (image_view); the kernels fill the sections into graph_buf.  Three small reads back, each a stream synchronise: the summary, the cut
+// points (only when the plan needs them and there are some), and the two per-tile maxima at the end (a refused GCN list adds one, for the
+// bad entry's values).
 
 // An int array of `n` elements carved from the engine's build scratch, 256-byte aligned (CUB's temporary storage is the last carve).
 struct ScratchCarver {
@@ -2028,41 +2029,34 @@ static bool on_device(const void* p, int device) {
     return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == device;
 }
 
-static int build_sparse_device(ggnn_engine* e, int32_t V, const int32_t* const* adj, const int32_t* num_edges, const float* indeg,
-                               bool msg_weighted, cudaStream_t st) {
-    if (msg_weighted && e->use_att)
-        return e->fail(GGNN_EUNSUPPORTED, "message weights with propagation attention are not supported (the probabilities are the slot weights)");
-    if (V < 0 || !adj || !num_edges) return e->fail(GGNN_EINVAL, "null/negative argument");
-    const int T = e->T;
-    int64_t M = 0;
-    for (int t = 0; t < T; ++t) {
-        if (num_edges[t] < 0 || (num_edges[t] > 0 && !adj[t])) return e->fail(GGNN_EINVAL, "adjacency list %d is null/negative", t);
-        M += num_edges[t];
-    }
-    if (M > 0x7fffffff || (int64_t)V * T + 1 > 0x7fffffff) return e->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
-    CU_TRY(e, cudaSetDevice(e->device));
-    for (int t = 0; t < T; ++t)
-        if (num_edges[t] > 0 && !on_device(adj[t], e->device))
-            return e->fail(GGNN_EINVAL, "adjacency list %d is not device memory of device %d", t, e->device);
-    if (indeg && V > 0 && !on_device(indeg, e->device))
-        return e->fail(GGNN_EINVAL, "num_incoming_edges_per_type is not device memory of device %d", e->device);
+// The GCN entry's feed: the caller's DEVICE [nnz, 2] int64 list of (row i = output, column j = input), which dg_gcn::gcn_pairs_kernel turns
+// into the one edge type (source j, target i) as gcn_pairs does on the host.
+struct GcnDeviceList {
+    const int64_t* list;
+};
 
+// The build both device entries share, on validated arguments.  `L` holds the edge lists and their type-major bases; for the GCN (`gcn`
+// set) T = 1, L.base[1] = nnz, and the one list is the pairs this build writes into its scratch.  The entries differ where build_gcn_image
+// calls build_sparse_image differently from the GGNN builders: `indeg` (GGNN: the DEVICE table, or NULL for the row counts; GCN: the
+// all-zero table, which the image memset leaves), build_plan's flags `weighted`, `stream_weighted` and `msg_weighted`, and the refusal text
+// of the first bad entry.
+static int build_sparse_device(ggnn_engine* e, int32_t V, dg::EdgeLists L, const float* indeg, const GcnDeviceList* gcn, bool weighted,
+                               bool stream_weighted, bool msg_weighted, cudaStream_t st) {
     const ModelShape& shape = *e;
-    const int64_t VT = (int64_t)V * T;
+    const int T = L.T;
+    const int64_t M = L.base[T], VT = (int64_t)V * T;
     const bool need_cuts = shape.precision == GGNN_PREC_FP32 ? shape.D <= 256 : shape.DP <= 128;   // as build_sparse_image
     const bool save = e->save;
-    dg::EdgeLists L{};
-    L.T = T;
-    for (int t = 0; t < T; ++t) { L.adj[t] = adj[t]; L.base[t + 1] = L.base[t] + num_edges[t]; }
 
-    // ---- scratch: row counts, cut-point arrays, per-message keys / ids / endpoints, virtual-row scans, the summary, tile starts, CUB's storage
+    // ---- scratch: row counts, cut-point arrays, per-message keys / ids / endpoints, virtual-row scans, the summary, tile starts, the GCN's
+    // int32 pairs, CUB's storage
     const size_t I = sizeof(int), Mr = (size_t)std::max<int64_t>(M, 1), rows = (size_t)VT + 1, Vr = (size_t)std::max(V, 1);
     ScratchCarver c;
     const size_t o_counts = c.take(I * rows), o_tcounts = c.take(I * rows), o_reach = c.take(I * Vr), o_far = c.take(I * Vr),
                  o_flag = c.take(I * Vr), o_pos = c.take(I * Vr), o_cuts = c.take(I * Vr), o_key = c.take(I * Mr), o_tkey = c.take(I * Mr),
                  o_ids = c.take(I * Mr), o_es = c.take(I * Mr), o_ed = c.take(I * Mr), o_key_out = c.take(I * Mr), o_tmsg = c.take(I * Mr),
                  o_slot_of = c.take(I * Mr), o_vid = c.take(I * rows), o_vm = c.take(I * rows), o_summary = c.take(I * dg::S_COUNT),
-                 o_maxima = c.take(I * 2), o_tiles = c.take(I * (Vr + 2)), o_temp = c.off;
+                 o_maxima = c.take(I * 2), o_tiles = c.take(I * (Vr + 2)), o_pairs = gcn ? c.take(2 * I * Mr) : 0, o_temp = c.off;
     const int key_bits = VT > 1 ? 32 - __builtin_clz((unsigned)(VT - 1)) : 1;
     size_t temp = 0, need = 0;
     CU_TRY(e, cub::DeviceScan::ExclusiveSum(nullptr, need, (int*)nullptr, (int*)nullptr, (int)rows, st));
@@ -2085,6 +2079,10 @@ static int build_sparse_device(ggnn_engine* e, int32_t V, const int32_t* const* 
     if (reach) CU_TRY(e, cudaMemsetAsync(reach, 0, I * Vr, st));
     CU_TRY(e, cudaMemsetAsync(summary, 0, I * dg::S_COUNT, st));
     CU_TRY(e, cudaMemsetAsync(summary + dg::S_BAD, 0xff, sizeof(unsigned), st));
+    if (gcn && M > 0) {
+        L.adj[0] = (const int32_t*)at(o_pairs);
+        dg_gcn::gcn_pairs_kernel<<<grid_for(e, M), 256, 0, st>>>(gcn->list, M, V, (int32_t*)at(o_pairs), summary);
+    }
     if (M > 0)
         dg::count_kernel<<<grid_for(e, M), 256, 0, st>>>(L, V, M, counts, tcounts, reach, at(o_key), save ? at(o_tkey) : nullptr, at(o_ids), at(o_es),
                                                          at(o_ed), summary);
@@ -2101,6 +2099,14 @@ static int build_sparse_device(ggnn_engine* e, int32_t V, const int32_t* const* 
     unsigned sum[dg::S_COUNT];
     CU_TRY(e, cudaMemcpyAsync(sum, summary, sizeof sum, cudaMemcpyDeviceToHost, st));
     CU_TRY(e, cudaStreamSynchronize(st));
+    if (sum[dg::S_BAD] != 0xffffffffu && gcn) {   // the entry's int64 values: one more 16-byte read, on this path only
+        const int64_t k = sum[dg::S_BAD];
+        int64_t ij[2];
+        CU_TRY(e, cudaMemcpyAsync(ij, gcn->list + 2 * k, sizeof ij, cudaMemcpyDeviceToHost, st));
+        CU_TRY(e, cudaStreamSynchronize(st));
+        return e->fail(GGNN_ERANGE, "adjacency_list[%lld] = (%lld, %lld) is out of range for %d nodes", (long long)k, (long long)ij[0],
+                       (long long)ij[1], V);
+    }
     if (sum[dg::S_BAD] != 0xffffffffu)
         return e->fail(GGNN_ERANGE, "edge %d of type %d = (%d,%d) is out of range for %d nodes", (int)sum[dg::S_BAD_I], (int)sum[dg::S_BAD_T],
                        (int)sum[dg::S_BAD_S], (int)sum[dg::S_BAD_D], V);
@@ -2114,7 +2120,7 @@ static int build_sparse_device(ggnn_engine* e, int32_t V, const int32_t* const* 
     if (V > 0) cuts.push_back(V);
     BatchPlan p;
     std::vector<int> tile_start;
-    if (int rc = build_plan(shape, V, msg_weighted, cuts, p, tile_start, e->err, msg_weighted, msg_weighted)) return rc;
+    if (int rc = build_plan(shape, V, weighted, cuts, p, tile_start, e->err, stream_weighted, msg_weighted)) return rc;
     if (msg_weighted) p.plan_text += " [message-weighted]";
     const int ntiles = p.ntiles;
     const int nv = p.stream ? (int)(p.all_virtual ? sum[dg::S_NV1] : sum[dg::S_NV2]) : 0;
@@ -2133,8 +2139,8 @@ static int build_sparse_device(ggnn_engine* e, int32_t V, const int32_t* const* 
     }
     if (V > 0) {
         if (indeg) CU_TRY(e, cudaMemcpyAsync(img.indeg, indeg, sizeof(float) * (size_t)VT, cudaMemcpyDeviceToDevice, st));
-        else dg::indeg_kernel<<<grid_for(e, VT), 256, 0, st>>>(counts, VT, img.indeg);
-        dg::denom_kernel<<<grid_for(e, V), 256, 0, st>>>(img.indeg, V, T, img.denom);
+        else if (!gcn) dg::indeg_kernel<<<grid_for(e, VT), 256, 0, st>>>(counts, VT, img.indeg);
+        dg::denom_kernel<<<grid_for(e, V), 256, 0, st>>>(img.indeg, V, T, img.denom);   // (GCN: zero in-degrees, denominators 1e-7f)
     }
     int* vid = nullptr;
     if (p.stream) {
@@ -2171,12 +2177,47 @@ static int build_sparse_device(ggnn_engine* e, int32_t V, const int32_t* const* 
 
 extern "C" {
 
-int ggnn_set_graph_sparse_device(ggnn_engine* e, int32_t num_nodes, const int32_t* const* adjacency_lists, const int32_t* num_edges,
-                                 const float* num_incoming_edges_per_type, int32_t message_weighted, ggnn_stream_t stream) {
+int ggnn_set_graph_sparse_device(ggnn_engine* e, int32_t V, const int32_t* const* adj, const int32_t* num_edges, const float* indeg,
+                                 int32_t message_weighted, ggnn_stream_t stream) {
     if (!e) return GGNN_EINVAL;
     GGNN_REQUIRE_MODEL(e, MODEL_GGNN);
     forget_batch(e);
-    return build_sparse_device(e, num_nodes, adjacency_lists, num_edges, num_incoming_edges_per_type, message_weighted != 0, (cudaStream_t)stream);
+    const bool mw = message_weighted != 0;
+    if (mw && e->use_att)
+        return e->fail(GGNN_EUNSUPPORTED, "message weights with propagation attention are not supported (the probabilities are the slot weights)");
+    if (V < 0 || !adj || !num_edges) return e->fail(GGNN_EINVAL, "null/negative argument");
+    const int T = e->T;
+    dg::EdgeLists L{};
+    L.T = T;
+    for (int t = 0; t < T; ++t) {
+        if (num_edges[t] < 0 || (num_edges[t] > 0 && !adj[t])) return e->fail(GGNN_EINVAL, "adjacency list %d is null/negative", t);
+        L.adj[t] = adj[t];
+        L.base[t + 1] = L.base[t] + num_edges[t];
+    }
+    if (L.base[T] > 0x7fffffff || (int64_t)V * T + 1 > 0x7fffffff) return e->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
+    CU_TRY(e, cudaSetDevice(e->device));
+    for (int t = 0; t < T; ++t)
+        if (num_edges[t] > 0 && !on_device(adj[t], e->device))
+            return e->fail(GGNN_EINVAL, "adjacency list %d is not device memory of device %d", t, e->device);
+    if (indeg && V > 0 && !on_device(indeg, e->device))
+        return e->fail(GGNN_EINVAL, "num_incoming_edges_per_type is not device memory of device %d", e->device);
+    return build_sparse_device(e, V, L, indeg, nullptr, mw, mw, mw, (cudaStream_t)stream);
+}
+
+int ggnn_set_graph_gcn_device(ggnn_engine* e, int32_t V, int64_t nnz, const int64_t* list, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    GGNN_REQUIRE_MODEL(e, MODEL_GCN);
+    forget_batch(e);
+    if (V < 0 || nnz < 0 || (nnz > 0 && !list)) return e->fail(GGNN_EINVAL, "null/negative argument");
+    if (nnz > 0x7fffffff || (int64_t)V + 1 > 0x7fffffff) return e->fail(GGNN_EUNSUPPORTED, "batch too large for int32 indexing");
+    CU_TRY(e, cudaSetDevice(e->device));
+    if (nnz > 0 && !on_device(list, e->device)) return e->fail(GGNN_EINVAL, "adjacency_list is not device memory of device %d", e->device);
+    dg::EdgeLists L{};
+    L.T = 1;
+    L.base[1] = nnz;
+    const GcnDeviceList gcn{list};
+    // build_gcn_image's message-weighted build: weighted, not stream-weighted, message-weighted
+    return build_sparse_device(e, V, L, nullptr, &gcn, true, false, true, (cudaStream_t)stream);
 }
 
 

@@ -1029,8 +1029,9 @@ class GCNEngine(PropagationEngine):
     ``wide_hidden`` (``ggnn_gcn_config.wide_hidden``): hidden sizes up to 512, and above 128 on bf16x3 / bf16 the streaming wgmma plan
     (a weighted gather and one GEMM launch per layer) instead of the fp32 kernel.  Batches and datasets must be prepared with the same value.
 
-    Adjacency weights on the device: ``prepare_graph_gcn_message_weighted`` + ``set_graph_prepared``, then ``set_message_weights(w)`` (the
-    inherited call) before every forward that should use new weights, and ``backward(..., d_adjacency_weights=)`` for their gradient."""
+    Adjacency weights on the device: ``prepare_graph_gcn_message_weighted`` + ``set_graph_prepared`` (or, with the list on the GPU,
+    ``set_graph_gcn_device``), then ``set_message_weights(w)`` (the inherited call) before every forward that should use new weights, and
+    ``backward(..., d_adjacency_weights=)`` for their gradient."""
 
     def __init__(self, hidden_size: int, num_layers: int, use_bias: bool = False, device: int = 0, precision: str = "fp32",
                  wide_hidden: bool = False):
@@ -1095,6 +1096,32 @@ class GCNEngine(PropagationEngine):
         g = reuse if reuse is not None else PreparedGraph(self.lib)
         return g._fill(self.lib.ggnn_prepare_graph_gcn_message_weighted, int(num_nodes), 1, self._h,
                        -1 if save_for_backward is None else int(bool(save_for_backward)), int(num_nodes), lst.shape[0], lst.ctypes.data)
+
+    def set_graph_gcn_device(self, num_nodes: int, adjacency_list):
+        """``prepare_graph_gcn_message_weighted`` + ``set_graph_prepared`` with the list already on the GPU (``ggnn_set_graph_gcn_device``):
+        ``adjacency_list`` a contiguous int64 CUDA tensor ``[nnz, 2]`` (row i = output, column j = input) on the engine's device.  The batch
+        is built on the device, with the host's plan, into the image the host builder would upload, byte for byte; follow with
+        ``set_message_weights(w)`` (``w`` fp32 CUDA ``[nnz]`` in list order) before a forward.  The call waits for the current stream for
+        three small reads at most; the tensor is kept alive until the next graph upload."""
+        import torch
+        V = int(num_nodes)
+        if V < 0:
+            raise GgnnError("num_nodes must be >= 0, got %d" % V)
+        a = adjacency_list
+        if not isinstance(a, torch.Tensor):
+            raise GgnnError("adjacency_list must be a torch tensor, got %s" % type(a).__name__)
+        if a.dtype != torch.int64:
+            raise GgnnError("adjacency_list must be int64, got %s" % a.dtype)
+        if a.dim() != 2 or a.shape[1] != 2:
+            raise GgnnError("adjacency_list must be [nnz, 2], got %s" % (tuple(a.shape),))
+        if not a.is_contiguous():
+            raise GgnnError("adjacency_list must be contiguous")
+        if a.device != torch.device("cuda", self.device):
+            raise GgnnError("adjacency_list must be on cuda:%d, got %s" % (self.device, a.device))
+        self.serial += 1
+        self._check(self.lib.ggnn_set_graph_gcn_device(self._h, V, a.shape[0], a.data_ptr() if a.shape[0] else None, self._stream()))
+        self.V = V
+        self._graph_keepalive = (a,)
 
     def backward(self, d_out, grads: Sequence[dict], d_h0=None, d_adjacency_weights=None):
         """``grads[l]``: dict with optional ``kernel`` [D, D] / ``bias`` [D] fp32 CUDA tensors, accumulated into.  With

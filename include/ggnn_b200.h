@@ -498,6 +498,22 @@ int ggnn_host_prepare_graph_gcn_message_weighted(const ggnn_gcn_config* cfg, int
                                                  int64_t nnz, const int64_t* adjacency_list, ggnn_prepared_graph** inout);
 int ggnn_gcn_backward_weighted(ggnn_engine* e, const float* d_h_out, const ggnn_gcn_layer_grads* grads, int32_t num_layers, float* d_h0,
                                float* d_adjacency_weights, ggnn_stream_t stream);
+/* ---- Sparse GCN graphs on the device: ggnn_prepare_graph_gcn_message_weighted + ggnn_set_graph_prepared with the list already in the
+ * engine's device memory.
+ *   adjacency_list   DEVICE pointer to the reference's [nnz, 2] int64 feed (chem_tensorflow_gcn.py:46): column 0 = the OUTPUT row i,
+ *                    column 1 = the INPUT column j, as in ggnn_prepare_graph_gcn (8-byte aligned; only its 16 * nnz bytes are read)
+ * The engine is left exactly as those two calls leave it, with the engine's save_for_backward flag: the same plan and plan text (ending in
+ * " [message-weighted]"), per-tile maxima, ggnn_num_messages (= nnz) and graph image, every byte included (pads, the zero slot-weight
+ * sections and, with save_for_backward, the source-keyed CSR's slot map).  The adjacency weights follow through ggnn_set_message_weights:
+ * a forward without them is GGNN_ESTATE, and ggnn_gcn_backward_weighted gives their gradient.  The list is turned into the one edge type
+ * (source j, target i) and the batch is built by the kernels of ggnn_set_graph_sparse_device on `stream` into the engine's graph buffer.
+ * No edge is copied to the host.  The call synchronises `stream` two or three times, each for a small read back: a summary (first bad
+ * entry, number of cut points), the cut points when the plan needs them and the batch has any, and the two per-tile maxima.  The image does
+ * not depend on the order of any atomic.  Refusals match the host builder: GGNN_ERANGE names the first out-of-range entry in list order with
+ * its int64 values (read back on that path only); GGNN_EINVAL for null / negative arguments and for a list that is not device memory of the
+ * engine's device; GGNN_EUNSUPPORTED for nnz > INT32_MAX, before any of the list is read.  A GGNN engine refuses the call.  Like every
+ * upload, a failed call first forgets the previous batch. */
+int ggnn_set_graph_gcn_device(ggnn_engine* e, int32_t num_nodes, int64_t nnz, const int64_t* adjacency_list, ggnn_stream_t stream);
 
 /* ---- Device-resident datasets: the training graphs uploaded once, every batch of whole graphs assembled on the device.
  * Graphs never share edges, so a batch's graph image is its graphs' pieces (CSR slice, in-degrees, denominators, source-keyed CSR,
