@@ -94,6 +94,9 @@ SYMBOLS = {
     "ggnn_forward_host_async":(C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ggnn_sync_check": (C.c_int, [C.c_void_p, C.c_void_p]),
     "ggnn_readout_set_graphs": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "ggnn_readout_set_graphs_device": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "ggnn_readout_map": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)] + [C.c_void_p] * 4
+                         + [C.c_void_p]),
     "ggnn_readout_forward": (C.c_int, [C.c_void_p] + [C.c_void_p] * 7 + [C.c_void_p]),
     "ggnn_readout_backward": (C.c_int, [C.c_void_p] + [C.c_void_p] * 12 + [C.c_void_p]),
     "ggnn_set_state_dropout": (C.c_int, [C.c_void_p, C.c_float, C.c_uint64]),

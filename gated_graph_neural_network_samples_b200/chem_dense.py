@@ -148,7 +148,10 @@ class DenseGGNNChemModel(ChemModel):
         return self.output
 
     def _set_readout_map(self) -> None:
-        mask = np.asarray(self.feed[self.placeholders['node_mask']], dtype=np.float32)
+        import torch
+        mask = self.feed[self.placeholders['node_mask']]
+        if not (torch.is_tensor(mask) and mask.is_cuda):   # a CUDA mask goes as it is: the map is built on the device
+            mask = np.asarray(mask, dtype=np.float32)
         self.engine.readout_set_graphs(mask.shape[0], nodes_per_graph=mask.shape[1], node_mask=mask)
 
     # ------------------------------------------------------------------ prediction (dense:230-265)

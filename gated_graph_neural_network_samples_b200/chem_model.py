@@ -459,12 +459,12 @@ class ChemModel(object):
         self.__dict__.setdefault('_dataset_batch_pool', []).append(batch)   # rebuilt in place later; a rebuild first waits for this upload
 
     def _graph_nodes_list(self):
-        """The batch's node -> graph map as a long tensor on the device: the feed's array, or for a device-data batch the graphs' node
-        counts expanded on the device."""
+        """The batch's node -> graph map as a long tensor on the device: the feed's array or tensor (a CUDA one is converted on the device, with
+        no host copy), or for a device-data batch the graphs' node counts expanded on the device."""
         import torch
         gnl = self.feed.get(self.placeholders['graph_nodes_list'])
         if gnl is not None:
-            return torch.as_tensor(np.asarray(gnl), device=self.device, dtype=torch.long)
+            return torch.as_tensor(gnl if torch.is_tensor(gnl) else np.asarray(gnl), device=self.device, dtype=torch.long)
         sizes = torch.as_tensor(self.feed['_graph_sizes'], device=self.device)
         return torch.repeat_interleave(torch.arange(sizes.shape[0], device=self.device), sizes)
 

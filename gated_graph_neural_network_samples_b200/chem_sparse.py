@@ -294,6 +294,7 @@ class SparseGGNNChemModel(ChemModel):
         return self.output
 
     def _set_readout_map(self) -> None:
+        # a host list goes through np.asarray in readout_set_graphs; a CUDA one as it is, and the map is built on the device
         self.engine.readout_set_graphs(int(self.feed[self.placeholders['num_graphs']]), graph_nodes_list=self.feed[self.placeholders['graph_nodes_list']])
 
     # ------------------------------------------------------------------ prediction (sparse:352-376)

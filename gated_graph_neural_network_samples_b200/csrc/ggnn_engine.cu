@@ -36,6 +36,7 @@
 #include "ggnn_msgw.cuh"
 #include "ggnn_dense_adj.cuh"
 #include "ggnn_device_graph.cuh"
+#include "ggnn_readout_map.cuh"
 #include "ggnn_tc_smem.h"
 
 #include <cub/device/device_radix_sort.cuh>
@@ -3330,6 +3331,98 @@ int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* gr
     if (node_mask) memcpy(base + e->ro_off_mask, node_mask, sizeof(float) * (size_t)V);
     CU_TRY(e, e->ro_stage.upload(e->ro_buf.ptr, grouped ? e->ro_off_perm : off, (cudaStream_t)stream));
     e->ro_V = V; e->ro_G = G; e->ro_grouped = grouped; e->ro_has_mask = node_mask != nullptr; e->ro_from_dataset = false;
+    return GGNN_OK;
+}
+
+// The host builder's sections from DEVICE arrays (ggnn_readout_map.cuh), built on `stream` into ro_buf.  A list costs one stream
+// synchronise for the summary (two on the refusal path, which reads the bad entry back); a dense map none.
+int ggnn_readout_set_graphs_device(ggnn_engine* e, int32_t num_nodes, const int32_t* graph_nodes_list, int32_t num_graphs,
+                                   int32_t nodes_per_graph, const float* node_mask, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    e->ro_V = -1;
+    if (num_nodes < 0 || num_graphs < 0) return e->fail(GGNN_EINVAL, "negative size");
+    if (!graph_nodes_list && (nodes_per_graph <= 0 || (int64_t)nodes_per_graph * num_graphs != num_nodes))
+        return e->fail(GGNN_EINVAL, "without a graph_nodes_list the batch must be num_graphs x nodes_per_graph (%d x %d != %d)", num_graphs, nodes_per_graph, num_nodes);
+    CU_TRY(e, cudaSetDevice(e->device));
+    const int V = num_nodes, G = num_graphs;
+    if (V > 0 && graph_nodes_list && !on_device(graph_nodes_list, e->device))
+        return e->fail(GGNN_EINVAL, "graph_nodes_list is not device memory of device %d", e->device);
+    if (V > 0 && node_mask && !on_device(node_mask, e->device))
+        return e->fail(GGNN_EINVAL, "node_mask is not device memory of device %d", e->device);
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t off = readout_layout(e, V, G);
+    CU_TRY(e, e->ro_buf.reserve(align_up(off + sizeof(float) * (size_t)std::max(V, 1), 16)));
+    char* base = (char*)e->ro_buf.ptr;
+    int* graph_of = (int*)(base + e->ro_off_graph_of);
+    int* start = (int*)(base + e->ro_off_start);
+    bool grouped = true;
+    if (graph_nodes_list) {
+        // scratch: per-graph counts [G+1] (the last stays 0, so the exclusive scan's entry G is V), the summary, the sort's keys out and
+        // node ids, CUB's storage
+        const size_t I = sizeof(int), Vr = (size_t)std::max(V, 1);
+        ScratchCarver c;
+        const size_t o_counts = c.take(I * ((size_t)G + 1)), o_summary = c.take(I * ro_map::S_COUNT), o_keys = c.take(I * Vr),
+                     o_ids = c.take(I * Vr), o_temp = c.off;
+        const int key_bits = G > 1 ? 32 - __builtin_clz((unsigned)(G - 1)) : 1;
+        size_t temp = 0, need = 0;
+        CU_TRY(e, cub::DeviceScan::ExclusiveSum(nullptr, need, (int*)nullptr, (int*)nullptr, G + 1, st));
+        temp = std::max(temp, need);
+        CU_TRY(e, cub::DeviceRadixSort::SortPairs(nullptr, need, (const int*)nullptr, (int*)nullptr, (const int*)nullptr, (int*)nullptr, (int)Vr, 0,
+                                                  key_bits, st));
+        temp = std::max(temp, need);
+        CU_TRY(e, e->dg_scratch.reserve(o_temp + temp));
+        char* s0 = (char*)e->dg_scratch.ptr;
+        int* counts = (int*)(s0 + o_counts);
+        unsigned* summary = (unsigned*)(s0 + o_summary);
+        CU_TRY(e, cudaMemsetAsync(counts, 0, I * ((size_t)G + 1), st));
+        CU_TRY(e, cudaMemsetAsync(summary + ro_map::S_BAD, 0xff, sizeof(unsigned), st));
+        CU_TRY(e, cudaMemsetAsync(summary + ro_map::S_UNGROUPED, 0, sizeof(unsigned), st));
+        if (V > 0) ro_map::graph_map_kernel<<<grid_for(e, V), 256, 0, st>>>(graph_nodes_list, V, G, graph_of, counts, summary);
+        CU_TRY(e, cub::DeviceScan::ExclusiveSum(s0 + o_temp, temp, counts, start, G + 1, st));
+        unsigned sum[ro_map::S_COUNT];
+        CU_TRY(e, cudaMemcpyAsync(sum, summary, sizeof sum, cudaMemcpyDeviceToHost, st));
+        CU_TRY(e, cudaStreamSynchronize(st));
+        if (sum[ro_map::S_BAD] != 0xffffffffu) {   // the entry's value: one more 4-byte read, on this path only
+            const int v = (int)sum[ro_map::S_BAD];
+            int32_t g = 0;
+            CU_TRY(e, cudaMemcpyAsync(&g, graph_nodes_list + v, sizeof g, cudaMemcpyDeviceToHost, st));
+            CU_TRY(e, cudaStreamSynchronize(st));
+            return e->fail(GGNN_ERANGE, "graph_nodes_list[%d] = %d is out of range for %d graphs", v, g, G);
+        }
+        grouped = sum[ro_map::S_UNGROUPED] == 0;
+        if (!grouped) {   // graph g owns perm[start[g] .. start[g+1]), its nodes in index order (deterministic mode)
+            int* ids = (int*)(s0 + o_ids);
+            ro_map::node_ids_kernel<<<grid_for(e, V), 256, 0, st>>>(V, ids);
+            CU_TRY(e, cub::DeviceRadixSort::SortPairs(s0 + o_temp, temp, graph_of, (int*)(s0 + o_keys), ids, (int*)(base + e->ro_off_perm), V, 0,
+                                                      key_bits, st));
+        }
+    } else {
+        ro_map::dense_map_kernel<<<grid_for(e, std::max<int64_t>(V, (int64_t)G + 1)), 256, 0, st>>>(V, G, nodes_per_graph, graph_of, start);
+    }
+    if (node_mask && V > 0) CU_TRY(e, cudaMemcpyAsync(base + e->ro_off_mask, node_mask, sizeof(float) * (size_t)V, cudaMemcpyDeviceToDevice, st));
+    CU_TRY(e, cudaGetLastError());
+    e->ro_V = V; e->ro_G = G; e->ro_grouped = grouped; e->ro_has_mask = node_mask != nullptr; e->ro_from_dataset = false;
+    return GGNN_OK;
+}
+
+int ggnn_readout_map(ggnn_engine* e, int32_t* num_nodes, int32_t* num_graphs, int32_t* flags, int32_t* graph_of, int32_t* start, int32_t* perm,
+                     float* node_mask, ggnn_stream_t stream) {
+    if (!e) return GGNN_EINVAL;
+    if (e->ro_V < 0) return e->fail(GGNN_ESTATE, "ggnn_readout_set_graphs has not been called for this batch");
+    const int V = e->ro_V, G = e->ro_G;
+    if (num_nodes) *num_nodes = V;
+    if (num_graphs) *num_graphs = G;
+    if (flags) *flags = (e->ro_grouped ? 1 : 0) | (e->ro_has_mask ? 2 : 0);
+    CU_TRY(e, cudaSetDevice(e->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    const char* base = (const char*)e->ro_buf.ptr;
+    if (graph_of && V > 0) CU_TRY(e, cudaMemcpyAsync(graph_of, base + e->ro_off_graph_of, sizeof(int) * (size_t)V, cudaMemcpyDeviceToHost, st));
+    if (start) CU_TRY(e, cudaMemcpyAsync(start, base + e->ro_off_start, sizeof(int) * ((size_t)G + 1), cudaMemcpyDeviceToHost, st));
+    if (perm && !e->ro_grouped && V > 0)
+        CU_TRY(e, cudaMemcpyAsync(perm, base + e->ro_off_perm, sizeof(int) * (size_t)V, cudaMemcpyDeviceToHost, st));
+    if (node_mask && e->ro_has_mask && V > 0)
+        CU_TRY(e, cudaMemcpyAsync(node_mask, base + e->ro_off_mask, sizeof(float) * (size_t)V, cudaMemcpyDeviceToHost, st));
+    CU_TRY(e, cudaStreamSynchronize(st));
     return GGNN_OK;
 }
 

@@ -916,7 +916,16 @@ class PropagationEngine:
     # ------------------------------------------------------------------ readout (gated_regression, sparse:220-231 / dense:119-129)
     def readout_set_graphs(self, num_graphs: int, graph_nodes_list=None, nodes_per_graph: int = 0, node_mask=None):
         """The batch's node -> graph map in the reference wire format: sparse ``graph_nodes_list`` [V] int32 (sparse:337), or
-        dense ``nodes_per_graph`` = num_vertices with ``node_mask`` [b, v] (dense:126).  HOST arrays."""
+        dense ``nodes_per_graph`` = num_vertices with ``node_mask`` [b, v] (dense:126).  HOST arrays, or CUDA tensors on the engine's device
+        (``ggnn_readout_set_graphs_device``: a contiguous int32 ``[V]`` list, a contiguous fp32 mask of V entries): the map is then built on
+        the GPU, the same map the host arrays give, and a list costs one wait for the current stream.  Host and CUDA arguments do not mix;
+        ``num_graphs`` is a host int either way."""
+        import torch
+        cuda = [torch.is_tensor(a) and a.is_cuda for a in (graph_nodes_list, node_mask) if a is not None]
+        if any(cuda):
+            if not all(cuda):
+                raise GgnnError("graph_nodes_list and node_mask must both be CUDA tensors or both host arrays")
+            return self._readout_set_graphs_device(int(num_graphs), graph_nodes_list, int(nodes_per_graph), node_mask)
         gnl = mask = None
         if graph_nodes_list is not None:
             gnl = np.ascontiguousarray(np.asarray(graph_nodes_list, dtype=np.int32).reshape(-1))
@@ -931,6 +940,52 @@ class PropagationEngine:
                                                      None if mask is None else mask.ctypes.data, self._stream()))
         self._readout_keepalive = (gnl, mask)
         self._readout_shape = (V, int(num_graphs))
+
+    def _readout_set_graphs_device(self, G: int, gnl, npg: int, mask):
+        """``readout_set_graphs`` with CUDA tensors: checks them, then ``ggnn_readout_set_graphs_device``; raises ``GgnnError`` before the
+        call for a bad feed.  The tensors are kept alive until the next map."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        if gnl is not None:
+            if gnl.dtype != torch.int32:
+                raise GgnnError("graph_nodes_list must be int32, got %s" % gnl.dtype)
+            if gnl.dim() != 1:
+                raise GgnnError("graph_nodes_list must be [V], got %s" % (tuple(gnl.shape),))
+            if not gnl.is_contiguous():
+                raise GgnnError("graph_nodes_list must be contiguous")
+            if gnl.device != dev:
+                raise GgnnError("graph_nodes_list must be on cuda:%d, got %s" % (self.device, gnl.device))
+            V = gnl.shape[0]
+        else:
+            V = G * npg
+        if mask is not None:
+            if mask.dtype != torch.float32:
+                raise GgnnError("node_mask must be float32, got %s" % mask.dtype)
+            if not mask.is_contiguous():
+                raise GgnnError("node_mask must be contiguous")
+            if mask.device != dev:
+                raise GgnnError("node_mask must be on cuda:%d, got %s" % (self.device, mask.device))
+            if mask.numel() != V:
+                raise GgnnError("node_mask has %d entries for %d nodes" % (mask.numel(), V))
+        # an empty tensor has no storage, and NULL means "no list" / "no mask" to the entry: one element stands in (none of it is read)
+        ptr = lambda t: None if t is None else (t if V else torch.empty(1, dtype=t.dtype, device=dev)).data_ptr()
+        lp, mp = ptr(gnl), ptr(mask)
+        self._check(self.lib.ggnn_readout_set_graphs_device(self._h, V, lp, G, npg, mp, self._stream()))
+        self._readout_keepalive = (gnl, mask)
+        self._readout_shape = (V, G)
+
+    def readout_map(self) -> dict:
+        """The current readout map copied back (``ggnn_readout_map``): ``graph_of`` [V], ``start`` [G+1], ``grouped``, ``perm`` [V] (an
+        ungrouped list's stable by-graph order, else None) and ``node_mask`` [V] (None without one), as NumPy arrays."""
+        V, G, flags = C.c_int32(), C.c_int32(), C.c_int32()
+        self._check(self.lib.ggnn_readout_map(self._h, C.byref(V), C.byref(G), C.byref(flags), None, None, None, None, self._stream()))
+        V, G, flags = V.value, G.value, flags.value
+        graph_of, start, perm, mask = np.empty(V, np.int32), np.empty(G + 1, np.int32), np.empty(V, np.int32), np.empty(V, np.float32)
+        self._check(self.lib.ggnn_readout_map(self._h, None, None, None, graph_of.ctypes.data, start.ctypes.data, perm.ctypes.data,
+                                              mask.ctypes.data, self._stream()))
+        grouped, has_mask = bool(flags & 1), bool(flags & 2)
+        return {"graph_of": graph_of, "start": start, "grouped": grouped, "perm": None if grouped else perm,
+                "node_mask": mask if has_mask else None}
 
     @staticmethod
     def _f32(t, n, what):

@@ -313,6 +313,23 @@ int ggnn_forward_host_async(ggnn_engine* e, const float* h0_host, float* h_out_h
  * to the current batch: a graph upload drops it, and the readout calls return GGNN_ESTATE until ggnn_readout_set_graphs runs again. */
 int ggnn_readout_set_graphs(ggnn_engine* e, int32_t num_nodes, const int32_t* graph_nodes_list, int32_t num_graphs,
                             int32_t nodes_per_graph, const float* node_mask, ggnn_stream_t stream);
+/* ---- The readout map from DEVICE arrays: ggnn_readout_set_graphs with graph_nodes_list [V] int32 and node_mask [V] fp32 in the engine's
+ * device memory (either may be NULL under the same rules; only their V entries are read).  The engine is left exactly as the host call
+ * leaves it: the same node -> graph map, per-graph node ranges, mask, grouped / ungrouped choice and, for an ungrouped list, the same
+ * stable by-graph permutation, so every readout call gives the host map's bits.  The map is built by kernels on `stream`; atomics only
+ * count, and the map does not depend on the order of any atomic.  With a list, the call synchronises `stream` once, for a small read
+ * back (the first bad node and whether the list is grouped); no node is copied to the host.  A dense map (no list) is built without a
+ * synchronisation.  Refusals match the host call: GGNN_ERANGE names the lowest out-of-range node with the host's text (its value is read
+ * back on that path only); GGNN_EINVAL for negative sizes, a missing list when nodes_per_graph * num_graphs != num_nodes, and a list or
+ * mask that is not device memory of the engine's device.  Like the host call, the entry first drops the current map, so a refused call
+ * leaves none (the readout calls return GGNN_ESTATE), and a graph upload drops a map built here. */
+int ggnn_readout_set_graphs_device(ggnn_engine* e, int32_t num_nodes, const int32_t* graph_nodes_list, int32_t num_graphs,
+                                   int32_t nodes_per_graph, const float* node_mask, ggnn_stream_t stream);
+/* The engine's current readout map copied back to HOST buffers (for tests comparing builders; any pointer may be NULL): num_nodes V,
+ * num_graphs G, flags (bit 0: the list is grouped, bit 1: the map has a mask), graph_of [V], start [G+1], perm [V] (written only for an
+ * ungrouped list) and node_mask [V] (written only when the map has a mask).  GGNN_ESTATE without a map.  Synchronises `stream`. */
+int ggnn_readout_map(ggnn_engine* e, int32_t* num_nodes, int32_t* num_graphs, int32_t* flags, int32_t* graph_of, int32_t* start, int32_t* perm,
+                     float* node_mask, ggnn_stream_t stream);
 int ggnn_readout_forward(ggnn_engine* e, const float* h_last, const float* h0, const float* w_gate, const float* b_gate,
                          const float* w_trans, const float* b_trans, float* out, ggnn_stream_t stream);
 int ggnn_readout_backward(ggnn_engine* e, const float* h_last, const float* h0, const float* w_gate, const float* b_gate,
